@@ -487,13 +487,18 @@ BTLE_HD uint32_t crc24_words(const uint32_t words[11], int nbody, uint32_t crc, 
 // length, reported only when sp.report_rejected); returns their number.  What a counted packet
 // contains does not influence the chain, so payload decode and CRC are left to decode_packet(), which the
 // kernel runs afterwards for all packets of a span at once (one lane per packet, converged).
-constexpr int kMaxRejectedPerChunk = 16;   // rejected hits reported per chunk (a degenerate mask can produce > 100)
+// With report_rejected a chunk reports up to BTLE_MAX_RECS_PER_CHUNK hits (include/btle_b200.h), without it at most
+// BTLE_MAX_PKTS_PER_CHUNK.
+// Rejected hits the resolver's per-chunk hit row holds on top of BTLE_MAX_PKTS_PER_CHUNK counted packets.  NOT a limit on
+// what is reported: a chunk with more hits is finished by its own lane (btle_rx_kernels.cu, resolver step 4).
+constexpr int kRejectedInHitRow = 16;
+constexpr int kMaxRejectedPerChunk = kRejectedInHitRow;   // former name of the same constant, kept so code using it still builds
 // search(R, n0_lim, n0&) -> bool: the reference's search_unique_bits restarted at sample R (see search_from)
 template <class Search, class Hit>
 BTLE_HD int chain_with(const uint32_t *pd, const StreamParams &sp, Search &search, Hit &hit) {
   int E = 0;                         // buf_len_eaten (int8 units), :2214
   int left = kSearchInt8 / 8;        // num_symbol_left, :2200
-  int count = 0, rejected = 0;
+  int count = 0;
   for (;;) {
     if (left <= 0) break;            // search loop would not run -> -1 -> break, :2218
     const int R = E >> 1;            // restart sample
@@ -512,7 +517,7 @@ BTLE_HD int chain_with(const uint32_t *pd, const StreamParams &sp, Search &searc
       if (sp.adv) {
         plen = (int)((w0 >> 8) & 0x3Fu);                 // :1962
         if (plen < 6 || plen > 37) {                     // :2291-2298 (cursor stays behind the header; not counted)
-          if (sp.report_rejected && rejected < kMaxRejectedPerChunk) { hit(count, n0, true); ++count; ++rejected; }   // -v "PktBAD"
+          if (sp.report_rejected) { hit(count, n0, true); ++count; }   // -v "PktBAD"
           continue;
         }
       } else {

@@ -369,6 +369,9 @@ struct Sinks {
     }
     ++pkt_count;                                                                // :2274 / :2319
     btle_b200_note_packet(&r);                                                  // receiver_status.crc_ok, :2320-2321
+    // A hit through the zeroed history of chunk k+1 (n0 < 0) can start before the previous packet of chunk k.  The
+    // reference stamps packets when it processes them (gettimeofday, :2323), so its clock never runs backwards.
+    if (t < t_prev) t = t_prev;
     const int time_diff = (int)llround((t - t_prev) * 1e6);
     t_prev = t;
     const int rssi = o.rssi ? rssi_from_mag(r.mag_sum) : INT_MIN;

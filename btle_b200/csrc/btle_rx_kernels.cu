@@ -98,9 +98,13 @@ struct Slot {
   StreamParams sp;
 };
 
-constexpr int kHitCap = BTLE_MAX_PKTS_PER_CHUNK + kMaxRejectedPerChunk + 1;    // counted + reported-rejected hits per chunk (68 x u16)
+// Hits the chain pass keeps per chunk (68 x u16): every counted packet fits.  With report_rejected a chunk may have up to
+// BTLE_MAX_RECS_PER_CHUNK hits; rows of that size would not fit next to the ring, so the hits behind the row are decoded by
+// the chunk's own lane, which runs the chain once more (resolver step 4).
+constexpr int kHitCap = BTLE_MAX_PKTS_PER_CHUNK + kRejectedInHitRow + 1;
+static_assert(kHitCap >= BTLE_MAX_PKTS_PER_CHUNK && kSpanChunks * BTLE_MAX_RECS_PER_CHUNK < 0x10000, "hit rows / u16 prefix");
 struct ResolveScratch {                        // per resolver warp, between the chain pass and the decode pass
-  uint16_t hit[kSpanChunks][kHitCap];          // n0 + 124 of every counted packet, per chunk, in the reference's order
+  uint16_t hit[kSpanChunks][kHitCap];          // n0 + 124 of the chunk's first kHitCap hits, in the reference's order
   uint16_t pre[kSpanChunks + 2];               // exclusive prefix of the per-chunk counts; [kSpanChunks] = total
   uint16_t xh[2 * kSpanChunks][kExactCap + 1]; // exact access-address hits per flag word (offsets inside the word); [kExactCap] = count
 };
@@ -503,7 +507,9 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
       if (lane < si.nch) {
         struct Note {
           uint16_t *row;
-          __device__ __forceinline__ void operator()(int i, int n0, bool rej) { row[i] = (uint16_t)((n0 + 124) | (rej ? 0x8000 : 0)); }
+          __device__ __forceinline__ void operator()(int i, int n0, bool rej) {
+            if (i < kHitCap) row[i] = (uint16_t)((n0 + 124) | (rej ? 0x8000 : 0));
+          }
         } note{RS.hit[lane]};
         const uint32_t *pdc = reinterpret_cast<const uint32_t *>(&S.pd[kGroupsPerChunk * lane]);
         const int c0 = RS.xh[2 * lane][kExactCap], c1 = RS.xh[2 * lane + 1][kExactCap];
@@ -532,20 +538,49 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
         const int j = j0 + lane;
         uint32_t words[11];
         int nbytes = 0, crc_bad = 0, n0 = 0, c = 0;
-        bool rej = false;
+        bool rej = false, live = false;
         if (j < total) {
           // chunk of packet j: pre[c] <= j < pre[c + 1]
 #pragma unroll
           for (int step = kSpanChunks / 2; step >= 1; step >>= 1)
             if ((int)RS.pre[c + step] <= j) c += step;
-          const int h = (int)RS.hit[c][j - (int)RS.pre[c]];
-          rej = (h & 0x8000) != 0;
-          n0 = (h & 0x7FFF) - 124;
-          decode_packet(reinterpret_cast<const uint32_t *>(&S.pd[kGroupsPerChunk * c]), S.sp, M.crc4, n0, rej, words, nbytes, crc_bad);
+          const int i = j - (int)RS.pre[c];
+          live = i < kHitCap;                               // hits behind the chunk's row are left to step 4
+          if (live) {
+            const int h = (int)RS.hit[c][i];
+            rej = (h & 0x8000) != 0;
+            n0 = (h & 0x7FFF) - 124;
+            decode_packet(reinterpret_cast<const uint32_t *>(&S.pd[kGroupsPerChunk * c]), S.sp, M.crc4, n0, rej, words, nbytes, crc_bad);
+          }
         }
         const unsigned base = __shfl_sync(0xFFFFFFFFu, my_base, 0);
-        if (j < total && base + (unsigned)j < cap)
+        if (live && base + (unsigned)j < cap)
           store_record(out + base + j, si.stream, si.chunk0 + c, n0, nbytes, crc_bad, rej, words, S.sp, cap_base, n_int8, lead);
+      }
+      // 4. only with report_rejected can a chunk have more hits than its row holds (degenerate masks, up to
+      //    BTLE_MAX_RECS_PER_CHUNK): the chunk's lane runs the same chain again and decodes and stores hits kHitCap.. itself
+      if (S.sp.report_rejected) {
+        const unsigned base = __shfl_sync(0xFFFFFFFFu, my_base, 0);
+        if (mine > kHitCap) {
+          struct Late {
+            const uint32_t *pd; const StreamParams &sp; const uint32_t *crc4;
+            btle_pkt_rec *out; unsigned first, cap; int stream, chunk; const int8_t *iq; long long n_int8, lead;
+            __device__ __forceinline__ void operator()(int i, int n0, bool rej) {
+              if (i < kHitCap || first + (unsigned)i >= cap) return;
+              uint32_t words[11];
+              int nbytes, crc_bad;
+              decode_packet(pd, sp, crc4, n0, rej, words, nbytes, crc_bad);
+              store_record(out + first + i, stream, chunk, n0, nbytes, crc_bad, rej, words, sp, iq, n_int8, lead);
+            }
+          };
+          const uint32_t *pdc = reinterpret_cast<const uint32_t *>(&S.pd[kGroupsPerChunk * lane]);
+          Late late{pdc, S.sp, M.crc4, out, base + RS.pre[lane], cap, si.stream, si.chunk0 + lane, cap_base, n_int8, lead};
+          const int c0 = RS.xh[2 * lane][kExactCap], c1 = RS.xh[2 * lane + 1][kExactCap];
+          if (c0 > kExactCap || c1 > kExactCap)
+            chain_chunk(pdc, &S.cand[kGroupsPerChunk * lane], &S.flagw[2 * lane], S.sp, late);
+          else
+            chain_chunk_lists(pdc, RS.xh[2 * lane], c0, RS.xh[2 * lane + 1], c1, S.sp, late);
+        }
       }
       BTLE_STAMP(9);
       __syncwarp();
@@ -1949,7 +1984,7 @@ int stream_collect(btle_b200_stream *s, int b) {
   H.busy = false;
   BTLE_CUDA(ctx, cudaStreamSynchronize(H.st));
   const size_t found = *H.h_count;
-  if (found > H.cap) { ctx->err = "stream segment produced more packets than BTLE_MAX_PKTS_PER_CHUNK allows"; return BTLE_EOVERFLOW; }
+  if (found > H.cap) { ctx->err = "stream segment produced more records than BTLE_MAX_RECS_PER_CHUNK allows"; return BTLE_EOVERFLOW; }
   if (!found) return BTLE_OK;
   BTLE_CUDA(ctx, cudaMemcpyAsync(H.h_recs, H.d_out, found * sizeof(btle_pkt_rec), cudaMemcpyDeviceToHost, H.st));
   BTLE_CUDA(ctx, cudaStreamSynchronize(H.st));
@@ -1985,7 +2020,7 @@ int btle_b200_stream_open(btle_b200_ctx *ctx, const btle_stream_cfg *cfg, size_t
   s->ctx = ctx; s->cfg = *cfg; s->seg_chunks = segment_chunks; s->seg_bytes = segment_chunks * (size_t)kChunkInt8;
   s->buf_bytes = s->seg_bytes + btle_b200_stream::kLook;
   for (auto &H : s->half) {
-    H.cap = segment_chunks * (BTLE_MAX_PKTS_PER_CHUNK + 16);
+    H.cap = segment_chunks * BTLE_MAX_RECS_PER_CHUNK;
     H.units = btle_b200_rx_units(ctx, 1, s->buf_bytes) + 1;
     if (cudaHostAlloc(reinterpret_cast<void **>(&H.h), btle_b200_stream::kLead + s->buf_bytes, cudaHostAllocDefault) != cudaSuccess ||
         cudaMalloc(reinterpret_cast<void **>(&H.d), btle_b200_stream::kLead + s->buf_bytes) != cudaSuccess ||

@@ -61,7 +61,9 @@ class BtleRx:
         ns, n = iq.shape
         cfgs = np.ascontiguousarray(cfgs, dtype=CFG_DTYPE)
         assert cfgs.shape == (ns,)
-        grow = cap is None                  # default capacity: typical worst case; grown once on BTLE_EOVERFLOW
+        # default capacity: typical worst case; grown once on BTLE_EOVERFLOW to the exact count, which is at most
+        # BTLE_MAX_PKTS_PER_CHUNK (51) records per chunk, or BTLE_MAX_RECS_PER_CHUNK (123) with BTLE_CFG_REPORT_REJECTED
+        grow = cap is None
         if cap is None:
             cap = ns * (n // 16384) * 34 + 16
         while True:

@@ -48,6 +48,13 @@ extern "C" {
  * 34 per chunk when bit 0 of the masked access address is set, 51 in the degenerate case mask == 0.  Real
  * captures hold a few; callers may size `cap` smaller and grow it on BTLE_EOVERFLOW (*n_out = needed). */
 #define BTLE_MAX_PKTS_PER_CHUNK 51
+/* Upper bound of records one chunk can return when BTLE_CFG_REPORT_REJECTED is set.  A rejected hit moves
+ * buf_len_eaten on by at least 2*n0' + 256 + 64*2 >= -248 + 384 = 136 int8 (the header is demodulated, then the
+ * search restarts behind it, :2291-2298), a counted packet by more, and hits start only while buf_len_eaten <= 16624
+ * (:2218): at most 16624/136 + 1 = 123 hits.  Mask 0 on an all-zero capture reaches it on channels 38 and 39: every
+ * window matches through the zeroed history, and every header is the channel's whitening sequence, whose length
+ * field is outside 6..37 there, so all 123 hits of a chunk are rejected. */
+#define BTLE_MAX_RECS_PER_CHUNK 123
 
 /* Per-capture receiver parameters == btle_rx's -c / -a / -m / -k / -r / -R options
  * (parse_commandline, btle_rx.c:1244-1458; defaults :1271-1301). */
@@ -60,8 +67,8 @@ typedef struct {
   int32_t rssi;          /* flag bits: BTLE_CFG_RSSI (-R) 1: also return sum|I|+|Q| over the AA samples
                             (:2234-2243); BTLE_CFG_REPORT_REJECTED (-v) 2: advertising-channel hits whose header
                             length is outside 6..37 — the reference prints "PktBAD" for them under -v and does not
-                            count them (:2291-2298) — come back as records with BTLE_REC_REJECTED set (at most 16
-                            per chunk)                                                                           */
+                            count them (:2291-2298) — come back as records with BTLE_REC_REJECTED set, every one
+                            of them, in the reference's order (up to BTLE_MAX_RECS_PER_CHUNK records per chunk)  */
 } btle_stream_cfg;
 #define BTLE_CFG_RSSI 1
 #define BTLE_CFG_REPORT_REJECTED 2

@@ -26,7 +26,7 @@ typedef struct {
   uint8_t channel;
   uint8_t n_bytes;     /* 42 in raw mode, else 2 + payload_len + 3                    */
   uint8_t crc_bad;     /* verdict of the reference's crc_check(): 1 = mismatch        */
-  uint8_t flags;       /* bit0 raw, bit1 advertising channel                          */
+  uint8_t flags;       /* bit0 raw, bit1 advertising channel, bit2 rejected hit        */
   uint32_t access_addr;
   uint16_t mag_sum;    /* sum |I|+|Q| over the 128 AA samples (RSSI, App. A.6)        */
   uint8_t bytes[42];   /* dewhitened header+payload+crc (raw mode: still whitened)    */
@@ -48,6 +48,12 @@ int orc_search(const uint8_t *d, int R, int left, uint32_t aa, uint32_t mask, in
 void orc_demod_bytes(const uint8_t *d, int n_first, int num_byte, uint8_t *out);
 int orc_receiver_chunk(const int8_t *win, const orc_cfg *cfg, orc_rec *out, int cap, int32_t stream, int32_t chunk);
 long orc_rx_stream(const int8_t *iq, long n_int8, const orc_cfg *cfg, int32_t stream, orc_rec *out, long cap);
+/* The same with -v: report_rejected != 0 returns the ADV hits whose header length is outside 6..37 too
+ * (printed as PktBAD, btle_rx.c:2291-2298), as records with flags bit2 set, n_bytes 2, the two header bytes. */
+int orc_receiver_chunk_ex(const int8_t *win, const orc_cfg *cfg, int report_rejected, orc_rec *out, int cap, int32_t stream,
+                          int32_t chunk);
+long orc_rx_stream_ex(const int8_t *iq, long n_int8, const orc_cfg *cfg, int report_rejected, int32_t stream, orc_rec *out,
+                      long cap);
 
 #ifdef __cplusplus
 }

@@ -3,7 +3,8 @@
 btle_tx.c from the reference sources compiled unmodified).  Run in the build container
 (needs the reference sources, BTLE_REFERENCE); the fixtures it writes are committed and travel to the GPU box.
 
-    python oracle/gen_golden.py
+    python oracle/gen_golden.py              (everything)
+    python oracle/gen_golden.py rejected     (only tests/golden/rejected_0.npz)
 """
 import json
 import os
@@ -48,9 +49,20 @@ def ref_tx(descriptor):
     return np.array([int(x) for x in re.findall(r"-?\d+", txt)], dtype=np.int8), out
 
 
+def rejected_cases():
+    """-v: full-scale noise on an advertising channel with a sparse mask (how unknown access addresses are looked for):
+    many hits whose header length is outside 6..37, which the reference rejects (PktBAD); chunk 7 has 30 of them."""
+    iq = np.random.default_rng(0).integers(-128, 128, 8 * 16384 + 3008, dtype=np.int8)
+    cfg = dict(channel=39, access_addr=0x8E89BED6, access_mask=0x0F000000, crc_init=0x555555, raw=0, report_rejected=1)
+    save("rejected_0.npz", iq, cfg)
+
+
 def main():
     os.makedirs(GOLD, exist_ok=True)
     subprocess.run(["make", "-C", os.path.join(ROOT, "oracle"), "ref", "oracle"], check=True, capture_output=True)
+    if sys.argv[1:] == ["rejected"]:                  # only the -v case
+        rejected_cases()
+        return
     # 1. tables / leaf known answers straight from the reference's own data
     kat = subprocess.run([orc.REF_DRIVER, "kat"], check=True, capture_output=True).stdout.decode()
     json.loads(kat)
@@ -100,6 +112,9 @@ def main():
     for i, cfg in enumerate(cases):
         iq = rng.integers(-128, 128, 4 * 16384 + 1234, dtype=np.int8)
         save(f"fuzz_{i}.npz", iq, cfg)
+
+    # 6. rejected hits (-v)
+    rejected_cases()
 
 
 if __name__ == "__main__":

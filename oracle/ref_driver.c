@@ -1,7 +1,9 @@
 /* Driver executable around oracle/_ref/libbtle_ref.so (the unmodified reference
  * receiver).  TEST INFRASTRUCTURE ONLY — see oracle/ref_wrap.c.
  *
- *   btle_ref_driver run  <iq.bin> <chan> <aa_hex> <crcinit_hex> <mask_hex> <raw> <out.rec>
+ *   btle_ref_driver run  <iq.bin> <chan> <aa_hex> <crcinit_hex> <mask_hex> <raw> <out.rec> [rejected]
+ *                                 ("rejected": also one record per hit rejected for its ADV header length, the
+ *                                  hits -v prints as PktBAD: nbytes 2, the two dewhitened header bytes)
  *   btle_ref_driver time <iq.bin> <chan> <aa_hex> <crcinit_hex> <mask_hex> <raw> <procs> <reps>
  *   btle_ref_driver sinks <iq.bin> <chan> <aa> <crcinit> <mask> <raw> <quiet> <json> <rssi> <pcap|-> <fadva|-> <fpdu|-> [verbose]
  *                                 (the reference's own text / NDJSON / pcap output for the capture)
@@ -32,6 +34,7 @@
 typedef struct { int32_t chunk, n0, nbytes, crc_bad; uint8_t bytes[48]; } ref_rec;
 
 extern void ref_note_demod(const int8_t *rxp, int num_byte);
+extern void ref_report_rejected(int on);
 extern long ref_run_chunks(const int8_t *iq, long k0, long k1, int channel, uint32_t aa, uint32_t mask,
                            uint32_t crc_init, int raw, ref_rec *out, long cap);
 extern long ref_run_sinks(const int8_t *iq, long k0, long k1, int channel, uint32_t aa, uint32_t mask, uint32_t crc_init,
@@ -105,8 +108,9 @@ int main(int argc, char **argv) {
   int raw = atoi(argv[7]);
   long nchunks = n_int8 / 16384;
   if (!strcmp(mode, "run")) {
-    long cap = nchunks * 64 + 16;   /* worst case is 51 per chunk (mask 0, include/btle_b200.h) */
+    long cap = nchunks * 123 + 16;  /* worst case is 123 per chunk (BTLE_MAX_RECS_PER_CHUNK, include/btle_b200.h) */
     ref_rec *out = (ref_rec *)calloc((size_t)cap, sizeof(ref_rec));
+    ref_report_rejected(argc > 9 && !strcmp(argv[9], "rejected"));
     long n = ref_run_chunks(iq, 0, nchunks, chan, aa, mask, crc, raw, out, cap);
     FILE *f = fopen(argv[8], "wb");
     fwrite(out, sizeof(ref_rec), (size_t)(n < cap ? n : cap), f);

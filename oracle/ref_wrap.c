@@ -38,9 +38,34 @@ static int g_chunk = 0, g_raw = 0, g_adv = 0;
 static const int8_t *g_chunk_base = 0;
 static const int8_t *g_hdr_ptr = 0;
 
+static int g_report_rejected = 0;
+void ref_report_rejected(int on) { g_report_rejected = on; }
+
+/* A header was demodulated and no packet was counted behind it: either receiver() rejected it for its ADV length
+ * (:2291-2298, printed as PktBAD under -v, the search goes on) or the length guard ended the chunk (:2308-2311).
+ * Called before the next header is demodulated and at the end of the chunk, when tmp_byte[0..1] still holds the
+ * dewhitened header; records the rejected ones (nbytes 2, the two header bytes) when asked to. */
+static void note_uncounted_header(void) {
+  if (!g_report_rejected || !g_hdr_ptr || g_raw || !g_adv) return;
+  const int plen = tmp_byte[1] & 0x3F;
+  if (plen >= 6 && plen <= 37) return;                 /* the length-guard break */
+  if (g_out && g_n < g_cap) {
+    ref_rec *r = &g_out[g_n];
+    memset(r, 0, sizeof(*r));
+    r->chunk = g_chunk;
+    r->n0 = (int32_t)((g_hdr_ptr - g_chunk_base) / 2 - 128);
+    r->nbytes = 2;
+    memcpy(r->bytes, tmp_byte, 2);
+  }
+  g_n++;
+}
+
 /* called by the interposed demod_byte() in the driver executable */
 void ref_note_demod(const int8_t *rxp, int num_byte) {
-  if (num_byte == 2 || (g_raw && num_byte == 42)) g_hdr_ptr = rxp;
+  if (num_byte == 2 || (g_raw && num_byte == 42)) {
+    note_uncounted_header();
+    g_hdr_ptr = rxp;
+  }
 }
 
 static long long g_virtual_us = 0;       /* hop mode: the time at which the chunk being processed was complete */
@@ -80,7 +105,8 @@ uint32_t ref_crc_init_reorder(uint32_t crc_init) { return crc_init_reorder(crc_i
 /* Replays main()'s chunking (btle_rx.c:2619-2651) over a linear buffer:
  * for k in [k0,k1): receiver(iq + 16384k, 248+16384, ...).  The caller must keep
  * >= 3010 readable int8 behind the last chunk.  Returns the number of packets
- * the reference counted (may exceed cap; only cap are stored). */
+ * the reference counted (may exceed cap; only cap are stored), plus the rejected
+ * hits after ref_report_rejected(1). */
 long ref_run_chunks(const int8_t *iq, long k0, long k1, int channel,
                     uint32_t access_addr, uint32_t access_mask, uint32_t crc_init,
                     int raw, ref_rec *out, long cap) {
@@ -97,6 +123,8 @@ long ref_run_chunks(const int8_t *iq, long k0, long k1, int channel,
     receiver_status.pkt_avaliable = 0;
     receiver((IQ_TYPE *)g_chunk_base, (LEN_DEMOD_BUF_ACCESS - 1) * 2 * SAMPLE_PER_SYMBOL + (LEN_BUF) / 2,
              channel, access_addr, crc_internal, 0, raw);      /* btle_rx.c:2651 */
+    note_uncounted_header();
+    g_hdr_ptr = 0;
   }
   g_chunk_base = 0;
   return g_n;

@@ -36,10 +36,11 @@ def lib():
 
 
 def rx_stream(iq, channel=37, access_addr=0x8E89BED6, access_mask=0xFFFFFFFF, crc_init=0x555555, raw=0, rssi=1,
-              stream=0, span_chunks=16):
+              stream=0, span_chunks=16, report_rejected=0):
+    """rssi: btle_stream_cfg flags (bit 0 RSSI, bit 1 report rejected hits); report_rejected=1 sets bit 1 as well."""
     iq = np.ascontiguousarray(iq, dtype=np.int8)
-    cfg = StreamCfg(channel, access_addr, access_mask, crc_init, raw, rssi)
-    cap = (iq.size // 16384) * 51 + 8      # BTLE_MAX_PKTS_PER_CHUNK
+    cfg = StreamCfg(channel, access_addr, access_mask, crc_init, raw, rssi | (2 if report_rejected else 0))
+    cap = (iq.size // 16384) * 123 + 8     # BTLE_MAX_RECS_PER_CHUNK
     out = np.zeros(cap, dtype=REC_DTYPE)
     n = lib().emul_rx_stream(iq.ctypes.data, iq.size, ctypes.byref(cfg), stream, span_chunks, out.ctypes.data, cap)
     assert n <= cap
@@ -51,7 +52,7 @@ def rx_batch_units(iq2d, cfgs, grid=132, reverse_units=False, force_walk=False):
     Returns (records as stored (block per unit), dir uint32 [n_units, 2])."""
     iq2d = np.ascontiguousarray(iq2d, dtype=np.int8)
     ns, n = iq2d.shape
-    cap = ns * (n // 16384) * 51 + 8
+    cap = ns * (n // 16384) * 123 + 8      # BTLE_MAX_RECS_PER_CHUNK
     out = np.zeros(cap, dtype=REC_DTYPE)
     dir_cap = ns * ((n // 16384 + 15) // 16) * 16 + 16
     d = np.zeros((dir_cap, 2), dtype=np.uint32)

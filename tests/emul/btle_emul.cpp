@@ -156,10 +156,14 @@ extern "C" long emul_rx_batch_units(const int8_t *iq, long n_streams, long strid
     // masks with more matches than a list holds, on the candidate words
     uint16_t xh[2 * kSpanChunks][kExactCap + 1];
     for (int t = 0; t < 2 * ui.nch; ++t) xh[t][kExactCap] = (uint16_t)enumerate_exact_hits(pd.data(), cand.data(), flagw[t], t, sp, xh[t]);
-    uint16_t hit[kSpanChunks][BTLE_MAX_PKTS_PER_CHUNK + kMaxRejectedPerChunk + 1];
+    constexpr int kHitCap = BTLE_MAX_PKTS_PER_CHUNK + kRejectedInHitRow + 1;    // the kernel's hit row; more hits are left to step 4
+    uint16_t hit[kSpanChunks][kHitCap];
     int mine[32] = {0};
     for (int lane = 0; lane < ui.nch; ++lane) {
-      struct Note { uint16_t *row; void operator()(int i, int n0, bool rej) { row[i] = (uint16_t)((n0 + 124) | (rej ? 0x8000 : 0)); } } note{hit[lane]};
+      struct Note {
+        uint16_t *row;
+        void operator()(int i, int n0, bool rej) { if (i < kHitCap) row[i] = (uint16_t)((n0 + 124) | (rej ? 0x8000 : 0)); }
+      } note{hit[lane]};
       const uint32_t *pdc = &pd[4 * (size_t)(kGroupsPerChunk * lane)];
       const int c0 = xh[2 * lane][kExactCap], c1 = xh[2 * lane + 1][kExactCap];
       if (c0 > kExactCap || c1 > kExactCap || force_walk)
@@ -178,6 +182,7 @@ extern "C" long emul_rx_batch_units(const int8_t *iq, long n_streams, long strid
       int c = 0;
       for (int step = kSpanChunks / 2; step >= 1; step >>= 1)
         if ((int)pre[c + step] <= j) c += step;
+      if (j - (int)pre[c] >= kHitCap) continue;           // behind the chunk's row: step 4
       const int h = (int)hit[c][j - (int)pre[c]];
       const bool rej = (h & 0x8000) != 0;
       const int n0 = (h & 0x7FFF) - 124;
@@ -188,6 +193,25 @@ extern "C" long emul_rx_batch_units(const int8_t *iq, long n_streams, long strid
         HostEmit e{out + base + j, 1, 0, ui.stream, ui.chunk0 + c, &sp, cap_base, n_int8, (long)(ui.chunk0 + c) * kChunkInt8};
         e(n0, nbytes, crc_bad, words, rej);
       }
+    }
+    // step 4: a chunk with more hits than its row holds runs its chain again and stores hits kHitCap.. itself
+    for (int lane = 0; lane < ui.nch; ++lane) {
+      if (!sp.report_rejected || mine[lane] <= kHitCap) continue;
+      const uint32_t *pdc = &pd[4 * (size_t)(kGroupsPerChunk * lane)];
+      const long first = base + pre[lane];
+      auto late = [&](int i, int n0, bool rej) {
+        if (i < kHitCap || first + i >= cap) return;
+        uint32_t words[11];
+        int nbytes, crc_bad;
+        decode_packet(pdc, sp, crc4, n0, rej, words, nbytes, crc_bad);
+        HostEmit e{out + first + i, 1, 0, ui.stream, ui.chunk0 + lane, &sp, cap_base, n_int8, (long)(ui.chunk0 + lane) * kChunkInt8};
+        e(n0, nbytes, crc_bad, words, rej);
+      };
+      const int c0 = xh[2 * lane][kExactCap], c1 = xh[2 * lane + 1][kExactCap];
+      if (c0 > kExactCap || c1 > kExactCap || force_walk)
+        chain_chunk(pdc, &cand[(size_t)kGroupsPerChunk * lane], &flagw[2 * (size_t)lane], sp, late);
+      else
+        chain_chunk_lists(pdc, xh[2 * lane], c0, xh[2 * lane + 1], c1, sp, late);
     }
   }
   return count;

@@ -26,7 +26,17 @@ def assert_matches_golden(rec, z):
         assert a["chunk"] == z["exp_chunk"][i] and a["n0"] == z["exp_n0"][i], (i, a["chunk"], a["n0"])
         nb = int(z["exp_nbytes"][i])
         assert a["n_bytes"] == nb and a["crc_bad"] == z["exp_crc_bad"][i], i
+        assert bool(a["flags"] & 4) == (nb == 2), i          # a rejected hit (-v) is the only header-only record
         assert bytes(a["bytes"][:nb]) == bytes(z["exp_bytes"][i][:nb]), i
+
+
+def rx_cfg(cfg):
+    """A golden case's configuration as keywords of BtleRx.rx / make_cfgs: report_rejected becomes flag bit 1
+    (BTLE_CFG_REPORT_REJECTED) of `rssi`."""
+    cfg = dict(cfg)
+    if cfg.pop("report_rejected", 0):
+        cfg["rssi"] = 2
+    return cfg
 
 
 def tables():

@@ -58,19 +58,35 @@ def lib():
         _lib.orc_rx_stream.restype = ctypes.c_long
         _lib.orc_rx_stream.argtypes = [ctypes.c_void_p, ctypes.c_long, ctypes.POINTER(OrcCfg), ctypes.c_int32,
                                        ctypes.c_void_p, ctypes.c_long]
+        _lib.orc_rx_stream_ex.restype = ctypes.c_long
+        _lib.orc_rx_stream_ex.argtypes = [ctypes.c_void_p, ctypes.c_long, ctypes.POINTER(OrcCfg), ctypes.c_int, ctypes.c_int32,
+                                          ctypes.c_void_p, ctypes.c_long]
     return _lib
 
 
+MAX_RECS_PER_CHUNK = 123                   # BTLE_MAX_RECS_PER_CHUNK (include/btle_b200.h)
+
+
 def rx_stream(iq: np.ndarray, channel=37, access_addr=0x8E89BED6, access_mask=0xFFFFFFFF, crc_init=0x555555,
-              raw=0, stream=0) -> np.ndarray:
-    """Our C restatement over one capture -> REC_DTYPE array in reference order."""
+              raw=0, stream=0, report_rejected=0) -> np.ndarray:
+    """Our C restatement over one capture -> REC_DTYPE array in reference order.  report_rejected (-v): the ADV hits
+    the reference prints as PktBAD come back too, as header-only records with flags bit 2 set."""
     iq = np.ascontiguousarray(iq, dtype=np.int8)
     cfg = OrcCfg(channel, access_addr, access_mask, crc_init, raw)
-    cap = (iq.size // 16384) * 51 + 8      # BTLE_MAX_PKTS_PER_CHUNK
+    cap = (iq.size // 16384) * MAX_RECS_PER_CHUNK + 8
     out = np.zeros(cap, dtype=REC_DTYPE)
-    n = lib().orc_rx_stream(iq.ctypes.data, iq.size, ctypes.byref(cfg), stream, out.ctypes.data, cap)
+    n = lib().orc_rx_stream_ex(iq.ctypes.data, iq.size, ctypes.byref(cfg), int(bool(report_rejected)), stream, out.ctypes.data, cap)
     assert n <= cap
     return out[:n]
+
+
+def rx_flags(iq: np.ndarray, flags: int, **cfg) -> np.ndarray:
+    """The oracle's records as the GPU returns them for btle_stream_cfg.rssi == flags: bit 0 (BTLE_CFG_RSSI) keeps
+    mag_sum (else 0), bit 1 (BTLE_CFG_REPORT_REJECTED) adds the rejected hits."""
+    rec = rx_stream(iq, report_rejected=(flags >> 1) & 1, **cfg)
+    if not flags & 1:
+        rec["mag_sum"] = 0
+    return rec
 
 
 def dbits(iq: np.ndarray) -> np.ndarray:
@@ -87,14 +103,15 @@ def ref_available() -> bool:
 
 
 def ref_rx_stream(iq: np.ndarray, channel=37, access_addr=0x8E89BED6, access_mask=0xFFFFFFFF, crc_init=0x555555,
-                  raw=0) -> np.ndarray:
-    """The unmodified reference receiver() over one capture -> REF_DTYPE array."""
+                  raw=0, report_rejected=0) -> np.ndarray:
+    """The unmodified reference receiver() over one capture -> REF_DTYPE array.  report_rejected: also the hits it
+    rejects for their ADV header length (what -v prints as PktBAD), as records with nbytes 2 and the two header bytes."""
     iq = np.ascontiguousarray(iq, dtype=np.int8)
     with tempfile.TemporaryDirectory() as td:
         fi, fo = os.path.join(td, "iq.bin"), os.path.join(td, "out.rec")
         iq.tofile(fi)
         subprocess.run([REF_DRIVER, "run", fi, str(channel), f"{access_addr:x}", f"{crc_init:x}", f"{access_mask:x}",
-                        str(int(raw)), fo], check=True, capture_output=True)
+                        str(int(raw)), fo] + (["rejected"] if report_rejected else []), check=True, capture_output=True)
         return np.fromfile(fo, dtype=REF_DTYPE)
 
 
@@ -112,5 +129,6 @@ def assert_same_as_ref(rec: np.ndarray, ref: np.ndarray):
     for a, b in zip(rec, ref):
         assert a["chunk"] == b["chunk"] and a["n0"] == b["n0"], (a["chunk"], a["n0"], b["chunk"], b["n0"])
         assert a["n_bytes"] == b["nbytes"] and a["crc_bad"] == b["crc_bad"]
+        assert bool(a["flags"] & 4) == (b["nbytes"] == 2), (a["chunk"], a["n0"])    # rejected hit <=> header only
         nb = int(b["nbytes"])
         assert bytes(a["bytes"][:nb]) == bytes(b["bytes"][:nb])

@@ -180,6 +180,28 @@ def test_cli_verbose_prints_the_reference_pktbad_lines(tmp_path):
 
 @pytest.mark.gpu
 @pytest.mark.skipif(not orc.ref_available(), reason="oracle/_ref not built")
+@pytest.mark.parametrize("kind", ["zero_mask0", "noise_sparse_mask"])
+def test_cli_verbose_reports_every_pktbad_line(tmp_path, kind):
+    """-v with degenerate and sparse masks: every rejected hit is printed, in the reference's order.  The zero capture with
+    mask 0 on channel 38 has 123 of them per chunk (BTLE_MAX_RECS_PER_CHUNK)."""
+    if kind == "zero_mask0":
+        iq, ch, aa, mask = np.zeros(3 * 16384 + 3008, dtype=np.int8), 38, 0, 0
+    else:
+        iq, ch, aa, mask = np.random.default_rng(0).integers(-128, 128, 8 * 16384 + 3008, dtype=np.int8), 39, 0x8E89BED6, 0x0F000000
+    f = tmp_path / "iq.bin"
+    iq.tofile(f)
+    p = run(["-i", str(f), "-c", str(ch), "-a", f"{aa:x}", "-m", f"{mask:x}", "-v", "-j"])
+    assert p.returncode == 0, p.stdout + p.stderr
+    q = subprocess.run([orc.REF_DRIVER, "sinks", str(f), str(ch), f"{aa:x}", "555555", f"{mask:x}", "0", "0", "1", "0", "-", "-", "-", "1"],
+                       capture_output=True, text=True, check=True)
+    mine, ref = _normalise_text(p.stdout), _normalise_text(q.stdout)
+    n_bad = sum(l.startswith("XXXus PktBAD") for l in ref)
+    assert n_bad == (3 * 123 if kind == "zero_mask0" else 97)
+    assert mine == ref
+
+
+@pytest.mark.gpu
+@pytest.mark.skipif(not orc.ref_available(), reason="oracle/_ref not built")
 def test_cli_hop_follows_the_connection_like_the_reference(tmp_path):
     """-o over per-channel captures (--iq-dir): text lines, packet events and hop events equal what the UNMODIFIED reference
     prints when its receiver() + receiver_controller() drive a virtual radio over the same 40 captures (oracle/_ref hop)."""

@@ -31,12 +31,14 @@ def _same(a, b):
 @pytest.mark.parametrize("name", G.cases())
 def test_gpu_matches_reference_golden(rx, name):
     z, cfg = G.load(name)
-    rec = rx.rx(z["iq"], **cfg)
+    rec = rx.rx(z["iq"], **G.rx_cfg(cfg))
     G.assert_matches_golden(rec, z)
 
 
 @pytest.mark.parametrize("seed", range(8))
 def test_gpu_equals_oracle_on_adversarial_fuzz(rx, seed):
+    """Sparse masks on full-scale noise; flags (RSSI, -v rejected hits) rotate through 1, 2, 3 with the seed."""
+    flags = (1, 2, 3)[seed % 3]
     rng = np.random.default_rng(1000 + seed)
     iq = rng.integers(-128, 128, 40 * 16384 + int(rng.integers(0, 16384)), dtype=np.int8)
     masks = [0x0000000F, 0x000000FF, 0x80000001, 0x00000000, 0xF0000000, 0x00010100, 0x0000FFFF, 0xFFFF0000]
@@ -44,7 +46,7 @@ def test_gpu_equals_oracle_on_adversarial_fuzz(rx, seed):
     for ch in (37, 5):
         for raw in (0, 1):
             cfg = dict(channel=ch, access_addr=aas[seed], access_mask=masks[seed], raw=raw, crc_init=0x123456)
-            _same(rx.rx(iq, rssi=1, **cfg), orc.rx_stream(iq, **cfg))
+            _same(rx.rx(iq, rssi=flags, **cfg), orc.rx_flags(iq, flags, **cfg))
 
 
 def test_gpu_equals_oracle_on_synth_streams(rx):
@@ -68,7 +70,7 @@ def test_gpu_ragged_empty_and_tiny(rx):
 def test_gpu_batch_of_40_channels(rx):
     """SURVEY §8d C3 in miniature: one stream per BLE channel, per-channel AA / CRCInit."""
     n = 20 * 16384
-    iqs, cfgs, exp = [], make_cfgs(40, rssi=1), []
+    iqs, cfgs, exp = [], make_cfgs(40), []
     for ch in range(40):
         adv = ch >= 37
         aa = 0x8E89BED6 if adv else 0x60850A1B + ch
@@ -76,8 +78,11 @@ def test_gpu_batch_of_40_channels(rx):
         iq, _ = synth.make_adv_stream(n, seed=1000 + ch, channel=ch, access_addr=aa, crc_init=ci,
                                       data_channel_pdu=not adv, corrupt_every=10, slot_samples=3000)
         iqs.append(iq.numpy())
-        cfgs[ch]["channel"], cfgs[ch]["access_addr"], cfgs[ch]["crc_init"] = ch, aa, ci
-        exp.append(orc.rx_stream(iqs[-1], channel=ch, access_addr=aa, crc_init=ci, stream=ch))
+        cfgs[ch]["channel"], cfgs[ch]["access_addr"], cfgs[ch]["crc_init"], cfgs[ch]["rssi"] = ch, aa, ci, ch % 4
+        if ch in (38, 39):                                                  # sparse mask: rejected hits with -v
+            cfgs[ch]["access_mask"] = 0x0F000000
+        exp.append(orc.rx_flags(iqs[-1], ch % 4, channel=ch, access_addr=aa, access_mask=int(cfgs[ch]["access_mask"]), crc_init=ci,
+                                stream=ch))
     got = rx.rx_batch(np.stack(iqs), cfgs)
     exp = np.concatenate(exp)
     assert len(exp) > 40 * 40
@@ -92,11 +97,12 @@ def test_gpu_randomised_configs_with_planted_bursts(rx):
     n_streams, nchunks = 48, 6
     n = nchunks * 16384 + 2500
     iq = np.zeros((n_streams, n), dtype=np.int8)
-    cfgs, exp = make_cfgs(n_streams, rssi=1), []
+    cfgs, exp = make_cfgs(n_streams), []
     for s in range(n_streams):
         ch = int(rng.integers(0, 40))
+        flags = int(rng.integers(0, 4))
         aa = int(rng.integers(0, 2**32))
-        mask = [0xFFFFFFFF, 0xFFFFFFFF, 0xFFFFFF00, 0x0FFFFFFF, 0xFFFF0000][s % 5]
+        mask = [0xFFFFFFFF, 0xFFFFFFFF, 0xFFFFFF00, 0x0FFFFFFF, 0xFFFF0000, 0x0F000000][s % 6]
         ci = int(rng.integers(0, 2**24))
         raw = int(s % 6 == 5)
         bg = rng.integers(-128, 128, n, dtype=np.int8) if s % 4 == 1 else rng.integers(-3, 4, n, dtype=np.int8)
@@ -112,8 +118,8 @@ def test_gpu_randomised_configs_with_planted_bursts(rx):
             bg[p2:p2 + m] = wav[:m] // 2
         iq[s] = bg
         c = cfgs[s]
-        c["channel"], c["access_addr"], c["access_mask"], c["crc_init"], c["raw"] = ch, aa, mask, ci, raw
-        exp.append(orc.rx_stream(bg, channel=ch, access_addr=aa, access_mask=mask, crc_init=ci, raw=raw, stream=s))
+        c["channel"], c["access_addr"], c["access_mask"], c["crc_init"], c["raw"], c["rssi"] = ch, aa, mask, ci, raw, flags
+        exp.append(orc.rx_flags(bg, flags, channel=ch, access_addr=aa, access_mask=mask, crc_init=ci, raw=raw, stream=s))
     exp = np.concatenate(exp)
     got = rx.rx_batch(iq, cfgs)
     assert len(exp) > 200
@@ -127,7 +133,7 @@ def test_gpu_many_short_streams(rx):
     for n_streams, nchunks in ((5, 1), (300, 2), (700, 3)):
         n = nchunks * 16384 + 4000
         iq = np.zeros((n_streams, n), dtype=np.int8)
-        cfgs, exp = make_cfgs(n_streams, rssi=1), []
+        cfgs, exp = make_cfgs(n_streams), []
         base, _ = synth.make_adv_stream(n, seed=9, channel=37, slot_samples=2600)
         base = base.numpy()
         for s in range(n_streams):
@@ -136,8 +142,8 @@ def test_gpu_many_short_streams(rx):
             if s % 7 == 3:
                 iq[s] = rng.integers(-128, 128, n, dtype=np.int8)
                 cfgs[s]["access_mask"] = 0x0000FFFF if s % 2 else 0x80000001
-            cfgs[s]["channel"] = ch
-            exp.append(orc.rx_stream(iq[s], channel=ch, access_mask=int(cfgs[s]["access_mask"]), stream=s))
+            cfgs[s]["channel"], cfgs[s]["rssi"] = ch, s % 4
+            exp.append(orc.rx_flags(iq[s], s % 4, channel=ch, access_mask=int(cfgs[s]["access_mask"]), stream=s))
         got = rx.rx_batch(iq, cfgs)
         _same(got, np.concatenate(exp))
 
@@ -149,7 +155,14 @@ def test_gpu_sc16q11_ingest(rx):
     iq16 = (iq8.numpy().astype(np.int16) << 4) | rng.integers(0, 16, iq8.numel(), dtype=np.int16)    # 12-bit samples
     iq16[::97] = rng.integers(-32768, 32767, iq16[::97].size, dtype=np.int16)                        # out-of-range junk wraps
     conv = ((iq16 >> 4) & 0xFF).astype(np.uint8).view(np.int8)
-    _same(rx.rx_iq16(iq16, 4, channel=38, rssi=1), orc.rx_stream(conv, channel=38))
+    for flags in (1, 2, 3):
+        _same(rx.rx_iq16(iq16, 4, channel=38, rssi=flags), orc.rx_flags(conv, flags, channel=38))
+    noise = rng.integers(-32768, 32767, 10 * 16384, dtype=np.int16)
+    conv = ((noise >> 4) & 0xFF).astype(np.uint8).view(np.int8)
+    for flags in (2, 3):
+        exp = orc.rx_flags(conv, flags, channel=39, access_mask=0x0F000000)
+        assert (exp["flags"] & 4).any()
+        _same(rx.rx_iq16(noise, 4, channel=39, access_mask=0x0F000000, rssi=flags), exp)
 
 
 def test_gpu_overflow_reports_needed_count(rx):
@@ -282,24 +295,29 @@ def test_gpu_unit_directory_walk_is_reference_order(rx):
     """rx_device_dir: one block per unit + directory; walking the directory equals the oracle's order, the sum of the
     directory counts equals the device counter, and every directory entry of the launch is written."""
     from btle_b200 import REC_DTYPE, DIR_DTYPE
-    ns, n = 3, 70 * 16384 + 500
+    ns, n = 4, 70 * 16384 + 500
     iq = np.zeros((ns, n), dtype=np.int8)
-    cfgs = make_cfgs(ns, rssi=1)
+    cfgs = make_cfgs(ns)
     exp = []
     for s_ in range(ns):
-        ch = [37, 9, 39][s_]
+        ch = [37, 9, 39, 38][s_]
         aa = 0x8E89BED6 if ch >= 37 else 0x60850A1B + ch
         ci = 0x555555 if ch >= 37 else 0xA77B22 ^ ch
         t, _ = synth.make_adv_stream(n, seed=300 + s_, channel=ch, access_addr=aa, crc_init=ci, corrupt_every=7, slot_samples=2100,
                                      data_channel_pdu=ch < 37, straddle_every=3)
         iq[s_] = t.numpy()
-        cfgs[s_]["channel"], cfgs[s_]["access_addr"], cfgs[s_]["crc_init"] = ch, aa, ci
-        exp.append(orc.rx_stream(iq[s_], channel=ch, access_addr=aa, crc_init=ci, stream=s_))
+        mask, flags = 0xFFFFFFFF, [1, 2, 3, 3][s_]
+        if s_ == 3:                                       # -v with a sparse mask on noise: rejected records in the blocks
+            iq[s_] = np.random.default_rng(5).integers(-128, 128, n, dtype=np.int8)
+            mask = 0x0F000000
+        cfgs[s_]["channel"], cfgs[s_]["access_addr"], cfgs[s_]["crc_init"], cfgs[s_]["access_mask"], cfgs[s_]["rssi"] = ch, aa, ci, mask, flags
+        exp.append(orc.rx_flags(iq[s_], flags, channel=ch, access_addr=aa, access_mask=mask, crc_init=ci, stream=s_))
     exp = np.concatenate(exp)
+    assert int(((exp["flags"] & 4) != 0).sum()) > 100
     d_iq = torch.zeros((ns, (n + 15) // 16 * 16), dtype=torch.int8, device="cuda")
     d_iq[:, :n] = torch.from_numpy(iq).cuda()
     units = rx.units(ns, n)
-    assert units > 3 * 5
+    assert units > ns * 5
     cap = len(exp) + 8
     d_out = torch.zeros(cap * 64, dtype=torch.uint8, device="cuda")
     d_dir = torch.full((units + 4, 2), -1, dtype=torch.int32, device="cuda")
@@ -356,3 +374,40 @@ def test_gpu_stream_session_equals_whole_capture(rx):
             parts.append(s_.finish())
         got = np.concatenate(parts)
         _same(got, exp)
+    # -v with a sparse mask on noise (rejected records in every segment), RSSI on and off
+    iq = np.random.default_rng(8).integers(-128, 128, 12 * 16384 + 777, dtype=np.int8)
+    for seg, flags in ((1, 3), (5, 2), (5, 3)):
+        exp = orc.rx_flags(iq, flags, channel=39, access_mask=0x0F000000)
+        assert int(((exp["flags"] & 4) != 0).sum()) > 50
+        with rx.stream(segment_chunks=seg, channel=39, access_mask=0x0F000000, rssi=flags) as s_:
+            got = np.concatenate([s_.push(iq[:70000]), s_.push(iq[70000:]), s_.finish()])
+        _same(got, exp)
+
+
+def test_gpu_worst_case_rejected_hits_per_chunk(rx):
+    """-v on the zero capture with mask 0 on channel 38: every window matches, every header has an impossible ADV length,
+    so each chunk returns BTLE_MAX_RECS_PER_CHUNK = 123 rejected records, more than the resolver's hit rows hold.  Through
+    rx (default capacity of 34 per chunk -> BTLE_EOVERFLOW -> retry), rx_device_dir and a stream session."""
+    from btle_b200 import REC_DTYPE, DIR_DTYPE
+    nch = 20
+    z = np.zeros(nch * 16384 + 3008, dtype=np.int8)
+    cfg = dict(channel=38, access_addr=0, access_mask=0)
+    for flags in (2, 3):
+        exp = orc.rx_flags(z, flags, **cfg)
+        assert len(exp) == nch * 123 and (exp["flags"] & 4).all()
+        _same(rx.rx(z, rssi=flags, **cfg), exp)
+        cfgs = make_cfgs(1, rssi=flags, **cfg)
+        d_iq = torch.zeros((1, (z.size + 15) // 16 * 16), dtype=torch.int8, device="cuda")
+        units = rx.units(1, z.size)
+        d_out = torch.zeros(len(exp) * 64, dtype=torch.uint8, device="cuda")
+        d_dir = torch.zeros((units, 2), dtype=torch.int32, device="cuda")
+        d_count = torch.zeros(1, dtype=torch.int32, device="cuda")
+        rx.rx_device_dir(d_iq[:, :z.size], cfgs, d_out, d_count, d_dir, torch.cuda.current_stream().cuda_stream)
+        torch.cuda.synchronize()
+        unit_dir = np.ascontiguousarray(d_dir.cpu().numpy().view(np.uint32)).view(DIR_DTYPE).reshape(-1)
+        assert int(unit_dir["count"].sum()) == int(d_count.item()) == len(exp)
+        _same(rx.gather_ordered(d_out.cpu().numpy().view(REC_DTYPE), unit_dir), exp)
+        for seg in (1, 5):
+            with rx.stream(segment_chunks=seg, rssi=flags, **cfg) as s_:
+                got = np.concatenate([s_.push(z), s_.finish()])
+            _same(got, exp)

@@ -202,3 +202,53 @@ def test_dense_loop_discriminator_is_exact_for_every_int8_input():
     checked on the PTX ISA's semantics of prmt / dp2a / dp4a (the instructions themselves are checked by the GPU parity tests;
     the emulator's unit path runs the same arithmetic against the oracle in the tests above)."""
     assert emul.check_discriminator() == 0
+
+
+# ---- -v: rejected hits (flags 2 and 3) ---------------------------------------------------------------------------------
+def _rejected_cases(rng):
+    """(iq, cfg) pairs with many rejected hits: the zero capture with mask 0 (123 per chunk on channels 38 / 39, more than
+    a hit row holds), full-scale noise with sparse masks, planted bad-length headers, and configs where -v changes nothing."""
+    z = np.zeros(3 * 16384 + 3008, dtype=np.int8)
+    out = [(z, dict(channel=ch, access_addr=0, access_mask=0)) for ch in (37, 38, 39)]
+    noise = np.random.default_rng(0).integers(-128, 128, 8 * 16384 + 3008, dtype=np.int8)
+    for mask in (0x00000000, 0x0000000F, 0x80000001, 0x0F000000, 0x000000FF):
+        out.append((noise, dict(channel=int(rng.choice([37, 38, 39])), access_mask=mask)))
+    out.append((noise, dict(channel=7, access_mask=0x0F000000)))
+    out.append((noise, dict(channel=38, access_mask=0x000000FF, raw=1)))
+    pdus = [synth.adv_pdu(0, 1, 0, bytes(range(6 + k))) for k in range(6)]
+    pdus.insert(1, synth.adv_pdu(0, 1, 0, b"\x01\x02\x03"))
+    pdus.insert(4, bytes([0x02, 45]) + bytes(range(20)))
+    out.append((synth.make_pdu_stream(pdus, 39, seed=9, corrupt={2}), dict(channel=39)))
+    return out
+
+
+@pytest.mark.parametrize("flags", [2, 3])
+def test_emul_rejected_hits_equal_oracle_per_chunk(flags):
+    for iq, cfg in _rejected_cases(np.random.default_rng(flags)):
+        for span in (1, 5, 16):
+            _same(emul.rx_stream(iq, rssi=flags, span_chunks=span, **cfg), orc.rx_flags(iq, flags, **cfg))
+
+
+@pytest.mark.parametrize("flags", [2, 3])
+@pytest.mark.parametrize("grid", [1, 5, 132])
+def test_emul_resolver_passes_report_every_rejected_hit(flags, grid):
+    """The kernel's chain pass keeps 68 hits per chunk; with -v a chunk may have up to 123 (BTLE_MAX_RECS_PER_CHUNK).  Through the
+    exact-hit lists and the candidate walk (force_walk), every unit finishing order: all of them, equal to the oracle."""
+    from btle_b200._native import CFG_DTYPE
+    cases = _rejected_cases(np.random.default_rng(10 * grid + flags))
+    n = max(iq.size for iq, _ in cases)
+    iq2d = np.zeros((len(cases), n), dtype=np.int8)
+    cfgs = np.zeros(len(cases), dtype=CFG_DTYPE)
+    exp = []
+    for s_, (iq, cfg) in enumerate(cases):
+        iq2d[s_, :iq.size] = iq
+        full = dict(channel=37, access_addr=0x8E89BED6, access_mask=0xFFFFFFFF, crc_init=0x555555, raw=0)
+        full.update(cfg)
+        cfgs[s_] = (full["channel"], full["access_addr"], full["access_mask"], full["crc_init"], full["raw"], flags)
+        exp.append(orc.rx_flags(iq2d[s_], flags, stream=s_, **full))
+    exp = np.concatenate(exp)
+    assert int(np.bincount(exp["chunk"][exp["stream"] == 1]).max()) == 123
+    for kw in (dict(), dict(reverse_units=True), dict(force_walk=True)):
+        rec, d = emul.rx_batch_units(iq2d, cfgs, grid=grid, **kw)
+        assert int(d[:, 1].sum()) == len(rec) == len(exp)
+        _same(_walk(rec, d), exp)

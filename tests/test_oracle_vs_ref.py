@@ -95,3 +95,66 @@ def test_worst_case_packets_per_chunk():
         for ch in (1, 9, 20):
             rec = _cmp(iq, channel=ch, access_addr=1, access_mask=1)
             assert len(rec) > 10 and int(np.bincount(rec["chunk"]).max()) <= 34
+
+
+# ---- -v: hits the reference rejects for their ADV header length (PktBAD, btle_rx.c:2291-2298) -------------------------
+def _cmp_rejected(iq, **cfg):
+    """Oracle with report_rejected against the reference's counted packets and rejected hits, in the reference's order."""
+    rec = orc.rx_stream(iq, report_rejected=1, **cfg)
+    orc.assert_same_as_ref(rec, orc.ref_rx_stream(iq, report_rejected=1, **cfg))
+    rej = rec[(rec["flags"] & 4) != 0]
+    assert (rej["n_bytes"] == 2).all() and not rej["crc_bad"].any() and not rej["bytes"][:, 2:].any()
+    assert rec[(rec["flags"] & 4) == 0].tobytes() == orc.rx_stream(iq, **cfg).tobytes()     # the flag only adds records
+    mag = [int(np.abs(iq[16384 * r["chunk"] + 2 * r["n0"]:][:256].astype(np.int32)).sum()) & 0xFFFF
+           for r in rej if 16384 * r["chunk"] + 2 * r["n0"] >= 0]
+    assert mag == [int(r["mag_sum"]) for r in rej if 16384 * r["chunk"] + 2 * r["n0"] >= 0]   # summed before the length check
+    return rec
+
+
+@needs_ref
+def test_rejected_hits_zero_capture_mask0_worst_case():
+    """Mask 0 on zeros: every window matches through the zeroed history, every header is the channel's whitening
+    sequence.  On channels 38 and 39 its length is outside 6..37: BTLE_MAX_RECS_PER_CHUNK = 123 rejected hits per chunk."""
+    z = np.zeros(3 * 16384 + 3008, dtype=np.int8)
+    for ch in (37, 38, 39):
+        rec = _cmp_rejected(z, channel=ch, access_addr=0, access_mask=0)
+        if ch != 37:
+            assert len(rec) == 3 * 123 and (rec["flags"] & 4).all()
+            assert list(np.bincount(rec["chunk"])) == [123] * 3
+
+
+@needs_ref
+@pytest.mark.parametrize("mask", [0x00000000, 0x0000000F, 0x80000001, 0x0F000000, 0x000000FF])
+def test_rejected_hits_noise_sparse_masks(mask):
+    rng = np.random.default_rng(mask & 0xFFFF)
+    iq = rng.integers(-128, 128, 8 * 16384 + 3008, dtype=np.int8)
+    n_rej = 0
+    for ch in (37, 38, 39):
+        rec = _cmp_rejected(iq, channel=ch, access_mask=mask)
+        n_rej += int(((rec["flags"] & 4) != 0).sum())
+    assert n_rej > 20
+
+
+@needs_ref
+def test_rejected_hits_planted_bad_lengths():
+    """Bursts whose ADV header says PloadL 3, 45 and 5 between valid ones, on a quiet floor, with the full mask."""
+    pdus = [synth.adv_pdu(0, 1, 0, bytes(range(6 + k))) for k in range(6)]
+    pdus.insert(1, synth.adv_pdu(0, 1, 0, b"\x01\x02\x03"))
+    pdus.insert(4, bytes([0x02, 45]) + bytes(range(20)))
+    pdus.append(synth.adv_pdu(6, 0, 1, bytes(5)))
+    for ch in (37, 39):
+        iq = synth.make_pdu_stream(pdus, ch, seed=9, corrupt={2})
+        rec = _cmp_rejected(iq, channel=ch)
+        rej = rec[(rec["flags"] & 4) != 0]
+        assert len(rej) == 3 and sorted(int(b[1]) & 0x3F for b in rej["bytes"]) == [3, 5, 45]
+        assert len(rec) == len(pdus)
+
+
+@needs_ref
+def test_rejected_flag_changes_nothing_on_data_channels_and_raw():
+    rng = np.random.default_rng(17)
+    iq = rng.integers(-128, 128, 6 * 16384 + 3008, dtype=np.int8)
+    for ch, raw in ((3, 0), (20, 0), (37, 1), (39, 1)):
+        for mask in (0, 0x0F000000):
+            rec = _cmp_rejected(iq, channel=ch, access_mask=mask, raw=raw)
+            assert len(rec) > 5 and not (rec["flags"] & 4).any()

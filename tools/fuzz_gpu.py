@@ -1,11 +1,11 @@
 #!/usr/bin/env python
 """GPU fuzz: the CUDA path through the C-ABI vs the oracle on random access addresses / masks / channels /
-CRC inits / raw mode and a mix of input kinds, several captures per batch.  FUZZ_SECONDS (default 120)."""
+CRC inits / raw mode / flags (RSSI, rejected hits) and a mix of input kinds, several captures per batch.  FUZZ_SECONDS (default 120)."""
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import numpy as np
-import orc
+from oracle_flags import expect
 from btle_b200 import BtleRx, CFG_DTYPE, synth
 
 rx = BtleRx(0)
@@ -43,10 +43,10 @@ while time.time() - t0 < float(os.environ.get("FUZZ_SECONDS", "120")):
         else:
             period = int(rng.choice([2, 4, 6, 8, 16, 64]))
             iq[s] = np.resize(rng.integers(-100, 101, period, dtype=np.int8), n)
-        cfgs[s] = (ch, aa, mask, crc_init, int(rng.integers(0, 4) == 0), 1)
-    exp = np.concatenate([orc.rx_stream(iq[s], channel=int(cfgs[s]["channel"]), access_addr=int(cfgs[s]["access_addr"]),
-                                        access_mask=int(cfgs[s]["access_mask"]), crc_init=int(cfgs[s]["crc_init"]),
-                                        raw=int(cfgs[s]["raw"]), stream=s) for s in range(ns)])
+        cfgs[s] = (ch, aa, mask, crc_init, int(rng.integers(0, 4) == 0), int(rng.integers(0, 4)))   # flags: RSSI, -v rejected hits
+    exp = np.concatenate([expect(iq[s], int(cfgs[s]["rssi"]), channel=int(cfgs[s]["channel"]), access_addr=int(cfgs[s]["access_addr"]),
+                                       access_mask=int(cfgs[s]["access_mask"]), crc_init=int(cfgs[s]["crc_init"]),
+                                       raw=int(cfgs[s]["raw"]), stream=s) for s in range(ns)])
     got = rx.rx_batch(iq, cfgs)
     assert got.tobytes() == exp.tobytes(), ("GPU != oracle", ns, n, cfgs.tolist(), len(got), len(exp))
     n_case += 1; n_pkt += len(exp)

@@ -5,7 +5,7 @@ import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
 import numpy as np, torch
-import orc
+from oracle_flags import expect
 from btle_b200 import BtleRx, make_cfgs, synth, REC_DTYPE
 
 rx = BtleRx(0)
@@ -19,8 +19,10 @@ while time.time() - t0 < float(os.environ.get("STRESS_SECONDS", "120")):
     base, _ = synth.make_adv_stream(n, seed=int(rng.integers(0, 1 << 30)), channel=37, slot_samples=int(rng.choice([1600, 2400, 4096])))
     base = base.numpy()
     iq = np.stack([np.roll(base, 2 * int(rng.integers(0, 3000))) for _ in range(n_streams)])
-    cfgs = make_cfgs(n_streams, rssi=1)
-    exp = np.concatenate([orc.rx_stream(iq[s], stream=s) for s in range(n_streams)])
+    flags = int(rng.integers(0, 4))                       # RSSI, -v rejected hits (more of them with the sparse mask)
+    mask = int(rng.choice([0xFFFFFFFF, 0x0F000000]))
+    cfgs = make_cfgs(n_streams, access_mask=mask, rssi=flags)
+    exp = np.concatenate([expect(iq[s], flags, access_mask=mask, stream=s) for s in range(n_streams)])
     got = rx.rx_batch(iq, cfgs)
     assert got.tobytes() == exp.tobytes(), (n_streams, nchunks, len(got), len(exp))
     ncase += 1
