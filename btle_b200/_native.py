@@ -50,7 +50,9 @@ EXPORTS = [
     "btle_b200_scramble_bits", "btle_b200_model_rx_batch_device", "btle_b200_model_rx_batch",
     "btle_b200_tx_modulate_device", "btle_b200_rx_iq16", "btle_b200_synth_streams_device", "btle_b200_rx_sps8", "btle_b200_sps8_hits_device", "btle_b200_ber_run",
     "btle_b200_stream_open", "btle_b200_stream_push", "btle_b200_stream_acquire", "btle_b200_stream_commit", "btle_b200_stream_finish",
-    "btle_b200_stream_close", "btle_b200_stream_set_cfg", "btle_b200_parse_adv_pdu_payload_byte", "btle_b200_parse_ll_pdu_payload_byte",
+    "btle_b200_stream_close", "btle_b200_stream_set_cfg",
+    "btle_b200_streams_open", "btle_b200_streams_acquire", "btle_b200_streams_commit", "btle_b200_streams_set_cfg",
+    "btle_b200_streams_finish", "btle_b200_streams_close", "btle_b200_parse_adv_pdu_payload_byte", "btle_b200_parse_ll_pdu_payload_byte",
     "btle_b200_receiver_controller", "btle_b200_receiver_status", "btle_b200_note_packet", "btle_b200_set_hop_hooks", "btle_b200_hop_reset",
     "btle_b200_get_freq_by_channel_number", "btle_b200_chm_is_full_map",
 ]
@@ -118,6 +120,13 @@ def load():
     L.btle_b200_sps8_hits_device.argtypes = [vp, vp, sz, u32, vp, sz, vp, vp]
     L.btle_b200_rx_sps8.argtypes = [vp, vp, sz, i32, u32, u32, vp, sz, ctypes.POINTER(sz)]
     L.btle_b200_synth_streams_device.argtypes = [vp, vp, sz, sz, sz, vp, vp, vp, sz, ctypes.POINTER(sz), vp]
+    L.btle_b200_streams_open.argtypes = [vp, vp, sz, sz, ctypes.POINTER(vp)]
+    L.btle_b200_streams_acquire.argtypes = [vp, sz, ctypes.POINTER(vp), ctypes.POINTER(sz)]
+    L.btle_b200_streams_commit.argtypes = [vp, sz, sz, vp, sz, ctypes.POINTER(sz)]
+    L.btle_b200_streams_set_cfg.argtypes = [vp, sz, vp]
+    L.btle_b200_streams_finish.argtypes = [vp, vp, sz, ctypes.POINTER(sz)]
+    L.btle_b200_streams_close.argtypes = [vp]
+    L.btle_b200_streams_close.restype = None
     _lib = L
     return L
 

@@ -14,8 +14,11 @@
 //       -i/--iq-file FILE        raw interleaved int8 (what rx_callback writes, btle_rx.c:531-540), '-' = stdin.  Read in
 //                                64 MiB segments straight into page-locked memory and decoded while the next segment is
 //                                being read (btle_b200_stream_*): the capture may be larger than host RAM or HBM.
-//       -i FILE:CH[:AA[:CRCINIT]]  (repeatable) several captures, each with its own channel / access address / CRC
-//                                init, decoded in ONE batched launch; packets are printed in time order.
+//       -i FILE:CH[:AA[:CRCINIT]]  (repeatable) several time-aligned captures (files or FIFOs, '-' for one of them),
+//                                each with its own channel / access address / CRC init.  Streamed through one session
+//                                (btle_b200_streams_*): poll() across the inputs, each segment set decoded in one
+//                                batched launch while the next one is read; packets are printed in time order, up to
+//                                the end of the shortest capture.
 //       --iq-dir DIR             DIR/ch00.bin .. DIR/ch39.bin, time-aligned captures of the BLE channels (missing
 //                                files are skipped).  Without -o: like 40 -i entries.  With -o: see below.
 //       --iq-txt FILE / --iq-sc16 FILE   text format of save_phy_sample (btle_rx.c:896-915) / int16 bladeRF samples.
@@ -26,7 +29,9 @@
 //     data captures with the connection's access address), the walk only picks what the radio would have seen.
 //   * time stamps are sample time (4 Msps) from the start of the capture, not wall clock; in hop mode the state
 //     machine's clock is the time at which a chunk (with its look-ahead) is complete.
+#include <fcntl.h>
 #include <getopt.h>
+#include <poll.h>
 #include <signal.h>
 #include <unistd.h>
 
@@ -61,7 +66,7 @@ struct Options {
   uint64_t freq_hz = 123;
   const char *pcap = nullptr, *iq_txt = nullptr, *iq_sc16 = nullptr, *iq_dir = nullptr, *iq_bin16 = nullptr;
   std::vector<std::string> iq_files;            // -i, possibly FILE:CH[:AA[:CRCINIT]]
-  size_t segment_chunks = 4096;
+  size_t segment_chunks = 0;                    // 0: the session default
   int filter_adva_set = 0;
   uint8_t filter_adva[6] = {0, 0, 0, 0, 0, 0};
   uint16_t filter_pdu_mask = 0xFFFF;
@@ -73,11 +78,14 @@ void usage() {
       "Usage:\n"
       "    -h --help\n      Print this help screen\n"
       "    -i --iq-file FILE[:CH[:AA[:CRCINIT]]]\n      raw interleaved int8 I,Q capture at 4 Msps ('-' = stdin)   [this build: no SDR]\n"
-      "      repeatable: several captures are decoded in one batch, each with its own channel / access address / CRC init\n"
-      "       --iq-dir DIR\n      DIR/ch00.bin .. DIR/ch39.bin (time-aligned per-channel captures); with -o the connection is followed across them\n"
+      "      repeatable: several time-aligned captures (files or FIFOs; '-' for at most one), each with its own channel /\n"
+      "      access address / CRC init, streamed through one session; packets in time order up to the shortest capture's end\n"
+      "       --iq-dir DIR\n      DIR/ch00.bin .. DIR/ch39.bin (time-aligned per-channel captures), streamed like several -i;\n"
+      "      with -o the connection is followed across them (whole files)\n"
       "       --iq-bin16 FILE\n      interleaved int16 I,Q at 8 Msps (8 samples per symbol): a `btle_ll -q` capture; decoded with the 8-phase\n"
       "      CRC-select receiver of the reference's Python / Verilog model (first sample phase whose CRC is ok wins)\n"
-      "       --segment-chunks N\n      chunks (16384 int8) per streamed segment of a single capture (default 4096 = 64 MiB)\n"
+      "       --segment-chunks N\n      chunks (16384 int8) per streamed segment of each capture (0 / default: 4096 = 64 MiB for one\n"
+      "      capture, max(16, 4096 / N rounded up to 16) for N captures)\n"
       "       --iq-txt FILE\n      capture in the text format written by save_phy_sample()\n"
       "       --iq-sc16 FILE\n      raw interleaved int16 I,Q (bladeRF SC16Q11); reduced with >>4 like btle_rx's bladeRF build\n"
       "    -c --chan\n      Channel number. default 37. valid range 0~39\n"
@@ -656,30 +664,107 @@ int main(int argc, char **argv) {
     btle_b200_set_hop_hooks(nullptr);
     t_end = (double)(n / 2) / 4.0e6;
   } else if (caps.size() > 1 || (caps.size() == 1 && o.iq_dir)) {
-    // ---- several captures: one batched launch, packets in time order ------------------------------------------------
-    std::vector<std::vector<int8_t>> iq(caps.size());
-    size_t n = SIZE_MAX;
-    for (size_t s_ = 0; s_ < caps.size(); ++s_) {
-      if (!load_raw(caps[s_].file.c_str(), iq[s_])) { btle_b200_destroy(ctx); return 1; }
-      n = std::min(n, iq[s_].size());
+    // ---- several captures, streamed through one session (btle_b200_streams_*): poll() across the inputs, read() into
+    //      whichever capture has data and room, one batched launch per segment set, packets in time order ----------------
+    const size_t ns = caps.size();
+    std::vector<int> fds(ns, -1);
+    auto close_inputs = [&]() { for (int fd : fds) if (fd > 0) close(fd); };
+    size_t n_stdin = 0;
+    for (size_t s_ = 0; s_ < ns; ++s_) {
+      if (caps[s_].file == "-") {
+        if (n_stdin++) { printf("'-' (stdin) can be the input of one capture only\n"); close_inputs(); btle_b200_destroy(ctx); return 1; }
+        fds[s_] = 0;
+        continue;
+      }
+      fds[s_] = open(caps[s_].file.c_str(), O_RDONLY);           // a FIFO: waits here until its writer has opened it
+      if (fds[s_] < 0) { perror(caps[s_].file.c_str()); close_inputs(); btle_b200_destroy(ctx); return 1; }
     }
-    const size_t stride = (n + 15) & ~size_t(15);
-    std::vector<int8_t> stage(stride * caps.size());
     std::vector<btle_stream_cfg> cfgs;
-    for (size_t s_ = 0; s_ < caps.size(); ++s_) {
-      memcpy(stage.data() + s_ * stride, iq[s_].data(), n);
-      iq[s_] = std::vector<int8_t>();
-      cfgs.push_back(btle_stream_cfg{caps[s_].chan, caps[s_].aa, o.mask, caps[s_].crc_init, o.raw, cfg_flags(o)});
+    for (const Capture &c : caps) cfgs.push_back(btle_stream_cfg{c.chan, c.aa, o.mask, c.crc_init, o.raw, cfg_flags(o)});
+    btle_b200_streams *ss = nullptr;
+    rc = btle_b200_streams_open(ctx, cfgs.data(), ns, o.segment_chunks, &ss);
+    if (rc) { close_inputs(); return fail("btle_b200_streams_open"); }
+    std::vector<btle_pkt_rec> recs(65536), pending;
+    long long max_chunk = -1;
+    // Records arrive per segment set in (stream, chunk, n0) order.  They are printed in time order (chunk*8192 + n0; ties in
+    // (stream, chunk, n0) order), as soon as no later record can sort in front of them: every record still to come lies in a
+    // later chunk, and a hit starts at most 124 samples before its chunk.
+    auto emit = [&](bool all) {
+      auto key = [](const btle_pkt_rec &r) { return (long long)r.chunk * 8192 + r.n0; };
+      std::stable_sort(pending.begin(), pending.end(), [&](const btle_pkt_rec &a, const btle_pkt_rec &b) {
+        if (key(a) != key(b)) return key(a) < key(b);
+        return a.stream != b.stream ? a.stream < b.stream : a.chunk < b.chunk;
+      });
+      const long long safe = (max_chunk + 1) * 8192 - 124;
+      size_t k = 0;
+      for (; k < pending.size() && (all || key(pending[k]) < safe); ++k) sinks.packet(pending[k], rec_time(pending[k]));
+      pending.erase(pending.begin(), pending.begin() + (long)k);
+      if (k) fflush(stdout);
+    };
+    auto keep = [&](size_t n) {
+      for (size_t i = 0; i < n; ++i) { pending.push_back(recs[i]); max_chunk = std::max<long long>(max_chunk, recs[i].chunk); }
+    };
+    std::vector<size_t> total(ns, 0);
+    std::vector<char> eof(ns, 0);
+    size_t shortest = SIZE_MAX;                                 // length of the shortest capture once one has ended
+    while (!g_stop && rc == 0) {
+      std::vector<pollfd> pf;
+      std::vector<size_t> who;
+      for (size_t s_ = 0; s_ < ns; ++s_) {
+        if (eof[s_] || total[s_] >= shortest) continue;         // bytes behind the shortest capture are not decoded
+        int8_t *buf; size_t space;
+        btle_b200_streams_acquire(ss, s_, &buf, &space);
+        if (space) { pf.push_back(pollfd{fds[s_], POLLIN, 0}); who.push_back(s_); }   // else: waits for the other captures
+      }
+      if (pf.empty()) break;
+      if (poll(pf.data(), pf.size(), -1) < 0) {
+        if (errno == EINTR) continue;
+        perror("poll");
+        break;
+      }
+      for (size_t k = 0; k < pf.size() && rc == 0; ++k) {
+        if (!(pf[k].revents & (POLLIN | POLLHUP | POLLERR))) continue;
+        const size_t s_ = who[k];
+        int8_t *buf; size_t space;
+        btle_b200_streams_acquire(ss, s_, &buf, &space);
+        const ssize_t got = read(fds[s_], buf, std::min(space, size_t(8) << 20));
+        if (got < 0 && errno == EINTR) continue;
+        if (got <= 0) {
+          if (got < 0) perror(caps[s_].file.c_str());
+          eof[s_] = 1;
+          shortest = std::min(shortest, total[s_]);
+          continue;
+        }
+        total[s_] += (size_t)got;
+        size_t n = 0;
+        rc = btle_b200_streams_commit(ss, s_, (size_t)got, recs.data(), recs.size(), &n);
+        keep(n);
+        while (rc == 0 && n == recs.size()) { rc = btle_b200_streams_commit(ss, s_, 0, recs.data(), recs.size(), &n); keep(n); }
+        emit(false);
+      }
     }
-    std::vector<btle_pkt_rec> recs;
-    rc = rx_batch_grow(ctx, stage.data(), caps.size(), stride, n, cfgs.data(), recs);
-    if (rc) return fail("btle_b200_rx_batch");
-    std::stable_sort(recs.begin(), recs.end(), [](const btle_pkt_rec &a, const btle_pkt_rec &b) {
-      const long long ta = (long long)a.chunk * 8192 + a.n0, tb = (long long)b.chunk * 8192 + b.n0;
-      return ta < tb;                                          // ties keep (stream, chunk, n0) order
-    });
-    for (const btle_pkt_rec &r : recs) { if (g_stop) break; sinks.packet(r, rec_time(r)); }
-    t_end = (double)(n / 2) / 4.0e6;
+    if (rc) { btle_b200_streams_close(ss); close_inputs(); return fail("btle_b200_streams_commit"); }
+    for (;;) {                                                  // end of input or SIGINT: decode up to the shortest capture
+      size_t n = 0;
+      rc = btle_b200_streams_finish(ss, recs.data(), recs.size(), &n);
+      keep(n);
+      if (rc != BTLE_EOVERFLOW) break;
+    }
+    btle_b200_streams_close(ss);
+    close_inputs();
+    if (rc) return fail("btle_b200_streams_finish");
+    const size_t n_read = *std::min_element(total.begin(), total.end());
+    if (g_stop) {
+      // stopped mid-stream: print only what a full run prints first — the chunks whose look-ahead had arrived on every
+      // capture (the tail decode read zeros behind them), up to where a later chunk's hit could sort in front
+      const long long done = n_read >= (size_t)BTLE_LOOKAHEAD_INT8 ? (long long)((n_read - BTLE_LOOKAHEAD_INT8) / BTLE_CHUNK_INT8) : 0;
+      pending.erase(std::remove_if(pending.begin(), pending.end(), [&](const btle_pkt_rec &r) { return r.chunk >= done; }), pending.end());
+      max_chunk = done - 1;
+      emit(false);
+    } else {
+      emit(true);
+    }
+    t_end = (double)(n_read / 2) / 4.0e6;
   } else if (o.iq_txt || o.iq_sc16) {
     // ---- whole-file formats ----------------------------------------------------------------------------------------
     std::vector<int8_t> iq;

@@ -1933,42 +1933,59 @@ int btle_b200_rx(btle_b200_ctx *ctx, const int8_t *iq, size_t n_int8, const btle
   return btle_b200_rx_batch(ctx, iq, 1, n_int8, n_int8, cfg, out, cap, n_out);
 }
 
-// ---- streaming session: one capture of unbounded length, pushed in pieces ---------------------------------------
+// ---- streaming sessions: N time-aligned captures of unbounded length, pushed in pieces ----------------------------
 }  // extern "C"
 
-struct btle_b200_stream {
+// One segment SET = `seg_chunks` chunks of every capture.  Capture i's part of a set sits at i * stride in the half's
+// buffers: kLead bytes of the previous set, the segment, kLook look-ahead bytes (the start of the next set).  A set is
+// decoded by ONE batched launch of the persistent kernel over the N parts once every capture has filled its own.
+struct btle_b200_streams {
   btle_b200_ctx *ctx = nullptr;
-  btle_stream_cfg cfg{};
-  size_t seg_chunks = 0, seg_bytes = 0, buf_bytes = 0;     // a segment = seg_chunks chunks (+ kLook look-ahead bytes behind it)
+  size_t n = 0;                                            // captures in the session
+  std::vector<btle_stream_cfg> cfgs;                       // what the next submitted set is decoded with
+  size_t seg_chunks = 0, seg_bytes = 0, buf_bytes = 0;     // a part = seg_chunks chunks (+ kLook look-ahead bytes behind it)
+  size_t stride = 0;                                       // kLead + buf_bytes: bytes from one capture's part to the next
   static constexpr size_t kLook = 4096;                    // >= 3008 + the kernel's 12-group tile (3072 + 4)
-  static constexpr size_t kLead = 256;                     // bytes of the previous segment kept in front (a hit may start up to 124 samples
+  static constexpr size_t kLead = 256;                     // bytes of the previous set kept in front (a hit may start up to 124 samples
                                                            // before its chunk; the RSSI sum reads the raw IQ there)
   struct Half {
-    int8_t *h = nullptr, *d = nullptr;                     // page-locked host / device IQ buffers
+    int8_t *h = nullptr, *d = nullptr;                     // page-locked host / device IQ buffers, n parts of `stride` bytes
     btle_pkt_rec *d_out = nullptr; btle_unit_dir *d_dir = nullptr; unsigned *d_count = nullptr;
     unsigned *h_count = nullptr; btle_unit_dir *h_dir = nullptr; btle_pkt_rec *h_recs = nullptr;
-    size_t cap = 0, units = 0, fill = 0, n_submitted = 0;
+    size_t cap = 0, units = 0, n_submitted = 0;
     long long first_chunk = 0;
     cudaStream_t st = nullptr;
     bool busy = false;
   } half[2];
+  std::vector<size_t> fill;                                // bytes in each capture's part of the half being filled
+  size_t n_full = 0;                                       // captures whose part of that half is complete
   int cur = 0;                                             // half being filled
   long long next_chunk = 0;                                // stream-wide index of the first chunk of the half being filled
   std::vector<btle_pkt_rec> ready;                         // decoded, not yet handed out
   size_t ready_pos = 0;
 };
 
+// the single-capture session is a one-capture btle_b200_streams
+struct btle_b200_stream {
+  btle_b200_streams *m = nullptr;
+};
+
 namespace {
-int stream_submit(btle_b200_stream *s, int b, size_t n_int8) {
+// decode the first n_int8 bytes of every capture's part of half b (bytes behind n_int8 read as 0)
+int streams_submit(btle_b200_streams *s, int b, size_t n_int8) {
   btle_b200_ctx *ctx = s->ctx;
   auto &H = s->half[b];
   H.n_submitted = n_int8;
   H.first_chunk = s->next_chunk;
   if (n_int8 < (size_t)kChunkInt8) { H.busy = false; return BTLE_OK; }
-  constexpr size_t L = btle_b200_stream::kLead;
-  BTLE_CUDA(ctx, cudaMemcpyAsync(H.d, H.h, L + n_int8, cudaMemcpyHostToDevice, H.st));
+  constexpr size_t L = btle_b200_streams::kLead;
+  if (L + n_int8 == s->stride || s->n == 1)
+    BTLE_CUDA(ctx, cudaMemcpyAsync(H.d, H.h, (s->n - 1) * s->stride + L + n_int8, cudaMemcpyHostToDevice, H.st));
+  else
+    BTLE_CUDA(ctx, cudaMemcpy2DAsync(H.d, s->stride, H.h, s->stride, L + n_int8, s->n, cudaMemcpyHostToDevice, H.st));
   ctx->lead_bytes = L;
-  const int rc = btle_b200_rx_device_dir(ctx, H.d + L, 1, s->buf_bytes, n_int8, &s->cfg, H.d_out, H.cap, H.d_count, H.d_dir, H.units, H.st);
+  const int rc = btle_b200_rx_device_dir(ctx, H.d + L, s->n, s->stride, n_int8, s->cfgs.data(), H.d_out, H.cap, H.d_count, H.d_dir,
+                                         H.units, H.st);
   ctx->lead_bytes = 0;
   if (rc) return rc;
   BTLE_CUDA(ctx, cudaMemcpyAsync(H.h_count, H.d_count, sizeof(unsigned), cudaMemcpyDeviceToHost, H.st));
@@ -1976,8 +1993,8 @@ int stream_submit(btle_b200_stream *s, int b, size_t n_int8) {
   H.busy = true;
   return BTLE_OK;
 }
-// wait for a submitted half, append its records (reference order, stream-wide chunk numbers) to s->ready
-int stream_collect(btle_b200_stream *s, int b) {
+// wait for a submitted half, append its records ((stream, chunk, n0) order, stream-wide chunk numbers) to s->ready
+int streams_collect(btle_b200_streams *s, int b) {
   btle_b200_ctx *ctx = s->ctx;
   auto &H = s->half[b];
   if (!H.busy) return BTLE_OK;
@@ -1988,7 +2005,7 @@ int stream_collect(btle_b200_stream *s, int b) {
   if (!found) return BTLE_OK;
   BTLE_CUDA(ctx, cudaMemcpyAsync(H.h_recs, H.d_out, found * sizeof(btle_pkt_rec), cudaMemcpyDeviceToHost, H.st));
   BTLE_CUDA(ctx, cudaStreamSynchronize(H.st));
-  const size_t units = btle_b200_rx_units(ctx, 1, H.n_submitted);
+  const size_t units = btle_b200_rx_units(ctx, s->n, H.n_submitted);
   const size_t at = s->ready.size();
   s->ready.resize(at + found);
   size_t got = 0;
@@ -1996,34 +2013,48 @@ int stream_collect(btle_b200_stream *s, int b) {
   for (size_t i = at; i < at + found; ++i) s->ready[i].chunk += (int32_t)H.first_chunk;
   return BTLE_OK;
 }
-size_t stream_take(btle_b200_stream *s, btle_pkt_rec *out, size_t cap) {
+size_t streams_take(btle_b200_streams *s, btle_pkt_rec *out, size_t cap) {
   const size_t n = std::min(cap, s->ready.size() - s->ready_pos);
   if (n) memcpy(out, s->ready.data() + s->ready_pos, n * sizeof(btle_pkt_rec));
   s->ready_pos += n;
   if (s->ready_pos == s->ready.size()) { s->ready.clear(); s->ready_pos = 0; }
   return n;
 }
+int streams_index(btle_b200_streams *s, size_t stream) {
+  if (stream < s->n) return BTLE_OK;
+  s->ctx->err = "stream index out of range";
+  return BTLE_EINVAL;
+}
 }  // namespace
 
 extern "C" {
 
-int btle_b200_stream_open(btle_b200_ctx *ctx, const btle_stream_cfg *cfg, size_t segment_chunks, btle_b200_stream **out) {
-  if (!ctx || !cfg || !out) return BTLE_EINVAL;
+int btle_b200_streams_open(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size_t n_streams, size_t segment_chunks,
+                           btle_b200_streams **out) {
+  if (!ctx || !out) return BTLE_EINVAL;
   *out = nullptr;
-  int rc = validate_cfgs(ctx, cfg, 1);
+  if (n_streams == 0) { ctx->err = "streams_open: no captures"; return BTLE_EINVAL; }
+  if (!cfgs) return BTLE_EINVAL;
+  int rc = validate_cfgs(ctx, cfgs, n_streams);
   if (rc) return rc;
-  if (segment_chunks == 0) segment_chunks = 4096;           // 64 MiB of IQ = 8.4 s of air per segment
+  // default: about 4096 chunks (64 MiB = 8.4 s of air of one capture) per half over all captures, so the footprint does
+  // not grow with the number of captures; at least 16 chunks per capture
+  if (segment_chunks == 0) segment_chunks = std::max<size_t>(16, (4096 / n_streams + 15) & ~size_t(15));
   if (segment_chunks > (1u << 20)) { ctx->err = "segment too large"; return BTLE_EINVAL; }
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
-  btle_b200_stream *s = new (std::nothrow) btle_b200_stream();
+  btle_b200_streams *s = new (std::nothrow) btle_b200_streams();
   if (!s) return BTLE_ENOMEM;
-  s->ctx = ctx; s->cfg = *cfg; s->seg_chunks = segment_chunks; s->seg_bytes = segment_chunks * (size_t)kChunkInt8;
-  s->buf_bytes = s->seg_bytes + btle_b200_stream::kLook;
+  s->ctx = ctx; s->n = n_streams; s->cfgs.assign(cfgs, cfgs + n_streams); s->fill.assign(n_streams, 0);
+  s->seg_chunks = segment_chunks; s->seg_bytes = segment_chunks * (size_t)kChunkInt8;
+  s->buf_bytes = s->seg_bytes + btle_b200_streams::kLook;
+  s->stride = btle_b200_streams::kLead + s->buf_bytes;     // a multiple of 16, as the batched kernel needs
   for (auto &H : s->half) {
-    H.cap = segment_chunks * BTLE_MAX_RECS_PER_CHUNK;
-    H.units = btle_b200_rx_units(ctx, 1, s->buf_bytes) + 1;
-    if (cudaHostAlloc(reinterpret_cast<void **>(&H.h), btle_b200_stream::kLead + s->buf_bytes, cudaHostAllocDefault) != cudaSuccess ||
-        cudaMalloc(reinterpret_cast<void **>(&H.d), btle_b200_stream::kLead + s->buf_bytes) != cudaSuccess ||
+    H.cap = n_streams * segment_chunks * BTLE_MAX_RECS_PER_CHUNK;
+    // a short tail can be cut into more units than a full set (make_plan: down to one chunk per unit, over whole 16-chunk
+    // spans), so the directory is sized for the most any launch of up to segment_chunks chunks per capture can have
+    H.units = n_streams * ((segment_chunks + 15) & ~size_t(15));
+    if (cudaHostAlloc(reinterpret_cast<void **>(&H.h), n_streams * s->stride, cudaHostAllocDefault) != cudaSuccess ||
+        cudaMalloc(reinterpret_cast<void **>(&H.d), n_streams * s->stride) != cudaSuccess ||
         cudaMalloc(reinterpret_cast<void **>(&H.d_out), H.cap * sizeof(btle_pkt_rec)) != cudaSuccess ||
         cudaMalloc(reinterpret_cast<void **>(&H.d_dir), H.units * sizeof(btle_unit_dir)) != cudaSuccess ||
         cudaMalloc(reinterpret_cast<void **>(&H.d_count), sizeof(unsigned)) != cudaSuccess ||
@@ -2032,17 +2063,17 @@ int btle_b200_stream_open(btle_b200_ctx *ctx, const btle_stream_cfg *cfg, size_t
         cudaHostAlloc(reinterpret_cast<void **>(&H.h_recs), H.cap * sizeof(btle_pkt_rec), cudaHostAllocDefault) != cudaSuccess ||
         cudaStreamCreateWithFlags(&H.st, cudaStreamNonBlocking) != cudaSuccess) {
       cudaGetLastError();
-      ctx->err = "stream_open: allocation failed";
-      btle_b200_stream_close(s);
+      ctx->err = "streams_open: allocation failed";
+      btle_b200_streams_close(s);
       return BTLE_ENOMEM;
     }
-    memset(H.h, 0, btle_b200_stream::kLead);                // nothing before the start of the stream
+    for (size_t i = 0; i < n_streams; ++i) memset(H.h + i * s->stride, 0, btle_b200_streams::kLead);   // nothing before the start
   }
   *out = s;
   return BTLE_OK;
 }
 
-void btle_b200_stream_close(btle_b200_stream *s) {
+void btle_b200_streams_close(btle_b200_streams *s) {
   if (!s) return;
   cudaSetDevice(s->ctx->device);
   for (auto &H : s->half) {
@@ -2056,43 +2087,105 @@ void btle_b200_stream_close(btle_b200_stream *s) {
   delete s;
 }
 
-int btle_b200_stream_set_cfg(btle_b200_stream *s, const btle_stream_cfg *cfg) {
+int btle_b200_streams_set_cfg(btle_b200_streams *s, size_t stream, const btle_stream_cfg *cfg) {
   if (!s || !cfg) return BTLE_EINVAL;
-  const int rc = validate_cfgs(s->ctx, cfg, 1);
+  int rc = streams_index(s, stream);
   if (rc) return rc;
-  s->cfg = *cfg;                                            // used from the next submitted segment on
+  rc = validate_cfgs(s->ctx, cfg, 1);
+  if (rc) return rc;
+  s->cfgs[stream] = *cfg;                                   // used from the next submitted segment set on
   return BTLE_OK;
 }
 
-int btle_b200_stream_acquire(btle_b200_stream *s, int8_t **buf, size_t *space) {
+int btle_b200_streams_acquire(btle_b200_streams *s, size_t stream, int8_t **buf, size_t *space) {
   if (!s || !buf || !space) return BTLE_EINVAL;
+  const int rc = streams_index(s, stream);
+  if (rc) return rc;
   auto &H = s->half[s->cur];
-  *buf = H.h + btle_b200_stream::kLead + H.fill;
-  *space = s->buf_bytes - H.fill;
+  *buf = H.h + stream * s->stride + btle_b200_streams::kLead + s->fill[stream];
+  *space = s->buf_bytes - s->fill[stream];                  // 0: this capture's part is complete, the others are behind
   return BTLE_OK;
 }
 
-int btle_b200_stream_commit(btle_b200_stream *s, size_t n_int8, btle_pkt_rec *out, size_t cap, size_t *n_out) {
+int btle_b200_streams_commit(btle_b200_streams *s, size_t stream, size_t n_int8, btle_pkt_rec *out, size_t cap, size_t *n_out) {
   if (!s || !n_out || (!out && cap)) return BTLE_EINVAL;
   *n_out = 0;
-  auto &H = s->half[s->cur];
-  if (n_int8 > s->buf_bytes - H.fill) { s->ctx->err = "stream_commit: more bytes than acquired"; return BTLE_EINVAL; }
+  int rc = streams_index(s, stream);
+  if (rc) return rc;
+  if (n_int8 > s->buf_bytes - s->fill[stream]) { s->ctx->err = "stream_commit: more bytes than acquired"; return BTLE_EINVAL; }
   BTLE_CUDA(s->ctx, cudaSetDevice(s->ctx->device));
-  H.fill += n_int8;
-  if (H.fill == s->buf_bytes) {                             // segment + look-ahead complete: hand it to the GPU
+  s->fill[stream] += n_int8;
+  if (n_int8 && s->fill[stream] == s->buf_bytes) ++s->n_full;
+  if (s->n_full == s->n) {                                  // every part + look-ahead complete: hand the set to the GPU
     const int b = s->cur, o = b ^ 1;
-    int rc = stream_collect(s, o);                          // the other half's previous segment must be done before its buffers are reused
+    rc = streams_collect(s, o);                             // the other half's previous set must be done before its buffers are reused
     if (rc) return rc;
-    rc = stream_submit(s, b, s->buf_bytes);
+    rc = streams_submit(s, b, s->buf_bytes);
     if (rc) return rc;
-    // the look-ahead bytes are the beginning of the next segment, the bytes in front of them its lead
-    memcpy(s->half[o].h, H.h + s->seg_bytes, btle_b200_stream::kLead + btle_b200_stream::kLook);
-    s->half[o].fill = btle_b200_stream::kLook;
+    // the look-ahead bytes are the beginning of the next set, the bytes in front of them its lead
+    for (size_t i = 0; i < s->n; ++i) {
+      memcpy(s->half[o].h + i * s->stride, s->half[b].h + i * s->stride + s->seg_bytes,
+             btle_b200_streams::kLead + btle_b200_streams::kLook);
+      s->fill[i] = btle_b200_streams::kLook;
+    }
+    s->n_full = 0;
     s->next_chunk += (long long)s->seg_chunks;
     s->cur = o;
   }
-  *n_out = stream_take(s, out, cap);
+  *n_out = streams_take(s, out, cap);
   return BTLE_OK;
+}
+
+int btle_b200_streams_finish(btle_b200_streams *s, btle_pkt_rec *out, size_t cap, size_t *n_out) {
+  if (!s || !n_out || (!out && cap)) return BTLE_EINVAL;
+  *n_out = 0;
+  BTLE_CUDA(s->ctx, cudaSetDevice(s->ctx->device));
+  const int b = s->cur, o = b ^ 1;
+  int rc = streams_collect(s, o);
+  if (rc) return rc;
+  // the tail: complete chunks of the SHORTEST capture; behind that length every capture reads as 0 (rx_batch's common n_int8)
+  const size_t n_int8 = *std::min_element(s->fill.begin(), s->fill.end());
+  if (n_int8 >= (size_t)kChunkInt8) {
+    rc = streams_submit(s, b, n_int8);
+    if (rc) return rc;
+    rc = streams_collect(s, b);
+    if (rc) return rc;
+    s->next_chunk += (long long)(n_int8 / kChunkInt8);
+  }
+  std::fill(s->fill.begin(), s->fill.end(), size_t(0));
+  s->n_full = 0;
+  *n_out = streams_take(s, out, cap);
+  return (s->ready.size() > s->ready_pos) ? BTLE_EOVERFLOW : BTLE_OK;   // call again with more room
+}
+
+// ---- single capture: a one-capture session ----
+int btle_b200_stream_open(btle_b200_ctx *ctx, const btle_stream_cfg *cfg, size_t segment_chunks, btle_b200_stream **out) {
+  if (!ctx || !cfg || !out) return BTLE_EINVAL;
+  *out = nullptr;
+  btle_b200_stream *w = new (std::nothrow) btle_b200_stream();
+  if (!w) return BTLE_ENOMEM;
+  const int rc = btle_b200_streams_open(ctx, cfg, 1, segment_chunks, &w->m);
+  if (rc) { delete w; return rc; }
+  *out = w;
+  return BTLE_OK;
+}
+
+void btle_b200_stream_close(btle_b200_stream *s) {
+  if (!s) return;
+  btle_b200_streams_close(s->m);
+  delete s;
+}
+
+int btle_b200_stream_set_cfg(btle_b200_stream *s, const btle_stream_cfg *cfg) {
+  return s ? btle_b200_streams_set_cfg(s->m, 0, cfg) : BTLE_EINVAL;
+}
+
+int btle_b200_stream_acquire(btle_b200_stream *s, int8_t **buf, size_t *space) {
+  return s ? btle_b200_streams_acquire(s->m, 0, buf, space) : BTLE_EINVAL;
+}
+
+int btle_b200_stream_commit(btle_b200_stream *s, size_t n_int8, btle_pkt_rec *out, size_t cap, size_t *n_out) {
+  return s ? btle_b200_streams_commit(s->m, 0, n_int8, out, cap, n_out) : BTLE_EINVAL;
 }
 
 int btle_b200_stream_push(btle_b200_stream *s, const int8_t *iq, size_t n_int8, btle_pkt_rec *out, size_t cap, size_t *n_out) {
@@ -2114,23 +2207,7 @@ int btle_b200_stream_push(btle_b200_stream *s, const int8_t *iq, size_t n_int8, 
 }
 
 int btle_b200_stream_finish(btle_b200_stream *s, btle_pkt_rec *out, size_t cap, size_t *n_out) {
-  if (!s || !n_out || (!out && cap)) return BTLE_EINVAL;
-  *n_out = 0;
-  BTLE_CUDA(s->ctx, cudaSetDevice(s->ctx->device));
-  const int b = s->cur, o = b ^ 1;
-  int rc = stream_collect(s, o);
-  if (rc) return rc;
-  auto &H = s->half[b];
-  if (H.fill >= (size_t)kChunkInt8) {                       // the tail: complete chunks only, bytes behind them are look-ahead
-    rc = stream_submit(s, b, H.fill);
-    if (rc) return rc;
-    rc = stream_collect(s, b);
-    if (rc) return rc;
-    s->next_chunk += (long long)(H.fill / kChunkInt8);
-  }
-  H.fill = 0;
-  *n_out = stream_take(s, out, cap);
-  return (s->ready.size() > s->ready_pos) ? BTLE_EOVERFLOW : BTLE_OK;   // call again with more room
+  return s ? btle_b200_streams_finish(s->m, out, cap, n_out) : BTLE_EINVAL;
 }
 
 // ---- leaf functions ------------------------------------------------------------------------------

@@ -116,6 +116,14 @@ class BtleRx:
         `chunk` counted from the start of the stream, as segments complete."""
         return RxStream(self, make_cfgs(1, **cfg), segment_chunks)
 
+    def streams(self, cfgs: np.ndarray, segment_chunks: int = 0) -> "RxStreams":
+        """Streaming session over N time-aligned captures (one per radio / channel), cfgs: CFG_DTYPE [N] (make_cfgs):
+        `with rx.streams(make_cfgs(3, channel=[37, 38, 39])) as s: recs = s.push(1, iq_piece) ...; recs = s.finish()`.
+        Equals rx_batch() on the captures cut to the shortest one.  Each segment set (segment_chunks chunks of every
+        capture; 0 = the library default) is decoded in one batched launch once every capture has filled its part;
+        records come back per set in (stream, chunk, n0) order, `chunk` counted from the start of the capture."""
+        return RxStreams(self, cfgs, segment_chunks)
+
     # ---- device-resident ------------------------------------------------------------------
     def rx_device(self, d_iq, cfgs: np.ndarray, d_out, d_count, stream_ptr: int = 0):
         """d_iq: torch int8 CUDA tensor [n_streams, n_int8]; d_out: torch uint8 CUDA tensor
@@ -250,6 +258,98 @@ class RxStream:
     def close(self):
         if getattr(self, "_h", None):
             self._L.btle_b200_stream_close(self._h)
+            self._h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+    __del__ = close
+
+
+class RxStreams:
+    """Python face of btle_b200_streams_open / acquire / commit / set_cfg / finish / close.
+
+    push(stream, iq) never blocks: bytes of a capture whose part of the current segment set is complete (the session waits
+    for the other captures) are kept here and fed in as soon as that set has been handed to the GPU."""
+
+    def __init__(self, rx: BtleRx, cfgs: np.ndarray, segment_chunks: int):
+        self._rx, self._L = rx, rx._L
+        self._cfgs = np.array(cfgs, dtype=CFG_DTYPE).reshape(-1)
+        self.n_streams = int(self._cfgs.size)
+        h = ctypes.c_void_p()
+        rx._check(self._L.btle_b200_streams_open(rx._h, self._cfgs.ctypes.data if self.n_streams else None, self.n_streams,
+                                                 int(segment_chunks), ctypes.byref(h)))
+        self._h = h
+        self._buf = np.empty(65536, dtype=REC_DTYPE)
+        self._pending = [[] for _ in range(self.n_streams)]     # per capture: arrays not yet taken by the session
+
+    def _acquire(self, stream):
+        buf, space = ctypes.c_void_p(), ctypes.c_size_t(0)
+        self._rx._check(self._L.btle_b200_streams_acquire(self._h, stream, ctypes.byref(buf), ctypes.byref(space)))
+        return buf.value, space.value
+
+    def _commit(self, stream, n_int8, out):
+        n = ctypes.c_size_t(0)
+        self._rx._check(self._L.btle_b200_streams_commit(self._h, stream, n_int8, self._buf.ctypes.data, self._buf.size, ctypes.byref(n)))
+        out.append(self._buf[:n.value].copy())
+        while n.value == self._buf.size:        # more records waiting than the buffer holds
+            self._rx._check(self._L.btle_b200_streams_commit(self._h, stream, 0, self._buf.ctypes.data, self._buf.size, ctypes.byref(n)))
+            out.append(self._buf[:n.value].copy())
+
+    def push(self, stream: int, iq) -> np.ndarray:
+        """Append bytes to capture `stream`; returns the records of the segment sets completed so far."""
+        stream = int(stream)
+        self._acquire(stream)                   # BtleError (BTLE_EINVAL) for an index out of range
+        iq = np.ascontiguousarray(iq, dtype=np.int8).reshape(-1)
+        if iq.size:
+            self._pending[stream].append(iq)
+        out, progress = [], True
+        while progress:                         # completing a set frees room for every capture's waiting bytes
+            progress = False
+            for i, q in enumerate(self._pending):
+                while q:
+                    buf, space = self._acquire(i)
+                    if space == 0:
+                        break
+                    k = min(space, q[0].size)
+                    ctypes.memmove(buf, q[0].ctypes.data, k)
+                    q[0] = q[0][k:]
+                    if q[0].size == 0:
+                        q.pop(0)
+                    self._commit(i, k, out)
+                    progress = True
+        q = self._pending[stream]
+        if q and np.may_share_memory(q[-1], iq):     # keep what waits independent of the caller's array
+            q[-1] = q[-1].copy()
+        return np.concatenate(out) if out else self._buf[:0].copy()
+
+    def set_cfg(self, stream: int, **cfg) -> None:
+        """Change fields of capture `stream`'s cfg (make_cfgs names), from the next segment set that is submitted on."""
+        c = self._cfgs[int(stream):int(stream) + 1].copy() if 0 <= int(stream) < self.n_streams else make_cfgs(1)
+        for k, v in cfg.items():
+            c[k] = v
+        self._rx._check(self._L.btle_b200_streams_set_cfg(self._h, int(stream), c.ctypes.data))
+        self._cfgs[int(stream)] = c[0]
+
+    def finish(self) -> np.ndarray:
+        """End of the captures: decodes up to the shortest one and returns every record still waiting."""
+        out = []
+        while True:
+            n = ctypes.c_size_t(0)
+            rc = self._L.btle_b200_streams_finish(self._h, self._buf.ctypes.data, self._buf.size, ctypes.byref(n))
+            out.append(self._buf[:n.value].copy())
+            if rc != BTLE_EOVERFLOW:
+                self._rx._check(rc)
+                break
+        self._pending = [[] for _ in range(self.n_streams)]   # bytes behind the shortest capture are not decoded
+        return np.concatenate(out)
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._L.btle_b200_streams_close(self._h)
             self._h = None
 
     def __enter__(self):

@@ -179,6 +179,29 @@ int btle_b200_stream_set_cfg(btle_b200_stream *s, const btle_stream_cfg *cfg);
 int btle_b200_stream_finish(btle_b200_stream *s, btle_pkt_rec *out, size_t cap, size_t *n_out);
 void btle_b200_stream_close(btle_b200_stream *s);
 
+/* ---- streaming session over N time-aligned captures (one per radio / channel), each pushed in pieces ---------------
+ * Defined to equal btle_b200_rx_batch() on the same captures, each cut to the length of the shortest.  The captures are
+ * cut into segment SETS: `segment_chunks` chunks of every capture (0 = default max(16, round_up(4096 / n_streams, 16)),
+ * so that one half holds about 64 MiB whatever N is).  A set is decoded, in ONE batched launch over the N captures, once
+ * every capture has filled its part (its segment plus the look-ahead); while the GPU decodes it, the caller fills the
+ * other half.  btle_b200_streams_acquire() hands out where capture `stream`'s next bytes go (page-locked memory, so a
+ * file or FIFO can be read() straight into it); *space == 0 means that capture's part is complete and the session waits
+ * for the others.  Records come back per set in (stream, chunk, n0) order, `stream` = index in the session, `chunk`
+ * counted from the start of the capture; records that do not fit `cap` wait for the next call (none are dropped).
+ * btle_b200_streams_finish() decodes the complete chunks up to the SHORTEST capture's end; in that last set bytes behind
+ * that length read as 0 for every capture.  It returns BTLE_EOVERFLOW while records are still waiting: call it again.
+ * btle_b200_streams_set_cfg() applies from the next set that is submitted.  BTLE_EINVAL (with btle_b200_last_error()
+ * set) for n_streams == 0, a stream index out of range, a commit of more bytes than acquired and a bad cfg; the session
+ * stays usable after the last three.  btle_b200_stream_* above is this session with one capture. */
+typedef struct btle_b200_streams btle_b200_streams;
+int btle_b200_streams_open(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size_t n_streams, size_t segment_chunks,
+                           btle_b200_streams **out);
+int btle_b200_streams_acquire(btle_b200_streams *s, size_t stream, int8_t **buf, size_t *space);
+int btle_b200_streams_commit(btle_b200_streams *s, size_t stream, size_t n_int8, btle_pkt_rec *out, size_t cap, size_t *n_out);
+int btle_b200_streams_set_cfg(btle_b200_streams *s, size_t stream, const btle_stream_cfg *cfg);
+int btle_b200_streams_finish(btle_b200_streams *s, btle_pkt_rec *out, size_t cap, size_t *n_out);
+void btle_b200_streams_close(btle_b200_streams *s);
+
 /* number of kernels the last rx call launched (bench.py's gpu_launches) */
 int btle_b200_last_launches(const btle_b200_ctx *ctx);
 
