@@ -38,6 +38,10 @@ BER_CFG_DTYPE = np.dtype([("seed", "<u8"), ("snr_db", "<f4"), ("ppm", "<f4"), ("
 BER_RESULT_DTYPE = np.dtype([("packets", "<u8"), ("pkt_err", "<u8"), ("bit_err", "<u8"), ("bit_total", "<u8"), ("aa_miss", "<u8"), ("seconds", "<f8")])
 assert BER_CFG_DTYPE.itemsize == 32 and BER_RESULT_DTYPE.itemsize == 48
 SPS8_REC_DTYPE = np.dtype([("sample", "<i8"), ("window", "<i8"), ("rx", MODEL_REC_DTYPE)])     # btle_sps8_rec
+# btle_conn_cand, 32 bytes: an empty-PDU candidate of connection discovery
+CAND_DTYPE = np.dtype([("sample", "<i8"), ("stream", "<i4"), ("access_addr", "<u4"), ("crc_init", "<u4"), ("channel", "u1"),
+                       ("header", "u1", 2), ("reserved", "u1", 9)])
+assert CAND_DTYPE.itemsize == 32
 assert REC_DTYPE.itemsize == 64 and CFG_DTYPE.itemsize == 24 and MODEL_REC_DTYPE.itemsize == 80 and SPS8_REC_DTYPE.itemsize == 96
 
 EXPORTS = [
@@ -54,7 +58,7 @@ EXPORTS = [
     "btle_b200_streams_open", "btle_b200_streams_acquire", "btle_b200_streams_commit", "btle_b200_streams_set_cfg",
     "btle_b200_streams_finish", "btle_b200_streams_close", "btle_b200_parse_adv_pdu_payload_byte", "btle_b200_parse_ll_pdu_payload_byte",
     "btle_b200_receiver_controller", "btle_b200_receiver_status", "btle_b200_note_packet", "btle_b200_set_hop_hooks", "btle_b200_hop_reset",
-    "btle_b200_get_freq_by_channel_number", "btle_b200_chm_is_full_map",
+    "btle_b200_get_freq_by_channel_number", "btle_b200_chm_is_full_map", "btle_b200_discover", "btle_b200_discover_device",
 ]
 
 
@@ -127,6 +131,8 @@ def load():
     L.btle_b200_streams_finish.argtypes = [vp, vp, sz, ctypes.POINTER(sz)]
     L.btle_b200_streams_close.argtypes = [vp]
     L.btle_b200_streams_close.restype = None
+    L.btle_b200_discover.argtypes = [vp, vp, sz, sz, sz, vp, vp, sz, ctypes.POINTER(sz)]
+    L.btle_b200_discover_device.argtypes = [vp, vp, sz, sz, sz, vp, vp, sz, vp, vp]
     _lib = L
     return L
 

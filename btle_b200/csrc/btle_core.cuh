@@ -655,4 +655,60 @@ BTLE_HD int resolve_chunk(const uint32_t *pd, const uint32_t *cand, const uint32
   return chain_chunk(pd, cand, flagw, sp, each);
 }
 
+// ---- connection discovery: the empty-PDU candidate rule (DESIGN.md §6.2) ------------------------------------------------
+// A window start n0 = 128 g + 4 i + ph of a data-channel capture is a CANDIDATE iff, on phase stream ph (symbol s0 = 32 g + i):
+//   preamble  S[s0-8 .. s0] alternate (8 inequalities: 0x55 and 0xAA both pass);
+//   header    the 16 symbols S[s0+32 .. s0+47] dewhitened with the first 16 whitening bits of the channel have LLID 1 and
+//             byte 1 == 0 (length 0, RFU 0); NESN, SN, MD and the byte-0 RFU bits are free;
+//   inside    every d[n] read lies in the capture (empty_pdu_inside).
+// w[0..4] = phase words of groups g-1 .. g+3 on phase ph; wh0 = whitening bits 0..31 of the channel (StreamParams::whiten[0]).
+// Bit i of the result: the window starting at symbol i of group g passes the preamble and header tests.
+constexpr uint32_t kEmptyPduFixed = 0xFF03u;        // header bits the rule pins: LLID (bits 0, 1) and byte 1
+BTLE_HD uint32_t empty_pdu_windows(const uint32_t w[5], uint32_t wh0) {
+  uint32_t m = 0xFFFFFFFFu;
+  uint32_t prev = funnel_r(w[0], w[1], 24u);                         // bit i = S[s0 - 8]
+#pragma unroll
+  for (int j = 1; j <= 8; ++j) {
+    const uint32_t cur = j < 8 ? funnel_r(w[0], w[1], (uint32_t)(24 + j)) : w[1];
+    m &= prev ^ cur;
+    prev = cur;
+  }
+  const uint32_t need = (wh0 ^ 1u) & kEmptyPduFixed;                 // received header bits: whitening ^ (LLID 1, all else 0)
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    if (!((kEmptyPduFixed >> j) & 1u)) continue;
+    m &= funnel_r(w[2], w[3], (uint32_t)j) ^ (((need >> j) & 1u) - 1u);   // keep bit i iff S[s0+32+j] == need bit j
+  }
+  return m;
+}
+// Window starts i of group g (phase ph) whose reads lie inside a capture of n_samples samples: n0 - 32 >= 0 and
+// n0 + 284 + 1 < n_samples (d[n] needs samples n and n+1).
+BTLE_HD uint32_t empty_pdu_inside(long long g, int ph, long long n_samples) {
+  const long long base = 128 * g + ph, lo = 32 - base, hi = n_samples - 286 - base;
+  if (hi < 0) return 0u;
+  const long long i_lo = lo <= 0 ? 0 : (lo + 3) / 4, i_hi = hi / 4 < 31 ? hi / 4 : 31;
+  if (i_lo > i_hi) return 0u;
+  const uint32_t upto = i_hi == 31 ? 0xFFFFFFFFu : ((1u << (i_hi + 1)) - 1u);
+  return upto & ~((1u << i_lo) - 1u);
+}
+// Fields of the window at symbol i: access address, dewhitened header (16 bits) and the received CRC (24 bits, dewhitened
+// with whitening bits 16..39); wh1 = whitening bits 32..63.
+BTLE_HD void empty_pdu_fields(const uint32_t w[5], int i, uint32_t wh0, uint32_t wh1, uint32_t &aa, uint32_t &header,
+                              uint32_t &crc_rx) {
+  aa = funnel_r(w[1], w[2], (uint32_t)i);
+  const uint32_t a = funnel_r(w[2], w[3], (uint32_t)i), b = funnel_r(w[3], w[4], (uint32_t)i);
+  header = (a ^ wh0) & 0xFFFFu;
+  crc_rx = (((a >> 16) | (b << 16)) ^ ((wh0 >> 16) | (wh1 << 16))) & 0xFFFFFFu;
+}
+// The CRC-24 register (crc24_words convention) from which `nbits` message bits (bit j = j-th bit sent) lead to `crc`.
+// One step of the LFSR is  c' = (c >> 1) ^ (f ? 0xDA6000 : 0), f = (c ^ bit) & 1;  bit 23 of c' is f, so every step can be
+// undone and the result is unique.  crc_init_reorder() of it is the -k value.
+BTLE_HD uint32_t crc24_unwind(uint32_t crc, uint32_t bits, int nbits) {
+  for (int j = nbits - 1; j >= 0; --j) {
+    const uint32_t f = (crc >> 23) & 1u;
+    crc = (((crc ^ (f ? 0xDA6000u : 0u)) << 1) | (f ^ ((bits >> j) & 1u))) & 0xFFFFFFu;
+  }
+  return crc;
+}
+
 }  // namespace btle

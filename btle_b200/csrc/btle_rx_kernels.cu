@@ -1116,6 +1116,86 @@ sps8_hits_kernel(const int16_t *__restrict__ iq, long long n_samples, long long 
   }
 }
 
+// ---- connection discovery: empty-PDU candidates with no access address given (btle_b200_discover*) --------------------
+// One CTA = kDiscGroups groups of window starts of one capture.  The rule (btle_core.cuh, empty_pdu_windows) reads the
+// phase words of one group in front of a window's group and three behind it, so the CTA stages kDiscThreads + 1 groups:
+//   load   cp.async of the groups' IQ (16-byte vectors, coalesced) into rows of kDiscPitch words: a lane's 16-byte reads
+//          of its own row are conflict-free within each quarter warp; bytes outside the capture read as 0
+//   pack   lane j turns group j into its four phase words (the dense receive loop, dbits_group_dense)
+//   test   lane j < kDiscGroups tests the 32 window starts of its group on each phase against the rule at once (funnel
+//          shifts of the neighbours' words); the rare survivor gets its access address, header and CRC-init (16 reverse
+//          LFSR steps) and one atomic on the counter places its 32-byte record
+// Like sps8_hits_kernel one tile per CTA: six CTAs per SM hide each other's load phase.
+constexpr int kDiscThreads = 128;
+constexpr int kDiscGroups = kDiscThreads - 4;                              // window-start groups per CTA
+constexpr int kDiscRows = kDiscThreads + 1;                                // staged groups (the last one for its first sample only)
+constexpr int kDiscPitch = 68;                                             // words per staged row (64 + 4 of padding)
+constexpr size_t kDiscSmem = ((size_t)kDiscRows * kDiscPitch + 4 * kDiscThreads) * sizeof(uint32_t);
+static_assert(sizeof(btle_conn_cand) == 32, "candidate record must be 32 bytes");
+__global__ void __launch_bounds__(kDiscThreads, 6)
+discover_kernel(const int8_t *__restrict__ iq, long long stride, long long n_int8, long long tiles_per_stream,
+                const StreamParams *__restrict__ params, btle_conn_cand *__restrict__ out, unsigned cap, unsigned *__restrict__ count) {
+  extern __shared__ __align__(16) uint32_t disc_smem[];
+  uint4 *pdw = reinterpret_cast<uint4 *>(disc_smem + kDiscRows * kDiscPitch);   // phase words of staged group j
+  const long long stream = blockIdx.x / tiles_per_stream, tile = blockIdx.x - stream * tiles_per_stream;
+  const int8_t *cap_base = iq + stream * stride;
+  const long long row0 = (tile * kDiscGroups - 1) * 256;                   // first byte of staged group 0
+  const bool interior = row0 >= 0 && row0 + kDiscRows * 256ll <= n_int8;
+  for (int k = threadIdx.x; k < kDiscThreads * 16 + 1; k += kDiscThreads) {   // 16 vectors per row, 1 of the last row
+    uint32_t *dst = disc_smem + (k >> 4) * kDiscPitch + 4 * (k & 15);
+    const long long b = row0 + 16ll * k;
+    if (interior || (b >= 0 && b + 16 <= n_int8)) {
+      cp_async16(dst, cap_base + b);
+    } else {
+      uint32_t v[4] = {0u, 0u, 0u, 0u};
+      for (int q = 0; q < 16; ++q)
+        if (b + q >= 0 && b + q < n_int8) v[q >> 2] |= (uint32_t)(uint8_t)cap_base[b + q] << (8 * (q & 3));
+      *reinterpret_cast<uint4 *>(dst) = make_uint4(v[0], v[1], v[2], v[3]);
+    }
+  }
+  asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
+  __syncthreads();
+  {
+    const uint4 *row = reinterpret_cast<const uint4 *>(disc_smem + threadIdx.x * kDiscPitch);
+    auto word = [&](int k) -> uint32_t {
+      if (k == 64) return row[kDiscPitch / 4].x;                            // first sample of the next group
+      const uint4 v = row[k >> 2];
+      return (k & 3) == 0 ? v.x : (k & 3) == 1 ? v.y : (k & 3) == 2 ? v.z : v.w;
+    };
+    uint32_t acc[4] = {0u, 0u, 0u, 0u};
+    dbits_group_dense(word, acc);
+    pdw[threadIdx.x] = make_uint4(acc[0], acc[1], acc[2], acc[3]);
+  }
+  __syncthreads();
+  const int j = threadIdx.x;
+  const long long g = tile * kDiscGroups + j, n_samples = n_int8 / 2;
+  if (j >= kDiscGroups || 128 * g > n_samples - 286) return;               // no window start of this group lies inside
+  const bool edge = g == 0 || 128 * g + 127 > n_samples - 286;
+  const uint32_t wh0 = __ldg(&params[stream].whiten[0]), wh1 = __ldg(&params[stream].whiten[1]);
+  const uint4 p0 = pdw[j], p1 = pdw[j + 1], p2 = pdw[j + 2], p3 = pdw[j + 3], p4 = pdw[j + 4];
+#pragma unroll
+  for (int ph = 0; ph < 4; ++ph) {
+    auto at = [&](const uint4 &p) { return ph == 0 ? p.x : ph == 1 ? p.y : ph == 2 ? p.z : p.w; };
+    const uint32_t w[5] = {at(p0), at(p1), at(p2), at(p3), at(p4)};
+    uint32_t m = empty_pdu_windows(w, wh0);
+    if (edge) m &= empty_pdu_inside(g, ph, n_samples);
+    while (m) {
+      const int i = __ffs((int)m) - 1;
+      m &= m - 1;
+      uint32_t aa, header, crc_rx;
+      empty_pdu_fields(w, i, wh0, wh1, aa, header, crc_rx);
+      const uint32_t crc_init = crc_init_reorder(crc24_unwind(crc_rx, header, 16));
+      const unsigned k = atomicAdd(count, 1u);
+      if (k < cap) {
+        const long long n0 = 128 * g + 4 * i + ph;
+        uint4 *d = reinterpret_cast<uint4 *>(out + k);
+        d[0] = make_uint4((uint32_t)n0, (uint32_t)(n0 >> 32), (uint32_t)stream, aa);
+        d[1] = make_uint4(crc_init, (uint32_t)__ldg(&params[stream].channel) | (header << 8), 0u, 0u);
+      }
+    }
+  }
+}
+
 // ---- BER flow of python/test_btle_ber.py on the device: packet source + channel + int16 truncation --------------------
 // One CTA per packet: 37 random payload bytes behind the fixed header 42 25 (test_btle_ber.py:27,:49), CRC-24, whitening,
 // the Python model's 8-sps modulator (same arithmetic as tx_modulate_kernel<8>), add_freq_sampling_error (linear
@@ -1428,6 +1508,8 @@ struct btle_b200_ctx {
   int8_t *h_stage[2] = {nullptr, nullptr}; size_t h_stage_bytes = 0;   // pinned staging for pageable callers
   cudaEvent_t stage_free[2] = {nullptr, nullptr};
   void *d_leaf = nullptr; size_t d_leaf_bytes = 0;
+  btle_conn_cand *d_cand = nullptr; size_t d_cand_bytes = 0;   // device candidates of btle_b200_discover
+  bool attr_disc_done = false;
 };
 
 namespace {
@@ -1700,11 +1782,52 @@ int launch_sps8_hits(btle_b200_ctx *ctx, const int16_t *d_iq16, size_t n_samples
 
 int leaf_buf(btle_b200_ctx *ctx, size_t bytes) { return ensure(ctx, &ctx->d_leaf, &ctx->d_leaf_bytes, bytes); }
 
+// Checks and launch of discover_kernel (the counter is zeroed here).  The channels travel as btle_stream_cfg through the
+// cfg cache, so the kernel reads each capture's whitening words from its StreamParams.
+int check_data_channels(btle_b200_ctx *ctx, const int32_t *channels, size_t n_streams) {
+  if (!channels && n_streams) { ctx->err = "discover: missing channel array"; return BTLE_EINVAL; }
+  for (size_t s = 0; s < n_streams; ++s)
+    if (channels[s] < 0 || channels[s] > 36) { ctx->err = "discover: data channel must be within 0~36"; return BTLE_EINVAL; }
+  return BTLE_OK;
+}
+
+int launch_discover(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8, const int32_t *channels,
+                    btle_conn_cand *d_out, size_t cap, unsigned *d_count, cudaStream_t st) {
+  if (!d_count || (!d_out && cap) || (!d_iq && n_streams && n_int8)) { ctx->err = "discover: missing buffer"; return BTLE_EINVAL; }
+  if ((reinterpret_cast<uintptr_t>(d_iq) & 15) || (n_streams > 1 && (stride & 15))) { ctx->err = "device IQ must be 16-byte aligned"; return BTLE_EINVAL; }
+  if (n_streams > 1 && stride < n_int8) { ctx->err = "stream stride smaller than stream length"; return BTLE_EINVAL; }
+  int rc = check_data_channels(ctx, channels, n_streams);
+  if (rc) return rc;
+  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
+  ctx->last_launches = 0;
+  BTLE_CUDA(ctx, cudaMemsetAsync(d_count, 0, sizeof(unsigned), st));
+  const long long n_samples = (long long)(n_int8 / 2);
+  if (!n_streams || n_samples < 32 + 286) return BTLE_OK;                  // no window fits
+  const long long groups = (n_samples - 286) / 128 + 1;                    // groups holding a window start inside the capture
+  const long long tiles = (groups + kDiscGroups - 1) / kDiscGroups;
+  if (tiles * (long long)n_streams > 0x7FFFFFFFll) { ctx->err = "batch too large for one launch"; return BTLE_EINVAL; }
+  std::vector<btle_stream_cfg> cfgs(n_streams);
+  for (size_t s = 0; s < n_streams; ++s) cfgs[s] = btle_stream_cfg{channels[s], 0x8E89BED6u, 0xFFFFFFFFu, 0x555555u, 0, 0};
+  CfgSlot *cs = nullptr;
+  rc = upload_cfgs(ctx, cfgs.data(), n_streams, st, &cs);
+  if (rc) return rc;
+  if (!ctx->attr_disc_done) {
+    BTLE_CUDA(ctx, cudaFuncSetAttribute(discover_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDiscSmem));
+    ctx->attr_disc_done = true;
+  }
+  discover_kernel<<<(unsigned)(tiles * (long long)n_streams), kDiscThreads, kDiscSmem, st>>>(
+      d_iq, (long long)stride, (long long)n_int8, tiles, cs->d_params, d_out, (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu), d_count);
+  BTLE_CUDA(ctx, cudaGetLastError());
+  BTLE_CUDA(ctx, cudaEventRecord(cs->last_use, st));
+  ctx->last_launches = 1;
+  return BTLE_OK;
+}
+
 }  // namespace
 
 extern "C" {
 
-uint32_t btle_b200_version(void) { return (0u << 16) | 1u; }
+uint32_t btle_b200_version(void) { return (0u << 16) | 2u; }
 
 const char *btle_b200_strerror(int code) {
   switch (code) {
@@ -1823,7 +1946,7 @@ void btle_b200_destroy(btle_b200_ctx *ctx) {
   cudaSetDevice(ctx->device);
   if (ctx->stream) cudaStreamDestroy(ctx->stream);
   if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
-  cudaFree(ctx->d_iq); cudaFree(ctx->d_out); cudaFree(ctx->d_dir); cudaFree(ctx->d_count); cudaFree(ctx->d_count_ring); cudaFree(ctx->d_leaf);
+  cudaFree(ctx->d_iq); cudaFree(ctx->d_out); cudaFree(ctx->d_dir); cudaFree(ctx->d_count); cudaFree(ctx->d_count_ring); cudaFree(ctx->d_leaf); cudaFree(ctx->d_cand);
   for (CfgSlot &c : ctx->cfg_slot) { cudaFree(c.d); cudaFree(c.d_params); if (c.last_use) cudaEventDestroy(c.last_use); }
   if (ctx->h_count) cudaFreeHost(ctx->h_count);
   if (ctx->h_recs) cudaFreeHost(ctx->h_recs);
@@ -2406,6 +2529,46 @@ int btle_b200_sps8_hits_device(btle_b200_ctx *ctx, const int16_t *d_iq16, size_t
   if (rc) return rc;
   BTLE_CUDA(ctx, cudaGetLastError());
   ctx->last_launches = 1;
+  return BTLE_OK;
+}
+
+int btle_b200_discover_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8,
+                              const int32_t *channels, btle_conn_cand *d_out, size_t cap, uint32_t *d_count, void *cuda_stream) {
+  if (!ctx) return BTLE_EINVAL;
+  return launch_discover(ctx, d_iq, n_streams, stride, n_int8, channels, d_out, cap, d_count, reinterpret_cast<cudaStream_t>(cuda_stream));
+}
+
+int btle_b200_discover(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stride, size_t n_int8, const int32_t *channels,
+                       btle_conn_cand *out, size_t cap, size_t *n_out) {
+  if (!ctx) return BTLE_EINVAL;
+  if (!n_out || (!out && cap) || (!iq && n_streams && n_int8)) { ctx->err = "discover: missing buffer"; return BTLE_EINVAL; }
+  *n_out = 0;
+  if (n_streams > 1 && stride < n_int8) { ctx->err = "stream stride smaller than stream length"; return BTLE_EINVAL; }
+  int rc = check_data_channels(ctx, channels, n_streams);                  // before any byte is copied
+  if (rc) return rc;
+  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t pitch = (n_int8 + 15) & ~size_t(15);
+  rc = ensure(ctx, reinterpret_cast<void **>(&ctx->d_iq), &ctx->d_iq_bytes, std::max<size_t>(pitch * n_streams, 16));
+  if (rc) return rc;
+  rc = ensure(ctx, reinterpret_cast<void **>(&ctx->d_cand), &ctx->d_cand_bytes, std::max<size_t>(cap, 1) * sizeof(btle_conn_cand));
+  if (rc) return rc;
+  rc = h2d_rows(ctx, ctx->d_iq, pitch, iq, n_streams > 1 ? stride : n_int8, n_int8, n_streams, st);
+  if (rc) return rc;
+  rc = launch_discover(ctx, ctx->d_iq, n_streams, pitch, n_int8, channels, ctx->d_cand, cap, ctx->d_count, st);
+  if (rc) return rc;
+  BTLE_CUDA(ctx, cudaMemcpyAsync(ctx->h_count, ctx->d_count, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+  BTLE_CUDA(ctx, cudaStreamSynchronize(st));
+  const size_t found = *ctx->h_count, n = std::min(found, cap);
+  *n_out = found;
+  if (n) {
+    BTLE_CUDA(ctx, cudaMemcpyAsync(out, ctx->d_cand, n * sizeof(btle_conn_cand), cudaMemcpyDeviceToHost, st));
+    BTLE_CUDA(ctx, cudaStreamSynchronize(st));
+    std::sort(out, out + n, [](const btle_conn_cand &a, const btle_conn_cand &b) {
+      return a.stream != b.stream ? a.stream < b.stream : a.sample < b.sample;
+    });
+  }
+  if (found > cap) { ctx->err = "output capacity too small"; return BTLE_EOVERFLOW; }
   return BTLE_OK;
 }
 

@@ -14,7 +14,9 @@ receive kernel over the 37 data-channel captures once per connection with that c
 the hop sequence is used to attribute each data packet to a connection event.  follow_connections_windowed(): the same
 result from three batched launches in total — only the windows the virtual radio of each connection would dwell in are
 decoded (about two single-channel passes per connection instead of 37).  Same rules as the reference: only full channel maps
-(`chm_is_full_map`, :2395-2400) are tracked, others are reported as dropped."""
+(`chm_is_full_map`, :2395-2400) are tracked, others are reported as dropped.
+discover_connections(): connections whose CONNECT_REQ was not captured, found from the empty PDUs on the data channels
+(the GPU candidate scan BtleRx.discover); follow_connections(discover=True) follows them as well."""
 from __future__ import annotations
 
 import numpy as np
@@ -49,12 +51,14 @@ def parse_connect_req(rec):
     }
 
 
-def _walk_events(c, per_ch, n_samples, max_events=10000):
+def _walk_events(c, per_ch, n_samples, max_events=10000, first_channel=None):
     """The reference's state machine (states 1-3 of receiver_controller, btle_rx.c:2455-2530) over per-channel lists of
     the connection's data-channel records.  Returns (events, queries): queries = the (channel, t_lo, t_hi) ranges the walk
-    looked at, so that a caller that decoded only windows can verify it had decoded all of them."""
+    looked at, so that a caller that decoded only windows can verify it had decoded all of them.  The walk waits from
+    c["t"] on its first channel: hop % 37 as after a CONNECT_REQ, or `first_channel` (a discovered connection)."""
     interval_s = c["interval"] * 1250e-6                                                  # :2430
-    events, queries, chan, t_mark, anchored = [], [], 0, None, True
+    chan = 0 if first_channel is None else (first_channel - c["hop"]) % 37
+    events, queries, t_mark, anchored = [], [], None, True
     for k in range(max_events):
         chan = (chan + c["hop"]) % 37                                                     # :2434 / :2476
         pk = per_ch[chan]
@@ -220,11 +224,15 @@ def follow_connections_windowed(rx, captures: np.ndarray, first_search_chunks: i
     return adv, conns
 
 
-def follow_connections(rx, captures: np.ndarray, max_events: int = 10000):
+def follow_connections(rx, captures: np.ndarray, max_events: int = 10000, discover: bool = False):
     """captures: int8 [40, n_int8], row c = BLE channel c, all rows time-aligned.
     `rx` needs `rx_batch(iq, cfgs)` (a BtleRx).  Returns (adv_records, connections) where each
     connection is the parse_connect_req dict plus `tracked`, and, if tracked, `events`: a list of
-    {"k", "channel", "t", "packets"} with `packets` the data-channel records of that event."""
+    {"k", "channel", "t", "packets"} with `packets` the data-channel records of that event.
+    discover=True (`rx` then also needs `discover(iq, channels)`): the connections discover_connections() finds on the
+    data channels are appended, and every tracked one whose access address is not that of a tracked CONNECT_REQ is
+    followed the same way, its walk starting on `first_channel` 1.25 ms before `t_first` (so that a master packet in
+    front of the first empty PDU anchors it)."""
     captures = np.ascontiguousarray(captures, dtype=np.int8)
     assert captures.shape[0] == 40
     adv = rx.rx_batch(captures[37:40], make_cfgs(3, channel=[37, 38, 39]))
@@ -239,17 +247,80 @@ def follow_connections(rx, captures: np.ndarray, max_events: int = 10000):
         # reported as not tracked here — a deliberate difference.)
         c["tracked"] = c["chm"] == "1fffffffff" and c["interval"] > 0
         conns.append(c)
-    for c in conns:
-        if not c["tracked"]:
-            continue
+    walks = [(c, c, None) for c in conns if c["tracked"]]
+    if discover:
+        known = {c["access_addr"] for c in conns if c["tracked"]}
+        found = discover_connections(rx, captures)
+        conns += found
+        walks += [(c, dict(c, t=c["t_first"] - DISCOVER_LEAD_S), c["first_channel"]) for c in found
+                  if c["tracked"] and c["access_addr"] not in known]
+    for c, walk, first_channel in walks:
         cfgs = make_cfgs(37, channel=list(range(37)), access_addr=c["access_addr"], crc_init=c["crc_init"])
         data = rx.rx_batch(captures[0:37], cfgs)
         per_ch = {ch: [] for ch in range(37)}
         for r in data:
-            if record_time(r) > c["t"]:
+            if record_time(r) > walk["t"]:
                 per_ch[int(r["channel"])].append(r)
-        c["events"] = _walk_events(c, per_ch, captures.shape[1] // 2, max_events)[0]
+        c["events"] = _walk_events(walk, per_ch, captures.shape[1] // 2, max_events, first_channel)[0]
     return adv, conns
+
+
+# ---- connections whose CONNECT_REQ was not captured (DESIGN.md §6.2) ----------------------------------------------------
+EVENT_SPAN_S = 3.75e-3   # candidates on one channel within half the shortest interval (7.5 ms) of the first are one event
+DISCOVER_LEAD_S = 1.25e-3   # a discovered connection's walk starts this long before its first empty PDU
+
+
+def _connection_from_events(aa, crc_init, events, n_candidates):
+    """events: [(t, channel)] in time order -> the discovered-connection dict.  The interval is the GCD of the gaps
+    between consecutive events in 1.25 ms units; with CSA#1 and a full channel map ch' = ch + hop (mod 37) per interval,
+    so a gap of m intervals gives hop = dch * m^-1 (mod 37).  `tracked` only if the interval lies in 6..3200 and every
+    pair gives the same non-zero hop; otherwise (a partial channel map, CSA#2) interval / hop are None."""
+    units = [int(round((b[0] - a[0]) / 1.25e-3)) for a, b in zip(events, events[1:])]
+    interval, hop = 0, None
+    for u in units:
+        interval = int(np.gcd(interval, u))
+    ok = 6 <= interval <= 3200
+    if ok:
+        hops = set()
+        for (_, ca), (_, cb), u in zip(events, events[1:], units):
+            m = (u // interval) % 37
+            if m == 0:                            # 37k intervals: back on the same channel, no information on the hop
+                ok = ok and ca == cb
+                continue
+            hops.add((cb - ca) * pow(m, -1, 37) % 37)
+        ok = ok and len(hops) == 1 and 0 not in hops
+        hop = hops.pop() if ok else None
+    return {"access_addr": aa, "crc_init": crc_init, "hop": hop, "interval": interval if ok else None, "chm": "1fffffffff",
+            "t_first": events[0][0], "first_channel": events[0][1], "n_events": len(events), "n_candidates": n_candidates,
+            "discovered": True, "adv_channel": None, "init_a": None, "adv_a": None, "tracked": ok}
+
+
+def discover_connections(rx, captures: np.ndarray, min_events: int = 4):
+    """Connections found from their empty PDUs alone, without a CONNECT_REQ.  captures: int8 [40, n_int8] as in
+    follow_connections(); rows 0..36 are scanned in one rx.discover() call.  Candidates are grouped by (access address,
+    CRC init); in a group, sorted by sample, candidates on the channel of the current event within 3.75 ms of its first
+    candidate belong to it, any other starts the next event (time = first candidate's sample / 4 Msps).  Groups with fewer
+    than `min_events` events are noise and are dropped.  Returns the _connection_from_events() dicts in order of t_first."""
+    captures = np.ascontiguousarray(captures, dtype=np.int8)
+    assert captures.shape[0] == 40
+    cand = rx.discover(captures[0:37], np.arange(37, dtype=np.int32))
+    if len(cand) == 0:
+        return []
+    cand = cand[np.lexsort((cand["sample"], cand["crc_init"], cand["access_addr"]))]
+    key = cand["access_addr"].astype(np.int64) << 24 | cand["crc_init"].astype(np.int64)
+    cuts = np.flatnonzero(np.diff(key)) + 1
+    conns = []
+    for grp in np.split(cand, cuts):
+        events = []
+        for r in grp:
+            t, ch = int(r["sample"]) / SAMPLE_RATE, int(r["channel"])
+            if events and ch == events[-1][1] and t - events[-1][0] < EVENT_SPAN_S:
+                continue
+            events.append((t, ch))
+        if len(events) >= min_events:
+            conns.append(_connection_from_events(int(grp[0]["access_addr"]), int(grp[0]["crc_init"]), events, len(grp)))
+    conns.sort(key=lambda c: (c["t_first"], c["access_addr"]))
+    return conns
 
 
 def channel_freq_mhz(channel: int) -> int:
@@ -271,12 +342,16 @@ def hop_events(conns) -> list:
     """The NDJSON `hop` events (btle_json.h:21-24) the reference's FSM emits for these connections
     (`btj_emit_hop` call sites btle_rx.c:2420, :2448, :2486, :2520), with sample time as `ts`:
       track_drop   0->0  CONNECT_REQ without a full channel map (:2417-2424), stays on the advertising channel
-      track_start  0->1  CONNECT_REQ accepted, first data channel (:2427-2450)
+      track_start  0->1  CONNECT_REQ accepted, first data channel (:2427-2450); for a tracked discovered connection
+                         (discover_connections) at t_first on first_channel
+    Untracked discovered connections emit nothing.
       chan_change  2->3  hop after an event that had a CRC-ok packet (:2472-2488)
       chan_change  3->3  hop after an event without one, "Hop: skip" (:2504-2522)
     Returns dicts in time order; hop_events_ndjson() formats them."""
     out = []
     for c in conns:
+        if c.get("discovered") and not c.get("tracked"):
+            continue                             # a channel sequence the follower cannot predict: nothing to emit
         base = {"v": 1, "t": "hop", "aa": f"{c['access_addr']:08x}", "crc_init": f"{c['crc_init'] & 0xFFFFFF:06x}",
                 "hop": c["hop"], "chm": c["chm"]}
         if not c.get("tracked"):
@@ -284,8 +359,11 @@ def hop_events(conns) -> list:
                             interval_us=0))
             continue
         interval_us = c["interval"] * 1250                                                    # :2430
-        first_ch = c["hop"] % 37                                                              # :2434
-        out.append(dict(base, ts=c["t"], event="track_start", state_from=0, state_to=1, ch=first_ch,
+        if c.get("discovered"):                  # no CONNECT_REQ: tracking starts with the first empty PDU seen
+            ts, first_ch = c["t_first"], c["first_channel"]
+        else:
+            ts, first_ch = c["t"], c["hop"] % 37                                              # :2434
+        out.append(dict(base, ts=ts, event="track_start", state_from=0, state_to=1, ch=first_ch,
                         freq_mhz=channel_freq_mhz(first_ch), interval_us=interval_us))
         ev = c.get("events", [])
         for prev, e in zip(ev, ev[1:]):

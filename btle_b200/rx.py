@@ -11,7 +11,7 @@ import ctypes
 import numpy as np
 
 from . import _native
-from ._native import BTLE_EOVERFLOW, BtleError, CFG_DTYPE, DIR_DTYPE, REC_DTYPE
+from ._native import BTLE_EOVERFLOW, BtleError, CAND_DTYPE, CFG_DTYPE, DIR_DTYPE, REC_DTYPE
 
 DEFAULT_ACCESS_ADDR = 0x8E89BED6     # btle_rx.c:231
 DEFAULT_CRC_INIT = 0x555555          # btle_rx.c:232
@@ -109,6 +109,28 @@ class BtleRx:
                                               ctypes.byref(n_out)))
         return out[:n_out.value]
 
+    def discover(self, iq: np.ndarray, channels, cap: int | None = None) -> np.ndarray:
+        """Empty-PDU candidates of connection discovery (btle_b200_discover): iq int8 [n_streams, n_int8] (or [n_int8]) of
+        data-channel captures, channels[s] in 0..36 the channel of capture s.  Returns CAND_DTYPE records sorted by
+        (stream, sample); `cap` defaults to a typical worst case and is grown once to the exact count on overflow."""
+        iq = np.ascontiguousarray(iq, dtype=np.int8)
+        if iq.ndim == 1:
+            iq = iq[None, :]
+        ns, n = iq.shape
+        ch = np.ascontiguousarray(np.broadcast_to(np.asarray(channels, dtype=np.int32), (ns,)))
+        grow = cap is None
+        if cap is None:
+            cap = ns * (n // 16384 + 1) * 8 + 256
+        while True:
+            out = np.empty(cap, dtype=CAND_DTYPE)
+            n_out = ctypes.c_size_t(0)
+            rc = self._L.btle_b200_discover(self._h, iq.ctypes.data, ns, n, n, ch.ctypes.data, out.ctypes.data, cap, ctypes.byref(n_out))
+            if rc == BTLE_EOVERFLOW and grow:
+                cap, grow = n_out.value, False
+                continue
+            self._check(rc)
+            return out[:n_out.value]
+
     # ---- unbounded capture, pushed in pieces (btle_b200_stream_*) -----------------------------
     def stream(self, segment_chunks: int = 0, **cfg) -> "RxStream":
         """Streaming session over one capture of any length: `with rx.stream(channel=37) as s: recs = s.push(iq_piece) ...;
@@ -135,6 +157,18 @@ class BtleRx:
         cap = d_out.numel() // 64
         rc = self._L.btle_b200_rx_device(self._h, d_iq.data_ptr(), ns, d_iq.stride(0), n, cfgs.ctypes.data,
                                          d_out.data_ptr(), cap, d_count.data_ptr(), ctypes.c_void_p(stream_ptr))
+        self._check(rc)
+
+    def discover_device(self, d_iq, channels, d_out, d_count, stream_ptr: int = 0):
+        """d_iq: torch int8 CUDA tensor [n_streams, n_int8] (16-byte aligned rows); channels: the data channel of each row;
+        d_out: torch CUDA tensor of cap * 32 bytes; d_count: torch int32 CUDA tensor [1].  Enqueues on `stream_ptr` (no
+        sync).  Candidates land unordered in d_out[:min(count, cap)] (view the bytes as CAND_DTYPE)."""
+        ns, n = d_iq.shape
+        assert d_iq.stride(1) == 1
+        ch = np.ascontiguousarray(np.broadcast_to(np.asarray(channels, dtype=np.int32), (ns,)))
+        cap = d_out.numel() * d_out.element_size() // 32
+        rc = self._L.btle_b200_discover_device(self._h, d_iq.data_ptr(), ns, d_iq.stride(0), n, ch.ctypes.data, d_out.data_ptr(), cap,
+                                               d_count.data_ptr(), ctypes.c_void_p(stream_ptr))
         self._check(rc)
 
     def units(self, n_streams: int, n_int8: int) -> int:

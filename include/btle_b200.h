@@ -202,6 +202,41 @@ int btle_b200_streams_set_cfg(btle_b200_streams *s, size_t stream, const btle_st
 int btle_b200_streams_finish(btle_b200_streams *s, btle_pkt_rec *out, size_t cap, size_t *n_out);
 void btle_b200_streams_close(btle_b200_streams *s);
 
+/* ---- connection discovery: empty-PDU candidates on data-channel captures, no access address given ------------------
+ * Connections whose CONNECT_REQ was not captured are found from their data packets: every idle connection event carries
+ * an empty PDU, whose header is fixed but for 3 bits and which is never encrypted.  Sample n0 of a capture on data
+ * channel `ch` (0..36) is a CANDIDATE iff, with d[n] = (I[n]Q[n+1] - I[n+1]Q[n]) > 0:
+ *   - the 9 bits d[n0 - 32 + 4j] (j = 0..7) and d[n0] alternate (preamble 0x55 or 0xAA);
+ *   - the 16 bits d[n0 + 4(32 + j)] (j = 0..15), LSB first, dewhitened with the first 16 whitening bits of `ch`, have
+ *     LLID 1 (bits 0..1) and byte 1 == 0 (length 0, RFU 0);
+ *   - every d[n] read lies inside the capture: n0 >= 32 and n0 + 285 < n_int8 / 2.
+ * Every sample index is tested; one packet usually gives 2-3 candidates at adjacent n0.  access_addr = d[n0 + 4i]
+ * (i = 0..31) LSB first; crc_init is the unique -k value for which the CRC-24 of the two header bytes equals the
+ * received CRC d[n0 + 4(48 + j)] (j = 0..23) dewhitened with whitening bits 16..39 (the LFSR is run backwards).
+ * For a packet that btle_b200_rx_batch() decodes with that access address and CRC init, sample == chunk * 8192 + n0
+ * of its record. */
+typedef struct {
+  int64_t sample;        /* n0: first IQ sample of the access address, from the start of the capture            */
+  int32_t stream;
+  uint32_t access_addr;
+  uint32_t crc_init;     /* -k convention (not reordered)                                                      */
+  uint8_t channel;
+  uint8_t header[2];     /* dewhitened: LLID 1, length 0                                                       */
+  uint8_t reserved[9];
+} btle_conn_cand;        /* 32 bytes */
+/* device: `d_iq` 16-byte aligned, stride a multiple of 16 and >= n_int8 when n_streams > 1; channels[s] (host array) is
+ * the data channel of capture s.  Candidates are unordered; *d_count (zeroed by the call) = number found,
+ * d_out[0..min(count, cap)) holds them.  Enqueued on cuda_stream, not synchronised.  n_streams == 0 and captures too
+ * short for one window give 0 candidates.  A channel outside 0..36, a misaligned pointer or stride or a missing buffer
+ * is BTLE_EINVAL with btle_b200_last_error() set. */
+int btle_b200_discover_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stream_stride_int8,
+                              size_t n_int8, const int32_t *channels, btle_conn_cand *d_out, size_t cap,
+                              uint32_t *d_count, void *cuda_stream);
+/* host buffers (page-locked or pageable, as btle_b200_rx_batch); out sorted by (stream, sample).  BTLE_EOVERFLOW with
+ * *n_out = the number found when that exceeds cap (out then holds cap of them, not necessarily the first ones). */
+int btle_b200_discover(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stream_stride_int8, size_t n_int8,
+                       const int32_t *channels, btle_conn_cand *out, size_t cap, size_t *n_out);
+
 /* number of kernels the last rx call launched (bench.py's gpu_launches) */
 int btle_b200_last_launches(const btle_b200_ctx *ctx);
 
