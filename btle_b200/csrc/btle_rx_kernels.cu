@@ -1469,12 +1469,21 @@ model_rx_batch_kernel(const int16_t *__restrict__ gi, const int16_t *__restrict_
 // ================================================================================================
 // C-ABI
 // ================================================================================================
+constexpr unsigned kCountRing = 64;  // context-owned allocation counters (launch_rx)
+constexpr int kSlotUsers = 4;        // streams whose last launch is tracked per cfg slot (more share one entry, see note_use)
+struct StreamUse {                   // the last launch a stream enqueued: CUDA's id of the stream + an event behind it
+  unsigned long long stream = 0;
+  cudaEvent_t ev = nullptr;
+  unsigned long long stamp = 0;      // 0: no launch recorded
+};
 struct CfgSlot {                     // one uploaded btle_stream_cfg array + the per-stream parameters derived from it
   btle_stream_cfg *d = nullptr; size_t cap = 0;   // (small LRU cache, see upload_cfgs)
   StreamParams *d_params = nullptr;
-  std::vector<StreamParams> host_params;
-  std::vector<btle_stream_cfg> host;
-  cudaEvent_t last_use = nullptr;
+  btle_stream_cfg *h = nullptr; StreamParams *h_params = nullptr;   // page-locked sources of the upload (cap entries)
+  size_t n = 0;                      // entries of the cached array (0: empty)
+  unsigned long long up_stream = 0;  // stream the upload was enqueued on
+  cudaEvent_t uploaded = nullptr;    // recorded behind the upload's two copies
+  StreamUse use[kSlotUsers];         // last launch of each stream that read this upload
   unsigned long long stamp = 0;
 };
 struct MapSlot {                     // encoded TMA tensor maps of one (pointer, shape) combination
@@ -1501,6 +1510,7 @@ struct btle_b200_ctx {
   unsigned *d_count = nullptr;
   unsigned *d_count_ring = nullptr; // kCountRing allocation counters for launches that do not hand in their own (no memset node)
   unsigned ring_pos = 0;
+  StreamUse ring_last[kCountRing / 2];   // [ring_pos % (kCountRing/2)]: the ring launch that next launch depends on (launch_rx)
   size_t lead_bytes = 0;            // bytes readable in front of d_iq (set by the stream session around its launches; RSSI of hits at a segment's very start)
   unsigned *h_count = nullptr;      // pinned
   btle_pkt_rec *h_recs = nullptr; size_t h_recs_cap = 0;   // pinned staging for records
@@ -1546,45 +1556,91 @@ int validate_cfgs(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size_t n) {
   return BTLE_OK;
 }
 
-// The cfg array of a launch must live on the device while the kernel runs.  Uploaded arrays are kept in a small
-// LRU cache keyed by content; re-using a slot whose last launch may still be running on ANOTHER stream is made safe
-// by a stream-side wait on that launch's event (no host or device-wide synchronisation).
-constexpr unsigned kCountRing = 64;
+// CUDA's id of a stream: unique for the life of the process (a handle can be re-used by a stream created later).
+int stream_id(btle_b200_ctx *ctx, cudaStream_t st, unsigned long long *sid) {
+  BTLE_CUDA(ctx, cudaStreamGetId(st, sid));
+  return BTLE_OK;
+}
 
-int upload_cfgs(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size_t n, cudaStream_t st, CfgSlot **slot_out) {
+// The cfg array of a launch must live on the device while the kernel runs.  Uploaded arrays are kept in a small LRU
+// cache keyed by content, shared by launches on any stream.  Two orders keep it right without host or device-wide
+// synchronisation:
+//   - a launch that finds its array in the cache waits for the upload when the upload went to another stream and this
+//     stream has not launched with it since (in steady state the event has long completed, and the wait is made once);
+//   - the upload that evicts a slot waits for the slot's previous upload and for the last launch of EVERY stream that
+//     read it (note_use), so a launch still held on one stream keeps its parameters.
+// A launch never waits for another stream's kernel: two pipes that alternate over the same arrays still overlap.
+// The copies come from page-locked staging, so enqueueing them never blocks the host behind a busy stream; the host
+// waits only when it must rewrite a staging buffer whose previous copy has not run yet.
+int upload_cfgs(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size_t n, cudaStream_t st, unsigned long long sid, CfgSlot **slot_out) {
   CfgSlot *pick = nullptr;
   for (CfgSlot &c : ctx->cfg_slot)
-    if (c.d && c.host.size() == n && !memcmp(c.host.data(), cfgs, n * sizeof(btle_stream_cfg))) { pick = &c; break; }
-  if (!pick) {
+    if (c.n == n && !memcmp(c.h, cfgs, n * sizeof(btle_stream_cfg))) { pick = &c; break; }
+  if (pick) {
+    bool seen = pick->up_stream == sid;
+    for (const StreamUse &u : pick->use) seen |= u.stamp && u.stream == sid;
+    if (!seen) BTLE_CUDA(ctx, cudaStreamWaitEvent(st, pick->uploaded, 0));
+  } else {
     pick = &ctx->cfg_slot[0];
     for (CfgSlot &c : ctx->cfg_slot) if (c.stamp < pick->stamp) pick = &c;
-    if (!pick->last_use) BTLE_CUDA(ctx, cudaEventCreateWithFlags(&pick->last_use, cudaEventDisableTiming));
+    if (!pick->uploaded) BTLE_CUDA(ctx, cudaEventCreateWithFlags(&pick->uploaded, cudaEventDisableTiming));
+    if (pick->n) {
+      if (pick->up_stream != sid) BTLE_CUDA(ctx, cudaStreamWaitEvent(st, pick->uploaded, 0));
+      for (const StreamUse &u : pick->use)
+        if (u.stamp && u.stream != sid) BTLE_CUDA(ctx, cudaStreamWaitEvent(st, u.ev, 0));
+    }
     if (pick->cap < n) {
-      if (pick->d) cudaFree(pick->d);                        // (cudaFree waits for work that still uses it)
+      if (pick->d) cudaFree(pick->d);                        // (cudaFree / cudaFreeHost wait for work that still uses them)
       if (pick->d_params) cudaFree(pick->d_params);
-      pick->d = nullptr; pick->d_params = nullptr; pick->cap = 0;
+      if (pick->h) cudaFreeHost(pick->h);
+      if (pick->h_params) cudaFreeHost(pick->h_params);
+      pick->d = nullptr; pick->d_params = nullptr; pick->h = nullptr; pick->h_params = nullptr; pick->cap = 0; pick->n = 0;
       const size_t want = n + n / 4 + 16;
-      if (cudaMalloc(&pick->d, want * sizeof(btle_stream_cfg)) != cudaSuccess || cudaMalloc(&pick->d_params, want * sizeof(StreamParams)) != cudaSuccess) {
+      if (cudaMalloc(&pick->d, want * sizeof(btle_stream_cfg)) != cudaSuccess || cudaMalloc(&pick->d_params, want * sizeof(StreamParams)) != cudaSuccess ||
+          cudaHostAlloc(&pick->h, want * sizeof(btle_stream_cfg), cudaHostAllocDefault) != cudaSuccess ||
+          cudaHostAlloc(&pick->h_params, want * sizeof(StreamParams), cudaHostAllocDefault) != cudaSuccess) {
         cudaGetLastError(); ctx->err = "cudaMalloc failed"; return BTLE_ENOMEM;
       }
       pick->cap = want;
-    } else if (pick->stamp) {
-      BTLE_CUDA(ctx, cudaStreamWaitEvent(st, pick->last_use, 0));
+    } else if (pick->n) {
+      BTLE_CUDA(ctx, cudaEventSynchronize(pick->uploaded));   // the staging still feeds the previous upload's copies
     }
-    pick->host.assign(cfgs, cfgs + n);
-    pick->host_params.resize(n);
+    pick->n = 0;
+    for (StreamUse &u : pick->use) u.stamp = 0;              // ordered before the new copies by the waits above
+    memcpy(pick->h, cfgs, n * sizeof(btle_stream_cfg));
     for (size_t i = 0; i < n; ++i) {                         // make_params(): btle_params.h, the same code the CPU emulator runs
       uint8_t row[48];
       make_whiten_row(cfgs[i].channel, row);
       uint32_t ww[12];
       memcpy(ww, row, 48);
-      make_params(cfgs[i], ww, pick->host_params[i]);
+      make_params(cfgs[i], ww, pick->h_params[i]);
     }
-    BTLE_CUDA(ctx, cudaMemcpyAsync(pick->d, pick->host.data(), n * sizeof(btle_stream_cfg), cudaMemcpyHostToDevice, st));
-    BTLE_CUDA(ctx, cudaMemcpyAsync(pick->d_params, pick->host_params.data(), n * sizeof(StreamParams), cudaMemcpyHostToDevice, st));
+    BTLE_CUDA(ctx, cudaMemcpyAsync(pick->d, pick->h, n * sizeof(btle_stream_cfg), cudaMemcpyHostToDevice, st));
+    BTLE_CUDA(ctx, cudaMemcpyAsync(pick->d_params, pick->h_params, n * sizeof(StreamParams), cudaMemcpyHostToDevice, st));
+    BTLE_CUDA(ctx, cudaEventRecord(pick->uploaded, st));
+    pick->up_stream = sid;
+    pick->n = n;
   }
   pick->stamp = ++ctx->tick;
   *slot_out = pick;
+  return BTLE_OK;
+}
+
+// After a launch on `st` that read `slot`: the event of st's entry now stands behind it.  With more than kSlotUsers
+// streams on one slot, the least recent entry is taken over, and st first waits for the launch it stood for, so the
+// entry still covers both (that orders st's LATER work behind the other stream; the launch just made runs freely).
+int note_use(btle_b200_ctx *ctx, CfgSlot *slot, cudaStream_t st, unsigned long long sid) {
+  StreamUse *u = nullptr;
+  for (StreamUse &x : slot->use) if (x.stamp && x.stream == sid) { u = &x; break; }
+  if (!u) {
+    u = &slot->use[0];
+    for (StreamUse &x : slot->use) if (x.stamp < u->stamp) u = &x;
+    if (!u->ev) BTLE_CUDA(ctx, cudaEventCreateWithFlags(&u->ev, cudaEventDisableTiming));
+    if (u->stamp) BTLE_CUDA(ctx, cudaStreamWaitEvent(st, u->ev, 0));
+  }
+  BTLE_CUDA(ctx, cudaEventRecord(u->ev, st));
+  u->stream = sid;
+  u->stamp = ++ctx->tick;
   return BTLE_OK;
 }
 
@@ -1633,15 +1689,9 @@ int launch_rx(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t s
   if (d_count) BTLE_CUDA(ctx, cudaMemsetAsync(d_count, 0, sizeof(unsigned), st));
   const long long nchunks = (long long)(n_int8 / kChunkInt8);
   if (nchunks == 0 || n_streams == 0) return BTLE_OK;
-  if (!d_count) {
-    // no counter from the caller (it reads the unit directory): take the next one of the context's ring.  It is zero —
-    // cleared at creation or by the launch kCountRing/2 launches ago — and this launch clears the one used kCountRing/2
-    // launches from now (no memset node in front of the kernel; far more launches than that cannot be in flight: every
-    // one occupies all SMs).
-    d_count = ctx->d_count_ring + ctx->ring_pos;
-    zero_next = ctx->d_count_ring + (ctx->ring_pos + kCountRing / 2) % kCountRing;
-    ctx->ring_pos = (ctx->ring_pos + 1) % kCountRing;
-  }
+  unsigned long long sid = 0;
+  int rc = stream_id(ctx, st, &sid);
+  if (rc) return rc;
   const long long spans = (nchunks + kSpanChunks - 1) / kSpanChunks;
   if (spans * (long long)n_streams > 0x07FFFFFFll || nchunks > 0x7FFFFFFFll) { ctx->err = "batch too large for one launch"; return BTLE_EINVAL; }
   const Plan plan = plan_for(ctx, n_streams, n_int8);
@@ -1651,17 +1701,37 @@ int launch_rx(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t s
     ctx->attr_done = true;
   }
   CfgSlot *cs = nullptr;
-  int rc = upload_cfgs(ctx, cfgs, n_streams, st, &cs);
+  rc = upload_cfgs(ctx, cfgs, n_streams, st, sid, &cs);
   if (rc) return rc;
   const MapSlot *ms = nullptr;
   rc = get_maps(ctx, d_iq, n_streams, stride, n_int8, &ms);
   if (rc) return rc;
+  StreamUse *ring = nullptr;
+  if (!d_count) {
+    // No counter from the caller (it reads the unit directory): take the next one of the context's ring, with no
+    // memset node in front of the kernel.  Launch i (counted over the ring launches that ran) takes counter i % 64,
+    // which launch i - 32 cleared, and clears counter (i + 32) % 64, which launch i - 32 used.  So launch i depends on
+    // launch i - 32 alone (and through it on all earlier ones).  On the same stream that order is given; on another
+    // stream this launch waits for its event.  One stream, or two in strict alternation, never waits.
+    ring = &ctx->ring_last[ctx->ring_pos % (kCountRing / 2)];
+    if (!ring->ev) BTLE_CUDA(ctx, cudaEventCreateWithFlags(&ring->ev, cudaEventDisableTiming));
+    if (ring->stamp && ring->stream != sid) BTLE_CUDA(ctx, cudaStreamWaitEvent(st, ring->ev, 0));
+    d_count = ctx->d_count_ring + ctx->ring_pos;
+    zero_next = ctx->d_count_ring + (ctx->ring_pos + kCountRing / 2) % kCountRing;
+  }
   const unsigned grid = (unsigned)std::min<long long>(plan.total_units, (long long)ctx->num_sms * kCtasPerSm);   // one persistent CTA per SM
   btle_rx_persistent_kernel<<<grid, kThreads, smem, st>>>(
       ms->map32, ms->map12, d_iq, (long long)stride, (long long)n_int8, cs->d_params, plan, d_out,
       (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu), d_count, reinterpret_cast<uint2 *>(d_dir), zero_next, (long long)ctx->lead_bytes);
   BTLE_CUDA(ctx, cudaGetLastError());
-  BTLE_CUDA(ctx, cudaEventRecord(cs->last_use, st));
+  if (ring) {                                                 // the position is taken only by a launch that was enqueued
+    ctx->ring_pos = (ctx->ring_pos + 1) % kCountRing;
+    BTLE_CUDA(ctx, cudaEventRecord(ring->ev, st));
+    ring->stream = sid;
+    ring->stamp = ++ctx->tick;
+  }
+  rc = note_use(ctx, cs, st, sid);
+  if (rc) return rc;
   ctx->last_launches = 1;
   return BTLE_OK;
 }
@@ -1808,8 +1878,11 @@ int launch_discover(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, si
   if (tiles * (long long)n_streams > 0x7FFFFFFFll) { ctx->err = "batch too large for one launch"; return BTLE_EINVAL; }
   std::vector<btle_stream_cfg> cfgs(n_streams);
   for (size_t s = 0; s < n_streams; ++s) cfgs[s] = btle_stream_cfg{channels[s], 0x8E89BED6u, 0xFFFFFFFFu, 0x555555u, 0, 0};
+  unsigned long long sid = 0;
+  rc = stream_id(ctx, st, &sid);
+  if (rc) return rc;
   CfgSlot *cs = nullptr;
-  rc = upload_cfgs(ctx, cfgs.data(), n_streams, st, &cs);
+  rc = upload_cfgs(ctx, cfgs.data(), n_streams, st, sid, &cs);
   if (rc) return rc;
   if (!ctx->attr_disc_done) {
     BTLE_CUDA(ctx, cudaFuncSetAttribute(discover_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDiscSmem));
@@ -1818,7 +1891,8 @@ int launch_discover(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, si
   discover_kernel<<<(unsigned)(tiles * (long long)n_streams), kDiscThreads, kDiscSmem, st>>>(
       d_iq, (long long)stride, (long long)n_int8, tiles, cs->d_params, d_out, (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu), d_count);
   BTLE_CUDA(ctx, cudaGetLastError());
-  BTLE_CUDA(ctx, cudaEventRecord(cs->last_use, st));
+  rc = note_use(ctx, cs, st, sid);
+  if (rc) return rc;
   ctx->last_launches = 1;
   return BTLE_OK;
 }
@@ -1947,7 +2021,14 @@ void btle_b200_destroy(btle_b200_ctx *ctx) {
   if (ctx->stream) cudaStreamDestroy(ctx->stream);
   if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
   cudaFree(ctx->d_iq); cudaFree(ctx->d_out); cudaFree(ctx->d_dir); cudaFree(ctx->d_count); cudaFree(ctx->d_count_ring); cudaFree(ctx->d_leaf); cudaFree(ctx->d_cand);
-  for (CfgSlot &c : ctx->cfg_slot) { cudaFree(c.d); cudaFree(c.d_params); if (c.last_use) cudaEventDestroy(c.last_use); }
+  for (CfgSlot &c : ctx->cfg_slot) {
+    cudaFree(c.d); cudaFree(c.d_params);
+    if (c.h) cudaFreeHost(c.h);
+    if (c.h_params) cudaFreeHost(c.h_params);
+    if (c.uploaded) cudaEventDestroy(c.uploaded);
+    for (StreamUse &u : c.use) if (u.ev) cudaEventDestroy(u.ev);
+  }
+  for (StreamUse &u : ctx->ring_last) if (u.ev) cudaEventDestroy(u.ev);
   if (ctx->h_count) cudaFreeHost(ctx->h_count);
   if (ctx->h_recs) cudaFreeHost(ctx->h_recs);
   if (ctx->h_dir) cudaFreeHost(ctx->h_dir);
@@ -2469,8 +2550,11 @@ int btle_b200_synth_streams_device(btle_b200_ctx *ctx, int8_t *d_iq, size_t n_st
   if (n_slots * n_streams > 0x7FFFFFFFull) { ctx->err = "synth: too many slots for one launch"; return BTLE_EINVAL; }
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+  unsigned long long sid = 0;
+  rc = stream_id(ctx, st, &sid);
+  if (rc) return rc;
   CfgSlot *cs = nullptr;
-  rc = upload_cfgs(ctx, cfgs, n_streams, st, &cs);
+  rc = upload_cfgs(ctx, cfgs, n_streams, st, sid, &cs);
   if (rc) return rc;
   synth_noise_kernel<<<ctx->num_sms * 8, 256, 0, st>>>(d_iq, (long long)stride, (long long)n_int8, (int)n_streams, sc->seed, sc->noise);
   BTLE_CUDA(ctx, cudaGetLastError());
@@ -2479,8 +2563,7 @@ int btle_b200_synth_streams_device(btle_b200_ctx *ctx, int8_t *d_iq, size_t n_st
                                                                           (long long)n_slots, d_truth);
     BTLE_CUDA(ctx, cudaGetLastError());
   }
-  BTLE_CUDA(ctx, cudaEventRecord(cs->last_use, st));
-  return BTLE_OK;
+  return note_use(ctx, cs, st, sid);
 }
 
 int btle_b200_model_rx_batch_device(btle_b200_ctx *ctx, const int16_t *d_i, const int16_t *d_q, size_t n_packets,

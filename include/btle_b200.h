@@ -142,7 +142,13 @@ int btle_b200_rx(btle_b200_ctx *ctx, const int8_t *iq, size_t n_int8, const btle
  * *d_count (uint32) is zeroed by the call; every d_dir entry of the launch is written (no memset needed).
  * btle_b200_rx_device_dir() accepts d_count == NULL: the block reservations then run on a context-owned counter (a ring
  * of them, each cleared by an earlier launch) and no memset is enqueued in front of the kernel — for callers that take
- * the packet count from the directory. */
+ * the packet count from the directory.
+ * Streams: the launches of one context may go to different CUDA streams (this call, btle_b200_rx_device,
+ * btle_b200_discover_device and btle_b200_synth_streams_device share the context's cached parameter arrays, and d_count
+ * == NULL launches share its counter ring).  Each launch is ordered after what it depends on — the upload of the
+ * parameters it reads, and the earlier ring launch that cleared its counter — without serialising the streams' kernels:
+ * a launch never waits for another stream's kernel that reads the same parameters, and launches on one stream, or
+ * alternating strictly between two, add no cross-stream wait.  Ordering the caller's own buffers is the caller's part. */
 typedef struct { uint32_t base, count; } btle_unit_dir;
 size_t btle_b200_rx_units(const btle_b200_ctx *ctx, size_t n_streams, size_t n_int8);
 int btle_b200_rx_device_dir(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stream_stride_int8,
