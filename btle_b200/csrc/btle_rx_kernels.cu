@@ -2,7 +2,7 @@
 //
 // btle_rx_persistent_kernel does the whole receive chain of the reference's receiver()
 // (btle_rx.c:2188-2391): one persistent, warp-specialised CTA per SM.
-//   dense warps     IQ tile (two TMA boxes, 128B swizzle) -> per-lane discriminator bits packed into
+//   dense warps     IQ tile (one TMA box, 128B swizzle) -> per-lane discriminator bits packed into
 //                   phase words (btle_core.cuh: 1 PRMT + 2 IDP.2A + 1 SHF per sample) -> 12-tap
 //                   bit-parallel prefilter of the 32-tap access-address match against the neighbour
 //                   lane's words (__shfl_down_sync) -> candidate words + group flags (ballot)
@@ -57,6 +57,13 @@ __device__ unsigned long long g_timing[132 * 16];
 __device__ __forceinline__ unsigned long long gtime() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 #define BTLE_STAMP(slot) do { if (lane == 0) atomicMax(&g_timing[(blockIdx.x % 132) * 16 + (slot)], gtime()); } while (0)
 #define BTLE_STAMP_MIN(slot) do { if (lane == 0) atomicMin(&g_timing[(blockIdx.x % 132) * 16 + (slot)], gtime()); } while (0)
+// cumulative SM cycles of one warp (slots 12..15: dense TMA waits, dense `empty` waits, resolver `full` waits, dense total)
+struct WaitClock {
+  long long t0 = 0, sum = 0;
+  __device__ __forceinline__ void begin() { t0 = clock64(); }
+  __device__ __forceinline__ void end() { sum += clock64() - t0; }
+};
+#define BTLE_WAIT_SUM(slot, v) do { if (lane == 0) atomicAdd(&g_timing[(blockIdx.x % 132) * 16 + (slot)], (unsigned long long)(v)); } while (0)
 extern "C" void btle_b200_debug_timing(unsigned long long *dst, int reset) {
   if (reset) { static unsigned long long z[132 * 16]; for (int i = 0; i < 132 * 16; ++i) z[i] = (i % 16 == 0 || i % 16 == 2) ? ~0ull : 0ull; cudaMemcpyToSymbol(g_timing, z, sizeof z); }
   else cudaMemcpyFromSymbol(dst, g_timing, sizeof(unsigned long long) * 132 * 16);
@@ -64,6 +71,12 @@ extern "C" void btle_b200_debug_timing(unsigned long long *dst, int reset) {
 #else
 #define BTLE_STAMP(slot) do { } while (0)
 #define BTLE_STAMP_MIN(slot) do { } while (0)
+struct WaitClock {
+  long long sum = 0;
+  __device__ __forceinline__ void begin() {}
+  __device__ __forceinline__ void end() {}
+};
+#define BTLE_WAIT_SUM(slot, v) do { } while (0)
 #endif
 
 namespace {
@@ -88,7 +101,7 @@ constexpr int kThreads = (kDenseWarps + kResolveWarps) * 32;
 // kSpanChunks = 16 chunks per span (btle_core.cuh): one resolver lane per chunk in the chain pass
 constexpr int kSlots = BTLE_SLOTS;             // ring of span buffers between producers and consumers
 constexpr int kSpanGroups = kGroupsPerChunk * kSpanChunks + kHaloGroups;   // 1036
-constexpr int kStageBytes = 8192;              // one warp tile (32 groups = 4096 samples), two 4 KB halves
+constexpr int kStageBytes = 8192;              // one warp tile (32 groups = 4096 samples), one TMA box
 constexpr int kHaloRows = kHaloGroups;         // rows of the last (look-ahead) tile of a span: always 12
 
 struct Slot {
@@ -114,7 +127,7 @@ struct Smem {
   uint32_t crc4[1024];
   ResolveScratch rs[kResolveWarps];
   alignas(1024) unsigned char stage[kDenseWarps][kStageBytes];
-  alignas(8) unsigned long long mbar[2 * kDenseWarps];   // TMA completion, two per dense warp
+  alignas(8) unsigned long long mbar[kDenseWarps];       // TMA completion, one per dense warp
   unsigned long long full[kSlots];                        // kDenseWarps arrivals: span published
   unsigned long long empty[kSlots];                       // 1 arrival: span consumed
 };
@@ -165,14 +178,13 @@ __device__ __forceinline__ void mbar_wait(unsigned long long *bar, uint32_t pari
       "DONE_%=:\n\t}"
       ::"r"(smem_u32(bar)), "r"(parity) : "memory");
 }
-// TMA tiled copy (cp.async.bulk.tensor, SASS UTMALDG): box {128 B, 1 half, rows, 1 stream} of the
-// IQ tensor {128 B, 2 halves, 256-byte runs, streams} -> shared, 128B-swizzled, completion counted
+// TMA tiled copy (cp.async.bulk.tensor, SASS UTMALDG): box {128 B, rows, 2 halves, 1 stream} of the
+// IQ tensor {128 B, 256-byte runs, 2 halves, streams} -> shared, 128B-swizzled, completion counted
 // in bytes on an mbarrier.
-__device__ __forceinline__ void tma_load_half(void *smem_dst, const CUtensorMap *map, int half, int run, int stream,
-                                              unsigned long long *bar) {
+__device__ __forceinline__ void tma_load_tile(void *smem_dst, const CUtensorMap *map, int run, int stream, unsigned long long *bar) {
   asm volatile(
       "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
-      ::"r"(smem_u32(smem_dst)), "l"(map), "r"(0), "r"(half), "r"(run), "r"(stream), "r"(smem_u32(bar)) : "memory");
+      ::"r"(smem_u32(smem_dst)), "l"(map), "r"(0), "r"(run), "r"(0), "r"(stream), "r"(smem_u32(bar)) : "memory");
 }
 // Writes one packet record.  Reads the raw IQ only when the caller asked for RSSI.
 __device__ __forceinline__ void store_record(btle_pkt_rec *dst, int stream, int chunk, int n0, int nbytes, int crc_bad, bool rejected,
@@ -218,7 +230,7 @@ __device__ __forceinline__ void load_params_warp(const StreamParams *__restrict_
 
 // One persistent CTA per SM.  Units of work (a span of 16 chunks of one capture, or a 4-chunk piece of one in the
 // last wave — Plan, btle_core.cuh) are dealt round-robin to CTAs.
-// Warps 0..15 (dense): per 4096-sample tile, two TMA boxes bring the tile into 128B-swizzled shared rows;
+// Warps 0..15 (dense): per 4096-sample tile, one TMA box brings the tile into 128B-swizzled shared rows;
 //   each lane turns its 128 samples into 4 phase words, prefilters the access-address match against
 //   the neighbour lane's words (warp shuffle) and publishes both in the unit's ring slot.
 // Warps 16..18 (resolvers, units k = r, r+3, ...): when a unit is complete,
@@ -245,12 +257,12 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
   if (zero_next && blockIdx.x == 0 && tid == 0) *zero_next = 0u;
   // ---- dense warps: (span, tile) iterator and TMA request helpers -------------------------------------
   // Each warp walks its own sequence of tiles (tile j of the CTA goes to warp j % 16, across
-  // unit boundaries).  A tile is fetched as two 4 KB TMA boxes — the upper and the lower 128
-  // bytes of every lane's 256-byte run — each into its own buffer; as soon as a half has been
-  // consumed the same half of the warp's NEXT tile is requested into that buffer, so the copy of
-  // the next tile overlaps the arithmetic of this one.
+  // unit boundaries).  A tile is fetched as ONE TMA box: row r of half h (the lower / upper 128
+  // bytes of the 256-byte run of group r) lands at (h * rows + r) * 128 B, 128B-swizzled.  As soon
+  // as the tile has been consumed the warp's NEXT tile is requested into the buffer; the other 15
+  // dense warps' copies are in flight meanwhile.
   unsigned char *stage = M.stage[warp < kDenseWarps ? warp : 0];
-  unsigned long long *mbar = &M.mbar[2 * (warp < kDenseWarps ? warp : 0)];   // [0] lower-half buffer, [1] upper-half buffer
+  unsigned long long *mbar = &M.mbar[warp < kDenseWarps ? warp : 0];
   // How a tile's bytes get into shared memory.  The tensor map has n_int8/256 rows per capture; rows behind them read
   // as ZERO through TMA (out-of-bounds fill), which is exactly what the reference-equivalent semantics want for the
   // look-ahead behind the end of a capture.  Only a capture whose length is not a multiple of 256 has one partial row
@@ -286,7 +298,7 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
   };
   // descriptor of the tile under the prefetch cursor, refreshed once per tile
   int nx_run0 = 0, nx_stream = 0;
-  uint32_t nx_bytes = 0;                                  // bytes per half; 0 = nothing to request by TMA
+  uint32_t nx_bytes = 0;                                  // bytes of the tile; 0 = nothing to request by TMA
   const CUtensorMap *nx_map = &map32;
   auto describe = [&](const Cursor &c) {
     nx_bytes = 0;
@@ -295,12 +307,12 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
     nx_run0 = c.chunk0 * 64 + c.t * 32;
     nx_stream = c.stream;
     nx_map = (rows == 32) ? &map32 : &map12;
-    if (tile_mode(nx_run0, rows) == 0) nx_bytes = (uint32_t)rows * 128u;   // else: filled by the consumer itself
+    if (tile_mode(nx_run0, rows) == 0) nx_bytes = (uint32_t)rows * 256u;   // else: filled by the consumer itself
   };
-  auto request_half = [&](int half) {                     // 1 = upper, 0 = lower half of the described tile
+  auto request = [&]() {                                  // the described tile
     if (lane == 0 && nx_bytes) {
-      mbar_expect_tx(&mbar[half], nx_bytes);
-      tma_load_half(stage + (half << 12), nx_map, half, nx_run0, nx_stream, &mbar[half]);
+      mbar_expect_tx(mbar, nx_bytes);
+      tma_load_tile(stage, nx_map, nx_run0, nx_stream, mbar);
     }
   };
   Cursor pf;                                              // the tile to request next
@@ -320,16 +332,14 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
   if (warp < kDenseWarps) {
     // the first tile is requested right away: its HBM round trip overlaps the rest of the start-up
     if (lane == 0) {
-      mbar_init(&mbar[0], 1);
-      mbar_init(&mbar[1], 1);
+      mbar_init(mbar, 1);
       asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncwarp();
     enter_unit(pf);
     while (pf.valid && pf.t >= pf.tiles) next_unit(pf);
     describe(pf);
-    request_half(1);
-    request_half(0);
+    request();
     next_tile(pf);
     describe(pf);
     BTLE_STAMP(10);
@@ -347,13 +357,17 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
 
   if (warp < kDenseWarps) {
     // =============================== dense producers ===============================
-    uint32_t tma_phase = 0;                               // bit h: parity to wait for on buffer h
+    uint32_t tma_phase = 0;                               // parity to wait for on the tile's mbarrier
     int rot = 0, k = 0;
+    WaitClock w_all, w_tma, w_empty;
+    w_all.begin();
     for (int unit = blockIdx.x; unit < total_units; unit += gridDim.x, ++k) {
       const int b = k % kSlots;
       Slot &S = M.slot[b];
       const uint32_t use = (uint32_t)(k / kSlots);
+      w_empty.begin();
       if (use > 0) mbar_wait_backoff(&M.empty[b], (use - 1) & 1u);   // resolver released the slot's previous unit
+      w_empty.end();
       const UnitInfo si = unit_info(unit, plan);
       const int8_t *cap_base = iq + (long long)si.stream * stream_stride;
       int t = warp - rot;
@@ -373,25 +387,24 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
             for (int bb = 0; bb < 4; ++bb)
               if (o + bb < n_int8) tail |= (uint32_t)(uint8_t)cap_base[o + bb] << (8 * bb);
         }
-        uint32_t acc[4] = {0u, 0u, 0u, 0u};
-        uint32_t carry = 0u, wtop = 0u;
-        int vtop = 0;
-#pragma unroll 1
-        for (int half = 1; half >= 0; --half) {
-          unsigned char *buf = stage + (half << 12);
-          if (tma) {
-            mbar_wait(&mbar[half], (tma_phase >> half) & 1u);
-            tma_phase ^= 1u << half;
-          } else if (mode == 2) {
-            if (lane < rows) {
+        if (tma) {
+          w_tma.begin();
+          mbar_wait(mbar, tma_phase);
+          w_tma.end();
+          tma_phase ^= 1u;
+        } else if (mode == 2) {
+          if (lane < rows) {
 #pragma unroll
-              for (int cc = 0; cc < 8; ++cc) *reinterpret_cast<uint4 *>(buf + (lane << 7) + (cc << 4)) = make_uint4(0u, 0u, 0u, 0u);
-            }
-            __syncwarp();
-          } else {
-            // the capture's partial last row: bytes past n_int8 read as 0 (same swizzled layout, generic stores)
-            if (lane < rows) {
+            for (int cc = 0; cc < 16; ++cc)
+              *reinterpret_cast<uint4 *>(stage + (((cc >> 3) * rows + lane) << 7) + ((cc & 7) << 4)) = make_uint4(0u, 0u, 0u, 0u);
+          }
+          __syncwarp();
+        } else {
+          // the capture's partial last row: bytes past n_int8 read as 0 (same swizzled layout, generic stores)
+          if (lane < rows) {
+            for (int half = 0; half < 2; ++half) {
               const long long row_off = tile_off + (long long)lane * 256 + 128 * half;
+              const int r = half * rows + lane;
               for (int wi = 0; wi < 32; ++wi) {
                 const long long o = row_off + 4ll * wi;
                 uint32_t w = 0;
@@ -399,15 +412,22 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
                 else
                   for (int bb = 0; bb < 4; ++bb)
                     if (o + bb < n_int8) w |= (uint32_t)(uint8_t)cap_base[o + bb] << (8 * bb);
-                reinterpret_cast<uint32_t *>(buf + (lane << 7) + ((((wi >> 2) ^ (lane & 7))) << 4))[wi & 3] = w;
+                reinterpret_cast<uint32_t *>(stage + (r << 7) + ((((wi >> 2) ^ (r & 7))) << 4))[wi & 3] = w;
               }
             }
-            __syncwarp();
           }
-          // 16-byte chunk cc of this lane's 128-byte row sits at cc ^ (lane & 7) (TMA SWIZZLE_128B):
-          // the 8 lanes of a quarter-warp hit 8 different bank groups -> conflict-free LDS.128
-          const unsigned char *row = buf + (lane << 7);
-          const uint32_t sw = (uint32_t)(lane & 7);
+          __syncwarp();
+        }
+        uint32_t acc[4] = {0u, 0u, 0u, 0u};
+        uint32_t carry = 0u, wtop = 0u;
+        int vtop = 0;
+#pragma unroll 1
+        for (int half = 1; half >= 0; --half) {
+          // 16-byte chunk cc of box row r sits at cc ^ (r & 7) (TMA SWIZZLE_128B): the 8 lanes of a quarter-warp
+          // hit 8 different bank groups -> conflict-free LDS.128
+          const int r = half * rows + lane;
+          const unsigned char *row = stage + (r << 7);
+          const uint32_t sw = (uint32_t)(r & 7);
           if (half == 0) {
             // now the neighbour's first word is here: redo the one bit that needed it (sample 127)
             const uint32_t first = reinterpret_cast<const uint4 *>(row + (sw << 4))->x;
@@ -439,9 +459,9 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
             // sample 127 was pushed first, so after all 32 pushes it is bit 31 of phase 3
             if (half == 0) acc[3] = (acc[3] & 0x7FFFFFFFu) | ((uint32_t)vtop & 0x80000000u);
           }
-          __syncwarp();                                   // everyone is done reading this buffer
-          request_half(half);                             // same half of the warp's next tile
         }
+        __syncwarp();                                     // everyone is done reading the buffer
+        request();                                        // the warp's next tile
         next_tile(pf);
         describe(pf);
         BTLE_STAMP_MIN(2);
@@ -465,6 +485,10 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
       if (lane == 0) mbar_arrive(&M.full[b]);             // release: this warp's share of the unit is published
       BTLE_STAMP(3);
     }
+    w_all.end();
+    BTLE_WAIT_SUM(12, w_tma.sum);
+    BTLE_WAIT_SUM(13, w_empty.sum);
+    BTLE_WAIT_SUM(15, w_all.sum);
   } else {
     // ================================== resolvers ==================================
     // the CRC tables are only needed here: built by the resolver warps while the first unit is in flight
@@ -481,10 +505,13 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
     // resolver warp r takes this CTA's units k = r, r + kResolveWarps, ...
     ResolveScratch &RS = M.rs[warp - kDenseWarps];
     int k = warp - kDenseWarps;
+    WaitClock w_full;
     for (int unit = blockIdx.x + k * gridDim.x; unit < total_units; unit += kResolveWarps * gridDim.x, k += kResolveWarps) {
       const int b = k % kSlots;
       Slot &S = M.slot[b];
+      w_full.begin();
       mbar_wait_backoff(&M.full[b], (uint32_t)(k / kSlots) & 1u);   // all tiles of the unit are published
+      w_full.end();
       BTLE_STAMP(4);
       const UnitInfo si = unit_info(unit, plan);
       const int8_t *cap_base = iq + (long long)si.stream * stream_stride;
@@ -594,6 +621,7 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
       if (lane == 0) mbar_arrive(&M.empty[b]);            // release the slot to the producers
       BTLE_STAMP(5);
     }
+    BTLE_WAIT_SUM(14, w_full.sum);
   }
 }
 
@@ -1644,9 +1672,9 @@ int note_use(btle_b200_ctx *ctx, CfgSlot *slot, cudaStream_t st, unsigned long l
   return BTLE_OK;
 }
 
-// IQ as a 4-D byte tensor {128 B, 2 halves, 256-byte runs, streams}; a box is one half of `rows` consecutive
-// runs, so each lane's 256-byte run lands as two conflict-free 128-byte rows.  Encoded maps are cached per
-// (pointer, shape): a streaming caller alternates between a few buffers.
+// IQ as a 4-D byte tensor {128 B, 256-byte runs, 2 halves, streams}; a box is `rows` consecutive runs, both
+// halves, so each lane's 256-byte run lands as two conflict-free 128-byte rows (row r of half h at h * rows + r).
+// Encoded maps are cached per (pointer, shape): a streaming caller alternates between a few buffers.
 int get_maps(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8, const MapSlot **out) {
   MapSlot *pick = nullptr;
   for (MapSlot &m : ctx->map_slot)
@@ -1659,11 +1687,11 @@ int get_maps(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t st
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
     encode_fn enc = reinterpret_cast<encode_fn>(ctx->encode_tiled);
     const cuuint64_t runs = (cuuint64_t)(n_int8 / 256);
-    const cuuint64_t dims[4] = {128, 2, runs, (cuuint64_t)n_streams};
-    const cuuint64_t strides[3] = {128, 256, (cuuint64_t)(n_streams > 1 ? stride : ((n_int8 + 255) & ~size_t(255)))};
+    const cuuint64_t dims[4] = {128, runs, 2, (cuuint64_t)n_streams};
+    const cuuint64_t strides[3] = {256, 128, (cuuint64_t)(n_streams > 1 ? stride : ((n_int8 + 255) & ~size_t(255)))};
     const cuuint32_t estr[4] = {1, 1, 1, 1};
     for (int which = 0; which < 2; ++which) {
-      const cuuint32_t box[4] = {128, 1, (cuuint32_t)(which ? kHaloRows : 32), 1};
+      const cuuint32_t box[4] = {128, (cuuint32_t)(which ? kHaloRows : 32), 2, 1};
       const CUresult r = enc(which ? &pick->map12 : &pick->map32, CU_TENSOR_MAP_DATA_TYPE_UINT8, 4, const_cast<int8_t *>(d_iq), dims,
                              strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);

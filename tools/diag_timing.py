@@ -11,6 +11,7 @@ cfgs = make_cfgs(1)
 d_out = torch.empty(400000 * 64, dtype=torch.uint8, device=dev); d_cnt = torch.zeros(1, dtype=torch.int32, device=dev)
 st = torch.cuda.current_stream()
 FULL = (1 << 30) / (16 * 16384 * 132)      # spans per CTA of a 1 GiB capture: 4096 spans over 132 CTAs
+DENSE, RESOLVE = 16, 3                     # dense and resolver warps per CTA (the default launch shape)
 for spans in (4, FULL):
     n_int8 = int(round(spans * 132)) * 16 * 16384
     v = iq[:n_int8].view(1, -1)
@@ -29,3 +30,8 @@ for spans in (4, FULL):
     print(f"spans/CTA {spans}: (us, median over CTAs / max)")
     for i, nm in enumerate(names):
         print(f"   {nm:22s} {np.median(rel[:, i]):8.1f} {rel[:, i].max():8.1f}")
+    # cumulative wait cycles (slots 12..15), per warp, as a share of a dense warp's cycles from start-up to its last unit
+    dense_total = t[:, 15].sum() / DENSE
+    print(f"   dense warp: TMA mbar_wait {t[:, 12].sum() / DENSE / dense_total:6.1%}, empty-slot wait "
+          f"{t[:, 13].sum() / DENSE / dense_total:6.1%};  resolver warp: idle on full {t[:, 14].sum() / RESOLVE / dense_total:6.1%}"
+          f"  (of {dense_total / 132:.0f} cycles per dense warp)")
