@@ -53,6 +53,7 @@ EXPORTS = [
     "btle_b200_dbits", "btle_b200_gfsk_demod_i16", "btle_b200_search_bit_sequence", "btle_b200_crc24_bits",
     "btle_b200_scramble_bits", "btle_b200_model_rx_batch_device", "btle_b200_model_rx_batch",
     "btle_b200_tx_modulate_device", "btle_b200_rx_iq16", "btle_b200_synth_streams_device", "btle_b200_rx_sps8", "btle_b200_sps8_hits_device", "btle_b200_ber_run",
+    "btle_b200_ber_synth_device",
     "btle_b200_stream_open", "btle_b200_stream_push", "btle_b200_stream_acquire", "btle_b200_stream_commit", "btle_b200_stream_finish",
     "btle_b200_stream_close", "btle_b200_stream_set_cfg",
     "btle_b200_streams_open", "btle_b200_streams_acquire", "btle_b200_streams_commit", "btle_b200_streams_set_cfg",
@@ -121,6 +122,7 @@ def load():
     L.btle_b200_tx_modulate_device.argtypes = [vp, vp, vp, sz, sz, i32, vp, vp, vp]
     L.btle_b200_rx_iq16.argtypes = [vp, vp, sz, i32, vp, vp, sz, ctypes.POINTER(sz)]
     L.btle_b200_ber_run.argtypes = [vp, vp, sz, vp]
+    L.btle_b200_ber_synth_device.argtypes = [vp, vp, ctypes.c_uint64, sz, vp, vp, vp, vp]
     L.btle_b200_sps8_hits_device.argtypes = [vp, vp, sz, u32, vp, sz, vp, vp]
     L.btle_b200_rx_sps8.argtypes = [vp, vp, sz, i32, u32, u32, vp, sz, ctypes.POINTER(sz)]
     L.btle_b200_synth_streams_device.argtypes = [vp, vp, sz, sz, sz, vp, vp, vp, sz, ctypes.POINTER(sz), vp]

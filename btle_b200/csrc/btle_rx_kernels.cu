@@ -1929,7 +1929,7 @@ int launch_discover(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, si
 
 extern "C" {
 
-uint32_t btle_b200_version(void) { return (0u << 16) | 2u; }
+uint32_t btle_b200_version(void) { return (0u << 16) | 3u; }
 
 const char *btle_b200_strerror(int code) {
   switch (code) {
@@ -2631,7 +2631,11 @@ int btle_b200_model_rx_batch(btle_b200_ctx *ctx, const int16_t *i, const int16_t
 
 int btle_b200_sps8_hits_device(btle_b200_ctx *ctx, const int16_t *d_iq16, size_t n_samples, uint32_t access_addr, int64_t *d_hits, size_t cap,
                                uint32_t *d_count, void *cuda_stream) {
-  if (!ctx || !d_iq16 || !d_count || (!d_hits && cap) || (reinterpret_cast<uintptr_t>(d_iq16) & 3)) return BTLE_EINVAL;
+  if (!ctx || !d_iq16 || !d_count || (!d_hits && cap)) return BTLE_EINVAL;
+  if (reinterpret_cast<uintptr_t>(d_iq16) & 15) {          // sps8_hits_kernel copies the capture in 16-byte vectors
+    ctx->err = "sps8_hits_device: the capture must be 16-byte aligned";
+    return BTLE_EINVAL;
+  }
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
   BTLE_CUDA(ctx, cudaMemsetAsync(d_count, 0, sizeof(unsigned), st));
@@ -2759,16 +2763,27 @@ int btle_b200_rx_sps8(btle_b200_ctx *ctx, const int16_t *iq16, size_t n_samples,
   return BTLE_OK;
 }
 
+// ber_synth_kernel reads sample (int)(m * (1 + ppm 1e-6)) of its packet: ppm must be finite and above -1e6 (the
+// reference's script uses -50..50), and the SNR must be a number
+static int check_ber_cfg(btle_b200_ctx *ctx, const btle_ber_cfg *cfg) {
+  if (cfg->channel < 0 || cfg->channel > 39) { ctx->err = "ber: channel must be 0..39"; return BTLE_EINVAL; }
+  if (!std::isfinite(cfg->ppm) || std::fabs(cfg->ppm) >= 1e6f) { ctx->err = "ber: ppm must be finite with |ppm| < 1e6"; return BTLE_EINVAL; }
+  if (std::isnan(cfg->snr_db)) { ctx->err = "ber: snr_db is NaN"; return BTLE_EINVAL; }
+  return BTLE_OK;
+}
+
 int btle_b200_ber_run(btle_b200_ctx *ctx, const btle_ber_cfg *cfg, size_t n_packets, btle_ber_result *out) {
-  if (!ctx || !cfg || !out || cfg->channel < 0 || cfg->channel > 39) return BTLE_EINVAL;
+  if (!ctx || !cfg || !out) return BTLE_EINVAL;
   memset(out, 0, sizeof *out);
+  int rc = check_ber_cfg(ctx, cfg);
+  if (rc) return rc;
   if (!n_packets) return BTLE_OK;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
   const size_t B = std::min<size_t>(n_packets, 32768);
   const size_t iq_bytes = B * kBerSamples * sizeof(int16_t);
   const size_t a_iq = (iq_bytes + 255) & ~size_t(255), a_tr = (B * 40 + 255) & ~size_t(255), a_rec = (B * sizeof(btle_model_rx_rec) + 255) & ~size_t(255);
-  int rc = leaf_buf(ctx, 2 * a_iq + a_tr + a_rec + 256);
+  rc = leaf_buf(ctx, 2 * a_iq + a_tr + a_rec + 256);
   if (rc) return rc;
   uint8_t *base = static_cast<uint8_t *>(ctx->d_leaf);
   int16_t *d_i = reinterpret_cast<int16_t *>(base), *d_q = reinterpret_cast<int16_t *>(base + a_iq);
@@ -2802,6 +2817,21 @@ int btle_b200_ber_run(btle_b200_ctx *ctx, const btle_ber_cfg *cfg, size_t n_pack
   out->bit_total = (uint64_t)n_packets * 8 * kBerPduBytes;
   out->seconds = ms * 1e-3;
   ctx->last_launches = launches;
+  return BTLE_OK;
+}
+
+static_assert(kBerSamples == BTLE_BER_SAMPLES, "include/btle_b200.h documents the BER packet length");
+int btle_b200_ber_synth_device(btle_b200_ctx *ctx, const btle_ber_cfg *cfg, uint64_t first_packet, size_t n_packets, int16_t *d_i,
+                               int16_t *d_q, uint8_t *d_truth, void *cuda_stream) {
+  if (!ctx || !cfg || !d_i || !d_q || !d_truth || n_packets > 0x7FFFFFFFu) return BTLE_EINVAL;
+  int rc = check_ber_cfg(ctx, cfg);
+  if (rc) return rc;
+  if (!n_packets) return BTLE_OK;
+  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
+  ber_synth_kernel<<<(unsigned)n_packets, 384, 0, reinterpret_cast<cudaStream_t>(cuda_stream)>>>(
+      *cfg, (unsigned long long)first_packet, (int)n_packets, d_i, d_q, d_truth);
+  BTLE_CUDA(ctx, cudaGetLastError());
+  ctx->last_launches = 1;
   return BTLE_OK;
 }
 

@@ -335,7 +335,8 @@ typedef struct {
 int btle_b200_rx_sps8(btle_b200_ctx *ctx, const int16_t *iq16, size_t n_samples, int channel, uint32_t crc_init,
                       uint32_t access_addr, btle_sps8_rec *out, size_t cap, size_t *n_out);
 /* step 1 alone on a device-resident capture: *d_count (zeroed by the call) = number of hits, d_hits[0..min(count, cap)) =
- * their sample indices in no particular order; enqueued on cuda_stream, not synchronised */
+ * their sample indices in no particular order; enqueued on cuda_stream, not synchronised.  `d_iq16` must be 16-byte
+ * aligned (the kernel copies the capture in 16-byte vectors): anything else is BTLE_EINVAL. */
 int btle_b200_sps8_hits_device(btle_b200_ctx *ctx, const int16_t *d_iq16, size_t n_samples, uint32_t access_addr,
                                int64_t *d_hits, size_t cap, uint32_t *d_count, void *cuda_stream);
 
@@ -347,8 +348,8 @@ int btle_b200_sps8_hits_device(btle_b200_ctx *ctx, const int16_t *d_iq16, size_t
  * hash of (seed, packet, sample), so a run is reproducible and packet k is the same whatever the batch size. */
 typedef struct {
   uint64_t seed;
-  float snr_db;
-  float ppm;               /* 0, or -50..50 like test_btle_ber.py                                                  */
+  float snr_db;            /* NaN: BTLE_EINVAL                                                                     */
+  float ppm;               /* 0, or -50..50 like test_btle_ber.py; not finite or |ppm| >= 1e6: BTLE_EINVAL         */
   int32_t channel;
   uint32_t crc_init;       /* as -k: 0x555555                                                                      */
   uint32_t access_addr;
@@ -359,6 +360,13 @@ typedef struct {
   double seconds;          /* device time of the run (CUDA events)                                                 */
 } btle_ber_result;
 int btle_b200_ber_run(btle_b200_ctx *ctx, const btle_ber_cfg *cfg, size_t n_packets, btle_ber_result *out);
+/* the packet source and channel of btle_b200_ber_run alone, for packets first_packet .. first_packet + n_packets - 1 of
+ * the run `cfg` describes (the same packets ber_run draws): d_i / d_q [n_packets][BTLE_BER_SAMPLES] int16 (planar, ready
+ * for btle_b200_model_rx_batch_device with sps 8), d_truth [n_packets][40] the 39 PDU bytes as sent (byte 39 is not
+ * written).  Device pointers; enqueued on cuda_stream, not synchronised. */
+#define BTLE_BER_SAMPLES 3024      /* 8 sps x 8 x (1 + 4 + 39 + 3) air bytes + 16 */
+int btle_b200_ber_synth_device(btle_b200_ctx *ctx, const btle_ber_cfg *cfg, uint64_t first_packet, size_t n_packets, int16_t *d_i,
+                               int16_t *d_q, uint8_t *d_truth, void *cuda_stream);
 
 /* ---- 16-bit IQ ingest (SURVEY.md §8f-3) ------------------------------------------------------------
  * bladeRF SC16Q11 samples are reduced to the receive chain's int8 exactly as the reference's

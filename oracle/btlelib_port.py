@@ -60,20 +60,23 @@ def demod_phase(i: np.ndarray, q: np.ndarray) -> np.ndarray:
     return (s > 0).astype(np.int8)
 
 
-def rx_window(i, q, channel=37, crc_init=0x555555, access_addr=0x8E89BED6):
-    """-> dict(pdu_bit, crc_ok, plen, phase, start, found) with btle_rx's meaning; `found` = 1 + last phase the access
-    address was found on (0: never); `start` = its symbol index on the reported phase."""
+def rx_window(i, q, channel=37, crc_init=0x555555, access_addr=0x8E89BED6, sps=SPS):
+    """-> dict(pdu_bit, crc_ok, plen, phase, start, found) with btle_rx's meaning at `sps` samples per symbol (the
+    reference's SAMPLE_PER_SYMBOL); `found` = 1 + last phase the access address was found on (0: never); `start` = its
+    symbol index on the reported phase.  Where the access address ends so close to the window's end that the length field
+    is not complete (start + 40 + 6 / 5 > num_bit), the reference raises IndexError; here, as in model_rx_batch_kernel,
+    the missing header bits read as 0 before dewhitening."""
     i = np.asarray(i).astype(np.int16)
     q = np.asarray(q).astype(np.int16)
     n = len(i)
-    num_bit = round(n / SPS) - 1
+    num_bit = round(n / sps) - 1
     aa = bits_lsb_first(access_addr, 4)
     init = crc_init_bits(crc_init)
     adv = channel in (37, 38, 39)
-    res = dict(pdu_bit=np.zeros(0, dtype=np.int8), crc_ok=False, plen=0, phase=SPS - 1, start=-1, found=0)
+    res = dict(pdu_bit=np.zeros(0, dtype=np.int8), crc_ok=False, plen=0, phase=sps - 1, start=-1, found=0)
     wh_cache = None
-    for ph in range(SPS):
-        b = demod_phase(i[ph::SPS], q[ph::SPS])
+    for ph in range(sps):
+        b = demod_phase(i[ph::sps], q[ph::sps])
         bits = np.zeros(num_bit, dtype=np.int8)
         m = min(len(b), num_bit)
         bits[:m] = b[:m]
@@ -87,12 +90,13 @@ def rx_window(i, q, channel=37, crc_init=0x555555, access_addr=0x8E89BED6):
             continue
         start = int(hit[0])
         phy = np.concatenate((np.zeros(8, dtype=np.int8), bits[start:]))
-        if wh_cache is None or len(wh_cache) < len(phy):
-            wh_cache = whitening(channel, max(len(phy), 400))
+        if wh_cache is None or len(wh_cache) < len(phy) + 16:
+            wh_cache = whitening(channel, max(len(phy) + 16, 400))
         info = phy.copy()
         info[40:] ^= wh_cache[: len(phy) - 40]
         nb = 6 if adv else 5
-        plen = int(sum(int(info[48 + k]) << k for k in range(nb))) if len(info) >= 48 + nb else 0
+        hdr = np.concatenate((phy, np.zeros(16, dtype=np.int8)))[40:56] ^ wh_cache[:16]
+        plen = int(sum(int(hdr[8 + k]) << k for k in range(nb)))
         crc_start = 56 + 8 * plen
         if crc_start + 24 > len(info):
             crc_start = len(info) - 24
@@ -148,6 +152,22 @@ def rx_stream(iq16: np.ndarray, channel=37, crc_init=0x555555, access_addr=0x8E8
         cursor = at + 8 * (32 + 16 + 8 * (r["plen"] if r["found"] else 0) + 24)
         out.append(dict(r, sample=at, window=w0))
     return out
+
+
+def phase_bits_to_iq(bits: np.ndarray, n: int | None = None, amp: int = 1000, sps: int = SPS) -> np.ndarray:
+    """int16 [n, 2] (I, Q) whose symbol-spaced differential bits on phase p are exactly bits[p] (bits [sps, m]): sample
+    a + sps is sample a turned by +90 degrees for a 1 and by -90 degrees for a 0, every sample one of (amp, 0), (0, amp),
+    (-amp, 0), (0, -amp), so bit k of phase p (samples p + sps k and p + sps (k + 1)) decides on +-amp^2.  n defaults to
+    sps (m + 1); samples beyond sps (m + 1) are not allowed."""
+    bits = np.asarray(bits, dtype=np.int64)
+    m = bits.shape[1]
+    n = sps * (m + 1) if n is None else n
+    assert bits.shape[0] == sps and n <= sps * (m + 1)
+    turn = np.where(bits > 0, 1, -1)
+    quadrant = np.concatenate((np.arange(sps)[:, None] % 4, np.cumsum(turn, axis=1) + np.arange(sps)[:, None] % 4), axis=1) % 4
+    pts = np.array([[amp, 0], [0, amp], [-amp, 0], [0, -amp]], dtype=np.int64)
+    iq = pts[quadrant.T.reshape(-1)][:n]                       # sample p + sps k = quadrant[p, k]
+    return iq.astype(np.int16)
 
 
 def tx_bits(pdu: bytes, channel=37, crc_init=0x555555, access_addr=0x8E89BED6) -> np.ndarray:

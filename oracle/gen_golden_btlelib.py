@@ -3,7 +3,9 @@
 python/btlelib.py here (from a writable copy: it writes table files next to itself on first TX
 call, btlelib.py:90-91,155).  Writes tests/golden/btlelib_rx.npz (committed); with --random, instead
 tests/golden/btlelib_rx_random.npz: the reference receiver's verdicts on the 60 random-packet windows of
-tests/test_oracle_btlelib_port.py, whose inputs the test rebuilds itself (checked here against btle_tx / add_noise)."""
+tests/test_oracle_btlelib_port.py, whose inputs the test rebuilds itself (checked here against btle_tx / add_noise); with
+--sps, tests/golden/btlelib_rx_sps.npz: the reference receiver at SAMPLE_PER_SYMBOL 1, 2, 4, 8 and 16 on crafted windows
+(sps_windows), inputs stored with the verdicts."""
 import os
 import shutil
 import sys
@@ -43,6 +45,107 @@ def random_cases(bl):
     np.savez_compressed(os.path.join(ROOT, "tests", "golden", "btlelib_rx_random.npz"), **out)
 
 
+SPS_SET = (1, 2, 4, 8, 16)
+ADV = (37, 0x555555, 0x8E89BED6)
+DATA = (11, 0xA77B22, 0x60850A1B)        # btle_rx -k / -a style values
+
+
+def sps_windows():
+    """Crafted windows for the model receiver at every sample rate: per-phase bit sequences (btlelib_port.phase_bits_to_iq)
+    with packets planted at exact symbol indices.  Yields (name, sps, (channel, crc_init, access_addr), i, q)."""
+    sys.path.insert(0, os.path.join(ROOT, "oracle"))
+    import btlelib_port as P
+    rng = np.random.default_rng(1234)
+
+    def pdu_for(cfg, plen, rfu=0):
+        if cfg[0] >= 37:
+            return bytes([0x40, plen]) + rng.integers(0, 256, plen, dtype=np.uint8).tobytes()
+        return bytes([0x01, plen | rfu]) + rng.integers(0, 256, plen, dtype=np.uint8).tobytes()
+
+    def window(sps, nsym, cfg, plants, amp=1000):
+        """plants: {phase: (symbol index of the access address, air bits from the access address on)}; other bits random"""
+        bits = rng.integers(0, 2, (sps, nsym - 1)).astype(np.int8)
+        for ph, (s, b) in plants.items():
+            b = b[: nsym - 1 - s]
+            bits[ph, s:s + len(b)] = b
+        iq = P.phase_bits_to_iq(bits, amp=amp, sps=sps)
+        return iq[:, 0].copy(), iq[:, 1].copy()
+
+    def air(cfg, pdu, flip_crc=False):
+        b = P.tx_bits(pdu, *cfg)[8:].copy()              # from the access address on
+        if flip_crc:
+            b[-3] ^= 1
+        return b
+
+    for sps in SPS_SET:
+        nsym = 400 if sps >= 8 else 2048
+        for cfg in (ADV, DATA):
+            tag = "adv" if cfg is ADV else "data"
+            # 37 = 0b100101 and a set RFU bit above the 5-bit data length: a length read with the other channel's mask differs
+            pdu = pdu_for(cfg, 37 if cfg is ADV else 27, rfu=0x20)
+            good, bad = air(cfg, pdu), air(cfg, pdu, flip_crc=True)
+            yield f"{tag}_clean", sps, cfg, *window(sps, nsym, cfg, {p: (20, good) for p in range(sps)})
+            if sps > 1:
+                later = {p: (20, bad) for p in range(sps // 2)}
+                later.update({p: (20, good) for p in range(sps // 2, sps)})
+                yield f"{tag}_ok_on_later_phase", sps, cfg, *window(sps, nsym, cfg, later)
+            yield f"{tag}_never_ok", sps, cfg, *window(sps, nsym, cfg, {p: (30, bad) for p in range(max(1, sps - 1))})
+            num_bit = nsym - 1
+            long_pdu = pdu_for(cfg, 31 if cfg is DATA else 37)
+            # CRC position clamped, crc_start >= 40: the header's length runs past the window
+            yield f"{tag}_clamp_ge40", sps, cfg, *window(sps, nsym, cfg, {0: (num_bit + 8 - 150, air(cfg, long_pdu))})
+            # crc_start < 40: the access address ends 13..23 bits before the window's end (len(info) 53/54 .. 63)
+            for li in ((54, 63) if cfg is ADV else (53, 60)):
+                yield f"{tag}_clamp_lt40_{li}", sps, cfg, *window(sps, nsym, cfg, {sps - 1: (num_bit + 8 - li, air(cfg, long_pdu))})
+            # the access address at the last index: the reference raises (no complete header)
+            yield f"{tag}_aa_last", sps, cfg, *window(sps, nsym, cfg, {0: (num_bit - 32, air(cfg, pdu))})
+        yield "never_found", sps, ADV, *window(sps, nsym, ADV, {})
+        yield "n34_noise", sps, ADV, *window(sps, 34, ADV, {})
+        for s in (0, 1):
+            yield f"n34_aa_at_{s}", sps, ADV, *window(sps, 34, ADV, {0: (s, air(ADV, pdu_for(ADV, 6)))})
+        if sps <= 4:
+            # the CRC's last bit is the window's last bit: the clamp's boundary (crc_start + 24 == len(info)) on its other side
+            yield "n2048_data_at_end", sps, DATA, *window(sps, 2048, DATA, {p: (2047 - (32 + 16 + 8 * 27 + 24), air(DATA, pdu_for(DATA, 27)))
+                                                                           for p in range(sps)})
+        # int16 extremes: a clean packet at full scale (-32767 -> -32768), and full-scale random samples
+        i, q = window(sps, 300, ADV, {p: (10, air(ADV, pdu_for(ADV, 20))) for p in range(sps)}, amp=32767)
+        i[i == -32767] = -32768
+        q[q == -32767] = -32768
+        yield "extreme_packet", sps, ADV, i, q
+        r = rng.choice(np.array([-32768, 32767], dtype=np.int16), (2, 300 * sps))
+        yield "extreme_random", sps, ADV, r[0].copy(), r[1].copy()
+
+
+def sps_cases(bl):
+    """tests/golden/btlelib_rx_sps.npz: the reference's btle_rx with SAMPLE_PER_SYMBOL 1, 2, 4, 8, 16 on sps_windows()."""
+    out, names = {}, []
+    for k, (name, sps, (ch, crc, aa), i, q) in enumerate(sps_windows()):
+        bl.SAMPLE_PER_SYMBOL = sps
+        args = [ch, bl.hex_string_to_bit(f"{crc:06X}"), aa.to_bytes(4, "little").hex().upper()]
+        raises = 0
+        try:
+            pdu_bit, crc_ok, plen, phy_bit, bit_all, _, phase = bl.btle_rx(i, q, *args)
+        except IndexError:
+            raises = 1
+        names.append(name)
+        out[f"w{k}_i"], out[f"w{k}_q"] = np.int16(i), np.int16(q)
+        meta = [sps, ch, crc, aa, raises]
+        if not raises:
+            aa_bits = bl.hex_string_to_bit(args[2])
+            found = [p for p in range(phase + 1) if bl.search_unique_bit_sequence(bit_all[p], aa_bits) >= 0]
+            start = (bit_all.shape[1] - (len(phy_bit) - 8)) if found else -1
+            meta += [int(bool(crc_ok)), int(plen), int(phase), 1 + found[-1] if found else 0, start]
+            out[f"w{k}_pdu_bit"] = np.asarray(pdu_bit, dtype=np.int8)
+        else:
+            meta += [0, 0, 0, 0, 0]
+            out[f"w{k}_pdu_bit"] = np.zeros(0, dtype=np.int8)
+        out[f"w{k}_meta"] = np.array(meta, dtype=np.int64)
+        print(k, name, "sps", sps, "ch", ch, "raises" if raises else meta[5:])
+    out["names"] = np.array(names)
+    bl.SAMPLE_PER_SYMBOL = 8
+    np.savez_compressed(os.path.join(ROOT, "tests", "golden", "btlelib_rx_sps.npz"), **out)
+
+
 def main():
     td = tempfile.mkdtemp()
     shutil.copytree(os.path.join(REF, "python"), os.path.join(td, "python"))
@@ -52,6 +155,9 @@ def main():
     import btlelib as bl
     if "--random" in sys.argv:
         random_cases(bl)
+        return
+    if "--sps" in sys.argv:
+        sps_cases(bl)
         return
     out = {}
     cases = [
