@@ -126,6 +126,14 @@ def load():
     L.btle_b200_sps8_hits_device.argtypes = [vp, vp, sz, u32, vp, sz, vp, vp]
     L.btle_b200_rx_sps8.argtypes = [vp, vp, sz, i32, u32, u32, vp, sz, ctypes.POINTER(sz)]
     L.btle_b200_synth_streams_device.argtypes = [vp, vp, sz, sz, sz, vp, vp, vp, sz, ctypes.POINTER(sz), vp]
+    L.btle_b200_stream_open.argtypes = [vp, vp, sz, ctypes.POINTER(vp)]
+    L.btle_b200_stream_acquire.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(sz)]
+    L.btle_b200_stream_commit.argtypes = [vp, sz, vp, sz, ctypes.POINTER(sz)]
+    L.btle_b200_stream_push.argtypes = [vp, vp, sz, vp, sz, ctypes.POINTER(sz)]
+    L.btle_b200_stream_set_cfg.argtypes = [vp, vp]
+    L.btle_b200_stream_finish.argtypes = [vp, vp, sz, ctypes.POINTER(sz)]
+    L.btle_b200_stream_close.argtypes = [vp]
+    L.btle_b200_stream_close.restype = None
     L.btle_b200_streams_open.argtypes = [vp, vp, sz, sz, ctypes.POINTER(vp)]
     L.btle_b200_streams_acquire.argtypes = [vp, sz, ctypes.POINTER(vp), ctypes.POINTER(sz)]
     L.btle_b200_streams_commit.argtypes = [vp, sz, sz, vp, sz, ctypes.POINTER(sz)]

@@ -1499,15 +1499,40 @@ model_rx_batch_kernel(const int16_t *__restrict__ gi, const int16_t *__restrict_
 // ================================================================================================
 constexpr unsigned kCountRing = 64;  // context-owned allocation counters (launch_rx)
 constexpr int kSlotUsers = 4;        // streams whose last launch is tracked per cfg slot (more share one entry, see note_use)
+
+// `n` elements of T in memory the buffer owns: device memory, or page-locked host memory (kHost).  It is released
+// through cudaFree / cudaFreeHost, which wait for work still using it, so a buffer may be regrown or dropped while a
+// launch that reads it is held on another stream.  The owner selects the context's device before that.
+template <class T, bool kHost = false>
+struct Buf {
+  T *p = nullptr;
+  size_t n = 0;
+  Buf() = default;
+  Buf(const Buf &) = delete;
+  Buf &operator=(const Buf &) = delete;
+  ~Buf() { release(); }
+  operator T *() const { return p; }
+  void release() {
+    if (p) { if (kHost) cudaFreeHost(p); else cudaFree(p); }
+    p = nullptr;
+    n = 0;
+  }
+  int alloc(btle_b200_ctx *ctx, size_t count);             // exactly `count` elements; the old ones are dropped
+  int reserve(btle_b200_ctx *ctx, size_t count) {          // at least `count`, with room to grow
+    return p && n >= count ? BTLE_OK : alloc(ctx, count + count / 8 + 4096 / sizeof(T));
+  }
+};
+template <class T> using HostBuf = Buf<T, true>;
+
 struct StreamUse {                   // the last launch a stream enqueued: CUDA's id of the stream + an event behind it
   unsigned long long stream = 0;
   cudaEvent_t ev = nullptr;
   unsigned long long stamp = 0;      // 0: no launch recorded
 };
 struct CfgSlot {                     // one uploaded btle_stream_cfg array + the per-stream parameters derived from it
-  btle_stream_cfg *d = nullptr; size_t cap = 0;   // (small LRU cache, see upload_cfgs)
-  StreamParams *d_params = nullptr;
-  btle_stream_cfg *h = nullptr; StreamParams *h_params = nullptr;   // page-locked sources of the upload (cap entries)
+  Buf<btle_stream_cfg> d;            // (small LRU cache, see upload_cfgs)
+  Buf<StreamParams> d_params;
+  HostBuf<btle_stream_cfg> h; HostBuf<StreamParams> h_params;   // page-locked sources of the upload
   size_t n = 0;                      // entries of the cached array (0: empty)
   unsigned long long up_stream = 0;  // stream the upload was enqueued on
   cudaEvent_t uploaded = nullptr;    // recorded behind the upload's two copies
@@ -1522,33 +1547,45 @@ struct MapSlot {                     // encoded TMA tensor maps of one (pointer,
 struct btle_b200_ctx {
   int device = 0;
   cudaStream_t stream = nullptr;
-  cudaStream_t copy_stream = nullptr;    // second stream of the segmented host-buffer path
   std::string err;
   int last_launches = 0;
-  bool attr_done = false, attr_sps8_done = false;
   int num_sms = 0;                  // cudaDevAttrMultiProcessorCount, read at creation
   void *encode_tiled = nullptr;     // cuTensorMapEncodeTiled, fetched through the runtime
   unsigned long long tick = 0;
   CfgSlot cfg_slot[4];
   MapSlot map_slot[4];
   // scratch owned by the context (host-buffer entry points)
-  int8_t *d_iq = nullptr; size_t d_iq_bytes = 0;
-  btle_pkt_rec *d_out = nullptr; size_t d_out_cap = 0;
-  btle_unit_dir *d_dir = nullptr; size_t d_dir_cap = 0;
-  unsigned *d_count = nullptr;
-  unsigned *d_count_ring = nullptr; // kCountRing allocation counters for launches that do not hand in their own (no memset node)
+  Buf<int8_t> d_iq;
+  Buf<btle_pkt_rec> d_out;
+  Buf<btle_unit_dir> d_dir;
+  Buf<unsigned> d_count;
+  Buf<unsigned> d_count_ring;       // kCountRing allocation counters for launches that do not hand in their own (no memset node)
   unsigned ring_pos = 0;
   StreamUse ring_last[kCountRing / 2];   // [ring_pos % (kCountRing/2)]: the ring launch that next launch depends on (launch_rx)
   size_t lead_bytes = 0;            // bytes readable in front of d_iq (set by the stream session around its launches; RSSI of hits at a segment's very start)
-  unsigned *h_count = nullptr;      // pinned
-  btle_pkt_rec *h_recs = nullptr; size_t h_recs_cap = 0;   // pinned staging for records
-  btle_unit_dir *h_dir = nullptr; size_t h_dir_cap = 0;    // pinned staging for the unit directory
-  int8_t *h_stage[2] = {nullptr, nullptr}; size_t h_stage_bytes = 0;   // pinned staging for pageable callers
+  HostBuf<unsigned> h_count;
+  HostBuf<btle_pkt_rec> h_recs;     // staging for records
+  HostBuf<btle_unit_dir> h_dir;     // staging for the unit directory
+  HostBuf<int8_t> h_stage[2];       // staging for pageable callers
   cudaEvent_t stage_free[2] = {nullptr, nullptr};
-  void *d_leaf = nullptr; size_t d_leaf_bytes = 0;
-  btle_conn_cand *d_cand = nullptr; size_t d_cand_bytes = 0;   // device candidates of btle_b200_discover
-  bool attr_disc_done = false;
+  Buf<uint8_t> d_leaf;              // scratch of the leaf entry points (leaf_layout)
+  Buf<btle_conn_cand> d_cand;       // device candidates of btle_b200_discover
 };
+
+template <class T, bool kHost>
+int Buf<T, kHost>::alloc(btle_b200_ctx *ctx, size_t count) {
+  release();
+  void *q = nullptr;
+  const cudaError_t e = kHost ? cudaHostAlloc(&q, count * sizeof(T), cudaHostAllocDefault) : cudaMalloc(&q, count * sizeof(T));
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    ctx->err = kHost ? "cudaHostAlloc failed" : "cudaMalloc failed";
+    return BTLE_ENOMEM;
+  }
+  p = static_cast<T *>(q);
+  n = count;
+  return BTLE_OK;
+}
 
 namespace {
 
@@ -1561,17 +1598,25 @@ namespace {
     }                                                                                     \
   } while (0)
 
-int ensure(btle_b200_ctx *ctx, void **p, size_t *have, size_t need) {
-  if (*have >= need && *p) return BTLE_OK;
-  if (*p) cudaFree(*p);
-  *p = nullptr; *have = 0;
-  const size_t want = need + need / 8 + 4096;
-  if (cudaMalloc(p, want) != cudaSuccess) {
-    cudaGetLastError();
-    ctx->err = "cudaMalloc failed";
-    return BTLE_ENOMEM;
-  }
-  *have = want;
+// Lays the leaf entry points' scratch out in ctx->d_leaf: piece(p, n) stands for n elements of T, and each piece starts
+// on a 256-byte boundary.  leaf_layout(ctx, piece(a, na), piece(b, nb), ...) reserves the whole and sets a, b, ...
+template <class T> struct Piece { T *&p; size_t n; };
+template <class T> Piece<T> piece(T *&p, size_t n) { return {p, n}; }
+constexpr size_t piece_bytes(size_t bytes) { return (bytes + 255) & ~size_t(255); }
+template <class... T>
+int leaf_layout(btle_b200_ctx *ctx, Piece<T>... pieces) {
+  const int rc = ctx->d_leaf.reserve(ctx, (piece_bytes(pieces.n * sizeof(T)) + ...));
+  if (rc) return rc;
+  uint8_t *at = ctx->d_leaf;
+  ((pieces.p = reinterpret_cast<T *>(at), at += piece_bytes(pieces.n * sizeof(T))), ...);
+  return BTLE_OK;
+}
+
+// The end of a leaf entry point: its kernel's launch checked, `bytes` of the kernel's output copied to `dst`, waited for.
+int leaf_result(btle_b200_ctx *ctx, void *dst, const void *src, size_t bytes) {
+  BTLE_CUDA(ctx, cudaGetLastError());
+  BTLE_CUDA(ctx, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  BTLE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return BTLE_OK;
 }
 
@@ -1617,23 +1662,12 @@ int upload_cfgs(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size_t n, cudaS
       for (const StreamUse &u : pick->use)
         if (u.stamp && u.stream != sid) BTLE_CUDA(ctx, cudaStreamWaitEvent(st, u.ev, 0));
     }
-    if (pick->cap < n) {
-      if (pick->d) cudaFree(pick->d);                        // (cudaFree / cudaFreeHost wait for work that still uses them)
-      if (pick->d_params) cudaFree(pick->d_params);
-      if (pick->h) cudaFreeHost(pick->h);
-      if (pick->h_params) cudaFreeHost(pick->h_params);
-      pick->d = nullptr; pick->d_params = nullptr; pick->h = nullptr; pick->h_params = nullptr; pick->cap = 0; pick->n = 0;
-      const size_t want = n + n / 4 + 16;
-      if (cudaMalloc(&pick->d, want * sizeof(btle_stream_cfg)) != cudaSuccess || cudaMalloc(&pick->d_params, want * sizeof(StreamParams)) != cudaSuccess ||
-          cudaHostAlloc(&pick->h, want * sizeof(btle_stream_cfg), cudaHostAllocDefault) != cudaSuccess ||
-          cudaHostAlloc(&pick->h_params, want * sizeof(StreamParams), cudaHostAllocDefault) != cudaSuccess) {
-        cudaGetLastError(); ctx->err = "cudaMalloc failed"; return BTLE_ENOMEM;
-      }
-      pick->cap = want;
-    } else if (pick->n) {
-      BTLE_CUDA(ctx, cudaEventSynchronize(pick->uploaded));   // the staging still feeds the previous upload's copies
-    }
+    // Staging that is kept still feeds the previous upload's copies; arrays that grow are freed by cudaFree /
+    // cudaFreeHost, which wait for the work that still uses them.
+    if (pick->n && pick->h.n >= n && pick->h_params.n >= n) BTLE_CUDA(ctx, cudaEventSynchronize(pick->uploaded));
     pick->n = 0;
+    if (pick->d.reserve(ctx, n) || pick->d_params.reserve(ctx, n) || pick->h.reserve(ctx, n) || pick->h_params.reserve(ctx, n))
+      return BTLE_ENOMEM;
     for (StreamUse &u : pick->use) u.stamp = 0;              // ordered before the new copies by the waits above
     memcpy(pick->h, cfgs, n * sizeof(btle_stream_cfg));
     for (size_t i = 0; i < n; ++i) {                         // make_params(): btle_params.h, the same code the CPU emulator runs
@@ -1723,11 +1757,6 @@ int launch_rx(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t s
   const long long spans = (nchunks + kSpanChunks - 1) / kSpanChunks;
   if (spans * (long long)n_streams > 0x07FFFFFFll || nchunks > 0x7FFFFFFFll) { ctx->err = "batch too large for one launch"; return BTLE_EINVAL; }
   const Plan plan = plan_for(ctx, n_streams, n_int8);
-  const size_t smem = sizeof(Smem);
-  if (!ctx->attr_done) {
-    BTLE_CUDA(ctx, cudaFuncSetAttribute(btle_rx_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    ctx->attr_done = true;
-  }
   CfgSlot *cs = nullptr;
   rc = upload_cfgs(ctx, cfgs, n_streams, st, sid, &cs);
   if (rc) return rc;
@@ -1748,7 +1777,7 @@ int launch_rx(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t s
     zero_next = ctx->d_count_ring + (ctx->ring_pos + kCountRing / 2) % kCountRing;
   }
   const unsigned grid = (unsigned)std::min<long long>(plan.total_units, (long long)ctx->num_sms * kCtasPerSm);   // one persistent CTA per SM
-  btle_rx_persistent_kernel<<<grid, kThreads, smem, st>>>(
+  btle_rx_persistent_kernel<<<grid, kThreads, sizeof(Smem), st>>>(
       ms->map32, ms->map12, d_iq, (long long)stride, (long long)n_int8, cs->d_params, plan, d_out,
       (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu), d_count, reinterpret_cast<uint2 *>(d_dir), zero_next, (long long)ctx->lead_bytes);
   BTLE_CUDA(ctx, cudaGetLastError());
@@ -1768,16 +1797,6 @@ bool rec_less(const btle_pkt_rec &a, const btle_pkt_rec &b) {
   if (a.stream != b.stream) return a.stream < b.stream;
   if (a.chunk != b.chunk) return a.chunk < b.chunk;
   return a.n0 < b.n0;
-}
-
-int ensure_pinned(btle_b200_ctx *ctx, void **p, size_t *have, size_t need) {
-  if (*have >= need && *p) return BTLE_OK;
-  if (*p) cudaFreeHost(*p);
-  *p = nullptr; *have = 0;
-  const size_t want = need + need / 4 + 4096;
-  if (cudaHostAlloc(p, want, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); ctx->err = "cudaHostAlloc failed"; return BTLE_ENOMEM; }
-  *have = want;
-  return BTLE_OK;
 }
 
 // memcpy with a few threads: one core moves ~10 GB/s, a PCIe 5 x16 link takes ~55 GB/s
@@ -1814,14 +1833,12 @@ int h2d_rows(btle_b200_ctx *ctx, int8_t *dst, size_t dpitch, const int8_t *src, 
     return BTLE_OK;
   }
   const size_t seg = size_t(32) << 20;
-  if (ctx->h_stage_bytes < seg) {
-    for (int b = 0; b < 2; ++b) {
-      if (ctx->h_stage[b]) cudaFreeHost(ctx->h_stage[b]);
-      ctx->h_stage[b] = nullptr;
-      if (cudaHostAlloc(reinterpret_cast<void **>(&ctx->h_stage[b]), seg, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); ctx->err = "cudaHostAlloc failed"; return BTLE_ENOMEM; }
-      if (!ctx->stage_free[b]) BTLE_CUDA(ctx, cudaEventCreateWithFlags(&ctx->stage_free[b], cudaEventDisableTiming));
+  for (int b = 0; b < 2; ++b) {
+    if (ctx->h_stage[b].n < seg) {
+      const int rc = ctx->h_stage[b].alloc(ctx, seg);
+      if (rc) return rc;
     }
-    ctx->h_stage_bytes = seg;
+    if (!ctx->stage_free[b]) BTLE_CUDA(ctx, cudaEventCreateWithFlags(&ctx->stage_free[b], cudaEventDisableTiming));
   }
   int b = 0;
   bool used[2] = {false, false};
@@ -1838,47 +1855,58 @@ int h2d_rows(btle_b200_ctx *ctx, int8_t *dst, size_t dpitch, const int8_t *src, 
   return BTLE_OK;
 }
 
+// Host captures (n_streams rows `stride` bytes apart, page-locked or pageable) -> ctx->d_iq, rows `*pitch` bytes apart.
+// Exactly the caller's bytes are read: n_int8 per capture, never the padding behind the last one.
+int ingest(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stride, size_t n_int8, size_t *pitch) {
+  if (n_streams > 1 && stride < n_int8) { ctx->err = "stream stride smaller than stream length"; return BTLE_EINVAL; }
+  *pitch = (n_int8 + 15) & ~size_t(15);
+  const int rc = ctx->d_iq.reserve(ctx, std::max<size_t>(*pitch * n_streams, 16));
+  if (rc) return rc;
+  return h2d_rows(ctx, ctx->d_iq, *pitch, iq, n_streams > 1 ? stride : n_int8, n_int8, n_streams, ctx->stream);
+}
+
+// After a launch on `st` that counted its results in ctx->d_count: the count to the host and a wait (*found = the
+// count); then, when n = min(count, cap) > 0, copy(n) enqueues the copies of the first n results and they are waited for.
+template <class Copy>
+int fetch_counted(btle_b200_ctx *ctx, cudaStream_t st, size_t cap, size_t *found, Copy &&copy) {
+  BTLE_CUDA(ctx, cudaMemcpyAsync(ctx->h_count, ctx->d_count, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+  BTLE_CUDA(ctx, cudaStreamSynchronize(st));
+  *found = *ctx->h_count;
+  const size_t n = std::min(*found, cap);
+  if (!n) return BTLE_OK;
+  const int rc = copy(n);
+  if (rc) return rc;
+  BTLE_CUDA(ctx, cudaStreamSynchronize(st));
+  return BTLE_OK;
+}
+
 // After a launch on `st`: count, records and unit directory to the host; records copied into `out` in reference
 // order (walk of the directory).  *n_out = packets found (may exceed cap -> BTLE_EOVERFLOW).
 int fetch_ordered(btle_b200_ctx *ctx, const btle_pkt_rec *d_out, const btle_unit_dir *d_dir, size_t n_units, btle_pkt_rec *out,
                   size_t cap, size_t *n_out, cudaStream_t st) {
-  BTLE_CUDA(ctx, cudaMemcpyAsync(ctx->h_count, ctx->d_count, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-  BTLE_CUDA(ctx, cudaStreamSynchronize(st));
-  const size_t found = *ctx->h_count;
-  const size_t n = std::min(found, cap);
-  *n_out = found;
-  if (n) {
-    size_t hb = ctx->h_recs_cap * sizeof(btle_pkt_rec), db = ctx->h_dir_cap * sizeof(btle_unit_dir);
-    int rc = ensure_pinned(ctx, reinterpret_cast<void **>(&ctx->h_recs), &hb, n * sizeof(btle_pkt_rec));
-    ctx->h_recs_cap = hb / sizeof(btle_pkt_rec);
-    if (rc) return rc;
-    rc = ensure_pinned(ctx, reinterpret_cast<void **>(&ctx->h_dir), &db, n_units * sizeof(btle_unit_dir));
-    ctx->h_dir_cap = db / sizeof(btle_unit_dir);
-    if (rc) return rc;
+  const int rc = fetch_counted(ctx, st, cap, n_out, [&](size_t n) {
+    if (ctx->h_recs.reserve(ctx, n) || ctx->h_dir.reserve(ctx, n_units)) return BTLE_ENOMEM;
     BTLE_CUDA(ctx, cudaMemcpyAsync(ctx->h_recs, d_out, n * sizeof(btle_pkt_rec), cudaMemcpyDeviceToHost, st));
     BTLE_CUDA(ctx, cudaMemcpyAsync(ctx->h_dir, d_dir, n_units * sizeof(btle_unit_dir), cudaMemcpyDeviceToHost, st));
-    BTLE_CUDA(ctx, cudaStreamSynchronize(st));
+    return BTLE_OK;
+  });
+  if (rc) return rc;
+  if (const size_t n = std::min(*n_out, cap)) {
     size_t got = 0;
     btle_b200_gather_ordered(ctx->h_recs, n, ctx->h_dir, n_units, out, cap, &got);
   }
-  if (found > cap) { ctx->err = "output capacity too small"; return BTLE_EOVERFLOW; }
+  if (*n_out > cap) { ctx->err = "output capacity too small"; return BTLE_EOVERFLOW; }
   return BTLE_OK;
 }
 
 int launch_sps8_hits(btle_b200_ctx *ctx, const int16_t *d_iq16, size_t n_samples, uint32_t aa, long long *d_hits, size_t cap, unsigned *d_count,
                      cudaStream_t st) {
-  if (!ctx->attr_sps8_done) {
-    BTLE_CUDA(ctx, cudaFuncSetAttribute(sps8_hits_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSps8Smem));
-    ctx->attr_sps8_done = true;
-  }
   const long long groups = ((long long)n_samples + 255) / 256, tiles = (groups + kSps8Groups - 1) / kSps8Groups;
   const unsigned grid = kSps8Bufs > 1 ? (unsigned)std::min<long long>(tiles, 3ll * ctx->num_sms) : (unsigned)std::min<long long>(tiles, 0x7FFFFFFF);
   sps8_hits_kernel<<<grid, 256, kSps8Smem, st>>>(d_iq16, (long long)n_samples, tiles, aa, d_hits, (unsigned)cap, d_count);
   BTLE_CUDA(ctx, cudaGetLastError());
   return BTLE_OK;
 }
-
-int leaf_buf(btle_b200_ctx *ctx, size_t bytes) { return ensure(ctx, &ctx->d_leaf, &ctx->d_leaf_bytes, bytes); }
 
 // Checks and launch of discover_kernel (the counter is zeroed here).  The channels travel as btle_stream_cfg through the
 // cfg cache, so the kernel reads each capture's whitening words from its StreamParams.
@@ -1912,10 +1940,6 @@ int launch_discover(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, si
   CfgSlot *cs = nullptr;
   rc = upload_cfgs(ctx, cfgs.data(), n_streams, st, sid, &cs);
   if (rc) return rc;
-  if (!ctx->attr_disc_done) {
-    BTLE_CUDA(ctx, cudaFuncSetAttribute(discover_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDiscSmem));
-    ctx->attr_disc_done = true;
-  }
   discover_kernel<<<(unsigned)(tiles * (long long)n_streams), kDiscThreads, kDiscSmem, st>>>(
       d_iq, (long long)stride, (long long)n_int8, tiles, cs->d_params, d_out, (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu), d_count);
   BTLE_CUDA(ctx, cudaGetLastError());
@@ -2031,10 +2055,12 @@ int btle_b200_create(btle_b200_ctx **out, int cuda_device) {
   if (cudaMemcpyToSymbol(c_noise_thr, thr, sizeof thr) != cudaSuccess ||
       cudaMemcpyToSymbol(c_whiten_words, ww, sizeof ww) != cudaSuccess ||
       cudaMemcpyToSymbol(c_crc4, crc, sizeof crc) != cudaSuccess ||
+      cudaFuncSetAttribute(btle_rx_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem)) != cudaSuccess ||
+      cudaFuncSetAttribute(sps8_hits_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSps8Smem) != cudaSuccess ||
+      cudaFuncSetAttribute(discover_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDiscSmem) != cudaSuccess ||
       cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaMalloc(&ctx->d_count, sizeof(unsigned)) != cudaSuccess ||
-      cudaMalloc(&ctx->d_count_ring, 64 * sizeof(unsigned)) != cudaSuccess || cudaMemset(ctx->d_count_ring, 0, 64 * sizeof(unsigned)) != cudaSuccess ||
-      cudaHostAlloc(&ctx->h_count, sizeof(unsigned), cudaHostAllocDefault) != cudaSuccess) {
+      ctx->d_count.alloc(ctx, 1) || ctx->d_count_ring.alloc(ctx, kCountRing) ||
+      cudaMemset(ctx->d_count_ring, 0, kCountRing * sizeof(unsigned)) != cudaSuccess || ctx->h_count.alloc(ctx, 1)) {
     cudaGetLastError();
     btle_b200_destroy(ctx);
     return BTLE_ECUDA;
@@ -2047,21 +2073,13 @@ void btle_b200_destroy(btle_b200_ctx *ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
   if (ctx->stream) cudaStreamDestroy(ctx->stream);
-  if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
-  cudaFree(ctx->d_iq); cudaFree(ctx->d_out); cudaFree(ctx->d_dir); cudaFree(ctx->d_count); cudaFree(ctx->d_count_ring); cudaFree(ctx->d_leaf); cudaFree(ctx->d_cand);
   for (CfgSlot &c : ctx->cfg_slot) {
-    cudaFree(c.d); cudaFree(c.d_params);
-    if (c.h) cudaFreeHost(c.h);
-    if (c.h_params) cudaFreeHost(c.h_params);
     if (c.uploaded) cudaEventDestroy(c.uploaded);
     for (StreamUse &u : c.use) if (u.ev) cudaEventDestroy(u.ev);
   }
   for (StreamUse &u : ctx->ring_last) if (u.ev) cudaEventDestroy(u.ev);
-  if (ctx->h_count) cudaFreeHost(ctx->h_count);
-  if (ctx->h_recs) cudaFreeHost(ctx->h_recs);
-  if (ctx->h_dir) cudaFreeHost(ctx->h_dir);
-  for (int b = 0; b < 2; ++b) { if (ctx->h_stage[b]) cudaFreeHost(ctx->h_stage[b]); if (ctx->stage_free[b]) cudaEventDestroy(ctx->stage_free[b]); }
-  delete ctx;
+  for (cudaEvent_t e : ctx->stage_free) if (e) cudaEventDestroy(e);
+  delete ctx;                                               // frees the buffers
 }
 
 size_t btle_b200_rx_units(const btle_b200_ctx *ctx, size_t n_streams, size_t n_int8) {
@@ -2087,12 +2105,9 @@ int btle_b200_rx_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams
   if (!ctx) return BTLE_EINVAL;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
   // the directory goes to context-owned scratch (callers of this entry point sort the records themselves)
-  const size_t units = btle_b200_rx_units(ctx, n_streams, n_int8);
-  size_t have = ctx->d_dir_cap * sizeof(btle_unit_dir);
-  const int rc = ensure(ctx, reinterpret_cast<void **>(&ctx->d_dir), &have, std::max<size_t>(units, 1) * sizeof(btle_unit_dir));
-  ctx->d_dir_cap = have / sizeof(btle_unit_dir);
+  const int rc = ctx->d_dir.reserve(ctx, std::max<size_t>(btle_b200_rx_units(ctx, n_streams, n_int8), 1));
   if (rc) return rc;
-  return btle_b200_rx_device_dir(ctx, d_iq, n_streams, stride, n_int8, cfgs, d_out, cap, d_count, ctx->d_dir, ctx->d_dir_cap, cuda_stream);
+  return btle_b200_rx_device_dir(ctx, d_iq, n_streams, stride, n_int8, cfgs, d_out, cap, d_count, ctx->d_dir, ctx->d_dir.n, cuda_stream);
 }
 
 void btle_b200_sort_records(btle_pkt_rec *recs, size_t n) { std::sort(recs, recs + n, rec_less); }
@@ -2117,18 +2132,12 @@ int btle_b200_rx_batch(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, s
                        const btle_stream_cfg *cfgs, btle_pkt_rec *out, size_t cap, size_t *n_out) {
   if (!ctx || !n_out || (!out && cap) || (!cfgs && n_streams) || (!iq && n_streams && n_int8)) return BTLE_EINVAL;
   *n_out = 0;
-  if (n_streams > 1 && stride < n_int8) { ctx->err = "stream stride smaller than stream length"; return BTLE_EINVAL; }
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
-  const size_t pitch = (n_int8 + 15) & ~size_t(15);
-  int rc = ensure(ctx, reinterpret_cast<void **>(&ctx->d_iq), &ctx->d_iq_bytes, std::max<size_t>(pitch * n_streams, 16));
+  size_t pitch = 0;
+  int rc = ingest(ctx, iq, n_streams, stride, n_int8, &pitch);
   if (rc) return rc;
-  size_t out_bytes = ctx->d_out_cap * sizeof(btle_pkt_rec);
-  rc = ensure(ctx, reinterpret_cast<void **>(&ctx->d_out), &out_bytes, std::max<size_t>(cap, 1) * sizeof(btle_pkt_rec));
-  ctx->d_out_cap = out_bytes / sizeof(btle_pkt_rec);
-  if (rc) return rc;
-  // exactly the caller's bytes are read: n_int8 per capture, never the padding behind the last one
-  rc = h2d_rows(ctx, ctx->d_iq, pitch, iq, n_streams > 1 ? stride : n_int8, n_int8, n_streams, st);
+  rc = ctx->d_out.reserve(ctx, std::max<size_t>(cap, 1));
   if (rc) return rc;
   rc = btle_b200_rx_device(ctx, ctx->d_iq, n_streams, pitch, n_int8, cfgs, ctx->d_out, cap, ctx->d_count, st);
   if (rc) return rc;
@@ -2142,20 +2151,15 @@ int btle_b200_rx_iq16(btle_b200_ctx *ctx, const int16_t *iq16, size_t n_int16, i
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
   const size_t pitch = (n_int16 + 255) & ~size_t(255);
-  int rc = ensure(ctx, reinterpret_cast<void **>(&ctx->d_iq), &ctx->d_iq_bytes, pitch + 2 * n_int16 + 512);
-  if (rc) return rc;
+  if (ctx->d_iq.reserve(ctx, pitch + 2 * n_int16 + 512) || ctx->d_out.reserve(ctx, std::max<size_t>(cap, 1))) return BTLE_ENOMEM;
   int16_t *d16 = reinterpret_cast<int16_t *>(ctx->d_iq + pitch + 256);      // behind the int8 capture
-  size_t out_bytes = ctx->d_out_cap * sizeof(btle_pkt_rec);
-  rc = ensure(ctx, reinterpret_cast<void **>(&ctx->d_out), &out_bytes, std::max<size_t>(cap, 1) * sizeof(btle_pkt_rec));
-  ctx->d_out_cap = out_bytes / sizeof(btle_pkt_rec);
-  if (rc) return rc;
   if (n_int16) {
-    rc = h2d_rows(ctx, reinterpret_cast<int8_t *>(d16), 2 * n_int16, reinterpret_cast<const int8_t *>(iq16), 2 * n_int16, 2 * n_int16, 1, st);
+    const int rc = h2d_rows(ctx, reinterpret_cast<int8_t *>(d16), 2 * n_int16, reinterpret_cast<const int8_t *>(iq16), 2 * n_int16, 2 * n_int16, 1, st);
     if (rc) return rc;
     iq16_to_iq8_kernel<<<(unsigned)std::min<size_t>((n_int16 + 255) / 256, (size_t)ctx->num_sms * 16), 256, 0, st>>>(d16, (long long)n_int16, shift, ctx->d_iq);
     BTLE_CUDA(ctx, cudaGetLastError());
   }
-  rc = btle_b200_rx_device(ctx, ctx->d_iq, 1, pitch, n_int16, cfg, ctx->d_out, cap, ctx->d_count, st);
+  const int rc = btle_b200_rx_device(ctx, ctx->d_iq, 1, pitch, n_int16, cfg, ctx->d_out, cap, ctx->d_count, st);
   if (rc) return rc;
   return fetch_ordered(ctx, ctx->d_out, ctx->d_dir, btle_b200_rx_units(ctx, 1, n_int16), out, cap, n_out, st);
 }
@@ -2180,11 +2184,11 @@ struct btle_b200_streams {
   static constexpr size_t kLook = 4096;                    // >= 3008 + the kernel's 12-group tile (3072 + 4)
   static constexpr size_t kLead = 256;                     // bytes of the previous set kept in front (a hit may start up to 124 samples
                                                            // before its chunk; the RSSI sum reads the raw IQ there)
-  struct Half {
-    int8_t *h = nullptr, *d = nullptr;                     // page-locked host / device IQ buffers, n parts of `stride` bytes
-    btle_pkt_rec *d_out = nullptr; btle_unit_dir *d_dir = nullptr; unsigned *d_count = nullptr;
-    unsigned *h_count = nullptr; btle_unit_dir *h_dir = nullptr; btle_pkt_rec *h_recs = nullptr;
-    size_t cap = 0, units = 0, n_submitted = 0;
+  struct Half {                                            // buffers sized once by btle_b200_streams_open
+    HostBuf<int8_t> h; Buf<int8_t> d;                      // page-locked host / device IQ buffers, n parts of `stride` bytes
+    Buf<btle_pkt_rec> d_out; Buf<btle_unit_dir> d_dir; Buf<unsigned> d_count;
+    HostBuf<unsigned> h_count; HostBuf<btle_unit_dir> h_dir; HostBuf<btle_pkt_rec> h_recs;
+    size_t n_submitted = 0;
     long long first_chunk = 0;
     cudaStream_t st = nullptr;
     bool busy = false;
@@ -2216,12 +2220,12 @@ int streams_submit(btle_b200_streams *s, int b, size_t n_int8) {
   else
     BTLE_CUDA(ctx, cudaMemcpy2DAsync(H.d, s->stride, H.h, s->stride, L + n_int8, s->n, cudaMemcpyHostToDevice, H.st));
   ctx->lead_bytes = L;
-  const int rc = btle_b200_rx_device_dir(ctx, H.d + L, s->n, s->stride, n_int8, s->cfgs.data(), H.d_out, H.cap, H.d_count, H.d_dir,
-                                         H.units, H.st);
+  const int rc = btle_b200_rx_device_dir(ctx, H.d + L, s->n, s->stride, n_int8, s->cfgs.data(), H.d_out, H.d_out.n, H.d_count, H.d_dir,
+                                         H.d_dir.n, H.st);
   ctx->lead_bytes = 0;
   if (rc) return rc;
   BTLE_CUDA(ctx, cudaMemcpyAsync(H.h_count, H.d_count, sizeof(unsigned), cudaMemcpyDeviceToHost, H.st));
-  BTLE_CUDA(ctx, cudaMemcpyAsync(H.h_dir, H.d_dir, H.units * sizeof(btle_unit_dir), cudaMemcpyDeviceToHost, H.st));
+  BTLE_CUDA(ctx, cudaMemcpyAsync(H.h_dir, H.d_dir, H.d_dir.n * sizeof(btle_unit_dir), cudaMemcpyDeviceToHost, H.st));
   H.busy = true;
   return BTLE_OK;
 }
@@ -2233,7 +2237,7 @@ int streams_collect(btle_b200_streams *s, int b) {
   H.busy = false;
   BTLE_CUDA(ctx, cudaStreamSynchronize(H.st));
   const size_t found = *H.h_count;
-  if (found > H.cap) { ctx->err = "stream segment produced more records than BTLE_MAX_RECS_PER_CHUNK allows"; return BTLE_EOVERFLOW; }
+  if (found > H.d_out.n) { ctx->err = "stream segment produced more records than BTLE_MAX_RECS_PER_CHUNK allows"; return BTLE_EOVERFLOW; }
   if (!found) return BTLE_OK;
   BTLE_CUDA(ctx, cudaMemcpyAsync(H.h_recs, H.d_out, found * sizeof(btle_pkt_rec), cudaMemcpyDeviceToHost, H.st));
   BTLE_CUDA(ctx, cudaStreamSynchronize(H.st));
@@ -2280,20 +2284,14 @@ int btle_b200_streams_open(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size
   s->seg_chunks = segment_chunks; s->seg_bytes = segment_chunks * (size_t)kChunkInt8;
   s->buf_bytes = s->seg_bytes + btle_b200_streams::kLook;
   s->stride = btle_b200_streams::kLead + s->buf_bytes;     // a multiple of 16, as the batched kernel needs
+  const size_t cap = n_streams * segment_chunks * BTLE_MAX_RECS_PER_CHUNK;
+  // a short tail can be cut into more units than a full set (make_plan: down to one chunk per unit, over whole 16-chunk
+  // spans), so the directory is sized for the most any launch of up to segment_chunks chunks per capture can have
+  const size_t units = n_streams * ((segment_chunks + 15) & ~size_t(15));
   for (auto &H : s->half) {
-    H.cap = n_streams * segment_chunks * BTLE_MAX_RECS_PER_CHUNK;
-    // a short tail can be cut into more units than a full set (make_plan: down to one chunk per unit, over whole 16-chunk
-    // spans), so the directory is sized for the most any launch of up to segment_chunks chunks per capture can have
-    H.units = n_streams * ((segment_chunks + 15) & ~size_t(15));
-    if (cudaHostAlloc(reinterpret_cast<void **>(&H.h), n_streams * s->stride, cudaHostAllocDefault) != cudaSuccess ||
-        cudaMalloc(reinterpret_cast<void **>(&H.d), n_streams * s->stride) != cudaSuccess ||
-        cudaMalloc(reinterpret_cast<void **>(&H.d_out), H.cap * sizeof(btle_pkt_rec)) != cudaSuccess ||
-        cudaMalloc(reinterpret_cast<void **>(&H.d_dir), H.units * sizeof(btle_unit_dir)) != cudaSuccess ||
-        cudaMalloc(reinterpret_cast<void **>(&H.d_count), sizeof(unsigned)) != cudaSuccess ||
-        cudaHostAlloc(reinterpret_cast<void **>(&H.h_count), sizeof(unsigned), cudaHostAllocDefault) != cudaSuccess ||
-        cudaHostAlloc(reinterpret_cast<void **>(&H.h_dir), H.units * sizeof(btle_unit_dir), cudaHostAllocDefault) != cudaSuccess ||
-        cudaHostAlloc(reinterpret_cast<void **>(&H.h_recs), H.cap * sizeof(btle_pkt_rec), cudaHostAllocDefault) != cudaSuccess ||
-        cudaStreamCreateWithFlags(&H.st, cudaStreamNonBlocking) != cudaSuccess) {
+    if (H.h.alloc(ctx, n_streams * s->stride) || H.d.alloc(ctx, n_streams * s->stride) || H.d_out.alloc(ctx, cap) ||
+        H.d_dir.alloc(ctx, units) || H.d_count.alloc(ctx, 1) || H.h_count.alloc(ctx, 1) || H.h_dir.alloc(ctx, units) ||
+        H.h_recs.alloc(ctx, cap) || cudaStreamCreateWithFlags(&H.st, cudaStreamNonBlocking) != cudaSuccess) {
       cudaGetLastError();
       ctx->err = "streams_open: allocation failed";
       btle_b200_streams_close(s);
@@ -2308,15 +2306,9 @@ int btle_b200_streams_open(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size
 void btle_b200_streams_close(btle_b200_streams *s) {
   if (!s) return;
   cudaSetDevice(s->ctx->device);
-  for (auto &H : s->half) {
+  for (auto &H : s->half)
     if (H.st) { cudaStreamSynchronize(H.st); cudaStreamDestroy(H.st); }
-    if (H.h) cudaFreeHost(H.h);
-    if (H.h_count) cudaFreeHost(H.h_count);
-    if (H.h_dir) cudaFreeHost(H.h_dir);
-    if (H.h_recs) cudaFreeHost(H.h_recs);
-    cudaFree(H.d); cudaFree(H.d_out); cudaFree(H.d_dir); cudaFree(H.d_count);
-  }
-  delete s;
+  delete s;                                                 // frees the halves' buffers
 }
 
 int btle_b200_streams_set_cfg(btle_b200_streams *s, size_t stream, const btle_stream_cfg *cfg) {
@@ -2447,17 +2439,32 @@ int btle_b200_dbits(btle_b200_ctx *ctx, const int8_t *iq, size_t n_samples, uint
   if (!ctx || !iq || !d_out) return BTLE_EINVAL;
   if (n_samples == 0) return BTLE_OK;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
-  const size_t in_bytes = 2 * n_samples + 2, in_al = (in_bytes + 255) & ~size_t(255);
-  int rc = leaf_buf(ctx, in_al + n_samples);
+  const size_t in_bytes = 2 * n_samples + 2;
+  int8_t *d_in;
+  uint8_t *d_d;
+  const int rc = leaf_layout(ctx, piece(d_in, in_bytes), piece(d_d, n_samples));
   if (rc) return rc;
-  int8_t *d_in = static_cast<int8_t *>(ctx->d_leaf);
-  uint8_t *d_d = reinterpret_cast<uint8_t *>(d_in) + in_al;
   BTLE_CUDA(ctx, cudaMemcpyAsync(d_in, iq, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
   dbits_kernel<<<(unsigned)((n_samples + 255) / 256), 256, 0, ctx->stream>>>(d_in, (long long)n_samples, d_d);
-  BTLE_CUDA(ctx, cudaGetLastError());
-  BTLE_CUDA(ctx, cudaMemcpyAsync(d_out, d_d, n_samples, cudaMemcpyDeviceToHost, ctx->stream));
-  BTLE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return BTLE_OK;
+  return leaf_result(ctx, d_out, d_d, n_samples);
+}
+
+// body of btle_b200_search_unique_bits: a BTLE_* code, the hit (or -1) in *res
+static int search_unique_bits(btle_b200_ctx *ctx, const int8_t *rxp, int search_len, const btle_stream_cfg &cfg, int *res) {
+  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
+  const size_t valid = 8 * (size_t)search_len + 2;          // int8 the reference reads (:1528-1529)
+  const int ngroups = (int)((4 * (size_t)search_len + 127) / 128);
+  const size_t in_bytes = ((size_t)ngroups + 1) * 256;      // ngroups * 128 samples + the carry word, zero behind `valid`
+  int8_t *d_in;
+  uint32_t *d_pd, *d_cand;
+  int *d_res;
+  const int rc = leaf_layout(ctx, piece(d_in, in_bytes), piece(d_pd, 4 * ((size_t)ngroups + 1)), piece(d_cand, (size_t)ngroups + 1),
+                             piece(d_res, 1));
+  if (rc) return rc;
+  BTLE_CUDA(ctx, cudaMemsetAsync(d_in, 0, in_bytes, ctx->stream));
+  BTLE_CUDA(ctx, cudaMemcpyAsync(d_in, rxp, valid, cudaMemcpyHostToDevice, ctx->stream));
+  search_kernel<<<1, 128, 0, ctx->stream>>>(d_in, search_len, cfg, ngroups, d_pd, d_cand, d_res);
+  return leaf_result(ctx, res, d_res, sizeof(int));
 }
 
 int btle_b200_search_unique_bits(btle_b200_ctx *ctx, const int8_t *rxp, int search_len, const uint8_t *unique_bits,
@@ -2467,32 +2474,15 @@ int btle_b200_search_unique_bits(btle_b200_ctx *ctx, const int8_t *rxp, int sear
   if (!ctx || !rxp || !unique_bits || !unique_bits_mask || num_bits != 32 || search_len < 0 || search_len > 4096)
     return BTLE_SEARCH_ERR(BTLE_EINVAL);      // the reference only ever passes LEN_DEMOD_BUF_ACCESS = 32
   if (search_len == 0) return -1;
-#define BTLE_CUDA_S(ctx, call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { (ctx)->err = std::string(#call) + ": " + cudaGetErrorString(e_); return BTLE_SEARCH_ERR(BTLE_ECUDA); } } while (0)
-  BTLE_CUDA_S(ctx, cudaSetDevice(ctx->device));
   btle_stream_cfg cfg{};
   cfg.channel = 37;
   for (int p = 0; p < 32; ++p) {
     cfg.access_addr |= (uint32_t)(unique_bits[p] & 1u) << p;
     cfg.access_mask |= (uint32_t)(unique_bits_mask[p] ? 1u : 0u) << p;
   }
-  const size_t valid = 8 * (size_t)search_len + 2;          // int8 the reference reads (:1528-1529)
-  const int ngroups = (int)((4 * (size_t)search_len + 127) / 128);
-  const size_t in_al = ((size_t)ngroups * 256 + 16 + 255) & ~size_t(255);
-  int rc = leaf_buf(ctx, in_al + ((size_t)ngroups + 1) * 20 + 16);
-  if (rc) return BTLE_SEARCH_ERR(rc);
-  int8_t *d_in = static_cast<int8_t *>(ctx->d_leaf);
-  uint32_t *d_pd = reinterpret_cast<uint32_t *>(reinterpret_cast<uint8_t *>(d_in) + in_al);
-  uint32_t *d_cand = d_pd + 4 * ((size_t)ngroups + 1);
-  int *d_res = reinterpret_cast<int *>(d_cand + (size_t)ngroups + 1);
-  BTLE_CUDA_S(ctx, cudaMemsetAsync(d_in, 0, in_al, ctx->stream));
-  BTLE_CUDA_S(ctx, cudaMemcpyAsync(d_in, rxp, valid, cudaMemcpyHostToDevice, ctx->stream));
-  search_kernel<<<1, 128, 0, ctx->stream>>>(d_in, search_len, cfg, ngroups, d_pd, d_cand, d_res);
-  BTLE_CUDA_S(ctx, cudaGetLastError());
   int res = -1;
-  BTLE_CUDA_S(ctx, cudaMemcpyAsync(&res, d_res, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  BTLE_CUDA_S(ctx, cudaStreamSynchronize(ctx->stream));
-  return res;
-#undef BTLE_CUDA_S
+  const int rc = search_unique_bits(ctx, rxp, search_len, cfg, &res);
+  return rc ? BTLE_SEARCH_ERR(rc) : res;
 }
 
 int btle_b200_demod_byte(btle_b200_ctx *ctx, const int8_t *rxp, int num_byte, uint8_t *out_byte) {
@@ -2500,16 +2490,13 @@ int btle_b200_demod_byte(btle_b200_ctx *ctx, const int8_t *rxp, int num_byte, ui
   if (num_byte == 0) return BTLE_OK;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
   const size_t in_bytes = 64 * (size_t)num_byte - 4;       // last read index: 8*(8n-1)+3
-  int rc = leaf_buf(ctx, 8192);
+  int8_t *d_in;
+  uint8_t *d_o;
+  const int rc = leaf_layout(ctx, piece(d_in, in_bytes), piece(d_o, num_byte));
   if (rc) return rc;
-  int8_t *d_in = static_cast<int8_t *>(ctx->d_leaf);
-  uint8_t *d_o = reinterpret_cast<uint8_t *>(d_in) + 4608;
   BTLE_CUDA(ctx, cudaMemcpyAsync(d_in, rxp, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
   demod_byte_kernel<<<1, 64, 0, ctx->stream>>>(d_in, num_byte, d_o);
-  BTLE_CUDA(ctx, cudaGetLastError());
-  BTLE_CUDA(ctx, cudaMemcpyAsync(out_byte, d_o, num_byte, cudaMemcpyDeviceToHost, ctx->stream));
-  BTLE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return BTLE_OK;
+  return leaf_result(ctx, out_byte, d_o, num_byte);
 }
 
 int btle_b200_scramble_byte(btle_b200_ctx *ctx, const uint8_t *byte_in, int num_byte, int channel, int table_offset,
@@ -2519,30 +2506,24 @@ int btle_b200_scramble_byte(btle_b200_ctx *ctx, const uint8_t *byte_in, int num_
     return BTLE_EINVAL;
   if (num_byte == 0) return BTLE_OK;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
-  int rc = leaf_buf(ctx, 256);
+  uint8_t *d_in, *d_o;
+  const int rc = leaf_layout(ctx, piece(d_in, num_byte), piece(d_o, num_byte));
   if (rc) return rc;
-  uint8_t *d_in = static_cast<uint8_t *>(ctx->d_leaf), *d_o = d_in + 64;
   BTLE_CUDA(ctx, cudaMemcpyAsync(d_in, byte_in, num_byte, cudaMemcpyHostToDevice, ctx->stream));
   scramble_kernel<<<1, 64, 0, ctx->stream>>>(d_in, num_byte, channel, table_offset, d_o);
-  BTLE_CUDA(ctx, cudaGetLastError());
-  BTLE_CUDA(ctx, cudaMemcpyAsync(byte_out, d_o, num_byte, cudaMemcpyDeviceToHost, ctx->stream));
-  BTLE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return BTLE_OK;
+  return leaf_result(ctx, byte_out, d_o, num_byte);
 }
 
 int btle_b200_crc24_byte(btle_b200_ctx *ctx, const uint8_t *byte_in, int num_byte, uint32_t init_hex, uint32_t *crc_out) {
   if (!ctx || (!byte_in && num_byte) || !crc_out || num_byte < 0 || num_byte > 4096) return BTLE_EINVAL;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
-  int rc = leaf_buf(ctx, 8192);
+  uint8_t *d_in;
+  uint32_t *d_o;
+  const int rc = leaf_layout(ctx, piece(d_in, num_byte), piece(d_o, 1));
   if (rc) return rc;
-  uint8_t *d_in = static_cast<uint8_t *>(ctx->d_leaf);
-  uint32_t *d_o = reinterpret_cast<uint32_t *>(d_in + 4096);
   if (num_byte) BTLE_CUDA(ctx, cudaMemcpyAsync(d_in, byte_in, num_byte, cudaMemcpyHostToDevice, ctx->stream));
   crc24_kernel<<<1, 1, 0, ctx->stream>>>(d_in, num_byte, init_hex, d_o);
-  BTLE_CUDA(ctx, cudaGetLastError());
-  BTLE_CUDA(ctx, cudaMemcpyAsync(crc_out, d_o, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-  BTLE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return BTLE_OK;
+  return leaf_result(ctx, crc_out, d_o, sizeof(uint32_t));
 }
 
 uint32_t btle_b200_crc_init_reorder(uint32_t crc_init) { return crc_init_reorder(crc_init); }
@@ -2614,12 +2595,11 @@ int btle_b200_model_rx_batch(btle_b200_ctx *ctx, const int16_t *i, const int16_t
   if (!ctx || !i || !q || !out) return BTLE_EINVAL;
   if (n_packets == 0) return BTLE_OK;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
-  const size_t nb = n_packets * n_samples * 2, a = (nb + 255) & ~size_t(255);
-  int rc = leaf_buf(ctx, 2 * a + n_packets * sizeof(btle_model_rx_rec) + 256);
+  const size_t nb = n_packets * n_samples * 2;
+  int16_t *d_i, *d_q;
+  btle_model_rx_rec *d_o;
+  int rc = leaf_layout(ctx, piece(d_i, n_packets * n_samples), piece(d_q, n_packets * n_samples), piece(d_o, n_packets));
   if (rc) return rc;
-  uint8_t *base = static_cast<uint8_t *>(ctx->d_leaf);
-  int16_t *d_i = reinterpret_cast<int16_t *>(base), *d_q = reinterpret_cast<int16_t *>(base + a);
-  btle_model_rx_rec *d_o = reinterpret_cast<btle_model_rx_rec *>(base + 2 * a);
   BTLE_CUDA(ctx, cudaMemcpyAsync(d_i, i, nb, cudaMemcpyHostToDevice, ctx->stream));
   BTLE_CUDA(ctx, cudaMemcpyAsync(d_q, q, nb, cudaMemcpyHostToDevice, ctx->stream));
   rc = btle_b200_model_rx_batch_device(ctx, d_i, d_q, n_packets, n_samples, sps, channel, crc_init, access_addr, d_o, ctx->stream);
@@ -2640,9 +2620,8 @@ int btle_b200_sps8_hits_device(btle_b200_ctx *ctx, const int16_t *d_iq16, size_t
   cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
   BTLE_CUDA(ctx, cudaMemsetAsync(d_count, 0, sizeof(unsigned), st));
   if (!n_samples) return BTLE_OK;
-  int rc = launch_sps8_hits(ctx, d_iq16, n_samples, access_addr, reinterpret_cast<long long *>(d_hits), std::min<size_t>(cap, 0xFFFFFFFFu), d_count, st);
+  const int rc = launch_sps8_hits(ctx, d_iq16, n_samples, access_addr, reinterpret_cast<long long *>(d_hits), std::min<size_t>(cap, 0xFFFFFFFFu), d_count, st);
   if (rc) return rc;
-  BTLE_CUDA(ctx, cudaGetLastError());
   ctx->last_launches = 1;
   return BTLE_OK;
 }
@@ -2658,32 +2637,26 @@ int btle_b200_discover(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, s
   if (!ctx) return BTLE_EINVAL;
   if (!n_out || (!out && cap) || (!iq && n_streams && n_int8)) { ctx->err = "discover: missing buffer"; return BTLE_EINVAL; }
   *n_out = 0;
-  if (n_streams > 1 && stride < n_int8) { ctx->err = "stream stride smaller than stream length"; return BTLE_EINVAL; }
   int rc = check_data_channels(ctx, channels, n_streams);                  // before any byte is copied
   if (rc) return rc;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
-  const size_t pitch = (n_int8 + 15) & ~size_t(15);
-  rc = ensure(ctx, reinterpret_cast<void **>(&ctx->d_iq), &ctx->d_iq_bytes, std::max<size_t>(pitch * n_streams, 16));
+  size_t pitch = 0;
+  rc = ingest(ctx, iq, n_streams, stride, n_int8, &pitch);
   if (rc) return rc;
-  rc = ensure(ctx, reinterpret_cast<void **>(&ctx->d_cand), &ctx->d_cand_bytes, std::max<size_t>(cap, 1) * sizeof(btle_conn_cand));
-  if (rc) return rc;
-  rc = h2d_rows(ctx, ctx->d_iq, pitch, iq, n_streams > 1 ? stride : n_int8, n_int8, n_streams, st);
+  rc = ctx->d_cand.reserve(ctx, std::max<size_t>(cap, 1));
   if (rc) return rc;
   rc = launch_discover(ctx, ctx->d_iq, n_streams, pitch, n_int8, channels, ctx->d_cand, cap, ctx->d_count, st);
   if (rc) return rc;
-  BTLE_CUDA(ctx, cudaMemcpyAsync(ctx->h_count, ctx->d_count, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-  BTLE_CUDA(ctx, cudaStreamSynchronize(st));
-  const size_t found = *ctx->h_count, n = std::min(found, cap);
-  *n_out = found;
-  if (n) {
+  rc = fetch_counted(ctx, st, cap, n_out, [&](size_t n) {
     BTLE_CUDA(ctx, cudaMemcpyAsync(out, ctx->d_cand, n * sizeof(btle_conn_cand), cudaMemcpyDeviceToHost, st));
-    BTLE_CUDA(ctx, cudaStreamSynchronize(st));
-    std::sort(out, out + n, [](const btle_conn_cand &a, const btle_conn_cand &b) {
-      return a.stream != b.stream ? a.stream < b.stream : a.sample < b.sample;
-    });
-  }
-  if (found > cap) { ctx->err = "output capacity too small"; return BTLE_EOVERFLOW; }
+    return BTLE_OK;
+  });
+  if (rc) return rc;
+  std::sort(out, out + std::min(*n_out, cap), [](const btle_conn_cand &a, const btle_conn_cand &b) {
+    return a.stream != b.stream ? a.stream < b.stream : a.sample < b.sample;
+  });
+  if (*n_out > cap) { ctx->err = "output capacity too small"; return BTLE_EOVERFLOW; }
   return BTLE_OK;
 }
 
@@ -2696,26 +2669,28 @@ int btle_b200_rx_sps8(btle_b200_ctx *ctx, const int16_t *iq16, size_t n_samples,
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
   const size_t bytes = n_samples * 4, hit_cap = n_samples / 256 + 4096;
-  int rc = ensure(ctx, reinterpret_cast<void **>(&ctx->d_iq), &ctx->d_iq_bytes, bytes + 256);
+  int rc = ctx->d_iq.reserve(ctx, bytes + 256);
   if (rc) return rc;
-  rc = leaf_buf(ctx, hit_cap * 8 + 256);
+  long long *d_hits;
+  rc = leaf_layout(ctx, piece(d_hits, hit_cap));
   if (rc) return rc;
-  long long *d_hits = static_cast<long long *>(ctx->d_leaf);
-  const int16_t *d_iq = reinterpret_cast<const int16_t *>(ctx->d_iq);
+  const int16_t *d_iq = reinterpret_cast<const int16_t *>(ctx->d_iq.p);
   rc = h2d_rows(ctx, ctx->d_iq, bytes, reinterpret_cast<const int8_t *>(iq16), bytes, bytes, 1, st);
   if (rc) return rc;
   BTLE_CUDA(ctx, cudaMemsetAsync(ctx->d_count, 0, sizeof(unsigned), st));
   rc = launch_sps8_hits(ctx, d_iq, n_samples, access_addr, d_hits, hit_cap, ctx->d_count, st);
   if (rc) return rc;
-  BTLE_CUDA(ctx, cudaMemcpyAsync(ctx->h_count, ctx->d_count, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-  BTLE_CUDA(ctx, cudaStreamSynchronize(st));
   ctx->last_launches = 1;
-  size_t n_hits = *ctx->h_count;
-  if (n_hits > hit_cap) { ctx->err = "rx_sps8: more access-address hits than the hit buffer holds"; return BTLE_EOVERFLOW; }
-  if (!n_hits) return BTLE_OK;
-  std::vector<long long> hits(n_hits);
-  BTLE_CUDA(ctx, cudaMemcpyAsync(hits.data(), d_hits, n_hits * 8, cudaMemcpyDeviceToHost, st));
-  BTLE_CUDA(ctx, cudaStreamSynchronize(st));
+  size_t n_hits = 0;
+  std::vector<long long> hits;
+  rc = fetch_counted(ctx, st, hit_cap, &n_hits, [&](size_t n) {
+    if (n_hits > hit_cap) { ctx->err = "rx_sps8: more access-address hits than the hit buffer holds"; return BTLE_EOVERFLOW; }
+    hits.resize(n);
+    BTLE_CUDA(ctx, cudaMemcpyAsync(hits.data(), d_hits, n * 8, cudaMemcpyDeviceToHost, st));
+    return BTLE_OK;
+  });
+  if (rc) return rc;
+  if (hits.empty()) return BTLE_OK;
   std::sort(hits.begin(), hits.end());
   // candidates: the first hit of every cluster (hits closer than the shortest possible packet belong to one packet: the same
   // access address seen on neighbouring sample phases), with its window
@@ -2732,10 +2707,10 @@ int btle_b200_rx_sps8(btle_b200_ctx *ctx, const int16_t *iq16, size_t n_samples,
   }
   if (cand.empty()) return BTLE_OK;
   const size_t nc = cand.size();
-  rc = leaf_buf(ctx, nc * 8 + nc * sizeof(btle_model_rx_rec) + 512);
+  long long *d_win;                                         // the hits are consumed: windows and records take their place
+  btle_model_rx_rec *d_rec;
+  rc = leaf_layout(ctx, piece(d_win, nc), piece(d_rec, nc));
   if (rc) return rc;
-  long long *d_win = static_cast<long long *>(ctx->d_leaf);
-  btle_model_rx_rec *d_rec = reinterpret_cast<btle_model_rx_rec *>(reinterpret_cast<uint8_t *>(ctx->d_leaf) + ((nc * 8 + 255) & ~size_t(255)));
   BTLE_CUDA(ctx, cudaMemcpyAsync(d_win, win.data(), nc * 8, cudaMemcpyHostToDevice, st));
   const int adv = (channel >= 37 && channel <= 39);
   model_rx_batch_kernel<<<(unsigned)((nc + 3) / 4), 128, 0, st>>>(d_iq, d_iq + 1, 2, d_win, (int)nc, BTLE_SPS8_WINDOW, 8, adv, channel, access_addr,
@@ -2781,20 +2756,20 @@ int btle_b200_ber_run(btle_b200_ctx *ctx, const btle_ber_cfg *cfg, size_t n_pack
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
   const size_t B = std::min<size_t>(n_packets, 32768);
-  const size_t iq_bytes = B * kBerSamples * sizeof(int16_t);
-  const size_t a_iq = (iq_bytes + 255) & ~size_t(255), a_tr = (B * 40 + 255) & ~size_t(255), a_rec = (B * sizeof(btle_model_rx_rec) + 255) & ~size_t(255);
-  rc = leaf_buf(ctx, 2 * a_iq + a_tr + a_rec + 256);
+  int16_t *d_i, *d_q;
+  uint8_t *d_truth;
+  btle_model_rx_rec *d_rec;
+  unsigned long long *d_acc;
+  rc = leaf_layout(ctx, piece(d_i, B * kBerSamples), piece(d_q, B * kBerSamples), piece(d_truth, B * 40), piece(d_rec, B), piece(d_acc, 3));
   if (rc) return rc;
-  uint8_t *base = static_cast<uint8_t *>(ctx->d_leaf);
-  int16_t *d_i = reinterpret_cast<int16_t *>(base), *d_q = reinterpret_cast<int16_t *>(base + a_iq);
-  uint8_t *d_truth = base + 2 * a_iq;
-  btle_model_rx_rec *d_rec = reinterpret_cast<btle_model_rx_rec *>(base + 2 * a_iq + a_tr);
-  unsigned long long *d_acc = reinterpret_cast<unsigned long long *>(base + 2 * a_iq + a_tr + a_rec);
   BTLE_CUDA(ctx, cudaMemsetAsync(d_acc, 0, 3 * sizeof(unsigned long long), st));
-  cudaEvent_t e0, e1;
-  BTLE_CUDA(ctx, cudaEventCreate(&e0));
-  BTLE_CUDA(ctx, cudaEventCreate(&e1));
-  BTLE_CUDA(ctx, cudaEventRecord(e0, st));
+  struct Timing {                                           // the two events are destroyed on every return
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    ~Timing() { if (e0) cudaEventDestroy(e0); if (e1) cudaEventDestroy(e1); }
+  } t;
+  BTLE_CUDA(ctx, cudaEventCreate(&t.e0));
+  BTLE_CUDA(ctx, cudaEventCreate(&t.e1));
+  BTLE_CUDA(ctx, cudaEventRecord(t.e0, st));
   const int adv = (cfg->channel >= 37);
   int launches = 0;
   for (size_t done = 0; done < n_packets; done += B) {
@@ -2806,13 +2781,12 @@ int btle_b200_ber_run(btle_b200_ctx *ctx, const btle_ber_cfg *cfg, size_t n_pack
     launches += 3;
   }
   BTLE_CUDA(ctx, cudaGetLastError());
-  BTLE_CUDA(ctx, cudaEventRecord(e1, st));
+  BTLE_CUDA(ctx, cudaEventRecord(t.e1, st));
   unsigned long long acc[3];
   BTLE_CUDA(ctx, cudaMemcpyAsync(acc, d_acc, sizeof acc, cudaMemcpyDeviceToHost, st));
   BTLE_CUDA(ctx, cudaStreamSynchronize(st));
   float ms = 0;
-  cudaEventElapsedTime(&ms, e0, e1);
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
+  BTLE_CUDA(ctx, cudaEventElapsedTime(&ms, t.e0, t.e1));
   out->packets = n_packets; out->pkt_err = acc[0]; out->bit_err = acc[1]; out->aa_miss = acc[2];
   out->bit_total = (uint64_t)n_packets * 8 * kBerPduBytes;
   out->seconds = ms * 1e-3;
@@ -2840,13 +2814,11 @@ int btle_b200_gfsk_demod_i16(btle_b200_ctx *ctx, const int16_t *i, const int16_t
   if (!ctx || !i || !q || !bit_out || !signal_out) return BTLE_EINVAL;
   if (n < 2) return BTLE_OK;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
-  const size_t a = (2 * n + 255) & ~size_t(255);
-  int rc = leaf_buf(ctx, 2 * a + 4 * n + n + 512);
+  int16_t *d_i, *d_q;
+  int32_t *d_s;
+  int8_t *d_b;
+  const int rc = leaf_layout(ctx, piece(d_i, n), piece(d_q, n), piece(d_s, n), piece(d_b, n));
   if (rc) return rc;
-  uint8_t *base = static_cast<uint8_t *>(ctx->d_leaf);
-  int16_t *d_i = reinterpret_cast<int16_t *>(base), *d_q = reinterpret_cast<int16_t *>(base + a);
-  int32_t *d_s = reinterpret_cast<int32_t *>(base + 2 * a);
-  int8_t *d_b = reinterpret_cast<int8_t *>(base + 2 * a + 4 * n);
   BTLE_CUDA(ctx, cudaMemcpyAsync(d_i, i, 2 * n, cudaMemcpyHostToDevice, ctx->stream));
   BTLE_CUDA(ctx, cudaMemcpyAsync(d_q, q, 2 * n, cudaMemcpyHostToDevice, ctx->stream));
   gfsk_demod_i16_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(d_i, d_q, (long long)n, d_b, d_s);
@@ -2857,54 +2829,51 @@ int btle_b200_gfsk_demod_i16(btle_b200_ctx *ctx, const int16_t *i, const int16_t
   return BTLE_OK;
 }
 
+// body of btle_b200_search_bit_sequence: a BTLE_* code, the first match (or -1) in *first
+static int search_bit_sequence(btle_b200_ctx *ctx, const int8_t *bit, size_t n, const int8_t *seq, size_t m, long long *first) {
+  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
+  int8_t *d_b, *d_s;
+  long long *d_first;
+  const int rc = leaf_layout(ctx, piece(d_b, n), piece(d_s, m), piece(d_first, 1));
+  if (rc) return rc;
+  *first = -1;                                              // all ones == "none" for the unsigned atomicMin
+  BTLE_CUDA(ctx, cudaMemcpyAsync(d_b, bit, n, cudaMemcpyHostToDevice, ctx->stream));
+  BTLE_CUDA(ctx, cudaMemcpyAsync(d_s, seq, m, cudaMemcpyHostToDevice, ctx->stream));
+  BTLE_CUDA(ctx, cudaMemcpyAsync(d_first, first, 8, cudaMemcpyHostToDevice, ctx->stream));
+  search_seq_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(d_b, (long long)n, d_s, (int)m, d_first);
+  return leaf_result(ctx, first, d_first, 8);
+}
+
 long btle_b200_search_bit_sequence(btle_b200_ctx *ctx, const int8_t *bit, size_t n, const int8_t *seq, size_t m) {
   if (!ctx || !bit || !seq || m == 0 || m > 4096) return BTLE_EINVAL - 1;     // -2: errors never collide with "-1 = not found"
   if (n < m) return -1;
-  if (cudaSetDevice(ctx->device) != cudaSuccess) return BTLE_ECUDA - 1;
-  const size_t a = (n + 255) & ~size_t(255);
-  if (leaf_buf(ctx, a + m + 512)) return BTLE_ENOMEM - 1;
-  int8_t *d_b = static_cast<int8_t *>(ctx->d_leaf), *d_s = d_b + a;
-  long long *d_first = reinterpret_cast<long long *>(d_b + a + ((m + 255) & ~size_t(255)));
-  long long first = -1;                                     // all ones == "none" for the unsigned atomicMin
-  cudaMemcpyAsync(d_b, bit, n, cudaMemcpyHostToDevice, ctx->stream);
-  cudaMemcpyAsync(d_s, seq, m, cudaMemcpyHostToDevice, ctx->stream);
-  cudaMemcpyAsync(d_first, &first, 8, cudaMemcpyHostToDevice, ctx->stream);
-  search_seq_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(d_b, (long long)n, d_s, (int)m, d_first);
-  cudaMemcpyAsync(&first, d_first, 8, cudaMemcpyDeviceToHost, ctx->stream);
-  if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) { ctx->err = cudaGetErrorString(cudaGetLastError()); return BTLE_ECUDA - 1; }
-  return (long)first;
+  long long first = -1;
+  const int rc = search_bit_sequence(ctx, bit, n, seq, m, &first);
+  return rc ? rc - 1 : (long)first;
 }
 
 int btle_b200_crc24_bits(btle_b200_ctx *ctx, const int8_t *bit_in, size_t n, const int8_t *state_init_bit, int8_t *crc_bits_out) {
   if (!ctx || (!bit_in && n) || !state_init_bit || !crc_bits_out) return BTLE_EINVAL;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
-  const size_t a = (n + 255) & ~size_t(255);
-  int rc = leaf_buf(ctx, a + 512);
+  int8_t *d_b, *d_i, *d_o;
+  const int rc = leaf_layout(ctx, piece(d_b, n), piece(d_i, 24), piece(d_o, 24));
   if (rc) return rc;
-  int8_t *d_b = static_cast<int8_t *>(ctx->d_leaf), *d_i = d_b + a, *d_o = d_b + a + 64;
   if (n) BTLE_CUDA(ctx, cudaMemcpyAsync(d_b, bit_in, n, cudaMemcpyHostToDevice, ctx->stream));
   BTLE_CUDA(ctx, cudaMemcpyAsync(d_i, state_init_bit, 24, cudaMemcpyHostToDevice, ctx->stream));
   crc24_bits_kernel<<<1, 1, 0, ctx->stream>>>(d_b, (long long)n, d_i, d_o);
-  BTLE_CUDA(ctx, cudaGetLastError());
-  BTLE_CUDA(ctx, cudaMemcpyAsync(crc_bits_out, d_o, 24, cudaMemcpyDeviceToHost, ctx->stream));
-  BTLE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return BTLE_OK;
+  return leaf_result(ctx, crc_bits_out, d_o, 24);
 }
 
 int btle_b200_scramble_bits(btle_b200_ctx *ctx, const int8_t *bit_in, size_t n, int channel, int8_t *bit_out) {
   if (!ctx || (!bit_in && n) || (!bit_out && n) || channel < 0 || channel > 63) return BTLE_EINVAL;
   if (n == 0) return BTLE_OK;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
-  const size_t a = (n + 255) & ~size_t(255);
-  int rc = leaf_buf(ctx, 2 * a);
+  int8_t *d_b, *d_o;
+  const int rc = leaf_layout(ctx, piece(d_b, n), piece(d_o, n));
   if (rc) return rc;
-  int8_t *d_b = static_cast<int8_t *>(ctx->d_leaf), *d_o = d_b + a;
   BTLE_CUDA(ctx, cudaMemcpyAsync(d_b, bit_in, n, cudaMemcpyHostToDevice, ctx->stream));
   scramble_bits_kernel<<<1, 1, 0, ctx->stream>>>(d_b, (long long)n, channel, d_o);
-  BTLE_CUDA(ctx, cudaGetLastError());
-  BTLE_CUDA(ctx, cudaMemcpyAsync(bit_out, d_o, n, cudaMemcpyDeviceToHost, ctx->stream));
-  BTLE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return BTLE_OK;
+  return leaf_result(ctx, bit_out, d_o, n);
 }
 
 void btle_b200_parse_adv_pdu_header_byte(const uint8_t *b, int *pdu_type, int *tx_add, int *rx_add, int *payload_len) {

@@ -7,6 +7,7 @@ device memory and the stream)."""
 from __future__ import annotations
 
 import ctypes
+from functools import partial
 
 import numpy as np
 
@@ -52,6 +53,30 @@ class BtleRx:
     def last_launches(self) -> int:
         return self._L.btle_b200_last_launches(self._h)
 
+    def _grow_once(self, call, dtype, cap: int, grow: bool = True) -> np.ndarray:
+        """call(out, cap, n_out) into `cap` records of `dtype`; on BTLE_EOVERFLOW, when `grow`, once more with the exact
+        count it reported."""
+        while True:
+            out = np.empty(cap, dtype=dtype)
+            n_out = ctypes.c_size_t(0)
+            rc = call(out.ctypes.data, cap, ctypes.byref(n_out))
+            if rc == BTLE_EOVERFLOW and grow:
+                cap, grow = n_out.value, False
+                continue
+            self._check(rc)
+            return out[:n_out.value]
+
+    def _drain(self, finish, h, buf: np.ndarray) -> np.ndarray:
+        """finish(h, buf, size, n_out) until it stops returning BTLE_EOVERFLOW: every record it hands out."""
+        out = []
+        while True:
+            n = ctypes.c_size_t(0)
+            rc = finish(h, buf.ctypes.data, buf.size, ctypes.byref(n))
+            out.append(buf[:n.value].copy())
+            if rc != BTLE_EOVERFLOW:
+                self._check(rc)
+                return np.concatenate(out)
+
     # ---- host buffers -------------------------------------------------------------------
     def rx_batch(self, iq: np.ndarray, cfgs: np.ndarray, cap: int | None = None) -> np.ndarray:
         """iq: int8 [n_streams, n_int8] (C-contiguous) or [n_int8]; cfgs: CFG_DTYPE [n_streams]."""
@@ -63,19 +88,8 @@ class BtleRx:
         assert cfgs.shape == (ns,)
         # default capacity: typical worst case; grown once on BTLE_EOVERFLOW to the exact count, which is at most
         # BTLE_MAX_PKTS_PER_CHUNK (51) records per chunk, or BTLE_MAX_RECS_PER_CHUNK (123) with BTLE_CFG_REPORT_REJECTED
-        grow = cap is None
-        if cap is None:
-            cap = ns * (n // 16384) * 34 + 16
-        while True:
-            out = np.empty(cap, dtype=REC_DTYPE)
-            n_out = ctypes.c_size_t(0)
-            rc = self._L.btle_b200_rx_batch(self._h, iq.ctypes.data, ns, n, n, cfgs.ctypes.data, out.ctypes.data, cap,
-                                            ctypes.byref(n_out))
-            if rc == BTLE_EOVERFLOW and grow:
-                cap, grow = n_out.value, False
-                continue
-            self._check(rc)
-            return out[:n_out.value]
+        return self._grow_once(partial(self._L.btle_b200_rx_batch, self._h, iq.ctypes.data, ns, n, n, cfgs.ctypes.data), REC_DTYPE,
+                               ns * (n // 16384) * 34 + 16 if cap is None else cap, grow=cap is None)
 
     def rx(self, iq: np.ndarray, **cfg) -> np.ndarray:
         return self.rx_batch(np.asarray(iq).reshape(1, -1), make_cfgs(1, **cfg))
@@ -84,17 +98,8 @@ class BtleRx:
         """int16 interleaved IQ (bladeRF SC16Q11: shift 4, btle_rx.c:307-308) -> records."""
         iq16 = np.ascontiguousarray(iq16, dtype=np.int16)
         cfgs = make_cfgs(1, **cfg)
-        cap = (iq16.size // 16384) * 34 + 16
-        for attempt in range(2):
-            out = np.empty(cap, dtype=REC_DTYPE)
-            n_out = ctypes.c_size_t(0)
-            rc = self._L.btle_b200_rx_iq16(self._h, iq16.ctypes.data, iq16.size, shift, cfgs.ctypes.data, out.ctypes.data, cap,
-                                           ctypes.byref(n_out))
-            if rc == BTLE_EOVERFLOW and attempt == 0:
-                cap = n_out.value
-                continue
-            self._check(rc)
-            return out[:n_out.value]
+        return self._grow_once(partial(self._L.btle_b200_rx_iq16, self._h, iq16.ctypes.data, iq16.size, shift, cfgs.ctypes.data), REC_DTYPE,
+                               (iq16.size // 16384) * 34 + 16)
 
     def rx_sps8(self, iq16: np.ndarray, channel=DEFAULT_CHANNEL, crc_init=DEFAULT_CRC_INIT, access_addr=DEFAULT_ACCESS_ADDR) -> np.ndarray:
         """Interleaved int16 I,Q at 8 samples per symbol (a `btle_ll -q` .bin capture) -> SPS8_REC_DTYPE array: the Python
@@ -118,18 +123,8 @@ class BtleRx:
             iq = iq[None, :]
         ns, n = iq.shape
         ch = np.ascontiguousarray(np.broadcast_to(np.asarray(channels, dtype=np.int32), (ns,)))
-        grow = cap is None
-        if cap is None:
-            cap = ns * (n // 16384 + 1) * 8 + 256
-        while True:
-            out = np.empty(cap, dtype=CAND_DTYPE)
-            n_out = ctypes.c_size_t(0)
-            rc = self._L.btle_b200_discover(self._h, iq.ctypes.data, ns, n, n, ch.ctypes.data, out.ctypes.data, cap, ctypes.byref(n_out))
-            if rc == BTLE_EOVERFLOW and grow:
-                cap, grow = n_out.value, False
-                continue
-            self._check(rc)
-            return out[:n_out.value]
+        return self._grow_once(partial(self._L.btle_b200_discover, self._h, iq.ctypes.data, ns, n, n, ch.ctypes.data), CAND_DTYPE,
+                               ns * (n // 16384 + 1) * 8 + 256 if cap is None else cap, grow=cap is None)
 
     # ---- unbounded capture, pushed in pieces (btle_b200_stream_*) -----------------------------
     def stream(self, segment_chunks: int = 0, **cfg) -> "RxStream":
@@ -255,12 +250,6 @@ class RxStream:
 
     def __init__(self, rx: BtleRx, cfgs: np.ndarray, segment_chunks: int):
         self._rx, self._L = rx, rx._L
-        self._L.btle_b200_stream_open.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.POINTER(ctypes.c_void_p)]
-        self._L.btle_b200_stream_push.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t,
-                                                  ctypes.POINTER(ctypes.c_size_t)]
-        self._L.btle_b200_stream_finish.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t)]
-        self._L.btle_b200_stream_close.argtypes = [ctypes.c_void_p]
-        self._L.btle_b200_stream_close.restype = None
         self._cfg = np.ascontiguousarray(cfgs, dtype=CFG_DTYPE)
         h = ctypes.c_void_p()
         rx._check(self._L.btle_b200_stream_open(rx._h, self._cfg.ctypes.data, int(segment_chunks), ctypes.byref(h)))
@@ -279,15 +268,7 @@ class RxStream:
         return np.concatenate(out) if out else self._buf[:0].copy()
 
     def finish(self) -> np.ndarray:
-        out = []
-        while True:
-            n = ctypes.c_size_t(0)
-            rc = self._L.btle_b200_stream_finish(self._h, self._buf.ctypes.data, self._buf.size, ctypes.byref(n))
-            out.append(self._buf[:n.value].copy())
-            if rc != BTLE_EOVERFLOW:
-                self._rx._check(rc)
-                break
-        return np.concatenate(out)
+        return self._rx._drain(self._L.btle_b200_stream_finish, self._h, self._buf)
 
     def close(self):
         if getattr(self, "_h", None):
@@ -370,16 +351,9 @@ class RxStreams:
 
     def finish(self) -> np.ndarray:
         """End of the captures: decodes up to the shortest one and returns every record still waiting."""
-        out = []
-        while True:
-            n = ctypes.c_size_t(0)
-            rc = self._L.btle_b200_streams_finish(self._h, self._buf.ctypes.data, self._buf.size, ctypes.byref(n))
-            out.append(self._buf[:n.value].copy())
-            if rc != BTLE_EOVERFLOW:
-                self._rx._check(rc)
-                break
+        out = self._rx._drain(self._L.btle_b200_streams_finish, self._h, self._buf)
         self._pending = [[] for _ in range(self.n_streams)]   # bytes behind the shortest capture are not decoded
-        return np.concatenate(out)
+        return out
 
     def close(self):
         if getattr(self, "_h", None):
