@@ -6,21 +6,29 @@
 
 namespace btle {
 
-// scramble_table[ch][i] (scramble_table.h:4): BLE data whitening, 7-bit LFSR x^7+x^4+1 whose
-// register starts as 1 followed by the 6 channel bits, MSB first (matlab/scramble_gen.m:3-41).
-// Compact form: position 0 = the constant 1, positions 1..6 = channel bits 5..0.
-BTLE_HD void make_whiten_row(int channel, uint8_t out[48]) {
-  uint32_t reg = 0;   // bit k = stage k
-  reg |= 1u;
+// BLE data whitening, 7-bit LFSR x^7+x^4+1 whose register starts as 1 followed by the 6 channel
+// bits, MSB first (matlab/scramble_gen.m:3-41).  Register bit k = stage k: stage 0 = the
+// constant 1, stages 1..6 = channel bits 5..0.
+BTLE_HD uint32_t whiten_seed(int channel) {
+  uint32_t reg = 1u;
   for (int i = 0; i < 6; ++i) reg |= ((uint32_t)(channel >> (5 - i)) & 1u) << (1 + i);
+  return reg;
+}
+
+// One LFSR step: returns the next whitening bit (stage 6) and advances the register.
+BTLE_HD uint32_t whiten_step(uint32_t &reg) {
+  const uint32_t o = (reg >> 6) & 1u;
+  reg = ((reg << 1) & 0x7Fu) | o;     // stages move up, stage0 <- old stage6
+  reg ^= o << 4;                      // stage4 <- old stage3 ^ old stage6
+  return o;
+}
+
+// scramble_table[ch][i] (scramble_table.h:4): the whitening bytes of a channel, LSB first.
+BTLE_HD void make_whiten_row(int channel, uint8_t out[48]) {
+  uint32_t reg = whiten_seed(channel);
   for (int b = 0; b < 48; ++b) {
     uint32_t v = 0;
-    for (int bit = 0; bit < 8; ++bit) {
-      const uint32_t o = (reg >> 6) & 1u;
-      v |= o << bit;
-      reg = ((reg << 1) & 0x7Fu) | o;     // stages move up, stage0 <- old stage6
-      reg ^= o << 4;                      // stage4 <- old stage3 ^ old stage6
-    }
+    for (int bit = 0; bit < 8; ++bit) v |= whiten_step(reg) << bit;
     out[b] = (b < 42) ? (uint8_t)v : 0;
   }
 }

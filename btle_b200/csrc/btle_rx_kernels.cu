@@ -11,7 +11,8 @@
 //                   parse, length guards, CRC-24 (4 bytes per step), 64-byte record appended
 //   ring            4 span slots between them, mbarrier full/empty protocol
 // Also here: leaf kernels with the reference's function signatures (unit parity), the Python
-// model's receiver batched one warp per packet, and the transmit PHY (4- and 8-sps modulators).
+// model's receiver batched one warp per packet, and the transmit PHY (one 4- and 8-sps modulator block,
+// gfsk_block, shared by the modulator, capture-synthesiser and BER kernels).
 // No tensor cores: the path has no dense contraction (integer compare / bit work on a stream).
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -685,11 +686,13 @@ __global__ void scramble_kernel(const uint8_t *in, int n, int channel, int off, 
   out[i] = in[i] ^ (uint8_t)(c_whiten_words[channel][t >> 2] >> (8 * (t & 3)));   // btle_rx.c:1232-1237
 }
 
-__global__ void crc24_kernel(const uint8_t *in, int n, uint32_t init, uint32_t *out) {
-  uint32_t crc = init & 0xFFFFFFu;
-  for (int i = 0; i < n; ++i) crc = c_crc4[(crc ^ in[i]) & 0xFFu] ^ (crc >> 8);    // btle_rx.c:1215-1218
-  *out = crc;
+// CRC-24 register after the bytes p[0..n), one table step per byte (btle_rx.c:1215-1218)
+__device__ __forceinline__ uint32_t crc24_bytes(uint32_t crc, const uint8_t *p, int n) {
+  for (int i = 0; i < n; ++i) crc = c_crc4[(crc ^ p[i]) & 0xFFu] ^ (crc >> 8);
+  return crc;
 }
+
+__global__ void crc24_kernel(const uint8_t *in, int n, uint32_t init, uint32_t *out) { *out = crc24_bytes(init & 0xFFFFFFu, in, n); }
 
 // stream_callback's sample reduction (btle_rx.c:307-308): int16 -> (x >> shift) & 0xFF
 __global__ void iq16_to_iq8_kernel(const int16_t *__restrict__ in, long long n, int shift, int8_t *__restrict__ out) {
@@ -730,34 +733,28 @@ __global__ void crc24_bits_kernel(const int8_t *in, long long n, const int8_t *i
 
 // scramble_core, btlelib.py:226-263: same LFSR as scramble_table.h, applied bit by bit.
 __global__ void scramble_bits_kernel(const int8_t *in, long long n, int channel, int8_t *out) {
-  uint32_t reg = 1u;
-  for (int i = 0; i < 6; ++i) reg |= ((uint32_t)(channel >> (5 - i)) & 1u) << (1 + i);
-  for (long long t = 0; t < n; ++t) {
-    const uint32_t o = (reg >> 6) & 1u;
-    out[t] = (int8_t)((o + (uint32_t)in[t]) & 1u);
-    reg = ((reg << 1) & 0x7Fu) | o;
-    reg ^= o << 4;
-  }
+  uint32_t reg = whiten_seed(channel);
+  for (long long t = 0; t < n; ++t) out[t] = (int8_t)((whiten_step(reg) + (uint32_t)in[t]) & 1u);
 }
 
-// Transmit PHY: one CTA per packet.  Every thread owns 8 consecutive output samples: frequency
-// word per sample from the (at most 3 / 17) filter taps that see an impulse, block-wide inclusive
-// scan for the phase, table lookup.  SPS == 4: btle_tx.c:1022-1063; SPS == 8: btlelib.py:146-189.
-template <int SPS>
-__global__ void __launch_bounds__(512)
-tx_modulate_kernel(const uint8_t *__restrict__ air, const int32_t *__restrict__ nbytes, int max_bytes,
-                   int8_t *__restrict__ out_i, int8_t *__restrict__ out_q) {
-  __shared__ uint8_t sb[128];
-  __shared__ int warp_tot[16];
-  const int pkt = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int nb = nbytes[pkt];
-  for (int i = tid; i < 128; i += blockDim.x) sb[i] = (i < nb) ? air[(size_t)pkt * max_bytes + i] : 0;
-  __syncthreads();
-  const int nbit = 8 * nb;
-  const int nsamp = nbit * SPS + 16, nsamp_max = 8 * max_bytes * SPS + 16;
+// Transmit PHY, run by one CTA per packet: the GFSK modulator of the air bits sb[0..nbit) (LSB first), nsamp = nbit * SPS
+// + 16 samples.  Each pass covers 8 samples per thread of the block, 8 consecutive ones per thread: frequency word per
+// sample from the (at most 3 / 17) filter taps that see an impulse, block-wide inclusive scan for the phase, carried from
+// pass to pass.  THREADS is the block size, or 0 to read it from blockDim.x.  (On an H100 80GB HBM3 at 700 W, a constant
+// made ber_synth_kernel about 15 % faster than reading blockDim.x, and tx_modulate_kernel<8> about 10 % slower.)
+// sink(m, ph) is called with the phase-table index of every sample m < n_out (words past the packet are 0).
+//   SPS 4 (btle_tx.c:1022-1063): sample m takes the phase before word m, modulo 1024
+//   SPS 8 (btlelib.py:146-189): sample m takes the phase including word m, modulo 2048
+// Every thread of the block must call it; it ends with a block barrier, so the sink's shared-memory writes are visible.
+template <int SPS, int THREADS, class Sink>
+__device__ __forceinline__ void gfsk_block(const uint8_t *sb, int nbit, int n_out, Sink sink) {
+  __shared__ int warp_tot[THREADS ? THREADS / 32 : 32];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const unsigned nthreads = THREADS ? THREADS : blockDim.x;
+  const int nsamp = nbit * SPS + 16;
   auto pm1 = [&](int k) { return ((sb[k >> 3] >> (k & 7)) & 1) ? 1 : -1; };
   int run = 0;                                             // phase carried through the whole packet
-  for (int base = 0; base < nsamp_max; base += 8 * blockDim.x) {
+  for (int base = 0; base < n_out; base += 8 * nthreads) {
     const int s0 = base + 8 * tid;
     int f[8];
 #pragma unroll
@@ -801,28 +798,57 @@ tx_modulate_kernel(const uint8_t *__restrict__ air, const int32_t *__restrict__ 
     if (lane == 31) warp_tot[warp] = incl;
     __syncthreads();
     int woff = 0, tot = 0;
-    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) { if (w < warp) woff += warp_tot[w]; tot += warp_tot[w]; }
+    for (int w = 0; w < (int)(nthreads >> 5); ++w) { if (w < warp) woff += warp_tot[w]; tot += warp_tot[w]; }
     const int excl = run + woff + incl - loc;              // sum of all frequency words before this thread's first
 #pragma unroll
     for (int u = 0; u < 8; ++u) {
       const int m = s0 + u;
-      if (m >= nsamp_max) break;
-      if (SPS == 4) {
-        // sample m uses the phase BEFORE frequency word m is added (sample[0] = table[0], btle_tx.c:1046-1061)
-        const int ph = (excl + (u ? f[u - 1] : 0)) & 1023;
-        const bool on = m < nsamp;
-        out_i[((size_t)pkt * nsamp_max + m) * 2] = on ? c_cos1024[ph] : 0;
-        out_i[((size_t)pkt * nsamp_max + m) * 2 + 1] = on ? c_sin1024[ph] : 0;
-      } else {
-        const int ph = (excl + f[u]) & 2047;               // cumsum includes the current word (btlelib.py:97)
-        const bool on = m < nsamp;
-        out_i[(size_t)pkt * nsamp_max + m] = on ? c_cos2048[ph] : 0;
-        out_q[(size_t)pkt * nsamp_max + m] = on ? c_sin2048[ph] : 0;
-      }
+      if (m >= n_out) break;
+      if (SPS == 4) sink(m, (excl + (u ? f[u - 1] : 0)) & 1023);   // sample[0] = table[0] (btle_tx.c:1046-1061)
+      else sink(m, (excl + f[u]) & 2047);                          // cumsum includes the current word (btlelib.py:97)
     }
     run += tot;
     __syncthreads();
   }
+}
+
+// Air bytes of one packet into sb[0..n_sb): preamble (0x55 / 0xAA by the access address's first bit), the access address
+// little-endian, then PDU + CRC-24 whitened for the channel, zeros behind.  crc_init is the reordered register
+// (crc_init_reorder).  corrupt_bit >= 0 flips that bit of PDU + CRC after the CRC is computed, so the packet fails it.
+__device__ __forceinline__ void build_air(const uint8_t *pdu, int pdu_len, uint32_t aa, uint32_t crc_init, int channel, int corrupt_bit,
+                                          uint8_t *sb, int n_sb) {
+  const uint32_t crc = crc24_bytes(crc_init, pdu, pdu_len);
+  sb[0] = (aa & 1u) ? 0x55 : 0xAA;
+  for (int b = 0; b < 4; ++b) sb[1 + b] = (uint8_t)(aa >> (8 * b));
+  for (int b = 0; b < pdu_len + 3; ++b) {
+    uint8_t v = b < pdu_len ? pdu[b] : (uint8_t)(crc >> (8 * (b - pdu_len)));
+    if (corrupt_bit >= 0 && b == corrupt_bit >> 3) v ^= (uint8_t)(1u << (corrupt_bit & 7));
+    sb[5 + b] = v ^ (uint8_t)(c_whiten_words[channel][b >> 2] >> (8 * (b & 3)));
+  }
+  for (int b = 5 + pdu_len + 3; b < n_sb; ++b) sb[b] = 0;
+}
+
+// The transmit PHY on a batch of air-byte rows: samples past a packet's own, up to the longest row's, are zero.
+template <int SPS>
+__global__ void __launch_bounds__(512)
+tx_modulate_kernel(const uint8_t *__restrict__ air, const int32_t *__restrict__ nbytes, int max_bytes,
+                   int8_t *__restrict__ out_i, int8_t *__restrict__ out_q) {
+  __shared__ uint8_t sb[128];
+  const int pkt = blockIdx.x;
+  const int nb = nbytes[pkt];
+  for (int i = threadIdx.x; i < 128; i += blockDim.x) sb[i] = (i < nb) ? air[(size_t)pkt * max_bytes + i] : 0;
+  __syncthreads();
+  const int nsamp = 8 * nb * SPS + 16, nsamp_max = 8 * max_bytes * SPS + 16;
+  gfsk_block<SPS, 0>(sb, 8 * nb, nsamp_max, [&](int m, int ph) {
+    const bool on = m < nsamp;
+    if (SPS == 4) {
+      out_i[((size_t)pkt * nsamp_max + m) * 2] = on ? c_cos1024[ph] : 0;
+      out_i[((size_t)pkt * nsamp_max + m) * 2 + 1] = on ? c_sin1024[ph] : 0;
+    } else {
+      out_i[(size_t)pkt * nsamp_max + m] = on ? c_cos2048[ph] : 0;
+      out_q[(size_t)pkt * nsamp_max + m] = on ? c_sin2048[ph] : 0;
+    }
+  });
 }
 
 // ---- capture synthesiser (test / benchmark input, SURVEY.md §8d C2-C5): noise floor + one burst per slot, all on
@@ -905,21 +931,19 @@ __device__ SynthSlot synth_slot_geometry(const btle_synth_cfg &sc, const btle_st
   return g;
 }
 
-// One CTA per (stream, slot): PDU from hashes -> CRC-24 -> whitening -> the btle_tx PHY (same arithmetic as
-// tx_modulate_kernel<4>, btle_tx.c:1022-1063) -> scaled by amplitude/127 (floor) and added to the floor with saturation.
+// One CTA per (stream, slot): PDU from hashes -> build_air -> the 4-sps transmit PHY (gfsk_block) -> scaled by
+// amplitude/127 (floor) and added to the floor with saturation.
 __global__ void __launch_bounds__(256)
 synth_bursts_kernel(int8_t *__restrict__ iq, long long stride, long long n_int8, const btle_stream_cfg *__restrict__ cfgs,
                     const btle_synth_cfg sc, long long n_slots, btle_synth_truth *__restrict__ truth) {
   __shared__ uint8_t sb[64];
-  __shared__ int warp_tot[8];
   __shared__ SynthSlot G;
   const long long gid = blockIdx.x;
   const int stream = (int)(gid / n_slots);
   const long long slot = gid - (long long)stream * n_slots;
   const btle_stream_cfg cfg = cfgs[stream];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const long long n_samples = n_int8 / 2;
-  if (tid == 0) {
+  if (threadIdx.x == 0) {
     G = synth_slot_geometry(sc, cfg, stream, slot, n_samples, true);
     const bool adv = cfg.channel >= 37;
     uint8_t pdu[48];
@@ -935,16 +959,7 @@ synth_bursts_kernel(int8_t *__restrict__ iq, long long stride, long long n_int8,
       pdu[1] = (uint8_t)plen;
       for (int b = 0; b < plen; ++b) pdu[2 + b] = (uint8_t)(draw(sc.seed, (uint64_t)stream, (uint64_t)slot, 3 + (b >> 3)) >> (8 * (b & 7)));
     }
-    uint32_t crc = crc_init_reorder(cfg.crc_init);
-    for (int b = 0; b < G.pdu_len; ++b) crc = c_crc4[(crc ^ pdu[b]) & 0xFFu] ^ (crc >> 8);
-    uint8_t body[48];
-    for (int b = 0; b < G.pdu_len; ++b) body[b] = pdu[b];
-    body[G.pdu_len] = (uint8_t)crc; body[G.pdu_len + 1] = (uint8_t)(crc >> 8); body[G.pdu_len + 2] = (uint8_t)(crc >> 16);
-    if (G.corrupt_bit >= 0) body[G.corrupt_bit >> 3] ^= (uint8_t)(1u << (G.corrupt_bit & 7));
-    sb[0] = (cfg.access_addr & 1u) ? 0x55 : 0xAA;
-    for (int b = 0; b < 4; ++b) sb[1 + b] = (uint8_t)(cfg.access_addr >> (8 * b));
-    for (int b = 0; b < G.pdu_len + 3; ++b) sb[5 + b] = body[b] ^ (uint8_t)(c_whiten_words[cfg.channel][b >> 2] >> (8 * (b & 3)));
-    for (int b = G.n_air; b < 64; ++b) sb[b] = 0;
+    build_air(pdu, G.pdu_len, cfg.access_addr, crc_init_reorder(cfg.crc_init), cfg.channel, G.corrupt_bit, sb, 64);
     if (truth) {
       btle_synth_truth t;
       memset(&t, 0, sizeof t);
@@ -955,53 +970,19 @@ synth_bursts_kernel(int8_t *__restrict__ iq, long long stride, long long n_int8,
     }
   }
   __syncthreads();
-  const int nbit = 8 * G.n_air, nsamp = 4 * nbit + 16;
-  auto pm1 = [&](int k) { return ((sb[k >> 3] >> (k & 7)) & 1) ? 1 : -1; };
-  int8_t *cap_base = iq + (long long)stream * stride;
-  // 8 samples per thread, 256 threads: 2048 >= 1520 samples, one pass
-  const int s0 = 8 * tid;
-  int f[8];
-#pragma unroll
-  for (int u = 0; u < 8; ++u) {
-    const int m = s0 + u;
-    int acc = 0;
-    if (m < nsamp - 1) {
-#pragma unroll
-      for (int j = 3; j <= 11; ++j) {
-        const int idx = m + j - 15;
-        if (idx >= 0 && (idx & 3) == 0 && (idx >> 2) < nbit) acc += c_gauss4[j - 3] * pm1(idx >> 2);
-      }
-    }
-    f[u] = acc;
-  }
-  int loc = 0;
-#pragma unroll
-  for (int u = 0; u < 8; ++u) { loc += f[u]; f[u] = loc; }
-  int incl = loc;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) { const int v = __shfl_up_sync(0xFFFFFFFFu, incl, d); if (lane >= d) incl += v; }
-  if (lane == 31) warp_tot[warp] = incl;
-  __syncthreads();
-  int woff = 0;
-  for (int w = 0; w < warp; ++w) woff += warp_tot[w];
-  const int excl = woff + incl - loc;
-#pragma unroll
-  for (int u = 0; u < 8; ++u) {
-    const int m = s0 + u;
-    if (m >= nsamp) break;
-    const int ph = (excl + (u ? f[u - 1] : 0)) & 1023;
-    const long long a = 2 * (G.start + m);
-    if (a + 1 >= n_int8) break;
-    auto addsat = [&](long long at, int wave) {
+  // 256 threads x 8 samples >= 1520 samples: one pass.  Samples behind the capture's last whole sample are not written.
+  int8_t *cap = iq + (long long)stream * stride + 2 * G.start;
+  const int nbit = 8 * G.n_air;
+  gfsk_block<4, 256>(sb, nbit, (int)min((long long)(4 * nbit + 16), n_samples - G.start), [&](int m, int ph) {
+    auto addsat = [&](int8_t &s, int wave) {
       const int p = wave * sc.amplitude;
       const int scaled = p >= 0 ? p / 127 : -((-p + 126) / 127);              // floor division, like the numpy generator
-      int v = (int)cap_base[at] + scaled;
-      v = v > 127 ? 127 : (v < -128 ? -128 : v);
-      cap_base[at] = (int8_t)v;
+      const int v = (int)s + scaled;
+      s = (int8_t)(v > 127 ? 127 : (v < -128 ? -128 : v));
     };
-    addsat(a, c_cos1024[ph]);
-    addsat(a + 1, c_sin1024[ph]);
-  }
+    addsat(cap[2 * m], c_cos1024[ph]);
+    addsat(cap[2 * m + 1], c_sin1024[ph]);
+  });
 }
 
 // ---- 8 samples per symbol, streaming (SURVEY.md 8f-3): where does the access address occur, on which sample phase? ----
@@ -1225,8 +1206,8 @@ discover_kernel(const int8_t *__restrict__ iq, long long stride, long long n_int
 }
 
 // ---- BER flow of python/test_btle_ber.py on the device: packet source + channel + int16 truncation --------------------
-// One CTA per packet: 37 random payload bytes behind the fixed header 42 25 (test_btle_ber.py:27,:49), CRC-24, whitening,
-// the Python model's 8-sps modulator (same arithmetic as tx_modulate_kernel<8>), add_freq_sampling_error (linear
+// One CTA per packet: 37 random payload bytes behind the fixed header 42 25 (test_btle_ber.py:27,:49), build_air,
+// the Python model's 8-sps modulator (gfsk_block<8>), add_freq_sampling_error (linear
 // resampling at 1 + ppm/1e6 and the matching carrier rotation at 2450 MHz, btlelib.py:823-857), add_noise (AWGN,
 // sigma = 127 / 10^(snr/20) / sqrt 2 per rail, :859-871), np.int16() truncation.  Counter-based randomness.
 constexpr int kBerPduBytes = 39, kBerAirBytes = 1 + 4 + kBerPduBytes + 3, kBerSamples = 8 * 8 * kBerAirBytes + 16;   // 3024
@@ -1242,69 +1223,23 @@ __global__ void __launch_bounds__(384)
 ber_synth_kernel(const btle_ber_cfg cfg, unsigned long long first_packet, int n_packets, int16_t *__restrict__ out_i, int16_t *__restrict__ out_q,
                  uint8_t *__restrict__ truth /*[n][40]*/) {
   __shared__ uint8_t sb[64];
-  __shared__ int warp_tot[12];
   __shared__ float txi[kBerSamples + 8], txq[kBerSamples + 8];
-  const int pkt = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int pkt = blockIdx.x, tid = threadIdx.x;
   if (pkt >= n_packets) return;
   const unsigned long long gp = first_packet + (unsigned long long)pkt;
   if (tid == 0) {
     uint8_t pdu[kBerPduBytes];
     pdu[0] = 0x42; pdu[1] = 0x25;
     for (int b = 2; b < kBerPduBytes; ++b) pdu[b] = (uint8_t)(draw(cfg.seed, gp, (uint64_t)(b >> 3), 9) >> (8 * (b & 7)));
-    uint32_t crc = crc_init_reorder(cfg.crc_init);
-    for (int b = 0; b < kBerPduBytes; ++b) crc = c_crc4[(crc ^ pdu[b]) & 0xFFu] ^ (crc >> 8);
-    sb[0] = (cfg.access_addr & 1u) ? 0x55 : 0xAA;
-    for (int b = 0; b < 4; ++b) sb[1 + b] = (uint8_t)(cfg.access_addr >> (8 * b));
-    for (int b = 0; b < kBerPduBytes + 3; ++b) {
-      const uint8_t v = b < kBerPduBytes ? pdu[b] : (uint8_t)(crc >> (8 * (b - kBerPduBytes)));
-      sb[5 + b] = v ^ (uint8_t)(c_whiten_words[cfg.channel][b >> 2] >> (8 * (b & 3)));
-    }
-    for (int b = kBerAirBytes; b < 64; ++b) sb[b] = 0;
+    build_air(pdu, kBerPduBytes, cfg.access_addr, crc_init_reorder(cfg.crc_init), cfg.channel, -1, sb, 64);
     for (int b = 0; b < kBerPduBytes; ++b) truth[(size_t)pkt * 40 + b] = pdu[b];
   }
   __syncthreads();
-  const int nbit = 8 * kBerAirBytes;
-  auto pm1 = [&](int k) { return ((sb[k >> 3] >> (k & 7)) & 1) ? 1 : -1; };
-  const int s0 = 8 * tid;
-  int f[8];
-#pragma unroll
-  for (int u = 0; u < 8; ++u) {
-    const int m = s0 + u;
-    int acc = 0;
-    if (m < kBerSamples) {
-      int y = 0;
-#pragma unroll
-      for (int j = 3; j <= 13; ++j) {
-        const int xi = 17 - j + m;
-        int x = 0;
-        if (xi < 17) x = -1; else if (xi - 17 < 8 * nbit) x = pm1((xi - 17) >> 3);
-        y += c_gauss8[j] * x;
-      }
-      acc = y >> 1;
-    }
-    f[u] = acc;
-  }
-  int loc = 0;
-#pragma unroll
-  for (int u = 0; u < 8; ++u) { loc += f[u]; f[u] = loc; }
-  int incl = loc;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) { const int v = __shfl_up_sync(0xFFFFFFFFu, incl, d); if (lane >= d) incl += v; }
-  if (lane == 31) warp_tot[warp] = incl;
-  __syncthreads();
-  int woff = 0;
-  for (int w = 0; w < warp; ++w) woff += warp_tot[w];
-  const int excl = woff + incl - loc;
-#pragma unroll
-  for (int u = 0; u < 8; ++u) {
-    const int m = s0 + u;
-    if (m < kBerSamples) {
-      const int ph = (excl + f[u]) & 2047;
-      txi[m] = (float)c_cos2048[ph];
-      txq[m] = (float)c_sin2048[ph];
-    }
-  }
-  __syncthreads();
+  // 384 threads x 8 samples >= 3024 samples: one pass
+  gfsk_block<8, 384>(sb, 8 * kBerAirBytes, kBerSamples, [&](int m, int ph) {
+    txi[m] = (float)c_cos2048[ph];
+    txq[m] = (float)c_sin2048[ph];
+  });
   const double e = (double)cfg.ppm * 1e-6;
   const float sigma = 127.0f / exp10f(cfg.snr_db / 20.0f) * 0.70710678f;
   // carrier offset fo = e * 2450e6 Hz at the new sampling time (1/8 us) * (1 + e): cycles per sample
@@ -1380,16 +1315,10 @@ model_rx_batch_kernel(const int16_t *__restrict__ gi, const int16_t *__restrict_
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int i = threadIdx.x; i < 256; i += blockDim.x) crc_tab[i] = c_crc4[i];
   if (threadIdx.x == 0) {                                  // scramble_core's LFSR (btlelib.py:226-263)
-    uint32_t reg = 1u;
-    for (int i = 0; i < 6; ++i) reg |= ((uint32_t)(channel >> (5 - i)) & 1u) << (1 + i);
+    uint32_t reg = whiten_seed(channel);
     for (int w = 0; w < 26; ++w) {
       uint32_t v = 0;
-      for (int b = 0; b < 32; ++b) {
-        const uint32_t o = (reg >> 6) & 1u;
-        v |= o << b;
-        reg = ((reg << 1) & 0x7Fu) | o;
-        reg ^= o << 4;
-      }
+      for (int b = 0; b < 32; ++b) v |= whiten_step(reg) << b;
       wh[w] = v;
     }
   }
