@@ -829,13 +829,14 @@ __device__ __forceinline__ void build_air(const uint8_t *pdu, int pdu_len, uint3
 }
 
 // The transmit PHY on a batch of air-byte rows: samples past a packet's own, up to the longest row's, are zero.
+// A row's length is clamped to 0..max_bytes, so it never reads another row's bytes or past the batch.
 template <int SPS>
 __global__ void __launch_bounds__(512)
 tx_modulate_kernel(const uint8_t *__restrict__ air, const int32_t *__restrict__ nbytes, int max_bytes,
                    int8_t *__restrict__ out_i, int8_t *__restrict__ out_q) {
   __shared__ uint8_t sb[128];
   const int pkt = blockIdx.x;
-  const int nb = nbytes[pkt];
+  const int nb = min(max(nbytes[pkt], 0), max_bytes);
   for (int i = threadIdx.x; i < 128; i += blockDim.x) sb[i] = (i < nb) ? air[(size_t)pkt * max_bytes + i] : 0;
   __syncthreads();
   const int nsamp = 8 * nb * SPS + 16, nsamp_max = 8 * max_bytes * SPS + 16;

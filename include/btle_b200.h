@@ -384,8 +384,9 @@ int btle_b200_rx_iq16(btle_b200_ctx *ctx, const int16_t *iq16, size_t n_int16, i
  *   sps == 8: gfsk_modulation_fixed_point (python/btlelib.py:146-189): NRZ preceded by 17 samples of
  *             -1, 17 integer taps, >>1, phase mod 2048.  d_out_i / d_out_q: planar int8
  *             [n_packets][64*max_bytes+16].
- * Samples behind a packet's own 8*nbytes*sps+16 samples are written as 0.  Device pointers; enqueued
- * on cuda_stream, not synchronised. */
+ * Samples behind a packet's own 8*nbytes*sps+16 samples are written as 0.  Each d_nbytes[k] is clamped to
+ * 0..max_bytes: a longer row is modulated as max_bytes bytes, a negative one as 0 bytes (16 samples).
+ * Device pointers; enqueued on cuda_stream, not synchronised. */
 int btle_b200_tx_modulate_device(btle_b200_ctx *ctx, const uint8_t *d_air, const int32_t *d_nbytes, size_t n_packets,
                                  size_t max_bytes, int sps, int8_t *d_out_i, int8_t *d_out_q, void *cuda_stream);
 
