@@ -692,7 +692,13 @@ __device__ __forceinline__ uint32_t crc24_bytes(uint32_t crc, const uint8_t *p, 
   return crc;
 }
 
-__global__ void crc24_kernel(const uint8_t *in, int n, uint32_t init, uint32_t *out) { *out = crc24_bytes(init & 0xFFFFFFu, in, n); }
+// crc24_byte (btle_rx.c:1224): crc_update starts from the full 32-bit init_hex and masks to 24 bits only after each
+// byte, so bits 24..31 of the init land in bits 16..23 on the first byte; with no byte the result is init & 0xFFFFFF
+__global__ void crc24_kernel(const uint8_t *in, int n, uint32_t init, uint32_t *out) {
+  if (n == 0) { *out = init & 0xFFFFFFu; return; }
+  const uint32_t crc = (c_crc4[(init ^ in[0]) & 0xFFu] ^ (init >> 8)) & 0xFFFFFFu;
+  *out = crc24_bytes(crc, in + 1, n - 1);
+}
 
 // stream_callback's sample reduction (btle_rx.c:307-308): int16 -> (x >> shift) & 0xFF
 __global__ void iq16_to_iq8_kernel(const int16_t *__restrict__ in, long long n, int shift, int8_t *__restrict__ out) {
@@ -710,10 +716,10 @@ __global__ void gfsk_demod_i16_kernel(const int16_t *i, const int16_t *q, long l
   bit[k] = (int8_t)((int32_t)s > 0);
 }
 
-__global__ void search_seq_kernel(const int8_t *bit, long long n, const int8_t *seq, int m, long long *first) {
+__global__ void search_seq_kernel(const int8_t *bit, long long n, const int8_t *seq, long long m, long long *first) {
   const long long s0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (s0 + m > n) return;
-  for (int j = 0; j < m; ++j)
+  for (long long j = 0; j < m; ++j)
     if (bit[s0 + j] != seq[j]) return;                    // btlelib.py:408
   atomicMin(reinterpret_cast<unsigned long long *>(first), (unsigned long long)s0);
 }
@@ -2407,6 +2413,8 @@ int btle_b200_search_unique_bits(btle_b200_ctx *ctx, const int8_t *rxp, int sear
   btle_stream_cfg cfg{};
   cfg.channel = 37;
   for (int p = 0; p < 32; ++p) {
+    // the reference compares a demodulated 0/1 with unique_bits[p] (:1539): a masked value other than 0 or 1 never matches
+    if (unique_bits_mask[p] && unique_bits[p] > 1) return -1;
     cfg.access_addr |= (uint32_t)(unique_bits[p] & 1u) << p;
     cfg.access_mask |= (uint32_t)(unique_bits_mask[p] ? 1u : 0u) << p;
   }
@@ -2770,12 +2778,13 @@ static int search_bit_sequence(btle_b200_ctx *ctx, const int8_t *bit, size_t n, 
   BTLE_CUDA(ctx, cudaMemcpyAsync(d_b, bit, n, cudaMemcpyHostToDevice, ctx->stream));
   BTLE_CUDA(ctx, cudaMemcpyAsync(d_s, seq, m, cudaMemcpyHostToDevice, ctx->stream));
   BTLE_CUDA(ctx, cudaMemcpyAsync(d_first, first, 8, cudaMemcpyHostToDevice, ctx->stream));
-  search_seq_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(d_b, (long long)n, d_s, (int)m, d_first);
+  search_seq_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(d_b, (long long)n, d_s, (long long)m, d_first);
   return leaf_result(ctx, first, d_first, 8);
 }
 
 long btle_b200_search_bit_sequence(btle_b200_ctx *ctx, const int8_t *bit, size_t n, const int8_t *seq, size_t m) {
-  if (!ctx || !bit || !seq || m == 0 || m > 4096) return BTLE_EINVAL - 1;     // -2: errors never collide with "-1 = not found"
+  if (!ctx || (!bit && n) || (!seq && m)) return BTLE_EINVAL - 1;     // -2: errors never collide with "-1 = not found"
+  if (m == 0) return 0;                                     // btlelib.py:408: the empty window at i = 0 matches
   if (n < m) return -1;
   long long first = -1;
   const int rc = search_bit_sequence(ctx, bit, n, seq, m, &first);
@@ -2795,14 +2804,15 @@ int btle_b200_crc24_bits(btle_b200_ctx *ctx, const int8_t *bit_in, size_t n, con
 }
 
 int btle_b200_scramble_bits(btle_b200_ctx *ctx, const int8_t *bit_in, size_t n, int channel, int8_t *bit_out) {
-  if (!ctx || (!bit_in && n) || (!bit_out && n) || channel < 0 || channel > 63) return BTLE_EINVAL;
+  if (!ctx || (!bit_in && n) || (!bit_out && n)) return BTLE_EINVAL;
   if (n == 0) return BTLE_OK;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
   int8_t *d_b, *d_o;
   const int rc = leaf_layout(ctx, piece(d_b, n), piece(d_o, n));
   if (rc) return rc;
   BTLE_CUDA(ctx, cudaMemcpyAsync(d_b, bit_in, n, cudaMemcpyHostToDevice, ctx->stream));
-  scramble_bits_kernel<<<1, 1, 0, ctx->stream>>>(d_b, (long long)n, channel, d_o);
+  // btlelib.py:238-243 seeds the register from bits 5..0 of any integer channel
+  scramble_bits_kernel<<<1, 1, 0, ctx->stream>>>(d_b, (long long)n, channel & 63, d_o);
   return leaf_result(ctx, bit_out, d_o, n);
 }
 

@@ -250,7 +250,8 @@ int btle_b200_last_launches(const btle_b200_ctx *ctx);
 /* search_unique_bits, btle_rx.c:1510: returns the int8 index of the first AA sample of the
  * first match when scanning `search_len` symbols from rxp with a zeroed history, or -1.
  * unique_bits / unique_bits_mask are 32 bytes of 0/1, LSB first (uint32_to_bit_array, :798).
- * Reads rxp[0 .. 8*search_len+1]; search_len <= 4096.  Errors: BTLE_SEARCH_ERR(BTLE_E*) (<= -1001). */
+ * A masked position whose unique_bits value is neither 0 nor 1 never matches a demodulated bit (:1539), so the
+ * result is then -1.  Reads rxp[0 .. 8*search_len+1]; search_len <= 4096.  Errors: BTLE_SEARCH_ERR(BTLE_E*) (<= -1001). */
 int btle_b200_search_unique_bits(btle_b200_ctx *ctx, const int8_t *rxp, int search_len,
                                  const uint8_t *unique_bits, const uint8_t *unique_bits_mask, int num_bits);
 /* demod_byte, btle_rx.c:1489: num_byte <= 64 bytes from rxp[0 .. 64*num_byte+3]. */
@@ -258,7 +259,9 @@ int btle_b200_demod_byte(btle_b200_ctx *ctx, const int8_t *rxp, int num_byte, ui
 /* scramble_byte with scramble_table[channel]+table_offset, btle_rx.c:1232 / scramble_table.h:4. */
 int btle_b200_scramble_byte(btle_b200_ctx *ctx, const uint8_t *byte_in, int num_byte, int channel,
                             int table_offset, uint8_t *byte_out);
-/* crc24_byte, btle_rx.c:1224 (init_hex already reordered), and crc_init_reorder, :1969. */
+/* crc24_byte, btle_rx.c:1224 (init_hex already reordered), and crc_init_reorder, :1969.  Any 32-bit init_hex behaves
+ * as in the reference: the first byte's step starts from all 32 bits, so bits 24..31 of init_hex fold into bits 16..23,
+ * and every step masks to 24 bits; with num_byte 0 the result is init_hex & 0xFFFFFF.  num_byte <= 4096. */
 int btle_b200_crc24_byte(btle_b200_ctx *ctx, const uint8_t *byte_in, int num_byte, uint32_t init_hex,
                          uint32_t *crc_out);
 uint32_t btle_b200_crc_init_reorder(uint32_t crc_init);
@@ -278,12 +281,14 @@ int btle_b200_dbits(btle_b200_ctx *ctx, const int8_t *iq, size_t n_samples, uint
 int btle_b200_gfsk_demod_i16(btle_b200_ctx *ctx, const int16_t *i, const int16_t *q, size_t n, int8_t *bit_out,
                              int32_t *signal_out);
 /* search_unique_bit_sequence(bit, bit_sequence), btlelib.py:402-412: first index where the
- * sequence occurs, or -1 (also the function's return; errors are <= -2... see BTLE_E*). */
+ * sequence occurs, or -1 (also the function's return; errors are <= -2... see BTLE_E*).  Any length m: m == 0
+ * returns 0 (the empty window at index 0 matches, also when n == 0), n < m returns -1. */
 long btle_b200_search_bit_sequence(btle_b200_ctx *ctx, const int8_t *bit, size_t n, const int8_t *seq, size_t m);
 /* crc24_core(bit_in, state_init_bit), btlelib.py:191-219: bit-serial CRC-24 LFSR, 24 result bits. */
 int btle_b200_crc24_bits(btle_b200_ctx *ctx, const int8_t *bit_in, size_t n, const int8_t *state_init_bit,
                          int8_t *crc_bits_out);
-/* scramble_core(bit_in, channel_number), btlelib.py:226-263: whitening of a bit array. */
+/* scramble_core(bit_in, channel_number), btlelib.py:226-263: whitening of a bit array.  Any int channel: the
+ * register is seeded from channel & 63, as the reference takes bits 5..0 of the integer (64 acts as 0, -1 as 63). */
 int btle_b200_scramble_bits(btle_b200_ctx *ctx, const int8_t *bit_in, size_t n, int channel, int8_t *bit_out);
 
 /* ---- the Python model's receiver, batched (BER sweep, BASELINE.json configs[3]) ----------------

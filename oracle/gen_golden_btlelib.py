@@ -5,7 +5,9 @@ call, btlelib.py:90-91,155).  Writes tests/golden/btlelib_rx.npz (committed); wi
 tests/golden/btlelib_rx_random.npz: the reference receiver's verdicts on the 60 random-packet windows of
 tests/test_oracle_btlelib_port.py, whose inputs the test rebuilds itself (checked here against btle_tx / add_noise); with
 --sps, tests/golden/btlelib_rx_sps.npz: the reference receiver at SAMPLE_PER_SYMBOL 1, 2, 4, 8 and 16 on crafted windows
-(sps_windows), inputs stored with the verdicts."""
+(sps_windows), inputs stored with the verdicts; with --leaves, tests/golden/btlelib_leaves.npz: the reference's leaf
+functions (gfsk_demodulation_fixed_point, crc24_core / crc24, scramble_core / scramble, search_unique_bit_sequence) at
+their edges (leaves_cases), written with fixed time stamps so that a rerun gives the same bytes."""
 import os
 import shutil
 import sys
@@ -146,6 +148,120 @@ def sps_cases(bl):
     np.savez_compressed(os.path.join(ROOT, "tests", "golden", "btlelib_rx_sps.npz"), **out)
 
 
+def save_npz_stable(path, arrays):
+    """np.savez_compressed, but with fixed member time stamps, so that the same arrays give the same file bytes."""
+    import io
+    import zipfile
+    with zipfile.ZipFile(path, "w", compression=zipfile.ZIP_DEFLATED) as zf:
+        for key, val in arrays.items():
+            buf = io.BytesIO()
+            np.lib.format.write_array(buf, np.asanyarray(val), allow_pickle=False)
+            info = zipfile.ZipInfo(key + ".npy", date_time=(1980, 1, 1, 0, 0, 0))
+            info.compress_type = zipfile.ZIP_DEFLATED
+            zf.writestr(info, buf.getvalue())
+
+
+def de_bruijn_pairs(k):
+    """A cyclic de Bruijn sequence of order 2 over 0..k-1 (every ordered pair once, cyclically), as a list."""
+    a, seq = [0] * (2 * k), []
+
+    def db(t, p):
+        if t > 2:
+            if 2 % p == 0:
+                seq.extend(a[1:p + 1])
+            return
+        a[t] = a[t - p]
+        db(t + 1, p)
+        for j in range(a[t - p] + 1, k):
+            a[t] = j
+            db(t + 1, t)
+    db(1, 1)
+    return seq
+
+
+def leaves_cases(bl):
+    """tests/golden/btlelib_leaves.npz: the reference's gfsk_demodulation_fixed_point, crc24_core / crc24, scramble_core /
+    scramble and search_unique_bit_sequence at their edges (tests/test_btlelib_leaves_gpu.py)."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from test_btlelib_leaves_gpu import big_search_input, seeded_bits
+    rng = np.random.default_rng(2024)
+    out = {}
+    # gfsk_demodulation_fixed_point: short lengths on full-range samples, then every (i[k], q[k], i[k+1], q[k+1]) over
+    # the int16 extremes: a de Bruijn sequence of the 36 (i, q) pairs, closed by its first pair
+    lens = (0, 1, 2, 3, 256, 257, 513)
+    for k, n in enumerate(lens):
+        i = rng.integers(-32768, 32768, n, dtype=np.int16)
+        q = rng.integers(-32768, 32768, n, dtype=np.int16)
+        i[::7], q[3::11] = -32768, 32767
+        b, s = bl.gfsk_demodulation_fixed_point(i, q)
+        out[f"gfsk{k}_i"], out[f"gfsk{k}_q"], out[f"gfsk{k}_bit"], out[f"gfsk{k}_sig"] = i, q, b, s
+    out["gfsk_n"] = len(lens)
+    vals = np.array([-32768, -32767, -1, 0, 1, 32767], dtype=np.int16)
+    sym = de_bruijn_pairs(36)
+    sym = np.array(sym + sym[:1])
+    i, q = vals[sym // 6], vals[sym % 6]
+    b, s = bl.gfsk_demodulation_fixed_point(i, q)
+    assert s.max() == 2147450880 and s.min() == -2147450880
+    out["gfsk_db_i"], out["gfsk_db_q"], out["gfsk_db_bit"], out["gfsk_db_sig"] = i, q, b, s
+    # crc24_core / crc24: bit counts around one register length and past the 40 bits crc24 skips
+    inits = [np.zeros(24, np.int8), np.ones(24, np.int8), np.array([1, 0] * 12, np.int8), rng.integers(0, 2, 24).astype(np.int8)]
+    k = 0
+    for n in (0, 1, 23, 24, 25, 400, 2000):
+        bits = rng.integers(0, 2, n).astype(np.int8)
+        for init in inits:
+            out[f"crc{k}_bits"], out[f"crc{k}_init"] = bits, init
+            out[f"crc{k}_core"] = bl.crc24_core(bits, init.copy())
+            out[f"crc{k}_full"] = bl.crc24(bits, init.copy())
+            k += 1
+    out["crc_n"] = k
+    # scramble_core / scramble: every 6-bit channel and integers outside 0..63, lengths across the 127-bit period
+    bits = rng.integers(0, 2, 1000).astype(np.int8)
+    chans = list(range(64)) + [64, 100, -1, -64]
+    scr_len = (1, 7, 127, 128, 254, 1000)
+    out["scr_bits"], out["scr_ch"], out["scr_len"] = bits, np.array(chans, np.int32), np.array(scr_len, np.int32)
+    out["scr_core"] = np.array([np.concatenate([bl.scramble_core(bits[:n], ch) for n in scr_len]) for ch in chans], np.int8)
+    out["scr_full"] = np.array([bl.scramble(bits, ch) for ch in chans], np.int8)
+    # search_unique_bit_sequence
+    seqs = []
+    base = rng.integers(0, 2, 300).astype(np.int8)
+    seqs.append((base, base[:32].copy()))                            # match at 0
+    b = base.copy(); s = rng.integers(0, 2, 40).astype(np.int8); b[-40:] = s
+    seqs.append((b, s))                                              # match at n - m
+    b = base.copy(); s = rng.integers(0, 2, 24).astype(np.int8)
+    for p in (50, 120, 200):
+        b[p:p + 24] = s
+    seqs.append((b, s))                                              # several matches: the first wins
+    seqs.append((base, base.copy()))                                 # m == n
+    s = base.copy(); s[-1] ^= 1
+    seqs.append((base, s))                                           # m == n, last bit differs
+    seqs.append((base, np.concatenate([base, [0]]).astype(np.int8)))  # m == n + 1
+    b = np.zeros(300, np.int8); b[173] = 1
+    seqs.append((b, np.ones(1, np.int8)))                            # m == 1
+    seqs.append((np.ones(300, np.int8), np.zeros(1, np.int8)))       # m == 1, never
+    seqs.append((base, np.zeros(0, np.int8)))                        # m == 0
+    seqs.append((np.zeros(0, np.int8), np.zeros(0, np.int8)))        # m == n == 0
+    seqs.append((np.zeros(0, np.int8), np.ones(1, np.int8)))         # n == 0, m == 1
+    long_bits = rng.integers(0, 2, 6000).astype(np.int8)
+    seqs.append((long_bits, long_bits[1904:].copy()))                # m 4096 at n - m
+    seqs.append((long_bits, long_bits[1000:].copy()))                # m 5000 at n - m
+    s = long_bits[700:5700].copy(); s[4321] ^= 1
+    seqs.append((long_bits, s))                                      # m 5000, one bit off
+    seqs.append((long_bits[:4999], long_bits[:5000].copy()))         # m 5000 > n
+    for k, (b, s) in enumerate(seqs):
+        out[f"seq{k}_bit"], out[f"seq{k}_seq"] = b, s
+    out["seq_idx"] = np.array([bl.search_unique_bit_sequence(b, s) for b, s in seqs], np.int64)
+    out["seq_n"] = len(seqs)
+    # a match in the last position of a 2^20-bit input, kept as (seed, n, m, position, result)
+    meta = np.array([777, 1 << 20, 48, (1 << 20) - 48, 0], np.int64)
+    b, s = big_search_input(meta)
+    meta[4] = bl.search_unique_bit_sequence(b, s)
+    out["seq_big"] = meta
+    out["seeded_probe"] = 4242
+    out["seeded_probe_bits"] = seeded_bits(4242, 4096)
+    print({k: v for k, v in zip(range(len(seqs)), out["seq_idx"].tolist())}, "big", meta.tolist())
+    save_npz_stable(os.path.join(ROOT, "tests", "golden", "btlelib_leaves.npz"), out)
+
+
 def main():
     td = tempfile.mkdtemp()
     shutil.copytree(os.path.join(REF, "python"), os.path.join(td, "python"))
@@ -158,6 +274,9 @@ def main():
         return
     if "--sps" in sys.argv:
         sps_cases(bl)
+        return
+    if "--leaves" in sys.argv:
+        leaves_cases(bl)
         return
     out = {}
     cases = [

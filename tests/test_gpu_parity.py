@@ -233,8 +233,8 @@ def test_leaf_demod_scramble_crc(rx):
         assert (rx.scramble_byte(data[:2], ch, 0) == (data[:2] ^ st[ch, :2])).all()
     for n in (0, 1, 2, 39, 300):
         data = rng.integers(0, 256, n, dtype=np.uint8)
-        init = int(rng.integers(0, 2**24))
-        assert rx.crc24_byte(data, init) == L.orc_crc24(data.ctypes.data, n, init)
+        for init in (int(rng.integers(0, 2**24)), int(rng.integers(0, 2**32, dtype=np.uint64))):   # bits 24..31 count too
+            assert rx.crc24_byte(data, init) == L.orc_crc24(data.ctypes.data, n, init)
     assert rx.crc24_byte(np.frombuffer(bytes.fromhex("0100"), np.uint8), rx.crc_init_reorder(0x123456)) == 0x50899B
 
 
