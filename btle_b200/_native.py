@@ -60,7 +60,9 @@ EXPORTS = [
     "btle_b200_streams_finish", "btle_b200_streams_close", "btle_b200_parse_adv_pdu_payload_byte", "btle_b200_parse_ll_pdu_payload_byte",
     "btle_b200_receiver_controller", "btle_b200_receiver_status", "btle_b200_note_packet", "btle_b200_set_hop_hooks", "btle_b200_hop_reset",
     "btle_b200_get_freq_by_channel_number", "btle_b200_chm_is_full_map", "btle_b200_discover", "btle_b200_discover_device",
+    "btle_b200_rx_multi", "btle_b200_rx_multi_units", "btle_b200_rx_multi_device_dir",
 ]
+MAX_CFGS_PER_CAPTURE = 8       # BTLE_MAX_CFGS_PER_CAPTURE
 
 
 class BtleError(RuntimeError):
@@ -143,6 +145,10 @@ def load():
     L.btle_b200_streams_close.restype = None
     L.btle_b200_discover.argtypes = [vp, vp, sz, sz, sz, vp, vp, sz, ctypes.POINTER(sz)]
     L.btle_b200_discover_device.argtypes = [vp, vp, sz, sz, sz, vp, vp, sz, vp, vp]
+    L.btle_b200_rx_multi.argtypes = [vp, vp, sz, sz, sz, vp, vp, sz, vp, sz, ctypes.POINTER(sz)]
+    L.btle_b200_rx_multi_units.argtypes = [vp, sz, vp, sz, sz]
+    L.btle_b200_rx_multi_units.restype = sz
+    L.btle_b200_rx_multi_device_dir.argtypes = [vp, vp, sz, sz, sz, vp, vp, sz, vp, sz, vp, vp, sz, vp]
     _lib = L
     return L
 

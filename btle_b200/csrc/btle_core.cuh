@@ -373,6 +373,46 @@ BTLE_HD uint32_t prefilter_any(const uint32_t lo[4], const uint32_t hi[4], const
          prefilter(lo[3], hi[3], sp);
 }
 
+// ---- several access addresses on one capture (btle_b200_rx_multi) ------------------------------------------------------
+// The dense pass of a capture read by up to kMaxCfgsPerCapture cfgs keeps, per cfg, only what its prefilter reads: the 12
+// tap positions and their expected bits, 16 bytes instead of a whole StreamParams.  The candidate word of a group is the
+// OR of the cfgs' candidate words, so it stays a superset of every cfg's exact matches; the resolver re-checks each
+// candidate exactly against each cfg's own access address and mask.
+constexpr int kMaxCfgsPerCapture = 8;      // BTLE_MAX_CFGS_PER_CAPTURE
+struct TapSet {
+  uint32_t pos[3];                         // byte t (t = 0..11) = tap_pos[t]
+  uint32_t flags;                          // bit t: tap t expects a 0 (tap_xor[t] == ~0); kTapsAll: every window passes (mask 0)
+};
+constexpr uint32_t kTapsAll = 1u << 16;
+BTLE_HD TapSet make_tapset(const StreamParams &sp) {
+  TapSet ts;
+  ts.pos[0] = ts.pos[1] = ts.pos[2] = 0u;
+  ts.flags = sp.ntaps == 0 ? kTapsAll : 0u;
+  for (int t = 0; t < kMaxTaps; ++t) {
+    ts.pos[t >> 2] |= (sp.tap_pos[t] & 31u) << (8 * (t & 3));
+    if (sp.tap_xor[t]) ts.flags |= 1u << t;
+  }
+  return ts;
+}
+// == prefilter_any() of the StreamParams the TapSet was made from (typed taps are a special case of the per-tap XOR)
+BTLE_HD uint32_t prefilter_tapset(const uint32_t lo[4], const uint32_t hi[4], const TapSet &ts) {
+  if (ts.flags & kTapsAll) return 0xFFFFFFFFu;
+  uint32_t m[4] = {0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};
+#pragma unroll
+  for (int t = 0; t < kMaxTaps; ++t) {
+    const uint32_t s = ts.pos[t >> 2] >> (8 * (t & 3)), x = 0u - ((ts.flags >> t) & 1u);
+#pragma unroll
+    for (int ph = 0; ph < 4; ++ph) m[ph] &= funnel_r(lo[ph], hi[ph], s) ^ x;   // funnel shifts read bits 0..4 of s
+  }
+  return m[0] | m[1] | m[2] | m[3];
+}
+// candidate word of a group for n cfgs: bit i set iff the window at symbol i passed at least one cfg's prefilter
+BTLE_HD uint32_t prefilter_union(const uint32_t lo[4], const uint32_t hi[4], const TapSet *ts, int n) {
+  uint32_t a = 0u;
+  for (int j = 0; j < n; ++j) a |= prefilter_tapset(lo, hi, ts[j]);
+  return a;
+}
+
 // 32 consecutive bits of phase stream `ph` starting at symbol s0 (may be negative or run past the
 // window: missing words read as 0).  pd points at the chunk's first group, 4 words per group.
 BTLE_HD uint32_t win32(const uint32_t *pd, int ph, int s0, int ngroups) {

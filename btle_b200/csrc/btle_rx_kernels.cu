@@ -28,6 +28,7 @@
 #include <new>
 #include <string>
 #include <thread>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/btle_b200.h"
@@ -105,11 +106,19 @@ constexpr int kSpanGroups = kGroupsPerChunk * kSpanChunks + kHaloGroups;   // 10
 constexpr int kStageBytes = 8192;              // one warp tile (32 groups = 4096 samples), one TMA box
 constexpr int kHaloRows = kHaloGroups;         // rows of the last (look-ahead) tile of a span: always 12
 
+// The cfgs of the capture a slot's unit reads, when several may read one capture (btle_b200_rx_multi): their prefilter
+// taps for the dense warps; each resolver pass loads one cfg's full StreamParams (Smem::rsp).
+struct MultiCfg {
+  TapSet taps[kMaxCfgsPerCapture];
+  int cfg0, ncfg, pad[2];                      // cfgs cfg0 .. cfg0 + ncfg - 1
+};
+// KC = most cfgs per capture the kernel instantiation decodes: 1 (btle_b200_rx_batch and friends) or kMaxCfgsPerCapture
+template <int KC>
 struct Slot {
   uint4 pd[kSpanGroups + 1];                   // phase words (+1 zero group behind the data)
-  uint32_t cand[kSpanGroups + 4];              // candidate word per group (prefilter, any phase)
+  uint32_t cand[kSpanGroups + 4];              // candidate word per group (prefilter, any phase, any cfg)
   uint32_t flagw[2 * kSpanChunks + 2];         // bit l of word t: group 32t+l has candidates
-  StreamParams sp;
+  std::conditional_t<KC == 1, StreamParams, MultiCfg> sp;
 };
 
 // Hits the chain pass keeps per chunk (68 x u16): every counted packet fits.  With report_rejected a chunk may have up to
@@ -123,8 +132,9 @@ struct ResolveScratch {                        // per resolver warp, between the
   uint16_t xh[2 * kSpanChunks][kExactCap + 1]; // exact access-address hits per flag word (offsets inside the word); [kExactCap] = count
 };
 
-struct Smem {
-  Slot slot[kSlots];
+template <int KC>
+struct SmemBase {
+  Slot<KC> slot[kSlots];
   uint32_t crc4[1024];
   ResolveScratch rs[kResolveWarps];
   alignas(1024) unsigned char stage[kDenseWarps][kStageBytes];
@@ -132,8 +142,14 @@ struct Smem {
   unsigned long long full[kSlots];                        // kDenseWarps arrivals: span published
   unsigned long long empty[kSlots];                       // 1 arrival: span consumed
 };
+template <int KC> struct Smem : SmemBase<KC> {};
+template <> struct Smem<kMaxCfgsPerCapture> : SmemBase<kMaxCfgsPerCapture> {
+  StreamParams rsp[kResolveWarps];                        // the cfg a resolver warp is decoding
+};
 
-static_assert(sizeof(Smem) <= (kCtasPerSm == 1 ? 232448 : 116224 - 1024), "Smem exceeds what a CTA can have on sm_90");
+static_assert(sizeof(Smem<1>) <= (kCtasPerSm == 1 ? 232448 : 116224 - 1024), "Smem exceeds what a CTA can have on sm_90");
+static_assert(sizeof(Smem<kMaxCfgsPerCapture>) <= (kCtasPerSm == 1 ? 232448 : 116224 - 1024), "Smem exceeds what a CTA can have on sm_90");
+static_assert(kMaxCfgsPerCapture == BTLE_MAX_CFGS_PER_CAPTURE && kMaxCfgsPerCapture <= 32, "one lane per cfg loads the taps");
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(unsigned long long *bar, int count) {
@@ -228,6 +244,13 @@ __device__ __forceinline__ void load_params_warp(const StreamParams *__restrict_
   d[lane] = a;
   if (lane + 32 < kParamWords) d[lane + 32] = b;
 }
+// The cfgs of capture group `vs` (vmap[vs] = {capture, first cfg, number of cfgs}) into a slot: lane j builds cfg j's taps.
+__device__ __forceinline__ void load_multi_warp(const StreamParams *__restrict__ params, const int4 *__restrict__ vmap, int vs,
+                                                MultiCfg &dst, int lane) {
+  const int4 v = __ldg(vmap + vs);
+  if (lane < v.z) dst.taps[lane] = make_tapset(params[v.y + lane]);
+  if (lane == 0) { dst.cfg0 = v.y; dst.ncfg = v.z; }
+}
 
 // One persistent CTA per SM.  Units of work (a span of 16 chunks of one capture, or a 4-chunk piece of one in the
 // last wave — Plan, btle_core.cuh) are dealt round-robin to CTAs.
@@ -242,16 +265,27 @@ __device__ __forceinline__ void load_params_warp(const StreamParams *__restrict_
 //      final position — records of a unit are contiguous and in the reference's order.
 // Producers and consumers are decoupled through a 4-slot ring with full/empty mbarriers, so the sparse
 // passes of unit k overlap the dense pass of units k+1 .. k+3.
+// KC > 1 (btle_b200_rx_multi): the plan's streams are capture GROUPS, vmap[g] = {capture, first cfg, number of cfgs}.  A
+// capture's IQ still becomes phase words once; the candidate words are the union of its cfgs' prefilters, and the resolver
+// runs steps 1a-4 once per cfg, each run with its own directory entry: cfg j's units sit at j * (units per group) + the
+// unit's index inside its group, so the directory walks in (cfg, chunk, n0) order.  Records carry stream = cfg index.
+template <int KC>
 __global__ void __launch_bounds__(kThreads, kCtasPerSm)
 btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __grid_constant__ CUtensorMap map12,
                           const int8_t *__restrict__ iq, long long stream_stride, long long n_int8,
                           const StreamParams *__restrict__ params, const Plan plan,
                           btle_pkt_rec *__restrict__ out, unsigned cap, unsigned *__restrict__ count,
-                          uint2 *__restrict__ dir, unsigned *__restrict__ zero_next, long long lead) {
+                          uint2 *__restrict__ dir, unsigned *__restrict__ zero_next, long long lead,
+                          const int4 *__restrict__ vmap) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  Smem &M = *reinterpret_cast<Smem *>(smem_raw);
+  Smem<KC> &M = *reinterpret_cast<Smem<KC> *>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int total_units = plan.total_units;
+  // capture that group `vs` reads
+  auto capture_of = [&](int vs) -> int {
+    if constexpr (KC == 1) return vs;
+    else return __ldg(&vmap[vs].x);
+  };
 
   BTLE_STAMP_MIN(0);
   // context-owned allocation counters rotate through a ring: this launch clears the one a launch half a ring later will use
@@ -283,7 +317,7 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
     c.valid = c.unit < total_units;
     if (c.valid) {
       const UnitInfo ui = unit_info(c.unit, plan);
-      c.tiles = ui.tiles; c.groups = ui.groups; c.chunk0 = ui.chunk0; c.stream = ui.stream;
+      c.tiles = ui.tiles; c.groups = ui.groups; c.chunk0 = ui.chunk0; c.stream = capture_of(ui.stream);
       c.t = warp - c.rot;
       if (c.t < 0) c.t += kDenseWarps;
     }
@@ -325,7 +359,7 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
   uint32_t pw0 = 0, pw1 = 0;
   const int first_unit = blockIdx.x + warp * gridDim.x;
   const bool has_params = warp < kSlots && first_unit < total_units;
-  if (has_params) {
+  if (KC == 1 && has_params) {
     const uint32_t *src = reinterpret_cast<const uint32_t *>(params + unit_info(first_unit, plan).stream);
     pw0 = __ldg(src + lane);
     if (lane + 32 < kParamWords) pw1 = __ldg(src + lane + 32);
@@ -347,9 +381,13 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
   }
   if (tid < kSlots) { mbar_init(&M.full[tid], kDenseWarps); mbar_init(&M.empty[tid], 1); }
   if (has_params) {
-    uint32_t *d = reinterpret_cast<uint32_t *>(&M.slot[warp].sp);
-    d[lane] = pw0;
-    if (lane + 32 < kParamWords) d[lane + 32] = pw1;
+    if constexpr (KC == 1) {
+      uint32_t *d = reinterpret_cast<uint32_t *>(&M.slot[warp].sp);
+      d[lane] = pw0;
+      if (lane + 32 < kParamWords) d[lane + 32] = pw1;
+    } else {
+      load_multi_warp(params, vmap, unit_info(first_unit, plan).stream, M.slot[warp].sp, lane);
+    }
     BTLE_STAMP(11);
   }
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -364,13 +402,13 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
     w_all.begin();
     for (int unit = blockIdx.x; unit < total_units; unit += gridDim.x, ++k) {
       const int b = k % kSlots;
-      Slot &S = M.slot[b];
+      auto &S = M.slot[b];
       const uint32_t use = (uint32_t)(k / kSlots);
       w_empty.begin();
       if (use > 0) mbar_wait_backoff(&M.empty[b], (use - 1) & 1u);   // resolver released the slot's previous unit
       w_empty.end();
       const UnitInfo si = unit_info(unit, plan);
-      const int8_t *cap_base = iq + (long long)si.stream * stream_stride;
+      const int8_t *cap_base = iq + (long long)capture_of(si.stream) * stream_stride;
       int t = warp - rot;
       if (t < 0) t += kDenseWarps;
       for (; t < si.tiles; t += kDenseWarps) {
@@ -473,7 +511,10 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
 #pragma unroll
         for (int ph = 0; ph < 4; ++ph) hi[ph] = __shfl_down_sync(0xFFFFFFFFu, acc[ph], 1);
         uint32_t a = 0u;
-        if (t < 2 * si.nch && lane < 31) a = prefilter_any(acc, hi, S.sp);
+        if (t < 2 * si.nch && lane < 31) {
+          if constexpr (KC == 1) a = prefilter_any(acc, hi, S.sp);
+          else a = prefilter_union(acc, hi, S.sp.taps, S.sp.ncfg);
+        }
         const uint32_t fw = __ballot_sync(0xFFFFFFFFu, a != 0u);
         if (lane < rows) S.cand[t * 32 + lane] = a;
         if (lane == 0) {
@@ -509,114 +550,140 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
     WaitClock w_full;
     for (int unit = blockIdx.x + k * gridDim.x; unit < total_units; unit += kResolveWarps * gridDim.x, k += kResolveWarps) {
       const int b = k % kSlots;
-      Slot &S = M.slot[b];
+      auto &S = M.slot[b];
       w_full.begin();
       mbar_wait_backoff(&M.full[b], (uint32_t)(k / kSlots) & 1u);   // all tiles of the unit are published
       w_full.end();
       BTLE_STAMP(4);
       const UnitInfo si = unit_info(unit, plan);
-      const int8_t *cap_base = iq + (long long)si.stream * stream_stride;
+      const int8_t *cap_base = iq + (long long)capture_of(si.stream) * stream_stride;
       for (int t = lane; t < 2 * si.nch; t += 32) {       // lane 31 of every full tile
         const int g = 32 * t + 31;
         const uint4 lo = S.pd[g], hi = S.pd[g + 1];
         const uint32_t l4[4] = {lo.x, lo.y, lo.z, lo.w}, h4[4] = {hi.x, hi.y, hi.z, hi.w};
-        const uint32_t a = prefilter_any(l4, h4, S.sp);
+        uint32_t a;
+        if constexpr (KC == 1) a = prefilter_any(l4, h4, S.sp);
+        else a = prefilter_union(l4, h4, S.sp.taps, S.sp.ncfg);
         S.cand[g] = a;
         if (a) S.flagw[t] |= 0x80000000u;
       }
       __syncwarp();
       BTLE_STAMP(6);
-      // 1a. exact access-address hits of the unit, all lanes (lane = flag word = 32 groups): the only data-dependent search
-      for (int t = lane; t < 2 * si.nch; t += 32)
-        RS.xh[t][kExactCap] = (uint16_t)enumerate_exact_hits(reinterpret_cast<const uint32_t *>(S.pd), S.cand, S.flagw[t], t, S.sp, RS.xh[t]);
-      __syncwarp();
-      // 1b. chain pass: which hits does the reference count?  (lane = chunk; walks the chunk's two hit lists)
-      int mine = 0;
-      if (lane < si.nch) {
-        struct Note {
-          uint16_t *row;
-          __device__ __forceinline__ void operator()(int i, int n0, bool rej) {
-            if (i < kHitCap) row[i] = (uint16_t)((n0 + 124) | (rej ? 0x8000 : 0));
-          }
-        } note{RS.hit[lane]};
-        const uint32_t *pdc = reinterpret_cast<const uint32_t *>(&S.pd[kGroupsPerChunk * lane]);
-        const int c0 = RS.xh[2 * lane][kExactCap], c1 = RS.xh[2 * lane + 1][kExactCap];
-        if (c0 > kExactCap || c1 > kExactCap)              // degenerate mask: too many matches to list, walk the candidates instead
-          mine = chain_chunk(pdc, &S.cand[kGroupsPerChunk * lane], &S.flagw[2 * lane], S.sp, note);
-        else
-          mine = chain_chunk_lists(pdc, RS.xh[2 * lane], c0, RS.xh[2 * lane + 1], c1, S.sp, note);
+      // steps 1a-4 once per cfg of the unit's capture (KC == 1: once, with the slot's parameters)
+      int ncfg = 1, cfg0 = 0, per_group = 0, local = 0;
+      if constexpr (KC > 1) {
+        ncfg = S.sp.ncfg;
+        cfg0 = S.sp.cfg0;
+        per_group = plan.big_units ? plan.spans_per_stream : plan.spans_per_stream << plan.piece_shift;   // the host plans evenly
+        local = unit - si.stream * per_group;
       }
-      BTLE_STAMP(7);
-      // 2. the unit's block of the output: exclusive scan of the per-chunk counts, one atomic for the unit
-      int incl = mine;
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) { const int v = __shfl_up_sync(0xFFFFFFFFu, incl, d); if (lane >= d) incl += v; }
-      const int total = __shfl_sync(0xFFFFFFFFu, incl, 31);
-      if (lane <= kSpanChunks) RS.pre[lane] = (uint16_t)(incl - mine);   // lanes >= nch hold `total`
-      unsigned my_base = 0;
-      if (lane == 0) {
-        if (total) my_base = atomicAdd(count, (unsigned)total);
-        dir[unit] = make_uint2(my_base, (unsigned)total);
-      }
-      __syncwarp();
-      BTLE_STAMP(8);
-      // 3. decode pass: one lane per packet, all lanes on the same instruction stream.  The reservation's result is
-      //    only needed when the records are stored, so the atomic's round trip to L2 overlaps the decode.
-      for (int j0 = 0; j0 < total; j0 += 32) {
-        const int j = j0 + lane;
-        uint32_t words[11];
-        int nbytes = 0, crc_bad = 0, n0 = 0, c = 0;
-        bool rej = false, live = false;
-        if (j < total) {
-          // chunk of packet j: pre[c] <= j < pre[c + 1]
-#pragma unroll
-          for (int step = kSpanChunks / 2; step >= 1; step >>= 1)
-            if ((int)RS.pre[c + step] <= j) c += step;
-          const int i = j - (int)RS.pre[c];
-          live = i < kHitCap;                               // hits behind the chunk's row are left to step 4
-          if (live) {
-            const int h = (int)RS.hit[c][i];
-            rej = (h & 0x8000) != 0;
-            n0 = (h & 0x7FFF) - 124;
-            decode_packet(reinterpret_cast<const uint32_t *>(&S.pd[kGroupsPerChunk * c]), S.sp, M.crc4, n0, rej, words, nbytes, crc_bad);
-          }
+      for (int jc = 0; jc < ncfg; ++jc) {
+        const StreamParams *spp;
+        if constexpr (KC == 1) spp = &S.sp;
+        else {
+          spp = &M.rsp[warp - kDenseWarps];
+          load_params_warp(params + cfg0 + jc, M.rsp[warp - kDenseWarps], lane);
+          __syncwarp();
         }
-        const unsigned base = __shfl_sync(0xFFFFFFFFu, my_base, 0);
-        if (live && base + (unsigned)j < cap)
-          store_record(out + base + j, si.stream, si.chunk0 + c, n0, nbytes, crc_bad, rej, words, S.sp, cap_base, n_int8, lead);
-      }
-      // 4. only with report_rejected can a chunk have more hits than its row holds (degenerate masks, up to
-      //    BTLE_MAX_RECS_PER_CHUNK): the chunk's lane runs the same chain again and decodes and stores hits kHitCap.. itself
-      if (S.sp.report_rejected) {
-        const unsigned base = __shfl_sync(0xFFFFFFFFu, my_base, 0);
-        if (mine > kHitCap) {
-          struct Late {
-            const uint32_t *pd; const StreamParams &sp; const uint32_t *crc4;
-            btle_pkt_rec *out; unsigned first, cap; int stream, chunk; const int8_t *iq; long long n_int8, lead;
+        const StreamParams &sp = *spp;
+        const int rec_stream = KC == 1 ? si.stream : cfg0 + jc;
+        const int dir_at = KC == 1 ? unit : (cfg0 + jc) * per_group + local;
+        // 1a. exact access-address hits of the unit, all lanes (lane = flag word = 32 groups): the only data-dependent search
+        for (int t = lane; t < 2 * si.nch; t += 32)
+          RS.xh[t][kExactCap] = (uint16_t)enumerate_exact_hits(reinterpret_cast<const uint32_t *>(S.pd), S.cand, S.flagw[t], t, sp, RS.xh[t]);
+        __syncwarp();
+        // 1b. chain pass: which hits does the reference count?  (lane = chunk; walks the chunk's two hit lists)
+        int mine = 0;
+        if (lane < si.nch) {
+          struct Note {
+            uint16_t *row;
             __device__ __forceinline__ void operator()(int i, int n0, bool rej) {
-              if (i < kHitCap || first + (unsigned)i >= cap) return;
-              uint32_t words[11];
-              int nbytes, crc_bad;
-              decode_packet(pd, sp, crc4, n0, rej, words, nbytes, crc_bad);
-              store_record(out + first + i, stream, chunk, n0, nbytes, crc_bad, rej, words, sp, iq, n_int8, lead);
+              if (i < kHitCap) row[i] = (uint16_t)((n0 + 124) | (rej ? 0x8000 : 0));
             }
-          };
+          } note{RS.hit[lane]};
           const uint32_t *pdc = reinterpret_cast<const uint32_t *>(&S.pd[kGroupsPerChunk * lane]);
-          Late late{pdc, S.sp, M.crc4, out, base + RS.pre[lane], cap, si.stream, si.chunk0 + lane, cap_base, n_int8, lead};
           const int c0 = RS.xh[2 * lane][kExactCap], c1 = RS.xh[2 * lane + 1][kExactCap];
-          if (c0 > kExactCap || c1 > kExactCap)
-            chain_chunk(pdc, &S.cand[kGroupsPerChunk * lane], &S.flagw[2 * lane], S.sp, late);
+          if (c0 > kExactCap || c1 > kExactCap)              // degenerate mask: too many matches to list, walk the candidates instead
+            mine = chain_chunk(pdc, &S.cand[kGroupsPerChunk * lane], &S.flagw[2 * lane], sp, note);
           else
-            chain_chunk_lists(pdc, RS.xh[2 * lane], c0, RS.xh[2 * lane + 1], c1, S.sp, late);
+            mine = chain_chunk_lists(pdc, RS.xh[2 * lane], c0, RS.xh[2 * lane + 1], c1, sp, note);
         }
+        BTLE_STAMP(7);
+        // 2. the unit's block of the output: exclusive scan of the per-chunk counts, one atomic for the unit
+        int incl = mine;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) { const int v = __shfl_up_sync(0xFFFFFFFFu, incl, d); if (lane >= d) incl += v; }
+        const int total = __shfl_sync(0xFFFFFFFFu, incl, 31);
+        if (lane <= kSpanChunks) RS.pre[lane] = (uint16_t)(incl - mine);   // lanes >= nch hold `total`
+        unsigned my_base = 0;
+        if (lane == 0) {
+          if (total) my_base = atomicAdd(count, (unsigned)total);
+          dir[dir_at] = make_uint2(my_base, (unsigned)total);
+        }
+        __syncwarp();
+        BTLE_STAMP(8);
+        // 3. decode pass: one lane per packet, all lanes on the same instruction stream.  The reservation's result is
+        //    only needed when the records are stored, so the atomic's round trip to L2 overlaps the decode.
+        for (int j0 = 0; j0 < total; j0 += 32) {
+          const int j = j0 + lane;
+          uint32_t words[11];
+          int nbytes = 0, crc_bad = 0, n0 = 0, c = 0;
+          bool rej = false, live = false;
+          if (j < total) {
+            // chunk of packet j: pre[c] <= j < pre[c + 1]
+#pragma unroll
+            for (int step = kSpanChunks / 2; step >= 1; step >>= 1)
+              if ((int)RS.pre[c + step] <= j) c += step;
+            const int i = j - (int)RS.pre[c];
+            live = i < kHitCap;                               // hits behind the chunk's row are left to step 4
+            if (live) {
+              const int h = (int)RS.hit[c][i];
+              rej = (h & 0x8000) != 0;
+              n0 = (h & 0x7FFF) - 124;
+              decode_packet(reinterpret_cast<const uint32_t *>(&S.pd[kGroupsPerChunk * c]), sp, M.crc4, n0, rej, words, nbytes, crc_bad);
+            }
+          }
+          const unsigned base = __shfl_sync(0xFFFFFFFFu, my_base, 0);
+          if (live && base + (unsigned)j < cap)
+            store_record(out + base + j, rec_stream, si.chunk0 + c, n0, nbytes, crc_bad, rej, words, sp, cap_base, n_int8, lead);
+        }
+        // 4. only with report_rejected can a chunk have more hits than its row holds (degenerate masks, up to
+        //    BTLE_MAX_RECS_PER_CHUNK): the chunk's lane runs the same chain again and decodes and stores hits kHitCap.. itself
+        if (sp.report_rejected) {
+          const unsigned base = __shfl_sync(0xFFFFFFFFu, my_base, 0);
+          if (mine > kHitCap) {
+            struct Late {
+              const uint32_t *pd; const StreamParams &sp; const uint32_t *crc4;
+              btle_pkt_rec *out; unsigned first, cap; int stream, chunk; const int8_t *iq; long long n_int8, lead;
+              __device__ __forceinline__ void operator()(int i, int n0, bool rej) {
+                if (i < kHitCap || first + (unsigned)i >= cap) return;
+                uint32_t words[11];
+                int nbytes, crc_bad;
+                decode_packet(pd, sp, crc4, n0, rej, words, nbytes, crc_bad);
+                store_record(out + first + i, stream, chunk, n0, nbytes, crc_bad, rej, words, sp, iq, n_int8, lead);
+              }
+            };
+            const uint32_t *pdc = reinterpret_cast<const uint32_t *>(&S.pd[kGroupsPerChunk * lane]);
+            Late late{pdc, sp, M.crc4, out, base + RS.pre[lane], cap, rec_stream, si.chunk0 + lane, cap_base, n_int8, lead};
+            const int c0 = RS.xh[2 * lane][kExactCap], c1 = RS.xh[2 * lane + 1][kExactCap];
+            if (c0 > kExactCap || c1 > kExactCap)
+              chain_chunk(pdc, &S.cand[kGroupsPerChunk * lane], &S.flagw[2 * lane], sp, late);
+            else
+              chain_chunk_lists(pdc, RS.xh[2 * lane], c0, RS.xh[2 * lane + 1], c1, sp, late);
+          }
+        }
+        BTLE_STAMP(9);
+        __syncwarp();                                       // (KC > 1: the next cfg's run reuses RS and rsp)
       }
-      BTLE_STAMP(9);
-      __syncwarp();
       // the slot is reused by unit k + kSlots of this CTA: refresh its parameters if the stream changes
       const int next = unit + kSlots * gridDim.x;
       if (next < total_units) {
         const int ns = unit_info(next, plan).stream;
-        if (ns != si.stream) load_params_warp(params + ns, S.sp, lane);
+        if constexpr (KC == 1) {
+          if (ns != si.stream) load_params_warp(params + ns, S.sp, lane);
+        } else {
+          if (ns != si.stream) load_multi_warp(params, vmap, ns, S.sp, lane);
+        }
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&M.empty[b]);            // release the slot to the producers
@@ -1470,6 +1537,13 @@ struct CfgSlot {                     // one uploaded btle_stream_cfg array + the
   Buf<StreamParams> d_params;
   HostBuf<btle_stream_cfg> h; HostBuf<StreamParams> h_params;   // page-locked sources of the upload
   size_t n = 0;                      // entries of the cached array (0: empty)
+  // btle_b200_rx_multi: the cfgs' capture indices are part of the key, and the capture groups derived from them
+  // ({capture, first cfg, number of cfgs} per capture read) are uploaded with the parameters
+  bool multi = false;
+  std::vector<int32_t> cfg_capture;
+  Buf<int4> d_vmap;
+  HostBuf<int4> h_vmap;
+  size_t n_vmap = 0;
   unsigned long long up_stream = 0;  // stream the upload was enqueued on
   cudaEvent_t uploaded = nullptr;    // recorded behind the upload's two copies
   StreamUse use[kSlotUsers];         // last launch of each stream that read this upload
@@ -1581,10 +1655,13 @@ int stream_id(btle_b200_ctx *ctx, cudaStream_t st, unsigned long long *sid) {
 // A launch never waits for another stream's kernel: two pipes that alternate over the same arrays still overlap.
 // The copies come from page-locked staging, so enqueueing them never blocks the host behind a busy stream; the host
 // waits only when it must rewrite a staging buffer whose previous copy has not run yet.
-int upload_cfgs(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size_t n, cudaStream_t st, unsigned long long sid, CfgSlot **slot_out) {
+// cfg_capture (btle_b200_rx_multi, else nullptr): cfg i decodes capture cfg_capture[i]; already validated.
+int upload_cfgs(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size_t n, cudaStream_t st, unsigned long long sid, CfgSlot **slot_out,
+                const int32_t *cfg_capture = nullptr) {
   CfgSlot *pick = nullptr;
   for (CfgSlot &c : ctx->cfg_slot)
-    if (c.n == n && !memcmp(c.h, cfgs, n * sizeof(btle_stream_cfg))) { pick = &c; break; }
+    if (c.n == n && c.multi == (cfg_capture != nullptr) && !memcmp(c.h, cfgs, n * sizeof(btle_stream_cfg)) &&
+        (!cfg_capture || !memcmp(c.cfg_capture.data(), cfg_capture, n * sizeof(int32_t)))) { pick = &c; break; }
   if (pick) {
     bool seen = pick->up_stream == sid;
     for (const StreamUse &u : pick->use) seen |= u.stamp && u.stream == sid;
@@ -1604,6 +1681,8 @@ int upload_cfgs(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size_t n, cudaS
     pick->n = 0;
     if (pick->d.reserve(ctx, n) || pick->d_params.reserve(ctx, n) || pick->h.reserve(ctx, n) || pick->h_params.reserve(ctx, n))
       return BTLE_ENOMEM;
+    // (h_vmap grows in step with h: when it is kept, so is h, and the wait above covered its previous copy)
+    if (cfg_capture && (pick->d_vmap.reserve(ctx, n) || pick->h_vmap.reserve(ctx, n))) return BTLE_ENOMEM;
     for (StreamUse &u : pick->use) u.stamp = 0;              // ordered before the new copies by the waits above
     memcpy(pick->h, cfgs, n * sizeof(btle_stream_cfg));
     for (size_t i = 0; i < n; ++i) {                         // make_params(): btle_params.h, the same code the CPU emulator runs
@@ -1615,6 +1694,16 @@ int upload_cfgs(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size_t n, cudaS
     }
     BTLE_CUDA(ctx, cudaMemcpyAsync(pick->d, pick->h, n * sizeof(btle_stream_cfg), cudaMemcpyHostToDevice, st));
     BTLE_CUDA(ctx, cudaMemcpyAsync(pick->d_params, pick->h_params, n * sizeof(StreamParams), cudaMemcpyHostToDevice, st));
+    pick->multi = cfg_capture != nullptr;
+    pick->n_vmap = 0;
+    if (cfg_capture) {
+      pick->cfg_capture.assign(cfg_capture, cfg_capture + n);
+      for (size_t i = 0; i < n; ++i) {
+        if (!i || cfg_capture[i] != cfg_capture[i - 1]) pick->h_vmap[pick->n_vmap++] = make_int4(cfg_capture[i], (int)i, 0, 0);
+        ++pick->h_vmap[pick->n_vmap - 1].z;
+      }
+      BTLE_CUDA(ctx, cudaMemcpyAsync(pick->d_vmap, pick->h_vmap, pick->n_vmap * sizeof(int4), cudaMemcpyHostToDevice, st));
+    }
     BTLE_CUDA(ctx, cudaEventRecord(pick->uploaded, st));
     pick->up_stream = sid;
     pick->n = n;
@@ -1678,23 +1767,51 @@ Plan plan_for(const btle_b200_ctx *ctx, size_t n_streams, size_t n_int8) {
   return make_plan((long long)n_streams, (long long)(n_int8 / kChunkInt8), ctx->num_sms * kCtasPerSm);
 }
 
-// enqueue the persistent kernel for device-resident inputs
+// Several cfgs per capture (btle_b200_rx_multi): cfg i decodes capture cfg_capture[i] (non-decreasing, in range, at most
+// kMaxCfgsPerCapture per capture; else BTLE_EINVAL).  *groups = number of distinct captures named.
+int check_cfg_capture(btle_b200_ctx *ctx, size_t n_captures, const int32_t *cfg_capture, size_t n_cfgs, size_t *groups) {
+  *groups = 0;
+  if (n_cfgs && !cfg_capture) { ctx->err = "rx_multi: missing cfg_capture"; return BTLE_EINVAL; }
+  size_t run = 0;
+  for (size_t i = 0; i < n_cfgs; ++i) {
+    const int32_t c = cfg_capture[i];
+    if (c < 0 || (size_t)c >= n_captures) { ctx->err = "rx_multi: cfg_capture out of range"; return BTLE_EINVAL; }
+    if (i && c < cfg_capture[i - 1]) { ctx->err = "rx_multi: cfg_capture must be non-decreasing"; return BTLE_EINVAL; }
+    run = (i && c == cfg_capture[i - 1]) ? run + 1 : 1;
+    if (run == 1) ++*groups;
+    if (run > (size_t)kMaxCfgsPerCapture) { ctx->err = "rx_multi: more than BTLE_MAX_CFGS_PER_CAPTURE cfgs on one capture"; return BTLE_EINVAL; }
+  }
+  return BTLE_OK;
+}
+// units of one capture group of an rx_multi launch over `groups` captures; every group has the same number
+size_t multi_units_per_group(const btle_b200_ctx *ctx, size_t groups, size_t n_int8) {
+  if (!groups || n_int8 < (size_t)kChunkInt8) return 0;
+  return (size_t)plan_for(ctx, groups, n_int8).total_units / groups;
+}
+
+// enqueue the persistent kernel for device-resident inputs; cfg_capture != nullptr: several cfgs per capture
+// (n_cfgs of them, checked by check_cfg_capture), the directory in (cfg, chunk) order
 int launch_rx(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8,
               const btle_stream_cfg *cfgs, btle_pkt_rec *d_out, size_t cap, unsigned *d_count, btle_unit_dir *d_dir,
-              cudaStream_t st) {
+              cudaStream_t st, const int32_t *cfg_capture = nullptr, size_t n_cfgs = 0, size_t groups = 0) {
   ctx->last_launches = 0;
   unsigned *zero_next = nullptr;
   if (d_count) BTLE_CUDA(ctx, cudaMemsetAsync(d_count, 0, sizeof(unsigned), st));
   const long long nchunks = (long long)(n_int8 / kChunkInt8);
-  if (nchunks == 0 || n_streams == 0) return BTLE_OK;
+  const bool multi = cfg_capture != nullptr;
+  if (nchunks == 0 || n_streams == 0 || (multi && n_cfgs == 0)) return BTLE_OK;
   unsigned long long sid = 0;
   int rc = stream_id(ctx, st, &sid);
   if (rc) return rc;
   const long long spans = (nchunks + kSpanChunks - 1) / kSpanChunks;
-  if (spans * (long long)n_streams > 0x07FFFFFFll || nchunks > 0x7FFFFFFFll) { ctx->err = "batch too large for one launch"; return BTLE_EINVAL; }
-  const Plan plan = plan_for(ctx, n_streams, n_int8);
+  if (spans * (long long)(multi ? n_cfgs : n_streams) > 0x07FFFFFFll || nchunks > 0x7FFFFFFFll) { ctx->err = "batch too large for one launch"; return BTLE_EINVAL; }
+  const Plan plan = plan_for(ctx, multi ? groups : n_streams, n_int8);
+  if (multi && (plan.tail_units || (plan.big_units && plan.big_units != plan.total_units))) {
+    ctx->err = "rx_multi: this build's unit plan is not the same for every capture";   // (A/B builds with a re-cut last wave)
+    return BTLE_EINVAL;
+  }
   CfgSlot *cs = nullptr;
-  rc = upload_cfgs(ctx, cfgs, n_streams, st, sid, &cs);
+  rc = upload_cfgs(ctx, cfgs, multi ? n_cfgs : n_streams, st, sid, &cs, cfg_capture);
   if (rc) return rc;
   const MapSlot *ms = nullptr;
   rc = get_maps(ctx, d_iq, n_streams, stride, n_int8, &ms);
@@ -1713,9 +1830,16 @@ int launch_rx(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t s
     zero_next = ctx->d_count_ring + (ctx->ring_pos + kCountRing / 2) % kCountRing;
   }
   const unsigned grid = (unsigned)std::min<long long>(plan.total_units, (long long)ctx->num_sms * kCtasPerSm);   // one persistent CTA per SM
-  btle_rx_persistent_kernel<<<grid, kThreads, sizeof(Smem), st>>>(
-      ms->map32, ms->map12, d_iq, (long long)stride, (long long)n_int8, cs->d_params, plan, d_out,
-      (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu), d_count, reinterpret_cast<uint2 *>(d_dir), zero_next, (long long)ctx->lead_bytes);
+  if (multi)
+    btle_rx_persistent_kernel<kMaxCfgsPerCapture><<<grid, kThreads, sizeof(Smem<kMaxCfgsPerCapture>), st>>>(
+        ms->map32, ms->map12, d_iq, (long long)stride, (long long)n_int8, cs->d_params, plan, d_out,
+        (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu), d_count, reinterpret_cast<uint2 *>(d_dir), zero_next, (long long)ctx->lead_bytes,
+        cs->d_vmap);
+  else
+    btle_rx_persistent_kernel<1><<<grid, kThreads, sizeof(Smem<1>), st>>>(
+        ms->map32, ms->map12, d_iq, (long long)stride, (long long)n_int8, cs->d_params, plan, d_out,
+        (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu), d_count, reinterpret_cast<uint2 *>(d_dir), zero_next, (long long)ctx->lead_bytes,
+        nullptr);
   BTLE_CUDA(ctx, cudaGetLastError());
   if (ring) {                                                 // the position is taken only by a launch that was enqueued
     ctx->ring_pos = (ctx->ring_pos + 1) % kCountRing;
@@ -1991,7 +2115,9 @@ int btle_b200_create(btle_b200_ctx **out, int cuda_device) {
   if (cudaMemcpyToSymbol(c_noise_thr, thr, sizeof thr) != cudaSuccess ||
       cudaMemcpyToSymbol(c_whiten_words, ww, sizeof ww) != cudaSuccess ||
       cudaMemcpyToSymbol(c_crc4, crc, sizeof crc) != cudaSuccess ||
-      cudaFuncSetAttribute(btle_rx_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem)) != cudaSuccess ||
+      cudaFuncSetAttribute(btle_rx_persistent_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem<1>)) != cudaSuccess ||
+      cudaFuncSetAttribute(btle_rx_persistent_kernel<kMaxCfgsPerCapture>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (int)sizeof(Smem<kMaxCfgsPerCapture>)) != cudaSuccess ||
       cudaFuncSetAttribute(sps8_hits_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSps8Smem) != cudaSuccess ||
       cudaFuncSetAttribute(discover_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDiscSmem) != cudaSuccess ||
       cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess ||
@@ -2103,6 +2229,72 @@ int btle_b200_rx_iq16(btle_b200_ctx *ctx, const int16_t *iq16, size_t n_int16, i
 int btle_b200_rx(btle_b200_ctx *ctx, const int8_t *iq, size_t n_int8, const btle_stream_cfg *cfg, btle_pkt_rec *out,
                  size_t cap, size_t *n_out) {
   return btle_b200_rx_batch(ctx, iq, 1, n_int8, n_int8, cfg, out, cap, n_out);
+}
+
+// ---- several cfgs per capture -------------------------------------------------------------------------------------
+size_t btle_b200_rx_multi_units(const btle_b200_ctx *ctx, size_t n_captures, const int32_t *cfg_capture, size_t n_cfgs, size_t n_int8) {
+  if (!ctx || !n_cfgs || !cfg_capture) return 0;
+  size_t groups = 0;
+  btle_b200_ctx *c = const_cast<btle_b200_ctx *>(ctx);
+  const std::string keep = c->err;                        // a query: leaves last_error as it was
+  const int rc = check_cfg_capture(c, n_captures, cfg_capture, n_cfgs, &groups);
+  c->err = keep;
+  return rc ? 0 : n_cfgs * multi_units_per_group(ctx, groups, n_int8);
+}
+
+int btle_b200_rx_multi_device_dir(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_captures, size_t stride, size_t n_int8,
+                                  const btle_stream_cfg *cfgs, const int32_t *cfg_capture, size_t n_cfgs, btle_pkt_rec *d_out,
+                                  size_t cap, uint32_t *d_count, btle_unit_dir *d_dir, size_t dir_cap, void *cuda_stream) {
+  if (!ctx) return BTLE_EINVAL;
+  if ((!d_out && cap) || (!cfgs && n_cfgs) || !d_dir) { ctx->err = "rx_multi: missing buffer"; return BTLE_EINVAL; }
+  if ((reinterpret_cast<uintptr_t>(d_iq) & 15) || (n_captures > 1 && (stride & 15))) { ctx->err = "device IQ must be 16-byte aligned"; return BTLE_EINVAL; }
+  if (n_captures > 1 && stride < n_int8) { ctx->err = "stream stride smaller than stream length"; return BTLE_EINVAL; }
+  size_t groups = 0;
+  int rc = check_cfg_capture(ctx, n_captures, cfg_capture, n_cfgs, &groups);
+  if (rc) return rc;
+  if (dir_cap < n_cfgs * multi_units_per_group(ctx, groups, n_int8)) { ctx->err = "unit directory too small (btle_b200_rx_multi_units)"; return BTLE_EINVAL; }
+  rc = validate_cfgs(ctx, cfgs, n_cfgs);
+  if (rc) return rc;
+  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
+  return launch_rx(ctx, d_iq, n_captures, stride, n_int8, cfgs, d_out, cap, d_count, d_dir, reinterpret_cast<cudaStream_t>(cuda_stream),
+                   cfg_capture, n_cfgs, groups);
+}
+
+int btle_b200_rx_multi(btle_b200_ctx *ctx, const int8_t *iq, size_t n_captures, size_t stride, size_t n_int8, const btle_stream_cfg *cfgs,
+                       const int32_t *cfg_capture, size_t n_cfgs, btle_pkt_rec *out, size_t cap, size_t *n_out) {
+  if (!ctx) return BTLE_EINVAL;
+  if (!n_out || (!out && cap) || (!cfgs && n_cfgs) || (!iq && n_captures && n_int8)) { ctx->err = "rx_multi: missing buffer"; return BTLE_EINVAL; }
+  *n_out = 0;
+  if (n_captures > 1 && stride < n_int8) { ctx->err = "stream stride smaller than stream length"; return BTLE_EINVAL; }
+  size_t groups = 0;
+  int rc = check_cfg_capture(ctx, n_captures, cfg_capture, n_cfgs, &groups);
+  if (rc) return rc;
+  rc = validate_cfgs(ctx, cfgs, n_cfgs);
+  if (rc) return rc;
+  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  // only the captures some cfg reads are copied, one after the other; cfg_capture is renumbered to match
+  const size_t pitch = (n_int8 + 15) & ~size_t(15), spitch = n_captures > 1 ? stride : n_int8;
+  rc = ctx->d_iq.reserve(ctx, std::max<size_t>(pitch * groups, 16));
+  if (rc) return rc;
+  std::vector<int32_t> local(n_cfgs), caps;
+  for (size_t i = 0; i < n_cfgs; ++i) {
+    if (!i || cfg_capture[i] != cfg_capture[i - 1]) caps.push_back(cfg_capture[i]);
+    local[i] = (int32_t)caps.size() - 1;
+  }
+  for (size_t g = 0; g < caps.size();) {                   // one copy per run of consecutive captures
+    size_t e = g + 1;
+    while (e < caps.size() && caps[e] == caps[e - 1] + 1) ++e;
+    if (g) BTLE_CUDA(ctx, cudaStreamSynchronize(st));      // a new copy may reuse the page-locked staging of the last one
+    rc = h2d_rows(ctx, ctx->d_iq + g * pitch, pitch, iq + (size_t)caps[g] * spitch, spitch, n_int8, e - g, st);
+    if (rc) return rc;
+    g = e;
+  }
+  const size_t units = n_cfgs * multi_units_per_group(ctx, groups, n_int8);
+  if (ctx->d_out.reserve(ctx, std::max<size_t>(cap, 1)) || ctx->d_dir.reserve(ctx, std::max<size_t>(units, 1))) return BTLE_ENOMEM;
+  rc = launch_rx(ctx, ctx->d_iq, groups, pitch, n_int8, cfgs, ctx->d_out, cap, ctx->d_count, ctx->d_dir, st, local.data(), n_cfgs, groups);
+  if (rc) return rc;
+  return fetch_ordered(ctx, ctx->d_out, ctx->d_dir, units, out, cap, n_out, st);
 }
 
 // ---- streaming sessions: N time-aligned captures of unbounded length, pushed in pieces ----------------------------

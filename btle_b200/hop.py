@@ -265,6 +265,50 @@ def follow_connections(rx, captures: np.ndarray, max_events: int = 10000, discov
     return adv, conns
 
 
+def decode_connections(rx, captures: np.ndarray, discover: bool = True):
+    """Every known connection's data-channel traffic, decoded without following it.  captures: int8 [40, n_int8] as in
+    follow_connections(); `rx` needs rx_batch, rx_multi and, with discover=True, discover (a BtleRx).
+    The connections are the CONNECT_REQ ones (tracked or not) plus, with discover=True, the discover_connections() ones
+    whose access address no CONNECT_REQ announced (tracked or not: a partial channel map or CSA#2 does not matter here).
+    With all 37 data channels captured, a connection's packets are found by its access address and CRC init alone, so
+    each connection gets `traffic`: every record on channels 0..36 decoded with them, in time order (chunk * 8192 + n0,
+    then channel).  Launches: one rx_batch over the advertising captures, one discover, and one rx_multi per
+    MAX_CFGS_PER_CAPTURE connections over captures[0:37] (each capture is read once per call, whatever the number of
+    connections in it).  Returns (adv_records, connections)."""
+    from ._native import MAX_CFGS_PER_CAPTURE
+    captures = np.ascontiguousarray(captures, dtype=np.int8)
+    assert captures.shape[0] == 40
+    adv = rx.rx_batch(captures[37:40], make_cfgs(3, channel=[37, 38, 39])).copy()
+    adv["stream"] += 37
+    conns = []
+    for r in adv:
+        c = parse_connect_req(r)
+        if c is None:
+            continue
+        c["tracked"] = c["chm"] == "1fffffffff" and c["interval"] > 0
+        conns.append(c)
+    if discover:
+        announced = {c["access_addr"] for c in conns}
+        conns += [c for c in discover_connections(rx, captures) if c["access_addr"] not in announced]
+    K = MAX_CFGS_PER_CAPTURE
+    for b0 in range(0, len(conns), K):
+        batch = conns[b0:b0 + K]
+        k = len(batch)
+        # cfg j = channel * k + i: connection i on data channel j // k (the cfgs of one capture are adjacent)
+        cfgs = make_cfgs(37 * k, channel=np.repeat(np.arange(37), k), access_addr=[c["access_addr"] for c in batch] * 37,
+                         crc_init=[c["crc_init"] for c in batch] * 37)
+        rec = rx.rx_multi(captures[0:37], cfgs, np.repeat(np.arange(37, dtype=np.int32), k))
+        owner = rec["stream"] % k
+        t = rec["chunk"].astype(np.int64) * 8192 + rec["n0"]
+        for i, c in enumerate(batch):
+            mine = rec[owner == i]
+            tm = t[owner == i]
+            tr = mine[np.lexsort((mine["channel"], tm))].copy()
+            tr["stream"] = tr["channel"]                 # the capture row, as in follow_connections()
+            c["traffic"] = tr
+    return adv, conns
+
+
 # ---- connections whose CONNECT_REQ was not captured (DESIGN.md §6.2) ----------------------------------------------------
 EVENT_SPAN_S = 3.75e-3   # candidates on one channel within half the shortest interval (7.5 ms) of the first are one event
 DISCOVER_LEAD_S = 1.25e-3   # a discovered connection's walk starts this long before its first empty PDU

@@ -91,6 +91,40 @@ class BtleRx:
         return self._grow_once(partial(self._L.btle_b200_rx_batch, self._h, iq.ctypes.data, ns, n, n, cfgs.ctypes.data), REC_DTYPE,
                                ns * (n // 16384) * 34 + 16 if cap is None else cap, grow=cap is None)
 
+    def rx_multi(self, iq: np.ndarray, cfgs: np.ndarray, capture, cap: int | None = None) -> np.ndarray:
+        """Several cfgs per capture in one read of the IQ (btle_b200_rx_multi): iq int8 [n_captures, n_int8] (or [n_int8]);
+        cfgs CFG_DTYPE [n_cfgs]; capture[j] = the capture cfg j decodes (non-decreasing, at most MAX_CFGS_PER_CAPTURE
+        per capture).  Returns what rx_batch() returns on iq[capture] with cfgs: records with stream = cfg index, in
+        (cfg, chunk, n0) order."""
+        iq = np.ascontiguousarray(iq, dtype=np.int8)
+        if iq.ndim == 1:
+            iq = iq[None, :]
+        ns, n = iq.shape
+        cfgs = np.ascontiguousarray(cfgs, dtype=CFG_DTYPE).reshape(-1)
+        cc = np.ascontiguousarray(capture, dtype=np.int32).reshape(-1)
+        assert cc.shape == cfgs.shape
+        return self._grow_once(partial(self._L.btle_b200_rx_multi, self._h, iq.ctypes.data, ns, n, n, cfgs.ctypes.data, cc.ctypes.data,
+                                       cfgs.size), REC_DTYPE, cfgs.size * (n // 16384) * 34 + 16 if cap is None else cap, grow=cap is None)
+
+    def multi_units(self, n_captures: int, capture, n_int8: int) -> int:
+        """Number of unit-directory entries an rx_multi launch over this shape writes (btle_b200_rx_multi_units)."""
+        cc = np.ascontiguousarray(capture, dtype=np.int32).reshape(-1)
+        return int(self._L.btle_b200_rx_multi_units(self._h, n_captures, cc.ctypes.data, cc.size, n_int8))
+
+    def rx_multi_device_dir(self, d_iq, cfgs: np.ndarray, capture, d_out, d_count, d_dir, stream_ptr: int = 0):
+        """rx_multi on device-resident captures, buffers as rx_device_dir (d_count may be None); d_dir holds at least
+        multi_units(...) * 8 bytes.  gather_ordered() of the launch gives rx_multi()'s result."""
+        ns, n = d_iq.shape
+        cfgs = np.ascontiguousarray(cfgs, dtype=CFG_DTYPE).reshape(-1)
+        cc = np.ascontiguousarray(capture, dtype=np.int32).reshape(-1)
+        assert d_iq.stride(1) == 1 and cc.shape == cfgs.shape
+        cap = d_out.numel() * d_out.element_size() // 64
+        dir_cap = d_dir.numel() * d_dir.element_size() // 8
+        rc = self._L.btle_b200_rx_multi_device_dir(self._h, d_iq.data_ptr(), ns, d_iq.stride(0), n, cfgs.ctypes.data, cc.ctypes.data,
+                                                   cfgs.size, d_out.data_ptr(), cap, d_count.data_ptr() if d_count is not None else None,
+                                                   d_dir.data_ptr(), dir_cap, ctypes.c_void_p(stream_ptr))
+        self._check(rc)
+
     def rx(self, iq: np.ndarray, **cfg) -> np.ndarray:
         return self.rx_batch(np.asarray(iq).reshape(1, -1), make_cfgs(1, **cfg))
 

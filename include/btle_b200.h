@@ -160,6 +160,28 @@ int btle_b200_rx_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams
                         size_t n_int8, const btle_stream_cfg *cfgs, btle_pkt_rec *d_out, size_t cap,
                         uint32_t *d_count, void *cuda_stream);
 void btle_b200_sort_records(btle_pkt_rec *recs, size_t n);
+/* ---- several access addresses per capture, one read of the IQ --------------------------------------------------------
+ * cfg j decodes capture cfg_capture[j].  cfg_capture is non-decreasing and lies in [0, n_captures), with at most
+ * BTLE_MAX_CFGS_PER_CAPTURE cfgs per capture; a capture that no cfg names is not read.  Every cfg field applies per cfg
+ * (two cfgs of one capture may differ in any of them, the access address included or not).  The result equals
+ * btle_b200_rx_batch() on a batch whose stream j is a copy of capture cfg_capture[j] decoded with cfgs[j]: every record
+ * field is equal, stream == j included, in (j, chunk, n0) order.  Each capture's IQ is turned into discriminator bits
+ * once, whatever the number of cfgs reading it; the prefilter flags the union of the cfgs' candidates, and every
+ * candidate is re-checked exactly per cfg.  Argument errors (a cfg_capture that decreases, leaves the range or names one
+ * capture more than BTLE_MAX_CFGS_PER_CAPTURE times; the alignment and stride rules of the calls above) are BTLE_EINVAL
+ * with btle_b200_last_error() set, and the context stays usable; BTLE_EOVERFLOW reports the needed count in *n_out. */
+#define BTLE_MAX_CFGS_PER_CAPTURE 8
+int btle_b200_rx_multi(btle_b200_ctx *ctx, const int8_t *iq, size_t n_captures, size_t stream_stride_int8, size_t n_int8,
+                       const btle_stream_cfg *cfgs, const int32_t *cfg_capture, size_t n_cfgs, btle_pkt_rec *out, size_t cap,
+                       size_t *n_out);
+/* directory entries of an rx_multi launch of this shape (0 for an invalid cfg_capture) */
+size_t btle_b200_rx_multi_units(const btle_b200_ctx *ctx, size_t n_captures, const int32_t *cfg_capture, size_t n_cfgs, size_t n_int8);
+/* device-resident form; directory, d_count (may be NULL: counter ring) and streams exactly as btle_b200_rx_device_dir():
+ * walking d_dir in index order gives the records in (j, chunk, n0) order, so btle_b200_gather_ordered() applies. */
+int btle_b200_rx_multi_device_dir(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_captures, size_t stream_stride_int8,
+                                  size_t n_int8, const btle_stream_cfg *cfgs, const int32_t *cfg_capture, size_t n_cfgs,
+                                  btle_pkt_rec *d_out, size_t cap, uint32_t *d_count, btle_unit_dir *d_dir, size_t dir_cap,
+                                  void *cuda_stream);
 /* Host helper: recs[0..n_recs) and dir[0..n_units) are host copies of a launch's d_out / d_dir; copies the
  * records into out[] in reference order.  *n_out = sum of the directory counts; BTLE_EOVERFLOW if that exceeds
  * `cap` or if blocks were cut off by n_recs (out then holds what was available, still in order). */
