@@ -61,6 +61,8 @@ EXPORTS = [
     "btle_b200_receiver_controller", "btle_b200_receiver_status", "btle_b200_note_packet", "btle_b200_set_hop_hooks", "btle_b200_hop_reset",
     "btle_b200_get_freq_by_channel_number", "btle_b200_chm_is_full_map", "btle_b200_discover", "btle_b200_discover_device",
     "btle_b200_rx_multi", "btle_b200_rx_multi_units", "btle_b200_rx_multi_device_dir",
+    "btle_b200_streams_add_cfg", "btle_b200_streams_remove_cfg", "btle_b200_streams_resident", "btle_b200_streams_set_discover",
+    "btle_b200_streams_take_cands",
 ]
 MAX_CFGS_PER_CAPTURE = 8       # BTLE_MAX_CFGS_PER_CAPTURE
 
@@ -149,6 +151,12 @@ def load():
     L.btle_b200_rx_multi_units.argtypes = [vp, sz, vp, sz, sz]
     L.btle_b200_rx_multi_units.restype = sz
     L.btle_b200_rx_multi_device_dir.argtypes = [vp, vp, sz, sz, sz, vp, vp, sz, vp, sz, vp, vp, sz, vp]
+    i64p = ctypes.POINTER(ctypes.c_int64)
+    L.btle_b200_streams_add_cfg.argtypes = [vp, sz, vp, ctypes.c_int64, ctypes.POINTER(sz)]
+    L.btle_b200_streams_remove_cfg.argtypes = [vp, sz, i64p]
+    L.btle_b200_streams_resident.argtypes = [vp, i64p]
+    L.btle_b200_streams_set_discover.argtypes = [vp, vp]
+    L.btle_b200_streams_take_cands.argtypes = [vp, vp, sz, ctypes.POINTER(sz)]
     _lib = L
     return L
 

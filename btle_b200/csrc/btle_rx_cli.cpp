@@ -27,6 +27,10 @@
 //     btle_rx.c:2403) on sample time: CONNECT_REQ on -c -> data channel (hop) -> hop every interval.  The decode for
 //     every channel the radio could be on is done up front in two batched launches (advertising capture; then all 37
 //     data captures with the connection's access address), the walk only picks what the radio would have seen.
+//   * --connections with --iq-dir (not with -o): every connection at once instead of the reference's one radio.  The
+//     session decodes the advertising captures; each CONNECT_REQ, and each connection found from its empty PDUs on the
+//     data captures (discovery, no CONNECT_REQ needed), gets its access address / CRC init on all 37 data captures from
+//     the oldest segment set still on the GPU on (the policy of btle_b200.hop.ConnectionMonitor).
 //   * time stamps are sample time (4 Msps) from the start of the capture, not wall clock; in hop mode the state
 //     machine's clock is the time at which a chunk (with its look-ahead) is complete.
 #include <fcntl.h>
@@ -44,6 +48,8 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
+#include <set>
 #include <string>
 #include <vector>
 
@@ -71,6 +77,7 @@ struct Options {
   uint8_t filter_adva[6] = {0, 0, 0, 0, 0, 0};
   uint16_t filter_pdu_mask = 0xFFFF;
   int device = 0;
+  int connections = 0;                          // --connections
 };
 
 void usage() {
@@ -82,6 +89,12 @@ void usage() {
       "      access address / CRC init, streamed through one session; packets in time order up to the shortest capture's end\n"
       "       --iq-dir DIR\n      DIR/ch00.bin .. DIR/ch39.bin (time-aligned per-channel captures), streamed like several -i;\n"
       "      with -o the connection is followed across them (whole files)\n"
+      "       --connections\n      with --iq-dir (all 40 captures; not with -o): decode every connection live, CONNECT_REQ or found from its\n"
+      "      empty PDUs, on all data captures; packets of all connections in time order; per connection start one line\n"
+      "        T Connection AA:aaaaaaaa CRCInit:cccccc SRC Interval:Nus Hop:H ChC FromChunk:K\n"
+      "      (T: seconds of sample time of the CONNECT_REQ / first empty PDU; SRC: CONNECT_REQ or discovered; Interval -1 and\n"
+      "      Hop -1 when the channel sequence is not CSA#1 on a full map; C: first data channel; K: first decoded chunk);\n"
+      "      with -j a `hop` track_start event per connection whose sequence is known\n"
       "       --iq-bin16 FILE\n      interleaved int16 I,Q at 8 Msps (8 samples per symbol): a `btle_ll -q` capture; decoded with the 8-phase\n"
       "      CRC-select receiver of the reference's Python / Verilog model (first sample phase whose CRC is ok wins)\n"
       "       --segment-chunks N\n      chunks (16384 int8) per streamed segment of each capture (0 / default: 4096 = 64 MiB for one\n"
@@ -143,7 +156,7 @@ Options parse_commandline(int argc, char **argv) {
       {"filter-pdu-type", required_argument, 0, 'T'}, {"iq-file", required_argument, 0, 'i'},
       {"iq-txt", required_argument, 0, 1000}, {"iq-sc16", required_argument, 0, 1001}, {"device", required_argument, 0, 'd'},
       {"iq-dir", required_argument, 0, 1002}, {"segment-chunks", required_argument, 0, 1003}, {"iq-bin16", required_argument, 0, 1004},
-      {0, 0, 0, 0}};
+      {"connections", no_argument, 0, 1005}, {0, 0, 0, 0}};
   for (;;) {
     int idx = 0;
     const int c = getopt_long(argc, argv, "hc:g:l:ba:k:vrf:m:os:jQRF:T:i:d:", longopts, &idx);   // + i:, d:
@@ -168,6 +181,7 @@ Options parse_commandline(int argc, char **argv) {
       case 'i': o.iq_files.push_back(optarg); break;
       case 1002: o.iq_dir = optarg; break;
       case 1004: o.iq_bin16 = optarg; break;
+      case 1005: o.connections = 1; break;
       case 1003: o.segment_chunks = (size_t)strtoul(optarg, &endp, 10); break;
       case 1000: o.iq_txt = optarg; break;
       case 1001: o.iq_sc16 = optarg; break;
@@ -192,6 +206,7 @@ Options parse_commandline(int argc, char **argv) {
   if (o.gain < 0 || o.gain > 62) { printf("rx gain must be within 0~%d!\n", 62); bad_args(); }            // :1437
   if (o.lna < 0 || o.lna > 40) { printf("lna gain must be within 0~%d!\n", 40); bad_args(); }            // :1442
   if (optind < argc) { printf("Error: unknown/extra arguments specified on command line!\n"); bad_args(); }
+  if (o.connections && (!o.iq_dir || o.hop)) { printf("--connections needs --iq-dir and cannot be combined with -o\n"); bad_args(); }
   return o;
 }
 
@@ -511,6 +526,157 @@ void hop_event(void *u, const btle_hop_event *e) {                              
 // time at which chunk k and its look-ahead are complete: what the reference's wall clock shows when it runs receiver() on it
 int64_t chunk_done_us(long long k) { return (int64_t)(((k + 1) * 8192ll + BTLE_LOOKAHEAD_INT8 / 2) / 4); }
 
+// ---- --connections: btle_b200.hop.ConnectionMonitor's policy over a 40-capture session (capture i = channel i) ----------
+struct ConnMonitor {
+  static constexpr double kEventSpan = 3.75e-3;        // hop.EVENT_SPAN_S
+  static constexpr int kMinEvents = 4;                 // discover_connections(min_events=4)
+  static constexpr double kGroupS = 8.0;               // ConnectionMonitor(group_s=8.0)
+  double t_now = 0.0;
+  btle_b200_streams *ss;
+  const Options &o;
+  struct Conn {
+    uint32_t aa, crc_init;
+    bool discovered, tracked = false, announced_start = false, stopped = false;
+    int interval = 0, hop = 0, first_ch = 0;           // interval in 1.25 ms units
+    double ts = 0.0;                                   // CONNECT_REQ time or first empty PDU
+    long long from = 0;
+    std::vector<size_t> cfgs;
+  };
+  struct Group { std::vector<std::pair<double, int>> ev; int conn = -1; };
+  std::vector<Conn> conns;
+  std::map<std::pair<uint32_t, uint32_t>, Group> groups;
+  std::set<uint32_t> announced;
+  int added = 0;                                       // cfgs added by the last hand_out
+  int rc = 0;
+
+  ConnMonitor(btle_b200_streams *s, const Options &opt) : ss(s), o(opt) {}
+
+  int begin() {
+    int64_t until;
+    for (size_t c = 0; c < 37 && !rc; ++c) rc = btle_b200_streams_remove_cfg(ss, c, &until);
+    std::vector<int32_t> ch(40, -1);
+    for (int c = 0; c < 37; ++c) ch[c] = c;
+    if (!rc) rc = btle_b200_streams_set_discover(ss, ch.data());
+    return rc;
+  }
+  void start(Conn &c) {
+    int64_t from = 0;
+    btle_b200_streams_resident(ss, &from);
+    c.from = from;
+    for (int ch = 0; ch < 37 && !rc; ++ch) {
+      const btle_stream_cfg cfg{ch, c.aa, 0xFFFFFFFFu, c.crc_init, 0, o.rssi ? BTLE_CFG_RSSI : 0};
+      size_t j = 0;
+      rc = btle_b200_streams_add_cfg(ss, (size_t)ch, &cfg, from, &j);
+      c.cfgs.push_back(j);
+      ++added;
+    }
+    if (!o.quiet)
+      printf("%.6f Connection AA:%08x CRCInit:%06x %s Interval:%dus Hop:%d Ch%d FromChunk:%lld\n", c.ts, c.aa, c.crc_init & 0xFFFFFFu,
+             c.discovered ? "discovered" : "CONNECT_REQ", c.tracked ? c.interval * 1250 : -1, c.tracked ? c.hop : -1, c.first_ch, c.from);
+    note_tracked(c);
+  }
+  void note_tracked(Conn &c) {                         // one hop track_start line, as hop.hop_events() forms it
+    if (!o.json || !c.tracked || c.announced_start) return;
+    c.announced_start = true;
+    printf("{\"v\":1,\"t\":\"hop\",\"ts\":%.6f,\"event\":\"track_start\",\"state_from\":0,\"state_to\":1,\"ch\":%d,\"freq_mhz\":%d,"
+           "\"aa\":\"%08x\",\"crc_init\":\"%06x\",\"interval_us\":%d,\"hop\":%d,\"chm\":\"1fffffffff\"}\n",
+           c.ts, c.first_ch, (int)(freq_by_channel(c.first_ch) / 1000000), c.aa, c.crc_init & 0xFFFFFFu, c.interval * 1250, c.hop);
+  }
+  void stop(Conn &c) {
+    int64_t until;
+    for (size_t j : c.cfgs) if (!rc) rc = btle_b200_streams_remove_cfg(ss, j, &until);
+    c.cfgs.clear();
+    c.stopped = true;
+  }
+  // hop._connection_from_events: interval = GCD of the gaps in 1.25 ms units, hop = dch * m^-1 (mod 37)
+  static void from_events(Conn &c, const std::vector<std::pair<double, int>> &ev) {
+    long long interval = 0;
+    std::vector<long long> units;
+    for (size_t i = 1; i < ev.size(); ++i) {
+      units.push_back((long long)std::nearbyint((ev[i].first - ev[i - 1].first) / 1.25e-3));   // round half to even, as Python
+      long long a = interval, b = std::llabs(units.back());
+      while (b) { const long long t = a % b; a = b; b = t; }
+      interval = a;
+    }
+    bool ok = interval >= 6 && interval <= 3200;
+    std::set<int> hops;
+    if (ok)
+      for (size_t i = 1; i < ev.size(); ++i) {
+        const int m = (int)(((units[i - 1] / interval) % 37 + 37) % 37);
+        if (m == 0) { ok = ok && ev[i].second == ev[i - 1].second; continue; }
+        int inv = 1;
+        while (inv * m % 37 != 1) ++inv;
+        hops.insert((((ev[i].second - ev[i - 1].second) * inv) % 37 + 37) % 37);
+      }
+    ok = ok && hops.size() == 1 && !hops.count(0);
+    c.tracked = ok;
+    c.interval = ok ? (int)interval : 0;
+    c.hop = ok ? *hops.begin() : 0;
+    c.ts = ev[0].first;
+    c.first_ch = ev[0].second;
+  }
+  // records just handed out (and the candidates of the same sets)
+  void hand_out(const btle_pkt_rec *r, size_t n) {
+    added = 0;
+    for (size_t i = 0; i < n && !rc; ++i) {
+      const uint8_t *b = r[i].bytes, *p = b + 2;
+      t_now = std::max(t_now, rec_time(r[i]));
+      if (r[i].stream < 37 || r[i].stream >= 40 || r[i].crc_bad || (b[0] & 0x0F) != 5 || (b[1] & 0x3F) != 34) continue;
+      Conn c{};
+      c.aa = (uint32_t)p[12] | (uint32_t)p[13] << 8 | (uint32_t)p[14] << 16 | (uint32_t)p[15] << 24;
+      c.crc_init = (uint32_t)p[16] << 16 | (uint32_t)p[17] << 8 | p[18];
+      c.interval = p[22] | p[23] << 8;
+      c.hop = p[33] & 0x1F;
+      c.tracked = p[28] == 0xFF && p[29] == 0xFF && p[30] == 0xFF && p[31] == 0xFF && p[32] == 0x1F && c.interval > 0;
+      c.discovered = false;
+      c.ts = rec_time(r[i]);
+      c.first_ch = c.hop % 37;
+      announced.insert(c.aa);
+      for (Conn &d : conns)                            // announced after all: the CONNECT_REQ connection takes it over
+        if (d.discovered && d.aa == c.aa && !d.stopped) stop(d);
+      conns.push_back(c);
+      start(conns.back());
+    }
+    std::vector<btle_conn_cand> cand(4096);
+    std::vector<btle_conn_cand> all;
+    for (;;) {
+      size_t got = 0;
+      const int q = btle_b200_streams_take_cands(ss, cand.data(), cand.size(), &got);
+      all.insert(all.end(), cand.begin(), cand.begin() + (long)got);
+      if (q != BTLE_EOVERFLOW) break;
+    }
+    std::stable_sort(all.begin(), all.end(), [](const btle_conn_cand &a, const btle_conn_cand &b) {
+      if (a.access_addr != b.access_addr) return a.access_addr < b.access_addr;
+      if (a.crc_init != b.crc_init) return a.crc_init < b.crc_init;
+      return a.sample < b.sample;
+    });
+    for (const btle_conn_cand &c : all) {
+      auto &ev = groups[{c.access_addr, c.crc_init}].ev;
+      const double t = (double)c.sample / 4.0e6;
+      if (!ev.empty() && c.channel == ev.back().second && t - ev.back().first < kEventSpan) continue;
+      ev.push_back({t, (int)c.channel});
+    }
+    for (const btle_conn_cand &c : all) t_now = std::max(t_now, (double)c.sample / 4.0e6);
+    for (auto it = groups.begin(); it != groups.end();)     // noise groups that stopped: forgotten (ConnectionMonitor.group_s)
+      it = it->second.conn < 0 && (int)it->second.ev.size() < kMinEvents && t_now - it->second.ev.back().first > kGroupS ? groups.erase(it) : std::next(it);
+    for (auto &kv : groups) {
+      Group &g = kv.second;
+      if ((int)g.ev.size() < kMinEvents || announced.count(kv.first.first) || rc) continue;
+      if (g.conn < 0) {
+        Conn c{};
+        c.aa = kv.first.first; c.crc_init = kv.first.second; c.discovered = true;
+        from_events(c, g.ev);
+        g.conn = (int)conns.size();
+        conns.push_back(c);
+        start(conns.back());
+      } else if (!conns[(size_t)g.conn].stopped) {
+        from_events(conns[(size_t)g.conn], g.ev);
+        note_tracked(conns[(size_t)g.conn]);
+      }
+    }
+  }
+};
+
 }  // namespace
 
 int main(int argc, char **argv) {
@@ -565,6 +731,7 @@ int main(int argc, char **argv) {
   }
   for (const Capture &c : caps)
     if (c.chan < 0 || c.chan > 39) { printf("channel number must be within 0~%d!\n", 39); btle_b200_destroy(ctx); return 1; }
+  if (o.connections && caps.size() != 40) { printf("--connections needs all 40 chNN.bin captures in %s\n", o.iq_dir); btle_b200_destroy(ctx); return 1; }
 
   if (o.iq_bin16) {
     // ---- 8 samples per symbol: the Python / Verilog model's receiver, streaming over the capture -------------------------
@@ -684,6 +851,8 @@ int main(int argc, char **argv) {
     btle_b200_streams *ss = nullptr;
     rc = btle_b200_streams_open(ctx, cfgs.data(), ns, o.segment_chunks, &ss);
     if (rc) { close_inputs(); return fail("btle_b200_streams_open"); }
+    ConnMonitor mon(ss, o);
+    if (o.connections && mon.begin()) { rc = mon.rc; btle_b200_streams_close(ss); close_inputs(); return fail("--connections"); }
     std::vector<btle_pkt_rec> recs(65536), pending;
     long long max_chunk = -1;
     // Records arrive per segment set in (stream, chunk, n0) order.  They are printed in time order (chunk*8192 + n0; ties in
@@ -695,7 +864,12 @@ int main(int argc, char **argv) {
         if (key(a) != key(b)) return key(a) < key(b);
         return a.stream != b.stream ? a.stream < b.stream : a.chunk < b.chunk;
       });
-      const long long safe = (max_chunk + 1) * 8192 - 124;
+      long long safe = (max_chunk + 1) * 8192 - 124;
+      if (o.connections) {                                     // a backfilled record can lie anywhere in the resident sets
+        int64_t res = 0;
+        btle_b200_streams_resident(ss, &res);
+        safe = std::min<long long>(safe, (long long)res * 8192 - 124);
+      }
       size_t k = 0;
       for (; k < pending.size() && (all || key(pending[k]) < safe); ++k) sinks.packet(pending[k], rec_time(pending[k]));
       pending.erase(pending.begin(), pending.begin() + (long)k);
@@ -703,6 +877,7 @@ int main(int argc, char **argv) {
     };
     auto keep = [&](size_t n) {
       for (size_t i = 0; i < n; ++i) { pending.push_back(recs[i]); max_chunk = std::max<long long>(max_chunk, recs[i].chunk); }
+      if (o.connections) { mon.hand_out(recs.data(), n); if (mon.rc && !rc) rc = mon.rc; }
     };
     std::vector<size_t> total(ns, 0);
     std::vector<char> eof(ns, 0);
@@ -744,11 +919,15 @@ int main(int argc, char **argv) {
       }
     }
     if (rc) { btle_b200_streams_close(ss); close_inputs(); return fail("btle_b200_streams_commit"); }
-    for (;;) {                                                  // end of input or SIGINT: decode up to the shortest capture
-      size_t n = 0;
-      rc = btle_b200_streams_finish(ss, recs.data(), recs.size(), &n);
-      keep(n);
-      if (rc != BTLE_EOVERFLOW) break;
+    for (bool more = true; more && rc == 0;) {                 // end of input or SIGINT: decode up to the shortest capture
+      more = false;
+      for (;;) {
+        size_t n = 0;
+        rc = btle_b200_streams_finish(ss, recs.data(), recs.size(), &n);
+        keep(n);
+        more |= o.connections && mon.added > 0;                // new connections: their backfill comes from the next finish
+        if (rc != BTLE_EOVERFLOW) break;
+      }
     }
     btle_b200_streams_close(ss);
     close_inputs();

@@ -22,9 +22,11 @@
 #include <unistd.h>
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <new>
 #include <string>
 #include <thread>
@@ -2303,15 +2305,36 @@ int btle_b200_rx_multi(btle_b200_ctx *ctx, const int8_t *iq, size_t n_captures, 
 // One segment SET = `seg_chunks` chunks of every capture.  Capture i's part of a set sits at i * stride in the half's
 // buffers: kLead bytes of the previous set, the segment, kLook look-ahead bytes (the start of the next set).  A set is
 // decoded by ONE batched launch of the persistent kernel over the N parts once every capture has filled its own.
+// Once the cfg list has changed (btle_b200_streams_add_cfg / remove_cfg) a set is decoded by rx_multi launches instead,
+// in rounds of at most kMaxCfgsPerCapture cfgs per capture; a cfg added for chunks that are still resident is decoded
+// over them by one more launch on the half that holds them (backfill).
 struct btle_b200_streams {
   btle_b200_ctx *ctx = nullptr;
   size_t n = 0;                                            // captures in the session
-  std::vector<btle_stream_cfg> cfgs;                       // what the next submitted set is decoded with
+  std::vector<btle_stream_cfg> cfgs;                       // what the next submitted set is decoded with (cfgs 0..n-1)
+  struct Entry {                                           // stable cfg index j: decodes `capture` for chunks [from, until)
+    btle_stream_cfg cfg; size_t capture; long long from, until;
+  };
+  std::vector<Entry> entries;                              // [0, n): the cfgs of streams_open (cfg mirrors cfgs[j])
+  bool listed = false;                                     // a cfg was added or removed: sets go through rx_multi rounds
+  std::vector<size_t> backfill;                            // cfgs added since the last commit / finish (streams_backfill)
+  int call_launches = 0;                                   // launches of the current commit / finish call
+  std::vector<int32_t> disc;                               // data channel scanned per capture, -1: none (set_discover)
+  std::vector<btle_conn_cand> cands;                       // candidates of the sets handed out, not yet taken
   size_t seg_chunks = 0, seg_bytes = 0, buf_bytes = 0;     // a part = seg_chunks chunks (+ kLook look-ahead bytes behind it)
   size_t stride = 0;                                       // kLead + buf_bytes: bytes from one capture's part to the next
   static constexpr size_t kLook = 4096;                    // >= 3008 + the kernel's 12-group tile (3072 + 4)
   static constexpr size_t kLead = 256;                     // bytes of the previous set kept in front (a hit may start up to 124 samples
                                                            // before its chunk; the RSSI sum reads the raw IQ there)
+  struct Job {                                             // one rx_multi launch on a half's IQ, collected with the half
+    std::vector<size_t> index;                             // launch position -> stable cfg index
+    size_t units = 0, cap = 0;
+    Buf<btle_pkt_rec> d_out; Buf<btle_unit_dir> d_dir; Buf<unsigned> d_count;
+    HostBuf<unsigned> h_count; HostBuf<btle_unit_dir> h_dir;
+  };
+  struct Scan {                                            // one discover launch over captures [first, first + count)
+    size_t first = 0, count = 0, off = 0, cap = 0;         // candidates at d_cand[off, off + cap)
+  };
   struct Half {                                            // buffers sized once by btle_b200_streams_open
     HostBuf<int8_t> h; Buf<int8_t> d;                      // page-locked host / device IQ buffers, n parts of `stride` bytes
     Buf<btle_pkt_rec> d_out; Buf<btle_unit_dir> d_dir; Buf<unsigned> d_count;
@@ -2319,7 +2342,16 @@ struct btle_b200_streams {
     size_t n_submitted = 0;
     long long first_chunk = 0;
     cudaStream_t st = nullptr;
-    bool busy = false;
+    bool busy = false;                                     // the single-cfg launch of the set waits to be collected
+    bool resident = false;                                 // d holds the set at first_chunk (lead, n_submitted bytes)
+    std::vector<std::unique_ptr<Job>> jobs;                // jobs[0, n_jobs) wait to be collected (grown, then reused)
+    size_t n_jobs = 0;
+    HostBuf<btle_pkt_rec> h_jrecs;                         // their records, grown to what they found
+    std::vector<Scan> scans;                               // discover launches waiting to be collected
+    std::vector<int32_t> scan_ch;                          // the channels they scanned, per capture
+    size_t scan_samples = 0;                               // window starts kept: local samples [128, 128 + scan_samples)
+    size_t scan_bytes = 0;                                 // bytes each scanned part was read with (lead included)
+    Buf<btle_conn_cand> d_cand; Buf<unsigned> d_ccount; HostBuf<unsigned> h_ccount; HostBuf<btle_conn_cand> h_cand;
   } half[2];
   std::vector<size_t> fill;                                // bytes in each capture's part of the half being filled
   size_t n_full = 0;                                       // captures whose part of that half is complete
@@ -2335,47 +2367,277 @@ struct btle_b200_stream {
 };
 
 namespace {
-// decode the first n_int8 bytes of every capture's part of half b (bytes behind n_int8 read as 0)
-int streams_submit(btle_b200_streams *s, int b, size_t n_int8) {
+using Streams = btle_b200_streams;
+
+// One rx_multi launch over half b's set, enqueued behind whatever its stream holds: cfgs `idx` (stable indices, sorted
+// by capture, at most kMaxCfgsPerCapture per capture) on the set's n_submitted bytes.  Collected by streams_collect.
+int streams_job(Streams *s, int b, const std::vector<size_t> &idx) {
+  btle_b200_ctx *ctx = s->ctx;
+  auto &H = s->half[b];
+  if (H.n_jobs == H.jobs.size()) {
+    H.jobs.emplace_back(new (std::nothrow) Streams::Job());
+    if (!H.jobs.back()) { H.jobs.pop_back(); return BTLE_ENOMEM; }
+  }
+  Streams::Job &J = *H.jobs[H.n_jobs];
+  const size_t k = idx.size(), nch = H.n_submitted / kChunkInt8;
+  std::vector<btle_stream_cfg> cfgs(k);
+  std::vector<int32_t> cc(k);
+  for (size_t i = 0; i < k; ++i) { cfgs[i] = s->entries[idx[i]].cfg; cc[i] = (int32_t)s->entries[idx[i]].capture; }
+  const size_t units = std::max<size_t>(btle_b200_rx_multi_units(ctx, s->n, cc.data(), k, H.n_submitted), 1);
+  const size_t cap = k * nch * BTLE_MAX_RECS_PER_CHUNK;      // the most a launch can find: never an overflow
+  if (J.d_out.reserve(ctx, cap) || J.d_dir.reserve(ctx, units) || J.h_dir.reserve(ctx, units) ||
+      (!J.d_count && (J.d_count.alloc(ctx, 1) || J.h_count.alloc(ctx, 1))))
+    return BTLE_ENOMEM;
+  ctx->lead_bytes = Streams::kLead;
+  const int rc = btle_b200_rx_multi_device_dir(ctx, H.d + Streams::kLead, s->n, s->stride, H.n_submitted, cfgs.data(), cc.data(), k,
+                                               J.d_out, cap, J.d_count, J.d_dir, J.d_dir.n, H.st);
+  ctx->lead_bytes = 0;
+  if (rc) return rc;
+  BTLE_CUDA(ctx, cudaMemcpyAsync(J.h_count, J.d_count, sizeof(unsigned), cudaMemcpyDeviceToHost, H.st));
+  BTLE_CUDA(ctx, cudaMemcpyAsync(J.h_dir, J.d_dir, units * sizeof(btle_unit_dir), cudaMemcpyDeviceToHost, H.st));
+  J.index = idx;
+  J.units = units;
+  J.cap = cap;
+  ++H.n_jobs;
+  return BTLE_OK;
+}
+
+// Those of the cfgs `cand` that decode some chunk of half b's set, sorted by capture, in rounds of at most
+// kMaxCfgsPerCapture per capture: one streams_job per round.  A capture no such cfg names is not read.  *launches counts
+// the launches.
+int streams_rounds(Streams *s, int b, const std::vector<size_t> &cand, int *launches) {
+  auto &H = s->half[b];
+  const long long lo = H.first_chunk, hi = lo + (long long)(H.n_submitted / kChunkInt8);
+  std::vector<size_t> live;
+  for (size_t j : cand)
+    if (s->entries[j].from < hi && s->entries[j].until > lo) live.push_back(j);
+  std::stable_sort(live.begin(), live.end(), [&](size_t x, size_t y) { return s->entries[x].capture < s->entries[y].capture; });
+  for (size_t r = 0;; ++r) {
+    std::vector<size_t> idx;
+    for (size_t i = 0; i < live.size();) {                  // [i, e): the live cfgs of one capture
+      size_t e = i;
+      while (e < live.size() && s->entries[live[e]].capture == s->entries[live[i]].capture) ++e;
+      for (size_t q = i + r * kMaxCfgsPerCapture; q < std::min(e, i + (r + 1) * kMaxCfgsPerCapture); ++q) idx.push_back(live[q]);
+      i = e;
+    }
+    if (idx.empty()) return BTLE_OK;
+    const int rc = streams_job(s, b, idx);
+    if (rc) return rc;
+    ++*launches;
+  }
+}
+
+// discover_kernel over every scanned capture's part of half b: `bytes` bytes from the start of its lead.  One launch
+// per run of adjacent scanned captures, each with its own counter and part of d_cand.
+int streams_scan(Streams *s, int b, size_t bytes, size_t keep_samples, int *launches) {
+  btle_b200_ctx *ctx = s->ctx;
+  auto &H = s->half[b];
+  H.scans.clear();
+  size_t total = 0;
+  for (size_t i = 0; i < s->n;) {
+    if (s->disc[i] < 0) { ++i; continue; }
+    size_t e = i + 1;
+    while (e < s->n && s->disc[e] >= 0) ++e;
+    Streams::Scan sc;
+    sc.first = i; sc.count = e - i; sc.off = total; sc.cap = sc.count * (bytes / kChunkInt8 + 1) * 8 + 256;
+    total += sc.cap;
+    H.scans.push_back(sc);
+    i = e;
+  }
+  if (H.scans.empty()) return BTLE_OK;
+  H.scan_ch = s->disc;
+  H.scan_bytes = bytes;
+  H.scan_samples = keep_samples;
+  if (H.d_cand.reserve(ctx, total) || H.d_ccount.reserve(ctx, H.scans.size()) || H.h_ccount.reserve(ctx, H.scans.size())) return BTLE_ENOMEM;
+  for (size_t r = 0; r < H.scans.size(); ++r) {
+    const Streams::Scan &sc = H.scans[r];
+    const int rc = launch_discover(ctx, H.d + sc.first * s->stride, sc.count, s->stride, bytes, H.scan_ch.data() + sc.first,
+                                   H.d_cand + sc.off, sc.cap, H.d_ccount + r, H.st);
+    if (rc) return rc;
+    BTLE_CUDA(ctx, cudaMemcpyAsync(H.h_ccount + r, H.d_ccount + r, sizeof(unsigned), cudaMemcpyDeviceToHost, H.st));
+    ++*launches;
+  }
+  return BTLE_OK;
+}
+
+// decode the first n_int8 bytes of every capture's part of half b (bytes behind n_int8 read as 0); `last`: the end of the
+// captures, so discovery keeps every window start of the n_int8 bytes instead of those of the segment
+int streams_submit(Streams *s, int b, size_t n_int8, bool last = false) {
   btle_b200_ctx *ctx = s->ctx;
   auto &H = s->half[b];
   H.n_submitted = n_int8;
   H.first_chunk = s->next_chunk;
-  if (n_int8 < (size_t)kChunkInt8) { H.busy = false; return BTLE_OK; }
+  const bool scan = std::any_of(s->disc.begin(), s->disc.end(), [](int32_t c) { return c >= 0; });
+  if (n_int8 < (size_t)kChunkInt8 && !(scan && n_int8)) { H.busy = false; H.resident = false; return BTLE_OK; }
   constexpr size_t L = btle_b200_streams::kLead;
   if (L + n_int8 == s->stride || s->n == 1)
     BTLE_CUDA(ctx, cudaMemcpyAsync(H.d, H.h, (s->n - 1) * s->stride + L + n_int8, cudaMemcpyHostToDevice, H.st));
   else
     BTLE_CUDA(ctx, cudaMemcpy2DAsync(H.d, s->stride, H.h, s->stride, L + n_int8, s->n, cudaMemcpyHostToDevice, H.st));
-  ctx->lead_bytes = L;
-  const int rc = btle_b200_rx_device_dir(ctx, H.d + L, s->n, s->stride, n_int8, s->cfgs.data(), H.d_out, H.d_out.n, H.d_count, H.d_dir,
-                                         H.d_dir.n, H.st);
-  ctx->lead_bytes = 0;
-  if (rc) return rc;
-  BTLE_CUDA(ctx, cudaMemcpyAsync(H.h_count, H.d_count, sizeof(unsigned), cudaMemcpyDeviceToHost, H.st));
-  BTLE_CUDA(ctx, cudaMemcpyAsync(H.h_dir, H.d_dir, H.d_dir.n * sizeof(btle_unit_dir), cudaMemcpyDeviceToHost, H.st));
-  H.busy = true;
+  H.resident = true;
+  int &launches = s->call_launches, rc = BTLE_OK;
+  if (n_int8 >= (size_t)kChunkInt8 && s->listed) {
+    std::vector<size_t> all(s->entries.size());
+    for (size_t j = 0; j < all.size(); ++j) all[j] = j;
+    rc = streams_rounds(s, b, all, &launches);
+    if (rc) return rc;
+  } else if (n_int8 >= (size_t)kChunkInt8) {
+    ctx->lead_bytes = L;
+    rc = btle_b200_rx_device_dir(ctx, H.d + L, s->n, s->stride, n_int8, s->cfgs.data(), H.d_out, H.d_out.n, H.d_count, H.d_dir,
+                                 H.d_dir.n, H.st);
+    ctx->lead_bytes = 0;
+    if (rc) return rc;
+    BTLE_CUDA(ctx, cudaMemcpyAsync(H.h_count, H.d_count, sizeof(unsigned), cudaMemcpyDeviceToHost, H.st));
+    BTLE_CUDA(ctx, cudaMemcpyAsync(H.h_dir, H.d_dir, H.d_dir.n * sizeof(btle_unit_dir), cudaMemcpyDeviceToHost, H.st));
+    H.busy = true;
+    launches += 1;
+  }
+  if (scan) {
+    rc = streams_scan(s, b, L + n_int8, (last ? n_int8 : s->seg_bytes) / 2, &launches);
+    if (rc) return rc;
+  }
   return BTLE_OK;
 }
-// wait for a submitted half, append its records ((stream, chunk, n0) order, stream-wide chunk numbers) to s->ready
-int streams_collect(btle_b200_streams *s, int b) {
+
+// Backfill of the cfgs added since the last call (s->backfill): on each resident set that holds chunks at or behind their
+// from_chunk, one streams_rounds pass over all of them (at most kMaxCfgsPerCapture per capture per launch), on that
+// half's stream.  Runs at the start of the next commit / finish, before any set is collected or submitted, so the
+// halves still hold the sets add_cfg saw.
+int streams_backfill(Streams *s) {
+  if (s->backfill.empty()) return BTLE_OK;
+  std::vector<size_t> cand;
+  cand.swap(s->backfill);
+  for (int b = 0; b < 2; ++b) {
+    const auto &H = s->half[b];
+    if (!H.resident || H.n_submitted < (size_t)kChunkInt8) continue;
+    const int rc = streams_rounds(s, b, cand, &s->call_launches);
+    if (rc) return rc;
+  }
+  return BTLE_OK;
+}
+// the number of launches a commit / finish call made, when the cfg list or discovery are in use (otherwise the
+// single-cfg launch reports itself)
+void streams_note_launches(Streams *s) {
+  const bool scan = std::any_of(s->disc.begin(), s->disc.end(), [](int32_t c) { return c >= 0; });
+  if ((s->listed || scan) && s->call_launches) s->ctx->last_launches = s->call_launches;
+}
+
+// the records of half b's rx_multi jobs: stable cfg index in `stream`, stream-wide chunks, each cfg's [from, until)
+// kept, in (cfg, chunk, n0) order, appended to s->ready
+int streams_collect_jobs(Streams *s, int b) {
   btle_b200_ctx *ctx = s->ctx;
   auto &H = s->half[b];
-  if (!H.busy) return BTLE_OK;
-  H.busy = false;
+  size_t total = 0;
+  for (size_t q = 0; q < H.n_jobs; ++q) {
+    const Streams::Job &J = *H.jobs[q];
+    if (*J.h_count > J.cap) { ctx->err = "stream segment produced more records than BTLE_MAX_RECS_PER_CHUNK allows"; return BTLE_EOVERFLOW; }
+    total += *J.h_count;
+  }
+  const size_t n_jobs = H.n_jobs;
+  H.n_jobs = 0;
+  if (!total) return BTLE_OK;
+  if (H.h_jrecs.reserve(ctx, total)) return BTLE_ENOMEM;
+  for (size_t q = 0, at = 0; q < n_jobs; at += *H.jobs[q]->h_count, ++q)
+    if (*H.jobs[q]->h_count)
+      BTLE_CUDA(ctx, cudaMemcpyAsync(H.h_jrecs + at, H.jobs[q]->d_out, *H.jobs[q]->h_count * sizeof(btle_pkt_rec), cudaMemcpyDeviceToHost, H.st));
   BTLE_CUDA(ctx, cudaStreamSynchronize(H.st));
-  const size_t found = *H.h_count;
-  if (found > H.d_out.n) { ctx->err = "stream segment produced more records than BTLE_MAX_RECS_PER_CHUNK allows"; return BTLE_EOVERFLOW; }
-  if (!found) return BTLE_OK;
-  BTLE_CUDA(ctx, cudaMemcpyAsync(H.h_recs, H.d_out, found * sizeof(btle_pkt_rec), cudaMemcpyDeviceToHost, H.st));
-  BTLE_CUDA(ctx, cudaStreamSynchronize(H.st));
-  const size_t units = btle_b200_rx_units(ctx, s->n, H.n_submitted);
-  const size_t at = s->ready.size();
-  s->ready.resize(at + found);
-  size_t got = 0;
-  btle_b200_gather_ordered(H.h_recs, found, H.h_dir, units, s->ready.data() + at, found, &got);
-  for (size_t i = at; i < at + found; ++i) s->ready[i].chunk += (int32_t)H.first_chunk;
+  std::vector<btle_pkt_rec> got(total), keep;
+  keep.reserve(total);
+  for (size_t q = 0, at = 0; q < n_jobs; ++q) {
+    const Streams::Job &J = *H.jobs[q];
+    const size_t found = *J.h_count;
+    size_t n_got = 0;
+    btle_b200_gather_ordered(H.h_jrecs + at, found, J.h_dir, J.units, got.data() + at, found, &n_got);
+    for (size_t i = at; i < at + found; ++i) {
+      btle_pkt_rec r = got[i];
+      const size_t j = J.index[(size_t)r.stream];
+      const long long chunk = r.chunk + H.first_chunk;
+      if (chunk < s->entries[j].from || chunk >= s->entries[j].until) continue;
+      r.stream = (int32_t)j;
+      r.chunk = (int32_t)chunk;
+      keep.push_back(r);
+    }
+    at += found;
+  }
+  std::stable_sort(keep.begin(), keep.end(), [](const btle_pkt_rec &x, const btle_pkt_rec &y) { return x.stream < y.stream; });
+  s->ready.insert(s->ready.end(), keep.begin(), keep.end());
   return BTLE_OK;
+}
+
+// the candidates of half b's discover launches: window starts inside the set's segment, stream-wide samples, capture
+// index in `stream`, sorted by (stream, sample), appended to s->cands.  A launch whose buffer overflowed is run again
+// on the still-resident set with room for all it found.
+int streams_collect_scans(Streams *s, int b) {
+  btle_b200_ctx *ctx = s->ctx;
+  auto &H = s->half[b];
+  if (H.scans.empty()) return BTLE_OK;
+  std::vector<Streams::Scan> scans;
+  scans.swap(H.scans);
+  std::vector<size_t> found(scans.size());
+  size_t total = 0;
+  for (size_t r = 0; r < scans.size(); ++r) total += (found[r] = H.h_ccount[r]);
+  if (H.h_cand.reserve(ctx, std::max<size_t>(total, 1))) return BTLE_ENOMEM;
+  for (size_t r = 0, at = 0; r < scans.size(); at += found[r], ++r)
+    if (found[r] && found[r] <= scans[r].cap)
+      BTLE_CUDA(ctx, cudaMemcpyAsync(H.h_cand + at, H.d_cand + scans[r].off, found[r] * sizeof(btle_conn_cand), cudaMemcpyDeviceToHost, H.st));
+  BTLE_CUDA(ctx, cudaStreamSynchronize(H.st));
+  for (size_t r = 0, at = 0; r < scans.size(); at += found[r], ++r) {
+    if (found[r] <= scans[r].cap) continue;
+    if (H.d_cand.reserve(ctx, found[r])) return BTLE_ENOMEM;   // (the other launches' candidates are on the host already)
+    const int rc = launch_discover(ctx, H.d + scans[r].first * s->stride, scans[r].count, s->stride, H.scan_bytes,
+                                   H.scan_ch.data() + scans[r].first, H.d_cand, found[r], H.d_ccount, H.st);
+    if (rc) return rc;
+    BTLE_CUDA(ctx, cudaMemcpyAsync(H.h_cand + at, H.d_cand, found[r] * sizeof(btle_conn_cand), cudaMemcpyDeviceToHost, H.st));
+    BTLE_CUDA(ctx, cudaStreamSynchronize(H.st));
+  }
+  const long long lead = (long long)(Streams::kLead / 2), base = H.first_chunk * (long long)(kChunkInt8 / 2) - lead;
+  const size_t at0 = s->cands.size();
+  for (size_t r = 0, at = 0; r < scans.size(); at += found[r], ++r)
+    for (size_t i = at; i < at + found[r]; ++i) {
+      btle_conn_cand c = H.h_cand[i];
+      if (c.sample < lead || c.sample >= lead + (long long)H.scan_samples || base + c.sample < 32) continue;
+      c.sample += base;
+      c.stream += (int32_t)scans[r].first;
+      s->cands.push_back(c);
+    }
+  std::sort(s->cands.begin() + at0, s->cands.end(), [](const btle_conn_cand &x, const btle_conn_cand &y) {
+    return x.stream != y.stream ? x.stream < y.stream : x.sample < y.sample;
+  });
+  return BTLE_OK;
+}
+
+// wait for half b's launches; append its records ((stream, chunk, n0) order, stream-wide chunk numbers) to s->ready and
+// its candidates to s->cands
+int streams_collect(Streams *s, int b) {
+  btle_b200_ctx *ctx = s->ctx;
+  auto &H = s->half[b];
+  if (!H.busy && !H.n_jobs && H.scans.empty()) return BTLE_OK;
+  BTLE_CUDA(ctx, cudaStreamSynchronize(H.st));
+  if (H.busy) {
+    H.busy = false;
+    const size_t found = *H.h_count;
+    if (found > H.d_out.n) { ctx->err = "stream segment produced more records than BTLE_MAX_RECS_PER_CHUNK allows"; return BTLE_EOVERFLOW; }
+    if (found) {
+      BTLE_CUDA(ctx, cudaMemcpyAsync(H.h_recs, H.d_out, found * sizeof(btle_pkt_rec), cudaMemcpyDeviceToHost, H.st));
+      BTLE_CUDA(ctx, cudaStreamSynchronize(H.st));
+      const size_t units = btle_b200_rx_units(ctx, s->n, H.n_submitted);
+      const size_t at = s->ready.size();
+      s->ready.resize(at + found);
+      size_t got = 0;
+      btle_b200_gather_ordered(H.h_recs, found, H.h_dir, units, s->ready.data() + at, found, &got);
+      for (size_t i = at; i < at + found; ++i) s->ready[i].chunk += (int32_t)H.first_chunk;
+    }
+  }
+  int rc = streams_collect_jobs(s, b);
+  if (rc) return rc;
+  return streams_collect_scans(s, b);
+}
+// first chunk of the oldest set whose IQ is still on the device (the next set's first chunk when none is)
+long long streams_resident(const Streams *s) {
+  long long r = s->next_chunk;
+  for (const auto &H : s->half)
+    if (H.resident) r = std::min(r, H.first_chunk);
+  return r;
 }
 size_t streams_take(btle_b200_streams *s, btle_pkt_rec *out, size_t cap) {
   const size_t n = std::min(cap, s->ready.size() - s->ready_pos);
@@ -2409,6 +2671,8 @@ int btle_b200_streams_open(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size
   btle_b200_streams *s = new (std::nothrow) btle_b200_streams();
   if (!s) return BTLE_ENOMEM;
   s->ctx = ctx; s->n = n_streams; s->cfgs.assign(cfgs, cfgs + n_streams); s->fill.assign(n_streams, 0);
+  for (size_t i = 0; i < n_streams; ++i) s->entries.push_back({cfgs[i], i, 0, LLONG_MAX});
+  s->disc.assign(n_streams, -1);
   s->seg_chunks = segment_chunks; s->seg_bytes = segment_chunks * (size_t)kChunkInt8;
   s->buf_bytes = s->seg_bytes + btle_b200_streams::kLook;
   s->stride = btle_b200_streams::kLead + s->buf_bytes;     // a multiple of 16, as the batched kernel needs
@@ -2446,6 +2710,7 @@ int btle_b200_streams_set_cfg(btle_b200_streams *s, size_t stream, const btle_st
   rc = validate_cfgs(s->ctx, cfg, 1);
   if (rc) return rc;
   s->cfgs[stream] = *cfg;                                   // used from the next submitted segment set on
+  s->entries[stream].cfg = *cfg;
   return BTLE_OK;
 }
 
@@ -2466,6 +2731,11 @@ int btle_b200_streams_commit(btle_b200_streams *s, size_t stream, size_t n_int8,
   if (rc) return rc;
   if (n_int8 > s->buf_bytes - s->fill[stream]) { s->ctx->err = "stream_commit: more bytes than acquired"; return BTLE_EINVAL; }
   BTLE_CUDA(s->ctx, cudaSetDevice(s->ctx->device));
+  s->call_launches = 0;
+  rc = streams_backfill(s);
+  if (rc) return rc;
+  rc = streams_collect(s, s->cur);                          // backfill launches on the set the filling half still holds
+  if (rc) return rc;
   s->fill[stream] += n_int8;
   if (n_int8 && s->fill[stream] == s->buf_bytes) ++s->n_full;
   if (s->n_full == s->n) {                                  // every part + look-ahead complete: hand the set to the GPU
@@ -2484,6 +2754,7 @@ int btle_b200_streams_commit(btle_b200_streams *s, size_t stream, size_t n_int8,
     s->next_chunk += (long long)s->seg_chunks;
     s->cur = o;
   }
+  streams_note_launches(s);
   *n_out = streams_take(s, out, cap);
   return BTLE_OK;
 }
@@ -2493,12 +2764,18 @@ int btle_b200_streams_finish(btle_b200_streams *s, btle_pkt_rec *out, size_t cap
   *n_out = 0;
   BTLE_CUDA(s->ctx, cudaSetDevice(s->ctx->device));
   const int b = s->cur, o = b ^ 1;
-  int rc = streams_collect(s, o);
+  s->call_launches = 0;
+  int rc = streams_backfill(s);
+  if (rc) return rc;
+  rc = streams_collect(s, b);                               // backfill launches
+  if (rc) return rc;
+  rc = streams_collect(s, o);
   if (rc) return rc;
   // the tail: complete chunks of the SHORTEST capture; behind that length every capture reads as 0 (rx_batch's common n_int8)
   const size_t n_int8 = *std::min_element(s->fill.begin(), s->fill.end());
-  if (n_int8 >= (size_t)kChunkInt8) {
-    rc = streams_submit(s, b, n_int8);
+  const bool scan = std::any_of(s->disc.begin(), s->disc.end(), [](int32_t c) { return c >= 0; });
+  if (n_int8 >= (size_t)kChunkInt8 || (scan && n_int8)) {   // (discovery reads the windows of a tail shorter than a chunk)
+    rc = streams_submit(s, b, n_int8, true);
     if (rc) return rc;
     rc = streams_collect(s, b);
     if (rc) return rc;
@@ -2506,8 +2783,62 @@ int btle_b200_streams_finish(btle_b200_streams *s, btle_pkt_rec *out, size_t cap
   }
   std::fill(s->fill.begin(), s->fill.end(), size_t(0));
   s->n_full = 0;
+  streams_note_launches(s);
   *n_out = streams_take(s, out, cap);
   return (s->ready.size() > s->ready_pos) ? BTLE_EOVERFLOW : BTLE_OK;   // call again with more room
+}
+
+int btle_b200_streams_resident(const btle_b200_streams *s, int64_t *first_chunk) {
+  if (!s || !first_chunk) return BTLE_EINVAL;
+  *first_chunk = streams_resident(s);
+  return BTLE_OK;
+}
+
+int btle_b200_streams_add_cfg(btle_b200_streams *s, size_t capture, const btle_stream_cfg *cfg, int64_t from_chunk, size_t *index) {
+  if (!s || !cfg || !index) return BTLE_EINVAL;
+  int rc = streams_index(s, capture);
+  if (rc) return rc;
+  rc = validate_cfgs(s->ctx, cfg, 1);
+  if (rc) return rc;
+  if (from_chunk < streams_resident(s)) {
+    s->ctx->err = "streams_add_cfg: from_chunk lies before the first resident chunk (btle_b200_streams_resident)";
+    return BTLE_EINVAL;
+  }
+  // backfill over the resident sets is enqueued by the next commit / finish, batched with every cfg added until then
+  const size_t j = s->entries.size();
+  s->entries.push_back({*cfg, capture, (long long)from_chunk, LLONG_MAX});
+  s->backfill.push_back(j);
+  s->listed = true;
+  *index = j;
+  return BTLE_OK;
+}
+
+int btle_b200_streams_remove_cfg(btle_b200_streams *s, size_t index, int64_t *until_chunk) {
+  if (!s || !until_chunk) return BTLE_EINVAL;
+  if (index >= s->entries.size()) { s->ctx->err = "streams_remove_cfg: cfg index out of range"; return BTLE_EINVAL; }
+  auto &e = s->entries[index];
+  if (e.until != LLONG_MAX) { s->ctx->err = "streams_remove_cfg: cfg already removed"; return BTLE_EINVAL; }
+  e.until = std::max(e.from, s->next_chunk);                // the next submitted set starts at next_chunk
+  s->listed = true;
+  *until_chunk = e.until;
+  return BTLE_OK;
+}
+
+int btle_b200_streams_set_discover(btle_b200_streams *s, const int32_t *channels) {
+  if (!s || !channels) return BTLE_EINVAL;
+  for (size_t i = 0; i < s->n; ++i)
+    if (channels[i] < -1 || channels[i] > 36) { s->ctx->err = "streams_set_discover: data channel must be within 0~36 or -1"; return BTLE_EINVAL; }
+  s->disc.assign(channels, channels + s->n);
+  return BTLE_OK;
+}
+
+int btle_b200_streams_take_cands(btle_b200_streams *s, btle_conn_cand *out, size_t cap, size_t *n_out) {
+  if (!s || !n_out || (!out && cap)) return BTLE_EINVAL;
+  const size_t n = std::min(cap, s->cands.size());
+  if (n) memcpy(out, s->cands.data(), n * sizeof(btle_conn_cand));
+  s->cands.erase(s->cands.begin(), s->cands.begin() + n);
+  *n_out = n;
+  return s->cands.empty() ? BTLE_OK : BTLE_EOVERFLOW;       // call again with more room
 }
 
 // ---- single capture: a one-capture session ----

@@ -426,3 +426,174 @@ def hop_events_ndjson(conns) -> str:
                      % (d["ts"], d["event"], d["state_from"], d["state_to"], d["ch"], d["freq_mhz"], d["aa"], d["crc_init"],
                         d["interval_us"], d["hop"], d["chm"]))
     return "\n".join(lines) + ("\n" if lines else "")
+
+
+# ---- live: every connection on a streaming session (DESIGN.md §6.4) -----------------------------------------------------
+class ConnectionMonitor:
+    """decode_connections() while the 40 channel captures are still arriving.  `session` is an RxStreams over 40 captures,
+    row c = BLE channel c (cfgs 0..39 as make_cfgs(40, channel=range(40))), fed only through this monitor.  It needs the
+    session's push, finish, add_cfg, remove_cfg, resident, set_discover and candidates.
+
+    Captures 37..39 keep their advertising cfg; the cfgs of 0..36 are removed and, with discover=True, discovery runs on
+    them.  After each hand-out of records, every CONNECT_REQ and every discovered (access address, CRC init) group that
+    has reached `min_events` events gets one cfg on each of the 37 data captures, from chunk `resident` on: the two sets
+    still on the device are decoded with it too (backfill).  A discovered group whose access address a CONNECT_REQ
+    announced is skipped, as in decode_connections().  Grouping is incremental with discover_connections()' rules; once
+    the captures have ended it gives the same connections.  Each connection carries `from_chunk` (its traffic starts
+    there: for a discovered connection, traffic before the set in front of the one in which it reached min_events is not
+    decoded) and `traffic`, in time order.  idle_s: a connection with no CRC-ok packet for that long stops being decoded
+    (`until_chunk`); None keeps every connection to the end, as decode_connections() does.  group_s: a candidate group
+    that has not reached min_events and has had no event for that long is forgotten, so that noise groups do not pile up
+    over a long session (the default, 8 s, is twice the longest connection interval; a group paused longer than that
+    starts again, where discover_connections() would continue it)."""
+
+    N_CAPTURES = 40
+
+    def __init__(self, session, min_events: int = 4, idle_s: float | None = None, discover: bool = True, group_s: float = 8.0):
+        self.session, self.min_events, self.idle_s, self.group_s = session, int(min_events), idle_s, group_s
+        for c in range(37):
+            session.remove_cfg(c)
+        if discover:
+            session.set_discover(list(range(37)) + [-1] * 3)
+        self._adv = []
+        self._creq, self._disc = [], {}          # CONNECT_REQ connections in arrival order; (aa, crc) -> discovered one
+        self._groups = {}                        # (aa, crc) -> [events [(t, channel)], n_candidates]
+        self._owner = {}                         # stable cfg index -> connection
+        self._t_now = 0.0
+
+    # ---- feeding ----
+    def push(self, capture: int, iq) -> np.ndarray:
+        """session.push(); returns the records handed out (advertising and connection cfgs alike)."""
+        recs = self.session.push(capture, iq)
+        self._hand_out(recs)
+        return recs
+
+    def finish(self) -> np.ndarray:
+        """session.finish(), repeated while connections found in the last records still get their backfill."""
+        out = []
+        while True:
+            recs = self.session.finish()
+            out.append(recs)
+            if not self._hand_out(recs):
+                return np.concatenate(out)
+
+    # ---- results ----
+    @property
+    def adv(self) -> np.ndarray:
+        """Advertising records handed out so far (stream = capture 37..39)."""
+        from ._native import REC_DTYPE
+        return np.concatenate(self._adv) if self._adv else np.zeros(0, dtype=REC_DTYPE)
+
+    def connections(self) -> list:
+        """decode_connections()' list so far: CONNECT_REQ connections in (advertising capture, time) order, then the
+        discovered ones by (t_first, access address); each with `from_chunk` and `traffic` (stream = channel)."""
+        creq = sorted(self._creq, key=lambda c: (c["adv_channel"], c["t"]))
+        disc = sorted((c for c in self._disc.values() if not c.get("_dropped")), key=lambda c: (c["t_first"], c["access_addr"]))
+        out = []
+        for c in creq + disc:
+            d = {k: v for k, v in c.items() if not k.startswith("_")}
+            d["traffic"] = self._traffic(c)
+            out.append(d)
+        return out
+
+    @staticmethod
+    def _traffic(c):
+        tr = np.concatenate(c["_traffic"])
+        t = tr["chunk"].astype(np.int64) * 8192 + tr["n0"]
+        tr = tr[np.lexsort((tr["channel"], t))].copy()
+        tr["stream"] = tr["channel"]
+        return tr
+
+    # ---- one hand-out ----
+    def _start(self, c, t_start):
+        s = self.session
+        frm = s.resident
+        c["from_chunk"], c["_cfgs"], c["_last_ok"] = frm, [], t_start
+        from ._native import REC_DTYPE
+        c["_traffic"] = [np.zeros(0, dtype=REC_DTYPE)]
+        for ch in range(37):
+            j, _ = s.add_cfg(ch, frm, channel=ch, access_addr=c["access_addr"], access_mask=0xFFFFFFFF, crc_init=c["crc_init"], raw=0, rssi=0)
+            c["_cfgs"].append(j)
+            self._owner[j] = c
+        return 37
+
+    def _stop(self, c):
+        for j in c.pop("_cfgs", []):
+            c["until_chunk"] = self.session.remove_cfg(j)
+
+    def _hand_out(self, recs) -> int:
+        """Records (and the candidates of the same sets) -> connections; returns the number of cfgs added."""
+        added = 0
+        if len(recs):
+            self._t_now = max(self._t_now, float((recs["chunk"].astype(np.int64) * 8192 + recs["n0"]).max()) / SAMPLE_RATE)
+        adv = recs[(recs["stream"] >= 37) & (recs["stream"] < self.N_CAPTURES)]
+        if len(adv):
+            self._adv.append(adv.copy())
+        for r in adv:
+            c = parse_connect_req(r)
+            if c is None:
+                continue
+            c["tracked"] = c["chm"] == "1fffffffff" and c["interval"] > 0
+            self._creq.append(c)
+            for d in self._disc.values():        # announced after all: the CONNECT_REQ connection takes it over
+                if d["access_addr"] == c["access_addr"] and not d.get("_dropped"):
+                    d["_dropped"] = True
+                    self._stop(d)
+            added += self._start(c, c["t"])
+        mine = recs[recs["stream"] >= self.N_CAPTURES]
+        if len(mine):
+            order = np.argsort(mine["stream"], kind="stable")
+            mine = mine[order]
+            cuts = np.flatnonzero(np.diff(mine["stream"])) + 1
+            for part in np.split(mine, cuts):
+                c = self._owner[int(part[0]["stream"])]
+                c["_traffic"].append(part.copy())
+                ok = part[part["crc_bad"] == 0]
+                if len(ok):
+                    c["_last_ok"] = max(c["_last_ok"], float((ok["chunk"].astype(np.int64) * 8192 + ok["n0"]).max()) / SAMPLE_RATE)
+        added += self._discover()
+        if self.idle_s is not None:
+            for c in self._creq + list(self._disc.values()):
+                if c.get("_cfgs") and self._t_now - c["_last_ok"] > self.idle_s:
+                    self._stop(c)
+        return added
+
+    def _discover(self) -> int:
+        cand = self.session.candidates()
+        changed = set()                          # groups with new events: only those can start or change a connection
+        if len(cand):
+            self._t_now = max(self._t_now, float(cand["sample"].max()) / SAMPLE_RATE)
+            # the sets' candidates all lie behind the previous hand-out's: grouping them in sample order continues the
+            # batch rule of discover_connections()
+            cand = cand[np.lexsort((cand["sample"], cand["crc_init"], cand["access_addr"]))]
+            key = cand["access_addr"].astype(np.int64) << 24 | cand["crc_init"].astype(np.int64)
+            for grp in np.split(cand, np.flatnonzero(np.diff(key)) + 1):
+                key_ = (int(grp[0]["access_addr"]), int(grp[0]["crc_init"]))
+                g = self._groups.setdefault(key_, [[], 0])
+                changed.add(key_)
+                events = g[0]
+                for r in grp:
+                    t, ch = int(r["sample"]) / SAMPLE_RATE, int(r["channel"])
+                    if events and ch == events[-1][1] and t - events[-1][0] < EVENT_SPAN_S:
+                        continue
+                    events.append((t, ch))
+                g[1] += len(grp)
+        if changed:
+            for key in [k for k, (ev, _) in self._groups.items() if len(ev) < self.min_events and self._t_now - ev[-1][0] > self.group_s]:
+                del self._groups[key]
+        added = 0
+        announced = {c["access_addr"] for c in self._creq}
+        for aa, crc in sorted(changed):
+            if (aa, crc) not in self._groups:
+                continue
+            events, n_cand = self._groups[(aa, crc)]
+            if len(events) < self.min_events or aa in announced:
+                continue
+            c = _connection_from_events(aa, crc, events, n_cand)
+            d = self._disc.get((aa, crc))
+            if d is None:
+                self._disc[(aa, crc)] = c
+                added += self._start(c, c["t_first"])
+            else:
+                d.update(c)
+        return added

@@ -383,6 +383,45 @@ class RxStreams:
         self._rx._check(self._L.btle_b200_streams_set_cfg(self._h, int(stream), c.ctypes.data))
         self._cfgs[int(stream)] = c[0]
 
+    # ---- per-capture cfg lists and discovery (btle_b200_streams_add_cfg / remove_cfg / set_discover) -------------------
+    @property
+    def resident(self) -> int:
+        """First chunk of the oldest segment set still on the device: the smallest from_chunk add_cfg() accepts."""
+        v = ctypes.c_int64(0)
+        self._rx._check(self._L.btle_b200_streams_resident(self._h, ctypes.byref(v)))
+        return v.value
+
+    def add_cfg(self, capture: int, from_chunk: int | None = None, **cfg) -> tuple:
+        """One more cfg on capture `capture`: capture's own cfg with the given fields (make_cfgs names) changed, decoding
+        chunks >= from_chunk (None: `resident`, so the sets still on the device are decoded with it too).  Returns
+        (index, from_chunk); records of this cfg carry `stream` = index.  Records of resident sets come back from the
+        next push() or finish()."""
+        capture = int(capture)
+        c = self._cfgs[capture:capture + 1].copy() if 0 <= capture < self.n_streams else make_cfgs(1)
+        for k, v in cfg.items():
+            c[k] = v
+        frm = self.resident if from_chunk is None else int(from_chunk)
+        idx = ctypes.c_size_t(0)
+        self._rx._check(self._L.btle_b200_streams_add_cfg(self._h, capture, c.ctypes.data, frm, ctypes.byref(idx)))
+        return idx.value, frm
+
+    def remove_cfg(self, index: int) -> int:
+        """Cfg `index` decodes no chunk from the next submitted segment set on; returns that set's first chunk."""
+        v = ctypes.c_int64(0)
+        self._rx._check(self._L.btle_b200_streams_remove_cfg(self._h, int(index), ctypes.byref(v)))
+        return v.value
+
+    def set_discover(self, channels) -> None:
+        """channels[i]: data channel 0..36 scanned for connection candidates on capture i, or -1; from the next set on."""
+        ch = np.ascontiguousarray(np.broadcast_to(np.asarray(channels, dtype=np.int32), (self.n_streams,)))
+        self._rx._check(self._L.btle_b200_streams_set_discover(self._h, ch.ctypes.data))
+
+    def candidates(self) -> np.ndarray:
+        """Discovery candidates (CAND_DTYPE) of the sets handed out since the last call, per set by (stream, sample);
+        `sample` counted from the capture's start, `stream` = capture index."""
+        buf = np.empty(16384, dtype=CAND_DTYPE)
+        return self._rx._drain(self._L.btle_b200_streams_take_cands, self._h, buf)
+
     def finish(self) -> np.ndarray:
         """End of the captures: decodes up to the shortest one and returns every record still waiting."""
         out = self._rx._drain(self._L.btle_b200_streams_finish, self._h, self._buf)

@@ -265,6 +265,37 @@ int btle_b200_discover_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_s
 int btle_b200_discover(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stream_stride_int8, size_t n_int8,
                        const int32_t *channels, btle_conn_cand *out, size_t cap, size_t *n_out);
 
+/* ---- connections on a streaming session (btle_b200_streams_*): per-capture cfg lists, backfill, discovery -----------
+ * Every cfg of a session has a stable index, never reused: the n_streams cfgs of btle_b200_streams_open are 0..n-1 (cfg
+ * i decodes capture i), each added cfg gets the next one.  A record's `stream` is that index.  The records of cfg j equal
+ * btle_b200_rx_batch() on cfg j's capture (cut to the shortest capture) decoded with cfg j, kept for
+ * from_chunk <= chunk < until_chunk; each is returned exactly once, per set in (j, chunk, n0) order.
+ * While no cfg was added or removed a set is decoded by the one single-cfg launch described above.  After that, a set's
+ * live cfgs are sorted by capture and decoded by btle_b200_rx_multi_device_dir launches, in rounds of at most
+ * BTLE_MAX_CFGS_PER_CAPTURE cfgs per capture; a capture no live cfg names is not read by the kernel.
+ * BACKFILL: the two most recent sets stay on the device (the one whose records were handed out last, and the one in
+ * flight).  add_cfg accepts any from_chunk >= btle_b200_streams_resident(); the next commit or finish call decodes every
+ * cfg added since the last one over the resident sets that hold chunks >= its from_chunk (rounds of at most
+ * BTLE_MAX_CFGS_PER_CAPTURE cfgs per capture, one launch each), and those records are handed out by that call or, for
+ * the set in flight, with it (finish returns them until none wait; btle_b200_last_launches counts these launches too).
+ * add_cfg does no GPU work: it fails only on bad arguments, and then adds nothing.  from_chunk < resident() is
+ * BTLE_EINVAL, the session stays usable.  Device record buffers are sized per launch for BTLE_MAX_RECS_PER_CHUNK records
+ * per chunk and cfg and reused by later launches; page-locked host memory holds only the records found. */
+int btle_b200_streams_add_cfg(btle_b200_streams *s, size_t capture, const btle_stream_cfg *cfg, int64_t from_chunk, size_t *index);
+/* cfg `index` decodes no chunk from the next submitted set on; *until_chunk = first chunk it no longer decodes.
+ * An index out of range or already removed is BTLE_EINVAL. */
+int btle_b200_streams_remove_cfg(btle_b200_streams *s, size_t index, int64_t *until_chunk);
+/* first chunk of the oldest set whose IQ is still on the device: the smallest from_chunk add_cfg accepts */
+int btle_b200_streams_resident(const btle_b200_streams *s, int64_t *first_chunk);
+/* DISCOVERY: channels[i] = data channel 0..36 of capture i, or -1 (not scanned); applies from the next submitted set.
+ * Each set's scanned parts (lead, segment and look-ahead) go through discover_kernel; the candidates whose window starts
+ * in the segment are kept, with `sample` counted from the capture's start and `stream` = capture index.  The union over
+ * the sets equals btle_b200_discover() on the whole captures cut to the shortest one; no candidate is dropped. */
+int btle_b200_streams_set_discover(btle_b200_streams *s, const int32_t *channels);
+/* candidates of the sets handed out so far, per set sorted by (stream, sample); taken ones are not returned again.
+ * BTLE_EOVERFLOW when more wait than `cap` holds: call again. */
+int btle_b200_streams_take_cands(btle_b200_streams *s, btle_conn_cand *out, size_t cap, size_t *n_out);
+
 /* number of kernels the last rx call launched (bench.py's gpu_launches) */
 int btle_b200_last_launches(const btle_b200_ctx *ctx);
 
