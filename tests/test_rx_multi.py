@@ -3,6 +3,7 @@
 import ctypes
 import os
 import subprocess
+import time
 
 import numpy as np
 import pytest
@@ -130,6 +131,22 @@ def test_multi_cfg_unit_path_equals_oracle_per_cfg(case):
         got = emul_rx_multi(iq, cfgs, capture, grid=grid)
         assert got.tobytes() == exp.tobytes(), (grid, len(got), len(exp))
     assert len(exp) > 0
+
+
+def test_multi_cfg_unit_path_fuzz_equals_oracle_per_cfg():
+    """Random launches of tests/multi_fuzz.py (the generator of tools/fuzz_multi_gpu.py, at most 12 captures of 16
+    chunks) for about 15 s, each at grid 132 and at a random grid, against the oracle per cfg."""
+    from multi_fuzz import draw
+    rng = np.random.default_rng(20261016)
+    t0, n, recs = time.time(), 0, 0
+    while time.time() - t0 < 15 or n < 20:
+        iq, cfgs, capture = draw(rng, max_captures=12, max_chunks=16)
+        exp = oracle_multi(iq, cfgs, capture)
+        for grid in (132, int(rng.integers(1, 300))):
+            got = emul_rx_multi(iq, cfgs, capture, grid=grid)
+            assert got.tobytes() == exp.tobytes(), (n, grid, iq.shape, cfgs.tolist(), capture.tolist(), len(got), len(exp))
+        n, recs = n + 1, recs + len(exp)
+    assert recs > 1000
 
 
 def test_tapset_prefilter_equals_prefilter_any():
