@@ -37,6 +37,15 @@ BER_CFG_DTYPE = np.dtype([("seed", "<u8"), ("snr_db", "<f4"), ("ppm", "<f4"), ("
                           ("reserved", "<u4")])
 BER_RESULT_DTYPE = np.dtype([("packets", "<u8"), ("pkt_err", "<u8"), ("bit_err", "<u8"), ("bit_total", "<u8"), ("aa_miss", "<u8"), ("seconds", "<f8")])
 assert BER_CFG_DTYPE.itemsize == 32 and BER_RESULT_DTYPE.itemsize == 48
+# btle_rx_ber_cfg (48 bytes), btle_rx_ber_truth (64 bytes), btle_rx_ber_result (88 bytes): error rates of the 4-Msps receiver
+RX_BER_CFG_DTYPE = np.dtype([("seed", "<u8"), ("snr_db", "<f4"), ("ppm", "<f4"), ("cfo_hz", "<f4"), ("amplitude", "<i4"), ("slot_samples", "<i4"),
+                             ("channel", "<i4"), ("access_addr", "<u4"), ("crc_init", "<u4"), ("reserved", "<u4", 2)])
+RX_BER_TRUTH_DTYPE = np.dtype([("aa_sample", "<i8"), ("offset", "<i4"), ("clipped", "<u4"), ("n_bytes", "u1"), ("delta4", "u1"), ("pdu", "u1", 39),
+                               ("reserved", "u1", 7)])
+RX_BER_COUNTERS = ("packets", "pkt_err", "bit_err", "bit_total", "aa_miss", "len_reject", "crc_ok_wrong", "extra_recs", "extra_crc_ok", "clipped")
+RX_BER_RESULT_DTYPE = np.dtype([(k, "<u8") for k in RX_BER_COUNTERS] + [("seconds", "<f8")])
+assert RX_BER_CFG_DTYPE.itemsize == 48 and RX_BER_TRUTH_DTYPE.itemsize == 64 and RX_BER_RESULT_DTYPE.itemsize == 88
+RX_BER_MAX_SLOT, RX_BER_MAX_UNITS = 12000, 12272       # BTLE_RX_BER_MAX_SLOT, BTLE_RX_BER_MAX_UNITS
 SPS8_REC_DTYPE = np.dtype([("sample", "<i8"), ("window", "<i8"), ("rx", MODEL_REC_DTYPE)])     # btle_sps8_rec
 # btle_conn_cand, 32 bytes: an empty-PDU candidate of connection discovery
 CAND_DTYPE = np.dtype([("sample", "<i8"), ("stream", "<i4"), ("access_addr", "<u4"), ("crc_init", "<u4"), ("channel", "u1"),
@@ -53,7 +62,7 @@ EXPORTS = [
     "btle_b200_dbits", "btle_b200_gfsk_demod_i16", "btle_b200_search_bit_sequence", "btle_b200_crc24_bits",
     "btle_b200_scramble_bits", "btle_b200_model_rx_batch_device", "btle_b200_model_rx_batch",
     "btle_b200_tx_modulate_device", "btle_b200_rx_iq16", "btle_b200_synth_streams_device", "btle_b200_rx_sps8", "btle_b200_sps8_hits_device", "btle_b200_ber_run",
-    "btle_b200_ber_synth_device",
+    "btle_b200_ber_synth_device", "btle_b200_rx_ber_run", "btle_b200_rx_ber_synth_device", "btle_b200_rx_ber_score_device",
     "btle_b200_stream_open", "btle_b200_stream_push", "btle_b200_stream_acquire", "btle_b200_stream_commit", "btle_b200_stream_finish",
     "btle_b200_stream_close", "btle_b200_stream_set_cfg",
     "btle_b200_streams_open", "btle_b200_streams_acquire", "btle_b200_streams_commit", "btle_b200_streams_set_cfg",
@@ -127,6 +136,9 @@ def load():
     L.btle_b200_rx_iq16.argtypes = [vp, vp, sz, i32, vp, vp, sz, ctypes.POINTER(sz)]
     L.btle_b200_ber_run.argtypes = [vp, vp, sz, vp]
     L.btle_b200_ber_synth_device.argtypes = [vp, vp, ctypes.c_uint64, sz, vp, vp, vp, vp]
+    L.btle_b200_rx_ber_run.argtypes = [vp, vp, sz, vp]
+    L.btle_b200_rx_ber_synth_device.argtypes = [vp, vp, ctypes.c_uint64, sz, vp, vp, vp]
+    L.btle_b200_rx_ber_score_device.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, vp]
     L.btle_b200_sps8_hits_device.argtypes = [vp, vp, sz, u32, vp, sz, vp, vp]
     L.btle_b200_rx_sps8.argtypes = [vp, vp, sz, i32, u32, u32, vp, sz, ctypes.POINTER(sz)]
     L.btle_b200_synth_streams_device.argtypes = [vp, vp, sz, sz, sz, vp, vp, vp, sz, ctypes.POINTER(sz), vp]

@@ -1376,8 +1376,214 @@ __global__ void ber_score_kernel(const btle_model_rx_rec *__restrict__ rec, cons
   }
 }
 
+// ---- error rates of the 4-Msps receive chain (btle_b200_rx_ber_*; the definition is in include/btle_b200.h) -----------
+// One CTA per slot of the capture: the packet from hashes (build_air), the btle_tx PHY at 4 sps (gfsk_block<4>) scaled
+// into shared memory, then every sample of the slot: resampling at (m - delta)(1 + e), the carrier rotation, AWGN, rintf
+// and int8 saturation, stored straight into the capture.  Slots at or behind n_live (global index) and samples at or
+// behind n_samples are not packets; slots from n_truth on (relative to the capture) write no truth row.
+constexpr int kRxBerPduAdv = 39, kRxBerPduData = 29, kRxBerMaxL = 32 * (1 + 4 + kRxBerPduAdv + 3) + 16;   // 1520
+__host__ __device__ __forceinline__ int rx_ber_pdu_bytes(int channel) { return channel >= 37 ? kRxBerPduAdv : kRxBerPduData; }
+__host__ __device__ __forceinline__ int rx_ber_len(int channel) { return 32 * (1 + 4 + rx_ber_pdu_bytes(channel) + 3) + 16; }
+__global__ void __launch_bounds__(256)
+rx_ber_synth_kernel(const btle_rx_ber_cfg cfg, unsigned long long first, unsigned long long n_live, long long n_samples,
+                    long long n_truth, int8_t *__restrict__ iq, btle_rx_ber_truth *__restrict__ truth) {
+  __shared__ uint8_t sb[64];
+  __shared__ float txi[kRxBerMaxL], txq[kRxBerMaxL];
+  __shared__ int s_off, s_delta4;
+  __shared__ unsigned s_clipped;
+  const long long slot = blockIdx.x;
+  const unsigned long long gk = first + (unsigned long long)slot;
+  const int S = cfg.slot_samples, L = rx_ber_len(cfg.channel), tid = threadIdx.x;
+  const bool live = gk < n_live;
+  if (tid == 0) {
+    s_clipped = 0;
+    const uint64_t r = draw(cfg.seed, gk, 0, 12);
+    s_off = (int)(r % (uint64_t)(S - L + 1));
+    s_delta4 = (int)((r >> 32) & 3);
+    if (live) {
+      const int nb = rx_ber_pdu_bytes(cfg.channel);
+      uint8_t pdu[kRxBerPduAdv];
+      if (cfg.channel >= 37) { pdu[0] = 0x42; pdu[1] = 0x25; }          // the PDU of btle_b200_ber_run
+      else { pdu[0] = 0x02; pdu[1] = kRxBerPduData - 2; }                 // LL data, LLID 2, length 27
+      for (int b = 2; b < nb; ++b) pdu[b] = (uint8_t)(draw(cfg.seed, gk, (uint64_t)(b >> 3), 9) >> (8 * (b & 7)));
+      build_air(pdu, nb, cfg.access_addr, crc_init_reorder(cfg.crc_init), cfg.channel, -1, sb, 64);
+      if (slot < n_truth) {
+        btle_rx_ber_truth t;
+        memset(&t, 0, sizeof t);
+        const double e = (double)cfg.ppm * 1e-6;
+        t.aa_sample = slot * S + s_off + (long long)floor(BTLE_RX_BER_AA_OFFSET / (1.0 + e) + 0.25 * s_delta4 + 0.5);
+        t.offset = s_off;
+        t.n_bytes = (uint8_t)nb;
+        t.delta4 = (uint8_t)s_delta4;
+        for (int b = 0; b < nb; ++b) t.pdu[b] = pdu[b];
+        truth[slot] = t;
+      }
+    }
+  }
+  __syncthreads();
+  const float scale = (float)cfg.amplitude / 127.0f;
+  if (live) {                                                  // 256 threads x 8 samples >= 1520 samples: one pass
+    gfsk_block<4, 256>(sb, (L - 16) / 4, L, [&](int m, int ph) {
+      txi[m] = (float)c_cos1024[ph] * scale;
+      txq[m] = (float)c_sin1024[ph] * scale;
+    });
+  }
+  const double e = (double)cfg.ppm * 1e-6, delta = 0.25 * s_delta4;
+  // turns per sample: the ppm's carrier error at the new sampling time (1 + e) / 4 Msps, plus the extra offset
+  const double rate = e * 2450e6 * (0.25e-6 * (1.0 + e)) + (double)cfg.cfo_hz / 4e6;
+  const float sigma = (float)cfg.amplitude / exp10f(cfg.snr_db / 20.0f) * 0.70710678f;
+  const int off = s_off;
+  const long long s0 = slot * S;
+  const int n_here = (int)min((long long)S, n_samples - s0);
+  unsigned clipped = 0;
+  for (int j = tid; j < n_here; j += blockDim.x) {
+    float vi = 0.0f, vq = 0.0f;
+    const int m = j - off;
+    if (live && m >= 0 && m < L) {
+      const double x = ((double)m - delta) * (1.0 + e);
+      if (x <= 0.0) { vi = txi[0]; vq = txq[0]; }                   // np.interp: clamped at both ends
+      else {
+        const int k = (int)x;
+        if (k >= L - 1) { vi = txi[L - 1]; vq = txq[L - 1]; }
+        else {
+          const float fr = (float)(x - (double)k);
+          vi = txi[k] + (txi[k + 1] - txi[k]) * fr;
+          vq = txq[k] + (txq[k + 1] - txq[k]) * fr;
+        }
+      }
+      if (rate != 0.0) {
+        double turns = rate * (double)m;
+        turns -= floor(turns);
+        float sn, cs;
+        sincospif(2.0f * (float)turns, &sn, &cs);
+        const float ri = vi * cs - vq * sn, rq = vi * sn + vq * cs;
+        vi = ri; vq = rq;
+      }
+    }
+    const float2 g = gauss_pair(draw(cfg.seed, gk, (uint64_t)j, 11));
+    const float ri = rintf(vi + sigma * g.x), rq = rintf(vq + sigma * g.y);
+    const int ii = (int)fminf(fmaxf(ri, -128.0f), 127.0f), qq = (int)fminf(fmaxf(rq, -128.0f), 127.0f);
+    clipped += (ri < -128.0f || ri > 127.0f || rq < -128.0f || rq > 127.0f) ? 1u : 0u;
+    reinterpret_cast<uint16_t *>(iq)[s0 + j] = (uint16_t)((uint32_t)(ii & 0xFF) | ((uint32_t)(qq & 0xFF) << 8));
+  }
+  if (live && slot < n_truth) {
+    for (int d = 16; d; d >>= 1) clipped += __shfl_down_sync(0xFFFFFFFFu, clipped, d);
+    if ((tid & 31) == 0 && clipped) atomicAdd(&s_clipped, clipped);
+    __syncthreads();
+    if (tid == 0) truth[slot].clipped = s_clipped;
+  }
+}
+
+// One thread per packet: its record is found in the launch's records through the unit directory, whose walk is the
+// reference order, (chunk, n0): an exclusive prefix of the directory counts in shared memory maps a position of that
+// order to its unit, a binary search finds the first record of the lowest chunk that can hold a match, and the records
+// from there on are read until the highest one.  The CTAs also share a pass over the stored records, which counts the
+// records and the CRC-ok ones; matched ones are taken off, so extra_recs / extra_crc_ok add up without a per-record
+// match table.  One atomic per warp and counter, as ber_score_kernel.
+__global__ void __launch_bounds__(256)
+rx_ber_score_kernel(const btle_rx_ber_truth *__restrict__ truth, int n, const btle_pkt_rec *__restrict__ recs, unsigned long long n_recs,
+                    const uint2 *__restrict__ dir, int n_units, unsigned long long *__restrict__ acc /* btle_rx_ber_result */) {
+  extern __shared__ unsigned rx_ber_pre[];                    // [n_units + 1]: records before unit u in the walk
+  __shared__ unsigned warp_sum[8];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  {
+    const int per = (n_units + 255) / 256, u0 = min(n_units, tid * per), u1 = min(n_units, u0 + per);
+    unsigned s = 0;
+    for (int u = u0; u < u1; ++u) s += __ldg(&dir[u].y);
+    unsigned incl = s;
+    for (int d = 1; d < 32; d <<= 1) {
+      const unsigned v = __shfl_up_sync(0xFFFFFFFFu, incl, d);
+      if (lane >= d) incl += v;
+    }
+    if (lane == 31) warp_sum[warp] = incl;
+    __syncthreads();
+    unsigned run = incl - s;
+    for (int w = 0; w < warp; ++w) run += warp_sum[w];
+    for (int u = u0; u < u1; ++u) { rx_ber_pre[u] = run; run += __ldg(&dir[u].y); }
+    if (tid == 255) rx_ber_pre[n_units] = run;
+    __syncthreads();
+  }
+  const unsigned total = rx_ber_pre[n_units];
+  // position i of the walk -> index into recs (or ~0ull when that record was not stored)
+  auto at = [&](unsigned i) -> unsigned long long {
+    int lo = 0, hi = n_units - 1;                            // last unit with pre <= i
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (rx_ber_pre[mid] <= i) lo = mid; else hi = mid - 1;
+    }
+    const unsigned long long r = (unsigned long long)__ldg(&dir[lo].x) + (i - rx_ber_pre[lo]);
+    return r < n_recs ? r : ~0ull;
+  };
+  unsigned long long c[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};   // btle_rx_ber_result's counters, in its order
+  long long matched = 0, matched_ok = 0;
+  const int p = blockIdx.x * blockDim.x + tid;
+  if (p < n) {
+    const btle_rx_ber_truth &t = truth[p];
+    const long long a = t.aa_sample;
+    const int nb = t.n_bytes;
+    const long long c_lo = (a - BTLE_RX_BER_MATCH) / kChunkSamples;                     // n0 <= 8191
+    const long long c_hi = (a + BTLE_RX_BER_MATCH + 124) / kChunkSamples;               // n0 >= -124
+    unsigned lo = 0, hi = total;                               // first position whose chunk >= c_lo
+    while (lo < hi) {
+      const unsigned mid = (lo + hi) >> 1;
+      const unsigned long long r = at(mid);
+      if (r != ~0ull && recs[r].chunk < c_lo) lo = mid + 1; else hi = mid;
+    }
+    const btle_pkt_rec *m = nullptr;
+    for (unsigned i = lo; i < total; ++i) {
+      const unsigned long long r = at(i);
+      if (r == ~0ull) break;
+      const btle_pkt_rec &x = recs[r];
+      if (x.chunk > c_hi) break;
+      const long long pos = (long long)x.chunk * kChunkSamples + x.n0;
+      if (pos >= a - BTLE_RX_BER_MATCH && pos <= a + BTLE_RX_BER_MATCH) { m = &x; break; }
+    }
+    c[0] = 1;
+    c[3] = 8ull * nb;
+    c[9] = t.clipped;
+    const bool rejected = m && (m->flags & BTLE_REC_REJECTED);
+    const bool ok = m && !rejected && !m->crc_bad;
+    int common = 0;
+    if (m) {
+      ++matched;
+      common = min(rejected ? 2 : (int)m->n_bytes - 3, nb);
+      if (common < 0) common = 0;
+    }
+    if (ok) {
+      ++matched_ok;
+      bool same = (int)m->n_bytes - 3 == nb;
+      for (int b = 0; b < nb && same; ++b) same = m->bytes[b] == t.pdu[b];
+      c[6] = same ? 0 : 1;
+    } else {
+      c[1] = 1;
+      if (!m) { c[4] = 1; c[2] = 8ull * nb; }
+      else {
+        c[5] = rejected ? 1 : 0;
+        unsigned err = 0;
+        for (int b = 0; b < common; ++b) err += __popc((unsigned)(m->bytes[b] ^ t.pdu[b]));
+        c[2] = err;
+      }
+    }
+  }
+  // every stored record once, over the CTAs: counted here, matched ones taken off above
+  const unsigned long long stored = min((unsigned long long)total, n_recs);
+  long long nrec = 0, nok = 0;
+  for (unsigned long long r = (unsigned long long)blockIdx.x * blockDim.x + tid; r < stored; r += (unsigned long long)gridDim.x * blockDim.x) {
+    ++nrec;
+    if (!(recs[r].flags & BTLE_REC_REJECTED) && !recs[r].crc_bad) ++nok;
+  }
+  c[7] = (unsigned long long)(nrec - matched);                 // may be "negative" per thread; the sums are exact modulo 2^64
+  c[8] = (unsigned long long)(nok - matched_ok);
+#pragma unroll
+  for (int k = 0; k < 10; ++k) {
+    unsigned long long v = c[k];
+    for (int d = 16; d; d >>= 1) v += __shfl_down_sync(0xFFFFFFFFu, v, d);
+    if (lane == 0 && v) atomicAdd(&acc[k], v);
+  }
+}
+
 // btlelib.btle_rx for a batch of packet windows: one warp per packet (see include/btle_b200.h).
-constexpr int kModelMaxWords = 64;                         // <= 2048 symbols per window
+constexpr int kModelMaxWords = 64;                        // <= 2048 symbols per window
 // Sample a of packet p sits at g{i,q}[(base(p) + a) * elem_stride], base(p) = win_off ? win_off[p] : p * n_samples:
 // a planar batch (elem_stride 1) or windows cut out of one interleaved int16 capture (gi = iq, gq = iq + 1, elem_stride 2).
 __global__ void __launch_bounds__(128)
@@ -3267,6 +3473,148 @@ int btle_b200_ber_synth_device(btle_b200_ctx *ctx, const btle_ber_cfg *cfg, uint
       *cfg, (unsigned long long)first_packet, (int)n_packets, d_i, d_q, d_truth);
   BTLE_CUDA(ctx, cudaGetLastError());
   ctx->last_launches = 1;
+  return BTLE_OK;
+}
+
+static_assert(sizeof(btle_rx_ber_cfg) == 48 && sizeof(btle_rx_ber_truth) == 64 && sizeof(btle_rx_ber_result) == 88,
+              "include/btle_b200.h documents these sizes");
+static_assert(kRxBerMaxL == 1520 && BTLE_RX_BER_MAX_SLOT / 16 * 16 + 16 <= BTLE_RX_BER_MAX_UNITS,
+              "a run's smallest batch (lcm(slot, 8192) samples) has a directory rx_ber_score_kernel takes");
+static int check_rx_ber_cfg(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg) {
+  if (cfg->channel < 0 || cfg->channel > 39) { ctx->err = "rx_ber: channel must be 0..39"; return BTLE_EINVAL; }
+  if (!std::isfinite(cfg->snr_db) || !std::isfinite(cfg->ppm) || !std::isfinite(cfg->cfo_hz)) {
+    ctx->err = "rx_ber: snr_db, ppm and cfo_hz must be finite";
+    return BTLE_EINVAL;
+  }
+  if (std::fabs(cfg->ppm) >= 1e6f) { ctx->err = "rx_ber: ppm must have |ppm| < 1e6"; return BTLE_EINVAL; }
+  if (cfg->amplitude < 1 || cfg->amplitude > 127) { ctx->err = "rx_ber: amplitude must be 1..127"; return BTLE_EINVAL; }
+  if (cfg->slot_samples < rx_ber_len(cfg->channel) || cfg->slot_samples > BTLE_RX_BER_MAX_SLOT) {
+    ctx->err = "rx_ber: slot_samples must hold the packet (" + std::to_string(rx_ber_len(cfg->channel)) + " samples on this channel) and be at most " +
+               std::to_string(BTLE_RX_BER_MAX_SLOT);
+    return BTLE_EINVAL;
+  }
+  return BTLE_OK;
+}
+
+// capture of `n_samples` samples from slot `first` on (packets while the global slot index is below n_live, truth rows
+// for the first n_truth slots)
+static int launch_rx_ber_synth(btle_b200_ctx *ctx, const btle_rx_ber_cfg &cfg, uint64_t first, uint64_t n_live, long long n_samples,
+                               long long n_truth, int8_t *d_iq, btle_rx_ber_truth *d_truth, cudaStream_t st) {
+  const long long slots = (n_samples + cfg.slot_samples - 1) / cfg.slot_samples;
+  if (slots > 0x7FFFFFFFll) { ctx->err = "rx_ber: too many slots for one launch"; return BTLE_EINVAL; }
+  rx_ber_synth_kernel<<<(unsigned)slots, 256, 0, st>>>(cfg, first, n_live, n_samples, n_truth, d_iq, d_truth);
+  BTLE_CUDA(ctx, cudaGetLastError());
+  return BTLE_OK;
+}
+
+static int launch_rx_ber_score(btle_b200_ctx *ctx, const btle_rx_ber_truth *d_truth, size_t n_packets, const btle_pkt_rec *d_recs, size_t n_recs,
+                               const btle_unit_dir *d_dir, size_t n_units, btle_rx_ber_result *d_result, cudaStream_t st) {
+  const unsigned grid = (unsigned)std::max<size_t>(1, (n_packets + 255) / 256);
+  rx_ber_score_kernel<<<grid, 256, (n_units + 1) * sizeof(unsigned), st>>>(d_truth, (int)n_packets, d_recs, (unsigned long long)n_recs,
+                                                                         reinterpret_cast<const uint2 *>(d_dir), (int)n_units,
+                                                                         reinterpret_cast<unsigned long long *>(d_result));
+  BTLE_CUDA(ctx, cudaGetLastError());
+  return BTLE_OK;
+}
+
+int btle_b200_rx_ber_synth_device(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg, uint64_t first_packet, size_t n_packets, int8_t *d_iq,
+                                  btle_rx_ber_truth *d_truth, void *cuda_stream) {
+  if (!ctx) return BTLE_EINVAL;
+  if (!cfg || (n_packets && (!d_iq || !d_truth))) { ctx->err = "rx_ber_synth: missing buffer"; return BTLE_EINVAL; }
+  int rc = check_rx_ber_cfg(ctx, cfg);
+  if (rc) return rc;
+  if (reinterpret_cast<uintptr_t>(d_iq) & 15) { ctx->err = "device IQ must be 16-byte aligned"; return BTLE_EINVAL; }
+  if (!n_packets) return BTLE_OK;
+  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
+  const long long n_samples = (long long)(BTLE_RX_BER_CAPTURE_INT8(n_packets, cfg->slot_samples) / 2);
+  rc = launch_rx_ber_synth(ctx, *cfg, first_packet, first_packet + n_packets, n_samples, (long long)n_packets, d_iq, d_truth,
+                           reinterpret_cast<cudaStream_t>(cuda_stream));
+  if (rc) return rc;
+  ctx->last_launches = 1;
+  return BTLE_OK;
+}
+
+int btle_b200_rx_ber_score_device(btle_b200_ctx *ctx, const btle_rx_ber_truth *d_truth, size_t n_packets, const btle_pkt_rec *d_recs,
+                                  size_t n_recs, const btle_unit_dir *d_dir, size_t n_units, btle_rx_ber_result *d_result,
+                                  void *cuda_stream) {
+  if (!ctx) return BTLE_EINVAL;
+  if (!d_result || (n_packets && !d_truth) || (n_recs && !d_recs) || (n_units && !d_dir)) { ctx->err = "rx_ber_score: missing buffer"; return BTLE_EINVAL; }
+  if (n_units > BTLE_RX_BER_MAX_UNITS) { ctx->err = "rx_ber_score: more than BTLE_RX_BER_MAX_UNITS directory entries"; return BTLE_EINVAL; }
+  if (n_packets > 0x7FFFFFFFu) { ctx->err = "rx_ber_score: too many packets for one launch"; return BTLE_EINVAL; }
+  if (!n_packets && !n_units) return BTLE_OK;
+  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
+  const int rc = launch_rx_ber_score(ctx, d_truth, n_packets, d_recs, n_recs, d_dir, n_units, d_result, reinterpret_cast<cudaStream_t>(cuda_stream));
+  if (rc) return rc;
+  ctx->last_launches = 1;
+  return BTLE_OK;
+}
+
+// Batches of B packets, B a multiple of 8192 / gcd(S, 8192): every batch but the last covers whole chunks and ends on a
+// slot boundary, so its capture is the run's one long capture from its first chunk on, and its look-ahead behind the last
+// chunk (BTLE_LOOKAHEAD_INT8) is written with the slots that follow.  The receiver decodes a chunk from that chunk and its
+// look-ahead alone (zeroed history at each chunk), so every batch's records are the long capture's records of its
+// chunks, and the counts do not depend on B.
+int btle_b200_rx_ber_run(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg, size_t n_packets, btle_rx_ber_result *out) {
+  if (!ctx) return BTLE_EINVAL;
+  if (!cfg || !out) { ctx->err = "rx_ber_run: missing argument"; return BTLE_EINVAL; }
+  memset(out, 0, sizeof *out);
+  int rc = check_rx_ber_cfg(ctx, cfg);
+  if (rc) return rc;
+  if (!n_packets) return BTLE_OK;
+  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const long long S = cfg->slot_samples;
+  long long g = kChunkSamples, b = S;
+  while (b) { const long long t = g % b; g = b; b = t; }
+  const long long q = kChunkSamples / g;                     // packets of the smallest batch: lcm(S, 8192) / S
+  size_t free_b = 0, total_b = 0;
+  BTLE_CUDA(ctx, cudaMemGetInfo(&free_b, &total_b));
+  const size_t per_chunk = kChunkInt8 + BTLE_MAX_RECS_PER_CHUNK * sizeof(btle_pkt_rec) + 8 * sizeof(btle_rx_ber_truth);
+  const long long want_chunks = (long long)std::min<size_t>(8192, std::max<size_t>(1, free_b / 2 / per_chunk));
+  const long long B = std::max(1ll, want_chunks * kChunkSamples / (q * S)) * q;
+  const size_t max_b = std::min<size_t>(n_packets, (size_t)B);
+  const long long max_chunks = ((long long)max_b * S + kChunkSamples - 1) / kChunkSamples;
+  const size_t max_int8 = (size_t)max_chunks * kChunkInt8 + BTLE_LOOKAHEAD_INT8, max_recs = (size_t)max_chunks * BTLE_MAX_RECS_PER_CHUNK;
+  if (ctx->d_iq.reserve(ctx, max_int8) || ctx->d_out.reserve(ctx, max_recs) ||
+      ctx->d_dir.reserve(ctx, (size_t)(max_chunks + kSpanChunks - 1) / kSpanChunks * kSpanChunks))   // >= units of any batch
+    return BTLE_ENOMEM;
+  btle_rx_ber_truth *d_truth;
+  btle_rx_ber_result *d_res;
+  rc = leaf_layout(ctx, piece(d_truth, max_b), piece(d_res, 1));
+  if (rc) return rc;
+  BTLE_CUDA(ctx, cudaMemsetAsync(d_res, 0, sizeof(btle_rx_ber_result), st));
+  struct Timing {                                           // the two events are destroyed on every return
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    ~Timing() { if (e0) cudaEventDestroy(e0); if (e1) cudaEventDestroy(e1); }
+  } t;
+  BTLE_CUDA(ctx, cudaEventCreate(&t.e0));
+  BTLE_CUDA(ctx, cudaEventCreate(&t.e1));
+  BTLE_CUDA(ctx, cudaEventRecord(t.e0, st));
+  const btle_stream_cfg scfg{cfg->channel, cfg->access_addr, 0xFFFFFFFFu, cfg->crc_init, 0, BTLE_CFG_REPORT_REJECTED};
+  int launches = 0;
+  for (size_t done = 0; done < n_packets; done += max_b) {
+    const size_t n = std::min(max_b, n_packets - done);
+    const bool last = done + n == n_packets;
+    const long long chunks = ((long long)n * S + kChunkSamples - 1) / kChunkSamples;
+    const size_t n_int8 = (size_t)chunks * kChunkInt8 + (last ? 0 : BTLE_LOOKAHEAD_INT8);
+    rc = launch_rx_ber_synth(ctx, *cfg, done, n_packets, (long long)(n_int8 / 2), (long long)n, ctx->d_iq, d_truth, st);
+    if (rc) return rc;
+    const size_t cap = (size_t)chunks * BTLE_MAX_RECS_PER_CHUNK, units = btle_b200_rx_units(ctx, 1, n_int8);
+    rc = launch_rx(ctx, ctx->d_iq, 1, n_int8, n_int8, &scfg, ctx->d_out, cap, ctx->d_count, ctx->d_dir, st);
+    if (rc) return rc;
+    rc = launch_rx_ber_score(ctx, d_truth, n, ctx->d_out, cap, ctx->d_dir, units, d_res, st);
+    if (rc) return rc;
+    launches += 3;
+  }
+  BTLE_CUDA(ctx, cudaEventRecord(t.e1, st));
+  btle_rx_ber_result res;
+  BTLE_CUDA(ctx, cudaMemcpyAsync(&res, d_res, sizeof res, cudaMemcpyDeviceToHost, st));
+  BTLE_CUDA(ctx, cudaStreamSynchronize(st));
+  float ms = 0;
+  BTLE_CUDA(ctx, cudaEventElapsedTime(&ms, t.e0, t.e1));
+  *out = res;
+  out->seconds = ms * 1e-3;
+  ctx->last_launches = launches;
   return BTLE_OK;
 }
 

@@ -426,6 +426,85 @@ int btle_b200_ber_run(btle_b200_ctx *ctx, const btle_ber_cfg *cfg, size_t n_pack
 int btle_b200_ber_synth_device(btle_b200_ctx *ctx, const btle_ber_cfg *cfg, uint64_t first_packet, size_t n_packets, int16_t *d_i,
                                int16_t *d_q, uint8_t *d_truth, void *cuda_stream);
 
+/* ---- error rates of the 4-Msps receive chain (btle_rx_persistent_kernel), impaired captures scored on the device -----
+ * Packet k of a run (k = 0, 1, ...); every draw is a hash of (seed, k, ...), so packet k is the same whatever the batch:
+ *   PDU      channels 37..39: header 42 25 + 37 random bytes drawn as btle_b200_ber_run draws them (same truth for the same
+ *            seed); channels 0..36: an LL data PDU, header 02 1B (LLID 2, length 27) + 27 random bytes, drawn the same way.
+ *   IQ       preamble, access address, PDU + CRC-24 whitened for the channel (cfg's access address / CRC init), the btle_tx
+ *            PHY at 4 sps (btle_b200_tx_modulate_device, sps 4): L = 32 * air bytes + 16 samples, times amplitude / 127.
+ *   channel  in this order, at packet sample m = 0 .. L-1:
+ *            1. clock and carrier error at ppm as btle_b200_ber_run applies it: the waveform read at (m - delta_k)(1 + e),
+ *               e = ppm 1e-6, linear interpolation clamped to the first / last sample, then a rotation by
+ *               e 2450e6 (1 + e) / 4e6 turns per sample; delta_k = j_k / 4, j_k drawn from 0..3 per packet;
+ *            2. an extra carrier offset of cfo_hz / 4e6 turns per sample (1. and 2. are one rotation, turns summed);
+ *            3. AWGN, sigma = amplitude / 10^(snr_db / 20) / sqrt 2 per rail, on every sample of the capture;
+ *            4. rintf, then saturation to -128..127 (what a radio's int8 ADC delivers).
+ *   capture  slot k holds samples [k S, (k+1) S), S = slot_samples >= L; packet k's L samples start at a drawn offset
+ *            0 .. S - L of its slot.  Every other sample is noise alone, rounded and saturated the same way.  The capture
+ *            of packets first .. first+n-1 starts with slot `first` at sample 0 and is BTLE_RX_BER_CAPTURE_INT8(n, S) int8
+ *            long: whole 8192-sample chunks, samples behind slot first+n-1 carrying noise only.
+ *   receiver btle_rx_persistent_kernel<1> (btle_b200_rx_device_dir) with BTLE_CFG_REPORT_REJECTED, mask 0xFFFFFFFF.
+ *   scoring  packet k's record is the first record in reference order whose access-address sample chunk * 8192 + n0
+ *            lies within +-3 of aa_sample (the synthesiser's access-address position, rounded).  pkt_err: no CRC-ok
+ *            counted record; bit errors only in those packets, over the PDU bytes the record and the truth have in common
+ *            (a counted record's PDU is its n_bytes - 3 bytes, a rejected one's its 2 header bytes), all 8 n_bytes bits
+ *            when there is no record (test_btle_ber.py:62-72, as ber_score_kernel applies them). */
+#define BTLE_RX_BER_AA_OFFSET 39       /* tx sample of the first access-address sample the receiver reports (n0)          */
+#define BTLE_RX_BER_MATCH 3            /* +- samples between a record's access address and the truth's                     */
+#define BTLE_RX_BER_MAX_SLOT 12000     /* largest slot_samples: a run's batches hold whole slots and whole chunks        */
+#define BTLE_RX_BER_MAX_UNITS 12272    /* largest unit directory btle_b200_rx_ber_score_device takes                      */
+#define BTLE_RX_BER_CAPTURE_INT8(n_packets, slot_samples) \
+  ((((uint64_t)(n_packets) * (uint64_t)(slot_samples) + 8191u) / 8192u) * 16384u)
+typedef struct {
+  uint64_t seed;
+  float snr_db;            /* NaN or infinite: BTLE_EINVAL                                                          */
+  float ppm;               /* not finite or |ppm| >= 1e6: BTLE_EINVAL                                               */
+  float cfo_hz;            /* extra carrier offset; not finite: BTLE_EINVAL                                         */
+  int32_t amplitude;       /* 1..127: the transmitted waveform's scale, amplitude / 127                             */
+  int32_t slot_samples;    /* L (1520 on channels 37..39, 1200 on 0..36) .. BTLE_RX_BER_MAX_SLOT                   */
+  int32_t channel;         /* 0..39                                                                                 */
+  uint32_t access_addr;
+  uint32_t crc_init;       /* as -k                                                                                 */
+  uint32_t reserved[2];    /* 0                                                                                     */
+} btle_rx_ber_cfg;         /* 48 bytes */
+typedef struct {
+  int64_t aa_sample;       /* first access-address sample, from the start of the capture: slot start + offset +
+                              round(BTLE_RX_BER_AA_OFFSET / (1 + e) + delta)                                          */
+  int32_t offset;          /* first sample of the packet's L samples in its slot                                    */
+  uint32_t clipped;        /* samples of the slot whose I or Q saturated                                            */
+  uint8_t n_bytes;         /* PDU bytes: 39 (channels 37..39) or 29                                                  */
+  uint8_t delta4;          /* 4 delta_k, 0..3                                                                         */
+  uint8_t pdu[39];         /* the PDU as sent (before CRC and whitening); zero behind n_bytes                        */
+  uint8_t reserved[7];
+} btle_rx_ber_truth;       /* 64 bytes */
+typedef struct {
+  uint64_t packets, pkt_err, bit_err, bit_total;
+  uint64_t aa_miss;        /* no record matched                                                                      */
+  uint64_t len_reject;     /* only a BTLE_REC_REJECTED record matched (header length outside 6..37)                  */
+  uint64_t crc_ok_wrong;   /* CRC ok, but the PDU differs from the truth (not a packet error, as in the model flow)   */
+  uint64_t extra_recs;     /* records matched to no packet                                                           */
+  uint64_t extra_crc_ok;   /* of those, counted records with a good CRC                                              */
+  uint64_t clipped;        /* saturated samples (I or Q) in the packets' slots                                       */
+  double seconds;          /* device time of the run (CUDA events)                                                   */
+} btle_rx_ber_result;      /* 88 bytes */
+/* n_packets packets 0 .. n_packets-1, in batches sized from free device memory; the result is independent of the batch
+ * size (every batch starts on a chunk and slot boundary, and its look-ahead behind the last chunk is the next slots').
+ * BTLE_EINVAL with btle_b200_last_error() for: snr_db, ppm or cfo_hz NaN or infinite, |ppm| >= 1e6, amplitude outside
+ * 1..127, slot_samples below L or above BTLE_RX_BER_MAX_SLOT, channel > 39; the context stays usable. */
+int btle_b200_rx_ber_run(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg, size_t n_packets, btle_rx_ber_result *out);
+/* the capture and truth of packets first_packet .. first_packet + n_packets - 1 alone: d_iq (16-byte aligned) receives
+ * BTLE_RX_BER_CAPTURE_INT8(n_packets, slot_samples) int8, d_truth n_packets rows.  Device pointers; enqueued on
+ * cuda_stream, not synchronised. */
+int btle_b200_rx_ber_synth_device(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg, uint64_t first_packet, size_t n_packets, int8_t *d_iq,
+                                  btle_rx_ber_truth *d_truth, void *cuda_stream);
+/* scores the records of one btle_b200_rx_device_dir launch over such a capture (d_recs with room for n_recs records,
+ * d_dir its n_units entries, n_units <= BTLE_RX_BER_MAX_UNITS) against d_truth[0 .. n_packets): ADDS this call's counts
+ * to the counters of the device struct *d_result (`seconds` is not touched; zero it before the first call).  Records
+ * past n_recs count as not returned.  Enqueued on cuda_stream, not synchronised. */
+int btle_b200_rx_ber_score_device(btle_b200_ctx *ctx, const btle_rx_ber_truth *d_truth, size_t n_packets, const btle_pkt_rec *d_recs,
+                                  size_t n_recs, const btle_unit_dir *d_dir, size_t n_units, btle_rx_ber_result *d_result,
+                                  void *cuda_stream);
+
 /* ---- 16-bit IQ ingest (SURVEY.md §8f-3) ------------------------------------------------------------
  * bladeRF SC16Q11 samples are reduced to the receive chain's int8 exactly as the reference's
  * stream_callback does: out = (in >> shift) & 0xFF, shift = 4 (btle_rx.c:307-308).  Host buffers;

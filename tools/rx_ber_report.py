@@ -1,0 +1,93 @@
+"""PER / BER of the reference's 4-Msps int8 receiver (btle_b200_rx_ber_run) next to the Python model's 8-sps receiver
+(btle_b200_ber_run) at the same SNR and ppm, plus the 4-Msps receiver under extra carrier offsets, and where the time of
+rx_ber_run goes (CUDA events around its three kernels on one batch).
+
+    python tools/rx_ber_report.py [--packets N] [--json out.json]
+
+Prints a markdown table (one row per point) and the throughput of both flows."""
+import argparse
+import ctypes
+import json
+import os
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+from btle_b200 import BtleRx, ber  # noqa: E402
+from btle_b200._native import DIR_DTYPE, RX_BER_RESULT_DTYPE  # noqa: E402,F401
+from btle_b200.rx import make_cfgs  # noqa: E402
+
+
+def kernel_times(rx, n_packets=32768, slot=2048, reps=5):
+    """ms per batch of synth, receive and score (median of reps), on one batch of n_packets packets"""
+    import torch
+    cfg = ber.rx_ber_cfg(6.0, slot_samples=slot, seed=3)
+    n_int8 = -(-n_packets * slot // 8192) * 16384
+    d_iq = torch.empty(n_int8, dtype=torch.int8, device="cuda")
+    d_truth = torch.empty((n_packets, 64), dtype=torch.uint8, device="cuda")
+    cap = (n_int8 // 16384) * 123
+    d_out = torch.empty(cap * 64, dtype=torch.uint8, device="cuda")
+    units = rx.units(1, n_int8)
+    d_dir = torch.empty(units * 8, dtype=torch.uint8, device="cuda")
+    d_res = torch.zeros(RX_BER_RESULT_DTYPE.itemsize, dtype=torch.uint8, device="cuda")
+    cfgs = make_cfgs(1, channel=37, rssi=2)
+    st = torch.cuda.current_stream()
+    sp = ctypes.c_void_p(st.cuda_stream)
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+    out = {"synth": [], "receive": [], "score": []}
+    for _ in range(reps + 1):
+        ev[0].record()
+        rx._check(rx._L.btle_b200_rx_ber_synth_device(rx._h, cfg.ctypes.data, 0, n_packets, d_iq.data_ptr(), d_truth.data_ptr(), sp))
+        ev[1].record()
+        rx.rx_device_dir(d_iq.view(1, -1), cfgs, d_out, None, d_dir, stream_ptr=st.cuda_stream)
+        ev[2].record()
+        rx._check(rx._L.btle_b200_rx_ber_score_device(rx._h, d_truth.data_ptr(), n_packets, d_out.data_ptr(), cap, d_dir.data_ptr(), units,
+                                                      d_res.data_ptr(), sp))
+        ev[3].record()
+        torch.cuda.synchronize()
+        for k, name in enumerate(out):
+            out[name].append(ev[k].elapsed_time(ev[k + 1]))
+    return {k: float(np.median(v[1:])) for k, v in out.items()} | {"packets": n_packets, "slot_samples": slot}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--packets", type=int, default=20000)
+    ap.add_argument("--json", default=None)
+    args = ap.parse_args()
+    rx = BtleRx(0)
+    snrs = list(range(-5, 31))             # the 4-sps receiver's curve falls between 15 and 30 dB
+    rows = []
+    for ppm in (0.0, 20.0, 50.0):
+        r4 = ber.rx_ber_sweep(snrs, args.packets, ppm=ppm, rx=rx)
+        r8 = ber.ber_sweep(snrs, args.packets, ppm=ppm, rx=rx)
+        for a, b in zip(r4, r8):
+            rows.append({"ppm": ppm, "cfo_hz": 0.0, "rx4": a, "model8": b})
+    for cfo in (25e3, 50e3, 100e3, 150e3):
+        for a in ber.rx_ber_sweep(snrs, args.packets, cfo_hz=cfo, rx=rx):
+            rows.append({"ppm": 0.0, "cfo_hz": cfo, "rx4": a, "model8": None})
+    print(f"| ppm | cfo kHz | SNR dB | 4-sps PER | 4-sps BER | aa_miss | len_reject | extra | 8-sps model PER | 8-sps model BER |")
+    print("|---:|---:|---:|---:|---:|---:|---:|---:|---:|---:|")
+    for r in rows:
+        a, b = r["rx4"], r["model8"]
+        m = f"{b['per']:.4f} | {b['ber']:.2e}" if b else "- | -"
+        print(f"| {r['ppm']:g} | {r['cfo_hz'] / 1e3:g} | {a['snr_db']:g} | {a['per']:.4f} | {a['ber']:.2e} | {a['aa_miss']} | {a['len_reject']} | "
+              f"{a['extra_recs']} | {m} |")
+    r4 = [r["rx4"] for r in rows]
+    r8 = [r["model8"] for r in rows if r["model8"]]
+    thr = {"rx4_packets_per_s": float(np.median([a["packets_per_s"] for a in r4])),
+           "rx4_generated_iq_gbytes_per_s": float(np.median([a["generated_iq_gbytes_per_s"] for a in r4])),
+           "model8_packets_per_s": float(np.median([b["packets_per_s"] for b in r8])),
+           "model8_generated_iq_gbytes_per_s": float(np.median([b["generated_iq_gbytes_per_s"] for b in r8]))}
+    kt = kernel_times(rx)
+    print(json.dumps({"throughput": thr, "kernel_ms_per_batch": kt}))
+    if args.json:
+        with open(args.json, "w") as f:
+            json.dump({"rows": rows, "throughput": thr, "kernel_ms_per_batch": kt}, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
