@@ -1780,7 +1780,6 @@ struct btle_b200_ctx {
   Buf<unsigned> d_count_ring;       // kCountRing allocation counters for launches that do not hand in their own (no memset node)
   unsigned ring_pos = 0;
   StreamUse ring_last[kCountRing / 2];   // [ring_pos % (kCountRing/2)]: the ring launch that next launch depends on (launch_rx)
-  size_t lead_bytes = 0;            // bytes readable in front of d_iq (set by the stream session around its launches; RSSI of hits at a segment's very start)
   HostBuf<unsigned> h_count;
   HostBuf<btle_pkt_rec> h_recs;     // staging for records
   HostBuf<btle_unit_dir> h_dir;     // staging for the unit directory
@@ -1997,11 +1996,12 @@ size_t multi_units_per_group(const btle_b200_ctx *ctx, size_t groups, size_t n_i
   return (size_t)plan_for(ctx, groups, n_int8).total_units / groups;
 }
 
-// enqueue the persistent kernel for device-resident inputs; cfg_capture != nullptr: several cfgs per capture
+// enqueue the persistent kernel for device-resident inputs; `lead`: bytes readable in front of each capture (the
+// stream session's lead: RSSI of hits at a segment's very start); cfg_capture != nullptr: several cfgs per capture
 // (n_cfgs of them, checked by check_cfg_capture), the directory in (cfg, chunk) order
 int launch_rx(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8,
               const btle_stream_cfg *cfgs, btle_pkt_rec *d_out, size_t cap, unsigned *d_count, btle_unit_dir *d_dir,
-              cudaStream_t st, const int32_t *cfg_capture = nullptr, size_t n_cfgs = 0, size_t groups = 0) {
+              cudaStream_t st, long long lead, const int32_t *cfg_capture = nullptr, size_t n_cfgs = 0, size_t groups = 0) {
   ctx->last_launches = 0;
   unsigned *zero_next = nullptr;
   if (d_count) BTLE_CUDA(ctx, cudaMemsetAsync(d_count, 0, sizeof(unsigned), st));
@@ -2041,13 +2041,11 @@ int launch_rx(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t s
   if (multi)
     btle_rx_persistent_kernel<kMaxCfgsPerCapture><<<grid, kThreads, sizeof(Smem<kMaxCfgsPerCapture>), st>>>(
         ms->map32, ms->map12, d_iq, (long long)stride, (long long)n_int8, cs->d_params, plan, d_out,
-        (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu), d_count, reinterpret_cast<uint2 *>(d_dir), zero_next, (long long)ctx->lead_bytes,
-        cs->d_vmap);
+        (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu), d_count, reinterpret_cast<uint2 *>(d_dir), zero_next, lead, cs->d_vmap);
   else
     btle_rx_persistent_kernel<1><<<grid, kThreads, sizeof(Smem<1>), st>>>(
         ms->map32, ms->map12, d_iq, (long long)stride, (long long)n_int8, cs->d_params, plan, d_out,
-        (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu), d_count, reinterpret_cast<uint2 *>(d_dir), zero_next, (long long)ctx->lead_bytes,
-        nullptr);
+        (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu), d_count, reinterpret_cast<uint2 *>(d_dir), zero_next, lead, nullptr);
   BTLE_CUDA(ctx, cudaGetLastError());
   if (ring) {                                                 // the position is taken only by a launch that was enqueued
     ctx->ring_pos = (ctx->ring_pos + 1) % kCountRing;
@@ -2366,7 +2364,7 @@ int btle_b200_rx_device_dir(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_str
   int rc = validate_cfgs(ctx, cfgs, n_streams);
   if (rc) return rc;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
-  return launch_rx(ctx, d_iq, n_streams, stride, n_int8, cfgs, d_out, cap, d_count, d_dir, reinterpret_cast<cudaStream_t>(cuda_stream));
+  return launch_rx(ctx, d_iq, n_streams, stride, n_int8, cfgs, d_out, cap, d_count, d_dir, reinterpret_cast<cudaStream_t>(cuda_stream), 0);
 }
 
 int btle_b200_rx_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8,
@@ -2464,7 +2462,7 @@ int btle_b200_rx_multi_device_dir(btle_b200_ctx *ctx, const int8_t *d_iq, size_t
   rc = validate_cfgs(ctx, cfgs, n_cfgs);
   if (rc) return rc;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
-  return launch_rx(ctx, d_iq, n_captures, stride, n_int8, cfgs, d_out, cap, d_count, d_dir, reinterpret_cast<cudaStream_t>(cuda_stream),
+  return launch_rx(ctx, d_iq, n_captures, stride, n_int8, cfgs, d_out, cap, d_count, d_dir, reinterpret_cast<cudaStream_t>(cuda_stream), 0,
                    cfg_capture, n_cfgs, groups);
 }
 
@@ -2500,7 +2498,7 @@ int btle_b200_rx_multi(btle_b200_ctx *ctx, const int8_t *iq, size_t n_captures, 
   }
   const size_t units = n_cfgs * multi_units_per_group(ctx, groups, n_int8);
   if (ctx->d_out.reserve(ctx, std::max<size_t>(cap, 1)) || ctx->d_dir.reserve(ctx, std::max<size_t>(units, 1))) return BTLE_ENOMEM;
-  rc = launch_rx(ctx, ctx->d_iq, groups, pitch, n_int8, cfgs, ctx->d_out, cap, ctx->d_count, ctx->d_dir, st, local.data(), n_cfgs, groups);
+  rc = launch_rx(ctx, ctx->d_iq, groups, pitch, n_int8, cfgs, ctx->d_out, cap, ctx->d_count, ctx->d_dir, st, 0, local.data(), n_cfgs, groups);
   if (rc) return rc;
   return fetch_ordered(ctx, ctx->d_out, ctx->d_dir, units, out, cap, n_out, st);
 }
@@ -2509,20 +2507,18 @@ int btle_b200_rx_multi(btle_b200_ctx *ctx, const int8_t *iq, size_t n_captures, 
 }  // extern "C"
 
 // One segment SET = `seg_chunks` chunks of every capture.  Capture i's part of a set sits at i * stride in the half's
-// buffers: kLead bytes of the previous set, the segment, kLook look-ahead bytes (the start of the next set).  A set is
-// decoded by ONE batched launch of the persistent kernel over the N parts once every capture has filled its own.
-// Once the cfg list has changed (btle_b200_streams_add_cfg / remove_cfg) a set is decoded by rx_multi launches instead,
-// in rounds of at most kMaxCfgsPerCapture cfgs per capture; a cfg added for chunks that are still resident is decoded
-// over them by one more launch on the half that holds them (backfill).
+// buffers: kLead bytes of the previous set, the segment, kLook look-ahead bytes (the start of the next set).  Once every
+// capture has filled its own, a set's live cfgs are decoded in rounds of at most kMaxCfgsPerCapture cfgs per capture,
+// one launch of the persistent kernel each: the single-cfg kernel for a round of one cfg per capture in capture order
+// (every set of a session whose cfg list never changed), rx_multi otherwise.  A cfg added for chunks that are still
+// resident is decoded over them by one more round on the half that holds them (backfill).
 struct btle_b200_streams {
   btle_b200_ctx *ctx = nullptr;
   size_t n = 0;                                            // captures in the session
-  std::vector<btle_stream_cfg> cfgs;                       // what the next submitted set is decoded with (cfgs 0..n-1)
   struct Entry {                                           // stable cfg index j: decodes `capture` for chunks [from, until)
     btle_stream_cfg cfg; size_t capture; long long from, until;
   };
-  std::vector<Entry> entries;                              // [0, n): the cfgs of streams_open (cfg mirrors cfgs[j])
-  bool listed = false;                                     // a cfg was added or removed: sets go through rx_multi rounds
+  std::vector<Entry> entries;                              // [0, n): the cfgs of streams_open
   std::vector<size_t> backfill;                            // cfgs added since the last commit / finish (streams_backfill)
   int call_launches = 0;                                   // launches of the current commit / finish call
   std::vector<int32_t> disc;                               // data channel scanned per capture, -1: none (set_discover)
@@ -2532,7 +2528,7 @@ struct btle_b200_streams {
   static constexpr size_t kLook = 4096;                    // >= 3008 + the kernel's 12-group tile (3072 + 4)
   static constexpr size_t kLead = 256;                     // bytes of the previous set kept in front (a hit may start up to 124 samples
                                                            // before its chunk; the RSSI sum reads the raw IQ there)
-  struct Job {                                             // one rx_multi launch on a half's IQ, collected with the half
+  struct Job {                                             // one round's launch on a half's IQ, collected with the half
     std::vector<size_t> index;                             // launch position -> stable cfg index
     size_t units = 0, cap = 0;
     Buf<btle_pkt_rec> d_out; Buf<btle_unit_dir> d_dir; Buf<unsigned> d_count;
@@ -2541,14 +2537,11 @@ struct btle_b200_streams {
   struct Scan {                                            // one discover launch over captures [first, first + count)
     size_t first = 0, count = 0, off = 0, cap = 0;         // candidates at d_cand[off, off + cap)
   };
-  struct Half {                                            // buffers sized once by btle_b200_streams_open
+  struct Half {
     HostBuf<int8_t> h; Buf<int8_t> d;                      // page-locked host / device IQ buffers, n parts of `stride` bytes
-    Buf<btle_pkt_rec> d_out; Buf<btle_unit_dir> d_dir; Buf<unsigned> d_count;
-    HostBuf<unsigned> h_count; HostBuf<btle_unit_dir> h_dir; HostBuf<btle_pkt_rec> h_recs;
     size_t n_submitted = 0;
     long long first_chunk = 0;
     cudaStream_t st = nullptr;
-    bool busy = false;                                     // the single-cfg launch of the set waits to be collected
     bool resident = false;                                 // d holds the set at first_chunk (lead, n_submitted bytes)
     std::vector<std::unique_ptr<Job>> jobs;                // jobs[0, n_jobs) wait to be collected (grown, then reused)
     size_t n_jobs = 0;
@@ -2575,8 +2568,10 @@ struct btle_b200_stream {
 namespace {
 using Streams = btle_b200_streams;
 
-// One rx_multi launch over half b's set, enqueued behind whatever its stream holds: cfgs `idx` (stable indices, sorted
-// by capture, at most kMaxCfgsPerCapture per capture) on the set's n_submitted bytes.  Collected by streams_collect.
+// One round's launch over half b's set, enqueued behind whatever its stream holds: cfgs `idx` (stable indices, sorted
+// by capture, at most kMaxCfgsPerCapture per capture) on the set's n_submitted bytes.  One cfg per capture in capture
+// order is a single-cfg launch (which, unlike rx_multi, also runs in builds with an uneven unit plan); any other round
+// is an rx_multi launch.  Buffers, strides and cfgs are the session's own, checked when made.  Collected by streams_collect.
 int streams_job(Streams *s, int b, const std::vector<size_t> &idx) {
   btle_b200_ctx *ctx = s->ctx;
   auto &H = s->half[b];
@@ -2588,16 +2583,21 @@ int streams_job(Streams *s, int b, const std::vector<size_t> &idx) {
   const size_t k = idx.size(), nch = H.n_submitted / kChunkInt8;
   std::vector<btle_stream_cfg> cfgs(k);
   std::vector<int32_t> cc(k);
-  for (size_t i = 0; i < k; ++i) { cfgs[i] = s->entries[idx[i]].cfg; cc[i] = (int32_t)s->entries[idx[i]].capture; }
-  const size_t units = std::max<size_t>(btle_b200_rx_multi_units(ctx, s->n, cc.data(), k, H.n_submitted), 1);
+  size_t groups = 0;                                         // captures the round reads
+  for (size_t i = 0; i < k; ++i) {
+    cfgs[i] = s->entries[idx[i]].cfg;
+    cc[i] = (int32_t)s->entries[idx[i]].capture;
+    groups += !i || cc[i] != cc[i - 1];
+  }
+  const bool single = k == s->n && groups == k;
+  const size_t units = std::max<size_t>(single ? btle_b200_rx_units(ctx, s->n, H.n_submitted)
+                                               : k * multi_units_per_group(ctx, groups, H.n_submitted), 1);
   const size_t cap = k * nch * BTLE_MAX_RECS_PER_CHUNK;      // the most a launch can find: never an overflow
   if (J.d_out.reserve(ctx, cap) || J.d_dir.reserve(ctx, units) || J.h_dir.reserve(ctx, units) ||
       (!J.d_count && (J.d_count.alloc(ctx, 1) || J.h_count.alloc(ctx, 1))))
     return BTLE_ENOMEM;
-  ctx->lead_bytes = Streams::kLead;
-  const int rc = btle_b200_rx_multi_device_dir(ctx, H.d + Streams::kLead, s->n, s->stride, H.n_submitted, cfgs.data(), cc.data(), k,
-                                               J.d_out, cap, J.d_count, J.d_dir, J.d_dir.n, H.st);
-  ctx->lead_bytes = 0;
+  const int rc = launch_rx(ctx, H.d + Streams::kLead, s->n, s->stride, H.n_submitted, cfgs.data(), J.d_out, cap, J.d_count, J.d_dir,
+                           H.st, Streams::kLead, single ? nullptr : cc.data(), k, groups);
   if (rc) return rc;
   BTLE_CUDA(ctx, cudaMemcpyAsync(J.h_count, J.d_count, sizeof(unsigned), cudaMemcpyDeviceToHost, H.st));
   BTLE_CUDA(ctx, cudaMemcpyAsync(J.h_dir, J.d_dir, units * sizeof(btle_unit_dir), cudaMemcpyDeviceToHost, H.st));
@@ -2674,7 +2674,7 @@ int streams_submit(Streams *s, int b, size_t n_int8, bool last = false) {
   H.n_submitted = n_int8;
   H.first_chunk = s->next_chunk;
   const bool scan = std::any_of(s->disc.begin(), s->disc.end(), [](int32_t c) { return c >= 0; });
-  if (n_int8 < (size_t)kChunkInt8 && !(scan && n_int8)) { H.busy = false; H.resident = false; return BTLE_OK; }
+  if (n_int8 < (size_t)kChunkInt8 && !(scan && n_int8)) { H.resident = false; return BTLE_OK; }
   constexpr size_t L = btle_b200_streams::kLead;
   if (L + n_int8 == s->stride || s->n == 1)
     BTLE_CUDA(ctx, cudaMemcpyAsync(H.d, H.h, (s->n - 1) * s->stride + L + n_int8, cudaMemcpyHostToDevice, H.st));
@@ -2682,21 +2682,11 @@ int streams_submit(Streams *s, int b, size_t n_int8, bool last = false) {
     BTLE_CUDA(ctx, cudaMemcpy2DAsync(H.d, s->stride, H.h, s->stride, L + n_int8, s->n, cudaMemcpyHostToDevice, H.st));
   H.resident = true;
   int &launches = s->call_launches, rc = BTLE_OK;
-  if (n_int8 >= (size_t)kChunkInt8 && s->listed) {
+  if (n_int8 >= (size_t)kChunkInt8) {
     std::vector<size_t> all(s->entries.size());
     for (size_t j = 0; j < all.size(); ++j) all[j] = j;
     rc = streams_rounds(s, b, all, &launches);
     if (rc) return rc;
-  } else if (n_int8 >= (size_t)kChunkInt8) {
-    ctx->lead_bytes = L;
-    rc = btle_b200_rx_device_dir(ctx, H.d + L, s->n, s->stride, n_int8, s->cfgs.data(), H.d_out, H.d_out.n, H.d_count, H.d_dir,
-                                 H.d_dir.n, H.st);
-    ctx->lead_bytes = 0;
-    if (rc) return rc;
-    BTLE_CUDA(ctx, cudaMemcpyAsync(H.h_count, H.d_count, sizeof(unsigned), cudaMemcpyDeviceToHost, H.st));
-    BTLE_CUDA(ctx, cudaMemcpyAsync(H.h_dir, H.d_dir, H.d_dir.n * sizeof(btle_unit_dir), cudaMemcpyDeviceToHost, H.st));
-    H.busy = true;
-    launches += 1;
   }
   if (scan) {
     rc = streams_scan(s, b, L + n_int8, (last ? n_int8 : s->seg_bytes) / 2, &launches);
@@ -2721,15 +2711,14 @@ int streams_backfill(Streams *s) {
   }
   return BTLE_OK;
 }
-// the number of launches a commit / finish call made, when the cfg list or discovery are in use (otherwise the
-// single-cfg launch reports itself)
+// the number of launches a commit / finish call made, when it made any
 void streams_note_launches(Streams *s) {
-  const bool scan = std::any_of(s->disc.begin(), s->disc.end(), [](int32_t c) { return c >= 0; });
-  if ((s->listed || scan) && s->call_launches) s->ctx->last_launches = s->call_launches;
+  if (s->call_launches) s->ctx->last_launches = s->call_launches;
 }
 
-// the records of half b's rx_multi jobs: stable cfg index in `stream`, stream-wide chunks, each cfg's [from, until)
-// kept, in (cfg, chunk, n0) order, appended to s->ready
+// the records of half b's jobs: stable cfg index in `stream`, stream-wide chunks, each cfg's [from, until) kept, in
+// (cfg, chunk, n0) order, appended to s->ready.  A job gathers in (launch position, chunk, n0) order, which is already
+// that order when positions map to ascending cfgs (always, while the cfg list is unchanged): only other orders are sorted.
 int streams_collect_jobs(Streams *s, int b) {
   btle_b200_ctx *ctx = s->ctx;
   auto &H = s->half[b];
@@ -2747,26 +2736,29 @@ int streams_collect_jobs(Streams *s, int b) {
     if (*H.jobs[q]->h_count)
       BTLE_CUDA(ctx, cudaMemcpyAsync(H.h_jrecs + at, H.jobs[q]->d_out, *H.jobs[q]->h_count * sizeof(btle_pkt_rec), cudaMemcpyDeviceToHost, H.st));
   BTLE_CUDA(ctx, cudaStreamSynchronize(H.st));
-  std::vector<btle_pkt_rec> got(total), keep;
-  keep.reserve(total);
+  const size_t at0 = s->ready.size();
+  s->ready.resize(at0 + total);
+  size_t end = at0;                                          // the records kept so far: s->ready[at0, end)
   for (size_t q = 0, at = 0; q < n_jobs; ++q) {
     const Streams::Job &J = *H.jobs[q];
     const size_t found = *J.h_count;
+    btle_pkt_rec *got = s->ready.data() + end;               // filtered in place: a record is written at or before its slot
     size_t n_got = 0;
-    btle_b200_gather_ordered(H.h_jrecs + at, found, J.h_dir, J.units, got.data() + at, found, &n_got);
-    for (size_t i = at; i < at + found; ++i) {
+    btle_b200_gather_ordered(H.h_jrecs + at, found, J.h_dir, J.units, got, found, &n_got);
+    for (size_t i = 0; i < found; ++i) {
       btle_pkt_rec r = got[i];
       const size_t j = J.index[(size_t)r.stream];
       const long long chunk = r.chunk + H.first_chunk;
       if (chunk < s->entries[j].from || chunk >= s->entries[j].until) continue;
       r.stream = (int32_t)j;
       r.chunk = (int32_t)chunk;
-      keep.push_back(r);
+      s->ready[end++] = r;
     }
     at += found;
   }
-  std::stable_sort(keep.begin(), keep.end(), [](const btle_pkt_rec &x, const btle_pkt_rec &y) { return x.stream < y.stream; });
-  s->ready.insert(s->ready.end(), keep.begin(), keep.end());
+  s->ready.resize(end);
+  const auto by_cfg = [](const btle_pkt_rec &x, const btle_pkt_rec &y) { return x.stream < y.stream; };
+  if (!std::is_sorted(s->ready.begin() + at0, s->ready.end(), by_cfg)) std::stable_sort(s->ready.begin() + at0, s->ready.end(), by_cfg);
   return BTLE_OK;
 }
 
@@ -2817,23 +2809,8 @@ int streams_collect_scans(Streams *s, int b) {
 int streams_collect(Streams *s, int b) {
   btle_b200_ctx *ctx = s->ctx;
   auto &H = s->half[b];
-  if (!H.busy && !H.n_jobs && H.scans.empty()) return BTLE_OK;
+  if (!H.n_jobs && H.scans.empty()) return BTLE_OK;
   BTLE_CUDA(ctx, cudaStreamSynchronize(H.st));
-  if (H.busy) {
-    H.busy = false;
-    const size_t found = *H.h_count;
-    if (found > H.d_out.n) { ctx->err = "stream segment produced more records than BTLE_MAX_RECS_PER_CHUNK allows"; return BTLE_EOVERFLOW; }
-    if (found) {
-      BTLE_CUDA(ctx, cudaMemcpyAsync(H.h_recs, H.d_out, found * sizeof(btle_pkt_rec), cudaMemcpyDeviceToHost, H.st));
-      BTLE_CUDA(ctx, cudaStreamSynchronize(H.st));
-      const size_t units = btle_b200_rx_units(ctx, s->n, H.n_submitted);
-      const size_t at = s->ready.size();
-      s->ready.resize(at + found);
-      size_t got = 0;
-      btle_b200_gather_ordered(H.h_recs, found, H.h_dir, units, s->ready.data() + at, found, &got);
-      for (size_t i = at; i < at + found; ++i) s->ready[i].chunk += (int32_t)H.first_chunk;
-    }
-  }
   int rc = streams_collect_jobs(s, b);
   if (rc) return rc;
   return streams_collect_scans(s, b);
@@ -2876,20 +2853,23 @@ int btle_b200_streams_open(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
   btle_b200_streams *s = new (std::nothrow) btle_b200_streams();
   if (!s) return BTLE_ENOMEM;
-  s->ctx = ctx; s->n = n_streams; s->cfgs.assign(cfgs, cfgs + n_streams); s->fill.assign(n_streams, 0);
+  s->ctx = ctx; s->n = n_streams; s->fill.assign(n_streams, 0);
   for (size_t i = 0; i < n_streams; ++i) s->entries.push_back({cfgs[i], i, 0, LLONG_MAX});
   s->disc.assign(n_streams, -1);
   s->seg_chunks = segment_chunks; s->seg_bytes = segment_chunks * (size_t)kChunkInt8;
   s->buf_bytes = s->seg_bytes + btle_b200_streams::kLook;
   s->stride = btle_b200_streams::kLead + s->buf_bytes;     // a multiple of 16, as the batched kernel needs
+  // each half's first job and h_jrecs are sized for a round of one cfg per capture, so a session whose cfg list never
+  // changes allocates nothing after this.  A short tail can be cut into more units than a full set (make_plan: down to
+  // one chunk per unit, over whole 16-chunk spans), so the directory holds the most any such launch can have.
   const size_t cap = n_streams * segment_chunks * BTLE_MAX_RECS_PER_CHUNK;
-  // a short tail can be cut into more units than a full set (make_plan: down to one chunk per unit, over whole 16-chunk
-  // spans), so the directory is sized for the most any launch of up to segment_chunks chunks per capture can have
   const size_t units = n_streams * ((segment_chunks + 15) & ~size_t(15));
   for (auto &H : s->half) {
-    if (H.h.alloc(ctx, n_streams * s->stride) || H.d.alloc(ctx, n_streams * s->stride) || H.d_out.alloc(ctx, cap) ||
-        H.d_dir.alloc(ctx, units) || H.d_count.alloc(ctx, 1) || H.h_count.alloc(ctx, 1) || H.h_dir.alloc(ctx, units) ||
-        H.h_recs.alloc(ctx, cap) || cudaStreamCreateWithFlags(&H.st, cudaStreamNonBlocking) != cudaSuccess) {
+    H.jobs.emplace_back(new (std::nothrow) Streams::Job());
+    Streams::Job *J = H.jobs.back().get();
+    if (!J || H.h.alloc(ctx, n_streams * s->stride) || H.d.alloc(ctx, n_streams * s->stride) || J->d_out.alloc(ctx, cap) ||
+        J->d_dir.alloc(ctx, units) || J->d_count.alloc(ctx, 1) || J->h_count.alloc(ctx, 1) || J->h_dir.alloc(ctx, units) ||
+        H.h_jrecs.alloc(ctx, cap) || cudaStreamCreateWithFlags(&H.st, cudaStreamNonBlocking) != cudaSuccess) {
       cudaGetLastError();
       ctx->err = "streams_open: allocation failed";
       btle_b200_streams_close(s);
@@ -2915,8 +2895,7 @@ int btle_b200_streams_set_cfg(btle_b200_streams *s, size_t stream, const btle_st
   if (rc) return rc;
   rc = validate_cfgs(s->ctx, cfg, 1);
   if (rc) return rc;
-  s->cfgs[stream] = *cfg;                                   // used from the next submitted segment set on
-  s->entries[stream].cfg = *cfg;
+  s->entries[stream].cfg = *cfg;                            // used from the next submitted segment set on
   return BTLE_OK;
 }
 
@@ -3014,7 +2993,6 @@ int btle_b200_streams_add_cfg(btle_b200_streams *s, size_t capture, const btle_s
   const size_t j = s->entries.size();
   s->entries.push_back({*cfg, capture, (long long)from_chunk, LLONG_MAX});
   s->backfill.push_back(j);
-  s->listed = true;
   *index = j;
   return BTLE_OK;
 }
@@ -3025,7 +3003,6 @@ int btle_b200_streams_remove_cfg(btle_b200_streams *s, size_t index, int64_t *un
   auto &e = s->entries[index];
   if (e.until != LLONG_MAX) { s->ctx->err = "streams_remove_cfg: cfg already removed"; return BTLE_EINVAL; }
   e.until = std::max(e.from, s->next_chunk);                // the next submitted set starts at next_chunk
-  s->listed = true;
   *until_chunk = e.until;
   return BTLE_OK;
 }
@@ -3600,7 +3577,7 @@ int btle_b200_rx_ber_run(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg, size_t 
     rc = launch_rx_ber_synth(ctx, *cfg, done, n_packets, (long long)(n_int8 / 2), (long long)n, ctx->d_iq, d_truth, st);
     if (rc) return rc;
     const size_t cap = (size_t)chunks * BTLE_MAX_RECS_PER_CHUNK, units = btle_b200_rx_units(ctx, 1, n_int8);
-    rc = launch_rx(ctx, ctx->d_iq, 1, n_int8, n_int8, &scfg, ctx->d_out, cap, ctx->d_count, ctx->d_dir, st);
+    rc = launch_rx(ctx, ctx->d_iq, 1, n_int8, n_int8, &scfg, ctx->d_out, cap, ctx->d_count, ctx->d_dir, st, 0);
     if (rc) return rc;
     rc = launch_rx_ber_score(ctx, d_truth, n, ctx->d_out, cap, ctx->d_dir, units, d_res, st);
     if (rc) return rc;

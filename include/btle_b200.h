@@ -270,9 +270,10 @@ int btle_b200_discover(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, s
  * i decodes capture i), each added cfg gets the next one.  A record's `stream` is that index.  The records of cfg j equal
  * btle_b200_rx_batch() on cfg j's capture (cut to the shortest capture) decoded with cfg j, kept for
  * from_chunk <= chunk < until_chunk; each is returned exactly once, per set in (j, chunk, n0) order.
- * While no cfg was added or removed a set is decoded by the one single-cfg launch described above.  After that, a set's
- * live cfgs are sorted by capture and decoded by btle_b200_rx_multi_device_dir launches, in rounds of at most
- * BTLE_MAX_CFGS_PER_CAPTURE cfgs per capture; a capture no live cfg names is not read by the kernel.
+ * A set's live cfgs are sorted by capture and decoded in rounds of at most BTLE_MAX_CFGS_PER_CAPTURE cfgs per capture,
+ * one launch per round: a round of one cfg per capture in capture order is the single-cfg launch described above (every
+ * set of a session whose cfg list never changed), any other round a btle_b200_rx_multi_device_dir launch.  A capture no
+ * live cfg names is not read by the kernel.
  * BACKFILL: the two most recent sets stay on the device (the one whose records were handed out last, and the one in
  * flight).  add_cfg accepts any from_chunk >= btle_b200_streams_resident(); the next commit or finish call decodes every
  * cfg added since the last one over the resident sets that hold chunks >= its from_chunk (rounds of at most

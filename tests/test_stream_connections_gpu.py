@@ -103,6 +103,38 @@ def test_no_added_cfg_keeps_the_single_launch(rx, traffic):
     _same(_by_cfg(got), rx.rx_batch(np.stack([c[:m] for c in traffic]), base))
 
 
+@pytest.mark.parametrize("seg", [1, 4, 17])
+def test_replaced_cfg_keeps_the_single_launch(rx, traffic, seg):
+    """Capture 1's cfg removed, then another access address added on capture 1 from chunk 0: one cfg per capture in
+    capture order again, but under index 4.  Every set is one launch, and the records are rx_batch with the replaced
+    cfg, stream = 4 for capture 1."""
+    base = make_cfgs(4, channel=[37, 5, 38, 22], crc_init=[0x555555, 0x227BA7, 0x555555, 0x227BA7], rssi=1)
+    f = dict(access_addr=AAS[1], crc_init=0x227BA7 ^ (AAS[1] & 0xFFFF))
+    new = base[1:2].copy()
+    for k, v in f.items():
+        new[k] = v
+    entries = {i: (i, base[i:i + 1], 0, 1 << 40) for i in (0, 2, 3)}
+    entries[4] = (1, new, 0, 1 << 40)
+    step = seg * CHUNK
+    with rx.streams(base, segment_chunks=seg) as s_:
+        assert s_.remove_cfg(1) == 0
+        assert s_.add_cfg(1, 0, **f) == (4, 0)
+        parts = []
+        for pos in range(0, max(c.size for c in traffic), step):
+            parts += [s_.push(i, traffic[i][pos:pos + step]) for i in range(4)]
+            if pos:                                            # sets 0.. are submitted from the second round on
+                assert rx.last_launches == 1, pos
+        parts.append(s_.finish())
+        assert rx.last_launches == 1                           # the tail set
+    for p in parts:                                            # inside a set: (cfg, chunk) order
+        key = np.stack([p["chunk"] // seg, p["stream"], p["chunk"]], axis=1)
+        assert all(tuple(a) <= tuple(b) for a, b in zip(key[:-1], key[1:]))
+    got = np.concatenate(parts)
+    exp = _expect(rx, traffic, entries)
+    assert (exp["stream"] == 4).sum() > 5 and len(exp) > 50
+    _same(_by_cfg(got), exp)
+
+
 def test_mid_stream_add_remove_and_backfill(rx, traffic):
     caps = traffic
     base = make_cfgs(4, channel=[37, 5, 38, 22], crc_init=[0x555555, 0x227BA7, 0x555555, 0x227BA7])
