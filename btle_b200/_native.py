@@ -39,7 +39,7 @@ BER_RESULT_DTYPE = np.dtype([("packets", "<u8"), ("pkt_err", "<u8"), ("bit_err",
 assert BER_CFG_DTYPE.itemsize == 32 and BER_RESULT_DTYPE.itemsize == 48
 # btle_rx_ber_cfg (48 bytes), btle_rx_ber_truth (64 bytes), btle_rx_ber_result (88 bytes): error rates of the 4-Msps receiver
 RX_BER_CFG_DTYPE = np.dtype([("seed", "<u8"), ("snr_db", "<f4"), ("ppm", "<f4"), ("cfo_hz", "<f4"), ("amplitude", "<i4"), ("slot_samples", "<i4"),
-                             ("channel", "<i4"), ("access_addr", "<u4"), ("crc_init", "<u4"), ("reserved", "<u4", 2)])
+                             ("channel", "<i4"), ("access_addr", "<u4"), ("crc_init", "<u4"), ("flags", "<u4"), ("reserved", "<u4")])
 RX_BER_TRUTH_DTYPE = np.dtype([("aa_sample", "<i8"), ("offset", "<i4"), ("clipped", "<u4"), ("n_bytes", "u1"), ("delta4", "u1"), ("pdu", "u1", 39),
                                ("reserved", "u1", 7)])
 RX_BER_COUNTERS = ("packets", "pkt_err", "bit_err", "bit_total", "aa_miss", "len_reject", "crc_ok_wrong", "extra_recs", "extra_crc_ok", "clipped")
@@ -74,6 +74,8 @@ EXPORTS = [
     "btle_b200_streams_take_cands",
 ]
 MAX_CFGS_PER_CAPTURE = 8       # BTLE_MAX_CFGS_PER_CAPTURE
+CFG_RSSI, CFG_REPORT_REJECTED, CFG_RECOVER = 1, 2, 4      # btle_stream_cfg.rssi flag bits (BTLE_CFG_*)
+REC_REJECTED, REC_RECOVERED = 4, 8                        # btle_pkt_rec.flags bits; a recovered record's alternative q is flags >> 4 & 3
 
 
 class BtleError(RuntimeError):

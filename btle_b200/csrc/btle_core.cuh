@@ -16,6 +16,8 @@
 #pragma once
 #include <stdint.h>
 
+#include "../../include/btle_b200.h"
+
 #if defined(__CUDACC__)
 #define BTLE_HD __host__ __device__ __forceinline__
 #define BTLE_HDM __host__ __device__ __forceinline__   // member functions
@@ -150,7 +152,8 @@ struct StreamParams {
   int32_t adv;                // channel in {37,38,39}, :2202
   int32_t rssi;               // -R
   int32_t report_rejected;    // -v: hits the reference drops for their ADV length (:2291-2298) are reported too (not counted)
-  int32_t tz;                 // min(31, index of lowest set bit of aa&mask (32 if none))
+  int32_t recover;            // BTLE_CFG_RECOVER and not raw: CRC-failed counted packets are demodulated again (recover_packet)
+  int32_t tz;                // min(31, index of lowest set bit of aa&mask (32 if none))
   int32_t ntaps;              // 0 => every group is flagged (mask == 0)
   int32_t typed;              // 1 => taps [0, kTapsOne) expect a 1 and taps [kTapsOne, kMaxTaps) expect a 0
   uint32_t tap_pos[kMaxTaps]; // prefilter tap positions p (mask bit set), padded by repetition
@@ -677,6 +680,72 @@ BTLE_HD void decode_packet(const uint32_t *pd, const StreamParams &sp, const uin
   nbytes_out = nbytes;
   crc_bad_out = crc_bad;
 }
+
+// ---- recovery of CRC-failed packets (BTLE_CFG_RECOVER, include/btle_b200.h) --------------------------------------------
+// The capture samples one chunk's recovery may read: sample s (relative to the chunk) is iq[2s], iq[2s+1] for 0 <= s < n,
+// n = what the capture holds of the chunk's receiver() window [0, kWinInt8 / 2); every other sample reads 0.
+struct IqWindow {
+  const int8_t *iq;            // the chunk's first sample
+  int n;
+};
+BTLE_HD IqWindow iq_window(const int8_t *capture, long long n_int8, long long chunk) {
+  const long long base = chunk * kChunkInt8, avail = (n_int8 - base) >> 1;
+  IqWindow w;
+  w.iq = capture + base;
+  w.n = avail < 0 ? 0 : (avail > kWinInt8 / 2 ? kWinInt8 / 2 : (int)avail);
+  return w;
+}
+// I and Q of sample s (0 outside the window)
+BTLE_HD void iq_at(const IqWindow &w, int s, int &i, int &q) {
+  i = q = 0;
+  if (s >= 0 && s < w.n) { i = w.iq[2 * s]; q = w.iq[2 * s + 1]; }
+}
+// Symbol-spaced discriminator bits: bit k of the result is e[s0 + 4k], e[s] = (I[s] Q[s+4] - I[s+4] Q[s]) > 0.
+BTLE_HD uint32_t sym_bits32(const IqWindow &w, int s0) {
+  int i0, q0;
+  iq_at(w, s0, i0, q0);
+  uint32_t r = 0u;
+#pragma unroll 4
+  for (int k = 0; k < 32; ++k) {
+    int i1, q1;
+    iq_at(w, s0 + 4 * k + 4, i1, q1);
+    r |= (uint32_t)(i0 * q1 - i1 * q0 > 0) << k;
+    i0 = i1;
+    q0 = q1;
+  }
+  return r;
+}
+// One counted packet whose access address starts at sample n0 and whose primary decode failed the CRC: alternatives
+// q = 0..3 (packet bit j = e[n0 + 4j + q - 2]) in order; the first whose CRC is good wins.  Returns q and writes that
+// alternative's bytes (words[11], zero behind n_bytes, as decode_packet) and n_bytes; returns -1 and leaves both
+// untouched when none passes.  Not for raw mode (sp.recover is 0 there).
+BTLE_HD int recover_packet(const IqWindow &w, const StreamParams &sp, const uint32_t *crc4, int n0, uint32_t words[11], int &nbytes_out) {
+  for (int q = 0; q < 4; ++q) {
+    const int s0 = n0 + 4 * 32 + q - 2;                  // packet bit 32: the first header bit
+    uint32_t alt[11];
+    alt[0] = sym_bits32(w, s0) ^ sp.whiten[0];
+    const int plen = (int)((alt[0] >> 8) & (sp.adv ? 0x3Fu : 0x1Fu));
+    if (sp.adv && (plen < 6 || plen > 37)) continue;
+    const int nbytes = plen + 5, nw = (nbytes + 3) >> 2, body = nbytes - 3;
+    const uint32_t last_mask = (nbytes & 3) ? ((1u << (8 * (nbytes & 3))) - 1u) : 0xFFFFFFFFu;
+#pragma unroll
+    for (int j = 1; j < 11; ++j) alt[j] = j < nw ? sym_bits32(w, s0 + 4 * 32 * j) ^ sp.whiten[j] : 0u;
+#pragma unroll
+    for (int j = 0; j < 11; ++j)
+      if (j == nw - 1) alt[j] &= last_mask;
+    const uint32_t crc = crc24_words(alt, body, sp.crc_init, crc4);
+    const uint32_t rx = (sym_bits32(w, s0 + 4 * 8 * body) ^ whiten32(sp, body)) & 0xFFFFFFu;
+    if (crc == rx) {
+#pragma unroll
+      for (int j = 0; j < 11; ++j) words[j] = alt[j];
+      nbytes_out = nbytes;
+      return q;
+    }
+  }
+  return -1;
+}
+// flags bits a recovered record carries on top of the primary decode's (alternative q)
+BTLE_HD uint32_t recovered_flags(int q) { return q < 0 ? 0u : (uint32_t)(BTLE_REC_RECOVERED | (q << 4)); }
 
 // Both parts back to back for one chunk (what the test-only CPU emulator runs, lane by lane):
 // emit(n0, n_bytes, crc_bad, words[11], rejected) per counted (or, with report_rejected, rejected) hit, in the reference's order.

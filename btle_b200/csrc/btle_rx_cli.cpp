@@ -67,7 +67,7 @@ const char *CTRL_NAME[15] = {"LL_CONNECTION_UPDATE_REQ", "LL_CHANNEL_MAP_REQ", "
                              "LL_REJECT_IND", "LL_RESERVED"};                              // :1060-1076
 
 struct Options {
-  int chan = 37, gain = 6, lna = 32, amp = 0, verbose = 0, raw = 0, hop = 0, json = 0, quiet = 0, rssi = 0;
+  int chan = 37, gain = 6, lna = 32, amp = 0, verbose = 0, raw = 0, hop = 0, json = 0, quiet = 0, rssi = 0, recover = 0;
   uint32_t aa = 0x8E89BED6u, crc_init = 0x555555u, mask = 0xFFFFFFFFu;
   uint64_t freq_hz = 123;
   const char *pcap = nullptr, *iq_txt = nullptr, *iq_sc16 = nullptr, *iq_dir = nullptr, *iq_bin16 = nullptr;
@@ -109,6 +109,8 @@ void usage() {
       "    -v --verbose / -r --raw / -o --hop\n"
       "    -s --filename\n      Store packets to pcap file (DLT 256, LE LL with PHDR)\n"
       "    -j --json / -Q --quiet-text / -R --rssi-est\n"
+      "       --recover\n      packets whose CRC fails are demodulated once more, symbol-spaced on four sample phases; the first\n"
+      "      phase whose CRC is ok replaces the packet (printed as CRC0; NDJSON adds \"recovered\":q).  Not with -o or --iq-bin16\n"
       "    -F --filter-adva AA:BB:CC:DD:EE:FF / -T --filter-pdu-type 0,3,4\n"
       "    -d --device N   CUDA device (default 0)\n");
 }
@@ -156,7 +158,7 @@ Options parse_commandline(int argc, char **argv) {
       {"filter-pdu-type", required_argument, 0, 'T'}, {"iq-file", required_argument, 0, 'i'},
       {"iq-txt", required_argument, 0, 1000}, {"iq-sc16", required_argument, 0, 1001}, {"device", required_argument, 0, 'd'},
       {"iq-dir", required_argument, 0, 1002}, {"segment-chunks", required_argument, 0, 1003}, {"iq-bin16", required_argument, 0, 1004},
-      {"connections", no_argument, 0, 1005}, {0, 0, 0, 0}};
+      {"connections", no_argument, 0, 1005}, {"recover", no_argument, 0, 1006}, {0, 0, 0, 0}};
   for (;;) {
     int idx = 0;
     const int c = getopt_long(argc, argv, "hc:g:l:ba:k:vrf:m:os:jQRF:T:i:d:", longopts, &idx);   // + i:, d:
@@ -182,6 +184,7 @@ Options parse_commandline(int argc, char **argv) {
       case 1002: o.iq_dir = optarg; break;
       case 1004: o.iq_bin16 = optarg; break;
       case 1005: o.connections = 1; break;
+      case 1006: o.recover = 1; break;
       case 1003: o.segment_chunks = (size_t)strtoul(optarg, &endp, 10); break;
       case 1000: o.iq_txt = optarg; break;
       case 1001: o.iq_sc16 = optarg; break;
@@ -207,6 +210,8 @@ Options parse_commandline(int argc, char **argv) {
   if (o.lna < 0 || o.lna > 40) { printf("lna gain must be within 0~%d!\n", 40); bad_args(); }            // :1442
   if (optind < argc) { printf("Error: unknown/extra arguments specified on command line!\n"); bad_args(); }
   if (o.connections && (!o.iq_dir || o.hop)) { printf("--connections needs --iq-dir and cannot be combined with -o\n"); bad_args(); }
+  // -o follows as the reference's follower does, from the reference's records; --iq-bin16 has a receiver of its own
+  if (o.recover && (o.hop || o.iq_bin16)) { printf("--recover cannot be combined with -o or --iq-bin16\n"); bad_args(); }
   return o;
 }
 
@@ -428,6 +433,7 @@ struct Sinks {
         if (has_a) printf("\"%02x:%02x:%02x:%02x:%02x:%02x\"", a[0], a[1], a[2], a[3], a[4], a[5]); else printf("null");
         printf(",\"payload_hex\":"); json_hex(b + 2, plen);
         if (rssi == INT_MIN) printf(",\"rssi_est\":null"); else printf(",\"rssi_est\":%d", rssi);
+        if (r.flags & BTLE_REC_RECOVERED) printf(",\"recovered\":%d", BTLE_REC_RECOVERED_Q(r.flags));
         printf("}\n");
       }
     } else {
@@ -449,6 +455,7 @@ struct Sinks {
         printf(",\"nesn\":%d,\"sn\":%d,\"md\":%d,\"plen\":%d,\"payload_hex\":", nesn, sn, md, plen);
         json_hex(b + 2, plen);
         if (rssi == INT_MIN) printf(",\"rssi_est\":null"); else printf(",\"rssi_est\":%d", rssi);
+        if (r.flags & BTLE_REC_RECOVERED) printf(",\"recovered\":%d", BTLE_REC_RECOVERED_Q(r.flags));
         printf("}\n");
       }
     }
@@ -490,7 +497,9 @@ Capture parse_capture(const std::string &spec, const Options &o) {
   return c;
 }
 
-int cfg_flags(const Options &o) { return (o.rssi ? BTLE_CFG_RSSI : 0) | (o.verbose ? BTLE_CFG_REPORT_REJECTED : 0); }
+int cfg_flags(const Options &o) {
+  return (o.rssi ? BTLE_CFG_RSSI : 0) | (o.verbose ? BTLE_CFG_REPORT_REJECTED : 0) | (o.recover ? BTLE_CFG_RECOVER : 0);
+}
 
 // rx_batch with a capacity that is grown once if the library asks
 int rx_batch_grow(btle_b200_ctx *ctx, const int8_t *iq, size_t ns, size_t stride, size_t n, const btle_stream_cfg *cfgs,
@@ -564,7 +573,7 @@ struct ConnMonitor {
     btle_b200_streams_resident(ss, &from);
     c.from = from;
     for (int ch = 0; ch < 37 && !rc; ++ch) {
-      const btle_stream_cfg cfg{ch, c.aa, 0xFFFFFFFFu, c.crc_init, 0, o.rssi ? BTLE_CFG_RSSI : 0};
+      const btle_stream_cfg cfg{ch, c.aa, 0xFFFFFFFFu, c.crc_init, 0, (o.rssi ? BTLE_CFG_RSSI : 0) | (o.recover ? BTLE_CFG_RECOVER : 0)};
       size_t j = 0;
       rc = btle_b200_streams_add_cfg(ss, (size_t)ch, &cfg, from, &j);
       c.cfgs.push_back(j);

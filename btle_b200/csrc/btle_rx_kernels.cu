@@ -206,9 +206,10 @@ __device__ __forceinline__ void tma_load_tile(void *smem_dst, const CUtensorMap 
       ::"r"(smem_u32(smem_dst)), "l"(map), "r"(0), "r"(run), "r"(0), "r"(stream), "r"(smem_u32(bar)) : "memory");
 }
 // Writes one packet record.  Reads the raw IQ only when the caller asked for RSSI.
+// `extra`: flags bits on top of raw / advertising / rejected (recovered_flags()).
 __device__ __forceinline__ void store_record(btle_pkt_rec *dst, int stream, int chunk, int n0, int nbytes, int crc_bad, bool rejected,
                                              const uint32_t words[11], const StreamParams &sp, const int8_t *iq,
-                                             long long n_int8, long long lead) {
+                                             long long n_int8, long long lead, uint32_t extra = 0u) {
   uint32_t mag = 0;
   if (sp.rssi) {                                            // btle_rx.c:2234-2243
     const long long first = (long long)chunk * kChunkInt8 + 2ll * n0;
@@ -223,7 +224,7 @@ __device__ __forceinline__ void store_record(btle_pkt_rec *dst, int stream, int 
   r[1] = (uint32_t)chunk;
   r[2] = (uint32_t)n0;
   r[3] = (uint32_t)sp.channel | ((uint32_t)nbytes << 8) | ((uint32_t)crc_bad << 16) |
-         ((uint32_t)((sp.raw ? 1 : 0) | (sp.adv ? 2 : 0) | (rejected ? BTLE_REC_REJECTED : 0)) << 24);
+         ((uint32_t)((sp.raw ? 1 : 0) | (sp.adv ? 2 : 0) | (rejected ? BTLE_REC_REJECTED : 0) | extra) << 24);
   r[4] = sp.aa;
   r[5] = (mag & 0xFFFFu) | (words[0] << 16);                // mag_sum, bytes[0..1]
 #pragma unroll
@@ -233,8 +234,21 @@ __device__ __forceinline__ void store_record(btle_pkt_rec *dst, int stream, int 
   for (int q = 0; q < 4; ++q) d4[q] = make_uint4(r[4 * q], r[4 * q + 1], r[4 * q + 2], r[4 * q + 3]);
 }
 
+// BTLE_CFG_RECOVER: stores the record of a counted packet whose primary decode failed the CRC when one of its
+// alternatives passes (recover_packet) and returns true; false: nothing stored, the caller stores the primary decode.
+// Out of line, so that the decode pass keeps its registers and the launches of cfgs without the flag pay one branch.
+__device__ __forceinline__ bool store_recovered(btle_pkt_rec *dst, int stream, int chunk, int n0, const StreamParams &sp, const uint32_t *crc4,
+                                             const int8_t *iq, long long n_int8, long long lead) {
+  uint32_t words[11];
+  int nbytes = 0;
+  const int q = recover_packet(iq_window(iq, n_int8, chunk), sp, crc4, n0, words, nbytes);
+  if (q < 0) return false;
+  store_record(dst, stream, chunk, n0, nbytes, 0, false, words, sp, iq, n_int8, lead, recovered_flags(q));
+  return true;
+}
+
 // Copy one stream's parameters (built on the host by make_params(), uploaded next to the cfg array) into a ring slot:
-// one coalesced load of sizeof(StreamParams) = 184 bytes by a warp, no dependent look-ups.
+// one coalesced load of sizeof(StreamParams) = 192 bytes by a warp, no dependent look-ups.
 constexpr int kParamWords = (int)(sizeof(StreamParams) / 4);
 static_assert(sizeof(StreamParams) % 4 == 0 && kParamWords <= 64, "StreamParams is copied as <= 2 words per lane");
 __device__ __forceinline__ void load_params_warp(const StreamParams *__restrict__ src, StreamParams &dst, int lane) {
@@ -645,8 +659,15 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
               decode_packet(reinterpret_cast<const uint32_t *>(&S.pd[kGroupsPerChunk * c]), sp, M.crc4, n0, rej, words, nbytes, crc_bad);
             }
           }
+          // 3b. BTLE_CFG_RECOVER (uniform per cfg): a counted packet whose CRC failed is demodulated again from the
+          //     capture's IQ, symbol-spaced on four sample phases; the lanes that need it run it together
           const unsigned base = __shfl_sync(0xFFFFFFFFu, my_base, 0);
-          if (live && base + (unsigned)j < cap)
+          bool stored = false;
+          if (sp.recover) {
+            if (live && crc_bad && !rej && base + (unsigned)j < cap)
+              stored = store_recovered(out + base + j, rec_stream, si.chunk0 + c, n0, sp, M.crc4, cap_base, n_int8, lead);
+          }
+          if (live && !stored && base + (unsigned)j < cap)
             store_record(out + base + j, rec_stream, si.chunk0 + c, n0, nbytes, crc_bad, rej, words, sp, cap_base, n_int8, lead);
         }
         // 4. only with report_rejected can a chunk have more hits than its row holds (degenerate masks, up to
@@ -662,6 +683,8 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
                 uint32_t words[11];
                 int nbytes, crc_bad;
                 decode_packet(pd, sp, crc4, n0, rej, words, nbytes, crc_bad);
+                if (sp.recover && crc_bad && !rej && store_recovered(out + first + i, stream, chunk, n0, sp, crc4, iq, n_int8, lead))
+                  return;                                             // as step 3b
                 store_record(out + first + i, stream, chunk, n0, nbytes, crc_bad, rej, words, sp, iq, n_int8, lead);
               }
             };
@@ -3465,6 +3488,7 @@ static int check_rx_ber_cfg(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg) {
   }
   if (std::fabs(cfg->ppm) >= 1e6f) { ctx->err = "rx_ber: ppm must have |ppm| < 1e6"; return BTLE_EINVAL; }
   if (cfg->amplitude < 1 || cfg->amplitude > 127) { ctx->err = "rx_ber: amplitude must be 1..127"; return BTLE_EINVAL; }
+  if (cfg->flags & ~(uint32_t)BTLE_CFG_RECOVER) { ctx->err = "rx_ber: flags may only hold BTLE_CFG_RECOVER"; return BTLE_EINVAL; }
   if (cfg->slot_samples < rx_ber_len(cfg->channel) || cfg->slot_samples > BTLE_RX_BER_MAX_SLOT) {
     ctx->err = "rx_ber: slot_samples must hold the packet (" + std::to_string(rx_ber_len(cfg->channel)) + " samples on this channel) and be at most " +
                std::to_string(BTLE_RX_BER_MAX_SLOT);
@@ -3567,7 +3591,7 @@ int btle_b200_rx_ber_run(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg, size_t 
   BTLE_CUDA(ctx, cudaEventCreate(&t.e0));
   BTLE_CUDA(ctx, cudaEventCreate(&t.e1));
   BTLE_CUDA(ctx, cudaEventRecord(t.e0, st));
-  const btle_stream_cfg scfg{cfg->channel, cfg->access_addr, 0xFFFFFFFFu, cfg->crc_init, 0, BTLE_CFG_REPORT_REJECTED};
+  const btle_stream_cfg scfg{cfg->channel, cfg->access_addr, 0xFFFFFFFFu, cfg->crc_init, 0, (int32_t)(BTLE_CFG_REPORT_REJECTED | cfg->flags)};
   int launches = 0;
   for (size_t done = 0; done < n_packets; done += max_b) {
     const size_t n = std::min(max_b, n_packets - done);

@@ -20,11 +20,24 @@ DEFAULT_CHANNEL = 37                 # btle_rx.c:230
 
 
 def make_cfgs(n_streams=1, channel=DEFAULT_CHANNEL, access_addr=DEFAULT_ACCESS_ADDR, access_mask=0xFFFFFFFF,
-              crc_init=DEFAULT_CRC_INIT, raw=0, rssi=0) -> np.ndarray:
-    """btle_stream_cfg array; every argument may be a scalar or a per-stream sequence."""
+              crc_init=DEFAULT_CRC_INIT, raw=0, rssi=0, recover=0) -> np.ndarray:
+    """btle_stream_cfg array; every argument may be a scalar or a per-stream sequence.  rssi holds the BTLE_CFG_* flag
+    bits; recover (true) adds BTLE_CFG_RECOVER: counted packets that fail the CRC are demodulated again
+    (include/btle_b200.h)."""
     c = np.zeros(n_streams, dtype=CFG_DTYPE)
     c["channel"], c["access_addr"], c["access_mask"] = channel, access_addr, access_mask
     c["crc_init"], c["raw"], c["rssi"] = crc_init, raw, rssi
+    c["rssi"] |= np.where(np.asarray(recover) != 0, _native.CFG_RECOVER, 0).astype(np.int32)
+    return c
+
+
+def _with_fields(c: np.ndarray, cfg: dict) -> np.ndarray:
+    """c (a btle_stream_cfg array) with the given make_cfgs fields changed; recover sets or clears BTLE_CFG_RECOVER"""
+    for k, v in cfg.items():
+        if k == "recover":
+            c["rssi"] = (c["rssi"] & ~_native.CFG_RECOVER) | (_native.CFG_RECOVER if v else 0)
+        else:
+            c[k] = v
     return c
 
 
@@ -377,9 +390,7 @@ class RxStreams:
 
     def set_cfg(self, stream: int, **cfg) -> None:
         """Change fields of capture `stream`'s cfg (make_cfgs names), from the next segment set that is submitted on."""
-        c = self._cfgs[int(stream):int(stream) + 1].copy() if 0 <= int(stream) < self.n_streams else make_cfgs(1)
-        for k, v in cfg.items():
-            c[k] = v
+        c = _with_fields(self._cfgs[int(stream):int(stream) + 1].copy() if 0 <= int(stream) < self.n_streams else make_cfgs(1), cfg)
         self._rx._check(self._L.btle_b200_streams_set_cfg(self._h, int(stream), c.ctypes.data))
         self._cfgs[int(stream)] = c[0]
 
@@ -397,9 +408,7 @@ class RxStreams:
         (index, from_chunk); records of this cfg carry `stream` = index.  Records of resident sets come back from the
         next push() or finish()."""
         capture = int(capture)
-        c = self._cfgs[capture:capture + 1].copy() if 0 <= capture < self.n_streams else make_cfgs(1)
-        for k, v in cfg.items():
-            c[k] = v
+        c = _with_fields(self._cfgs[capture:capture + 1].copy() if 0 <= capture < self.n_streams else make_cfgs(1), cfg)
         frm = self.resident if from_chunk is None else int(from_chunk)
         idx = ctypes.c_size_t(0)
         self._rx._check(self._L.btle_b200_streams_add_cfg(self._h, capture, c.ctypes.data, frm, ctypes.byref(idx)))

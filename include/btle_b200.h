@@ -68,10 +68,31 @@ typedef struct {
                             (:2234-2243); BTLE_CFG_REPORT_REJECTED (-v) 2: advertising-channel hits whose header
                             length is outside 6..37 — the reference prints "PktBAD" for them under -v and does not
                             count them (:2291-2298) — come back as records with BTLE_REC_REJECTED set, every one
-                            of them, in the reference's order (up to BTLE_MAX_RECS_PER_CHUNK records per chunk)  */
+                            of them, in the reference's order (up to BTLE_MAX_RECS_PER_CHUNK records per chunk);
+                            BTLE_CFG_RECOVER 4: CRC-failed packets are demodulated once more (below)            */
 } btle_stream_cfg;
 #define BTLE_CFG_RSSI 1
 #define BTLE_CFG_REPORT_REJECTED 2
+/* BTLE_CFG_RECOVER: opt-in recovery of packets that fail the CRC.  Not part of the reference's receiver; without it the
+ * records are the reference's, bit for bit.
+ * The chain (which hits are counted or rejected, their n0, restart points and length guards) is exactly the
+ * reference's, computed from the primary decode.  Then every COUNTED record with crc_bad == 1 of a cfg with the flag
+ * and raw == 0 is demodulated again:
+ *   1. window   capture samples are read only inside [8192 chunk, 8192 chunk + 9696) (receiver()'s demod_buf_len,
+ *               19392 int8); samples behind that range, or behind the capture's end, read as 0.  So the result does not
+ *               depend on how a capture was cut into batches, segments or sets.
+ *   2. bits     symbol-spaced: e[s] = (I[s] Q[s+4] - I[s+4] Q[s]) > 0, s relative to the chunk, products in int32.
+ *   3. alternatives q = 0, 1, 2, 3, tried in that order.  Packet bit j of alternative q (j = 0: first access-address
+ *               bit) is e[n0 + 4j + q - 2].  Bits j >= 32 are read into bytes, LSB first, and dewhitened with the
+ *               channel's table (as the primary decode).  The header length comes from the alternative's own header:
+ *               6 bits on channels 37..39, 5 bits on 0..36.  On advertising channels an alternative whose length is
+ *               outside 6..37 is skipped.  Otherwise n_bytes = length + 5 and the CRC is checked as crc_check() does.
+ *   4. result   the first alternative with a good CRC replaces the record's bytes (zero behind n_bytes) and n_bytes,
+ *               with crc_bad = 0; flags gets BTLE_REC_RECOVERED and q in bits 4..5.  stream, chunk, n0, channel,
+ *               access_addr and mag_sum stay.  If no alternative passes, the record is the reference's, byte for byte.
+ * Rejected (BTLE_CFG_REPORT_REJECTED) records, raw-mode records and CRC-ok records are never touched; the flag does
+ * nothing in raw mode. */
+#define BTLE_CFG_RECOVER 4
 
 /* One packet the reference would have counted (pkt_count++, btle_rx.c:2274/:2319). 64 bytes. */
 typedef struct {
@@ -83,7 +104,8 @@ typedef struct {
   uint8_t n_bytes;       /* 42 in raw mode, else 2 + payload_len + 3                          */
   uint8_t crc_bad;       /* crc_check() verdict, 1 = mismatch (btle_rx.c:2015); 0 in raw mode */
   uint8_t flags;         /* bit0 raw, bit1 advertising channel, bit2 BTLE_REC_REJECTED: not a packet the
-                            reference counts — only bytes[0..1] (the header) are valid, n_bytes = 2      */
+                            reference counts — only bytes[0..1] (the header) are valid, n_bytes = 2;
+                            bit3 BTLE_REC_RECOVERED: bytes from alternative q = bits 4..5 (BTLE_CFG_RECOVER) */
   uint32_t access_addr;
   uint16_t mag_sum;      /* sum |I|+|Q| over the 128 AA samples if cfg.rssi, else 0           */
   uint8_t bytes[42];     /* == reference tmp_byte[] (btle_rx.c:1485): dewhitened header,
@@ -91,6 +113,8 @@ typedef struct {
 } btle_pkt_rec;
 
 #define BTLE_REC_REJECTED 4
+#define BTLE_REC_RECOVERED 8
+#define BTLE_REC_RECOVERED_Q(flags) (((flags) >> 4) & 3)
 
 typedef struct btle_b200_ctx btle_b200_ctx;
 
@@ -444,7 +468,8 @@ int btle_b200_ber_synth_device(btle_b200_ctx *ctx, const btle_ber_cfg *cfg, uint
  *            0 .. S - L of its slot.  Every other sample is noise alone, rounded and saturated the same way.  The capture
  *            of packets first .. first+n-1 starts with slot `first` at sample 0 and is BTLE_RX_BER_CAPTURE_INT8(n, S) int8
  *            long: whole 8192-sample chunks, samples behind slot first+n-1 carrying noise only.
- *   receiver btle_rx_persistent_kernel<1> (btle_b200_rx_device_dir) with BTLE_CFG_REPORT_REJECTED, mask 0xFFFFFFFF.
+ *   receiver btle_rx_persistent_kernel<1> (btle_b200_rx_device_dir) with BTLE_CFG_REPORT_REJECTED | cfg.flags, mask
+ *            0xFFFFFFFF.
  *   scoring  packet k's record is the first record in reference order whose access-address sample chunk * 8192 + n0
  *            lies within +-3 of aa_sample (the synthesiser's access-address position, rounded).  pkt_err: no CRC-ok
  *            counted record; bit errors only in those packets, over the PDU bytes the record and the truth have in common
@@ -466,7 +491,8 @@ typedef struct {
   int32_t channel;         /* 0..39                                                                                 */
   uint32_t access_addr;
   uint32_t crc_init;       /* as -k                                                                                 */
-  uint32_t reserved[2];    /* 0                                                                                     */
+  uint32_t flags;          /* 0 or BTLE_CFG_RECOVER (given to the receiver); any other bit: BTLE_EINVAL             */
+  uint32_t reserved;       /* 0                                                                                     */
 } btle_rx_ber_cfg;         /* 48 bytes */
 typedef struct {
   int64_t aa_sample;       /* first access-address sample, from the start of the capture: slot start + offset +
@@ -491,7 +517,8 @@ typedef struct {
 /* n_packets packets 0 .. n_packets-1, in batches sized from free device memory; the result is independent of the batch
  * size (every batch starts on a chunk and slot boundary, and its look-ahead behind the last chunk is the next slots').
  * BTLE_EINVAL with btle_b200_last_error() for: snr_db, ppm or cfo_hz NaN or infinite, |ppm| >= 1e6, amplitude outside
- * 1..127, slot_samples below L or above BTLE_RX_BER_MAX_SLOT, channel > 39; the context stays usable. */
+ * 1..127, slot_samples below L or above BTLE_RX_BER_MAX_SLOT, channel > 39, a flags bit other than BTLE_CFG_RECOVER;
+ * the context stays usable. */
 int btle_b200_rx_ber_run(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg, size_t n_packets, btle_rx_ber_result *out);
 /* the capture and truth of packets first_packet .. first_packet + n_packets - 1 alone: d_iq (16-byte aligned) receives
  * BTLE_RX_BER_CAPTURE_INT8(n_packets, slot_samples) int8, d_truth n_packets rows.  Device pointers; enqueued on

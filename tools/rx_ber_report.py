@@ -2,7 +2,9 @@
 (btle_b200_ber_run) at the same SNR and ppm, plus the 4-Msps receiver under extra carrier offsets, and where the time of
 rx_ber_run goes (CUDA events around its three kernels on one batch).
 
-    python tools/rx_ber_report.py [--packets N] [--json out.json]
+    python tools/rx_ber_report.py [--packets N] [--json out.json] [--recover]
+
+--recover adds the 4-sps PER / BER with BTLE_CFG_RECOVER (CRC-failed packets demodulated again) next to the plain ones.
 
 Prints a markdown table (one row per point) and the throughput of both flows."""
 import argparse
@@ -57,6 +59,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--packets", type=int, default=20000)
     ap.add_argument("--json", default=None)
+    ap.add_argument("--recover", action="store_true", help="also measure the receiver with BTLE_CFG_RECOVER")
     args = ap.parse_args()
     rx = BtleRx(0)
     snrs = list(range(-5, 31))             # the 4-sps receiver's curve falls between 15 and 30 dB
@@ -64,17 +67,22 @@ def main():
     for ppm in (0.0, 20.0, 50.0):
         r4 = ber.rx_ber_sweep(snrs, args.packets, ppm=ppm, rx=rx)
         r8 = ber.ber_sweep(snrs, args.packets, ppm=ppm, rx=rx)
-        for a, b in zip(r4, r8):
-            rows.append({"ppm": ppm, "cfo_hz": 0.0, "rx4": a, "model8": b})
+        rr = ber.rx_ber_sweep(snrs, args.packets, ppm=ppm, rx=rx, recover=True) if args.recover else [None] * len(r4)
+        for a, b, c in zip(r4, r8, rr):
+            rows.append({"ppm": ppm, "cfo_hz": 0.0, "rx4": a, "model8": b, "rx4_recover": c})
     for cfo in (25e3, 50e3, 100e3, 150e3):
-        for a in ber.rx_ber_sweep(snrs, args.packets, cfo_hz=cfo, rx=rx):
-            rows.append({"ppm": 0.0, "cfo_hz": cfo, "rx4": a, "model8": None})
-    print(f"| ppm | cfo kHz | SNR dB | 4-sps PER | 4-sps BER | aa_miss | len_reject | extra | 8-sps model PER | 8-sps model BER |")
-    print("|---:|---:|---:|---:|---:|---:|---:|---:|---:|---:|")
+        r4 = ber.rx_ber_sweep(snrs, args.packets, cfo_hz=cfo, rx=rx)
+        rr = ber.rx_ber_sweep(snrs, args.packets, cfo_hz=cfo, rx=rx, recover=True) if args.recover else [None] * len(r4)
+        for a, c in zip(r4, rr):
+            rows.append({"ppm": 0.0, "cfo_hz": cfo, "rx4": a, "model8": None, "rx4_recover": c})
+    rec_h = " 4-sps PER recover | 4-sps BER recover |" if args.recover else ""
+    print(f"| ppm | cfo kHz | SNR dB | 4-sps PER | 4-sps BER |{rec_h} aa_miss | len_reject | extra | 8-sps model PER | 8-sps model BER |")
+    print("|---:|---:|---:|---:|---:|" + ("---:|---:|" if args.recover else "") + "---:|---:|---:|---:|---:|")
     for r in rows:
-        a, b = r["rx4"], r["model8"]
+        a, b, c = r["rx4"], r["model8"], r["rx4_recover"]
         m = f"{b['per']:.4f} | {b['ber']:.2e}" if b else "- | -"
-        print(f"| {r['ppm']:g} | {r['cfo_hz'] / 1e3:g} | {a['snr_db']:g} | {a['per']:.4f} | {a['ber']:.2e} | {a['aa_miss']} | {a['len_reject']} | "
+        rc = f" {c['per']:.4f} | {c['ber']:.2e} |" if c else ""
+        print(f"| {r['ppm']:g} | {r['cfo_hz'] / 1e3:g} | {a['snr_db']:g} | {a['per']:.4f} | {a['ber']:.2e} |{rc} {a['aa_miss']} | {a['len_reject']} | "
               f"{a['extra_recs']} | {m} |")
     r4 = [r["rx4"] for r in rows]
     r8 = [r["model8"] for r in rows if r["model8"]]
