@@ -71,10 +71,13 @@ EXPORTS = [
     "btle_b200_get_freq_by_channel_number", "btle_b200_chm_is_full_map", "btle_b200_discover", "btle_b200_discover_device",
     "btle_b200_rx_multi", "btle_b200_rx_multi_units", "btle_b200_rx_multi_device_dir",
     "btle_b200_streams_add_cfg", "btle_b200_streams_remove_cfg", "btle_b200_streams_resident", "btle_b200_streams_set_discover",
-    "btle_b200_streams_take_cands",
+    "btle_b200_streams_take_cands", "btle_b200_rx_batch_offset", "btle_b200_rx_device_dir_offset", "btle_b200_rx_multi_offset",
+    "btle_b200_rx_multi_device_dir_offset", "btle_b200_rec_offset_device", "btle_b200_rec_offset",
+    "btle_b200_streams_set_offset", "btle_b200_stream_set_offset",
 ]
 MAX_CFGS_PER_CAPTURE = 8       # BTLE_MAX_CFGS_PER_CAPTURE
 CFG_RSSI, CFG_REPORT_REJECTED, CFG_RECOVER = 1, 2, 4      # btle_stream_cfg.rssi flag bits (BTLE_CFG_*)
+MAX_OFFSET_HZ = 500000       # BTLE_MAX_OFFSET_HZ: largest |offset_hz| of the carrier-offset correction
 REC_REJECTED, REC_RECOVERED = 4, 8                        # btle_pkt_rec.flags bits; a recovered record's alternative q is flags >> 4 & 3
 
 
@@ -171,6 +174,14 @@ def load():
     L.btle_b200_streams_resident.argtypes = [vp, i64p]
     L.btle_b200_streams_set_discover.argtypes = [vp, vp]
     L.btle_b200_streams_take_cands.argtypes = [vp, vp, sz, ctypes.POINTER(sz)]
+    L.btle_b200_rx_batch_offset.argtypes = [vp, vp, sz, sz, sz, vp, vp, vp, sz, ctypes.POINTER(sz)]
+    L.btle_b200_rx_device_dir_offset.argtypes = [vp, vp, sz, sz, sz, vp, vp, vp, sz, vp, vp, sz, vp]
+    L.btle_b200_rx_multi_offset.argtypes = [vp, vp, sz, sz, sz, vp, vp, sz, vp, vp, sz, ctypes.POINTER(sz)]
+    L.btle_b200_rx_multi_device_dir_offset.argtypes = [vp, vp, sz, sz, sz, vp, vp, sz, vp, vp, sz, vp, vp, sz, vp]
+    L.btle_b200_rec_offset_device.argtypes = [vp, vp, sz, sz, vp, sz, vp, vp]
+    L.btle_b200_rec_offset.argtypes = [vp, vp, sz, sz, sz, vp, sz, vp]
+    L.btle_b200_streams_set_offset.argtypes = [vp, sz, ctypes.c_float]
+    L.btle_b200_stream_set_offset.argtypes = [vp, ctypes.c_float]
     _lib = L
     return L
 

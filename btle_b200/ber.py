@@ -53,19 +53,59 @@ def rx_ber_cfg(snr_db: float, ppm: float = 0.0, cfo_hz: float = 0.0, amplitude: 
     return cfg
 
 
+def _rx_ber_corrected(rx: BtleRx, cfg: np.ndarray, n_packets: int, offset_hz: float) -> np.ndarray:
+    """btle_b200_rx_ber_run's counters with the receiver corrected by offset_hz: rx_ber_synth_device -> the rotated receive
+    kernel (rx_device_dir with offset_hz) -> rx_ber_score_device.  Batches of whole slots, each a capture of its own (its
+    last chunk's look-ahead is noise, not the next batch's slots); one batch up to 8192 chunks, as btle_b200_rx_ber_run."""
+    import torch
+    from .rx import make_cfgs
+    dev = torch.device("cuda", rx.device)
+    st = torch.cuda.current_stream(dev)
+    S = int(cfg["slot_samples"][0])
+    per_batch = max(1, 8192 * 8192 // S)
+    scfg = make_cfgs(1, channel=int(cfg["channel"][0]), access_addr=int(cfg["access_addr"][0]), crc_init=int(cfg["crc_init"][0]),
+                     rssi=_native.CFG_REPORT_REJECTED | int(cfg["flags"][0]))
+    d_res = torch.zeros(_native.RX_BER_RESULT_DTYPE.itemsize, dtype=torch.uint8, device=dev)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(st)
+    for done in range(0, n_packets, per_batch):
+        n = min(per_batch, n_packets - done)
+        chunks = (n * S + 8191) // 8192
+        d_iq = torch.empty((1, chunks * 16384), dtype=torch.int8, device=dev)
+        d_truth = torch.empty(n * _native.RX_BER_TRUTH_DTYPE.itemsize, dtype=torch.uint8, device=dev)
+        rx._check(rx._L.btle_b200_rx_ber_synth_device(rx._h, cfg.ctypes.data, done, n, d_iq.data_ptr(), d_truth.data_ptr(), st.cuda_stream))
+        cap, units = chunks * 123, rx.units(1, chunks * 16384)           # BTLE_MAX_RECS_PER_CHUNK per chunk
+        d_out = torch.empty(cap * 64, dtype=torch.uint8, device=dev)
+        d_dir = torch.empty(max(units, 1) * 8, dtype=torch.uint8, device=dev)
+        rx.rx_device_dir(d_iq, scfg, d_out, None, d_dir, st.cuda_stream, offset_hz=offset_hz)
+        rx._check(rx._L.btle_b200_rx_ber_score_device(rx._h, d_truth.data_ptr(), n, d_out.data_ptr(), cap, d_dir.data_ptr(), units,
+                                                      d_res.data_ptr(), st.cuda_stream))
+    e1.record(st)
+    st.synchronize()
+    res = d_res.cpu().numpy().view(_native.RX_BER_RESULT_DTYPE).copy()
+    res["seconds"] = e0.elapsed_time(e1) * 1e-3
+    return res
+
+
 def rx_ber_point(rx: BtleRx, snr_db: float, n_packets: int, ppm: float = 0.0, cfo_hz: float = 0.0, amplitude: int = 64,
                  slot_samples: int = 2048, channel: int = 37, crc_init: int = 0x555555, access_addr: int = 0x8E89BED6, seed: int = 1,
-                 recover: bool = False) -> dict:
+                 recover: bool = False, offset_hz: float | None = None) -> dict:
     """PER / BER of the reference's 4-Msps int8 receiver (btle_rx_persistent_kernel) at one channel point: ber_point()'s dict
     plus cfo_hz, amplitude and the counters len_reject, crc_ok_wrong, extra_recs, extra_crc_ok and clipped.
-    generated_iq_gbytes_per_s counts the int8 capture the run synthesised and decoded (2 bytes per sample)."""
+    generated_iq_gbytes_per_s counts the int8 capture the run synthesised and decoded (2 bytes per sample).
+    offset_hz: the receiver corrects that carrier offset (the *_offset entry points; the sign of cfo_hz, so offset_hz =
+    cfo_hz undoes the impairment); None: btle_b200_rx_ber_run, uncorrected."""
     cfg = rx_ber_cfg(snr_db, ppm, cfo_hz, amplitude, slot_samples, channel, crc_init, access_addr, seed, recover)
-    res = np.zeros(1, dtype=_native.RX_BER_RESULT_DTYPE)
-    rx._check(rx._L.btle_b200_rx_ber_run(rx._h, cfg.ctypes.data, int(n_packets), res.ctypes.data))
+    if offset_hz is None:
+        res = np.zeros(1, dtype=_native.RX_BER_RESULT_DTYPE)
+        rx._check(rx._L.btle_b200_rx_ber_run(rx._h, cfg.ctypes.data, int(n_packets), res.ctypes.data))
+    else:
+        res = _rx_ber_corrected(rx, cfg, int(n_packets), float(offset_hz))
     r = res[0]
     c = {k: int(r[k]) for k in _native.RX_BER_COUNTERS}
     sec = float(r["seconds"])
-    return {"snr_db": float(snr_db), "ppm": float(ppm), "cfo_hz": float(cfo_hz), "amplitude": int(amplitude), "recover": bool(recover), **c,
+    return {"snr_db": float(snr_db), "ppm": float(ppm), "cfo_hz": float(cfo_hz), "amplitude": int(amplitude), "recover": bool(recover),
+            "offset_hz": offset_hz, **c,
             "ber": c["bit_err"] / max(c["bit_total"], 1), "per": c["pkt_err"] / max(c["packets"], 1), "seconds": sec,
             "packets_per_s": c["packets"] / sec if sec > 0 else 0.0,
             "generated_iq_gbytes_per_s": c["packets"] * slot_samples * 2 / sec / 1e9 if sec > 0 else 0.0}
@@ -73,8 +113,8 @@ def rx_ber_point(rx: BtleRx, snr_db: float, n_packets: int, ppm: float = 0.0, cf
 
 def rx_ber_sweep(snr_db, n_packets: int, ppm: float = 0.0, cfo_hz: float = 0.0, amplitude: int = 64, slot_samples: int = 2048,
                  channel: int = 37, crc_init: int = 0x555555, access_addr: int = 0x8E89BED6, seed: int = 1, device: int = 0,
-                 rx: BtleRx | None = None, recover: bool = False):
+                 rx: BtleRx | None = None, recover: bool = False, offset_hz: float | None = None):
     """One rx_ber_point dict per SNR point (seeds as ber_sweep)."""
     rx = rx or BtleRx(device)
-    return [rx_ber_point(rx, s, n_packets, ppm, cfo_hz, amplitude, slot_samples, channel, crc_init, access_addr, seed + 7919 * k, recover)
-            for k, s in enumerate(snr_db)]
+    return [rx_ber_point(rx, s, n_packets, ppm, cfo_hz, amplitude, slot_samples, channel, crc_init, access_addr, seed + 7919 * k, recover,
+                         offset_hz) for k, s in enumerate(snr_db)]

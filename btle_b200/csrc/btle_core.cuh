@@ -345,6 +345,62 @@ BTLE_DENSE void dbits_group_dense(WordAt &word, uint32_t acc[4]) {
 #undef BTLE_DENSE_STEP
 }
 
+// ---- carrier-offset correction (the *_offset entry points, include/btle_b200.h) -----------------------------------------
+// d[n] = C (I0 Q1 - I1 Q0) - S (I0 I1 + Q0 Q1) > 0, (C, S) = round(2^14 (cos, sin) phi).  As a sign: d = 1 <=> u < 0 with
+// u = C v + S r, v = Q0 I1 - I0 Q1, r = I0 I1 + Q0 Q1.  |v|, |r| <= 2^15 and |C|, |S| <= 2^14, so |u| < 2^30: exact in int32.
+BTLE_HD int rot_disc(int i0, int q0, int i1, int q1, int c, int s) { return c * (q0 * i1 - i0 * q1) + s * (i0 * i1 + q0 * q1); }
+// Dense form, per sample: v as dbits8() builds it (one byte-permute of the I-complemented word, two IDP.2A against the raw
+// bytes of the next sample), r from one byte-permute of the raw word ([sext16 I | sext16 Q]) and one IDP.2A, then two
+// integer multiply-adds; the sign bits are gathered as in dbits8_dense (add_bits reads only the sign of u).
+#if defined(__CUDACC__)
+template <unsigned SEL>
+__device__ __forceinline__ int prmt1(uint32_t w) {
+  int r;
+  asm("prmt.b32 %0, %1, 0, %2;" : "=r"(r) : "r"(w), "n"(SEL));
+  return r;
+}
+#else
+template <unsigned SEL>
+inline int prmt1(uint32_t w) { return (int)prmt_b32(w, 0u, SEL); }
+#endif
+// u of the sample in bytes (2 HALF, 2 HALF + 1) of w (wc = w with its I bytes complemented); b holds the next sample in
+// its bytes (0, 1) when HALF is 1 and (2, 3) when HALF is 0
+template <int HALF>
+BTLE_DENSE int rot_u(uint32_t w, uint32_t wc, uint32_t b, int c, int s) {
+  const int a_im = prmt1<HALF ? 0xA2B3u : 0x8091u>(wc), a_re = prmt1<HALF ? 0xB3A2u : 0x9180u>(w);
+  const int v = HALF ? __dp2a_lo(a_im, (int)b, __dp2a_lo(0x00010000, (int)b, 0)) : __dp2a_hi(a_im, (int)b, __dp2a_hi(0x00010000, (int)b, 0));
+  const int r = HALF ? __dp2a_lo(a_re, (int)b, 0) : __dp2a_hi(a_re, (int)b, 0);
+  return c * v + s * r;
+}
+template <int CM>
+BTLE_DENSE void dbits8_rot(uint32_t w0, uint32_t w1, uint32_t w2, uint32_t w3, uint32_t wnext, int c, int s, uint32_t acc[4]) {
+  const uint32_t c0 = w0 ^ 0x00FF00FFu, c1 = w1 ^ 0x00FF00FFu, c2 = w2 ^ 0x00FF00FFu, c3 = w3 ^ 0x00FF00FFu;
+  const int t0 = rot_u<0>(w0, c0, w0, c, s), t1 = rot_u<1>(w0, c0, w1, c, s);
+  const int t2 = rot_u<0>(w1, c1, w1, c, s), t3 = rot_u<1>(w1, c1, w2, c, s);
+  const int t4 = rot_u<0>(w2, c2, w2, c, s), t5 = rot_u<1>(w2, c2, w3, c, s);
+  const int t6 = rot_u<0>(w3, c3, w3, c, s), t7 = rot_u<1>(w3, c3, wnext, c, s);
+  acc[0] = add_bits<CM>(acc[0], t0, t4);
+  acc[1] = add_bits<CM>(acc[1], t1, t5);
+  acc[2] = add_bits<CM>(acc[2], t2, t6);
+  acc[3] = add_bits<CM>(acc[3], t3, t7);
+}
+// dbits_group_dense() with the rotated discriminator
+template <class WordAt>
+BTLE_DENSE void dbits_group_rot(WordAt &word, int c, int s, uint32_t acc[4]) {
+  uint32_t carry = word(64);
+  for (int C = 15; C >= 0; --C) {
+    const uint32_t w0 = word(4 * C), w1 = word(4 * C + 1), w2 = word(4 * C + 2), w3 = word(4 * C + 3);
+    if ((C & 3) == 3) { acc[0] <<= 8; acc[1] <<= 8; acc[2] <<= 8; acc[3] <<= 8; }
+    switch (C & 3) {
+      case 3: dbits8_rot<3>(w0, w1, w2, w3, carry, c, s, acc); break;
+      case 2: dbits8_rot<2>(w0, w1, w2, w3, carry, c, s, acc); break;
+      case 1: dbits8_rot<1>(w0, w1, w2, w3, carry, c, s, acc); break;
+      default: dbits8_rot<0>(w0, w1, w2, w3, carry, c, s, acc); break;
+    }
+    carry = w0;
+  }
+}
+
 // Dense-pass prefilter: bit i of the result is 1 iff the window starting at symbol i of `lo`
 // agrees with the access address on the (<=16) prefilter taps.  A superset of the true matches;
 // the sparse pass re-checks every candidate exactly (search_from()).
@@ -701,7 +757,9 @@ BTLE_HD void iq_at(const IqWindow &w, int s, int &i, int &q) {
   if (s >= 0 && s < w.n) { i = w.iq[2 * s]; q = w.iq[2 * s + 1]; }
 }
 // Symbol-spaced discriminator bits: bit k of the result is e[s0 + 4k], e[s] = (I[s] Q[s+4] - I[s+4] Q[s]) > 0.
-BTLE_HD uint32_t sym_bits32(const IqWindow &w, int s0) {
+// ROT: e[s] = C4 (I[s] Q[s+4] - I[s+4] Q[s]) - S4 (I[s] I[s+4] + Q[s] Q[s+4]) > 0 (rot_disc with the 4-sample rotation).
+template <bool ROT = false>
+BTLE_HD uint32_t sym_bits32(const IqWindow &w, int s0, int c4 = 0, int s4 = 0) {
   int i0, q0;
   iq_at(w, s0, i0, q0);
   uint32_t r = 0u;
@@ -709,7 +767,8 @@ BTLE_HD uint32_t sym_bits32(const IqWindow &w, int s0) {
   for (int k = 0; k < 32; ++k) {
     int i1, q1;
     iq_at(w, s0 + 4 * k + 4, i1, q1);
-    r |= (uint32_t)(i0 * q1 - i1 * q0 > 0) << k;
+    if constexpr (ROT) r |= (uint32_t)(rot_disc(i0, q0, i1, q1, c4, s4) < 0) << k;
+    else r |= (uint32_t)(i0 * q1 - i1 * q0 > 0) << k;
     i0 = i1;
     q0 = q1;
   }
@@ -718,23 +777,25 @@ BTLE_HD uint32_t sym_bits32(const IqWindow &w, int s0) {
 // One counted packet whose access address starts at sample n0 and whose primary decode failed the CRC: alternatives
 // q = 0..3 (packet bit j = e[n0 + 4j + q - 2]) in order; the first whose CRC is good wins.  Returns q and writes that
 // alternative's bytes (words[11], zero behind n_bytes, as decode_packet) and n_bytes; returns -1 and leaves both
-// untouched when none passes.  Not for raw mode (sp.recover is 0 there).
-BTLE_HD int recover_packet(const IqWindow &w, const StreamParams &sp, const uint32_t *crc4, int n0, uint32_t words[11], int &nbytes_out) {
+// untouched when none passes.  Not for raw mode (sp.recover is 0 there).  ROT: the bits of sym_bits32<true>(.., c4, s4).
+template <bool ROT = false>
+BTLE_HD int recover_packet(const IqWindow &w, const StreamParams &sp, const uint32_t *crc4, int n0, uint32_t words[11], int &nbytes_out,
+                           int c4 = 0, int s4 = 0) {
   for (int q = 0; q < 4; ++q) {
     const int s0 = n0 + 4 * 32 + q - 2;                  // packet bit 32: the first header bit
     uint32_t alt[11];
-    alt[0] = sym_bits32(w, s0) ^ sp.whiten[0];
+    alt[0] = sym_bits32<ROT>(w, s0, c4, s4) ^ sp.whiten[0];
     const int plen = (int)((alt[0] >> 8) & (sp.adv ? 0x3Fu : 0x1Fu));
     if (sp.adv && (plen < 6 || plen > 37)) continue;
     const int nbytes = plen + 5, nw = (nbytes + 3) >> 2, body = nbytes - 3;
     const uint32_t last_mask = (nbytes & 3) ? ((1u << (8 * (nbytes & 3))) - 1u) : 0xFFFFFFFFu;
 #pragma unroll
-    for (int j = 1; j < 11; ++j) alt[j] = j < nw ? sym_bits32(w, s0 + 4 * 32 * j) ^ sp.whiten[j] : 0u;
+    for (int j = 1; j < 11; ++j) alt[j] = j < nw ? sym_bits32<ROT>(w, s0 + 4 * 32 * j, c4, s4) ^ sp.whiten[j] : 0u;
 #pragma unroll
     for (int j = 0; j < 11; ++j)
       if (j == nw - 1) alt[j] &= last_mask;
     const uint32_t crc = crc24_words(alt, body, sp.crc_init, crc4);
-    const uint32_t rx = (sym_bits32(w, s0 + 4 * 8 * body) ^ whiten32(sp, body)) & 0xFFFFFFu;
+    const uint32_t rx = (sym_bits32<ROT>(w, s0 + 4 * 8 * body, c4, s4) ^ whiten32(sp, body)) & 0xFFFFFFu;
     if (crc == rx) {
 #pragma unroll
       for (int j = 0; j < 11; ++j) words[j] = alt[j];

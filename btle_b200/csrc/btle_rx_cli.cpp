@@ -14,7 +14,7 @@
 //       -i/--iq-file FILE        raw interleaved int8 (what rx_callback writes, btle_rx.c:531-540), '-' = stdin.  Read in
 //                                64 MiB segments straight into page-locked memory and decoded while the next segment is
 //                                being read (btle_b200_stream_*): the capture may be larger than host RAM or HBM.
-//       -i FILE:CH[:AA[:CRCINIT]]  (repeatable) several time-aligned captures (files or FIFOs, '-' for one of them),
+//       -i FILE:CH[:AA[:CRCINIT[:HZ]]]  (repeatable) several time-aligned captures (files or FIFOs, '-' for one of them),
 //                                each with its own channel / access address / CRC init.  Streamed through one session
 //                                (btle_b200_streams_*): poll() across the inputs, each segment set decoded in one
 //                                batched launch while the next one is read; packets are printed in time order, up to
@@ -36,6 +36,7 @@
 #include <fcntl.h>
 #include <getopt.h>
 #include <poll.h>
+#include <sys/stat.h>
 #include <signal.h>
 #include <unistd.h>
 
@@ -71,13 +72,15 @@ struct Options {
   uint32_t aa = 0x8E89BED6u, crc_init = 0x555555u, mask = 0xFFFFFFFFu;
   uint64_t freq_hz = 123;
   const char *pcap = nullptr, *iq_txt = nullptr, *iq_sc16 = nullptr, *iq_dir = nullptr, *iq_bin16 = nullptr;
-  std::vector<std::string> iq_files;            // -i, possibly FILE:CH[:AA[:CRCINIT]]
+  std::vector<std::string> iq_files;            // -i, possibly FILE:CH[:AA[:CRCINIT[:HZ]]] (HZ: --offset)
   size_t segment_chunks = 0;                    // 0: the session default
   int filter_adva_set = 0;
   uint8_t filter_adva[6] = {0, 0, 0, 0, 0, 0};
   uint16_t filter_pdu_mask = 0xFFFF;
   int device = 0;
   int connections = 0;                          // --connections
+  int offset_set = 0, offset_auto = 0;          // --offset HZ / --offset auto
+  float offset_hz = 0.0f;
 };
 
 void usage() {
@@ -111,6 +114,9 @@ void usage() {
       "    -j --json / -Q --quiet-text / -R --rssi-est\n"
       "       --recover\n      packets whose CRC fails are demodulated once more, symbol-spaced on four sample phases; the first\n"
       "      phase whose CRC is ok replaces the packet (printed as CRC0; NDJSON adds \"recovered\":q).  Not with -o or --iq-bin16\n"
+      "       --offset HZ|auto\n      carrier-offset correction of every capture, HZ = received minus nominal carrier (|HZ| <= 500000); a capture\n"
+      "      given as FILE:CH:AA:CRCINIT:HZ takes its own.  auto (regular files only): a first pass without correction, the\n"
+      "      median offset estimate of its CRC-ok packets printed on stderr, then the decode with it.  Not with --iq-bin16\n"
       "    -F --filter-adva AA:BB:CC:DD:EE:FF / -T --filter-pdu-type 0,3,4\n"
       "    -d --device N   CUDA device (default 0)\n");
 }
@@ -158,7 +164,8 @@ Options parse_commandline(int argc, char **argv) {
       {"filter-pdu-type", required_argument, 0, 'T'}, {"iq-file", required_argument, 0, 'i'},
       {"iq-txt", required_argument, 0, 1000}, {"iq-sc16", required_argument, 0, 1001}, {"device", required_argument, 0, 'd'},
       {"iq-dir", required_argument, 0, 1002}, {"segment-chunks", required_argument, 0, 1003}, {"iq-bin16", required_argument, 0, 1004},
-      {"connections", no_argument, 0, 1005}, {"recover", no_argument, 0, 1006}, {0, 0, 0, 0}};
+      {"connections", no_argument, 0, 1005}, {"recover", no_argument, 0, 1006},
+      {"offset", required_argument, 0, 1007}, {0, 0, 0, 0}};
   for (;;) {
     int idx = 0;
     const int c = getopt_long(argc, argv, "hc:g:l:ba:k:vrf:m:os:jQRF:T:i:d:", longopts, &idx);   // + i:, d:
@@ -185,6 +192,15 @@ Options parse_commandline(int argc, char **argv) {
       case 1004: o.iq_bin16 = optarg; break;
       case 1005: o.connections = 1; break;
       case 1006: o.recover = 1; break;
+      case 1007:
+        o.offset_set = 1;
+        if (!strcmp(optarg, "auto")) { o.offset_auto = 1; break; }
+        o.offset_hz = strtof(optarg, &endp);
+        if (endp == optarg || *endp || !std::isfinite(o.offset_hz) || std::fabs(o.offset_hz) > (float)BTLE_MAX_OFFSET_HZ) {
+          printf("Invalid --offset value: %s (expect Hz within +-%d, or auto)\n", optarg, BTLE_MAX_OFFSET_HZ);
+          bad_args();
+        }
+        break;
       case 1003: o.segment_chunks = (size_t)strtoul(optarg, &endp, 10); break;
       case 1000: o.iq_txt = optarg; break;
       case 1001: o.iq_sc16 = optarg; break;
@@ -212,6 +228,8 @@ Options parse_commandline(int argc, char **argv) {
   if (o.connections && (!o.iq_dir || o.hop)) { printf("--connections needs --iq-dir and cannot be combined with -o\n"); bad_args(); }
   // -o follows as the reference's follower does, from the reference's records; --iq-bin16 has a receiver of its own
   if (o.recover && (o.hop || o.iq_bin16)) { printf("--recover cannot be combined with -o or --iq-bin16\n"); bad_args(); }
+  // the 8-sps model receiver has no carrier-offset correction
+  if (o.offset_set && o.iq_bin16) { printf("--offset cannot be combined with --iq-bin16 (the 8-sps receiver has no offset correction)\n"); bad_args(); }
   return o;
 }
 
@@ -467,11 +485,20 @@ double rec_time(const btle_pkt_rec &r) { return ((double)r.chunk * 8192.0 + r.n0
 volatile sig_atomic_t g_stop = 0;
 void on_sigint(int) { g_stop = 1; }                                             // btle_rx.c:100-104
 
-struct Capture { std::string file; int chan; uint32_t aa, crc_init; };
+struct Capture { std::string file; int chan; uint32_t aa, crc_init; float hz; bool own_hz; };
 
-// "FILE[:CH[:AA[:CRCINIT]]]"
+// a whole decimal number of Hz within the correction's range
+bool parse_hz(const std::string &f, float *hz) {
+  char *e = nullptr;
+  const float v = strtof(f.c_str(), &e);
+  if (f.empty() || *e || !std::isfinite(v) || std::fabs(v) > (float)BTLE_MAX_OFFSET_HZ) return false;
+  *hz = v;
+  return true;
+}
+
+// "FILE[:CH[:AA[:CRCINIT[:HZ]]]]"
 Capture parse_capture(const std::string &spec, const Options &o) {
-  Capture c{spec, o.chan, o.aa, o.crc_init};
+  Capture c{spec, o.chan, o.aa, o.crc_init, o.offset_hz, false};
   std::vector<std::string> parts;
   size_t pos = 0;
   for (;;) {
@@ -479,6 +506,18 @@ Capture parse_capture(const std::string &spec, const Options &o) {
     parts.push_back(spec.substr(pos, q == std::string::npos ? q : q - pos));
     if (q == std::string::npos) break;
     pos = q + 1;
+  }
+  // FILE:CH:AA:CRCINIT:HZ: the fifth field is the capture's carrier offset (may be negative)
+  if (parts.size() >= 5) {
+    float hz;
+    bool hexes = true;
+    for (size_t k = parts.size() - 4; k < parts.size() - 1; ++k)
+      hexes &= !parts[k].empty() && parts[k].find_first_not_of("0123456789abcdefABCDEF") == std::string::npos;
+    if (hexes && parse_hz(parts.back(), &hz)) {
+      c.hz = hz;
+      c.own_hz = true;
+      parts.pop_back();
+    }
   }
   // a ':' inside a path: only trailing fields that look like numbers are taken as parameters
   size_t nfield = 0;
@@ -501,19 +540,42 @@ int cfg_flags(const Options &o) {
   return (o.rssi ? BTLE_CFG_RSSI : 0) | (o.verbose ? BTLE_CFG_REPORT_REJECTED : 0) | (o.recover ? BTLE_CFG_RECOVER : 0);
 }
 
-// rx_batch with a capacity that is grown once if the library asks
+// rx_batch with a capacity that is grown once if the library asks; offset_hz: one per capture, or NULL (no correction)
 int rx_batch_grow(btle_b200_ctx *ctx, const int8_t *iq, size_t ns, size_t stride, size_t n, const btle_stream_cfg *cfgs,
-                  std::vector<btle_pkt_rec> &recs) {
+                  std::vector<btle_pkt_rec> &recs, const float *offset_hz = nullptr) {
   size_t cap = ns * (n / BTLE_CHUNK_INT8) * 4 + 1024, got = 0;
   int rc = 0;
   for (int attempt = 0; attempt < 2; ++attempt) {
     recs.resize(cap);
-    rc = btle_b200_rx_batch(ctx, iq, ns, stride, n, cfgs, recs.data(), cap, &got);
+    rc = btle_b200_rx_batch_offset(ctx, iq, ns, stride, n, cfgs, offset_hz, recs.data(), cap, &got);
     if (rc != BTLE_EOVERFLOW) break;
     cap = got;
   }
   recs.resize(rc ? 0 : got);
   return rc;
+}
+
+// --offset auto: the median of btle_b200_rec_offset over the CRC-ok counted packets of a first pass without correction
+// (not raw, no flags); 0 when no packet passes.  *n_ok = the packets it took.
+int estimate_offset(btle_b200_ctx *ctx, const std::vector<int8_t> &iq, btle_stream_cfg cfg, float *hz, size_t *n_ok) {
+  cfg.raw = 0;
+  cfg.rssi = 0;
+  std::vector<btle_pkt_rec> recs;
+  *hz = 0.0f;
+  *n_ok = 0;
+  int rc = rx_batch_grow(ctx, iq.data(), 1, iq.size(), iq.size(), &cfg, recs);
+  if (rc) return rc;
+  recs.erase(std::remove_if(recs.begin(), recs.end(), [](const btle_pkt_rec &r) { return r.crc_bad || (r.flags & BTLE_REC_REJECTED); }),
+             recs.end());
+  if (recs.empty()) return 0;
+  std::vector<float> e(recs.size());
+  rc = btle_b200_rec_offset(ctx, iq.data(), 1, iq.size(), iq.size(), recs.data(), recs.size(), e.data());
+  if (rc) return rc;
+  std::sort(e.begin(), e.end());
+  const size_t m = e.size() / 2;
+  *hz = e.size() & 1 ? e[m] : 0.5f * (e[m - 1] + e[m]);
+  *n_ok = e.size();
+  return 0;
 }
 
 // ---- hop mode: a virtual radio over per-channel captures (receiver_controller semantics) -------------------------
@@ -734,13 +796,35 @@ int main(int argc, char **argv) {
       snprintf(name, sizeof name, "%s/ch%02d.bin", o.iq_dir, ch);
       if (access(name, R_OK) != 0) continue;
       const bool adv = ch >= 37;
-      caps.push_back(Capture{name, ch, adv ? 0x8E89BED6u : o.aa, adv ? 0x555555u : o.crc_init});
+      caps.push_back(Capture{name, ch, adv ? 0x8E89BED6u : o.aa, adv ? 0x555555u : o.crc_init, o.offset_hz, false});
     }
     if (caps.empty()) { printf("no chNN.bin capture found in %s\n", o.iq_dir); btle_b200_destroy(ctx); return 1; }
   }
   for (const Capture &c : caps)
     if (c.chan < 0 || c.chan > 39) { printf("channel number must be within 0~%d!\n", 39); btle_b200_destroy(ctx); return 1; }
   if (o.connections && caps.size() != 40) { printf("--connections needs all 40 chNN.bin captures in %s\n", o.iq_dir); btle_b200_destroy(ctx); return 1; }
+  // carrier-offset correction: --offset HZ for every capture, FILE:CH:AA:CRCINIT:HZ for one, --offset auto from a first pass
+  bool use_off = o.offset_set;
+  for (const Capture &c : caps) use_off |= c.own_hz;
+  if (o.offset_auto) {
+    for (Capture &c : caps) {
+      if (c.own_hz) continue;
+      struct stat sb;
+      if (c.file == "-" || stat(c.file.c_str(), &sb) != 0 || !S_ISREG(sb.st_mode)) {
+        printf("--offset auto needs regular files (%s is not one)\n", c.file.c_str());
+        btle_b200_destroy(ctx);
+        return 1;
+      }
+      std::vector<int8_t> iq;
+      if (!load_raw(c.file.c_str(), iq)) { btle_b200_destroy(ctx); return 1; }
+      size_t n_ok = 0;
+      rc = estimate_offset(ctx, iq, btle_stream_cfg{c.chan, c.aa, o.mask, c.crc_init, 0, 0}, &c.hz, &n_ok);
+      if (rc) return fail("--offset auto");
+      fprintf(stderr, "offset estimate %s: %.1f Hz (%zu CRC-ok packets)\n", c.file.c_str(), c.hz, n_ok);
+    }
+  }
+  std::vector<float> hz_of(40, 0.0f);                        // -o: the offset of each channel's capture
+  for (const Capture &c : caps) hz_of[c.chan] = c.hz;
 
   if (o.iq_bin16) {
     // ---- 8 samples per symbol: the Python / Verilog model's receiver, streaming over the capture -------------------------
@@ -785,7 +869,7 @@ int main(int argc, char **argv) {
     // pass A: the start channel with the command line's access address, all chunks
     std::vector<btle_pkt_rec> recs;
     btle_stream_cfg cfg0{o.chan, o.aa, o.mask, o.crc_init, o.raw, cfg_flags(o)};
-    rc = rx_batch_grow(ctx, iq[o.chan].data(), 1, n, n, &cfg0, recs);
+    rc = rx_batch_grow(ctx, iq[o.chan].data(), 1, n, n, &cfg0, recs, use_off ? &hz_of[o.chan] : nullptr);
     if (rc) return fail("btle_b200_rx_batch");
     size_t ri = 0;
     long long k = 0;
@@ -803,12 +887,14 @@ int main(int argc, char **argv) {
       for (int c = 0; c < 37; ++c) if (!iq[c].empty()) chan_of.push_back(c);
       std::vector<int8_t> stage(stride * chan_of.size());
       std::vector<btle_stream_cfg> cfgs;
+      std::vector<float> hz;
       for (size_t s_ = 0; s_ < chan_of.size(); ++s_) {
         memcpy(stage.data() + s_ * stride, iq[chan_of[s_]].data() + off, n2);
         cfgs.push_back(btle_stream_cfg{chan_of[s_], st->access_addr, o.mask, st->crc_init, o.raw, cfg_flags(o)});
+        hz.push_back(hz_of[chan_of[s_]]);
       }
       std::vector<btle_pkt_rec> data;
-      rc = rx_batch_grow(ctx, stage.data(), chan_of.size(), stride, n2, cfgs.data(), data);
+      rc = rx_batch_grow(ctx, stage.data(), chan_of.size(), stride, n2, cfgs.data(), data, use_off ? hz.data() : nullptr);
       if (rc) return fail("btle_b200_rx_batch");
       // index: first record of every (stream, chunk)
       std::vector<size_t> first(chan_of.size() * (size_t)(nchunks - k) + 1, 0);
@@ -860,6 +946,8 @@ int main(int argc, char **argv) {
     btle_b200_streams *ss = nullptr;
     rc = btle_b200_streams_open(ctx, cfgs.data(), ns, o.segment_chunks, &ss);
     if (rc) { close_inputs(); return fail("btle_b200_streams_open"); }
+    for (size_t s_ = 0; s_ < ns && use_off && !rc; ++s_) rc = btle_b200_streams_set_offset(ss, s_, caps[s_].hz);
+    if (rc) { btle_b200_streams_close(ss); close_inputs(); return fail("btle_b200_streams_set_offset"); }
     ConnMonitor mon(ss, o);
     if (o.connections && mon.begin()) { rc = mon.rc; btle_b200_streams_close(ss); close_inputs(); return fail("--connections"); }
     std::vector<btle_pkt_rec> recs(65536), pending;
@@ -958,13 +1046,27 @@ int main(int argc, char **argv) {
     std::vector<int8_t> iq;
     if (o.iq_sc16 ? !load_raw(o.iq_sc16, iq) : !load_txt(o.iq_txt, iq)) { btle_b200_destroy(ctx); return 1; }
     btle_stream_cfg cfg{o.chan, o.aa, o.mask, o.crc_init, o.raw, cfg_flags(o)};
+    float hz = o.offset_hz;
+    if (o.offset_set && o.iq_sc16) {                                     // the reduction of btle_b200_rx_iq16, here on the host
+      const int16_t *p16 = reinterpret_cast<const int16_t *>(iq.data());
+      std::vector<int8_t> r(iq.size() / 2);
+      for (size_t i = 0; i < r.size(); ++i) r[i] = (int8_t)((p16[i] >> 4) & 0xFF);      // btle_rx.c:307-308
+      iq.swap(r);
+      o.iq_sc16 = nullptr;
+    }
+    if (o.offset_auto) {
+      size_t n_ok = 0;
+      rc = estimate_offset(ctx, iq, cfg, &hz, &n_ok);
+      if (rc) return fail("--offset auto");
+      fprintf(stderr, "offset estimate %s: %.1f Hz (%zu CRC-ok packets)\n", o.iq_txt ? o.iq_txt : "capture", hz, n_ok);
+    }
     const size_t n_iq = o.iq_sc16 ? iq.size() / 2 : iq.size();          // int8 values after the optional reduction
     size_t cap = (n_iq / BTLE_CHUNK_INT8) * 4 + 1024, n = 0;
     std::vector<btle_pkt_rec> recs;
     for (int attempt = 0; attempt < 2; ++attempt) {
       recs.resize(cap);
       if (o.iq_sc16) rc = btle_b200_rx_iq16(ctx, reinterpret_cast<const int16_t *>(iq.data()), n_iq, 4, &cfg, recs.data(), cap, &n);   // btle_rx.c:307-308
-      else rc = btle_b200_rx(ctx, iq.data(), iq.size(), &cfg, recs.data(), cap, &n);
+      else rc = btle_b200_rx_batch_offset(ctx, iq.data(), 1, iq.size(), iq.size(), &cfg, o.offset_set ? &hz : nullptr, recs.data(), cap, &n);
       if (rc != BTLE_EOVERFLOW) break;
       cap = n;
     }
@@ -980,6 +1082,7 @@ int main(int argc, char **argv) {
     btle_b200_stream *st = nullptr;
     rc = btle_b200_stream_open(ctx, &cfg, o.segment_chunks, &st);
     if (rc) return fail("btle_b200_stream_open");
+    if (use_off && (rc = btle_b200_stream_set_offset(st, c.hz))) { btle_b200_stream_close(st); return fail("btle_b200_stream_set_offset"); }
     std::vector<btle_pkt_rec> recs(65536);
     size_t total = 0;
     const int fd = fileno(f);

@@ -237,11 +237,13 @@ __device__ __forceinline__ void store_record(btle_pkt_rec *dst, int stream, int 
 // BTLE_CFG_RECOVER: stores the record of a counted packet whose primary decode failed the CRC when one of its
 // alternatives passes (recover_packet) and returns true; false: nothing stored, the caller stores the primary decode.
 // Out of line, so that the decode pass keeps its registers and the launches of cfgs without the flag pay one branch.
+// ROT: the symbol-spaced bits are rotated by (c4, s4) (carrier-offset correction).
+template <bool ROT>
 __device__ __forceinline__ bool store_recovered(btle_pkt_rec *dst, int stream, int chunk, int n0, const StreamParams &sp, const uint32_t *crc4,
-                                             const int8_t *iq, long long n_int8, long long lead) {
+                                             const int8_t *iq, long long n_int8, long long lead, int c4 = 0, int s4 = 0) {
   uint32_t words[11];
   int nbytes = 0;
-  const int q = recover_packet(iq_window(iq, n_int8, chunk), sp, crc4, n0, words, nbytes);
+  const int q = recover_packet<ROT>(iq_window(iq, n_int8, chunk), sp, crc4, n0, words, nbytes, c4, s4);
   if (q < 0) return false;
   store_record(dst, stream, chunk, n0, nbytes, 0, false, words, sp, iq, n_int8, lead, recovered_flags(q));
   return true;
@@ -285,14 +287,17 @@ __device__ __forceinline__ void load_multi_warp(const StreamParams *__restrict__
 // capture's IQ still becomes phase words once; the candidate words are the union of its cfgs' prefilters, and the resolver
 // runs steps 1a-4 once per cfg, each run with its own directory entry: cfg j's units sit at j * (units per group) + the
 // unit's index inside its group, so the directory walks in (cfg, chunk, n0) order.  Records carry stream = cfg index.
-template <int KC>
+// ROT (the *_offset entry points): rot[i] = {C, S, C4, S4} of cfg i (make_rot); the dense warps build the phase words from
+// the rotated discriminator (dbits8_rot, with the rotation of the capture's first cfg) and recovery rotates its
+// symbol-spaced bits by (C4, S4).  Without ROT, rot is not read.
+template <int KC, bool ROT>
 __global__ void __launch_bounds__(kThreads, kCtasPerSm)
 btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __grid_constant__ CUtensorMap map12,
                           const int8_t *__restrict__ iq, long long stream_stride, long long n_int8,
                           const StreamParams *__restrict__ params, const Plan plan,
                           btle_pkt_rec *__restrict__ out, unsigned cap, unsigned *__restrict__ count,
                           uint2 *__restrict__ dir, unsigned *__restrict__ zero_next, long long lead,
-                          const int4 *__restrict__ vmap) {
+                          const int4 *__restrict__ vmap, const int4 *__restrict__ rot) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Smem<KC> &M = *reinterpret_cast<Smem<KC> *>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -413,7 +418,7 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
   if (warp < kDenseWarps) {
     // =============================== dense producers ===============================
     uint32_t tma_phase = 0;                               // parity to wait for on the tile's mbarrier
-    int rot = 0, k = 0;
+    int rot_w = 0, k = 0;
     WaitClock w_all, w_tma, w_empty;
     w_all.begin();
     for (int unit = blockIdx.x; unit < total_units; unit += gridDim.x, ++k) {
@@ -425,7 +430,13 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
       w_empty.end();
       const UnitInfo si = unit_info(unit, plan);
       const int8_t *cap_base = iq + (long long)capture_of(si.stream) * stream_stride;
-      int t = warp - rot;
+      int rc = 0, rs = 0;                                 // (C, S) of the capture
+      if constexpr (ROT) {
+        const int4 r = __ldg(rot + (KC == 1 ? si.stream : __ldg(&vmap[si.stream].y)));
+        rc = r.x;
+        rs = r.y;
+      }
+      int t = warp - rot_w;
       if (t < 0) t += kDenseWarps;
       for (; t < si.tiles; t += kDenseWarps) {
         const int rows = min(32, si.groups - t * 32);
@@ -488,13 +499,28 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
             const uint32_t first = reinterpret_cast<const uint4 *>(row + (sw << 4))->x;
             uint32_t nb = __shfl_down_sync(0xFFFFFFFFu, first, 1);
             if (lane == rows - 1) nb = tail;
-            vtop = sext8<3>(wtop) * sext8<0>(nb) - sext8<2>(wtop) * sext8<1>(nb);
+            if constexpr (ROT) vtop = rot_disc(sext8<2>(wtop), sext8<3>(wtop), sext8<0>(nb), sext8<1>(nb), rc, rs);
+            else vtop = sext8<3>(wtop) * sext8<0>(nb) - sext8<2>(wtop) * sext8<1>(nb);
           }
           if (lane < rows) {
 #pragma unroll
             for (int cc = 7; cc >= 0; --cc) {
               const uint4 w = *reinterpret_cast<const uint4 *>(row + ((((uint32_t)cc ^ sw)) << 4));
               if (half == 1 && cc == 7) wtop = w.w;
+              if constexpr (ROT) {
+                if ((cc & 3) == 3) {
+#pragma unroll
+                  for (int ph = 0; ph < 4; ++ph) acc[ph] <<= 8;
+                }
+                switch (cc & 3) {
+                  case 3: dbits8_rot<3>(w.x, w.y, w.z, w.w, carry, rc, rs, acc); break;
+                  case 2: dbits8_rot<2>(w.x, w.y, w.z, w.w, carry, rc, rs, acc); break;
+                  case 1: dbits8_rot<1>(w.x, w.y, w.z, w.w, carry, rc, rs, acc); break;
+                  default: dbits8_rot<0>(w.x, w.y, w.z, w.w, carry, rc, rs, acc); break;
+                }
+                carry = w.x;
+                continue;
+              }
 #ifdef BTLE_DBITS_PUSH
               dbits8(w.x, w.y, w.z, w.w, carry, acc);
 #else
@@ -538,7 +564,7 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
           if (t == si.tiles - 1) S.pd[si.groups] = make_uint4(0u, 0u, 0u, 0u);
         }
       }
-      rot = (rot + si.tiles) % kDenseWarps;
+      rot_w = (rot_w + si.tiles) % kDenseWarps;
       __syncwarp();
       if (lane == 0) mbar_arrive(&M.full[b]);             // release: this warp's share of the unit is published
       BTLE_STAMP(3);
@@ -603,6 +629,12 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
         }
         const StreamParams &sp = *spp;
         const int rec_stream = KC == 1 ? si.stream : cfg0 + jc;
+        int c4 = 0, s4 = 0;                                 // (C4, S4) of the cfg: recovery's rotation
+        if constexpr (ROT) {
+          const int4 r = __ldg(rot + rec_stream);
+          c4 = r.z;
+          s4 = r.w;
+        }
         const int dir_at = KC == 1 ? unit : (cfg0 + jc) * per_group + local;
         // 1a. exact access-address hits of the unit, all lanes (lane = flag word = 32 groups): the only data-dependent search
         for (int t = lane; t < 2 * si.nch; t += 32)
@@ -665,7 +697,7 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
           bool stored = false;
           if (sp.recover) {
             if (live && crc_bad && !rej && base + (unsigned)j < cap)
-              stored = store_recovered(out + base + j, rec_stream, si.chunk0 + c, n0, sp, M.crc4, cap_base, n_int8, lead);
+              stored = store_recovered<ROT>(out + base + j, rec_stream, si.chunk0 + c, n0, sp, M.crc4, cap_base, n_int8, lead, c4, s4);
           }
           if (live && !stored && base + (unsigned)j < cap)
             store_record(out + base + j, rec_stream, si.chunk0 + c, n0, nbytes, crc_bad, rej, words, sp, cap_base, n_int8, lead);
@@ -677,19 +709,19 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
           if (mine > kHitCap) {
             struct Late {
               const uint32_t *pd; const StreamParams &sp; const uint32_t *crc4;
-              btle_pkt_rec *out; unsigned first, cap; int stream, chunk; const int8_t *iq; long long n_int8, lead;
+              btle_pkt_rec *out; unsigned first, cap; int stream, chunk; const int8_t *iq; long long n_int8, lead; int c4, s4;
               __device__ __forceinline__ void operator()(int i, int n0, bool rej) {
                 if (i < kHitCap || first + (unsigned)i >= cap) return;
                 uint32_t words[11];
                 int nbytes, crc_bad;
                 decode_packet(pd, sp, crc4, n0, rej, words, nbytes, crc_bad);
-                if (sp.recover && crc_bad && !rej && store_recovered(out + first + i, stream, chunk, n0, sp, crc4, iq, n_int8, lead))
+                if (sp.recover && crc_bad && !rej && store_recovered<ROT>(out + first + i, stream, chunk, n0, sp, crc4, iq, n_int8, lead, c4, s4))
                   return;                                             // as step 3b
                 store_record(out + first + i, stream, chunk, n0, nbytes, crc_bad, rej, words, sp, iq, n_int8, lead);
               }
             };
             const uint32_t *pdc = reinterpret_cast<const uint32_t *>(&S.pd[kGroupsPerChunk * lane]);
-            Late late{pdc, sp, M.crc4, out, base + RS.pre[lane], cap, rec_stream, si.chunk0 + lane, cap_base, n_int8, lead};
+            Late late{pdc, sp, M.crc4, out, base + RS.pre[lane], cap, rec_stream, si.chunk0 + lane, cap_base, n_int8, lead, c4, s4};
             const int c0 = RS.xh[2 * lane][kExactCap], c1 = RS.xh[2 * lane + 1][kExactCap];
             if (c0 > kExactCap || c1 > kExactCap)
               chain_chunk(pdc, &S.cand[kGroupsPerChunk * lane], &S.flagw[2 * lane], sp, late);
@@ -924,6 +956,48 @@ __device__ __forceinline__ void build_air(const uint8_t *pdu, int pdu_len, uint3
     sb[5 + b] = v ^ (uint8_t)(c_whiten_words[channel][b >> 2] >> (8 * (b & 3)));
   }
   for (int b = 5 + pdu_len + 3; b < n_sb; ++b) sb[b] = 0;
+}
+
+// ---- per-packet carrier-offset estimate (btle_b200_rec_offset_device; definition in include/btle_b200.h) -------------
+// One warp per record.  Turn k (k = 0 .. kOffTurns-1) is arg(conj(x[n]) x[n+1]), n = n0 - 32 + k, read through the record's
+// chunk window (iq_window); the reference turn is the same over the btle_tx waveform (gfsk_block<4>: phase before
+// frequency word m, int8 table samples) of the preamble and access address alone, tx sample m = n - n0 +
+// BTLE_RX_BER_AA_OFFSET.  The turns end 4 samples before the header: later ones see its first bit through the filter.
+constexpr int kOffLead = 32, kOffTurns = 156;
+__device__ __forceinline__ int tx4_freq(const uint8_t *sb, int nbit, int m) {   // frequency word m of gfsk_block<4>
+  int acc = 0;
+#pragma unroll
+  for (int j = 3; j <= 11; ++j) {
+    const int idx = m + j - 15;
+    if (idx >= 0 && (idx & 3) == 0 && (idx >> 2) < nbit) acc += c_gauss4[j - 3] * (((sb[idx >> 5] >> ((idx >> 2) & 7)) & 1) ? 1 : -1);
+  }
+  return acc;
+}
+__global__ void rec_offset_kernel(const int8_t *__restrict__ iq, long long stride, long long n_int8, const btle_pkt_rec *__restrict__ recs,
+                                  long long n, float *__restrict__ hz) {
+  const long long r = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (r >= n) return;
+  const int stream = recs[r].stream, chunk = recs[r].chunk, n0 = recs[r].n0;
+  const uint32_t aa = recs[r].access_addr;
+  const uint8_t sb[5] = {(uint8_t)((aa & 1u) ? 0x55 : 0xAA), (uint8_t)aa, (uint8_t)(aa >> 8), (uint8_t)(aa >> 16), (uint8_t)(aa >> 24)};
+  const IqWindow w = iq_window(iq + (long long)stream * stride, n_int8, chunk);
+  const int m_first = BTLE_RX_BER_AA_OFFSET - kOffLead;
+  int ph = 0, m = 0;                                        // phase before frequency word m of the reference
+  float sum = 0.0f;
+  for (int k = lane; k < kOffTurns; k += 32) {
+    for (; m < m_first + k; ++m) ph += tx4_freq(sb, 40, m);
+    const int p1 = ph + tx4_freq(sb, 40, m);
+    const int ri0 = c_cos1024[ph & 1023], rq0 = c_sin1024[ph & 1023], ri1 = c_cos1024[p1 & 1023], rq1 = c_sin1024[p1 & 1023];
+    int i0, q0, i1, q1;
+    iq_at(w, n0 - kOffLead + k, i0, q0);
+    iq_at(w, n0 - kOffLead + k + 1, i1, q1);
+    sum += atan2f((float)(i0 * q1 - q0 * i1), (float)(i0 * i1 + q0 * q1)) -
+           atan2f((float)(ri0 * rq1 - rq0 * ri1), (float)(ri0 * ri1 + rq0 * rq1));
+  }
+#pragma unroll
+  for (int d = 16; d >= 1; d >>= 1) sum += __shfl_xor_sync(0xFFFFFFFFu, sum, d);
+  if (lane == 0) hz[r] = sum * (float)(4e6 / (6.283185307179586 * kOffTurns));
 }
 
 // The transmit PHY on a batch of air-byte rows: samples past a packet's own, up to the longest row's, are zero.
@@ -1775,6 +1849,10 @@ struct CfgSlot {                     // one uploaded btle_stream_cfg array + the
   Buf<int4> d_vmap;
   HostBuf<int4> h_vmap;
   size_t n_vmap = 0;
+  // the *_offset entry points: {C, S, C4, S4} per cfg (make_rot), part of the key; empty: the launch is not rotated
+  std::vector<int4> rot;
+  Buf<int4> d_rot;
+  HostBuf<int4> h_rot;
   unsigned long long up_stream = 0;  // stream the upload was enqueued on
   cudaEvent_t uploaded = nullptr;    // recorded behind the upload's two copies
   StreamUse use[kSlotUsers];         // last launch of each stream that read this upload
@@ -1799,6 +1877,7 @@ struct btle_b200_ctx {
   Buf<int8_t> d_iq;
   Buf<btle_pkt_rec> d_out;
   Buf<btle_unit_dir> d_dir;
+  Buf<float> d_hz;                      // btle_b200_rec_offset's estimates
   Buf<unsigned> d_count;
   Buf<unsigned> d_count_ring;       // kCountRing allocation counters for launches that do not hand in their own (no memset node)
   unsigned ring_pos = 0;
@@ -1886,12 +1965,14 @@ int stream_id(btle_b200_ctx *ctx, cudaStream_t st, unsigned long long *sid) {
 // The copies come from page-locked staging, so enqueueing them never blocks the host behind a busy stream; the host
 // waits only when it must rewrite a staging buffer whose previous copy has not run yet.
 // cfg_capture (btle_b200_rx_multi, else nullptr): cfg i decodes capture cfg_capture[i]; already validated.
+// rot (the *_offset entry points, else nullptr): n rotations, uploaded with the parameters and part of the key.
 int upload_cfgs(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size_t n, cudaStream_t st, unsigned long long sid, CfgSlot **slot_out,
-                const int32_t *cfg_capture = nullptr) {
+                const int32_t *cfg_capture = nullptr, const int4 *rot = nullptr) {
   CfgSlot *pick = nullptr;
   for (CfgSlot &c : ctx->cfg_slot)
     if (c.n == n && c.multi == (cfg_capture != nullptr) && !memcmp(c.h, cfgs, n * sizeof(btle_stream_cfg)) &&
-        (!cfg_capture || !memcmp(c.cfg_capture.data(), cfg_capture, n * sizeof(int32_t)))) { pick = &c; break; }
+        (!cfg_capture || !memcmp(c.cfg_capture.data(), cfg_capture, n * sizeof(int32_t))) &&
+        c.rot.empty() == (rot == nullptr) && (!rot || !memcmp(c.rot.data(), rot, n * sizeof(int4)))) { pick = &c; break; }
   if (pick) {
     bool seen = pick->up_stream == sid;
     for (const StreamUse &u : pick->use) seen |= u.stamp && u.stream == sid;
@@ -1913,6 +1994,7 @@ int upload_cfgs(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size_t n, cudaS
       return BTLE_ENOMEM;
     // (h_vmap grows in step with h: when it is kept, so is h, and the wait above covered its previous copy)
     if (cfg_capture && (pick->d_vmap.reserve(ctx, n) || pick->h_vmap.reserve(ctx, n))) return BTLE_ENOMEM;
+    if (rot && (pick->d_rot.reserve(ctx, n) || pick->h_rot.reserve(ctx, n))) return BTLE_ENOMEM;
     for (StreamUse &u : pick->use) u.stamp = 0;              // ordered before the new copies by the waits above
     memcpy(pick->h, cfgs, n * sizeof(btle_stream_cfg));
     for (size_t i = 0; i < n; ++i) {                         // make_params(): btle_params.h, the same code the CPU emulator runs
@@ -1933,6 +2015,11 @@ int upload_cfgs(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size_t n, cudaS
         ++pick->h_vmap[pick->n_vmap - 1].z;
       }
       BTLE_CUDA(ctx, cudaMemcpyAsync(pick->d_vmap, pick->h_vmap, pick->n_vmap * sizeof(int4), cudaMemcpyHostToDevice, st));
+    }
+    pick->rot.assign(rot ? rot : nullptr, rot ? rot + n : nullptr);
+    if (rot) {
+      memcpy(pick->h_rot, rot, n * sizeof(int4));
+      BTLE_CUDA(ctx, cudaMemcpyAsync(pick->d_rot, pick->h_rot, n * sizeof(int4), cudaMemcpyHostToDevice, st));
     }
     BTLE_CUDA(ctx, cudaEventRecord(pick->uploaded, st));
     pick->up_stream = sid;
@@ -2022,9 +2109,29 @@ size_t multi_units_per_group(const btle_b200_ctx *ctx, size_t groups, size_t n_i
 // enqueue the persistent kernel for device-resident inputs; `lead`: bytes readable in front of each capture (the
 // stream session's lead: RSSI of hits at a segment's very start); cfg_capture != nullptr: several cfgs per capture
 // (n_cfgs of them, checked by check_cfg_capture), the directory in (cfg, chunk) order
+// {C, S, C4, S4} of a carrier offset (include/btle_b200.h): round(2^14 (cos, sin)) of phi and of 4 phi, phi = 2 pi hz / 4 MHz
+int4 make_rot(float hz) {
+  const double ph = 6.283185307179586476925286766559 * (double)hz / 4e6;
+  return make_int4((int)lrint(16384.0 * cos(ph)), (int)lrint(16384.0 * sin(ph)), (int)lrint(16384.0 * cos(4.0 * ph)),
+                   (int)lrint(16384.0 * sin(4.0 * ph)));
+}
+// rotations of n cfgs from one offset per capture (cfg i reads capture cap_of[i], or i when cap_of is nullptr)
+int make_rots(btle_b200_ctx *ctx, const float *offset_hz, size_t n_captures, const int32_t *cap_of, size_t n, std::vector<int4> &rot) {
+  for (size_t c = 0; c < n_captures; ++c)
+    if (!std::isfinite(offset_hz[c]) || std::fabs(offset_hz[c]) > (float)BTLE_MAX_OFFSET_HZ) {
+      ctx->err = "offset_hz must be finite and within +-BTLE_MAX_OFFSET_HZ";
+      return BTLE_EINVAL;
+    }
+  rot.resize(n);
+  for (size_t i = 0; i < n; ++i) rot[i] = make_rot(offset_hz[cap_of ? cap_of[i] : i]);
+  return BTLE_OK;
+}
+
+// rot != nullptr: one rotation per cfg (make_rot), the rotated kernel variant
 int launch_rx(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8,
               const btle_stream_cfg *cfgs, btle_pkt_rec *d_out, size_t cap, unsigned *d_count, btle_unit_dir *d_dir,
-              cudaStream_t st, long long lead, const int32_t *cfg_capture = nullptr, size_t n_cfgs = 0, size_t groups = 0) {
+              cudaStream_t st, long long lead, const int32_t *cfg_capture = nullptr, size_t n_cfgs = 0, size_t groups = 0,
+              const int4 *rot = nullptr) {
   ctx->last_launches = 0;
   unsigned *zero_next = nullptr;
   if (d_count) BTLE_CUDA(ctx, cudaMemsetAsync(d_count, 0, sizeof(unsigned), st));
@@ -2042,7 +2149,7 @@ int launch_rx(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t s
     return BTLE_EINVAL;
   }
   CfgSlot *cs = nullptr;
-  rc = upload_cfgs(ctx, cfgs, multi ? n_cfgs : n_streams, st, sid, &cs, cfg_capture);
+  rc = upload_cfgs(ctx, cfgs, multi ? n_cfgs : n_streams, st, sid, &cs, cfg_capture, rot);
   if (rc) return rc;
   const MapSlot *ms = nullptr;
   rc = get_maps(ctx, d_iq, n_streams, stride, n_int8, &ms);
@@ -2061,14 +2168,24 @@ int launch_rx(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t s
     zero_next = ctx->d_count_ring + (ctx->ring_pos + kCountRing / 2) % kCountRing;
   }
   const unsigned grid = (unsigned)std::min<long long>(plan.total_units, (long long)ctx->num_sms * kCtasPerSm);   // one persistent CTA per SM
-  if (multi)
-    btle_rx_persistent_kernel<kMaxCfgsPerCapture><<<grid, kThreads, sizeof(Smem<kMaxCfgsPerCapture>), st>>>(
-        ms->map32, ms->map12, d_iq, (long long)stride, (long long)n_int8, cs->d_params, plan, d_out,
-        (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu), d_count, reinterpret_cast<uint2 *>(d_dir), zero_next, lead, cs->d_vmap);
+  const unsigned cap32 = (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu);
+  uint2 *dir2 = reinterpret_cast<uint2 *>(d_dir);
+  if (multi && rot)
+    btle_rx_persistent_kernel<kMaxCfgsPerCapture, true><<<grid, kThreads, sizeof(Smem<kMaxCfgsPerCapture>), st>>>(
+        ms->map32, ms->map12, d_iq, (long long)stride, (long long)n_int8, cs->d_params, plan, d_out, cap32, d_count, dir2, zero_next, lead,
+        cs->d_vmap, cs->d_rot);
+  else if (multi)
+    btle_rx_persistent_kernel<kMaxCfgsPerCapture, false><<<grid, kThreads, sizeof(Smem<kMaxCfgsPerCapture>), st>>>(
+        ms->map32, ms->map12, d_iq, (long long)stride, (long long)n_int8, cs->d_params, plan, d_out, cap32, d_count, dir2, zero_next, lead,
+        cs->d_vmap, nullptr);
+  else if (rot)
+    btle_rx_persistent_kernel<1, true><<<grid, kThreads, sizeof(Smem<1>), st>>>(
+        ms->map32, ms->map12, d_iq, (long long)stride, (long long)n_int8, cs->d_params, plan, d_out, cap32, d_count, dir2, zero_next, lead,
+        nullptr, cs->d_rot);
   else
-    btle_rx_persistent_kernel<1><<<grid, kThreads, sizeof(Smem<1>), st>>>(
-        ms->map32, ms->map12, d_iq, (long long)stride, (long long)n_int8, cs->d_params, plan, d_out,
-        (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu), d_count, reinterpret_cast<uint2 *>(d_dir), zero_next, lead, nullptr);
+    btle_rx_persistent_kernel<1, false><<<grid, kThreads, sizeof(Smem<1>), st>>>(
+        ms->map32, ms->map12, d_iq, (long long)stride, (long long)n_int8, cs->d_params, plan, d_out, cap32, d_count, dir2, zero_next, lead,
+        nullptr, nullptr);
   BTLE_CUDA(ctx, cudaGetLastError());
   if (ring) {                                                 // the position is taken only by a launch that was enqueued
     ctx->ring_pos = (ctx->ring_pos + 1) % kCountRing;
@@ -2344,8 +2461,11 @@ int btle_b200_create(btle_b200_ctx **out, int cuda_device) {
   if (cudaMemcpyToSymbol(c_noise_thr, thr, sizeof thr) != cudaSuccess ||
       cudaMemcpyToSymbol(c_whiten_words, ww, sizeof ww) != cudaSuccess ||
       cudaMemcpyToSymbol(c_crc4, crc, sizeof crc) != cudaSuccess ||
-      cudaFuncSetAttribute(btle_rx_persistent_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem<1>)) != cudaSuccess ||
-      cudaFuncSetAttribute(btle_rx_persistent_kernel<kMaxCfgsPerCapture>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+      cudaFuncSetAttribute(btle_rx_persistent_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem<1>)) != cudaSuccess ||
+      cudaFuncSetAttribute(btle_rx_persistent_kernel<kMaxCfgsPerCapture, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (int)sizeof(Smem<kMaxCfgsPerCapture>)) != cudaSuccess ||
+      cudaFuncSetAttribute(btle_rx_persistent_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem<1>)) != cudaSuccess ||
+      cudaFuncSetAttribute(btle_rx_persistent_kernel<kMaxCfgsPerCapture, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            (int)sizeof(Smem<kMaxCfgsPerCapture>)) != cudaSuccess ||
       cudaFuncSetAttribute(sps8_hits_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSps8Smem) != cudaSuccess ||
       cudaFuncSetAttribute(discover_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDiscSmem) != cudaSuccess ||
@@ -2378,16 +2498,25 @@ size_t btle_b200_rx_units(const btle_b200_ctx *ctx, size_t n_streams, size_t n_i
   return (size_t)plan_for(ctx, n_streams, n_int8).total_units;
 }
 
-int btle_b200_rx_device_dir(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8,
-                            const btle_stream_cfg *cfgs, btle_pkt_rec *d_out, size_t cap, uint32_t *d_count,
-                            btle_unit_dir *d_dir, size_t dir_cap, void *cuda_stream) {
+int btle_b200_rx_device_dir_offset(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8,
+                                   const btle_stream_cfg *cfgs, const float *offset_hz, btle_pkt_rec *d_out, size_t cap, uint32_t *d_count,
+                                   btle_unit_dir *d_dir, size_t dir_cap, void *cuda_stream) {
   if (!ctx || (!d_out && cap) || (!cfgs && n_streams) || !d_dir) return BTLE_EINVAL;
   if ((reinterpret_cast<uintptr_t>(d_iq) & 15) || (n_streams > 1 && (stride & 15))) { ctx->err = "device IQ must be 16-byte aligned"; return BTLE_EINVAL; }
   if (dir_cap < btle_b200_rx_units(ctx, n_streams, n_int8)) { ctx->err = "unit directory too small (btle_b200_rx_units)"; return BTLE_EINVAL; }
   int rc = validate_cfgs(ctx, cfgs, n_streams);
   if (rc) return rc;
+  std::vector<int4> rot;
+  if (offset_hz && (rc = make_rots(ctx, offset_hz, n_streams, nullptr, n_streams, rot))) return rc;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
-  return launch_rx(ctx, d_iq, n_streams, stride, n_int8, cfgs, d_out, cap, d_count, d_dir, reinterpret_cast<cudaStream_t>(cuda_stream), 0);
+  return launch_rx(ctx, d_iq, n_streams, stride, n_int8, cfgs, d_out, cap, d_count, d_dir, reinterpret_cast<cudaStream_t>(cuda_stream), 0,
+                   nullptr, 0, 0, offset_hz ? rot.data() : nullptr);
+}
+
+int btle_b200_rx_device_dir(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8,
+                            const btle_stream_cfg *cfgs, btle_pkt_rec *d_out, size_t cap, uint32_t *d_count,
+                            btle_unit_dir *d_dir, size_t dir_cap, void *cuda_stream) {
+  return btle_b200_rx_device_dir_offset(ctx, d_iq, n_streams, stride, n_int8, cfgs, nullptr, d_out, cap, d_count, d_dir, dir_cap, cuda_stream);
 }
 
 int btle_b200_rx_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8,
@@ -2419,8 +2548,8 @@ int btle_b200_gather_ordered(const btle_pkt_rec *recs, size_t n_recs, const btle
   return total > cap || pos < total ? BTLE_EOVERFLOW : BTLE_OK;
 }
 
-int btle_b200_rx_batch(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stride, size_t n_int8,
-                       const btle_stream_cfg *cfgs, btle_pkt_rec *out, size_t cap, size_t *n_out) {
+int btle_b200_rx_batch_offset(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stride, size_t n_int8,
+                              const btle_stream_cfg *cfgs, const float *offset_hz, btle_pkt_rec *out, size_t cap, size_t *n_out) {
   if (!ctx || !n_out || (!out && cap) || (!cfgs && n_streams) || (!iq && n_streams && n_int8)) return BTLE_EINVAL;
   *n_out = 0;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -2428,11 +2557,51 @@ int btle_b200_rx_batch(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, s
   size_t pitch = 0;
   int rc = ingest(ctx, iq, n_streams, stride, n_int8, &pitch);
   if (rc) return rc;
-  rc = ctx->d_out.reserve(ctx, std::max<size_t>(cap, 1));
+  const size_t units = btle_b200_rx_units(ctx, n_streams, n_int8);
+  if (ctx->d_out.reserve(ctx, std::max<size_t>(cap, 1)) || ctx->d_dir.reserve(ctx, std::max<size_t>(units, 1))) return BTLE_ENOMEM;
+  rc = btle_b200_rx_device_dir_offset(ctx, ctx->d_iq, n_streams, pitch, n_int8, cfgs, offset_hz, ctx->d_out, cap, ctx->d_count, ctx->d_dir,
+                                      ctx->d_dir.n, st);
   if (rc) return rc;
-  rc = btle_b200_rx_device(ctx, ctx->d_iq, n_streams, pitch, n_int8, cfgs, ctx->d_out, cap, ctx->d_count, st);
+  return fetch_ordered(ctx, ctx->d_out, ctx->d_dir, units, out, cap, n_out, st);
+}
+
+int btle_b200_rx_batch(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stride, size_t n_int8,
+                       const btle_stream_cfg *cfgs, btle_pkt_rec *out, size_t cap, size_t *n_out) {
+  return btle_b200_rx_batch_offset(ctx, iq, n_streams, stride, n_int8, cfgs, nullptr, out, cap, n_out);
+}
+
+int btle_b200_rec_offset_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t stride, size_t n_int8, const btle_pkt_rec *d_recs, size_t n,
+                                float *d_hz, void *cuda_stream) {
+  if (!ctx) return BTLE_EINVAL;
+  if (n && (!d_recs || !d_hz || (!d_iq && n_int8))) { ctx->err = "rec_offset: missing buffer"; return BTLE_EINVAL; }
+  if (!n) return BTLE_OK;
+  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
+  const long long blocks = ((long long)n + 7) / 8;                 // 8 warps (records) per block
+  if (blocks > 0x7FFFFFFFll) { ctx->err = "rec_offset: too many records"; return BTLE_EINVAL; }
+  rec_offset_kernel<<<(unsigned)blocks, 256, 0, reinterpret_cast<cudaStream_t>(cuda_stream)>>>(d_iq, (long long)stride, (long long)n_int8, d_recs,
+                                                                                           (long long)n, d_hz);
+  BTLE_CUDA(ctx, cudaGetLastError());
+  return BTLE_OK;
+}
+
+int btle_b200_rec_offset(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stride, size_t n_int8, const btle_pkt_rec *recs, size_t n,
+                         float *hz) {
+  if (!ctx || (n && (!recs || !hz)) || (!iq && n_streams && n_int8)) return BTLE_EINVAL;
+  for (size_t i = 0; i < n; ++i)
+    if (recs[i].stream < 0 || (size_t)recs[i].stream >= n_streams) { ctx->err = "rec_offset: record stream out of range"; return BTLE_EINVAL; }
+  if (!n) return BTLE_OK;
+  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  size_t pitch = 0;
+  int rc = ingest(ctx, iq, n_streams, stride, n_int8, &pitch);
   if (rc) return rc;
-  return fetch_ordered(ctx, ctx->d_out, ctx->d_dir, btle_b200_rx_units(ctx, n_streams, n_int8), out, cap, n_out, st);
+  if (ctx->d_out.reserve(ctx, n) || ctx->d_hz.reserve(ctx, n)) return BTLE_ENOMEM;
+  BTLE_CUDA(ctx, cudaMemcpyAsync(ctx->d_out, recs, n * sizeof(btle_pkt_rec), cudaMemcpyHostToDevice, st));
+  rc = btle_b200_rec_offset_device(ctx, ctx->d_iq, pitch, n_int8, ctx->d_out, n, ctx->d_hz, st);
+  if (rc) return rc;
+  BTLE_CUDA(ctx, cudaMemcpyAsync(hz, ctx->d_hz, n * sizeof(float), cudaMemcpyDeviceToHost, st));
+  BTLE_CUDA(ctx, cudaStreamSynchronize(st));
+  return BTLE_OK;
 }
 
 int btle_b200_rx_iq16(btle_b200_ctx *ctx, const int16_t *iq16, size_t n_int16, int shift, const btle_stream_cfg *cfg,
@@ -2471,9 +2640,10 @@ size_t btle_b200_rx_multi_units(const btle_b200_ctx *ctx, size_t n_captures, con
   return rc ? 0 : n_cfgs * multi_units_per_group(ctx, groups, n_int8);
 }
 
-int btle_b200_rx_multi_device_dir(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_captures, size_t stride, size_t n_int8,
-                                  const btle_stream_cfg *cfgs, const int32_t *cfg_capture, size_t n_cfgs, btle_pkt_rec *d_out,
-                                  size_t cap, uint32_t *d_count, btle_unit_dir *d_dir, size_t dir_cap, void *cuda_stream) {
+int btle_b200_rx_multi_device_dir_offset(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_captures, size_t stride, size_t n_int8,
+                                         const btle_stream_cfg *cfgs, const int32_t *cfg_capture, size_t n_cfgs, const float *offset_hz,
+                                         btle_pkt_rec *d_out, size_t cap, uint32_t *d_count, btle_unit_dir *d_dir, size_t dir_cap,
+                                         void *cuda_stream) {
   if (!ctx) return BTLE_EINVAL;
   if ((!d_out && cap) || (!cfgs && n_cfgs) || !d_dir) { ctx->err = "rx_multi: missing buffer"; return BTLE_EINVAL; }
   if ((reinterpret_cast<uintptr_t>(d_iq) & 15) || (n_captures > 1 && (stride & 15))) { ctx->err = "device IQ must be 16-byte aligned"; return BTLE_EINVAL; }
@@ -2484,13 +2654,27 @@ int btle_b200_rx_multi_device_dir(btle_b200_ctx *ctx, const int8_t *d_iq, size_t
   if (dir_cap < n_cfgs * multi_units_per_group(ctx, groups, n_int8)) { ctx->err = "unit directory too small (btle_b200_rx_multi_units)"; return BTLE_EINVAL; }
   rc = validate_cfgs(ctx, cfgs, n_cfgs);
   if (rc) return rc;
+  std::vector<int4> rot;
+  if (offset_hz && (rc = make_rots(ctx, offset_hz, n_captures, cfg_capture, n_cfgs, rot))) return rc;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
   return launch_rx(ctx, d_iq, n_captures, stride, n_int8, cfgs, d_out, cap, d_count, d_dir, reinterpret_cast<cudaStream_t>(cuda_stream), 0,
-                   cfg_capture, n_cfgs, groups);
+                   cfg_capture, n_cfgs, groups, offset_hz ? rot.data() : nullptr);
+}
+
+int btle_b200_rx_multi_device_dir(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_captures, size_t stride, size_t n_int8,
+                                  const btle_stream_cfg *cfgs, const int32_t *cfg_capture, size_t n_cfgs, btle_pkt_rec *d_out,
+                                  size_t cap, uint32_t *d_count, btle_unit_dir *d_dir, size_t dir_cap, void *cuda_stream) {
+  return btle_b200_rx_multi_device_dir_offset(ctx, d_iq, n_captures, stride, n_int8, cfgs, cfg_capture, n_cfgs, nullptr, d_out, cap, d_count,
+                                              d_dir, dir_cap, cuda_stream);
 }
 
 int btle_b200_rx_multi(btle_b200_ctx *ctx, const int8_t *iq, size_t n_captures, size_t stride, size_t n_int8, const btle_stream_cfg *cfgs,
                        const int32_t *cfg_capture, size_t n_cfgs, btle_pkt_rec *out, size_t cap, size_t *n_out) {
+  return btle_b200_rx_multi_offset(ctx, iq, n_captures, stride, n_int8, cfgs, cfg_capture, n_cfgs, nullptr, out, cap, n_out);
+}
+
+int btle_b200_rx_multi_offset(btle_b200_ctx *ctx, const int8_t *iq, size_t n_captures, size_t stride, size_t n_int8, const btle_stream_cfg *cfgs,
+                              const int32_t *cfg_capture, size_t n_cfgs, const float *offset_hz, btle_pkt_rec *out, size_t cap, size_t *n_out) {
   if (!ctx) return BTLE_EINVAL;
   if (!n_out || (!out && cap) || (!cfgs && n_cfgs) || (!iq && n_captures && n_int8)) { ctx->err = "rx_multi: missing buffer"; return BTLE_EINVAL; }
   *n_out = 0;
@@ -2500,6 +2684,8 @@ int btle_b200_rx_multi(btle_b200_ctx *ctx, const int8_t *iq, size_t n_captures, 
   if (rc) return rc;
   rc = validate_cfgs(ctx, cfgs, n_cfgs);
   if (rc) return rc;
+  std::vector<int4> rot;
+  if (offset_hz && (rc = make_rots(ctx, offset_hz, n_captures, cfg_capture, n_cfgs, rot))) return rc;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
   // only the captures some cfg reads are copied, one after the other; cfg_capture is renumbered to match
@@ -2521,7 +2707,8 @@ int btle_b200_rx_multi(btle_b200_ctx *ctx, const int8_t *iq, size_t n_captures, 
   }
   const size_t units = n_cfgs * multi_units_per_group(ctx, groups, n_int8);
   if (ctx->d_out.reserve(ctx, std::max<size_t>(cap, 1)) || ctx->d_dir.reserve(ctx, std::max<size_t>(units, 1))) return BTLE_ENOMEM;
-  rc = launch_rx(ctx, ctx->d_iq, groups, pitch, n_int8, cfgs, ctx->d_out, cap, ctx->d_count, ctx->d_dir, st, 0, local.data(), n_cfgs, groups);
+  rc = launch_rx(ctx, ctx->d_iq, groups, pitch, n_int8, cfgs, ctx->d_out, cap, ctx->d_count, ctx->d_dir, st, 0, local.data(), n_cfgs, groups,
+                 offset_hz ? rot.data() : nullptr);
   if (rc) return rc;
   return fetch_ordered(ctx, ctx->d_out, ctx->d_dir, units, out, cap, n_out, st);
 }
@@ -2545,6 +2732,7 @@ struct btle_b200_streams {
   std::vector<size_t> backfill;                            // cfgs added since the last commit / finish (streams_backfill)
   int call_launches = 0;                                   // launches of the current commit / finish call
   std::vector<int32_t> disc;                               // data channel scanned per capture, -1: none (set_discover)
+  std::vector<float> offset;                               // carrier offset per capture (set_offset); empty: never set, default kernel
   std::vector<btle_conn_cand> cands;                       // candidates of the sets handed out, not yet taken
   size_t seg_chunks = 0, seg_bytes = 0, buf_bytes = 0;     // a part = seg_chunks chunks (+ kLook look-ahead bytes behind it)
   size_t stride = 0;                                       // kLead + buf_bytes: bytes from one capture's part to the next
@@ -2564,6 +2752,7 @@ struct btle_b200_streams {
     HostBuf<int8_t> h; Buf<int8_t> d;                      // page-locked host / device IQ buffers, n parts of `stride` bytes
     size_t n_submitted = 0;
     long long first_chunk = 0;
+    std::vector<float> offset;                             // the session's offsets when the set was submitted (backfill reuses them)
     cudaStream_t st = nullptr;
     bool resident = false;                                 // d holds the set at first_chunk (lead, n_submitted bytes)
     std::vector<std::unique_ptr<Job>> jobs;                // jobs[0, n_jobs) wait to be collected (grown, then reused)
@@ -2607,10 +2796,12 @@ int streams_job(Streams *s, int b, const std::vector<size_t> &idx) {
   std::vector<btle_stream_cfg> cfgs(k);
   std::vector<int32_t> cc(k);
   size_t groups = 0;                                         // captures the round reads
+  std::vector<int4> rot;                                     // H.offset non-empty: the rotated kernel, capture cc[i]'s offset
   for (size_t i = 0; i < k; ++i) {
     cfgs[i] = s->entries[idx[i]].cfg;
     cc[i] = (int32_t)s->entries[idx[i]].capture;
     groups += !i || cc[i] != cc[i - 1];
+    if (!H.offset.empty()) rot.push_back(make_rot(H.offset[cc[i]]));
   }
   const bool single = k == s->n && groups == k;
   const size_t units = std::max<size_t>(single ? btle_b200_rx_units(ctx, s->n, H.n_submitted)
@@ -2620,7 +2811,7 @@ int streams_job(Streams *s, int b, const std::vector<size_t> &idx) {
       (!J.d_count && (J.d_count.alloc(ctx, 1) || J.h_count.alloc(ctx, 1))))
     return BTLE_ENOMEM;
   const int rc = launch_rx(ctx, H.d + Streams::kLead, s->n, s->stride, H.n_submitted, cfgs.data(), J.d_out, cap, J.d_count, J.d_dir,
-                           H.st, Streams::kLead, single ? nullptr : cc.data(), k, groups);
+                           H.st, Streams::kLead, single ? nullptr : cc.data(), k, groups, rot.empty() ? nullptr : rot.data());
   if (rc) return rc;
   BTLE_CUDA(ctx, cudaMemcpyAsync(J.h_count, J.d_count, sizeof(unsigned), cudaMemcpyDeviceToHost, H.st));
   BTLE_CUDA(ctx, cudaMemcpyAsync(J.h_dir, J.d_dir, units * sizeof(btle_unit_dir), cudaMemcpyDeviceToHost, H.st));
@@ -2696,6 +2887,7 @@ int streams_submit(Streams *s, int b, size_t n_int8, bool last = false) {
   auto &H = s->half[b];
   H.n_submitted = n_int8;
   H.first_chunk = s->next_chunk;
+  H.offset = s->offset;
   const bool scan = std::any_of(s->disc.begin(), s->disc.end(), [](int32_t c) { return c >= 0; });
   if (n_int8 < (size_t)kChunkInt8 && !(scan && n_int8)) { H.resident = false; return BTLE_OK; }
   constexpr size_t L = btle_b200_streams::kLead;
@@ -2922,6 +3114,17 @@ int btle_b200_streams_set_cfg(btle_b200_streams *s, size_t stream, const btle_st
   return BTLE_OK;
 }
 
+int btle_b200_streams_set_offset(btle_b200_streams *s, size_t capture, float offset_hz) {
+  if (!s) return BTLE_EINVAL;
+  int rc = streams_index(s, capture);
+  if (rc) return rc;
+  std::vector<int4> rot;
+  if ((rc = make_rots(s->ctx, &offset_hz, 1, nullptr, 1, rot))) return rc;
+  if (s->offset.empty()) s->offset.assign(s->n, 0.0f);    // from now on every set takes the rotated kernel
+  s->offset[capture] = offset_hz;                           // used from the next submitted segment set on
+  return BTLE_OK;
+}
+
 int btle_b200_streams_acquire(btle_b200_streams *s, size_t stream, int8_t **buf, size_t *space) {
   if (!s || !buf || !space) return BTLE_EINVAL;
   const int rc = streams_index(s, stream);
@@ -3067,6 +3270,10 @@ void btle_b200_stream_close(btle_b200_stream *s) {
 
 int btle_b200_stream_set_cfg(btle_b200_stream *s, const btle_stream_cfg *cfg) {
   return s ? btle_b200_streams_set_cfg(s->m, 0, cfg) : BTLE_EINVAL;
+}
+
+int btle_b200_stream_set_offset(btle_b200_stream *s, float offset_hz) {
+  return s ? btle_b200_streams_set_offset(s->m, 0, offset_hz) : BTLE_EINVAL;
 }
 
 int btle_b200_stream_acquire(btle_b200_stream *s, int8_t **buf, size_t *space) {

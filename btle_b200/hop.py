@@ -265,7 +265,7 @@ def follow_connections(rx, captures: np.ndarray, max_events: int = 10000, discov
     return adv, conns
 
 
-def decode_connections(rx, captures: np.ndarray, discover: bool = True):
+def decode_connections(rx, captures: np.ndarray, discover: bool = True, offset_hz=None):
     """Every known connection's data-channel traffic, decoded without following it.  captures: int8 [40, n_int8] as in
     follow_connections(); `rx` needs rx_batch, rx_multi and, with discover=True, discover (a BtleRx).
     The connections are the CONNECT_REQ ones (tracked or not) plus, with discover=True, the discover_connections() ones
@@ -274,11 +274,17 @@ def decode_connections(rx, captures: np.ndarray, discover: bool = True):
     each connection gets `traffic`: every record on channels 0..36 decoded with them, in time order (chunk * 8192 + n0,
     then channel).  Launches: one rx_batch over the advertising captures, one discover, and one rx_multi per
     MAX_CFGS_PER_CAPTURE connections over captures[0:37] (each capture is read once per call, whatever the number of
-    connections in it).  Returns (adv_records, connections)."""
+    connections in it).  offset_hz (a scalar or one per capture, None: no correction) is passed to those rx_batch and
+    rx_multi calls (carrier-offset correction); discovery reads the captures uncorrected.  Returns (adv_records,
+    connections)."""
     from ._native import MAX_CFGS_PER_CAPTURE
     captures = np.ascontiguousarray(captures, dtype=np.int8)
     assert captures.shape[0] == 40
-    adv = rx.rx_batch(captures[37:40], make_cfgs(3, channel=[37, 38, 39])).copy()
+    # offsets are only passed when given: `rx` may be any object with BtleRx's rx_batch / rx_multi
+    off = None if offset_hz is None else np.broadcast_to(np.asarray(offset_hz, dtype=np.float32), (40,))
+    adv_kw = {} if off is None else {"offset_hz": off[37:40]}
+    data_kw = {} if off is None else {"offset_hz": off[0:37]}
+    adv = rx.rx_batch(captures[37:40], make_cfgs(3, channel=[37, 38, 39]), **adv_kw).copy()
     adv["stream"] += 37
     conns = []
     for r in adv:
@@ -297,7 +303,7 @@ def decode_connections(rx, captures: np.ndarray, discover: bool = True):
         # cfg j = channel * k + i: connection i on data channel j // k (the cfgs of one capture are adjacent)
         cfgs = make_cfgs(37 * k, channel=np.repeat(np.arange(37), k), access_addr=[c["access_addr"] for c in batch] * 37,
                          crc_init=[c["crc_init"] for c in batch] * 37)
-        rec = rx.rx_multi(captures[0:37], cfgs, np.repeat(np.arange(37, dtype=np.int32), k))
+        rec = rx.rx_multi(captures[0:37], cfgs, np.repeat(np.arange(37, dtype=np.int32), k), **data_kw)
         owner = rec["stream"] % k
         t = rec["chunk"].astype(np.int64) * 8192 + rec["n0"]
         for i, c in enumerate(batch):
@@ -445,12 +451,17 @@ class ConnectionMonitor:
     (`until_chunk`); None keeps every connection to the end, as decode_connections() does.  group_s: a candidate group
     that has not reached min_events and has had no event for that long is forgotten, so that noise groups do not pile up
     over a long session (the default, 8 s, is twice the longest connection interval; a group paused longer than that
-    starts again, where discover_connections() would continue it)."""
+    starts again, where discover_connections() would continue it).  offset_hz (a scalar or one per capture): the
+    session's carrier-offset correction of each capture (RxStreams.set_offset), from the first set on."""
 
     N_CAPTURES = 40
 
-    def __init__(self, session, min_events: int = 4, idle_s: float | None = None, discover: bool = True, group_s: float = 8.0):
+    def __init__(self, session, min_events: int = 4, idle_s: float | None = None, discover: bool = True, group_s: float = 8.0,
+                 offset_hz=None):
         self.session, self.min_events, self.idle_s, self.group_s = session, int(min_events), idle_s, group_s
+        if offset_hz is not None:
+            for c, hz in enumerate(np.broadcast_to(np.asarray(offset_hz, dtype=np.float32), (self.N_CAPTURES,))):
+                session.set_offset(c, float(hz))
         for c in range(37):
             session.remove_cfg(c)
         if discover:

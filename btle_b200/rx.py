@@ -41,6 +41,13 @@ def _with_fields(c: np.ndarray, cfg: dict) -> np.ndarray:
     return c
 
 
+def _offsets(offset_hz, n: int):
+    """float32 [n] of a scalar or per-capture offset, or None (no correction: the default kernels)"""
+    if offset_hz is None:
+        return None
+    return np.ascontiguousarray(np.broadcast_to(np.asarray(offset_hz, dtype=np.float32), (n,)))
+
+
 class BtleRx:
     def __init__(self, device: int = 0):
         self._L = _native.load()
@@ -91,24 +98,29 @@ class BtleRx:
                 return np.concatenate(out)
 
     # ---- host buffers -------------------------------------------------------------------
-    def rx_batch(self, iq: np.ndarray, cfgs: np.ndarray, cap: int | None = None) -> np.ndarray:
-        """iq: int8 [n_streams, n_int8] (C-contiguous) or [n_int8]; cfgs: CFG_DTYPE [n_streams]."""
+    def rx_batch(self, iq: np.ndarray, cfgs: np.ndarray, cap: int | None = None, offset_hz=None) -> np.ndarray:
+        """iq: int8 [n_streams, n_int8] (C-contiguous) or [n_int8]; cfgs: CFG_DTYPE [n_streams].  offset_hz (a scalar or one
+        per capture, Hz, received minus nominal carrier): carrier-offset correction (btle_b200_rx_batch_offset)."""
         iq = np.ascontiguousarray(iq, dtype=np.int8)
         if iq.ndim == 1:
             iq = iq[None, :]
         ns, n = iq.shape
         cfgs = np.ascontiguousarray(cfgs, dtype=CFG_DTYPE)
         assert cfgs.shape == (ns,)
+        off = _offsets(offset_hz, ns)
         # default capacity: typical worst case; grown once on BTLE_EOVERFLOW to the exact count, which is at most
         # BTLE_MAX_PKTS_PER_CHUNK (51) records per chunk, or BTLE_MAX_RECS_PER_CHUNK (123) with BTLE_CFG_REPORT_REJECTED
-        return self._grow_once(partial(self._L.btle_b200_rx_batch, self._h, iq.ctypes.data, ns, n, n, cfgs.ctypes.data), REC_DTYPE,
-                               ns * (n // 16384) * 34 + 16 if cap is None else cap, grow=cap is None)
+        if off is None:
+            call = partial(self._L.btle_b200_rx_batch, self._h, iq.ctypes.data, ns, n, n, cfgs.ctypes.data)
+        else:
+            call = partial(self._L.btle_b200_rx_batch_offset, self._h, iq.ctypes.data, ns, n, n, cfgs.ctypes.data, off.ctypes.data)
+        return self._grow_once(call, REC_DTYPE, ns * (n // 16384) * 34 + 16 if cap is None else cap, grow=cap is None)
 
-    def rx_multi(self, iq: np.ndarray, cfgs: np.ndarray, capture, cap: int | None = None) -> np.ndarray:
+    def rx_multi(self, iq: np.ndarray, cfgs: np.ndarray, capture, cap: int | None = None, offset_hz=None) -> np.ndarray:
         """Several cfgs per capture in one read of the IQ (btle_b200_rx_multi): iq int8 [n_captures, n_int8] (or [n_int8]);
         cfgs CFG_DTYPE [n_cfgs]; capture[j] = the capture cfg j decodes (non-decreasing, at most MAX_CFGS_PER_CAPTURE
         per capture).  Returns what rx_batch() returns on iq[capture] with cfgs: records with stream = cfg index, in
-        (cfg, chunk, n0) order."""
+        (cfg, chunk, n0) order.  offset_hz: a scalar or one per capture (carrier-offset correction)."""
         iq = np.ascontiguousarray(iq, dtype=np.int8)
         if iq.ndim == 1:
             iq = iq[None, :]
@@ -116,30 +128,77 @@ class BtleRx:
         cfgs = np.ascontiguousarray(cfgs, dtype=CFG_DTYPE).reshape(-1)
         cc = np.ascontiguousarray(capture, dtype=np.int32).reshape(-1)
         assert cc.shape == cfgs.shape
-        return self._grow_once(partial(self._L.btle_b200_rx_multi, self._h, iq.ctypes.data, ns, n, n, cfgs.ctypes.data, cc.ctypes.data,
-                                       cfgs.size), REC_DTYPE, cfgs.size * (n // 16384) * 34 + 16 if cap is None else cap, grow=cap is None)
+        off = _offsets(offset_hz, ns)
+        if off is None:
+            call = partial(self._L.btle_b200_rx_multi, self._h, iq.ctypes.data, ns, n, n, cfgs.ctypes.data, cc.ctypes.data, cfgs.size)
+        else:
+            call = partial(self._L.btle_b200_rx_multi_offset, self._h, iq.ctypes.data, ns, n, n, cfgs.ctypes.data, cc.ctypes.data, cfgs.size,
+                           off.ctypes.data)
+        return self._grow_once(call, REC_DTYPE, cfgs.size * (n // 16384) * 34 + 16 if cap is None else cap, grow=cap is None)
 
     def multi_units(self, n_captures: int, capture, n_int8: int) -> int:
         """Number of unit-directory entries an rx_multi launch over this shape writes (btle_b200_rx_multi_units)."""
         cc = np.ascontiguousarray(capture, dtype=np.int32).reshape(-1)
         return int(self._L.btle_b200_rx_multi_units(self._h, n_captures, cc.ctypes.data, cc.size, n_int8))
 
-    def rx_multi_device_dir(self, d_iq, cfgs: np.ndarray, capture, d_out, d_count, d_dir, stream_ptr: int = 0):
+    def rx_multi_device_dir(self, d_iq, cfgs: np.ndarray, capture, d_out, d_count, d_dir, stream_ptr: int = 0, offset_hz=None):
         """rx_multi on device-resident captures, buffers as rx_device_dir (d_count may be None); d_dir holds at least
-        multi_units(...) * 8 bytes.  gather_ordered() of the launch gives rx_multi()'s result."""
+        multi_units(...) * 8 bytes.  gather_ordered() of the launch gives rx_multi()'s result.  offset_hz as rx_multi."""
         ns, n = d_iq.shape
         cfgs = np.ascontiguousarray(cfgs, dtype=CFG_DTYPE).reshape(-1)
         cc = np.ascontiguousarray(capture, dtype=np.int32).reshape(-1)
         assert d_iq.stride(1) == 1 and cc.shape == cfgs.shape
         cap = d_out.numel() * d_out.element_size() // 64
         dir_cap = d_dir.numel() * d_dir.element_size() // 8
-        rc = self._L.btle_b200_rx_multi_device_dir(self._h, d_iq.data_ptr(), ns, d_iq.stride(0), n, cfgs.ctypes.data, cc.ctypes.data,
-                                                   cfgs.size, d_out.data_ptr(), cap, d_count.data_ptr() if d_count is not None else None,
-                                                   d_dir.data_ptr(), dir_cap, ctypes.c_void_p(stream_ptr))
+        off = _offsets(offset_hz, ns)
+        head = (self._h, d_iq.data_ptr(), ns, d_iq.stride(0), n, cfgs.ctypes.data, cc.ctypes.data, cfgs.size)
+        tail = (d_out.data_ptr(), cap, d_count.data_ptr() if d_count is not None else None, d_dir.data_ptr(), dir_cap, ctypes.c_void_p(stream_ptr))
+        if off is None:
+            rc = self._L.btle_b200_rx_multi_device_dir(*head, *tail)
+        else:
+            rc = self._L.btle_b200_rx_multi_device_dir_offset(*head, off.ctypes.data, *tail)
         self._check(rc)
 
-    def rx(self, iq: np.ndarray, **cfg) -> np.ndarray:
-        return self.rx_batch(np.asarray(iq).reshape(1, -1), make_cfgs(1, **cfg))
+    def rx(self, iq: np.ndarray, offset_hz=None, **cfg) -> np.ndarray:
+        return self.rx_batch(np.asarray(iq).reshape(1, -1), make_cfgs(1, **cfg), offset_hz=offset_hz)
+
+    # ---- carrier offset -------------------------------------------------------------------
+    def rec_offsets(self, iq: np.ndarray, recs: np.ndarray) -> np.ndarray:
+        """float32 [len(recs)]: the carrier-offset estimate of each record in Hz (btle_b200_rec_offset; definition in
+        include/btle_b200.h).  iq as rx_batch's; a record's `stream` is its capture."""
+        iq = np.ascontiguousarray(iq, dtype=np.int8)
+        if iq.ndim == 1:
+            iq = iq[None, :]
+        ns, n = iq.shape
+        recs = np.ascontiguousarray(recs, dtype=REC_DTYPE)
+        hz = np.zeros(recs.size, dtype=np.float32)
+        self._check(self._L.btle_b200_rec_offset(self._h, iq.ctypes.data, ns, n, n, recs.ctypes.data, recs.size, hz.ctypes.data))
+        return hz
+
+    def estimate_offset(self, iq: np.ndarray, **cfg):
+        """Carrier offset of one capture in Hz: decoded without correction, the median of the per-record estimates
+        (btle_b200_rec_offset_device) over the counted records with a good CRC; None when there is none.  The capture is
+        copied to the device once and both passes read that copy.  Pass the result back as rx(..., offset_hz=)."""
+        import torch
+        iq = np.ascontiguousarray(np.asarray(iq, dtype=np.int8).reshape(1, -1))
+        n = iq.shape[1]
+        dev = torch.device("cuda", self.device)
+        st = torch.cuda.current_stream(dev)
+        d_iq = torch.from_numpy(np.pad(iq, ((0, 0), (0, -n % 16)))).to(dev)[:, :n]
+        cap = (n // 16384) * 123 + 16                                   # BTLE_MAX_RECS_PER_CHUNK per chunk: never an overflow
+        d_out = torch.empty(cap * 64, dtype=torch.uint8, device=dev)
+        d_dir = torch.empty(max(self.units(1, n), 1) * 8, dtype=torch.uint8, device=dev)
+        self.rx_device_dir(d_iq, make_cfgs(1, **cfg), d_out, None, d_dir, st.cuda_stream)
+        st.synchronize()
+        recs = self.gather_ordered(d_out.cpu().numpy().view(REC_DTYPE), d_dir.cpu().numpy().view(DIR_DTYPE))
+        ok = np.ascontiguousarray(recs[(recs["crc_bad"] == 0) & ((recs["flags"] & (1 | _native.REC_REJECTED)) == 0)])
+        if ok.size == 0:
+            return None
+        d_ok = torch.from_numpy(ok.view(np.uint8).copy()).to(dev)
+        d_hz = torch.empty(ok.size, dtype=torch.float32, device=dev)
+        self.rec_offsets_device(d_iq, d_ok, ok.size, d_hz, st.cuda_stream)
+        st.synchronize()
+        return float(np.median(d_hz.cpu().numpy()))
 
     def rx_iq16(self, iq16: np.ndarray, shift: int = 4, **cfg) -> np.ndarray:
         """int16 interleaved IQ (bladeRF SC16Q11: shift 4, btle_rx.c:307-308) -> records."""
@@ -217,21 +276,33 @@ class BtleRx:
         """Number of unit-directory entries a launch over this shape writes (btle_b200_rx_units)."""
         return int(self._L.btle_b200_rx_units(self._h, n_streams, n_int8))
 
-    def rx_device_dir(self, d_iq, cfgs: np.ndarray, d_out, d_count, d_dir, stream_ptr: int = 0):
+    def rx_device_dir(self, d_iq, cfgs: np.ndarray, d_out, d_count, d_dir, stream_ptr: int = 0, offset_hz=None):
         """Like rx_device, with the unit directory in the caller's buffer: d_dir is a torch CUDA tensor of at least
         units(...) * 8 bytes.  d_out / d_dir may be views of PEER memory (another GPU's buffer mapped here): the kernel
         then stores records and directory straight over NVLink.  Walking the directory (gather_ordered) yields the
         records in the reference's order.  d_count may be None (the packet count is the sum of the directory's counts):
-        no memset is then enqueued in front of the kernel."""
+        no memset is then enqueued in front of the kernel.  offset_hz as rx_batch's (btle_b200_rx_device_dir_offset)."""
         ns, n = d_iq.shape
         cfgs = np.ascontiguousarray(cfgs, dtype=CFG_DTYPE)
         assert d_iq.stride(1) == 1 and cfgs.shape == (ns,)
         cap = d_out.numel() * d_out.element_size() // 64
         dir_cap = d_dir.numel() * d_dir.element_size() // 8
-        rc = self._L.btle_b200_rx_device_dir(self._h, d_iq.data_ptr(), ns, d_iq.stride(0), n, cfgs.ctypes.data, d_out.data_ptr(),
-                                             cap, d_count.data_ptr() if d_count is not None else None, d_dir.data_ptr(), dir_cap,
-                                             ctypes.c_void_p(stream_ptr))
+        off = _offsets(offset_hz, ns)
+        head = (self._h, d_iq.data_ptr(), ns, d_iq.stride(0), n, cfgs.ctypes.data)
+        tail = (d_out.data_ptr(), cap, d_count.data_ptr() if d_count is not None else None, d_dir.data_ptr(), dir_cap, ctypes.c_void_p(stream_ptr))
+        if off is None:
+            rc = self._L.btle_b200_rx_device_dir(*head, *tail)
+        else:
+            rc = self._L.btle_b200_rx_device_dir_offset(*head, off.ctypes.data, *tail)
         self._check(rc)
+
+    def rec_offsets_device(self, d_iq, d_recs, n: int, d_hz, stream_ptr: int = 0):
+        """rec_offsets on the device: d_iq as rx_device_dir's, d_recs n records (uint8 CUDA tensor of n * 64 bytes),
+        d_hz float32 CUDA tensor [n]; enqueued on `stream_ptr` (no sync)."""
+        ns, nb = d_iq.shape
+        assert d_iq.stride(1) == 1 and d_hz.numel() >= n
+        self._check(self._L.btle_b200_rec_offset_device(self._h, d_iq.data_ptr(), d_iq.stride(0), nb, d_recs.data_ptr(), n, d_hz.data_ptr(),
+                                                        ctypes.c_void_p(stream_ptr)))
 
     def gather_ordered(self, recs: np.ndarray, unit_dir: np.ndarray) -> np.ndarray:
         """Host copies of a launch's record buffer and unit directory -> records in reference order."""
@@ -317,6 +388,10 @@ class RxStream:
     def finish(self) -> np.ndarray:
         return self._rx._drain(self._L.btle_b200_stream_finish, self._h, self._buf)
 
+    def set_offset(self, offset_hz: float) -> None:
+        """Carrier-offset correction of the capture from the next submitted segment on (btle_b200_stream_set_offset)."""
+        self._rx._check(self._L.btle_b200_stream_set_offset(self._h, float(offset_hz)))
+
     def close(self):
         if getattr(self, "_h", None):
             self._L.btle_b200_stream_close(self._h)
@@ -393,6 +468,11 @@ class RxStreams:
         c = _with_fields(self._cfgs[int(stream):int(stream) + 1].copy() if 0 <= int(stream) < self.n_streams else make_cfgs(1), cfg)
         self._rx._check(self._L.btle_b200_streams_set_cfg(self._h, int(stream), c.ctypes.data))
         self._cfgs[int(stream)] = c[0]
+
+    def set_offset(self, stream: int, offset_hz: float) -> None:
+        """Carrier-offset correction of capture `stream` (Hz, received minus nominal carrier), from the next segment set
+        that is submitted on; from the first call on, every set takes the rotated kernel (btle_b200_streams_set_offset)."""
+        self._rx._check(self._L.btle_b200_streams_set_offset(self._h, int(stream), float(offset_hz)))
 
     # ---- per-capture cfg lists and discovery (btle_b200_streams_add_cfg / remove_cfg / set_discover) -------------------
     @property

@@ -93,6 +93,19 @@ typedef struct {
  * Rejected (BTLE_CFG_REPORT_REJECTED) records, raw-mode records and CRC-ok records are never touched; the flag does
  * nothing in raw mode. */
 #define BTLE_CFG_RECOVER 4
+/* Carrier-offset correction: the *_offset entry points take one float offset_hz per capture, the received carrier minus
+ * the nominal one in Hz (the sign of btle_rx_ber_cfg.cfo_hz: correcting by cfo_hz undoes that impairment).  Not part of the
+ * reference's receiver.  With phi = 2 pi offset_hz / 4 MHz and C = round(2^14 cos phi), S = round(2^14 sin phi) (nearest,
+ * ties to even; computed in double on the host), every discriminator bit becomes
+ *     d[n] = C (I[n] Q[n+1] - I[n+1] Q[n]) - S (I[n] I[n+1] + Q[n] Q[n+1]) > 0      (int32, |each product sum| <= 2^15)
+ * i.e. the sign of Im(conj(x[n]) x[n+1] e^(-j phi)).  The samples are not changed.  Everything the chain derives from these
+ * bits — the access-address search, the greedy chain, the length guards, the bytes, the CRC, -v rejected hits — follows
+ * unchanged.  For offset 0, (C, S) = (16384, 0) and every record equals the reference's, bit for bit; a non-NULL offset_hz
+ * always takes the rotated kernel, also when every value is 0.  BTLE_CFG_RECOVER's symbol-spaced bits use the rotation
+ * over 4 samples: (C4, S4) from 4 phi in the same formula, e[s] = C4 (I[s] Q[s+4] - I[s+4] Q[s]) - S4 (I[s] I[s+4] +
+ * Q[s] Q[s+4]) > 0.  mag_sum (RSSI) reads the raw samples and is unaffected.  In rx_multi the cfgs of one capture share
+ * its offset.  Values that are not finite, or with |offset_hz| > BTLE_MAX_OFFSET_HZ, are BTLE_EINVAL. */
+#define BTLE_MAX_OFFSET_HZ 500000
 
 /* One packet the reference would have counted (pkt_count++, btle_rx.c:2274/:2319). 64 bytes. */
 typedef struct {
@@ -145,6 +158,9 @@ uint32_t btle_b200_version(void);
 int btle_b200_rx_batch(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stream_stride_int8,
                        size_t n_int8, const btle_stream_cfg *cfgs, btle_pkt_rec *out, size_t cap,
                        size_t *n_out);
+/* The same with carrier-offset correction (BTLE_MAX_OFFSET_HZ above): offset_hz[s] for capture s; NULL: as btle_b200_rx_batch. */
+int btle_b200_rx_batch_offset(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stream_stride_int8, size_t n_int8,
+                              const btle_stream_cfg *cfgs, const float *offset_hz, btle_pkt_rec *out, size_t cap, size_t *n_out);
 /* Single capture convenience wrapper. */
 int btle_b200_rx(btle_b200_ctx *ctx, const int8_t *iq, size_t n_int8, const btle_stream_cfg *cfg,
                  btle_pkt_rec *out, size_t cap, size_t *n_out);
@@ -178,6 +194,9 @@ size_t btle_b200_rx_units(const btle_b200_ctx *ctx, size_t n_streams, size_t n_i
 int btle_b200_rx_device_dir(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stream_stride_int8,
                             size_t n_int8, const btle_stream_cfg *cfgs, btle_pkt_rec *d_out, size_t cap,
                             uint32_t *d_count, btle_unit_dir *d_dir, size_t dir_cap, void *cuda_stream);
+int btle_b200_rx_device_dir_offset(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stream_stride_int8,
+                                   size_t n_int8, const btle_stream_cfg *cfgs, const float *offset_hz, btle_pkt_rec *d_out, size_t cap,
+                                   uint32_t *d_count, btle_unit_dir *d_dir, size_t dir_cap, void *cuda_stream);
 /* Same with the directory kept in context-owned scratch: for callers that only want the set of records
  * (btle_b200_sort_records() on the host copy gives reference order). */
 int btle_b200_rx_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stream_stride_int8,
@@ -198,6 +217,10 @@ void btle_b200_sort_records(btle_pkt_rec *recs, size_t n);
 int btle_b200_rx_multi(btle_b200_ctx *ctx, const int8_t *iq, size_t n_captures, size_t stream_stride_int8, size_t n_int8,
                        const btle_stream_cfg *cfgs, const int32_t *cfg_capture, size_t n_cfgs, btle_pkt_rec *out, size_t cap,
                        size_t *n_out);
+/* with carrier-offset correction: offset_hz[c] for capture c (host array of n_captures), shared by capture c's cfgs */
+int btle_b200_rx_multi_offset(btle_b200_ctx *ctx, const int8_t *iq, size_t n_captures, size_t stream_stride_int8, size_t n_int8,
+                              const btle_stream_cfg *cfgs, const int32_t *cfg_capture, size_t n_cfgs, const float *offset_hz,
+                              btle_pkt_rec *out, size_t cap, size_t *n_out);
 /* directory entries of an rx_multi launch of this shape (0 for an invalid cfg_capture) */
 size_t btle_b200_rx_multi_units(const btle_b200_ctx *ctx, size_t n_captures, const int32_t *cfg_capture, size_t n_cfgs, size_t n_int8);
 /* device-resident form; directory, d_count (may be NULL: counter ring) and streams exactly as btle_b200_rx_device_dir():
@@ -206,6 +229,23 @@ int btle_b200_rx_multi_device_dir(btle_b200_ctx *ctx, const int8_t *d_iq, size_t
                                   size_t n_int8, const btle_stream_cfg *cfgs, const int32_t *cfg_capture, size_t n_cfgs,
                                   btle_pkt_rec *d_out, size_t cap, uint32_t *d_count, btle_unit_dir *d_dir, size_t dir_cap,
                                   void *cuda_stream);
+int btle_b200_rx_multi_device_dir_offset(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_captures, size_t stream_stride_int8,
+                                         size_t n_int8, const btle_stream_cfg *cfgs, const int32_t *cfg_capture, size_t n_cfgs,
+                                         const float *offset_hz, btle_pkt_rec *d_out, size_t cap, uint32_t *d_count, btle_unit_dir *d_dir,
+                                         size_t dir_cap, void *cuda_stream);
+/* Per-packet carrier-offset estimate, one float per record (the record itself is not changed).  Record r's capture is
+ * `stream` (records of btle_b200_rx_batch / rx_device_dir over the same captures); its samples are read with recovery's
+ * window rule (outside [8192 chunk, 8192 chunk + 9696) or outside the capture: 0).  With z[n] = conj(x[n]) x[n+1]:
+ *     hz[r] = 4e6 / (2 pi 156) * sum_{n = n0-32 .. n0+123} (atan2(Im z[n], Re z[n]) - ref[n - n0])
+ * ref = the same turns of the noiseless btle_tx waveform (the 4-sps modulator of btle_b200_tx_modulate_device, int8 table
+ * samples) of the packet's preamble and access address, tx sample BTLE_RX_BER_AA_OFFSET at n0: the preamble and access
+ * address, up to 4 samples before the header, whose first bit the Gaussian filter lets into later turns.  So a noiseless
+ * packet of the project's own transmitter, aligned, estimates 0.  Device form: d_iq (captures stride apart), d_recs and
+ * d_hz device pointers, enqueued on cuda_stream, one warp per record; host form: host buffers, synchronised. */
+int btle_b200_rec_offset_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t stream_stride_int8, size_t n_int8, const btle_pkt_rec *d_recs,
+                                size_t n, float *d_hz, void *cuda_stream);
+int btle_b200_rec_offset(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stream_stride_int8, size_t n_int8,
+                         const btle_pkt_rec *recs, size_t n, float *hz);
 /* Host helper: recs[0..n_recs) and dir[0..n_units) are host copies of a launch's d_out / d_dir; copies the
  * records into out[] in reference order.  *n_out = sum of the directory counts; BTLE_EOVERFLOW if that exceeds
  * `cap` or if blocks were cut off by n_recs (out then holds what was available, still in order). */
@@ -227,6 +267,8 @@ int btle_b200_stream_commit(btle_b200_stream *s, size_t n_int8, btle_pkt_rec *ou
 int btle_b200_stream_push(btle_b200_stream *s, const int8_t *iq, size_t n_int8, btle_pkt_rec *out, size_t cap, size_t *n_out);
 /* retune: channel / access address / CRC init used from the next segment on (hop following on a live stream) */
 int btle_b200_stream_set_cfg(btle_b200_stream *s, const btle_stream_cfg *cfg);
+/* carrier-offset correction (BTLE_MAX_OFFSET_HZ) of the capture, from the next submitted segment on: btle_b200_streams_set_offset */
+int btle_b200_stream_set_offset(btle_b200_stream *s, float offset_hz);
 /* end of stream: decodes the tail, returns what is left (BTLE_EOVERFLOW: call again, more records are waiting) */
 int btle_b200_stream_finish(btle_b200_stream *s, btle_pkt_rec *out, size_t cap, size_t *n_out);
 void btle_b200_stream_close(btle_b200_stream *s);
@@ -251,6 +293,12 @@ int btle_b200_streams_open(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size
 int btle_b200_streams_acquire(btle_b200_streams *s, size_t stream, int8_t **buf, size_t *space);
 int btle_b200_streams_commit(btle_b200_streams *s, size_t stream, size_t n_int8, btle_pkt_rec *out, size_t cap, size_t *n_out);
 int btle_b200_streams_set_cfg(btle_b200_streams *s, size_t stream, const btle_stream_cfg *cfg);
+/* Carrier-offset correction (BTLE_MAX_OFFSET_HZ) of capture `capture`, shared by all its cfgs, used from the next submitted
+ * segment set on, like set_cfg.  From the first call on, every set of the session is decoded by the rotated kernel (the
+ * other captures at offset 0, which returns the default kernel's records), and a set keeps the offsets it was submitted
+ * with, also for a backfill of cfgs added later.  So a record of chunk k equals that of btle_b200_rx_batch_offset on the
+ * whole captures at the offsets in force when the set holding chunk k was submitted. */
+int btle_b200_streams_set_offset(btle_b200_streams *s, size_t capture, float offset_hz);
 int btle_b200_streams_finish(btle_b200_streams *s, btle_pkt_rec *out, size_t cap, size_t *n_out);
 void btle_b200_streams_close(btle_b200_streams *s);
 
