@@ -2088,7 +2088,6 @@ Plan plan_for(const btle_b200_ctx *ctx, size_t n_streams, size_t n_int8) {
 // kMaxCfgsPerCapture per capture; else BTLE_EINVAL).  *groups = number of distinct captures named.
 int check_cfg_capture(btle_b200_ctx *ctx, size_t n_captures, const int32_t *cfg_capture, size_t n_cfgs, size_t *groups) {
   *groups = 0;
-  if (n_cfgs && !cfg_capture) { ctx->err = "rx_multi: missing cfg_capture"; return BTLE_EINVAL; }
   size_t run = 0;
   for (size_t i = 0; i < n_cfgs; ++i) {
     const int32_t c = cfg_capture[i];
@@ -2100,15 +2099,14 @@ int check_cfg_capture(btle_b200_ctx *ctx, size_t n_captures, const int32_t *cfg_
   }
   return BTLE_OK;
 }
-// units of one capture group of an rx_multi launch over `groups` captures; every group has the same number
-size_t multi_units_per_group(const btle_b200_ctx *ctx, size_t groups, size_t n_int8) {
+// Directory entries of a launch of n_cfgs cfgs over the `groups` captures they name: the plan's units over those
+// captures, or with several cfgs on a capture every capture's (equal) share of them once per cfg
+size_t rx_units(const btle_b200_ctx *ctx, size_t groups, size_t n_cfgs, size_t n_int8) {
   if (!groups || n_int8 < (size_t)kChunkInt8) return 0;
-  return (size_t)plan_for(ctx, groups, n_int8).total_units / groups;
+  const size_t total = (size_t)plan_for(ctx, groups, n_int8).total_units;
+  return n_cfgs == groups ? total : n_cfgs * (total / groups);
 }
 
-// enqueue the persistent kernel for device-resident inputs; `lead`: bytes readable in front of each capture (the
-// stream session's lead: RSSI of hits at a segment's very start); cfg_capture != nullptr: several cfgs per capture
-// (n_cfgs of them, checked by check_cfg_capture), the directory in (cfg, chunk) order
 // {C, S, C4, S4} of a carrier offset (include/btle_b200.h): round(2^14 (cos, sin)) of phi and of 4 phi, phi = 2 pi hz / 4 MHz
 int4 make_rot(float hz) {
   const double ph = 6.283185307179586476925286766559 * (double)hz / 4e6;
@@ -2127,29 +2125,48 @@ int make_rots(btle_b200_ctx *ctx, const float *offset_hz, size_t n_captures, con
   return BTLE_OK;
 }
 
-// rot != nullptr: one rotation per cfg (make_rot), the rotated kernel variant
-int launch_rx(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8,
-              const btle_stream_cfg *cfgs, btle_pkt_rec *d_out, size_t cap, unsigned *d_count, btle_unit_dir *d_dir,
-              cudaStream_t st, long long lead, const int32_t *cfg_capture = nullptr, size_t n_cfgs = 0, size_t groups = 0,
-              const int4 *rot = nullptr) {
+template <int KC, bool ROT>
+void enqueue_rx(unsigned grid, cudaStream_t st, const MapSlot *ms, const int8_t *d_iq, size_t stride, size_t n_int8, const CfgSlot *cs,
+                const Plan &plan, btle_pkt_rec *d_out, unsigned cap32, unsigned *d_count, btle_unit_dir *d_dir, unsigned *zero_next,
+                long long lead) {
+  btle_rx_persistent_kernel<KC, ROT><<<grid, kThreads, sizeof(Smem<KC>), st>>>(
+      ms->map32, ms->map12, d_iq, (long long)stride, (long long)n_int8, cs->d_params, plan, d_out, cap32, d_count,
+      reinterpret_cast<uint2 *>(d_dir), zero_next, lead, KC > 1 ? cs->d_vmap.p : nullptr, ROT ? cs->d_rot.p : nullptr);
+}
+
+// Enqueue the persistent kernel for device-resident inputs: n_cfgs cfgs on n_streams captures, cfg i decoding capture
+// cfg_capture[i] (checked by check_cfg_capture), or capture i when cfg_capture is nullptr (then n_cfgs == n_streams).
+// A list that maps cfg i to capture i for every capture runs btle_rx_persistent_kernel<1>, the directory in unit order;
+// any other list runs <kMaxCfgsPerCapture> over the captures it names, the directory in (cfg, chunk) order.
+// rot != nullptr: one rotation per cfg (make_rot), the rotated kernel variant.  `lead`: bytes readable in front of each
+// capture (the stream session's lead: RSSI of hits at a segment's very start).
+int launch_rx(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8, const btle_stream_cfg *cfgs,
+              const int32_t *cfg_capture, size_t n_cfgs, const int4 *rot, btle_pkt_rec *d_out, size_t cap, unsigned *d_count,
+              btle_unit_dir *d_dir, cudaStream_t st, long long lead) {
   ctx->last_launches = 0;
   unsigned *zero_next = nullptr;
   if (d_count) BTLE_CUDA(ctx, cudaMemsetAsync(d_count, 0, sizeof(unsigned), st));
   const long long nchunks = (long long)(n_int8 / kChunkInt8);
+  if (nchunks == 0 || n_streams == 0 || n_cfgs == 0) return BTLE_OK;
+  size_t groups = n_streams;                                  // captures the launch reads
+  if (cfg_capture) {
+    groups = 0;
+    for (size_t i = 0; i < n_cfgs; ++i) groups += !i || cfg_capture[i] != cfg_capture[i - 1];
+    if (groups == n_cfgs && n_cfgs == n_streams) cfg_capture = nullptr;   // cfg i on capture i
+  }
   const bool multi = cfg_capture != nullptr;
-  if (nchunks == 0 || n_streams == 0 || (multi && n_cfgs == 0)) return BTLE_OK;
   unsigned long long sid = 0;
   int rc = stream_id(ctx, st, &sid);
   if (rc) return rc;
   const long long spans = (nchunks + kSpanChunks - 1) / kSpanChunks;
-  if (spans * (long long)(multi ? n_cfgs : n_streams) > 0x07FFFFFFll || nchunks > 0x7FFFFFFFll) { ctx->err = "batch too large for one launch"; return BTLE_EINVAL; }
-  const Plan plan = plan_for(ctx, multi ? groups : n_streams, n_int8);
+  if (spans * (long long)n_cfgs > 0x07FFFFFFll || nchunks > 0x7FFFFFFFll) { ctx->err = "batch too large for one launch"; return BTLE_EINVAL; }
+  const Plan plan = plan_for(ctx, groups, n_int8);
   if (multi && (plan.tail_units || (plan.big_units && plan.big_units != plan.total_units))) {
     ctx->err = "rx_multi: this build's unit plan is not the same for every capture";   // (A/B builds with a re-cut last wave)
     return BTLE_EINVAL;
   }
   CfgSlot *cs = nullptr;
-  rc = upload_cfgs(ctx, cfgs, multi ? n_cfgs : n_streams, st, sid, &cs, cfg_capture, rot);
+  rc = upload_cfgs(ctx, cfgs, n_cfgs, st, sid, &cs, cfg_capture, rot);
   if (rc) return rc;
   const MapSlot *ms = nullptr;
   rc = get_maps(ctx, d_iq, n_streams, stride, n_int8, &ms);
@@ -2168,24 +2185,9 @@ int launch_rx(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t s
     zero_next = ctx->d_count_ring + (ctx->ring_pos + kCountRing / 2) % kCountRing;
   }
   const unsigned grid = (unsigned)std::min<long long>(plan.total_units, (long long)ctx->num_sms * kCtasPerSm);   // one persistent CTA per SM
-  const unsigned cap32 = (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu);
-  uint2 *dir2 = reinterpret_cast<uint2 *>(d_dir);
-  if (multi && rot)
-    btle_rx_persistent_kernel<kMaxCfgsPerCapture, true><<<grid, kThreads, sizeof(Smem<kMaxCfgsPerCapture>), st>>>(
-        ms->map32, ms->map12, d_iq, (long long)stride, (long long)n_int8, cs->d_params, plan, d_out, cap32, d_count, dir2, zero_next, lead,
-        cs->d_vmap, cs->d_rot);
-  else if (multi)
-    btle_rx_persistent_kernel<kMaxCfgsPerCapture, false><<<grid, kThreads, sizeof(Smem<kMaxCfgsPerCapture>), st>>>(
-        ms->map32, ms->map12, d_iq, (long long)stride, (long long)n_int8, cs->d_params, plan, d_out, cap32, d_count, dir2, zero_next, lead,
-        cs->d_vmap, nullptr);
-  else if (rot)
-    btle_rx_persistent_kernel<1, true><<<grid, kThreads, sizeof(Smem<1>), st>>>(
-        ms->map32, ms->map12, d_iq, (long long)stride, (long long)n_int8, cs->d_params, plan, d_out, cap32, d_count, dir2, zero_next, lead,
-        nullptr, cs->d_rot);
-  else
-    btle_rx_persistent_kernel<1, false><<<grid, kThreads, sizeof(Smem<1>), st>>>(
-        ms->map32, ms->map12, d_iq, (long long)stride, (long long)n_int8, cs->d_params, plan, d_out, cap32, d_count, dir2, zero_next, lead,
-        nullptr, nullptr);
+  const auto enqueue = multi ? (rot ? enqueue_rx<kMaxCfgsPerCapture, true> : enqueue_rx<kMaxCfgsPerCapture, false>)
+                             : (rot ? enqueue_rx<1, true> : enqueue_rx<1, false>);
+  enqueue(grid, st, ms, d_iq, stride, n_int8, cs, plan, d_out, (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu), d_count, d_dir, zero_next, lead);
   BTLE_CUDA(ctx, cudaGetLastError());
   if (ring) {                                                 // the position is taken only by a launch that was enqueued
     ctx->ring_pos = (ctx->ring_pos + 1) % kCountRing;
@@ -2261,14 +2263,25 @@ int h2d_rows(btle_b200_ctx *ctx, int8_t *dst, size_t dpitch, const int8_t *src, 
   return BTLE_OK;
 }
 
-// Host captures (n_streams rows `stride` bytes apart, page-locked or pageable) -> ctx->d_iq, rows `*pitch` bytes apart.
-// Exactly the caller's bytes are read: n_int8 per capture, never the padding behind the last one.
-int ingest(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stride, size_t n_int8, size_t *pitch) {
-  if (n_streams > 1 && stride < n_int8) { ctx->err = "stream stride smaller than stream length"; return BTLE_EINVAL; }
+// Host captures (n_captures rows `stride` bytes apart, page-locked or pageable) -> ctx->d_iq, rows `*pitch` bytes apart:
+// captures caps[0, n_read) (ascending; nullptr: captures 0 .. n_read - 1) one after the other, one copy per run of
+// consecutive captures.  Exactly the caller's bytes are read: n_int8 per capture, never the padding behind the last one.
+int ingest(btle_b200_ctx *ctx, const int8_t *iq, size_t n_captures, size_t stride, size_t n_int8, const int32_t *caps, size_t n_read,
+           size_t *pitch) {
+  if (n_captures > 1 && stride < n_int8) { ctx->err = "stream stride smaller than stream length"; return BTLE_EINVAL; }
   *pitch = (n_int8 + 15) & ~size_t(15);
-  const int rc = ctx->d_iq.reserve(ctx, std::max<size_t>(*pitch * n_streams, 16));
+  const size_t spitch = n_captures > 1 ? stride : n_int8;
+  int rc = ctx->d_iq.reserve(ctx, std::max<size_t>(*pitch * n_read, 16));
   if (rc) return rc;
-  return h2d_rows(ctx, ctx->d_iq, *pitch, iq, n_streams > 1 ? stride : n_int8, n_int8, n_streams, ctx->stream);
+  for (size_t g = 0; g < n_read;) {
+    size_t e = caps ? g + 1 : n_read;
+    while (e < n_read && caps[e] == caps[e - 1] + 1) ++e;
+    if (g) BTLE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // a new copy may reuse the page-locked staging of the last one
+    rc = h2d_rows(ctx, ctx->d_iq + g * *pitch, *pitch, iq + (caps ? (size_t)caps[g] : 0) * spitch, spitch, n_int8, e - g, ctx->stream);
+    if (rc) return rc;
+    g = e;
+  }
+  return BTLE_OK;
 }
 
 // After a launch on `st` that counted its results in ctx->d_count: the count to the host and a wait (*found = the
@@ -2303,6 +2316,59 @@ int fetch_ordered(btle_b200_ctx *ctx, const btle_pkt_rec *d_out, const btle_unit
   }
   if (*n_out > cap) { ctx->err = "output capacity too small"; return BTLE_EOVERFLOW; }
   return BTLE_OK;
+}
+
+// The receive entry points: cfg i decodes capture cfg_capture[i], or capture i when cfg_capture is nullptr (then
+// n_cfgs == n_captures).  rx_device_path checks and enqueues a launch on device-resident captures.
+int rx_device_path(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_captures, size_t stride, size_t n_int8, const btle_stream_cfg *cfgs,
+                   const int32_t *cfg_capture, size_t n_cfgs, const float *offset_hz, btle_pkt_rec *d_out, size_t cap, uint32_t *d_count,
+                   btle_unit_dir *d_dir, size_t dir_cap, void *cuda_stream) {
+  if (!ctx) return BTLE_EINVAL;
+  if ((!d_out && cap) || (!cfgs && n_cfgs) || !d_dir) { ctx->err = "rx: missing buffer"; return BTLE_EINVAL; }
+  if ((reinterpret_cast<uintptr_t>(d_iq) & 15) || (n_captures > 1 && (stride & 15))) { ctx->err = "device IQ must be 16-byte aligned"; return BTLE_EINVAL; }
+  if (n_captures > 1 && stride < n_int8) { ctx->err = "stream stride smaller than stream length"; return BTLE_EINVAL; }
+  size_t groups = n_cfgs;
+  int rc = cfg_capture ? check_cfg_capture(ctx, n_captures, cfg_capture, n_cfgs, &groups) : BTLE_OK;
+  if (rc) return rc;
+  if (dir_cap < rx_units(ctx, groups, n_cfgs, n_int8)) { ctx->err = "unit directory too small (btle_b200_rx_units / _rx_multi_units)"; return BTLE_EINVAL; }
+  rc = validate_cfgs(ctx, cfgs, n_cfgs);
+  if (rc) return rc;
+  std::vector<int4> rot;
+  if (offset_hz && (rc = make_rots(ctx, offset_hz, n_captures, cfg_capture, n_cfgs, rot))) return rc;
+  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
+  return launch_rx(ctx, d_iq, n_captures, stride, n_int8, cfgs, cfg_capture, n_cfgs, offset_hz ? rot.data() : nullptr, d_out, cap, d_count,
+                   d_dir, reinterpret_cast<cudaStream_t>(cuda_stream), 0);
+}
+
+// Host captures in, records out in reference order: only the captures some cfg reads are copied, one after the other,
+// and the list is renumbered to match (a list that names each capture it reads once is then cfg i on capture i).
+int rx_host_path(btle_b200_ctx *ctx, const int8_t *iq, size_t n_captures, size_t stride, size_t n_int8, const btle_stream_cfg *cfgs,
+                 const int32_t *cfg_capture, size_t n_cfgs, const float *offset_hz, btle_pkt_rec *out, size_t cap, size_t *n_out) {
+  if (!ctx) return BTLE_EINVAL;
+  if (!n_out || (!out && cap) || (!cfgs && n_cfgs) || (!iq && n_captures && n_int8)) { ctx->err = "rx: missing buffer"; return BTLE_EINVAL; }
+  *n_out = 0;
+  size_t groups = n_cfgs;
+  int rc = cfg_capture ? check_cfg_capture(ctx, n_captures, cfg_capture, n_cfgs, &groups) : BTLE_OK;
+  if (rc) return rc;
+  rc = validate_cfgs(ctx, cfgs, n_cfgs);
+  if (rc) return rc;
+  std::vector<int4> rot;
+  if (offset_hz && (rc = make_rots(ctx, offset_hz, n_captures, cfg_capture, n_cfgs, rot))) return rc;
+  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
+  std::vector<int32_t> caps, local;                          // the captures read, in order; cfg i reads caps[local[i]]
+  for (size_t i = 0; cfg_capture && i < n_cfgs; ++i) {
+    if (!i || cfg_capture[i] != cfg_capture[i - 1]) caps.push_back(cfg_capture[i]);
+    local.push_back((int32_t)caps.size() - 1);
+  }
+  size_t pitch = 0;
+  rc = ingest(ctx, iq, n_captures, stride, n_int8, cfg_capture ? caps.data() : nullptr, groups, &pitch);
+  if (rc) return rc;
+  const size_t units = rx_units(ctx, groups, n_cfgs, n_int8);
+  if (ctx->d_out.reserve(ctx, std::max<size_t>(cap, 1)) || ctx->d_dir.reserve(ctx, std::max<size_t>(units, 1))) return BTLE_ENOMEM;
+  rc = launch_rx(ctx, ctx->d_iq, groups, pitch, n_int8, cfgs, cfg_capture ? local.data() : nullptr, n_cfgs, offset_hz ? rot.data() : nullptr,
+                 ctx->d_out, cap, ctx->d_count, ctx->d_dir, ctx->stream, 0);
+  if (rc) return rc;
+  return fetch_ordered(ctx, ctx->d_out, ctx->d_dir, units, out, cap, n_out, ctx->stream);
 }
 
 int launch_sps8_hits(btle_b200_ctx *ctx, const int16_t *d_iq16, size_t n_samples, uint32_t aa, long long *d_hits, size_t cap, unsigned *d_count,
@@ -2494,29 +2560,21 @@ void btle_b200_destroy(btle_b200_ctx *ctx) {
 }
 
 size_t btle_b200_rx_units(const btle_b200_ctx *ctx, size_t n_streams, size_t n_int8) {
-  if (!ctx || !n_streams || n_int8 < (size_t)kChunkInt8) return 0;
-  return (size_t)plan_for(ctx, n_streams, n_int8).total_units;
+  return ctx ? rx_units(ctx, n_streams, n_streams, n_int8) : 0;
 }
 
 int btle_b200_rx_device_dir_offset(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8,
                                    const btle_stream_cfg *cfgs, const float *offset_hz, btle_pkt_rec *d_out, size_t cap, uint32_t *d_count,
                                    btle_unit_dir *d_dir, size_t dir_cap, void *cuda_stream) {
-  if (!ctx || (!d_out && cap) || (!cfgs && n_streams) || !d_dir) return BTLE_EINVAL;
-  if ((reinterpret_cast<uintptr_t>(d_iq) & 15) || (n_streams > 1 && (stride & 15))) { ctx->err = "device IQ must be 16-byte aligned"; return BTLE_EINVAL; }
-  if (dir_cap < btle_b200_rx_units(ctx, n_streams, n_int8)) { ctx->err = "unit directory too small (btle_b200_rx_units)"; return BTLE_EINVAL; }
-  int rc = validate_cfgs(ctx, cfgs, n_streams);
-  if (rc) return rc;
-  std::vector<int4> rot;
-  if (offset_hz && (rc = make_rots(ctx, offset_hz, n_streams, nullptr, n_streams, rot))) return rc;
-  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
-  return launch_rx(ctx, d_iq, n_streams, stride, n_int8, cfgs, d_out, cap, d_count, d_dir, reinterpret_cast<cudaStream_t>(cuda_stream), 0,
-                   nullptr, 0, 0, offset_hz ? rot.data() : nullptr);
+  return rx_device_path(ctx, d_iq, n_streams, stride, n_int8, cfgs, nullptr, n_streams, offset_hz, d_out, cap, d_count, d_dir, dir_cap,
+                        cuda_stream);
 }
 
 int btle_b200_rx_device_dir(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8,
                             const btle_stream_cfg *cfgs, btle_pkt_rec *d_out, size_t cap, uint32_t *d_count,
                             btle_unit_dir *d_dir, size_t dir_cap, void *cuda_stream) {
-  return btle_b200_rx_device_dir_offset(ctx, d_iq, n_streams, stride, n_int8, cfgs, nullptr, d_out, cap, d_count, d_dir, dir_cap, cuda_stream);
+  return rx_device_path(ctx, d_iq, n_streams, stride, n_int8, cfgs, nullptr, n_streams, nullptr, d_out, cap, d_count, d_dir, dir_cap,
+                        cuda_stream);
 }
 
 int btle_b200_rx_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8,
@@ -2527,7 +2585,8 @@ int btle_b200_rx_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams
   // the directory goes to context-owned scratch (callers of this entry point sort the records themselves)
   const int rc = ctx->d_dir.reserve(ctx, std::max<size_t>(btle_b200_rx_units(ctx, n_streams, n_int8), 1));
   if (rc) return rc;
-  return btle_b200_rx_device_dir(ctx, d_iq, n_streams, stride, n_int8, cfgs, d_out, cap, d_count, ctx->d_dir, ctx->d_dir.n, cuda_stream);
+  return rx_device_path(ctx, d_iq, n_streams, stride, n_int8, cfgs, nullptr, n_streams, nullptr, d_out, cap, d_count, ctx->d_dir,
+                        ctx->d_dir.n, cuda_stream);
 }
 
 void btle_b200_sort_records(btle_pkt_rec *recs, size_t n) { std::sort(recs, recs + n, rec_less); }
@@ -2550,24 +2609,12 @@ int btle_b200_gather_ordered(const btle_pkt_rec *recs, size_t n_recs, const btle
 
 int btle_b200_rx_batch_offset(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stride, size_t n_int8,
                               const btle_stream_cfg *cfgs, const float *offset_hz, btle_pkt_rec *out, size_t cap, size_t *n_out) {
-  if (!ctx || !n_out || (!out && cap) || (!cfgs && n_streams) || (!iq && n_streams && n_int8)) return BTLE_EINVAL;
-  *n_out = 0;
-  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
-  size_t pitch = 0;
-  int rc = ingest(ctx, iq, n_streams, stride, n_int8, &pitch);
-  if (rc) return rc;
-  const size_t units = btle_b200_rx_units(ctx, n_streams, n_int8);
-  if (ctx->d_out.reserve(ctx, std::max<size_t>(cap, 1)) || ctx->d_dir.reserve(ctx, std::max<size_t>(units, 1))) return BTLE_ENOMEM;
-  rc = btle_b200_rx_device_dir_offset(ctx, ctx->d_iq, n_streams, pitch, n_int8, cfgs, offset_hz, ctx->d_out, cap, ctx->d_count, ctx->d_dir,
-                                      ctx->d_dir.n, st);
-  if (rc) return rc;
-  return fetch_ordered(ctx, ctx->d_out, ctx->d_dir, units, out, cap, n_out, st);
+  return rx_host_path(ctx, iq, n_streams, stride, n_int8, cfgs, nullptr, n_streams, offset_hz, out, cap, n_out);
 }
 
 int btle_b200_rx_batch(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stride, size_t n_int8,
                        const btle_stream_cfg *cfgs, btle_pkt_rec *out, size_t cap, size_t *n_out) {
-  return btle_b200_rx_batch_offset(ctx, iq, n_streams, stride, n_int8, cfgs, nullptr, out, cap, n_out);
+  return rx_host_path(ctx, iq, n_streams, stride, n_int8, cfgs, nullptr, n_streams, nullptr, out, cap, n_out);
 }
 
 int btle_b200_rec_offset_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t stride, size_t n_int8, const btle_pkt_rec *d_recs, size_t n,
@@ -2593,7 +2640,7 @@ int btle_b200_rec_offset(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams,
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
   size_t pitch = 0;
-  int rc = ingest(ctx, iq, n_streams, stride, n_int8, &pitch);
+  int rc = ingest(ctx, iq, n_streams, stride, n_int8, nullptr, n_streams, &pitch);
   if (rc) return rc;
   if (ctx->d_out.reserve(ctx, n) || ctx->d_hz.reserve(ctx, n)) return BTLE_ENOMEM;
   BTLE_CUDA(ctx, cudaMemcpyAsync(ctx->d_out, recs, n * sizeof(btle_pkt_rec), cudaMemcpyHostToDevice, st));
@@ -2626,7 +2673,7 @@ int btle_b200_rx_iq16(btle_b200_ctx *ctx, const int16_t *iq16, size_t n_int16, i
 
 int btle_b200_rx(btle_b200_ctx *ctx, const int8_t *iq, size_t n_int8, const btle_stream_cfg *cfg, btle_pkt_rec *out,
                  size_t cap, size_t *n_out) {
-  return btle_b200_rx_batch(ctx, iq, 1, n_int8, n_int8, cfg, out, cap, n_out);
+  return rx_host_path(ctx, iq, 1, n_int8, n_int8, cfg, nullptr, 1, nullptr, out, cap, n_out);
 }
 
 // ---- several cfgs per capture -------------------------------------------------------------------------------------
@@ -2637,28 +2684,16 @@ size_t btle_b200_rx_multi_units(const btle_b200_ctx *ctx, size_t n_captures, con
   const std::string keep = c->err;                        // a query: leaves last_error as it was
   const int rc = check_cfg_capture(c, n_captures, cfg_capture, n_cfgs, &groups);
   c->err = keep;
-  return rc ? 0 : n_cfgs * multi_units_per_group(ctx, groups, n_int8);
+  return rc ? 0 : rx_units(ctx, groups, n_cfgs, n_int8);
 }
 
 int btle_b200_rx_multi_device_dir_offset(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_captures, size_t stride, size_t n_int8,
                                          const btle_stream_cfg *cfgs, const int32_t *cfg_capture, size_t n_cfgs, const float *offset_hz,
                                          btle_pkt_rec *d_out, size_t cap, uint32_t *d_count, btle_unit_dir *d_dir, size_t dir_cap,
                                          void *cuda_stream) {
-  if (!ctx) return BTLE_EINVAL;
-  if ((!d_out && cap) || (!cfgs && n_cfgs) || !d_dir) { ctx->err = "rx_multi: missing buffer"; return BTLE_EINVAL; }
-  if ((reinterpret_cast<uintptr_t>(d_iq) & 15) || (n_captures > 1 && (stride & 15))) { ctx->err = "device IQ must be 16-byte aligned"; return BTLE_EINVAL; }
-  if (n_captures > 1 && stride < n_int8) { ctx->err = "stream stride smaller than stream length"; return BTLE_EINVAL; }
-  size_t groups = 0;
-  int rc = check_cfg_capture(ctx, n_captures, cfg_capture, n_cfgs, &groups);
-  if (rc) return rc;
-  if (dir_cap < n_cfgs * multi_units_per_group(ctx, groups, n_int8)) { ctx->err = "unit directory too small (btle_b200_rx_multi_units)"; return BTLE_EINVAL; }
-  rc = validate_cfgs(ctx, cfgs, n_cfgs);
-  if (rc) return rc;
-  std::vector<int4> rot;
-  if (offset_hz && (rc = make_rots(ctx, offset_hz, n_captures, cfg_capture, n_cfgs, rot))) return rc;
-  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
-  return launch_rx(ctx, d_iq, n_captures, stride, n_int8, cfgs, d_out, cap, d_count, d_dir, reinterpret_cast<cudaStream_t>(cuda_stream), 0,
-                   cfg_capture, n_cfgs, groups, offset_hz ? rot.data() : nullptr);
+  if (ctx && n_cfgs && !cfg_capture) { ctx->err = "rx_multi: missing cfg_capture"; return BTLE_EINVAL; }
+  return rx_device_path(ctx, d_iq, n_captures, stride, n_int8, cfgs, cfg_capture, n_cfgs, offset_hz, d_out, cap, d_count, d_dir, dir_cap,
+                        cuda_stream);
 }
 
 int btle_b200_rx_multi_device_dir(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_captures, size_t stride, size_t n_int8,
@@ -2675,42 +2710,8 @@ int btle_b200_rx_multi(btle_b200_ctx *ctx, const int8_t *iq, size_t n_captures, 
 
 int btle_b200_rx_multi_offset(btle_b200_ctx *ctx, const int8_t *iq, size_t n_captures, size_t stride, size_t n_int8, const btle_stream_cfg *cfgs,
                               const int32_t *cfg_capture, size_t n_cfgs, const float *offset_hz, btle_pkt_rec *out, size_t cap, size_t *n_out) {
-  if (!ctx) return BTLE_EINVAL;
-  if (!n_out || (!out && cap) || (!cfgs && n_cfgs) || (!iq && n_captures && n_int8)) { ctx->err = "rx_multi: missing buffer"; return BTLE_EINVAL; }
-  *n_out = 0;
-  if (n_captures > 1 && stride < n_int8) { ctx->err = "stream stride smaller than stream length"; return BTLE_EINVAL; }
-  size_t groups = 0;
-  int rc = check_cfg_capture(ctx, n_captures, cfg_capture, n_cfgs, &groups);
-  if (rc) return rc;
-  rc = validate_cfgs(ctx, cfgs, n_cfgs);
-  if (rc) return rc;
-  std::vector<int4> rot;
-  if (offset_hz && (rc = make_rots(ctx, offset_hz, n_captures, cfg_capture, n_cfgs, rot))) return rc;
-  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
-  // only the captures some cfg reads are copied, one after the other; cfg_capture is renumbered to match
-  const size_t pitch = (n_int8 + 15) & ~size_t(15), spitch = n_captures > 1 ? stride : n_int8;
-  rc = ctx->d_iq.reserve(ctx, std::max<size_t>(pitch * groups, 16));
-  if (rc) return rc;
-  std::vector<int32_t> local(n_cfgs), caps;
-  for (size_t i = 0; i < n_cfgs; ++i) {
-    if (!i || cfg_capture[i] != cfg_capture[i - 1]) caps.push_back(cfg_capture[i]);
-    local[i] = (int32_t)caps.size() - 1;
-  }
-  for (size_t g = 0; g < caps.size();) {                   // one copy per run of consecutive captures
-    size_t e = g + 1;
-    while (e < caps.size() && caps[e] == caps[e - 1] + 1) ++e;
-    if (g) BTLE_CUDA(ctx, cudaStreamSynchronize(st));      // a new copy may reuse the page-locked staging of the last one
-    rc = h2d_rows(ctx, ctx->d_iq + g * pitch, pitch, iq + (size_t)caps[g] * spitch, spitch, n_int8, e - g, st);
-    if (rc) return rc;
-    g = e;
-  }
-  const size_t units = n_cfgs * multi_units_per_group(ctx, groups, n_int8);
-  if (ctx->d_out.reserve(ctx, std::max<size_t>(cap, 1)) || ctx->d_dir.reserve(ctx, std::max<size_t>(units, 1))) return BTLE_ENOMEM;
-  rc = launch_rx(ctx, ctx->d_iq, groups, pitch, n_int8, cfgs, ctx->d_out, cap, ctx->d_count, ctx->d_dir, st, 0, local.data(), n_cfgs, groups,
-                 offset_hz ? rot.data() : nullptr);
-  if (rc) return rc;
-  return fetch_ordered(ctx, ctx->d_out, ctx->d_dir, units, out, cap, n_out, st);
+  if (ctx && n_cfgs && !cfg_capture) { ctx->err = "rx_multi: missing cfg_capture"; return BTLE_EINVAL; }
+  return rx_host_path(ctx, iq, n_captures, stride, n_int8, cfgs, cfg_capture, n_cfgs, offset_hz, out, cap, n_out);
 }
 
 // ---- streaming sessions: N time-aligned captures of unbounded length, pushed in pieces ----------------------------
@@ -2719,8 +2720,8 @@ int btle_b200_rx_multi_offset(btle_b200_ctx *ctx, const int8_t *iq, size_t n_cap
 // One segment SET = `seg_chunks` chunks of every capture.  Capture i's part of a set sits at i * stride in the half's
 // buffers: kLead bytes of the previous set, the segment, kLook look-ahead bytes (the start of the next set).  Once every
 // capture has filled its own, a set's live cfgs are decoded in rounds of at most kMaxCfgsPerCapture cfgs per capture,
-// one launch of the persistent kernel each: the single-cfg kernel for a round of one cfg per capture in capture order
-// (every set of a session whose cfg list never changed), rx_multi otherwise.  A cfg added for chunks that are still
+// one launch of the persistent kernel each (launch_rx: the single-cfg kernel for a round of one cfg per capture in
+// capture order, as every set of a session whose cfg list never changed is).  A cfg added for chunks that are still
 // resident is decoded over them by one more round on the half that holds them (backfill).
 struct btle_b200_streams {
   btle_b200_ctx *ctx = nullptr;
@@ -2781,9 +2782,8 @@ namespace {
 using Streams = btle_b200_streams;
 
 // One round's launch over half b's set, enqueued behind whatever its stream holds: cfgs `idx` (stable indices, sorted
-// by capture, at most kMaxCfgsPerCapture per capture) on the set's n_submitted bytes.  One cfg per capture in capture
-// order is a single-cfg launch (which, unlike rx_multi, also runs in builds with an uneven unit plan); any other round
-// is an rx_multi launch.  Buffers, strides and cfgs are the session's own, checked when made.  Collected by streams_collect.
+// by capture, at most kMaxCfgsPerCapture per capture) on the set's n_submitted bytes.  Buffers, strides and cfgs are the
+// session's own, checked when made.  Collected by streams_collect.
 int streams_job(Streams *s, int b, const std::vector<size_t> &idx) {
   btle_b200_ctx *ctx = s->ctx;
   auto &H = s->half[b];
@@ -2803,15 +2803,13 @@ int streams_job(Streams *s, int b, const std::vector<size_t> &idx) {
     groups += !i || cc[i] != cc[i - 1];
     if (!H.offset.empty()) rot.push_back(make_rot(H.offset[cc[i]]));
   }
-  const bool single = k == s->n && groups == k;
-  const size_t units = std::max<size_t>(single ? btle_b200_rx_units(ctx, s->n, H.n_submitted)
-                                               : k * multi_units_per_group(ctx, groups, H.n_submitted), 1);
+  const size_t units = std::max<size_t>(rx_units(ctx, groups, k, H.n_submitted), 1);
   const size_t cap = k * nch * BTLE_MAX_RECS_PER_CHUNK;      // the most a launch can find: never an overflow
   if (J.d_out.reserve(ctx, cap) || J.d_dir.reserve(ctx, units) || J.h_dir.reserve(ctx, units) ||
       (!J.d_count && (J.d_count.alloc(ctx, 1) || J.h_count.alloc(ctx, 1))))
     return BTLE_ENOMEM;
-  const int rc = launch_rx(ctx, H.d + Streams::kLead, s->n, s->stride, H.n_submitted, cfgs.data(), J.d_out, cap, J.d_count, J.d_dir,
-                           H.st, Streams::kLead, single ? nullptr : cc.data(), k, groups, rot.empty() ? nullptr : rot.data());
+  const int rc = launch_rx(ctx, H.d + Streams::kLead, s->n, s->stride, H.n_submitted, cfgs.data(), cc.data(), k,
+                           rot.empty() ? nullptr : rot.data(), J.d_out, cap, J.d_count, J.d_dir, H.st, Streams::kLead);
   if (rc) return rc;
   BTLE_CUDA(ctx, cudaMemcpyAsync(J.h_count, J.d_count, sizeof(unsigned), cudaMemcpyDeviceToHost, H.st));
   BTLE_CUDA(ctx, cudaMemcpyAsync(J.h_dir, J.d_dir, units * sizeof(btle_unit_dir), cudaMemcpyDeviceToHost, H.st));
@@ -3516,7 +3514,7 @@ int btle_b200_discover(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, s
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
   size_t pitch = 0;
-  rc = ingest(ctx, iq, n_streams, stride, n_int8, &pitch);
+  rc = ingest(ctx, iq, n_streams, stride, n_int8, nullptr, n_streams, &pitch);
   if (rc) return rc;
   rc = ctx->d_cand.reserve(ctx, std::max<size_t>(cap, 1));
   if (rc) return rc;
@@ -3808,7 +3806,7 @@ int btle_b200_rx_ber_run(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg, size_t 
     rc = launch_rx_ber_synth(ctx, *cfg, done, n_packets, (long long)(n_int8 / 2), (long long)n, ctx->d_iq, d_truth, st);
     if (rc) return rc;
     const size_t cap = (size_t)chunks * BTLE_MAX_RECS_PER_CHUNK, units = btle_b200_rx_units(ctx, 1, n_int8);
-    rc = launch_rx(ctx, ctx->d_iq, 1, n_int8, n_int8, &scfg, ctx->d_out, cap, ctx->d_count, ctx->d_dir, st, 0);
+    rc = launch_rx(ctx, ctx->d_iq, 1, n_int8, n_int8, &scfg, nullptr, 1, nullptr, ctx->d_out, cap, ctx->d_count, ctx->d_dir, st, 0);
     if (rc) return rc;
     rc = launch_rx_ber_score(ctx, d_truth, n, ctx->d_out, cap, ctx->d_dir, units, d_res, st);
     if (rc) return rc;

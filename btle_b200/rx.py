@@ -48,6 +48,11 @@ def _offsets(offset_hz, n: int):
     return np.ascontiguousarray(np.broadcast_to(np.asarray(offset_hz, dtype=np.float32), (n,)))
 
 
+def _ptr(a):
+    """a's data pointer, or None (NULL) for None"""
+    return None if a is None else a.ctypes.data
+
+
 class BtleRx:
     def __init__(self, device: int = 0):
         self._L = _native.load()
@@ -110,10 +115,7 @@ class BtleRx:
         off = _offsets(offset_hz, ns)
         # default capacity: typical worst case; grown once on BTLE_EOVERFLOW to the exact count, which is at most
         # BTLE_MAX_PKTS_PER_CHUNK (51) records per chunk, or BTLE_MAX_RECS_PER_CHUNK (123) with BTLE_CFG_REPORT_REJECTED
-        if off is None:
-            call = partial(self._L.btle_b200_rx_batch, self._h, iq.ctypes.data, ns, n, n, cfgs.ctypes.data)
-        else:
-            call = partial(self._L.btle_b200_rx_batch_offset, self._h, iq.ctypes.data, ns, n, n, cfgs.ctypes.data, off.ctypes.data)
+        call = partial(self._L.btle_b200_rx_batch_offset, self._h, iq.ctypes.data, ns, n, n, cfgs.ctypes.data, _ptr(off))
         return self._grow_once(call, REC_DTYPE, ns * (n // 16384) * 34 + 16 if cap is None else cap, grow=cap is None)
 
     def rx_multi(self, iq: np.ndarray, cfgs: np.ndarray, capture, cap: int | None = None, offset_hz=None) -> np.ndarray:
@@ -129,11 +131,8 @@ class BtleRx:
         cc = np.ascontiguousarray(capture, dtype=np.int32).reshape(-1)
         assert cc.shape == cfgs.shape
         off = _offsets(offset_hz, ns)
-        if off is None:
-            call = partial(self._L.btle_b200_rx_multi, self._h, iq.ctypes.data, ns, n, n, cfgs.ctypes.data, cc.ctypes.data, cfgs.size)
-        else:
-            call = partial(self._L.btle_b200_rx_multi_offset, self._h, iq.ctypes.data, ns, n, n, cfgs.ctypes.data, cc.ctypes.data, cfgs.size,
-                           off.ctypes.data)
+        call = partial(self._L.btle_b200_rx_multi_offset, self._h, iq.ctypes.data, ns, n, n, cfgs.ctypes.data, cc.ctypes.data, cfgs.size,
+                       _ptr(off))
         return self._grow_once(call, REC_DTYPE, cfgs.size * (n // 16384) * 34 + 16 if cap is None else cap, grow=cap is None)
 
     def multi_units(self, n_captures: int, capture, n_int8: int) -> int:
@@ -151,13 +150,9 @@ class BtleRx:
         cap = d_out.numel() * d_out.element_size() // 64
         dir_cap = d_dir.numel() * d_dir.element_size() // 8
         off = _offsets(offset_hz, ns)
-        head = (self._h, d_iq.data_ptr(), ns, d_iq.stride(0), n, cfgs.ctypes.data, cc.ctypes.data, cfgs.size)
-        tail = (d_out.data_ptr(), cap, d_count.data_ptr() if d_count is not None else None, d_dir.data_ptr(), dir_cap, ctypes.c_void_p(stream_ptr))
-        if off is None:
-            rc = self._L.btle_b200_rx_multi_device_dir(*head, *tail)
-        else:
-            rc = self._L.btle_b200_rx_multi_device_dir_offset(*head, off.ctypes.data, *tail)
-        self._check(rc)
+        self._check(self._L.btle_b200_rx_multi_device_dir_offset(
+            self._h, d_iq.data_ptr(), ns, d_iq.stride(0), n, cfgs.ctypes.data, cc.ctypes.data, cfgs.size, _ptr(off), d_out.data_ptr(), cap,
+            d_count.data_ptr() if d_count is not None else None, d_dir.data_ptr(), dir_cap, ctypes.c_void_p(stream_ptr)))
 
     def rx(self, iq: np.ndarray, offset_hz=None, **cfg) -> np.ndarray:
         return self.rx_batch(np.asarray(iq).reshape(1, -1), make_cfgs(1, **cfg), offset_hz=offset_hz)
@@ -288,13 +283,9 @@ class BtleRx:
         cap = d_out.numel() * d_out.element_size() // 64
         dir_cap = d_dir.numel() * d_dir.element_size() // 8
         off = _offsets(offset_hz, ns)
-        head = (self._h, d_iq.data_ptr(), ns, d_iq.stride(0), n, cfgs.ctypes.data)
-        tail = (d_out.data_ptr(), cap, d_count.data_ptr() if d_count is not None else None, d_dir.data_ptr(), dir_cap, ctypes.c_void_p(stream_ptr))
-        if off is None:
-            rc = self._L.btle_b200_rx_device_dir(*head, *tail)
-        else:
-            rc = self._L.btle_b200_rx_device_dir_offset(*head, off.ctypes.data, *tail)
-        self._check(rc)
+        self._check(self._L.btle_b200_rx_device_dir_offset(
+            self._h, d_iq.data_ptr(), ns, d_iq.stride(0), n, cfgs.ctypes.data, _ptr(off), d_out.data_ptr(), cap,
+            d_count.data_ptr() if d_count is not None else None, d_dir.data_ptr(), dir_cap, ctypes.c_void_p(stream_ptr)))
 
     def rec_offsets_device(self, d_iq, d_recs, n: int, d_hz, stream_ptr: int = 0):
         """rec_offsets on the device: d_iq as rx_device_dir's, d_recs n records (uint8 CUDA tensor of n * 64 bytes),

@@ -165,7 +165,7 @@ int btle_b200_rx_batch_offset(btle_b200_ctx *ctx, const int8_t *iq, size_t n_str
 int btle_b200_rx(btle_b200_ctx *ctx, const int8_t *iq, size_t n_int8, const btle_stream_cfg *cfg,
                  btle_pkt_rec *out, size_t cap, size_t *n_out);
 
-/* Device-resident variant: `d_iq` (16-byte aligned; stride a multiple of 16 when n_streams > 1), `d_out`, `d_count`
+/* Device-resident variant: `d_iq` (16-byte aligned; stride a multiple of 16 and >= n_int8 when n_streams > 1), `d_out`, `d_count`
  * and `d_dir` are device pointers usable from the context's device (local HBM or PEER memory of another GPU —
  * that is how the multi-GPU gather works: every rank's kernel stores its records straight into rank 0's buffer
  * over NVLink); work is enqueued on `cuda_stream` (a cudaStream_t, may be NULL) and NOT synchronised.
@@ -212,7 +212,10 @@ void btle_b200_sort_records(btle_pkt_rec *recs, size_t n);
  * once, whatever the number of cfgs reading it; the prefilter flags the union of the cfgs' candidates, and every
  * candidate is re-checked exactly per cfg.  Argument errors (a cfg_capture that decreases, leaves the range or names one
  * capture more than BTLE_MAX_CFGS_PER_CAPTURE times; the alignment and stride rules of the calls above) are BTLE_EINVAL
- * with btle_b200_last_error() set, and the context stays usable; BTLE_EOVERFLOW reports the needed count in *n_out. */
+ * with btle_b200_last_error() set, and the context stays usable; BTLE_EOVERFLOW reports the needed count in *n_out.
+ * A cfg_capture that maps cfg j to capture j for every capture is the launch of btle_b200_rx_batch / _rx_device_dir (same
+ * kernel, same directory); btle_b200_rx_multi copies only the captures named, so there a list that names each of them
+ * once is that launch too. */
 #define BTLE_MAX_CFGS_PER_CAPTURE 8
 int btle_b200_rx_multi(btle_b200_ctx *ctx, const int8_t *iq, size_t n_captures, size_t stream_stride_int8, size_t n_int8,
                        const btle_stream_cfg *cfgs, const int32_t *cfg_capture, size_t n_cfgs, btle_pkt_rec *out, size_t cap,
@@ -343,9 +346,9 @@ int btle_b200_discover(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, s
  * btle_b200_rx_batch() on cfg j's capture (cut to the shortest capture) decoded with cfg j, kept for
  * from_chunk <= chunk < until_chunk; each is returned exactly once, per set in (j, chunk, n0) order.
  * A set's live cfgs are sorted by capture and decoded in rounds of at most BTLE_MAX_CFGS_PER_CAPTURE cfgs per capture,
- * one launch per round: a round of one cfg per capture in capture order is the single-cfg launch described above (every
- * set of a session whose cfg list never changed), any other round a btle_b200_rx_multi_device_dir launch.  A capture no
- * live cfg names is not read by the kernel.
+ * one btle_b200_rx_multi_device_dir launch per round (so a round of one cfg per capture in capture order, as every set
+ * of a session whose cfg list never changed has, is the single-cfg launch described above).  A capture no live cfg names
+ * is not read by the kernel.
  * BACKFILL: the two most recent sets stay on the device (the one whose records were handed out last, and the one in
  * flight).  add_cfg accepts any from_chunk >= btle_b200_streams_resident(); the next commit or finish call decodes every
  * cfg added since the last one over the resident sets that hold chunks >= its from_chunk (rounds of at most

@@ -32,6 +32,11 @@ def lib():
         _lib.emul_rx_stream.restype = ctypes.c_long
         _lib.emul_rx_stream.argtypes = [ctypes.c_void_p, ctypes.c_long, ctypes.POINTER(StreamCfg), ctypes.c_int,
                                         ctypes.c_int, ctypes.c_void_p, ctypes.c_long]
+        vp, lg = ctypes.c_void_p, ctypes.c_long
+        _lib.emul_rx_units.restype = lg
+        _lib.emul_rx_units.argtypes = [vp, lg, lg, lg, vp, vp, lg, ctypes.c_int, ctypes.c_int, vp, lg, vp, lg, ctypes.POINTER(lg)]
+        _lib.emul_check_tapset.restype = lg
+        _lib.emul_check_tapset.argtypes = [vp, vp, lg]
     return _lib
 
 
@@ -47,26 +52,42 @@ def rx_stream(iq, channel=37, access_addr=0x8E89BED6, access_mask=0xFFFFFFFF, cr
     return out[:n]
 
 
-def rx_batch_units(iq2d, cfgs, grid=132, reverse_units=False, force_walk=False):
-    """The kernel's unit plan + resolver passes on the CPU.  iq2d: int8 [n_streams, n_int8]; cfgs: CFG_DTYPE array.
-    Returns (records as stored (block per unit), dir uint32 [n_units, 2])."""
+def rx_units(iq2d, cfgs, capture=None, grid=132, reverse_units=False, force_walk=False):
+    """The kernel's unit plan + resolver passes on the CPU (emul_rx_units), the kernel chosen as launch_rx chooses it.
+    iq2d: int8 [n_captures, n_int8]; cfgs: CFG_DTYPE array; capture[j]: the capture cfg j decodes (None: cfg j on capture j).
+    Returns (count, records as stored (block per (cfg, unit)), dir uint32 [n_entries, 2]); count is -1 for a refused launch."""
     iq2d = np.ascontiguousarray(iq2d, dtype=np.int8)
     ns, n = iq2d.shape
-    cap = ns * (n // 16384) * 123 + 8      # BTLE_MAX_RECS_PER_CHUNK
+    cfgs = np.ascontiguousarray(cfgs).reshape(-1)
+    cc = None if capture is None else np.ascontiguousarray(capture, dtype=np.int32)
+    cap = cfgs.size * (n // 16384) * 123 + 8      # BTLE_MAX_RECS_PER_CHUNK
     out = np.zeros(cap, dtype=REC_DTYPE)
-    dir_cap = ns * ((n // 16384 + 15) // 16) * 16 + 16
+    dir_cap = cfgs.size * ((n // 16384 + 15) // 16 * 16 + 16)
     d = np.zeros((dir_cap, 2), dtype=np.uint32)
-    nu = ctypes.c_long(0)
-    L = lib()
-    L.emul_rx_batch_units.restype = ctypes.c_long
-    L.emul_rx_batch_units.argtypes = [ctypes.c_void_p, ctypes.c_long, ctypes.c_long, ctypes.c_long, ctypes.c_void_p, ctypes.c_int,
-                                      ctypes.c_int, ctypes.c_void_p, ctypes.c_long, ctypes.c_void_p, ctypes.c_long,
-                                      ctypes.POINTER(ctypes.c_long)]
-    cfgs = np.ascontiguousarray(cfgs)
-    cnt = L.emul_rx_batch_units(iq2d.ctypes.data, ns, n, n, cfgs.ctypes.data, grid, int(reverse_units) | (2 if force_walk else 0), out.ctypes.data, cap,
-                                d.ctypes.data, dir_cap, ctypes.byref(nu))
-    assert 0 <= cnt <= cap
-    return out[:cnt], d[:nu.value]
+    nd = ctypes.c_long(0)
+    cnt = lib().emul_rx_units(iq2d.ctypes.data, ns, n, n, cfgs.ctypes.data, None if cc is None else cc.ctypes.data, cfgs.size, grid,
+                              int(reverse_units) | (2 if force_walk else 0), out.ctypes.data, cap, d.ctypes.data, dir_cap, ctypes.byref(nd))
+    assert cnt <= cap
+    return cnt, out[:max(cnt, 0)], d[:nd.value]
+
+
+def rx_batch_units(iq2d, cfgs, grid=132, reverse_units=False, force_walk=False):
+    """rx_units with one cfg per capture: (records as stored (block per unit), dir uint32 [n_units, 2])."""
+    cnt, out, d = rx_units(iq2d, cfgs, None, grid, reverse_units, force_walk)
+    assert cnt >= 0
+    return out, d
+
+
+def rx_multi(iq2d, cfgs, capture, grid=132, reverse_units=False, force_walk=False):
+    """rx_units with a cfg list, records gathered through the unit directory (reference order)."""
+    cnt, out, d = rx_units(iq2d, cfgs, capture, grid, reverse_units, force_walk)
+    assert cnt >= 0
+    return np.concatenate([out[b:b + c] for b, c in d]) if len(d) else out[:0]
+
+
+def check_tapset(cfg, words):
+    """prefilter_union of one cfg against prefilter_any, over consecutive (lo, hi) word pairs; returns the mismatches."""
+    return int(lib().emul_check_tapset(cfg.ctypes.data, words.ctypes.data, words.size))
 
 
 def tables():

@@ -104,37 +104,64 @@ extern "C" long emul_rx_stream(const int8_t *iq, long n_int8, const btle_stream_
 
 // The kernel's unit decomposition and resolver passes, lane by lane: Plan / unit_info (last wave cut into pieces),
 // chain pass into per-chunk hit rows, exclusive prefix, the decode pass's binary search for a packet's chunk,
-// one block of the output per unit + directory entry.  `order` permutes the order in which units reserve their
-// block (on the GPU that is the order they finish in).  Mirrors btle_rx_persistent_kernel; keep in step with it.
-extern "C" long emul_rx_batch_units(const int8_t *iq, long n_streams, long stride, long n_int8, const btle_stream_cfg *cfgs,
-                                    int grid, int reverse_units_and_flags, btle_pkt_rec *out, long cap, uint32_t *dir /*2 per unit*/,
-                                    long dir_cap, long *n_units_out) {
+// one block of the output per (cfg, unit) + directory entry.  cfg i decodes capture cfg_capture[i] (non-decreasing, at most
+// kMaxCfgsPerCapture per capture), or capture i when cfg_capture is NULL (then n_cfgs == n_captures).  The kernel is
+// launch_rx's choice:
+//   - a list that maps cfg i to capture i for every capture: btle_rx_persistent_kernel<1>, prefilter_any on the cfg's
+//     StreamParams, directory entry = unit;
+//   - any other list: <kMaxCfgsPerCapture>.  The plan runs over capture GROUPS (the captures some cfg names); per unit the
+//     phase words are built once, the candidate words are the union of the group's cfgs' prefilters (prefilter_union on
+//     make_tapset), and the resolver passes run once per cfg, directory entry cfg * (units per group) + the unit's index in
+//     its group.
+// flags: bit 0 permutes the order in which units reserve their block (on the GPU that is the order they finish in),
+// bit 1 takes the candidate walk for every chunk.  Records carry stream = cfg index.  Returns the number of records (one
+// block per (cfg, unit), stored in reservation order), or -1 for an invalid cfg_capture, an uneven plan under
+// <kMaxCfgsPerCapture> or a directory that is too small.  dir: 2 words per entry; *n_dir_out = entries written.
+// Mirrors btle_rx_persistent_kernel; keep in step with it.
+extern "C" long emul_rx_units(const int8_t *iq, long n_captures, long stride, long n_int8, const btle_stream_cfg *cfgs,
+                              const int32_t *cfg_capture, long n_cfgs, int grid, int flags, btle_pkt_rec *out, long cap, uint32_t *dir,
+                              long dir_cap, long *n_dir_out) {
+  const int reverse_units = flags & 1, force_walk = (flags >> 1) & 1;
+  *n_dir_out = 0;
+  std::vector<int> caps, cfg0, ncfg;                       // per capture group: its capture, first cfg, number of cfgs
+  for (long i = 0; i < n_cfgs; ++i) {
+    const int c = cfg_capture ? cfg_capture[i] : (int)i;
+    if (c < 0 || c >= n_captures || (i && c < caps.back())) return -1;
+    if (!i || c != caps.back()) { caps.push_back(c); cfg0.push_back((int)i); ncfg.push_back(0); }
+    if (++ncfg.back() > kMaxCfgsPerCapture) return -1;
+  }
+  const bool single = (long)caps.size() == n_cfgs && n_cfgs == n_captures;
   const long nchunks = n_int8 / kChunkInt8;
-  const int reverse_units = reverse_units_and_flags & 1, force_walk = (reverse_units_and_flags >> 1) & 1;   // bit 1: candidate walk for every chunk
-  *n_units_out = 0;
-  if (nchunks == 0 || n_streams == 0) return 0;
-  const Plan pl = make_plan(n_streams, nchunks, grid);
-  *n_units_out = pl.total_units;
-  if (pl.total_units > dir_cap) return -1;
+  if (nchunks == 0 || caps.empty()) return 0;
+  const Plan pl = make_plan((long long)caps.size(), nchunks, grid);
+  const int per_group = pl.big_units ? pl.spans_per_stream : pl.spans_per_stream << pl.piece_shift;
+  if (!single && (pl.tail_units || (pl.big_units && pl.big_units != pl.total_units) || per_group * (long)caps.size() != pl.total_units)) return -1;
+  const long n_dir = single ? pl.total_units : (long)per_group * n_cfgs;
+  if (n_dir > dir_cap) return -1;
+  *n_dir_out = n_dir;
+  std::vector<StreamParams> sps(n_cfgs);
+  for (long i = 0; i < n_cfgs; ++i) {
+    uint8_t wrow[48];
+    make_whiten_row(cfgs[i].channel, wrow);
+    uint32_t ww[12];
+    memcpy(ww, wrow, 48);
+    make_params(cfgs[i], ww, sps[i]);
+  }
   uint32_t crc4[1024];
   make_crc4(crc4);
+  constexpr int kHitCap = BTLE_MAX_PKTS_PER_CHUNK + kRejectedInHitRow + 1;    // the kernel's hit row; more hits are left to step 4
   long count = 0;
   for (int uu = 0; uu < pl.total_units; ++uu) {
     const int u = reverse_units ? pl.total_units - 1 - uu : uu;
     const UnitInfo ui = unit_info(u, pl);
-    const btle_stream_cfg &cfg = cfgs[ui.stream];
-    uint8_t wrow[48];
-    make_whiten_row(cfg.channel, wrow);
-    uint32_t ww[12];
-    memcpy(ww, wrow, 48);
-    StreamParams sp;
-    make_params(cfg, ww, sp);
-    const int8_t *cap_base = iq + (long)ui.stream * stride;
+    const int vs = ui.stream;
+    const int8_t *cap_base = iq + (long)caps[vs] * stride;
     auto word_at = [&](long byte_off) -> uint32_t {
       uint32_t w = 0;
       for (int b = 0; b < 4; ++b) { long a = byte_off + b; if (a >= 0 && a < n_int8) w |= (uint32_t)(uint8_t)cap_base[a] << (8 * b); }
       return w;
     };
+    // dense pass, once per unit whatever the number of cfgs
     const int G = ui.groups;
     std::vector<uint32_t> pd(4 * (size_t)(G + 1) + 4, 0u), cand((size_t)G + 4, 0u), flagw(2 * (size_t)kSpanChunks + 2, 0u);
     const long base_off = (long)ui.chunk0 * kChunkInt8;
@@ -147,74 +174,97 @@ extern "C" long emul_rx_batch_units(const int8_t *iq, long n_streams, long strid
       dbits_group_dense(word, acc);
       for (int ph = 0; ph < 4; ++ph) pd[4 * g + ph] = acc[ph];
     }
+    TapSet taps[kMaxCfgsPerCapture];
+    for (int j = 0; !single && j < ncfg[vs]; ++j) taps[j] = make_tapset(sps[cfg0[vs] + j]);
     for (int g = 0; g < kGroupsPerChunk * ui.nch; ++g) {
-      const uint32_t a = prefilter_any(&pd[4 * (size_t)g], &pd[4 * (size_t)(g + 1)], sp);
+      const uint32_t *lo = &pd[4 * (size_t)g], *hi = &pd[4 * (size_t)(g + 1)];
+      const uint32_t a = single ? prefilter_any(lo, hi, sps[cfg0[vs]]) : prefilter_union(lo, hi, taps, ncfg[vs]);
       cand[g] = a;
       if (a) flagw[g >> 5] |= 1u << (g & 31);
     }
-    // exact hits per flag word (lane = flag word), then the chain pass (lane = chunk) on the lists — or, for degenerate
-    // masks with more matches than a list holds, on the candidate words
-    uint16_t xh[2 * kSpanChunks][kExactCap + 1];
-    for (int t = 0; t < 2 * ui.nch; ++t) xh[t][kExactCap] = (uint16_t)enumerate_exact_hits(pd.data(), cand.data(), flagw[t], t, sp, xh[t]);
-    constexpr int kHitCap = BTLE_MAX_PKTS_PER_CHUNK + kRejectedInHitRow + 1;    // the kernel's hit row; more hits are left to step 4
-    uint16_t hit[kSpanChunks][kHitCap];
-    int mine[32] = {0};
-    for (int lane = 0; lane < ui.nch; ++lane) {
-      struct Note {
-        uint16_t *row;
-        void operator()(int i, int n0, bool rej) { if (i < kHitCap) row[i] = (uint16_t)((n0 + 124) | (rej ? 0x8000 : 0)); }
-      } note{hit[lane]};
-      const uint32_t *pdc = &pd[4 * (size_t)(kGroupsPerChunk * lane)];
-      const int c0 = xh[2 * lane][kExactCap], c1 = xh[2 * lane + 1][kExactCap];
-      if (c0 > kExactCap || c1 > kExactCap || force_walk)
-        mine[lane] = chain_chunk(pdc, &cand[(size_t)kGroupsPerChunk * lane], &flagw[2 * (size_t)lane], sp, note);
-      else
-        mine[lane] = chain_chunk_lists(pdc, xh[2 * lane], c0, xh[2 * lane + 1], c1, sp, note);
-    }
-    uint16_t pre[kSpanChunks + 2];
-    int incl = 0;
-    for (int lane = 0; lane <= kSpanChunks; ++lane) { pre[lane] = (uint16_t)incl; incl += mine[lane]; }
-    const int total = incl;
-    const long base = count;
-    count += total;
-    dir[2 * u] = (uint32_t)base; dir[2 * u + 1] = (uint32_t)total;
-    for (int j = 0; j < total; ++j) {
-      int c = 0;
-      for (int step = kSpanChunks / 2; step >= 1; step >>= 1)
-        if ((int)pre[c + step] <= j) c += step;
-      if (j - (int)pre[c] >= kHitCap) continue;           // behind the chunk's row: step 4
-      const int h = (int)hit[c][j - (int)pre[c]];
-      const bool rej = (h & 0x8000) != 0;
-      const int n0 = (h & 0x7FFF) - 124;
-      uint32_t words[11];
-      int nbytes, crc_bad;
-      decode_packet(&pd[4 * (size_t)(kGroupsPerChunk * c)], sp, crc4, n0, rej, words, nbytes, crc_bad);
-      if (base + j < cap) {
-        HostEmit e{out + base + j, 1, 0, ui.stream, ui.chunk0 + c, &sp, cap_base, n_int8, (long)(ui.chunk0 + c) * kChunkInt8};
-        e(n0, nbytes, crc_bad, words, rej);
+    // resolver passes, once per cfg
+    for (int jc = 0; jc < ncfg[vs]; ++jc) {
+      const int j = cfg0[vs] + jc;
+      const StreamParams &sp = sps[j];
+      // exact hits per flag word (lane = flag word), then the chain pass (lane = chunk) on the lists — or, for degenerate
+      // masks with more matches than a list holds, on the candidate words
+      uint16_t xh[2 * kSpanChunks][kExactCap + 1];
+      for (int t = 0; t < 2 * ui.nch; ++t) xh[t][kExactCap] = (uint16_t)enumerate_exact_hits(pd.data(), cand.data(), flagw[t], t, sp, xh[t]);
+      uint16_t hit[kSpanChunks][kHitCap];
+      int mine[32] = {0};
+      for (int lane = 0; lane < ui.nch; ++lane) {
+        struct Note {
+          uint16_t *row;
+          void operator()(int i, int n0, bool rej) { if (i < kHitCap) row[i] = (uint16_t)((n0 + 124) | (rej ? 0x8000 : 0)); }
+        } note{hit[lane]};
+        const uint32_t *pdc = &pd[4 * (size_t)(kGroupsPerChunk * lane)];
+        const int c0 = xh[2 * lane][kExactCap], c1 = xh[2 * lane + 1][kExactCap];
+        if (c0 > kExactCap || c1 > kExactCap || force_walk)
+          mine[lane] = chain_chunk(pdc, &cand[(size_t)kGroupsPerChunk * lane], &flagw[2 * (size_t)lane], sp, note);
+        else
+          mine[lane] = chain_chunk_lists(pdc, xh[2 * lane], c0, xh[2 * lane + 1], c1, sp, note);
       }
-    }
-    // step 4: a chunk with more hits than its row holds runs its chain again and stores hits kHitCap.. itself
-    for (int lane = 0; lane < ui.nch; ++lane) {
-      if (!sp.report_rejected || mine[lane] <= kHitCap) continue;
-      const uint32_t *pdc = &pd[4 * (size_t)(kGroupsPerChunk * lane)];
-      const long first = base + pre[lane];
-      auto late = [&](int i, int n0, bool rej) {
-        if (i < kHitCap || first + i >= cap) return;
+      uint16_t pre[kSpanChunks + 2];
+      int incl = 0;
+      for (int lane = 0; lane <= kSpanChunks; ++lane) { pre[lane] = (uint16_t)incl; incl += mine[lane]; }
+      const int total = incl;
+      const long base = count;
+      count += total;
+      const long d = single ? u : (long)j * per_group + (u - vs * per_group);
+      dir[2 * d] = (uint32_t)base; dir[2 * d + 1] = (uint32_t)total;
+      for (int k = 0; k < total; ++k) {
+        int c = 0;
+        for (int step = kSpanChunks / 2; step >= 1; step >>= 1)
+          if ((int)pre[c + step] <= k) c += step;
+        if (k - (int)pre[c] >= kHitCap) continue;           // behind the chunk's row: step 4
+        const int h = (int)hit[c][k - (int)pre[c]];
+        const bool rej = (h & 0x8000) != 0;
+        const int n0 = (h & 0x7FFF) - 124;
         uint32_t words[11];
         int nbytes, crc_bad;
-        decode_packet(pdc, sp, crc4, n0, rej, words, nbytes, crc_bad);
-        HostEmit e{out + first + i, 1, 0, ui.stream, ui.chunk0 + lane, &sp, cap_base, n_int8, (long)(ui.chunk0 + lane) * kChunkInt8};
-        e(n0, nbytes, crc_bad, words, rej);
-      };
-      const int c0 = xh[2 * lane][kExactCap], c1 = xh[2 * lane + 1][kExactCap];
-      if (c0 > kExactCap || c1 > kExactCap || force_walk)
-        chain_chunk(pdc, &cand[(size_t)kGroupsPerChunk * lane], &flagw[2 * (size_t)lane], sp, late);
-      else
-        chain_chunk_lists(pdc, xh[2 * lane], c0, xh[2 * lane + 1], c1, sp, late);
+        decode_packet(&pd[4 * (size_t)(kGroupsPerChunk * c)], sp, crc4, n0, rej, words, nbytes, crc_bad);
+        if (base + k < cap) {
+          HostEmit e{out + base + k, 1, 0, j, ui.chunk0 + c, &sp, cap_base, n_int8, (long)(ui.chunk0 + c) * kChunkInt8};
+          e(n0, nbytes, crc_bad, words, rej);
+        }
+      }
+      // step 4: a chunk with more hits than its row holds runs its chain again and stores hits kHitCap.. itself
+      for (int lane = 0; lane < ui.nch; ++lane) {
+        if (!sp.report_rejected || mine[lane] <= kHitCap) continue;
+        const uint32_t *pdc = &pd[4 * (size_t)(kGroupsPerChunk * lane)];
+        const long first = base + pre[lane];
+        auto late = [&](int i, int n0, bool rej) {
+          if (i < kHitCap || first + i >= cap) return;
+          uint32_t words[11];
+          int nbytes, crc_bad;
+          decode_packet(pdc, sp, crc4, n0, rej, words, nbytes, crc_bad);
+          HostEmit e{out + first + i, 1, 0, j, ui.chunk0 + lane, &sp, cap_base, n_int8, (long)(ui.chunk0 + lane) * kChunkInt8};
+          e(n0, nbytes, crc_bad, words, rej);
+        };
+        const int c0 = xh[2 * lane][kExactCap], c1 = xh[2 * lane + 1][kExactCap];
+        if (c0 > kExactCap || c1 > kExactCap || force_walk)
+          chain_chunk(pdc, &cand[(size_t)kGroupsPerChunk * lane], &flagw[2 * (size_t)lane], sp, late);
+        else
+          chain_chunk_lists(pdc, xh[2 * lane], c0, xh[2 * lane + 1], c1, sp, late);
+      }
     }
   }
   return count;
+}
+
+// prefilter_union of one cfg against prefilter_any of its StreamParams, for every (lo, hi) pair of the given words
+extern "C" long emul_check_tapset(const btle_stream_cfg *cfg, const uint32_t *words, long n) {
+  uint8_t wrow[48];
+  make_whiten_row(cfg->channel, wrow);
+  uint32_t ww[12];
+  memcpy(ww, wrow, 48);
+  StreamParams sp;
+  make_params(*cfg, ww, sp);
+  const TapSet ts = make_tapset(sp);
+  long bad = 0;
+  for (long i = 0; i + 8 <= n; i += 4)
+    if (prefilter_union(words + i, words + i + 4, &ts, 1) != prefilter_any(words + i, words + i + 4, sp)) ++bad;
+  return bad;
 }
 
 extern "C" uint32_t emul_crc24_words(const uint8_t *bytes, int n, uint32_t init) {

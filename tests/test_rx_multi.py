@@ -1,8 +1,5 @@
 """Several cfgs per capture (btle_b200_rx_multi) without a GPU: the kernel's multi-cfg unit path on the CPU emulator
-(tests/emul/btle_multi_emul.cpp) against the oracle run once per cfg, and hop.decode_connections() on an oracle backend."""
-import ctypes
-import os
-import subprocess
+(tests/emul/btle_emul.cpp) against the oracle run once per cfg, and hop.decode_connections() on an oracle backend."""
 import time
 
 import numpy as np
@@ -10,51 +7,13 @@ import pytest
 import torch
 
 import discover_ref as R
+import emul
 import orc
 from btle_b200 import synth
-from btle_b200._native import CFG_DTYPE, MAX_CFGS_PER_CAPTURE, REC_DTYPE
+from btle_b200._native import MAX_CFGS_PER_CAPTURE, REC_DTYPE
 from btle_b200.hop import decode_connections, record_time
 from btle_b200.rx import make_cfgs
 from test_hop import _place
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-EMUL_SRC = os.path.join(HERE, "emul", "btle_multi_emul.cpp")
-EMUL_SO = os.path.join(HERE, "emul", "libbtle_multi_emul.so")      # built by __graft_entry__.build()
-EMUL_DEPS = [EMUL_SRC, os.path.join(ROOT, "btle_b200", "csrc", "btle_core.cuh"), os.path.join(ROOT, "btle_b200", "csrc", "btle_params.h"),
-             os.path.join(ROOT, "include", "btle_b200.h")]
-_emul_lib = None
-
-
-def _emul():
-    global _emul_lib
-    if _emul_lib is None:
-        if (not os.path.exists(EMUL_SO)) or any(os.path.getmtime(EMUL_SO) < os.path.getmtime(d) for d in EMUL_DEPS):
-            subprocess.run(["g++", "-O2", "-fPIC", "-shared", "-std=c++17", "-x", "c++", "-o", EMUL_SO, EMUL_SRC], check=True)
-        L = _emul_lib = ctypes.CDLL(EMUL_SO)
-        vp, lg = ctypes.c_void_p, ctypes.c_long
-        L.emul_rx_multi_units.restype = lg
-        L.emul_rx_multi_units.argtypes = [vp, lg, lg, lg, vp, vp, lg, ctypes.c_int, vp, lg, vp, lg, ctypes.POINTER(lg)]
-        L.emul_check_tapset.restype = lg
-        L.emul_check_tapset.argtypes = [vp, vp, lg]
-    return _emul_lib
-
-
-def emul_rx_multi(iq2d, cfgs, capture, grid=132):
-    """The multi-cfg kernel path on the CPU, records gathered through the unit directory (reference order)."""
-    iq2d = np.ascontiguousarray(iq2d, dtype=np.int8)
-    ns, n = iq2d.shape
-    cfgs = np.ascontiguousarray(cfgs, dtype=CFG_DTYPE)
-    cc = np.ascontiguousarray(capture, dtype=np.int32)
-    cap = cfgs.size * (n // 16384) * 123 + 8
-    out = np.zeros(cap, dtype=REC_DTYPE)
-    dir_cap = cfgs.size * ((n // 16384 + 15) // 16 * 16 + 16)
-    d = np.zeros((dir_cap, 2), dtype=np.uint32)
-    nd = ctypes.c_long(0)
-    cnt = _emul().emul_rx_multi_units(iq2d.ctypes.data, ns, n, n, cfgs.ctypes.data, cc.ctypes.data, cfgs.size, grid, out.ctypes.data, cap,
-                                      d.ctypes.data, dir_cap, ctypes.byref(nd))
-    assert 0 <= cnt <= cap
-    return np.concatenate([out[b:b + c] for b, c in d[:nd.value]]) if nd.value else out[:0]
 
 
 def oracle_multi(iq2d, cfgs, capture):
@@ -105,7 +64,8 @@ def multi_cases():
         c = make_cfgs(len(cfgs))
         for j, v in enumerate(cfgs):
             c[j] = v
-        cases.append((f"K{K}", iq, c, np.array(cap, dtype=np.int32)))
+        # K = 1: one more capture, which no cfg reads, keeps the list from mapping cfg j to capture j (the single-cfg kernel)
+        cases.append((f"K{K}", iq if K > 1 else np.concatenate([iq, iq[:1]]), c, np.array(cap, dtype=np.int32)))
     # one AA twice with different CRC inits (a discovery noise group), different channels on one capture
     c = make_cfgs(4, channel=[5, 5, 6, 5], access_addr=[0x60850A1B, 0x60850A1B, 0x60850A1B, 0x50850A1C],
                   crc_init=[0x227BA7 ^ 0x0A1B, 0x123456, 0x227BA7 ^ 0x0A1B, 0x227BA7 ^ 0x0A1C], rssi=[1, 0, 1, 2])
@@ -128,7 +88,7 @@ def test_multi_cfg_unit_path_equals_oracle_per_cfg(case):
     _, iq, cfgs, capture = case
     exp = oracle_multi(iq, cfgs, capture)
     for grid in (132, 7):                                      # whole spans, and pieces of them
-        got = emul_rx_multi(iq, cfgs, capture, grid=grid)
+        got = emul.rx_multi(iq, cfgs, capture, grid=grid)
         assert got.tobytes() == exp.tobytes(), (grid, len(got), len(exp))
     assert len(exp) > 0
 
@@ -143,7 +103,7 @@ def test_multi_cfg_unit_path_fuzz_equals_oracle_per_cfg():
         iq, cfgs, capture = draw(rng, max_captures=12, max_chunks=16)
         exp = oracle_multi(iq, cfgs, capture)
         for grid in (132, int(rng.integers(1, 300))):
-            got = emul_rx_multi(iq, cfgs, capture, grid=grid)
+            got = emul.rx_multi(iq, cfgs, capture, grid=grid)
             assert got.tobytes() == exp.tobytes(), (n, grid, iq.shape, cfgs.tolist(), capture.tolist(), len(got), len(exp))
         n, recs = n + 1, recs + len(exp)
     assert recs > 1000
@@ -156,20 +116,13 @@ def test_tapset_prefilter_equals_prefilter_any():
     for aa, mask in [(0x8E89BED6, 0xFFFFFFFF), (0x60850A1B, 0), (0x0000000F, 0xFFFFFFFF), (0xFFFFFFFF, 0x0000F00F), (0x12345679, 0x00000003)]:
         cfg = make_cfgs(1, access_addr=aa, access_mask=mask)
         for w in (words, sparse):
-            assert _emul().emul_check_tapset(cfg.ctypes.data, w.ctypes.data, w.size) == 0, (hex(aa), hex(mask))
+            assert emul.check_tapset(cfg, w) == 0, (hex(aa), hex(mask))
 
 
 def test_bad_cfg_capture_is_refused():
     iq = np.zeros((2, 16384), dtype=np.int8)
-    L = _emul()
     for cc in ([1, 0], [0, 2], [-1, 0], [0] * (MAX_CFGS_PER_CAPTURE + 1)):
-        cfgs = make_cfgs(len(cc))
-        cc = np.array(cc, dtype=np.int32)
-        out = np.zeros(16, dtype=REC_DTYPE)
-        d = np.zeros((64, 2), dtype=np.uint32)
-        nd = ctypes.c_long(0)
-        assert L.emul_rx_multi_units(iq.ctypes.data, 2, 16384, 16384, cfgs.ctypes.data, cc.ctypes.data, cc.size, 132, out.ctypes.data, 16,
-                                     d.ctypes.data, 64, ctypes.byref(nd)) == -1
+        assert emul.rx_units(iq, make_cfgs(len(cc)), cc)[0] == -1
 
 
 # ---- decode_connections ------------------------------------------------------------------------------------------------
