@@ -11,14 +11,14 @@
 // Differences, on purpose:
 //   * IQ source instead of an SDR (without one the program exits with status 1, the reference's "board failure"
 //     code, :2586):
-//       -i/--iq-file FILE        raw interleaved int8 (what rx_callback writes, btle_rx.c:531-540), '-' = stdin.  Read in
-//                                64 MiB segments straight into page-locked memory and decoded while the next segment is
-//                                being read (btle_b200_stream_*): the capture may be larger than host RAM or HBM.
-//       -i FILE:CH[:AA[:CRCINIT[:HZ]]]  (repeatable) several time-aligned captures (files or FIFOs, '-' for one of them),
-//                                each with its own channel / access address / CRC init.  Streamed through one session
-//                                (btle_b200_streams_*): poll() across the inputs, each segment set decoded in one
-//                                batched launch while the next one is read; packets are printed in time order, up to
-//                                the end of the shortest capture.
+//       -i/--iq-file FILE[:CH[:AA[:CRCINIT[:HZ]]]]  (repeatable) raw interleaved int8 (what rx_callback writes,
+//                                btle_rx.c:531-540), files or FIFOs, '-' = stdin for one of them; several -i are
+//                                time-aligned captures, each with its own channel / access address / CRC init.  One session
+//                                (btle_b200_streams_*) serves any number of -i: poll() across the inputs, read() into
+//                                page-locked segments, each segment set decoded in one batched launch while the next is
+//                                read (a capture may be larger than host RAM or HBM), up to the shortest capture's end.
+//                                Packets are printed in time order, except that each capture's keep their own order
+//                                (print_in_order): one capture's output is the reference's processing order.
 //       --iq-dir DIR             DIR/ch00.bin .. DIR/ch39.bin, time-aligned captures of the BLE channels (missing
 //                                files are skipped).  Without -o: like 40 -i entries.  With -o: see below.
 //       --iq-txt FILE / --iq-sc16 FILE   text format of save_phy_sample (btle_rx.c:896-915) / int16 bladeRF samples.
@@ -50,6 +50,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <set>
 #include <string>
 #include <vector>
@@ -283,6 +284,15 @@ bool load_raw(const char *name, std::vector<int8_t> &iq) {
   return true;
 }
 
+// ---- owners: what a mode opens is closed on every return -------------------------------------------------------------
+struct CtxClose { void operator()(btle_b200_ctx *c) const { btle_b200_destroy(c); } };
+struct StreamsClose { void operator()(btle_b200_streams *s) const { btle_b200_streams_close(s); } };
+struct FileClose { void operator()(FILE *f) const { fclose(f); } };
+struct Inputs {                                       // the session's input descriptors; 0 (stdin) is left open
+  std::vector<int> fds;
+  ~Inputs() { for (int fd : fds) if (fd > 0) close(fd); }
+};
+
 // ---- sinks ----------------------------------------------------------------------------------------
 void put_be32(FILE *f, uint32_t v) { const uint8_t b[4] = {(uint8_t)(v >> 24), (uint8_t)(v >> 16), (uint8_t)(v >> 8), (uint8_t)v}; fwrite(b, 1, 4, f); }
 
@@ -395,7 +405,7 @@ int rssi_from_mag(unsigned mag_sum) {                 // btle_rx.c:2244-2249
 // ---- what receiver() does with a counted packet after crc_check(): filters, sinks (btle_rx.c:2318-2389) -----------
 struct Sinks {
   const Options &o;
-  FILE *pcap = nullptr;
+  std::unique_ptr<FILE, FileClose> pcap;
   int pkt_count = 0;
   double t_prev = 0.0;
   explicit Sinks(const Options &opt) : o(opt) {}
@@ -438,7 +448,7 @@ struct Sinks {
       uint8_t a[6];
       const bool has_a = adv_a(b + 2, type, a);
       if (o.filter_adva_set && has_a && memcmp(a, o.filter_adva, 6)) return;    // :2345-2348
-      if (pcap) pcap_write(pcap, t, b, plen + 2, ch, aa, rssi);                 // :2361-2362
+      if (pcap) pcap_write(pcap.get(), t, b, plen + 2, ch, aa, rssi);           // :2361-2362
       if (!o.quiet) {
         printf("%07dus Pkt%03d Ch%d AA:%08x ", time_diff, pkt_count, ch, aa);
         printf("ADV_PDU_t%d:%s T%d R%d PloadL%d ", type, ADV_NAME[type], tx, rx, plen);
@@ -461,7 +471,7 @@ struct Sinks {
       const int op = btle_b200_parse_ll_pdu_payload_byte(b + 2, plen, llid, &parsed);
       if (op < 0) return;                                                       // :2350-2353
       if (o.filter_adva_set) return;                                            // :2355-2357
-      if (pcap) pcap_write(pcap, t, b, plen + 2, ch, aa, rssi);
+      if (pcap) pcap_write(pcap.get(), t, b, plen + 2, ch, aa, rssi);
       if (!o.quiet) {
         printf("%07dus Pkt%03d Ch%d AA:%08x ", time_diff, pkt_count, ch, aa);
         printf("LL_PDU_t%d:%s NESN%d SN%d MD%d PloadL%d ", llid, LL_NAME[llid], nesn, sn, md, plen);
@@ -481,6 +491,32 @@ struct Sinks {
 };
 
 double rec_time(const btle_pkt_rec &r) { return ((double)r.chunk * 8192.0 + r.n0) / 4.0e6; }   // sample time of the access address
+
+// Prints a session's pending records in sample-time order (chunk × 8192 + n0, ties to the lower stream) while that lies
+// before `safe`, except that each stream's records keep the order the session handed them out in, chunk by chunk.  That
+// is the reference's processing order, in which a hit at n0 < 0 in chunk k+1 can start before a late packet of chunk k
+// (Sinks::packet); so a record sorts at the latest time among its stream's records up to it.  Returns how many it printed.
+size_t print_in_order(std::vector<btle_pkt_rec> &pending, Sinks &sinks, long long safe) {
+  const auto before_safe = [&](const btle_pkt_rec &r) { return (long long)r.chunk * 8192 + r.n0 < safe; };
+  if (std::none_of(pending.begin(), pending.end(), before_safe)) return 0;   // a sort time is never before the record's own
+  std::stable_sort(pending.begin(), pending.end(), [](const btle_pkt_rec &a, const btle_pkt_rec &b) {
+    return a.stream != b.stream ? a.stream < b.stream : a.chunk < b.chunk;
+  });
+  std::vector<long long> t(pending.size());
+  std::vector<size_t> idx(pending.size());
+  for (size_t i = 0; i < pending.size(); ++i) {
+    const long long own = (long long)pending[i].chunk * 8192 + pending[i].n0;
+    t[i] = i && pending[i - 1].stream == pending[i].stream ? std::max(own, t[i - 1]) : own;
+    idx[i] = i;
+  }
+  std::stable_sort(idx.begin(), idx.end(), [&](size_t a, size_t b) { return t[a] != t[b] ? t[a] < t[b] : pending[a].stream < pending[b].stream; });
+  size_t n = 0;
+  for (; n < idx.size() && t[idx[n]] < safe; ++n) sinks.packet(pending[idx[n]], rec_time(pending[idx[n]]));
+  std::vector<btle_pkt_rec> rest;
+  for (size_t k = n; k < idx.size(); ++k) rest.push_back(pending[idx[k]]);
+  pending.swap(rest);
+  return n;
+}
 
 volatile sig_atomic_t g_stop = 0;
 void on_sigint(int) { g_stop = 1; }                                             // btle_rx.c:100-104
@@ -540,6 +576,11 @@ int cfg_flags(const Options &o) {
   return (o.rssi ? BTLE_CFG_RSSI : 0) | (o.verbose ? BTLE_CFG_REPORT_REJECTED : 0) | (o.recover ? BTLE_CFG_RECOVER : 0);
 }
 
+int fail(btle_b200_ctx *ctx, int rc, const char *what) {
+  printf("%s: %s (%s)\n", what, btle_b200_strerror(rc), btle_b200_last_error(ctx));
+  return 1;
+}
+
 // rx_batch with a capacity that is grown once if the library asks; offset_hz: one per capture, or NULL (no correction)
 int rx_batch_grow(btle_b200_ctx *ctx, const int8_t *iq, size_t ns, size_t stride, size_t n, const btle_stream_cfg *cfgs,
                   std::vector<btle_pkt_rec> &recs, const float *offset_hz = nullptr) {
@@ -556,25 +597,21 @@ int rx_batch_grow(btle_b200_ctx *ctx, const int8_t *iq, size_t ns, size_t stride
 }
 
 // --offset auto: the median of btle_b200_rec_offset over the CRC-ok counted packets of a first pass without correction
-// (not raw, no flags); 0 when no packet passes.  *n_ok = the packets it took.
-int estimate_offset(btle_b200_ctx *ctx, const std::vector<int8_t> &iq, btle_stream_cfg cfg, float *hz, size_t *n_ok) {
+// (not raw, no flags), 0 when no packet passes; printed on stderr under `name`.  Returns the exit status.
+int estimate_offset(btle_b200_ctx *ctx, const std::vector<int8_t> &iq, btle_stream_cfg cfg, const char *name, float *hz) {
   cfg.raw = 0;
   cfg.rssi = 0;
   std::vector<btle_pkt_rec> recs;
-  *hz = 0.0f;
-  *n_ok = 0;
   int rc = rx_batch_grow(ctx, iq.data(), 1, iq.size(), iq.size(), &cfg, recs);
-  if (rc) return rc;
   recs.erase(std::remove_if(recs.begin(), recs.end(), [](const btle_pkt_rec &r) { return r.crc_bad || (r.flags & BTLE_REC_REJECTED); }),
              recs.end());
-  if (recs.empty()) return 0;
   std::vector<float> e(recs.size());
-  rc = btle_b200_rec_offset(ctx, iq.data(), 1, iq.size(), iq.size(), recs.data(), recs.size(), e.data());
-  if (rc) return rc;
+  if (!rc && !e.empty()) rc = btle_b200_rec_offset(ctx, iq.data(), 1, iq.size(), iq.size(), recs.data(), recs.size(), e.data());
+  if (rc) return fail(ctx, rc, "--offset auto");
   std::sort(e.begin(), e.end());
   const size_t m = e.size() / 2;
-  *hz = e.size() & 1 ? e[m] : 0.5f * (e[m - 1] + e[m]);
-  *n_ok = e.size();
+  *hz = e.empty() ? 0.0f : e.size() & 1 ? e[m] : 0.5f * (e[m - 1] + e[m]);
+  fprintf(stderr, "offset estimate %s: %.1f Hz (%zu CRC-ok packets)\n", name, *hz, e.size());
   return 0;
 }
 
@@ -748,6 +785,279 @@ struct ConnMonitor {
   }
 };
 
+// The raw captures: every -i, then DIR/chNN.bin of --iq-dir, with their carrier offsets (--offset auto: estimated here
+// from a first pass).  *use_off: some capture has a correction.  Returns the exit status.
+int load_captures(btle_b200_ctx *ctx, const Options &o, std::vector<Capture> &caps, bool *use_off) {
+  for (const std::string &f : o.iq_files) caps.push_back(parse_capture(f, o));
+  if (o.iq_dir) {
+    for (int ch = 0; ch < 40; ++ch) {
+      char name[512];
+      snprintf(name, sizeof name, "%s/ch%02d.bin", o.iq_dir, ch);
+      if (access(name, R_OK) != 0) continue;
+      const bool adv = ch >= 37;
+      caps.push_back(Capture{name, ch, adv ? 0x8E89BED6u : o.aa, adv ? 0x555555u : o.crc_init, o.offset_hz, false});
+    }
+    if (caps.empty()) { printf("no chNN.bin capture found in %s\n", o.iq_dir); return 1; }
+  }
+  for (const Capture &c : caps)
+    if (c.chan < 0 || c.chan > 39) { printf("channel number must be within 0~%d!\n", 39); return 1; }
+  if (o.connections && caps.size() != 40) { printf("--connections needs all 40 chNN.bin captures in %s\n", o.iq_dir); return 1; }
+  // carrier-offset correction: --offset HZ for every capture, FILE:CH:AA:CRCINIT:HZ for one, --offset auto from a first pass
+  *use_off = o.offset_set;
+  for (const Capture &c : caps) *use_off |= c.own_hz;
+  if (!o.offset_auto) return 0;
+  for (Capture &c : caps) {
+    if (c.own_hz) continue;
+    struct stat sb;
+    if (c.file == "-" || stat(c.file.c_str(), &sb) != 0 || !S_ISREG(sb.st_mode)) {
+      printf("--offset auto needs regular files (%s is not one)\n", c.file.c_str());
+      return 1;
+    }
+    std::vector<int8_t> iq;
+    if (!load_raw(c.file.c_str(), iq)) return 1;
+    if (estimate_offset(ctx, iq, btle_stream_cfg{c.chan, c.aa, o.mask, c.crc_init, 0, 0}, c.file.c_str(), &c.hz)) return 1;
+  }
+  return 0;
+}
+
+// Each mode returns the exit status and, when it is 0, the sample time at which the input ended (*t_end).
+
+// ---- --iq-bin16: 8 samples per symbol, the Python / Verilog model's receiver over the capture ------------------------------
+int run_sps8(btle_b200_ctx *ctx, const Options &o, Sinks &sinks, double *t_end) {
+  std::vector<int8_t> raw;
+  if (!load_raw(o.iq_bin16, raw)) return 1;
+  const size_t n_samples = raw.size() / 4;
+  std::vector<btle_sps8_rec> recs(n_samples / 576 + 16);
+  size_t n = 0;
+  const int rc = btle_b200_rx_sps8(ctx, reinterpret_cast<const int16_t *>(raw.data()), n_samples, o.chan, o.crc_init, o.aa, recs.data(), recs.size(), &n);
+  if (rc) return fail(ctx, rc, "btle_b200_rx_sps8");
+  const bool adv = (o.chan == 37 || o.chan == 38 || o.chan == 39);
+  for (size_t i = 0; i < n && !g_stop; ++i) {
+    const btle_model_rx_rec &m = recs[i].rx;
+    if (!m.found || m.n_pdu_bits < 16) continue;         // no header decoded: nothing the sinks could show
+    btle_pkt_rec r;
+    memset(&r, 0, sizeof r);
+    const int have = m.n_pdu_bits / 8;                    // header + payload bytes that were decoded (CRC clamp, btlelib.py:488-490)
+    memcpy(r.bytes, m.pdu, (size_t)std::min(have, 39));
+    const int plen = std::min(have - 2, (int)(r.bytes[1] & (adv ? 0x3F : 0x1F)));
+    r.bytes[1] = (uint8_t)((r.bytes[1] & (adv ? 0xC0 : 0xE0)) | plen);
+    r.channel = (uint8_t)o.chan; r.access_addr = o.aa; r.flags = adv ? 2 : 0;
+    r.crc_bad = m.crc_ok ? 0 : 1;
+    r.n_bytes = (uint8_t)(plen + 5);
+    sinks.packet(r, (double)recs[i].sample / 8.0e6);
+  }
+  *t_end = (double)n_samples / 8.0e6;
+  return 0;
+}
+
+// ---- -o with --iq-dir: connection following over per-channel captures -------------------------------------------------
+int run_hop(btle_b200_ctx *ctx, const Options &o, const std::vector<Capture> &caps, bool use_off, Sinks &sinks, double *t_end) {
+  std::vector<std::vector<int8_t>> iq(40);
+  std::vector<float> hz_of(40, 0.0f);                        // the offset of each channel's capture
+  size_t n = SIZE_MAX;
+  for (const Capture &c : caps) {
+    if (!load_raw(c.file.c_str(), iq[c.chan])) return 1;
+    n = std::min(n, iq[c.chan].size());
+    hz_of[c.chan] = c.hz;
+  }
+  if (iq[o.chan].empty()) { printf("no capture of the start channel %d in %s\n", o.chan, o.iq_dir); return 1; }
+  const long long nchunks = (long long)(n / BTLE_CHUNK_INT8);
+  HopRun run{&o};
+  btle_hop_hooks hooks{hop_now, hop_set_freq, hop_event, &run, o.quiet};
+  btle_b200_set_hop_hooks(&hooks);
+  int chan = o.chan;
+  uint32_t aa = o.aa, crc_internal = btle_b200_crc_init_reorder(o.crc_init);
+  // pass A: the start channel with the command line's access address, all chunks
+  std::vector<btle_pkt_rec> recs;
+  btle_stream_cfg cfg0{o.chan, o.aa, o.mask, o.crc_init, o.raw, cfg_flags(o)};
+  int rc = rx_batch_grow(ctx, iq[o.chan].data(), 1, n, n, &cfg0, recs, use_off ? &hz_of[o.chan] : nullptr);
+  if (rc) return fail(ctx, rc, "btle_b200_rx_batch");
+  size_t ri = 0;
+  long long k = 0;
+  for (; k < nchunks && !g_stop; ++k) {
+    for (; ri < recs.size() && recs[ri].chunk == k; ++ri) sinks.packet(recs[ri], rec_time(recs[ri]));
+    run.now = chunk_done_us(k);
+    if (btle_b200_receiver_controller(nullptr, o.verbose, &chan, &aa, &crc_internal) != 0) break;   // :2655-2658
+    if (chan != o.chan) { ++k; break; }                    // track start: the radio now sits on a data channel
+  }
+  if (chan != o.chan && k < nchunks) {
+    // pass B: every data channel from chunk k on, with the connection's parameters, one batched launch
+    const btle_receiver_status *st = btle_b200_receiver_status();
+    const size_t off = (size_t)k * BTLE_CHUNK_INT8, n2 = n - off, stride = (n2 + 15) & ~size_t(15);
+    std::vector<int> chan_of;
+    for (int c = 0; c < 37; ++c) if (!iq[c].empty()) chan_of.push_back(c);
+    std::vector<int8_t> stage(stride * chan_of.size());
+    std::vector<btle_stream_cfg> cfgs;
+    std::vector<float> hz;
+    for (size_t s_ = 0; s_ < chan_of.size(); ++s_) {
+      memcpy(stage.data() + s_ * stride, iq[chan_of[s_]].data() + off, n2);
+      cfgs.push_back(btle_stream_cfg{chan_of[s_], st->access_addr, o.mask, st->crc_init, o.raw, cfg_flags(o)});
+      hz.push_back(hz_of[chan_of[s_]]);
+    }
+    std::vector<btle_pkt_rec> data;
+    rc = rx_batch_grow(ctx, stage.data(), chan_of.size(), stride, n2, cfgs.data(), data, use_off ? hz.data() : nullptr);
+    if (rc) return fail(ctx, rc, "btle_b200_rx_batch");
+    // index: first record of every (stream, chunk)
+    std::vector<size_t> first(chan_of.size() * (size_t)(nchunks - k) + 1, 0);
+    {
+      size_t p = 0;
+      for (size_t b = 0; b + 1 < first.size(); ++b) {
+        const int s_ = (int)(b / (size_t)(nchunks - k)), c = (int)(b % (size_t)(nchunks - k));
+        while (p < data.size() && (data[p].stream < s_ || (data[p].stream == s_ && data[p].chunk < c))) ++p;
+        first[b] = p;
+      }
+      first.back() = data.size();
+    }
+    std::vector<int> stream_of(40, -1);
+    for (size_t s_ = 0; s_ < chan_of.size(); ++s_) stream_of[chan_of[s_]] = (int)s_;
+    for (; k < nchunks && !g_stop; ++k) {
+      const int s_ = stream_of[chan];
+      if (s_ >= 0) {
+        const size_t b = (size_t)s_ * (size_t)(nchunks - (long long)(off / BTLE_CHUNK_INT8)) + (size_t)(k - (long long)(off / BTLE_CHUNK_INT8));
+        for (size_t p = first[b]; p < first[b + 1]; ++p) {
+          btle_pkt_rec r = data[p];
+          r.chunk += (int32_t)(off / BTLE_CHUNK_INT8);
+          sinks.packet(r, rec_time(r));
+        }
+      }
+      run.now = chunk_done_us(k);
+      if (btle_b200_receiver_controller(nullptr, o.verbose, &chan, &aa, &crc_internal) != 0) break;
+    }
+  }
+  btle_b200_set_hop_hooks(nullptr);
+  *t_end = (double)(n / 2) / 4.0e6;
+  return 0;
+}
+
+// ---- --iq-txt / --iq-sc16: whole-file formats, one rx_batch call ----------------------------------------------------
+int run_whole_file(btle_b200_ctx *ctx, const Options &o, Sinks &sinks, double *t_end) {
+  std::vector<int8_t> iq;
+  if (o.iq_sc16 ? !load_raw(o.iq_sc16, iq) : !load_txt(o.iq_txt, iq)) return 1;
+  if (o.iq_sc16) {                                           // SC16Q11 to int8 as btle_rx's bladeRF build does, btle_rx.c:307-308
+    const int16_t *p16 = reinterpret_cast<const int16_t *>(iq.data());
+    std::vector<int8_t> r(iq.size() / 2);
+    for (size_t i = 0; i < r.size(); ++i) r[i] = (int8_t)((p16[i] >> 4) & 0xFF);
+    iq.swap(r);
+  }
+  btle_stream_cfg cfg{o.chan, o.aa, o.mask, o.crc_init, o.raw, cfg_flags(o)};
+  float hz = o.offset_hz;
+  if (o.offset_auto && estimate_offset(ctx, iq, cfg, o.iq_txt ? o.iq_txt : "capture", &hz)) return 1;
+  std::vector<btle_pkt_rec> recs;
+  const int rc = rx_batch_grow(ctx, iq.data(), 1, iq.size(), iq.size(), &cfg, recs, o.offset_set ? &hz : nullptr);
+  if (rc) return fail(ctx, rc, "btle_b200_rx");
+  for (size_t i = 0; i < recs.size() && !g_stop; ++i) sinks.packet(recs[i], rec_time(recs[i]));
+  *t_end = (double)(iq.size() / 2) / 4.0e6;
+  return 0;
+}
+
+// ---- raw captures (every -i, --iq-dir without -o), streamed through one session (btle_b200_streams_*): poll() across the
+//      inputs, read() into whichever capture has data and room, one batched launch per segment set --------------------------
+int run_session(btle_b200_ctx *ctx, const Options &o, const std::vector<Capture> &caps, bool use_off, Sinks &sinks, double *t_end) {
+  const size_t ns = caps.size();
+  Inputs in;
+  size_t n_stdin = 0;
+  for (const Capture &c : caps) {
+    if (c.file == "-") {
+      if (n_stdin++) { printf("'-' (stdin) can be the input of one capture only\n"); return 1; }
+      in.fds.push_back(0);
+      continue;
+    }
+    in.fds.push_back(open(c.file.c_str(), O_RDONLY));         // a FIFO: waits here until its writer has opened it
+    if (in.fds.back() < 0) { perror(c.file.c_str()); return 1; }
+  }
+  std::vector<btle_stream_cfg> cfgs;
+  for (const Capture &c : caps) cfgs.push_back(btle_stream_cfg{c.chan, c.aa, o.mask, c.crc_init, o.raw, cfg_flags(o)});
+  btle_b200_streams *ss = nullptr;
+  int rc = btle_b200_streams_open(ctx, cfgs.data(), ns, o.segment_chunks, &ss);
+  const std::unique_ptr<btle_b200_streams, StreamsClose> session(ss);
+  if (rc) return fail(ctx, rc, "btle_b200_streams_open");
+  for (size_t s_ = 0; s_ < ns && use_off && !rc; ++s_) rc = btle_b200_streams_set_offset(ss, s_, caps[s_].hz);
+  if (rc) return fail(ctx, rc, "btle_b200_streams_set_offset");
+  ConnMonitor mon(ss, o);
+  if (o.connections && mon.begin()) return fail(ctx, mon.rc, "--connections");
+  std::vector<btle_pkt_rec> recs(65536), pending;
+  long long max_chunk = -1;
+  // A record is printed once no record still to come can sort in front of it: every such record lies in a chunk behind
+  // max_chunk, and a hit starts at most 124 samples before its chunk.
+  auto emit = [&](bool all) {
+    long long safe = (max_chunk + 1) * 8192 - 124;
+    if (o.connections) {                                     // a backfilled record can lie anywhere in the resident sets
+      int64_t res = 0;
+      btle_b200_streams_resident(ss, &res);
+      safe = std::min<long long>(safe, (long long)res * 8192 - 124);
+    }
+    if (print_in_order(pending, sinks, all ? LLONG_MAX : safe)) fflush(stdout);
+  };
+  auto keep = [&](size_t n) {
+    for (size_t i = 0; i < n; ++i) { pending.push_back(recs[i]); max_chunk = std::max<long long>(max_chunk, recs[i].chunk); }
+    if (o.connections) { mon.hand_out(recs.data(), n); if (mon.rc && !rc) rc = mon.rc; }
+  };
+  std::vector<size_t> total(ns, 0);
+  std::vector<char> eof(ns, 0);
+  size_t shortest = SIZE_MAX;                                 // length of the shortest capture once one has ended
+  while (!g_stop && rc == 0) {
+    std::vector<pollfd> pf;
+    std::vector<size_t> who;
+    for (size_t s_ = 0; s_ < ns; ++s_) {
+      if (eof[s_] || total[s_] >= shortest) continue;         // bytes behind the shortest capture are not decoded
+      int8_t *buf; size_t space;
+      btle_b200_streams_acquire(ss, s_, &buf, &space);
+      if (space) { pf.push_back(pollfd{in.fds[s_], POLLIN, 0}); who.push_back(s_); }   // else: waits for the other captures
+    }
+    if (pf.empty()) break;
+    if (poll(pf.data(), pf.size(), -1) < 0) {
+      if (errno == EINTR) continue;
+      perror("poll");
+      break;
+    }
+    for (size_t k = 0; k < pf.size() && rc == 0; ++k) {
+      if (!(pf[k].revents & (POLLIN | POLLHUP | POLLERR))) continue;
+      const size_t s_ = who[k];
+      int8_t *buf; size_t space;
+      btle_b200_streams_acquire(ss, s_, &buf, &space);
+      const ssize_t got = read(in.fds[s_], buf, std::min(space, size_t(8) << 20));
+      if (got < 0 && errno == EINTR) continue;
+      if (got <= 0) {
+        if (got < 0) perror(caps[s_].file.c_str());
+        eof[s_] = 1;
+        shortest = std::min(shortest, total[s_]);
+        continue;
+      }
+      total[s_] += (size_t)got;
+      size_t n = 0;
+      rc = btle_b200_streams_commit(ss, s_, (size_t)got, recs.data(), recs.size(), &n);
+      keep(n);
+      while (rc == 0 && n == recs.size()) { rc = btle_b200_streams_commit(ss, s_, 0, recs.data(), recs.size(), &n); keep(n); }
+      emit(false);
+    }
+  }
+  if (rc) return fail(ctx, rc, "btle_b200_streams_commit");
+  for (bool more = true; more && rc == 0;) {                 // end of input or SIGINT: decode up to the shortest capture
+    more = false;
+    for (;;) {
+      size_t n = 0;
+      rc = btle_b200_streams_finish(ss, recs.data(), recs.size(), &n);
+      keep(n);
+      more |= o.connections && mon.added > 0;                // new connections: their backfill comes from the next finish
+      if (rc != BTLE_EOVERFLOW) break;
+    }
+  }
+  if (rc) return fail(ctx, rc, "btle_b200_streams_finish");
+  const size_t n_read = *std::min_element(total.begin(), total.end());
+  if (g_stop) {
+    // stopped mid-stream: print only what a full run prints first — the chunks whose look-ahead had arrived on every
+    // capture (the tail decode read zeros behind them), up to where a later chunk's hit could sort in front
+    const long long done = n_read >= (size_t)BTLE_LOOKAHEAD_INT8 ? (long long)((n_read - BTLE_LOOKAHEAD_INT8) / BTLE_CHUNK_INT8) : 0;
+    pending.erase(std::remove_if(pending.begin(), pending.end(), [&](const btle_pkt_rec &r) { return r.chunk >= done; }), pending.end());
+    max_chunk = done - 1;
+    emit(false);
+  } else {
+    emit(true);
+  }
+  *t_end = (double)(n_read / 2) / 4.0e6;
+  return 0;
+}
+
 }  // namespace
 
 int main(int argc, char **argv) {
@@ -760,7 +1070,7 @@ int main(int argc, char **argv) {
   Sinks sinks(o);
   if (o.pcap) {
     if (!o.quiet) printf("will store packets to: %s\n", o.pcap);
-    sinks.pcap = pcap_open(o.pcap);
+    sinks.pcap.reset(pcap_open(o.pcap));
     if (!sinks.pcap) { perror(o.pcap); return 1; }
   }
   if (o.json) json_status(0.0, "start", o);
@@ -776,346 +1086,25 @@ int main(int argc, char **argv) {
   sigaction(SIGTERM, &sa, nullptr);
 
   btle_b200_bind_host_numa(o.device, nullptr);                                  // page-locked buffers next to the GPU
-  btle_b200_ctx *ctx = nullptr;
-  int rc = btle_b200_create(&ctx, o.device);
+  btle_b200_ctx *created = nullptr;
+  const int rc = btle_b200_create(&created, o.device);
+  const std::unique_ptr<btle_b200_ctx, CtxClose> ctx(created);
   if (rc) { printf("btle_b200_create: %s\n", btle_b200_strerror(rc)); return 1; }
   btle_b200_hop_reset();
-  auto fail = [&](const char *what) {
-    printf("%s: %s (%s)\n", what, btle_b200_strerror(rc), btle_b200_last_error(ctx));
-    btle_b200_destroy(ctx);
-    return 1;
-  };
-  double t_end = 0.0;
-
-  // ---------------------------------------------------------------------------------------------------------------
   std::vector<Capture> caps;
-  for (const std::string &f : o.iq_files) caps.push_back(parse_capture(f, o));
-  if (o.iq_dir) {
-    for (int ch = 0; ch < 40; ++ch) {
-      char name[512];
-      snprintf(name, sizeof name, "%s/ch%02d.bin", o.iq_dir, ch);
-      if (access(name, R_OK) != 0) continue;
-      const bool adv = ch >= 37;
-      caps.push_back(Capture{name, ch, adv ? 0x8E89BED6u : o.aa, adv ? 0x555555u : o.crc_init, o.offset_hz, false});
-    }
-    if (caps.empty()) { printf("no chNN.bin capture found in %s\n", o.iq_dir); btle_b200_destroy(ctx); return 1; }
-  }
-  for (const Capture &c : caps)
-    if (c.chan < 0 || c.chan > 39) { printf("channel number must be within 0~%d!\n", 39); btle_b200_destroy(ctx); return 1; }
-  if (o.connections && caps.size() != 40) { printf("--connections needs all 40 chNN.bin captures in %s\n", o.iq_dir); btle_b200_destroy(ctx); return 1; }
-  // carrier-offset correction: --offset HZ for every capture, FILE:CH:AA:CRCINIT:HZ for one, --offset auto from a first pass
-  bool use_off = o.offset_set;
-  for (const Capture &c : caps) use_off |= c.own_hz;
-  if (o.offset_auto) {
-    for (Capture &c : caps) {
-      if (c.own_hz) continue;
-      struct stat sb;
-      if (c.file == "-" || stat(c.file.c_str(), &sb) != 0 || !S_ISREG(sb.st_mode)) {
-        printf("--offset auto needs regular files (%s is not one)\n", c.file.c_str());
-        btle_b200_destroy(ctx);
-        return 1;
-      }
-      std::vector<int8_t> iq;
-      if (!load_raw(c.file.c_str(), iq)) { btle_b200_destroy(ctx); return 1; }
-      size_t n_ok = 0;
-      rc = estimate_offset(ctx, iq, btle_stream_cfg{c.chan, c.aa, o.mask, c.crc_init, 0, 0}, &c.hz, &n_ok);
-      if (rc) return fail("--offset auto");
-      fprintf(stderr, "offset estimate %s: %.1f Hz (%zu CRC-ok packets)\n", c.file.c_str(), c.hz, n_ok);
-    }
-  }
-  std::vector<float> hz_of(40, 0.0f);                        // -o: the offset of each channel's capture
-  for (const Capture &c : caps) hz_of[c.chan] = c.hz;
+  bool use_off = false;
+  if (const int st = load_captures(ctx.get(), o, caps, &use_off)) return st;
 
-  if (o.iq_bin16) {
-    // ---- 8 samples per symbol: the Python / Verilog model's receiver, streaming over the capture -------------------------
-    std::vector<int8_t> raw;
-    if (!load_raw(o.iq_bin16, raw)) { btle_b200_destroy(ctx); return 1; }
-    const size_t n_samples = raw.size() / 4;
-    std::vector<btle_sps8_rec> recs(n_samples / 576 + 16);
-    size_t n = 0;
-    rc = btle_b200_rx_sps8(ctx, reinterpret_cast<const int16_t *>(raw.data()), n_samples, o.chan, o.crc_init, o.aa, recs.data(), recs.size(), &n);
-    if (rc) return fail("btle_b200_rx_sps8");
-    const bool adv = (o.chan == 37 || o.chan == 38 || o.chan == 39);
-    for (size_t i = 0; i < n && !g_stop; ++i) {
-      const btle_model_rx_rec &m = recs[i].rx;
-      if (!m.found || m.n_pdu_bits < 16) continue;         // no header decoded: nothing the sinks could show
-      btle_pkt_rec r;
-      memset(&r, 0, sizeof r);
-      const int have = m.n_pdu_bits / 8;                    // header + payload bytes that were decoded (CRC clamp, btlelib.py:488-490)
-      memcpy(r.bytes, m.pdu, (size_t)std::min(have, 39));
-      const int plen = std::min(have - 2, (int)(r.bytes[1] & (adv ? 0x3F : 0x1F)));
-      r.bytes[1] = (uint8_t)((r.bytes[1] & (adv ? 0xC0 : 0xE0)) | plen);
-      r.channel = (uint8_t)o.chan; r.access_addr = o.aa; r.flags = adv ? 2 : 0;
-      r.crc_bad = m.crc_ok ? 0 : 1;
-      r.n_bytes = (uint8_t)(plen + 5);
-      sinks.packet(r, (double)recs[i].sample / 8.0e6);
-    }
-    t_end = (double)n_samples / 8.0e6;
-  } else if (o.hop && o.iq_dir) {
-    // ---- connection following over per-channel captures ---------------------------------------------------------
-    std::vector<std::vector<int8_t>> iq(40);
-    size_t n = SIZE_MAX;
-    for (const Capture &c : caps) {
-      if (!load_raw(c.file.c_str(), iq[c.chan])) { btle_b200_destroy(ctx); return 1; }
-      n = std::min(n, iq[c.chan].size());
-    }
-    if (iq[o.chan].empty()) { printf("no capture of the start channel %d in %s\n", o.chan, o.iq_dir); btle_b200_destroy(ctx); return 1; }
-    const long long nchunks = (long long)(n / BTLE_CHUNK_INT8);
-    HopRun run{&o};
-    btle_hop_hooks hooks{hop_now, hop_set_freq, hop_event, &run, o.quiet};
-    btle_b200_set_hop_hooks(&hooks);
-    int chan = o.chan;
-    uint32_t aa = o.aa, crc_internal = btle_b200_crc_init_reorder(o.crc_init);
-    // pass A: the start channel with the command line's access address, all chunks
-    std::vector<btle_pkt_rec> recs;
-    btle_stream_cfg cfg0{o.chan, o.aa, o.mask, o.crc_init, o.raw, cfg_flags(o)};
-    rc = rx_batch_grow(ctx, iq[o.chan].data(), 1, n, n, &cfg0, recs, use_off ? &hz_of[o.chan] : nullptr);
-    if (rc) return fail("btle_b200_rx_batch");
-    size_t ri = 0;
-    long long k = 0;
-    for (; k < nchunks && !g_stop; ++k) {
-      for (; ri < recs.size() && recs[ri].chunk == k; ++ri) sinks.packet(recs[ri], rec_time(recs[ri]));
-      run.now = chunk_done_us(k);
-      if (btle_b200_receiver_controller(nullptr, o.verbose, &chan, &aa, &crc_internal) != 0) break;   // :2655-2658
-      if (chan != o.chan) { ++k; break; }                    // track start: the radio now sits on a data channel
-    }
-    if (chan != o.chan && k < nchunks) {
-      // pass B: every data channel from chunk k on, with the connection's parameters, one batched launch
-      const btle_receiver_status *st = btle_b200_receiver_status();
-      const size_t off = (size_t)k * BTLE_CHUNK_INT8, n2 = n - off, stride = (n2 + 15) & ~size_t(15);
-      std::vector<int> chan_of;
-      for (int c = 0; c < 37; ++c) if (!iq[c].empty()) chan_of.push_back(c);
-      std::vector<int8_t> stage(stride * chan_of.size());
-      std::vector<btle_stream_cfg> cfgs;
-      std::vector<float> hz;
-      for (size_t s_ = 0; s_ < chan_of.size(); ++s_) {
-        memcpy(stage.data() + s_ * stride, iq[chan_of[s_]].data() + off, n2);
-        cfgs.push_back(btle_stream_cfg{chan_of[s_], st->access_addr, o.mask, st->crc_init, o.raw, cfg_flags(o)});
-        hz.push_back(hz_of[chan_of[s_]]);
-      }
-      std::vector<btle_pkt_rec> data;
-      rc = rx_batch_grow(ctx, stage.data(), chan_of.size(), stride, n2, cfgs.data(), data, use_off ? hz.data() : nullptr);
-      if (rc) return fail("btle_b200_rx_batch");
-      // index: first record of every (stream, chunk)
-      std::vector<size_t> first(chan_of.size() * (size_t)(nchunks - k) + 1, 0);
-      {
-        size_t p = 0;
-        for (size_t b = 0; b + 1 < first.size(); ++b) {
-          const int s_ = (int)(b / (size_t)(nchunks - k)), c = (int)(b % (size_t)(nchunks - k));
-          while (p < data.size() && (data[p].stream < s_ || (data[p].stream == s_ && data[p].chunk < c))) ++p;
-          first[b] = p;
-        }
-        first.back() = data.size();
-      }
-      std::vector<int> stream_of(40, -1);
-      for (size_t s_ = 0; s_ < chan_of.size(); ++s_) stream_of[chan_of[s_]] = (int)s_;
-      for (; k < nchunks && !g_stop; ++k) {
-        const int s_ = stream_of[chan];
-        if (s_ >= 0) {
-          const size_t b = (size_t)s_ * (size_t)(nchunks - (long long)(off / BTLE_CHUNK_INT8)) + (size_t)(k - (long long)(off / BTLE_CHUNK_INT8));
-          for (size_t p = first[b]; p < first[b + 1]; ++p) {
-            btle_pkt_rec r = data[p];
-            r.chunk += (int32_t)(off / BTLE_CHUNK_INT8);
-            sinks.packet(r, rec_time(r));
-          }
-        }
-        run.now = chunk_done_us(k);
-        if (btle_b200_receiver_controller(nullptr, o.verbose, &chan, &aa, &crc_internal) != 0) break;
-      }
-    }
-    btle_b200_set_hop_hooks(nullptr);
-    t_end = (double)(n / 2) / 4.0e6;
-  } else if (caps.size() > 1 || (caps.size() == 1 && o.iq_dir)) {
-    // ---- several captures, streamed through one session (btle_b200_streams_*): poll() across the inputs, read() into
-    //      whichever capture has data and room, one batched launch per segment set, packets in time order ----------------
-    const size_t ns = caps.size();
-    std::vector<int> fds(ns, -1);
-    auto close_inputs = [&]() { for (int fd : fds) if (fd > 0) close(fd); };
-    size_t n_stdin = 0;
-    for (size_t s_ = 0; s_ < ns; ++s_) {
-      if (caps[s_].file == "-") {
-        if (n_stdin++) { printf("'-' (stdin) can be the input of one capture only\n"); close_inputs(); btle_b200_destroy(ctx); return 1; }
-        fds[s_] = 0;
-        continue;
-      }
-      fds[s_] = open(caps[s_].file.c_str(), O_RDONLY);           // a FIFO: waits here until its writer has opened it
-      if (fds[s_] < 0) { perror(caps[s_].file.c_str()); close_inputs(); btle_b200_destroy(ctx); return 1; }
-    }
-    std::vector<btle_stream_cfg> cfgs;
-    for (const Capture &c : caps) cfgs.push_back(btle_stream_cfg{c.chan, c.aa, o.mask, c.crc_init, o.raw, cfg_flags(o)});
-    btle_b200_streams *ss = nullptr;
-    rc = btle_b200_streams_open(ctx, cfgs.data(), ns, o.segment_chunks, &ss);
-    if (rc) { close_inputs(); return fail("btle_b200_streams_open"); }
-    for (size_t s_ = 0; s_ < ns && use_off && !rc; ++s_) rc = btle_b200_streams_set_offset(ss, s_, caps[s_].hz);
-    if (rc) { btle_b200_streams_close(ss); close_inputs(); return fail("btle_b200_streams_set_offset"); }
-    ConnMonitor mon(ss, o);
-    if (o.connections && mon.begin()) { rc = mon.rc; btle_b200_streams_close(ss); close_inputs(); return fail("--connections"); }
-    std::vector<btle_pkt_rec> recs(65536), pending;
-    long long max_chunk = -1;
-    // Records arrive per segment set in (stream, chunk, n0) order.  They are printed in time order (chunk*8192 + n0; ties in
-    // (stream, chunk, n0) order), as soon as no later record can sort in front of them: every record still to come lies in a
-    // later chunk, and a hit starts at most 124 samples before its chunk.
-    auto emit = [&](bool all) {
-      auto key = [](const btle_pkt_rec &r) { return (long long)r.chunk * 8192 + r.n0; };
-      std::stable_sort(pending.begin(), pending.end(), [&](const btle_pkt_rec &a, const btle_pkt_rec &b) {
-        if (key(a) != key(b)) return key(a) < key(b);
-        return a.stream != b.stream ? a.stream < b.stream : a.chunk < b.chunk;
-      });
-      long long safe = (max_chunk + 1) * 8192 - 124;
-      if (o.connections) {                                     // a backfilled record can lie anywhere in the resident sets
-        int64_t res = 0;
-        btle_b200_streams_resident(ss, &res);
-        safe = std::min<long long>(safe, (long long)res * 8192 - 124);
-      }
-      size_t k = 0;
-      for (; k < pending.size() && (all || key(pending[k]) < safe); ++k) sinks.packet(pending[k], rec_time(pending[k]));
-      pending.erase(pending.begin(), pending.begin() + (long)k);
-      if (k) fflush(stdout);
-    };
-    auto keep = [&](size_t n) {
-      for (size_t i = 0; i < n; ++i) { pending.push_back(recs[i]); max_chunk = std::max<long long>(max_chunk, recs[i].chunk); }
-      if (o.connections) { mon.hand_out(recs.data(), n); if (mon.rc && !rc) rc = mon.rc; }
-    };
-    std::vector<size_t> total(ns, 0);
-    std::vector<char> eof(ns, 0);
-    size_t shortest = SIZE_MAX;                                 // length of the shortest capture once one has ended
-    while (!g_stop && rc == 0) {
-      std::vector<pollfd> pf;
-      std::vector<size_t> who;
-      for (size_t s_ = 0; s_ < ns; ++s_) {
-        if (eof[s_] || total[s_] >= shortest) continue;         // bytes behind the shortest capture are not decoded
-        int8_t *buf; size_t space;
-        btle_b200_streams_acquire(ss, s_, &buf, &space);
-        if (space) { pf.push_back(pollfd{fds[s_], POLLIN, 0}); who.push_back(s_); }   // else: waits for the other captures
-      }
-      if (pf.empty()) break;
-      if (poll(pf.data(), pf.size(), -1) < 0) {
-        if (errno == EINTR) continue;
-        perror("poll");
-        break;
-      }
-      for (size_t k = 0; k < pf.size() && rc == 0; ++k) {
-        if (!(pf[k].revents & (POLLIN | POLLHUP | POLLERR))) continue;
-        const size_t s_ = who[k];
-        int8_t *buf; size_t space;
-        btle_b200_streams_acquire(ss, s_, &buf, &space);
-        const ssize_t got = read(fds[s_], buf, std::min(space, size_t(8) << 20));
-        if (got < 0 && errno == EINTR) continue;
-        if (got <= 0) {
-          if (got < 0) perror(caps[s_].file.c_str());
-          eof[s_] = 1;
-          shortest = std::min(shortest, total[s_]);
-          continue;
-        }
-        total[s_] += (size_t)got;
-        size_t n = 0;
-        rc = btle_b200_streams_commit(ss, s_, (size_t)got, recs.data(), recs.size(), &n);
-        keep(n);
-        while (rc == 0 && n == recs.size()) { rc = btle_b200_streams_commit(ss, s_, 0, recs.data(), recs.size(), &n); keep(n); }
-        emit(false);
-      }
-    }
-    if (rc) { btle_b200_streams_close(ss); close_inputs(); return fail("btle_b200_streams_commit"); }
-    for (bool more = true; more && rc == 0;) {                 // end of input or SIGINT: decode up to the shortest capture
-      more = false;
-      for (;;) {
-        size_t n = 0;
-        rc = btle_b200_streams_finish(ss, recs.data(), recs.size(), &n);
-        keep(n);
-        more |= o.connections && mon.added > 0;                // new connections: their backfill comes from the next finish
-        if (rc != BTLE_EOVERFLOW) break;
-      }
-    }
-    btle_b200_streams_close(ss);
-    close_inputs();
-    if (rc) return fail("btle_b200_streams_finish");
-    const size_t n_read = *std::min_element(total.begin(), total.end());
-    if (g_stop) {
-      // stopped mid-stream: print only what a full run prints first — the chunks whose look-ahead had arrived on every
-      // capture (the tail decode read zeros behind them), up to where a later chunk's hit could sort in front
-      const long long done = n_read >= (size_t)BTLE_LOOKAHEAD_INT8 ? (long long)((n_read - BTLE_LOOKAHEAD_INT8) / BTLE_CHUNK_INT8) : 0;
-      pending.erase(std::remove_if(pending.begin(), pending.end(), [&](const btle_pkt_rec &r) { return r.chunk >= done; }), pending.end());
-      max_chunk = done - 1;
-      emit(false);
-    } else {
-      emit(true);
-    }
-    t_end = (double)(n_read / 2) / 4.0e6;
-  } else if (o.iq_txt || o.iq_sc16) {
-    // ---- whole-file formats ----------------------------------------------------------------------------------------
-    std::vector<int8_t> iq;
-    if (o.iq_sc16 ? !load_raw(o.iq_sc16, iq) : !load_txt(o.iq_txt, iq)) { btle_b200_destroy(ctx); return 1; }
-    btle_stream_cfg cfg{o.chan, o.aa, o.mask, o.crc_init, o.raw, cfg_flags(o)};
-    float hz = o.offset_hz;
-    if (o.offset_set && o.iq_sc16) {                                     // the reduction of btle_b200_rx_iq16, here on the host
-      const int16_t *p16 = reinterpret_cast<const int16_t *>(iq.data());
-      std::vector<int8_t> r(iq.size() / 2);
-      for (size_t i = 0; i < r.size(); ++i) r[i] = (int8_t)((p16[i] >> 4) & 0xFF);      // btle_rx.c:307-308
-      iq.swap(r);
-      o.iq_sc16 = nullptr;
-    }
-    if (o.offset_auto) {
-      size_t n_ok = 0;
-      rc = estimate_offset(ctx, iq, cfg, &hz, &n_ok);
-      if (rc) return fail("--offset auto");
-      fprintf(stderr, "offset estimate %s: %.1f Hz (%zu CRC-ok packets)\n", o.iq_txt ? o.iq_txt : "capture", hz, n_ok);
-    }
-    const size_t n_iq = o.iq_sc16 ? iq.size() / 2 : iq.size();          // int8 values after the optional reduction
-    size_t cap = (n_iq / BTLE_CHUNK_INT8) * 4 + 1024, n = 0;
-    std::vector<btle_pkt_rec> recs;
-    for (int attempt = 0; attempt < 2; ++attempt) {
-      recs.resize(cap);
-      if (o.iq_sc16) rc = btle_b200_rx_iq16(ctx, reinterpret_cast<const int16_t *>(iq.data()), n_iq, 4, &cfg, recs.data(), cap, &n);   // btle_rx.c:307-308
-      else rc = btle_b200_rx_batch_offset(ctx, iq.data(), 1, iq.size(), iq.size(), &cfg, o.offset_set ? &hz : nullptr, recs.data(), cap, &n);
-      if (rc != BTLE_EOVERFLOW) break;
-      cap = n;
-    }
-    if (rc) return fail("btle_b200_rx");
-    for (size_t i = 0; i < n && !g_stop; ++i) sinks.packet(recs[i], rec_time(recs[i]));
-    t_end = (double)(n_iq / 2) / 4.0e6;
-  } else {
-    // ---- one raw capture, streamed: read() straight into page-locked segments while the GPU decodes the previous one ----
-    const Capture c = caps[0];
-    FILE *f = strcmp(c.file.c_str(), "-") ? fopen(c.file.c_str(), "rb") : stdin;
-    if (!f) { perror(c.file.c_str()); btle_b200_destroy(ctx); return 1; }
-    btle_stream_cfg cfg{c.chan, c.aa, o.mask, c.crc_init, o.raw, cfg_flags(o)};
-    btle_b200_stream *st = nullptr;
-    rc = btle_b200_stream_open(ctx, &cfg, o.segment_chunks, &st);
-    if (rc) return fail("btle_b200_stream_open");
-    if (use_off && (rc = btle_b200_stream_set_offset(st, c.hz))) { btle_b200_stream_close(st); return fail("btle_b200_stream_set_offset"); }
-    std::vector<btle_pkt_rec> recs(65536);
-    size_t total = 0;
-    const int fd = fileno(f);
-    bool eof = false;
-    while (!eof && !g_stop) {
-      int8_t *buf; size_t space;
-      btle_b200_stream_acquire(st, &buf, &space);
-      const ssize_t got = read(fd, buf, std::min(space, size_t(8) << 20));
-      if (got < 0) { if (errno == EINTR) continue; perror("read"); break; }
-      if (got == 0) { eof = true; break; }
-      total += (size_t)got;
-      size_t n = 0;
-      rc = btle_b200_stream_commit(st, (size_t)got, recs.data(), recs.size(), &n);
-      if (rc) { btle_b200_stream_close(st); return fail("btle_b200_stream_commit"); }
-      for (size_t i = 0; i < n; ++i) sinks.packet(recs[i], rec_time(recs[i]));
-      if (n) fflush(stdout);
-    }
-    for (;;) {
-      size_t n = 0;
-      rc = btle_b200_stream_finish(st, recs.data(), recs.size(), &n);
-      for (size_t i = 0; i < n; ++i) sinks.packet(recs[i], rec_time(recs[i]));
-      if (rc != BTLE_EOVERFLOW) break;
-    }
-    btle_b200_stream_close(st);
-    if (rc) return fail("btle_b200_stream_finish");
-    if (f != stdin) fclose(f);
-    t_end = (double)(total / 2) / 4.0e6;
-  }
+  double t_end = 0.0;
+  int st;
+  if (o.iq_bin16) st = run_sps8(ctx.get(), o, sinks, &t_end);
+  else if (o.hop && o.iq_dir) st = run_hop(ctx.get(), o, caps, use_off, sinks, &t_end);
+  else if ((o.iq_txt || o.iq_sc16) && !o.iq_dir && caps.size() <= 1) st = run_whole_file(ctx.get(), o, sinks, &t_end);
+  else st = run_session(ctx.get(), o, caps, use_off, sinks, &t_end);
+  if (st) return st;
 
   fflush(stdout);
   if (!o.quiet) printf("Exit main loop ...\n");                                 // :2664
   if (o.json) json_status(t_end, "stop", o);
-  if (sinks.pcap) fclose(sinks.pcap);
-  btle_b200_destroy(ctx);
   return 0;
 }

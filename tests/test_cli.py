@@ -147,11 +147,17 @@ def test_cli_sc16_input_equals_int8_input(tmp_path):
     iq8 = iq8.numpy()
     (tmp_path / "a.int8").write_bytes(iq8.tobytes())
     (tmp_path / "a.sc16").write_bytes((iq8.astype(np.int16) << 4).tobytes())
+    # save_phy_sample's text layout (btle_rx.c:896-915): a newline before every 64 values, each value followed by ", "
+    (tmp_path / "a.txt").write_text("".join(("\n" if i % 64 == 0 else "") + f"{v}, " for i, v in enumerate(iq8.tolist())) + "\n")
     a = run(["-i", str(tmp_path / "a.int8"), "-Q", "-j"])
-    b = run(["--iq-sc16", str(tmp_path / "a.sc16"), "-Q", "-j"])
-    assert a.returncode == 0 and b.returncode == 0
+    assert a.returncode == 0
     pk = lambda s_: [l for l in s_.splitlines() if '"t":"pkt"' in l]
-    assert len(pk(a.stdout)) > 10 and pk(a.stdout) == pk(b.stdout)
+    assert len(pk(a.stdout)) > 10
+    for args in (["--iq-sc16", str(tmp_path / "a.sc16")], ["--iq-sc16", str(tmp_path / "a.sc16"), "--offset", "0"],
+                 ["--iq-txt", str(tmp_path / "a.txt")]):
+        b = run(args + ["-Q", "-j"])
+        assert b.returncode == 0, args
+        assert pk(b.stdout) == pk(a.stdout), args
 
 
 @pytest.mark.gpu
@@ -248,8 +254,10 @@ def test_cli_multi_capture_batch_equals_single_runs(tmp_path):
 
 @pytest.mark.gpu
 def test_cli_streams_a_capture_in_segments_and_from_a_pipe(tmp_path):
-    """A single capture is read in segments straight into page-locked buffers and decoded while the next segment is read
-    (btle_b200_stream_*): any segment size, a file or a pipe, gives the records of the whole-capture call."""
+    """A single capture goes through the same session as several (btle_b200_streams_*, which serves any number of -i): it
+    is read in segments straight into page-locked buffers and decoded while the next segment is read.  Any segment size,
+    a file or a pipe, gives the records of the whole-capture call, printed in the reference's processing order (sample
+    time, except that a capture's records never move in front of an earlier one of the same capture)."""
     iq, _ = synth.make_adv_stream(45 * 16384 + 5000, seed=31, channel=38, slot_samples=2300, straddle_every=3, corrupt_every=5)
     f = tmp_path / "iq.bin"
     iq.numpy().tofile(f)
