@@ -401,6 +401,76 @@ BTLE_DENSE void dbits_group_rot(WordAt &word, int c, int s, uint32_t acc[4]) {
   }
 }
 
+// ---- symbol-spaced bits (BTLE_CFG_SYMBOL_SPACED, include/btle_b200.h) --------------------------------------------------
+// d[n] = I[n-2] Q[n+2] - I[n+2] Q[n-2] > 0.  Samples n - 2 and n + 2 sit in the words in front of and behind sample n's word,
+// at its byte position, so dbits8_dense's identity t = 256 v + (127 - Q1) carries over with the a-operand built from the
+// word in front and the b-operand taken from the same half of the word behind: one byte-permute and one IDP.2A per sample.
+// wprev = the IQ word in front of w0, wnext the word behind w3; the bits of the step's 8 samples go where dbits8_dense puts them.
+template <int CM>
+BTLE_DENSE void dbits8_sym(uint32_t wprev, uint32_t w0, uint32_t w1, uint32_t w2, uint32_t w3, uint32_t wnext, uint32_t acc[4]) {
+  const uint32_t cp = wprev ^ 0x00FF00FFu, c0 = w0 ^ 0x00FF00FFu, c1 = w1 ^ 0x00FF00FFu, c2 = w2 ^ 0x00FF00FFu;
+  const int t0 = __dp2a_lo(dp_a2<0>(cp), (int)w1, 127), t1 = __dp2a_hi(dp_a2<1>(cp), (int)w1, 127);
+  const int t2 = __dp2a_lo(dp_a2<0>(c0), (int)w2, 127), t3 = __dp2a_hi(dp_a2<1>(c0), (int)w2, 127);
+  const int t4 = __dp2a_lo(dp_a2<0>(c1), (int)w3, 127), t5 = __dp2a_hi(dp_a2<1>(c1), (int)w3, 127);
+  const int t6 = __dp2a_lo(dp_a2<0>(c2), (int)wnext, 127), t7 = __dp2a_hi(dp_a2<1>(c2), (int)wnext, 127);
+  acc[0] = add_bits<CM>(acc[0], t0, t4);
+  acc[1] = add_bits<CM>(acc[1], t1, t5);
+  acc[2] = add_bits<CM>(acc[2], t2, t6);
+  acc[3] = add_bits<CM>(acc[3], t3, t7);
+}
+// rot_u with the second sample in the SAME half of b as the first one in w (rotated symbol-spaced bit, (c, s) = (C4, S4))
+template <int HALF>
+BTLE_DENSE int rot_u_sym(uint32_t w, uint32_t wc, uint32_t b, int c, int s) {
+  const int a_im = prmt1<HALF ? 0xA2B3u : 0x8091u>(wc), a_re = prmt1<HALF ? 0xB3A2u : 0x9180u>(w);
+  const int v = HALF ? __dp2a_hi(a_im, (int)b, __dp2a_hi(0x00010000, (int)b, 0)) : __dp2a_lo(a_im, (int)b, __dp2a_lo(0x00010000, (int)b, 0));
+  const int r = HALF ? __dp2a_hi(a_re, (int)b, 0) : __dp2a_lo(a_re, (int)b, 0);
+  return c * v + s * r;
+}
+template <int CM>
+BTLE_DENSE void dbits8_sym_rot(uint32_t wprev, uint32_t w0, uint32_t w1, uint32_t w2, uint32_t w3, uint32_t wnext, int c, int s,
+                               uint32_t acc[4]) {
+  const uint32_t cp = wprev ^ 0x00FF00FFu, c0 = w0 ^ 0x00FF00FFu, c1 = w1 ^ 0x00FF00FFu, c2 = w2 ^ 0x00FF00FFu;
+  const int t0 = rot_u_sym<0>(wprev, cp, w1, c, s), t1 = rot_u_sym<1>(wprev, cp, w1, c, s);
+  const int t2 = rot_u_sym<0>(w0, c0, w2, c, s), t3 = rot_u_sym<1>(w0, c0, w2, c, s);
+  const int t4 = rot_u_sym<0>(w1, c1, w3, c, s), t5 = rot_u_sym<1>(w1, c1, w3, c, s);
+  const int t6 = rot_u_sym<0>(w2, c2, wnext, c, s), t7 = rot_u_sym<1>(w2, c2, wnext, c, s);
+  acc[0] = add_bits<CM>(acc[0], t0, t4);
+  acc[1] = add_bits<CM>(acc[1], t1, t5);
+  acc[2] = add_bits<CM>(acc[2], t2, t6);
+  acc[3] = add_bits<CM>(acc[3], t3, t7);
+}
+// one step of the symbol-spaced walk; ROT: rotated by (c, s) = (C4, S4)
+template <bool ROT>
+BTLE_DENSE void dbits8_sym_step(int cm, uint32_t wprev, uint32_t w0, uint32_t w1, uint32_t w2, uint32_t w3, uint32_t wnext, int c, int s,
+                                uint32_t acc[4]) {
+  if constexpr (ROT) {
+    switch (cm) {
+      case 3: dbits8_sym_rot<3>(wprev, w0, w1, w2, w3, wnext, c, s, acc); break;
+      case 2: dbits8_sym_rot<2>(wprev, w0, w1, w2, w3, wnext, c, s, acc); break;
+      case 1: dbits8_sym_rot<1>(wprev, w0, w1, w2, w3, wnext, c, s, acc); break;
+      default: dbits8_sym_rot<0>(wprev, w0, w1, w2, w3, wnext, c, s, acc); break;
+    }
+  } else {
+    switch (cm) {
+      case 3: dbits8_sym<3>(wprev, w0, w1, w2, w3, wnext, acc); break;
+      case 2: dbits8_sym<2>(wprev, w0, w1, w2, w3, wnext, acc); break;
+      case 1: dbits8_sym<1>(wprev, w0, w1, w2, w3, wnext, acc); break;
+      default: dbits8_sym<0>(wprev, w0, w1, w2, w3, wnext, acc); break;
+    }
+  }
+}
+// dbits_group_dense() with the symbol-spaced discriminator: word(-1) .. word(64) are read
+template <bool ROT, class WordAt>
+BTLE_DENSE void dbits_group_sym(WordAt &word, int c, int s, uint32_t acc[4]) {
+  uint32_t carry = word(64);
+  for (int C = 15; C >= 0; --C) {
+    const uint32_t w0 = word(4 * C), w1 = word(4 * C + 1), w2 = word(4 * C + 2), w3 = word(4 * C + 3);
+    if ((C & 3) == 3) { acc[0] <<= 8; acc[1] <<= 8; acc[2] <<= 8; acc[3] <<= 8; }
+    dbits8_sym_step<ROT>(C & 3, word(4 * C - 1), w0, w1, w2, w3, carry, c, s, acc);
+    carry = w0;
+  }
+}
+
 // Dense-pass prefilter: bit i of the result is 1 iff the window starting at symbol i of `lo`
 // agrees with the access address on the (<=16) prefilter taps.  A superset of the true matches;
 // the sparse pass re-checks every candidate exactly (search_from()).

@@ -270,6 +270,50 @@ __device__ __forceinline__ void load_multi_warp(const StreamParams *__restrict__
   if (lane == 0) { dst.cfg0 = v.y; dst.ncfg = v.z; }
 }
 
+// BTLE_CFG_SYMBOL_SPACED: the four phase words of this lane's group of a tile in `stage` (2 * rows box rows, SWIZZLE_128B),
+// walked from its end as the default dense loop walks it; head = the IQ word in front of the tile (read by lane 0), tail
+// the word behind it (lane rows - 1).  Samples -2, -1 come from the previous lane's last word and 128, 129 from the next
+// lane's first word, both exchanged before the walk, so every bit is final when it is made.  A step needs the word in front
+// of its 16 bytes: the walk loads the next-lower 16 bytes before it decodes the current ones.  ROT: (c, s) = (C4, S4).
+template <bool ROT>
+__device__ __forceinline__ void dense_sym_group(const unsigned char *stage, int rows, int lane, uint32_t head, uint32_t tail, int c, int s,
+                                                uint32_t acc[4]) {
+  auto word_of = [&](int r, int k) {                       // word k (0..31) of box row r
+    return reinterpret_cast<const uint32_t *>(stage + (r << 7) + ((((uint32_t)(k >> 2)) ^ (uint32_t)(r & 7)) << 4))[k & 3];
+  };
+  const bool mine = lane < rows;
+  const uint32_t first = mine ? word_of(lane, 0) : 0u, last = mine ? word_of(rows + lane, 31) : 0u, mid = mine ? word_of(lane, 31) : 0u;
+  uint32_t nb = __shfl_down_sync(0xFFFFFFFFu, first, 1), pv = __shfl_up_sync(0xFFFFFFFFu, last, 1);
+  if (lane == rows - 1) nb = tail;
+  if (lane == 0) pv = head;
+  if (!mine) return;
+  uint32_t carry = nb;
+#pragma unroll 1
+  for (int half = 1; half >= 0; --half) {
+    const int r = half * rows + lane;
+    const unsigned char *row = stage + (r << 7);
+    const uint32_t sw = (uint32_t)(r & 7);
+    const uint32_t below = half ? mid : pv;                // the word in front of the half's first word
+    uint4 cur = *reinterpret_cast<const uint4 *>(row + ((7u ^ sw) << 4));
+#pragma unroll
+    for (int cc = 7; cc >= 0; --cc) {
+      uint4 nxt = cur;
+      uint32_t wprev = below;
+      if (cc > 0) {
+        nxt = *reinterpret_cast<const uint4 *>(row + ((((uint32_t)(cc - 1)) ^ sw) << 4));
+        wprev = nxt.w;
+      }
+      if ((cc & 3) == 3) {
+#pragma unroll
+        for (int ph = 0; ph < 4; ++ph) acc[ph] <<= 8;
+      }
+      dbits8_sym_step<ROT>(cc & 3, wprev, cur.x, cur.y, cur.z, cur.w, carry, c, s, acc);
+      carry = cur.x;
+      cur = nxt;
+    }
+  }
+}
+
 // One persistent CTA per SM.  Units of work (a span of 16 chunks of one capture, or a 4-chunk piece of one in the
 // last wave — Plan, btle_core.cuh) are dealt round-robin to CTAs.
 // Warps 0..15 (dense): per 4096-sample tile, one TMA box brings the tile into 128B-swizzled shared rows;
@@ -290,7 +334,9 @@ __device__ __forceinline__ void load_multi_warp(const StreamParams *__restrict__
 // ROT (the *_offset entry points): rot[i] = {C, S, C4, S4} of cfg i (make_rot); the dense warps build the phase words from
 // the rotated discriminator (dbits8_rot, with the rotation of the capture's first cfg) and recovery rotates its
 // symbol-spaced bits by (C4, S4).  Without ROT, rot is not read.
-template <int KC, bool ROT>
+// SYM (BTLE_CFG_SYMBOL_SPACED): the dense warps build the phase words from the symbol-spaced discriminator (dense_sym_group;
+// with ROT rotated by the capture's first cfg's (C4, S4)).  Everything behind the phase words is the same code.
+template <int KC, bool ROT, bool SYM>
 __global__ void __launch_bounds__(kThreads, kCtasPerSm)
 btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __grid_constant__ CUtensorMap map12,
                           const int8_t *__restrict__ iq, long long stream_stride, long long n_int8,
@@ -433,8 +479,8 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
       int rc = 0, rs = 0;                                 // (C, S) of the capture
       if constexpr (ROT) {
         const int4 r = __ldg(rot + (KC == 1 ? si.stream : __ldg(&vmap[si.stream].y)));
-        rc = r.x;
-        rs = r.y;
+        rc = SYM ? r.z : r.x;
+        rs = SYM ? r.w : r.y;
       }
       int t = warp - rot_w;
       if (t < 0) t += kDenseWarps;
@@ -452,6 +498,16 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
           else
             for (int bb = 0; bb < 4; ++bb)
               if (o + bb < n_int8) tail |= (uint32_t)(uint8_t)cap_base[o + bb] << (8 * bb);
+        }
+        uint32_t head = 0;                                // SYM: the IQ word in front of the tile (`lead` bytes are readable)
+        if constexpr (SYM) {
+          if (lane == 0) {
+            const long long o = tile_off - 4;
+            if (o >= -lead && o + 4 <= n_int8) head = __ldg(reinterpret_cast<const uint32_t *>(cap_base + o));
+            else
+              for (int bb = 0; bb < 4; ++bb)
+                if (o + bb >= -lead && o + bb < n_int8) head |= (uint32_t)(uint8_t)cap_base[o + bb] << (8 * bb);
+          }
         }
         if (tma) {
           w_tma.begin();
@@ -485,6 +541,8 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
           __syncwarp();
         }
         uint32_t acc[4] = {0u, 0u, 0u, 0u};
+        if constexpr (SYM) dense_sym_group<ROT>(stage, rows, lane, head, tail, rc, rs, acc);
+        else {
         uint32_t carry = 0u, wtop = 0u;
         int vtop = 0;
 #pragma unroll 1
@@ -540,6 +598,7 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
             // sample 127 was pushed first, so after all 32 pushes it is bit 31 of phase 3
             if (half == 0) acc[3] = (acc[3] & 0x7FFFFFFFu) | ((uint32_t)vtop & 0x80000000u);
           }
+        }
         }
         __syncwarp();                                     // everyone is done reading the buffer
         request();                                        // the warp's next tile
@@ -1945,6 +2004,12 @@ int validate_cfgs(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size_t n) {
       ctx->err = "channel number must be within 0~39";
       return BTLE_EINVAL;
     }
+  // one dense loop per kernel instantiation: every cfg of a launch (or of a session) is in the same discriminator mode
+  for (size_t i = 1; i < n; ++i)
+    if ((cfgs[i].rssi ^ cfgs[0].rssi) & BTLE_CFG_SYMBOL_SPACED) {
+      ctx->err = "all cfgs of one launch must agree on BTLE_CFG_SYMBOL_SPACED";
+      return BTLE_EINVAL;
+    }
   return BTLE_OK;
 }
 
@@ -2125,11 +2190,11 @@ int make_rots(btle_b200_ctx *ctx, const float *offset_hz, size_t n_captures, con
   return BTLE_OK;
 }
 
-template <int KC, bool ROT>
+template <int KC, bool ROT, bool SYM>
 void enqueue_rx(unsigned grid, cudaStream_t st, const MapSlot *ms, const int8_t *d_iq, size_t stride, size_t n_int8, const CfgSlot *cs,
                 const Plan &plan, btle_pkt_rec *d_out, unsigned cap32, unsigned *d_count, btle_unit_dir *d_dir, unsigned *zero_next,
                 long long lead) {
-  btle_rx_persistent_kernel<KC, ROT><<<grid, kThreads, sizeof(Smem<KC>), st>>>(
+  btle_rx_persistent_kernel<KC, ROT, SYM><<<grid, kThreads, sizeof(Smem<KC>), st>>>(
       ms->map32, ms->map12, d_iq, (long long)stride, (long long)n_int8, cs->d_params, plan, d_out, cap32, d_count,
       reinterpret_cast<uint2 *>(d_dir), zero_next, lead, KC > 1 ? cs->d_vmap.p : nullptr, ROT ? cs->d_rot.p : nullptr);
 }
@@ -2139,7 +2204,8 @@ void enqueue_rx(unsigned grid, cudaStream_t st, const MapSlot *ms, const int8_t 
 // A list that maps cfg i to capture i for every capture runs btle_rx_persistent_kernel<1>, the directory in unit order;
 // any other list runs <kMaxCfgsPerCapture> over the captures it names, the directory in (cfg, chunk) order.
 // rot != nullptr: one rotation per cfg (make_rot), the rotated kernel variant.  `lead`: bytes readable in front of each
-// capture (the stream session's lead: RSSI of hits at a segment's very start).
+// capture (the stream session's lead: RSSI of hits at a segment's very start, the symbol-spaced bits of its first samples).
+// cfgs with BTLE_CFG_SYMBOL_SPACED (all or none, validate_cfgs) run the symbol-spaced variant.
 int launch_rx(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8, const btle_stream_cfg *cfgs,
               const int32_t *cfg_capture, size_t n_cfgs, const int4 *rot, btle_pkt_rec *d_out, size_t cap, unsigned *d_count,
               btle_unit_dir *d_dir, cudaStream_t st, long long lead) {
@@ -2185,8 +2251,12 @@ int launch_rx(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t s
     zero_next = ctx->d_count_ring + (ctx->ring_pos + kCountRing / 2) % kCountRing;
   }
   const unsigned grid = (unsigned)std::min<long long>(plan.total_units, (long long)ctx->num_sms * kCtasPerSm);   // one persistent CTA per SM
-  const auto enqueue = multi ? (rot ? enqueue_rx<kMaxCfgsPerCapture, true> : enqueue_rx<kMaxCfgsPerCapture, false>)
-                             : (rot ? enqueue_rx<1, true> : enqueue_rx<1, false>);
+  // BTLE_CFG_SYMBOL_SPACED: validate_cfgs made every cfg of the launch agree on it
+  const bool sym = (cfgs[0].rssi & BTLE_CFG_SYMBOL_SPACED) != 0;
+  const auto enqueue = sym ? (multi ? (rot ? enqueue_rx<kMaxCfgsPerCapture, true, true> : enqueue_rx<kMaxCfgsPerCapture, false, true>)
+                                    : (rot ? enqueue_rx<1, true, true> : enqueue_rx<1, false, true>))
+                           : (multi ? (rot ? enqueue_rx<kMaxCfgsPerCapture, true, false> : enqueue_rx<kMaxCfgsPerCapture, false, false>)
+                                    : (rot ? enqueue_rx<1, true, false> : enqueue_rx<1, false, false>));
   enqueue(grid, st, ms, d_iq, stride, n_int8, cs, plan, d_out, (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu), d_count, d_dir, zero_next, lead);
   BTLE_CUDA(ctx, cudaGetLastError());
   if (ring) {                                                 // the position is taken only by a launch that was enqueued
@@ -2527,11 +2597,17 @@ int btle_b200_create(btle_b200_ctx **out, int cuda_device) {
   if (cudaMemcpyToSymbol(c_noise_thr, thr, sizeof thr) != cudaSuccess ||
       cudaMemcpyToSymbol(c_whiten_words, ww, sizeof ww) != cudaSuccess ||
       cudaMemcpyToSymbol(c_crc4, crc, sizeof crc) != cudaSuccess ||
-      cudaFuncSetAttribute(btle_rx_persistent_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem<1>)) != cudaSuccess ||
-      cudaFuncSetAttribute(btle_rx_persistent_kernel<kMaxCfgsPerCapture, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+      cudaFuncSetAttribute(btle_rx_persistent_kernel<1, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem<1>)) != cudaSuccess ||
+      cudaFuncSetAttribute(btle_rx_persistent_kernel<kMaxCfgsPerCapture, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            (int)sizeof(Smem<kMaxCfgsPerCapture>)) != cudaSuccess ||
-      cudaFuncSetAttribute(btle_rx_persistent_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem<1>)) != cudaSuccess ||
-      cudaFuncSetAttribute(btle_rx_persistent_kernel<kMaxCfgsPerCapture, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+      cudaFuncSetAttribute(btle_rx_persistent_kernel<1, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem<1>)) != cudaSuccess ||
+      cudaFuncSetAttribute(btle_rx_persistent_kernel<kMaxCfgsPerCapture, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (int)sizeof(Smem<kMaxCfgsPerCapture>)) != cudaSuccess ||
+      cudaFuncSetAttribute(btle_rx_persistent_kernel<1, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem<1>)) != cudaSuccess ||
+      cudaFuncSetAttribute(btle_rx_persistent_kernel<kMaxCfgsPerCapture, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (int)sizeof(Smem<kMaxCfgsPerCapture>)) != cudaSuccess ||
+      cudaFuncSetAttribute(btle_rx_persistent_kernel<1, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem<1>)) != cudaSuccess ||
+      cudaFuncSetAttribute(btle_rx_persistent_kernel<kMaxCfgsPerCapture, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            (int)sizeof(Smem<kMaxCfgsPerCapture>)) != cudaSuccess ||
       cudaFuncSetAttribute(sps8_hits_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSps8Smem) != cudaSuccess ||
       cudaFuncSetAttribute(discover_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDiscSmem) != cudaSuccess ||
@@ -3047,6 +3123,13 @@ int streams_index(btle_b200_streams *s, size_t stream) {
   s->ctx->err = "stream index out of range";
   return BTLE_EINVAL;
 }
+// a session decodes in the BTLE_CFG_SYMBOL_SPACED mode of the cfgs it was opened with (entries[0] keeps it), so every
+// round, backfill included, is one launch of one kernel variant
+int streams_check_mode(btle_b200_streams *s, const btle_stream_cfg *cfg) {
+  if (!((cfg->rssi ^ s->entries[0].cfg.rssi) & BTLE_CFG_SYMBOL_SPACED)) return BTLE_OK;
+  s->ctx->err = "a session's cfgs must all agree on BTLE_CFG_SYMBOL_SPACED (the mode of streams_open)";
+  return BTLE_EINVAL;
+}
 }  // namespace
 
 extern "C" {
@@ -3108,6 +3191,7 @@ int btle_b200_streams_set_cfg(btle_b200_streams *s, size_t stream, const btle_st
   if (rc) return rc;
   rc = validate_cfgs(s->ctx, cfg, 1);
   if (rc) return rc;
+  if ((rc = streams_check_mode(s, cfg))) return rc;
   s->entries[stream].cfg = *cfg;                            // used from the next submitted segment set on
   return BTLE_OK;
 }
@@ -3209,6 +3293,7 @@ int btle_b200_streams_add_cfg(btle_b200_streams *s, size_t capture, const btle_s
   if (rc) return rc;
   rc = validate_cfgs(s->ctx, cfg, 1);
   if (rc) return rc;
+  if ((rc = streams_check_mode(s, cfg))) return rc;
   if (from_chunk < streams_resident(s)) {
     s->ctx->err = "streams_add_cfg: from_chunk lies before the first resident chunk (btle_b200_streams_resident)";
     return BTLE_EINVAL;
@@ -3693,7 +3778,10 @@ static int check_rx_ber_cfg(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg) {
   }
   if (std::fabs(cfg->ppm) >= 1e6f) { ctx->err = "rx_ber: ppm must have |ppm| < 1e6"; return BTLE_EINVAL; }
   if (cfg->amplitude < 1 || cfg->amplitude > 127) { ctx->err = "rx_ber: amplitude must be 1..127"; return BTLE_EINVAL; }
-  if (cfg->flags & ~(uint32_t)BTLE_CFG_RECOVER) { ctx->err = "rx_ber: flags may only hold BTLE_CFG_RECOVER"; return BTLE_EINVAL; }
+  if (cfg->flags & ~(uint32_t)(BTLE_CFG_RECOVER | BTLE_CFG_SYMBOL_SPACED)) {
+    ctx->err = "rx_ber: flags may only hold BTLE_CFG_RECOVER and BTLE_CFG_SYMBOL_SPACED";
+    return BTLE_EINVAL;
+  }
   if (cfg->slot_samples < rx_ber_len(cfg->channel) || cfg->slot_samples > BTLE_RX_BER_MAX_SLOT) {
     ctx->err = "rx_ber: slot_samples must hold the packet (" + std::to_string(rx_ber_len(cfg->channel)) + " samples on this channel) and be at most " +
                std::to_string(BTLE_RX_BER_MAX_SLOT);
@@ -3780,8 +3868,14 @@ int btle_b200_rx_ber_run(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg, size_t 
   const long long B = std::max(1ll, want_chunks * kChunkSamples / (q * S)) * q;
   const size_t max_b = std::min<size_t>(n_packets, (size_t)B);
   const long long max_chunks = ((long long)max_b * S + kChunkSamples - 1) / kChunkSamples;
-  const size_t max_int8 = (size_t)max_chunks * kChunkInt8 + BTLE_LOOKAHEAD_INT8, max_recs = (size_t)max_chunks * BTLE_MAX_RECS_PER_CHUNK;
-  if (ctx->d_iq.reserve(ctx, max_int8) || ctx->d_out.reserve(ctx, max_recs) ||
+  // BTLE_CFG_SYMBOL_SPACED: d[n] reads samples n - 2 .. n + 2, so a batch is decoded with the 2 samples in front of it
+  // (kSymLead bytes of lead, the tail of the previous slot, synthesised again into `prev`) and 2 more behind its look-ahead
+  const bool sym = (cfg->flags & BTLE_CFG_SYMBOL_SPACED) != 0;
+  constexpr size_t kSymLead = 16;                            // keeps the capture 16-byte aligned
+  const size_t lead = sym ? kSymLead : 0, look = BTLE_LOOKAHEAD_INT8 + (sym ? 4 : 0);
+  const size_t max_int8 = (size_t)max_chunks * kChunkInt8 + look, max_recs = (size_t)max_chunks * BTLE_MAX_RECS_PER_CHUNK;
+  const size_t prev_at = (lead + max_int8 + 15) & ~size_t(15);
+  if (ctx->d_iq.reserve(ctx, sym ? prev_at + 2 * (size_t)S : max_int8) || ctx->d_out.reserve(ctx, max_recs) ||
       ctx->d_dir.reserve(ctx, (size_t)(max_chunks + kSpanChunks - 1) / kSpanChunks * kSpanChunks))   // >= units of any batch
     return BTLE_ENOMEM;
   btle_rx_ber_truth *d_truth;
@@ -3802,11 +3896,20 @@ int btle_b200_rx_ber_run(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg, size_t 
     const size_t n = std::min(max_b, n_packets - done);
     const bool last = done + n == n_packets;
     const long long chunks = ((long long)n * S + kChunkSamples - 1) / kChunkSamples;
-    const size_t n_int8 = (size_t)chunks * kChunkInt8 + (last ? 0 : BTLE_LOOKAHEAD_INT8);
-    rc = launch_rx_ber_synth(ctx, *cfg, done, n_packets, (long long)(n_int8 / 2), (long long)n, ctx->d_iq, d_truth, st);
+    const size_t n_int8 = (size_t)chunks * kChunkInt8 + (last ? 0 : look);
+    int8_t *d_cap = ctx->d_iq + lead;
+    if (sym && done == 0) BTLE_CUDA(ctx, cudaMemsetAsync(ctx->d_iq.p, 0, lead, st));   // nothing in front of the capture
+    if (sym && done > 0) {
+      int8_t *prev = ctx->d_iq + prev_at;                     // slot done - 1 alone (no truth row), its last lead bytes
+      rc = launch_rx_ber_synth(ctx, *cfg, done - 1, n_packets, S, 0, prev, d_truth, st);
+      if (rc) return rc;
+      BTLE_CUDA(ctx, cudaMemcpyAsync(ctx->d_iq.p, prev + 2 * S - lead, lead, cudaMemcpyDeviceToDevice, st));
+      ++launches;
+    }
+    rc = launch_rx_ber_synth(ctx, *cfg, done, n_packets, (long long)(n_int8 / 2), (long long)n, d_cap, d_truth, st);
     if (rc) return rc;
     const size_t cap = (size_t)chunks * BTLE_MAX_RECS_PER_CHUNK, units = btle_b200_rx_units(ctx, 1, n_int8);
-    rc = launch_rx(ctx, ctx->d_iq, 1, n_int8, n_int8, &scfg, nullptr, 1, nullptr, ctx->d_out, cap, ctx->d_count, ctx->d_dir, st, 0);
+    rc = launch_rx(ctx, d_cap, 1, n_int8, n_int8, &scfg, nullptr, 1, nullptr, ctx->d_out, cap, ctx->d_count, ctx->d_dir, st, (long long)lead);
     if (rc) return rc;
     rc = launch_rx_ber_score(ctx, d_truth, n, ctx->d_out, cap, ctx->d_dir, units, d_res, st);
     if (rc) return rc;

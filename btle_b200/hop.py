@@ -265,7 +265,7 @@ def follow_connections(rx, captures: np.ndarray, max_events: int = 10000, discov
     return adv, conns
 
 
-def decode_connections(rx, captures: np.ndarray, discover: bool = True, offset_hz=None):
+def decode_connections(rx, captures: np.ndarray, discover: bool = True, offset_hz=None, symbol_spaced: bool = False):
     """Every known connection's data-channel traffic, decoded without following it.  captures: int8 [40, n_int8] as in
     follow_connections(); `rx` needs rx_batch, rx_multi and, with discover=True, discover (a BtleRx).
     The connections are the CONNECT_REQ ones (tracked or not) plus, with discover=True, the discover_connections() ones
@@ -275,8 +275,9 @@ def decode_connections(rx, captures: np.ndarray, discover: bool = True, offset_h
     then channel).  Launches: one rx_batch over the advertising captures, one discover, and one rx_multi per
     MAX_CFGS_PER_CAPTURE connections over captures[0:37] (each capture is read once per call, whatever the number of
     connections in it).  offset_hz (a scalar or one per capture, None: no correction) is passed to those rx_batch and
-    rx_multi calls (carrier-offset correction); discovery reads the captures uncorrected.  Returns (adv_records,
-    connections)."""
+    rx_multi calls (carrier-offset correction); discovery reads the captures uncorrected.  symbol_spaced: every receive
+    cfg of those calls carries BTLE_CFG_SYMBOL_SPACED (the symbol-spaced discriminator); discovery keeps its own rule.
+    Returns (adv_records, connections)."""
     from ._native import MAX_CFGS_PER_CAPTURE
     captures = np.ascontiguousarray(captures, dtype=np.int8)
     assert captures.shape[0] == 40
@@ -284,7 +285,7 @@ def decode_connections(rx, captures: np.ndarray, discover: bool = True, offset_h
     off = None if offset_hz is None else np.broadcast_to(np.asarray(offset_hz, dtype=np.float32), (40,))
     adv_kw = {} if off is None else {"offset_hz": off[37:40]}
     data_kw = {} if off is None else {"offset_hz": off[0:37]}
-    adv = rx.rx_batch(captures[37:40], make_cfgs(3, channel=[37, 38, 39]), **adv_kw).copy()
+    adv = rx.rx_batch(captures[37:40], make_cfgs(3, channel=[37, 38, 39], symbol_spaced=symbol_spaced), **adv_kw).copy()
     adv["stream"] += 37
     conns = []
     for r in adv:
@@ -302,7 +303,7 @@ def decode_connections(rx, captures: np.ndarray, discover: bool = True, offset_h
         k = len(batch)
         # cfg j = channel * k + i: connection i on data channel j // k (the cfgs of one capture are adjacent)
         cfgs = make_cfgs(37 * k, channel=np.repeat(np.arange(37), k), access_addr=[c["access_addr"] for c in batch] * 37,
-                         crc_init=[c["crc_init"] for c in batch] * 37)
+                         crc_init=[c["crc_init"] for c in batch] * 37, symbol_spaced=symbol_spaced)
         rec = rx.rx_multi(captures[0:37], cfgs, np.repeat(np.arange(37, dtype=np.int32), k), **data_kw)
         owner = rec["stream"] % k
         t = rec["chunk"].astype(np.int64) * 8192 + rec["n0"]
@@ -452,13 +453,16 @@ class ConnectionMonitor:
     that has not reached min_events and has had no event for that long is forgotten, so that noise groups do not pile up
     over a long session (the default, 8 s, is twice the longest connection interval; a group paused longer than that
     starts again, where discover_connections() would continue it).  offset_hz (a scalar or one per capture): the
-    session's carrier-offset correction of each capture (RxStreams.set_offset), from the first set on."""
+    session's carrier-offset correction of each capture (RxStreams.set_offset), from the first set on.  symbol_spaced:
+    the connection cfgs carry BTLE_CFG_SYMBOL_SPACED; the session must have been opened with cfgs that carry it (a
+    session has one discriminator mode).  Discovery keeps its own rule."""
 
     N_CAPTURES = 40
 
     def __init__(self, session, min_events: int = 4, idle_s: float | None = None, discover: bool = True, group_s: float = 8.0,
-                 offset_hz=None):
+                 offset_hz=None, symbol_spaced: bool = False):
         self.session, self.min_events, self.idle_s, self.group_s = session, int(min_events), idle_s, group_s
+        self._symbol_spaced = bool(symbol_spaced)
         if offset_hz is not None:
             for c, hz in enumerate(np.broadcast_to(np.asarray(offset_hz, dtype=np.float32), (self.N_CAPTURES,))):
                 session.set_offset(c, float(hz))
@@ -523,7 +527,8 @@ class ConnectionMonitor:
         from ._native import REC_DTYPE
         c["_traffic"] = [np.zeros(0, dtype=REC_DTYPE)]
         for ch in range(37):
-            j, _ = s.add_cfg(ch, frm, channel=ch, access_addr=c["access_addr"], access_mask=0xFFFFFFFF, crc_init=c["crc_init"], raw=0, rssi=0)
+            j, _ = s.add_cfg(ch, frm, channel=ch, access_addr=c["access_addr"], access_mask=0xFFFFFFFF, crc_init=c["crc_init"], raw=0, rssi=0,
+                           symbol_spaced=self._symbol_spaced)
             c["_cfgs"].append(j)
             self._owner[j] = c
         return 37

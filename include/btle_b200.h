@@ -69,7 +69,8 @@ typedef struct {
                             length is outside 6..37 — the reference prints "PktBAD" for them under -v and does not
                             count them (:2291-2298) — come back as records with BTLE_REC_REJECTED set, every one
                             of them, in the reference's order (up to BTLE_MAX_RECS_PER_CHUNK records per chunk);
-                            BTLE_CFG_RECOVER 4: CRC-failed packets are demodulated once more (below)            */
+                            BTLE_CFG_RECOVER 4: CRC-failed packets are demodulated once more (below);
+                            BTLE_CFG_SYMBOL_SPACED 16: the symbol-spaced discriminator (below)                   */
 } btle_stream_cfg;
 #define BTLE_CFG_RSSI 1
 #define BTLE_CFG_REPORT_REJECTED 2
@@ -93,6 +94,22 @@ typedef struct {
  * Rejected (BTLE_CFG_REPORT_REJECTED) records, raw-mode records and CRC-ok records are never touched; the flag does
  * nothing in raw mode. */
 #define BTLE_CFG_RECOVER 4
+/* BTLE_CFG_SYMBOL_SPACED: opt-in symbol-spaced discriminator.  Not part of the reference's receiver; without it the records
+ * are the reference's, bit for bit.  With it every discriminator bit of the capture is
+ *     d[n] = I[n-2] Q[n+2] - I[n+2] Q[n-2] > 0      (int32; x[n] = sample n of the capture)
+ * a phase step over one symbol (+-pi/2 nominal) instead of a quarter symbol, centred on n as the reference's bit is centred
+ * on n + 1/2, so n0, mag_sum, the BER scorer's +-3-sample match and btle_b200_rec_offset keep their meaning.  Samples in
+ * front of the capture read as 0 unless the launch makes them readable (the stream sessions keep 256 bytes of the previous
+ * segment set in front of each set), samples behind its end read as 0: a chunk's bits are a function of the capture, not
+ * of how it was cut.  d[n] equals BTLE_CFG_RECOVER's alternative q = 0 bit e[n - 2] (which reads only its chunk window).
+ * With carrier-offset correction (the *_offset entry points) the bit is rotated by (C4, S4) from 4 phi:
+ *     d[n] = C4 (I[n-2] Q[n+2] - I[n+2] Q[n-2]) - S4 (I[n-2] I[n+2] + Q[n-2] Q[n+2]) > 0.
+ * Everything the chain derives from d follows unchanged: the access-address search, the greedy chain and its length guards,
+ * dewhitening, the CRC, -v rejected hits, BTLE_MAX_RECS_PER_CHUNK; BTLE_CFG_RECOVER keeps its own alternatives.
+ * One mode per launch: every cfg of one rx_batch / rx_multi / device call must agree on this flag, else BTLE_EINVAL (with
+ * last_error set).  A stream session's mode is that of the cfgs given to streams_open; a set_cfg or add_cfg with the other
+ * value is BTLE_EINVAL.  btle_rx_ber_cfg.flags accepts it too. */
+#define BTLE_CFG_SYMBOL_SPACED 16
 /* Carrier-offset correction: the *_offset entry points take one float offset_hz per capture, the received carrier minus
  * the nominal one in Hz (the sign of btle_rx_ber_cfg.cfo_hz: correcting by cfo_hz undoes that impairment).  Not part of the
  * reference's receiver.  With phi = 2 pi offset_hz / 4 MHz and C = round(2^14 cos phi), S = round(2^14 sin phi) (nearest,
@@ -542,7 +559,8 @@ typedef struct {
   int32_t channel;         /* 0..39                                                                                 */
   uint32_t access_addr;
   uint32_t crc_init;       /* as -k                                                                                 */
-  uint32_t flags;          /* 0 or BTLE_CFG_RECOVER (given to the receiver); any other bit: BTLE_EINVAL             */
+  uint32_t flags;          /* BTLE_CFG_RECOVER and / or BTLE_CFG_SYMBOL_SPACED (given to the receiver); any other
+                              bit: BTLE_EINVAL                                                                        */
   uint32_t reserved;       /* 0                                                                                     */
 } btle_rx_ber_cfg;         /* 48 bytes */
 typedef struct {
@@ -566,9 +584,11 @@ typedef struct {
   double seconds;          /* device time of the run (CUDA events)                                                   */
 } btle_rx_ber_result;      /* 88 bytes */
 /* n_packets packets 0 .. n_packets-1, in batches sized from free device memory; the result is independent of the batch
- * size (every batch starts on a chunk and slot boundary, and its look-ahead behind the last chunk is the next slots').
+ * size (every batch starts on a chunk and slot boundary, and its look-ahead behind the last chunk is the next slots'; with
+ * BTLE_CFG_SYMBOL_SPACED a batch also reads the 2 samples in front of it and 2 more behind its look-ahead).
  * BTLE_EINVAL with btle_b200_last_error() for: snr_db, ppm or cfo_hz NaN or infinite, |ppm| >= 1e6, amplitude outside
- * 1..127, slot_samples below L or above BTLE_RX_BER_MAX_SLOT, channel > 39, a flags bit other than BTLE_CFG_RECOVER;
+ * 1..127, slot_samples below L or above BTLE_RX_BER_MAX_SLOT, channel > 39, a flags bit other than BTLE_CFG_RECOVER and
+ * BTLE_CFG_SYMBOL_SPACED;
  * the context stays usable. */
 int btle_b200_rx_ber_run(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg, size_t n_packets, btle_rx_ber_result *out);
 /* the capture and truth of packets first_packet .. first_packet + n_packets - 1 alone: d_iq (16-byte aligned) receives

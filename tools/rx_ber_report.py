@@ -2,9 +2,11 @@
 (btle_b200_ber_run) at the same SNR and ppm, plus the 4-Msps receiver under extra carrier offsets, and where the time of
 rx_ber_run goes (CUDA events around its three kernels on one batch).
 
-    python tools/rx_ber_report.py [--packets N] [--json out.json] [--recover]
+    python tools/rx_ber_report.py [--packets N] [--json out.json] [--recover] [--symbol-spaced] [--snrs 8:31] [--no-cfo]
 
 --recover adds the 4-sps PER / BER with BTLE_CFG_RECOVER (CRC-failed packets demodulated again) next to the plain ones.
+--symbol-spaced adds them with BTLE_CFG_SYMBOL_SPACED (the symbol-spaced discriminator), and with --recover also with both.
+--snrs LO:HI sweeps SNR LO .. HI-1 dB (default -5:31); --no-cfo leaves out the extra-carrier-offset rows.
 
 Prints a markdown table (one row per point) and the throughput of both flows."""
 import argparse
@@ -60,28 +62,37 @@ def main():
     ap.add_argument("--packets", type=int, default=20000)
     ap.add_argument("--json", default=None)
     ap.add_argument("--recover", action="store_true", help="also measure the receiver with BTLE_CFG_RECOVER")
+    ap.add_argument("--symbol-spaced", action="store_true", help="also measure the receiver with BTLE_CFG_SYMBOL_SPACED")
+    ap.add_argument("--snrs", default="-5:31", help="LO:HI, SNR points LO .. HI-1 dB")
+    ap.add_argument("--no-cfo", action="store_true", help="leave out the extra-carrier-offset rows")
     args = ap.parse_args()
     rx = BtleRx(0)
-    snrs = list(range(-5, 31))             # the 4-sps receiver's curve falls between 15 and 30 dB
+    lo, hi = (int(v) for v in args.snrs.split(":"))
+    snrs = list(range(lo, hi))             # the 4-sps receiver's curve falls between 15 and 30 dB
+    # the 4-sps variants: (key, recover, symbol_spaced)
+    ways = [("rx4_recover", True, False)] if args.recover else []
+    if args.symbol_spaced:
+        ways += [("rx4_symbol", False, True)] + ([("rx4_symbol_recover", True, True)] if args.recover else [])
     rows = []
     for ppm in (0.0, 20.0, 50.0):
         r4 = ber.rx_ber_sweep(snrs, args.packets, ppm=ppm, rx=rx)
         r8 = ber.ber_sweep(snrs, args.packets, ppm=ppm, rx=rx)
-        rr = ber.rx_ber_sweep(snrs, args.packets, ppm=ppm, rx=rx, recover=True) if args.recover else [None] * len(r4)
-        for a, b, c in zip(r4, r8, rr):
-            rows.append({"ppm": ppm, "cfo_hz": 0.0, "rx4": a, "model8": b, "rx4_recover": c})
-    for cfo in (25e3, 50e3, 100e3, 150e3):
+        rw = {k: ber.rx_ber_sweep(snrs, args.packets, ppm=ppm, rx=rx, recover=rc, symbol_spaced=sy) for k, rc, sy in ways}
+        for i, (a, b) in enumerate(zip(r4, r8)):
+            rows.append({"ppm": ppm, "cfo_hz": 0.0, "rx4": a, "model8": b, **{k: v[i] for k, v in rw.items()}})
+    for cfo in () if args.no_cfo else (25e3, 50e3, 100e3, 150e3):
         r4 = ber.rx_ber_sweep(snrs, args.packets, cfo_hz=cfo, rx=rx)
-        rr = ber.rx_ber_sweep(snrs, args.packets, cfo_hz=cfo, rx=rx, recover=True) if args.recover else [None] * len(r4)
-        for a, c in zip(r4, rr):
-            rows.append({"ppm": 0.0, "cfo_hz": cfo, "rx4": a, "model8": None, "rx4_recover": c})
-    rec_h = " 4-sps PER recover | 4-sps BER recover |" if args.recover else ""
-    print(f"| ppm | cfo kHz | SNR dB | 4-sps PER | 4-sps BER |{rec_h} aa_miss | len_reject | extra | 8-sps model PER | 8-sps model BER |")
-    print("|---:|---:|---:|---:|---:|" + ("---:|---:|" if args.recover else "") + "---:|---:|---:|---:|---:|")
+        rw = {k: ber.rx_ber_sweep(snrs, args.packets, cfo_hz=cfo, rx=rx, recover=rc, symbol_spaced=sy) for k, rc, sy in ways}
+        for i, a in enumerate(r4):
+            rows.append({"ppm": 0.0, "cfo_hz": cfo, "rx4": a, "model8": None, **{k: v[i] for k, v in rw.items()}})
+    label = {"rx4_recover": "recover", "rx4_symbol": "symbol", "rx4_symbol_recover": "symbol+recover"}
+    extra_h = "".join(f" 4-sps PER {label[k]} | 4-sps BER {label[k]} | aa_miss {label[k]} |" for k, _, _ in ways)
+    print(f"| ppm | cfo kHz | SNR dB | 4-sps PER | 4-sps BER |{extra_h} aa_miss | len_reject | extra | 8-sps model PER | 8-sps model BER |")
+    print("|---:|---:|---:|---:|---:|" + "---:|---:|---:|" * len(ways) + "---:|---:|---:|---:|---:|")
     for r in rows:
-        a, b, c = r["rx4"], r["model8"], r["rx4_recover"]
+        a, b = r["rx4"], r["model8"]
         m = f"{b['per']:.4f} | {b['ber']:.2e}" if b else "- | -"
-        rc = f" {c['per']:.4f} | {c['ber']:.2e} |" if c else ""
+        rc = "".join(f" {r[k]['per']:.4f} | {r[k]['ber']:.2e} | {r[k]['aa_miss']} |" for k, _, _ in ways)
         print(f"| {r['ppm']:g} | {r['cfo_hz'] / 1e3:g} | {a['snr_db']:g} | {a['per']:.4f} | {a['ber']:.2e} |{rc} {a['aa_miss']} | {a['len_reject']} | "
               f"{a['extra_recs']} | {m} |")
     r4 = [r["rx4"] for r in rows]
