@@ -1040,7 +1040,8 @@ __global__ void rec_offset_kernel(const int8_t *__restrict__ iq, long long strid
   const int stream = recs[r].stream, chunk = recs[r].chunk, n0 = recs[r].n0;
   const uint32_t aa = recs[r].access_addr;
   const uint8_t sb[5] = {(uint8_t)((aa & 1u) ? 0x55 : 0xAA), (uint8_t)aa, (uint8_t)(aa >> 8), (uint8_t)(aa >> 16), (uint8_t)(aa >> 24)};
-  const IqWindow w = iq_window(iq + (long long)stream * stride, n_int8, chunk);
+  IqWindow w = iq_window(iq + (long long)stream * stride, n_int8, chunk);
+  if (chunk < 0) w.n = 0;                                   // records come from the caller: never read in front of the row
   const int m_first = BTLE_RX_BER_AA_OFFSET - kOffLead;
   int ph = 0, m = 0;                                        // phase before frequency word m of the reference
   float sum = 0.0f;
@@ -2710,8 +2711,10 @@ int btle_b200_rec_offset_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t s
 int btle_b200_rec_offset(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stride, size_t n_int8, const btle_pkt_rec *recs, size_t n,
                          float *hz) {
   if (!ctx || (n && (!recs || !hz)) || (!iq && n_streams && n_int8)) return BTLE_EINVAL;
-  for (size_t i = 0; i < n; ++i)
+  for (size_t i = 0; i < n; ++i) {
     if (recs[i].stream < 0 || (size_t)recs[i].stream >= n_streams) { ctx->err = "rec_offset: record stream out of range"; return BTLE_EINVAL; }
+    if (recs[i].chunk < 0) { ctx->err = "rec_offset: record chunk negative"; return BTLE_EINVAL; }
+  }
   if (!n) return BTLE_OK;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;

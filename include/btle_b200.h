@@ -261,7 +261,9 @@ int btle_b200_rx_multi_device_dir_offset(btle_b200_ctx *ctx, const int8_t *d_iq,
  * samples) of the packet's preamble and access address, tx sample BTLE_RX_BER_AA_OFFSET at n0: the preamble and access
  * address, up to 4 samples before the header, whose first bit the Gaussian filter lets into later turns.  So a noiseless
  * packet of the project's own transmitter, aligned, estimates 0.  Device form: d_iq (captures stride apart), d_recs and
- * d_hz device pointers, enqueued on cuda_stream, one warp per record; host form: host buffers, synchronised. */
+ * d_hz device pointers, enqueued on cuda_stream, one warp per record; a record with chunk < 0 reads no sample (every
+ * sample 0), so it never reads in front of its capture.  Host form: host buffers, synchronised; BTLE_EINVAL (and
+ * btle_b200_last_error set) for a record whose stream is outside [0, n_streams) or whose chunk is negative. */
 int btle_b200_rec_offset_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t stream_stride_int8, size_t n_int8, const btle_pkt_rec *d_recs,
                                 size_t n, float *d_hz, void *cuda_stream);
 int btle_b200_rec_offset(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stream_stride_int8, size_t n_int8,

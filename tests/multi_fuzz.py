@@ -6,9 +6,12 @@ A draw: 1..max_captures captures of k x 16384 + {0, 1, 2, 255, 256, 3007, 3008, 
 (some captures no cfg names), each cfg with its own channel 0..39, access address, mask of popcount 0..32, 24-bit CRC
 init, raw about a quarter of the time and flags 0..3.  Captures are uniform noise, +-1 values, all zeros (with mask 0
 and -v the worst case of 123 records per chunk), a short periodic pattern, or bursts of the capture's own cfgs' access
-addresses over a low noise floor: across chunk boundaries, cut by both ends of the capture, some with a corrupted CRC."""
+addresses over a low noise floor: across chunk boundaries, cut by both ends of the capture, some with a corrupted CRC.
+draw_mode() puts a draw in a mode (ROT, SYM) of tests/mode_ref.py: every cfg symbol-spaced or not and, with ROT, every
+capture at an offset of its own, rotated onto it."""
 import numpy as np
 
+import mode_ref
 from btle_b200 import synth
 from btle_b200._native import MAX_CFGS_PER_CAPTURE
 from btle_b200.rx import make_cfgs
@@ -77,3 +80,10 @@ def draw(rng, max_captures=40, max_chunks=24):
             if mine.size:
                 _bursts(rng, iq[s], cfgs[mine])
     return iq, cfgs, capture
+
+
+def draw_mode(rng, mode, **kw):
+    """(iq, cfgs, capture, offsets): a draw() in `mode`; offsets (Hz per capture) are None unless the mode has ROT."""
+    iq, cfgs, capture = draw(rng, **kw)
+    offsets = mode_ref.draw_offsets(rng, iq.shape[0], mode)
+    return mode_ref.rotate_all(iq, offsets), mode_ref.with_mode(cfgs, mode), capture, offsets

@@ -6,6 +6,7 @@ import pytest
 import torch
 
 import golden_util as G
+import mode_ref
 import orc
 from btle_b200 import BtleRx, make_cfgs, synth
 
@@ -129,6 +130,17 @@ def test_gpu_randomised_configs_with_planted_bursts(rx):
 def test_gpu_many_short_streams(rx):
     """Hundreds of 1-3 chunk captures: spans with fewer tiles than dense warps, a parameter
     refresh at every span, more CTAs than spans and the opposite."""
+    _many_short_streams(rx, (0, 0))
+
+
+@pytest.mark.parametrize("mode", mode_ref.NEW_MODES, ids=mode_ref.mode_id)
+def test_gpu_many_short_streams_in_modes(rx, mode):
+    """The same with the rotated and symbol-spaced kernels against tests/mode_ref.py, every capture at its own offset
+    (distinct from its neighbours'), so a unit that took another capture's rotation would decode wrong bits."""
+    _many_short_streams(rx, mode)
+
+
+def _many_short_streams(rx, mode):
     rng = np.random.default_rng(21)
     for n_streams, nchunks in ((5, 1), (300, 2), (700, 3)):
         n = nchunks * 16384 + 4000
@@ -143,8 +155,14 @@ def test_gpu_many_short_streams(rx):
                 iq[s] = rng.integers(-128, 128, n, dtype=np.int8)
                 cfgs[s]["access_mask"] = 0x0000FFFF if s % 2 else 0x80000001
             cfgs[s]["channel"], cfgs[s]["rssi"] = ch, s % 4
-            exp.append(orc.rx_flags(iq[s], s % 4, channel=ch, access_mask=int(cfgs[s]["access_mask"]), stream=s))
-        got = rx.rx_batch(iq, cfgs)
+            if mode == (0, 0):
+                exp.append(orc.rx_flags(iq[s], s % 4, channel=ch, access_mask=int(cfgs[s]["access_mask"]), stream=s))
+        if mode != (0, 0):
+            offsets = mode_ref.draw_offsets(rng, n_streams, mode)
+            iq, cfgs = mode_ref.rotate_all(iq, offsets), mode_ref.with_mode(cfgs, mode)
+            exp = [mode_ref.rx_multi(iq, cfgs, np.arange(n_streams), offsets)]
+            assert (exp[0]["crc_bad"] == 0).sum() > n_streams
+        got = rx.rx_batch(iq, cfgs, offset_hz=None if mode == (0, 0) else offsets)
         _same(got, np.concatenate(exp))
 
 

@@ -20,6 +20,7 @@ import numpy as np
 import pytest
 import torch
 
+import mode_ref
 import orc
 from btle_b200 import CAND_DTYPE, DIR_DTYPE, REC_DTYPE, make_cfgs, synth
 from btle_b200._native import BTLE_EOVERFLOW
@@ -340,8 +341,25 @@ def _walk(rx, d_out, d_dir, units):
 @pytest.mark.parametrize("n_int8", LENGTHS)
 def test_rx_device_dir_poisoned_views(rx, n_int8):
     """Every byte outside [0, n_int8) of a view is poison; records == the oracle on the capture with zeros around it."""
+    _poisoned_views(rx, n_int8, (0, 0))
+
+
+@pytest.mark.parametrize("mode", mode_ref.NEW_MODES, ids=mode_ref.mode_id)
+@pytest.mark.parametrize("n_int8", LENGTHS)
+def test_rx_device_dir_poisoned_views_in_modes(rx, n_int8, mode):
+    """The same with the rotated and symbol-spaced one-cfg kernels, each capture at its own offset, against
+    tests/mode_ref.py: the symbol-spaced loop's word in front of a capture's first tile lies in the poison."""
+    _poisoned_views(rx, n_int8, mode)
+
+
+def _poisoned_views(rx, n_int8, mode):
     rng = np.random.default_rng(n_int8)
     iqs, cfgs, exp = _batch(n_int8, 4, seed=n_int8 % 1013)
+    offsets = mode_ref.draw_offsets(np.random.default_rng(n_int8 + 5), 4, mode)
+    if mode != (0, 0):
+        iqs = list(mode_ref.rotate_all(np.stack(iqs), offsets))
+        cfgs = mode_ref.with_mode(cfgs, mode)
+        exp = mode_ref.rx_multi(np.stack(iqs), cfgs, np.arange(4), offsets)
     assert ((exp["chunk"] == 0) & (exp["n0"] == -124)).any() and ((exp["chunk"] == 0) & (exp["n0"] < 0) & ((exp["flags"] & 4) == 0)).any()
     st = torch.cuda.current_stream().cuda_stream
     for ns in (1, 4):
@@ -353,7 +371,7 @@ def test_rx_device_dir_poisoned_views(rx, n_int8):
             d_out = torch.zeros(max(len(want), 1) * 64, dtype=torch.uint8, device="cuda")
             d_dir = torch.zeros((units, 2), dtype=torch.int32, device="cuda")
             d_count = torch.zeros(1, dtype=torch.int32, device="cuda")
-            rx.rx_device_dir(view, cfgs[:ns], d_out, d_count, d_dir, st)
+            rx.rx_device_dir(view, cfgs[:ns], d_out, d_count, d_dir, st, offset_hz=None if offsets is None else offsets[:ns])
             torch.cuda.synchronize()
             assert int(d_count.item()) == len(want)
             got, _ = _walk(rx, d_out, d_dir, units)

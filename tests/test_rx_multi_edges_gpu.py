@@ -11,6 +11,10 @@ zeros around it (oracle_multi), byte for byte:
 5. poisoned device views at every tile mode, and host captures copied from every kind of host memory, only the named
    ones, in runs.
 
+2, 3, 4 and 5 also run in each mode the default kernels do not reach (tests/mode_ref.py): carrier-offset correction with
+an offset of its own on every capture, the symbol-spaced discriminator, and both, against mode_ref.rx_multi, so that
+every instantiation btle_rx_persistent_kernel<1|8, ROT, SYM> meets the spans and reuse regimes of the unit plan.
+
 RSSI is on (flags 1 or 3) wherever bytes outside a capture could be read, so a stray read shows in mag_sum."""
 import ctypes
 import os
@@ -23,8 +27,9 @@ import pytest
 import torch
 
 from btle_b200 import CFG_DTYPE, DIR_DTYPE, REC_DTYPE, make_cfgs, synth
-from btle_b200._native import BTLE_EOVERFLOW
-from test_ingest_edges_gpu import CHUNK, LENGTHS, SEG, SOURCES, HostBuf, _capture, _device_view, _plan, _poison, _same
+from btle_b200._native import BTLE_EOVERFLOW, CFG_RECOVER
+import mode_ref
+from test_ingest_edges_gpu import CHUNK, LENGTHS, SEG, SOURCES, HostBuf, _capture, _device_view, _plan, _poison, _same, _walk
 from test_rx_multi import _traffic, oracle_multi
 
 pytestmark = pytest.mark.gpu
@@ -81,29 +86,31 @@ def _per_entry(exp, capture, plan, per):
     return out
 
 
-def _launch(rx, d_iq, cfgs, capture, cap, room, with_count):
-    """One btle_b200_rx_multi_device_dir launch with record capacity `cap` into `room` records of CANARY bytes; the directory
-    and counter start as -1.  Returns (record bytes [room, 64], directory, counter or None)."""
+def _launch(rx, d_iq, cfgs, capture, cap, room, with_count, offsets=None):
+    """One btle_b200_rx_multi_device_dir(_offset) launch with record capacity `cap` into `room` records of CANARY bytes;
+    the directory and counter start as -1.  Returns (record bytes [room, 64], directory, counter or None)."""
     ns, n = d_iq.shape
     cc = np.ascontiguousarray(capture, dtype=np.int32)
+    off = None if offsets is None else np.ascontiguousarray(offsets, dtype=np.float32)
     units = rx.multi_units(ns, cc, n)
     d_out = torch.full((room, 64), CANARY, dtype=torch.uint8, device="cuda")
     d_dir = torch.full((units, 2), -1, dtype=torch.int32, device="cuda")
     d_count = torch.full((1,), -1, dtype=torch.int32, device="cuda") if with_count else None
-    rx._check(rx._L.btle_b200_rx_multi_device_dir(rx._h, d_iq.data_ptr(), ns, d_iq.stride(0), n, cfgs.ctypes.data, cc.ctypes.data, cfgs.size,
-                                                  d_out.data_ptr(), cap, d_count.data_ptr() if with_count else None, d_dir.data_ptr(), units,
-                                                  ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
+    rx._check(rx._L.btle_b200_rx_multi_device_dir_offset(rx._h, d_iq.data_ptr(), ns, d_iq.stride(0), n, cfgs.ctypes.data, cc.ctypes.data,
+                                                         cfgs.size, None if off is None else off.ctypes.data, d_out.data_ptr(), cap,
+                                                         d_count.data_ptr() if with_count else None, d_dir.data_ptr(), units,
+                                                         ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
     torch.cuda.synchronize()
     ud = np.ascontiguousarray(d_dir.cpu().numpy().view(np.uint32)).view(DIR_DTYPE).reshape(-1)
     return d_out.cpu().numpy(), ud, int(d_count.item()) if with_count else None
 
 
-def _check_launch(rx, d_iq, cfgs, capture, exp, plan, per, cap, with_count):
+def _check_launch(rx, d_iq, cfgs, capture, exp, plan, per, cap, with_count, offsets=None):
     """A launch with capacity `cap` (<= the record count): nothing at or behind cap is written; the counter and the
     directory count every record; entry j * per + u holds cfg j's records of unit u (those below cap); blocks tile
     [0, total); gather_ordered returns the stored records in order, and BTLE_EOVERFLOW when some were cut."""
     total = len(exp)
-    host, ud, count = _launch(rx, d_iq, cfgs, capture, cap, total + 64, with_count)
+    host, ud, count = _launch(rx, d_iq, cfgs, capture, cap, total + 64, with_count, offsets)
     assert (host[cap:] == CANARY).all(), f"cap {cap}: records stored at or behind cap"
     recs = host.reshape(-1).view(REC_DTYPE)
     if with_count:
@@ -168,30 +175,43 @@ def _mixed_cfgs():
                      rssi=[1, 3, 3, 1, 3], raw=[0, 0, 0, 1, 0])
 
 
-@pytest.fixture(scope="module")
-def worst():
-    """Captures [zero, zero, traffic on channel 37], cfgs [8 rejected-hit cfgs, 8 counted-packet cfgs, the mixed five]."""
+def _worst(mode):
+    """Captures [zero, zero, traffic on channel 37], cfgs [8 rejected-hit cfgs, 8 counted-packet cfgs, the mixed five], in
+    `mode`, where the -v cfgs also recover and the traffic capture sits at its own offset.  (iq, cfgs, capture, exp, offsets)."""
     iq = np.zeros((3, N_WORST), dtype=np.int8)
     iq[2] = _traffic(N_WORST, [37], AAS[:5], seed=29)[0]
     cfgs = np.concatenate([_rejected_cfgs(), _counted_cfgs(), _mixed_cfgs()])
     capture = np.repeat(np.arange(3, dtype=np.int32), [8, 8, 5])
-    exp = oracle_multi(iq, cfgs, capture)
+    offsets = mode_ref.draw_offsets(np.random.default_rng(3 + mode[1]), 3, mode)
+    if mode != (0, 0):
+        cfgs = mode_ref.with_mode(cfgs, mode)
+        cfgs["rssi"] |= np.where(cfgs["rssi"] & 2, CFG_RECOVER, 0).astype(np.int32)
+        iq = mode_ref.rotate_all(iq, offsets)
+    exp = mode_ref.rx_multi(iq, cfgs, capture, offsets)
     per_cfg = np.bincount(exp["stream"], minlength=len(cfgs))
     assert (per_cfg[:8] == 20 * 123).all() and (per_cfg[8:16] == 20 * 51).all()
     assert (exp["stream"] == 17).sum() > 20 * 5 and ((exp["stream"] >= 16) & (exp["crc_bad"] == 0) & (exp["stream"] != 17)).sum() > 10
-    return iq, cfgs, capture, exp
+    return iq, cfgs, capture, exp, offsets
+
+
+@pytest.fixture(scope="module")
+def worst():
+    return _worst((0, 0))[:4]
+
+
+def _densities(rx, iq, cfgs, capture, exp, offsets=None):
+    assert len(exp) > len(cfgs) * 20 * 34 + 16
+    _same(rx.rx_multi(iq, cfgs, capture, offset_hz=offsets), exp)
+    d_iq = _device(iq)
+    plan, per = _multi_plan(rx, 3, capture, N_WORST)
+    for with_count in (True, False):
+        _check_launch(rx, d_iq, cfgs, capture, exp, plan, per, len(exp), with_count, offsets)
 
 
 def test_worst_case_densities_host_and_device(rx, worst):
     """rx_multi (its default capacity of 34 per chunk overflows: one retry at the exact count) and rx_multi_device_dir with a
     counter and with the counter ring, the directory checked entry by entry."""
-    iq, cfgs, capture, exp = worst
-    assert len(exp) > len(cfgs) * 20 * 34 + 16
-    _same(rx.rx_multi(iq, cfgs, capture), exp)
-    d_iq = _device(iq)
-    plan, per = _multi_plan(rx, 3, capture, N_WORST)
-    for with_count in (True, False):
-        _check_launch(rx, d_iq, cfgs, capture, exp, plan, per, len(exp), with_count)
+    _densities(rx, *worst)
 
 
 @pytest.mark.parametrize("seg", [1, 16])
@@ -246,6 +266,10 @@ def _regime(G, name):
 
 @pytest.mark.parametrize("regime", ["pieces1", "pieces4", "spans", "reuse"])
 def test_every_unit_plan(rx, regime):
+    _every_unit_plan(rx, regime, (0, 0))
+
+
+def _every_unit_plan(rx, regime, mode):
     G = _sms()
     groups, n = _regime(G, regime)
     counts = []
@@ -254,6 +278,10 @@ def test_every_unit_plan(rx, regime):
     d_iq, ch = _spliced(len(counts), n, seed=len(counts) * 7 + n % 1000)
     iq = d_iq.cpu().numpy()
     rng = np.random.default_rng(n)
+    offsets = mode_ref.draw_offsets(np.random.default_rng(n + 1), len(counts), mode)
+    if offsets is not None:
+        iq = mode_ref.rotate_all(iq, offsets)
+        d_iq = _device(iq)
     cfgs, capture = [], []
     for c, k in enumerate(counts):
         for a in rng.permutation(8)[:k]:
@@ -261,17 +289,41 @@ def test_every_unit_plan(rx, regime):
                                   access_mask=int(rng.choice([0xFFFFFFFF, 0xFFFFFFFF, 0xFFFF00FF, 0xFFFFFFF0, 0x7FFFFFFE])),
                                   rssi=int(rng.choice([1, 3, 1, 3, 0, 2]))))
             capture.append(c)
-    cfgs, capture = np.concatenate(cfgs), np.array(capture, dtype=np.int32)
+    cfgs, capture = mode_ref.with_mode(np.concatenate(cfgs), mode), np.array(capture, dtype=np.int32)
     plan, per = _multi_plan(rx, len(counts), capture, n)
     spans = -(-(n // CHUNK) // 16)
     S = groups * spans
     assert plan[:, 2].max() == {"pieces1": 1, "pieces4": 4, "spans": 16, "reuse": 16}[regime]
     assert {"pieces1": S < G / 4, "pieces4": G / 4 <= S < G, "spans": G <= S <= 4 * G, "reuse": S > 4 * G}[regime]
-    exp = oracle_multi(iq, cfgs, capture)
+    exp = mode_ref.rx_multi(iq, cfgs, capture, offsets)
     per_cfg = np.bincount(exp["stream"], minlength=len(cfgs))
     assert (per_cfg[cfgs["access_mask"] == 0xFFFFFFFF] > 0).all() and len(exp) > 4 * len(cfgs)
     for with_count in (True, False):
-        _check_launch(rx, d_iq, cfgs, capture, exp, plan, per, len(exp), with_count)
+        _check_launch(rx, d_iq, cfgs, capture, exp, plan, per, len(exp), with_count, offsets)
+    if mode == (0, 0):
+        return
+    # <1, ROT, SYM>: one cfg per capture (the first its list would hold, an exact mask), rx_batch and rx_device_dir
+    ones = mode_ref.with_mode(make_cfgs(len(counts), channel=ch, access_addr=[AAS[c % 8] for c in range(len(counts))],
+                                        crc_init=[CRCS[c % 8] for c in range(len(counts))], rssi=[1, 3] * (len(counts) // 2) + [1] * (len(counts) % 2)),
+                              mode)
+    exp1 = mode_ref.rx_multi(iq, ones, np.arange(len(counts)), offsets)
+    assert (np.bincount(exp1["stream"], minlength=len(counts)) > 0).all()
+    _same(rx.rx_batch(iq, ones, offset_hz=offsets), exp1)
+    units = rx.units(len(counts), n)
+    assert units == len(_plan(rx, len(counts), n))
+    d_out = torch.zeros(len(exp1) * 64 + 64, dtype=torch.uint8, device="cuda")
+    d_dir = torch.zeros((units, 2), dtype=torch.int32, device="cuda")
+    rx.rx_device_dir(d_iq, ones, d_out, None, d_dir, torch.cuda.current_stream().cuda_stream, offset_hz=offsets)
+    torch.cuda.synchronize()
+    _same(_walk(rx, d_out, d_dir, units)[0], exp1)
+
+
+@pytest.mark.parametrize("mode", mode_ref.NEW_MODES, ids=mode_ref.mode_id)
+@pytest.mark.parametrize("regime", ["pieces1", "pieces4", "spans", "reuse"])
+def test_every_unit_plan_in_modes(rx, regime, mode):
+    """Every regime with the rotated and symbol-spaced kernels: the multi-cfg kernel <8, ROT, SYM> (the cfg list is not
+    the identity) and the one-cfg kernel <1, ROT, SYM> through rx_batch and rx_device_dir on the same captures."""
+    _every_unit_plan(rx, regime, mode)
 
 
 # ---- 4. capacity cuts inside units -----------------------------------------------------------------------------------------
@@ -280,31 +332,48 @@ def test_capacity_cut_inside_units(rx, worst):
     are block boundaries whatever the order the blocks are reserved in; cuts at 0 and 1, at a boundary, inside a block's
     hit row (+40, +67) and inside its late rows (+68, +100), at total - 1 and at total.  Then a mixed traffic batch with
     cuts inside blocks."""
-    iq, cfgs, capture, exp = worst
+    _capacity_cuts(rx, *worst)
+
+
+@pytest.mark.parametrize("mode", mode_ref.NEW_MODES, ids=mode_ref.mode_id)
+def test_worst_case_densities_and_capacity_cuts_in_modes(rx, mode):
+    """The two tests above with the rotated and symbol-spaced kernels, recovery on the -v cfgs."""
+    w = _worst(mode)
+    _densities(rx, *w)
+    _capacity_cuts(rx, *w, mode=mode)
+
+
+def _capacity_cuts(rx, iq, cfgs, capture, exp, offsets=None, mode=(0, 0)):
     cfgs, capture, exp = cfgs[:8], capture[:8], exp[exp["stream"] < 8]
+    off1 = None if offsets is None else offsets[:1]
     d_iq = _device(iq[:1])
     plan, per = _multi_plan(rx, 1, capture, N_WORST)
     assert (plan[:, 2] <= 1).all()
     total = len(exp)
     for with_count in (True, False):
         for cap in (0, 1, 5 * 123, 5 * 123 + 40, 5 * 123 + 67, 5 * 123 + 68, 5 * 123 + 100, total - 1, total):
-            _check_launch(rx, d_iq, cfgs, capture, exp, plan, per, cap, with_count)
+            _check_launch(rx, d_iq, cfgs, capture, exp, plan, per, cap, with_count, off1)
 
     n = 40 * CHUNK + 777
     iq = _traffic(n, [37, 5, 38, 22], AAS[:5], seed=9)
+    offsets = mode_ref.draw_offsets(np.random.default_rng(8), 4, mode)
+    iq = mode_ref.rotate_all(iq, offsets)
     cfgs = make_cfgs(9, channel=[37, 37, 37, 5, 5, 38, 22, 22, 22],
                      access_addr=[AAS[0], AAS[4], AAS[1], AAS[1], AAS[3], AAS[2], AAS[4], AAS[3], AAS[0]],
                      access_mask=[0xFFFFFFFF, 0, 0xFFFFFFFF, 0xFFFFFFFF, 0xFFFF00FF, 0xFFFFFFFF, 0xFFFFFFFF, 0xFFFFFFFF, 0xFFFFFFF0],
                      crc_init=[0x555555, 0x555555, 0x555555, 0x227BA7 ^ 0x0A1B, 0x227BA7 ^ 0x5679, 0x555555, 0x227BA7 ^ 0x96E1,
                                0x227BA7 ^ 0x5679, 0x123456], rssi=[1, 3, 3, 1, 3, 1, 3, 1, 2])
+    cfgs = mode_ref.with_mode(cfgs, mode)
+    if mode != (0, 0):
+        cfgs["rssi"] |= np.where(cfgs["rssi"] & 2, CFG_RECOVER, 0).astype(np.int32)
     capture = np.array([0, 0, 0, 1, 1, 2, 3, 3, 3], dtype=np.int32)
-    exp = oracle_multi(iq, cfgs, capture)
+    exp = mode_ref.rx_multi(iq, cfgs, capture, offsets)
     assert len(exp) > 500 and (np.bincount(exp["stream"], minlength=9) > 0).all()
     d_iq = _device(iq)
     plan, per = _multi_plan(rx, 4, capture, n)
     for with_count in (True, False):
         for cap in (3, len(exp) // 3 + 1, len(exp) - 5, len(exp)):
-            _check_launch(rx, d_iq, cfgs, capture, exp, plan, per, cap, with_count)
+            _check_launch(rx, d_iq, cfgs, capture, exp, plan, per, cap, with_count, offsets)
 
 
 # ---- 5. poisoned device views and host ingest ------------------------------------------------------------------------------
@@ -322,14 +391,29 @@ def _view_cfgs():
 def test_rx_multi_device_dir_poisoned_views(rx, n_int8):
     """Every byte outside [0, n_int8) of a view is poison; all three captures, and captures 0 and 2 alone (capture 1 is then
     read by no cfg)."""
+    _poisoned_views(rx, n_int8, (0, 0))
+
+
+@pytest.mark.parametrize("mode", mode_ref.NEW_MODES, ids=mode_ref.mode_id)
+@pytest.mark.parametrize("n_int8", LENGTHS)
+def test_rx_multi_device_dir_poisoned_views_in_modes(rx, n_int8, mode):
+    """The same with the rotated and symbol-spaced kernels: the symbol-spaced dense loop reads the word in front of each
+    tile (`head`), which for a capture's first tile lies in the poison and must read as 0."""
+    _poisoned_views(rx, n_int8, mode)
+
+
+def _poisoned_views(rx, n_int8, mode):
     rng = np.random.default_rng(n_int8 + 1)
     iq = np.stack([_capture(n_int8, n_int8 % 1013, "burst", phase=1), _capture(n_int8, n_int8 % 1013 + 1, "noise"),
                    _capture(n_int8, n_int8 % 1013 + 2, "burst", phase=3)])
+    offsets = mode_ref.draw_offsets(np.random.default_rng(n_int8), 3, mode)
+    iq = mode_ref.rotate_all(iq, offsets)
     cfgs, capture = _view_cfgs()
-    exp = oracle_multi(iq, cfgs, capture)
+    cfgs = mode_ref.with_mode(cfgs, mode)
+    exp = mode_ref.rx_multi(iq, cfgs, capture, offsets)
     assert ((exp["chunk"] == 0) & (exp["n0"] == -124)).any() and ((exp["chunk"] == 0) & (exp["n0"] < 0) & ((exp["flags"] & 4) == 0)).any()
     skip = capture != 1
-    exp_skip = oracle_multi(iq, cfgs[skip], capture[skip])
+    exp_skip = mode_ref.rx_multi(iq, cfgs[skip], capture[skip], offsets)
     for front, extra in ((16, 0), (256, 48), (4096, 4096)):
         stride = (n_int8 + 15) // 16 * 16 + extra
         buf, view = _device_view(list(iq), stride, front, rng, random_poison=front != 256)
@@ -338,7 +422,8 @@ def test_rx_multi_device_dir_poisoned_views(rx, n_int8):
             d_out = torch.zeros(len(want) + 16, 64, dtype=torch.uint8, device="cuda")
             d_dir = torch.zeros(n_units, 2, dtype=torch.int32, device="cuda")
             d_count = torch.zeros(1, dtype=torch.int32, device="cuda")
-            rx.rx_multi_device_dir(view, cfgs[sel], capture[sel], d_out, d_count, d_dir, torch.cuda.current_stream().cuda_stream)
+            rx.rx_multi_device_dir(view, cfgs[sel], capture[sel], d_out, d_count, d_dir, torch.cuda.current_stream().cuda_stream,
+                                   offset_hz=offsets)
             torch.cuda.synchronize()
             assert int(d_count.item()) == len(want)
             ud = np.ascontiguousarray(d_dir.cpu().numpy().view(np.uint32)).view(DIR_DTYPE).reshape(-1)
@@ -349,26 +434,31 @@ def test_rx_multi_device_dir_poisoned_views(rx, n_int8):
 NAMED = [1, 2, 4, 7]                                           # of 8 captures: copy runs [1, 2], [4], [7]
 
 
-def _host_case(n_int8, seed, device=None):
-    """Captures NAMED of 8 (the others are never read), 2 or 3 cfgs each; (captures [8, n_int8], cfgs, capture, oracle)."""
+def _host_case(n_int8, seed, device=None, mode=(0, 0)):
+    """Captures NAMED of 8 (the others are never read), 2 or 3 cfgs each, in `mode`; (captures [8, n_int8], cfgs, capture,
+    expected records, offsets)."""
     iq = np.zeros((8, n_int8), dtype=np.int8)
+    offsets = mode_ref.draw_offsets(np.random.default_rng(seed), 8, mode)
     for k, c in enumerate(NAMED):
         iq[c] = _capture(n_int8, seed + c, "noise" if k == 2 else "burst", device, phase=k)
+        if offsets is not None:
+            iq[c] = mode_ref.rotate(iq[c], float(offsets[c]))
     per = [dict(channel=[37, 37, 38], access_mask=[0xFFFFFF00, 0xFFFFFFFF, 0], access_addr=[0x8E89BED6, 0x8E89BED6, 0x12345679], rssi=[3, 1, 3]),
            dict(channel=[37, 39], access_mask=[0xFFFFFFFF, 0xFFFFFF00], rssi=[1, 3]),
            dict(channel=[38, 37], access_addr=[0, 0x8E89BED6], access_mask=[0, 0x0000000F], rssi=[3, 3]),
            dict(channel=[37, 37, 22], access_mask=[0xFFFFFF00, 0xFFFFFFFF, 0xFFFFFFFF], access_addr=[0x8E89BED6, 0x8E89BED6, 0x3A5C96E1],
                 crc_init=[0x555555, 0x555555, 0x227BA7 ^ 0x96E1], rssi=[1, 3, 1])]
     parts = [make_cfgs(len(p["channel"]), **p) for p in per]
-    cfgs = np.concatenate(parts)
+    cfgs = mode_ref.with_mode(np.concatenate(parts), mode)
     capture = np.repeat(np.array(NAMED, dtype=np.int32), [len(p) for p in parts])
-    return iq, cfgs, capture, oracle_multi(iq, cfgs, capture)
+    return iq, cfgs, capture, mode_ref.rx_multi(iq, cfgs, capture, offsets), offsets
 
 
-def _rx_multi_host(rx, ptr, stride, n_int8, cfgs, capture):
+def _rx_multi_host(rx, ptr, stride, n_int8, cfgs, capture, offsets=None):
     cc = np.ascontiguousarray(capture, dtype=np.int32)
-    return rx._grow_once(partial(rx._L.btle_b200_rx_multi, rx._h, ptr, 8, stride, n_int8, cfgs.ctypes.data, cc.ctypes.data, cfgs.size),
-                         REC_DTYPE, cfgs.size * (n_int8 // CHUNK) * 34 + 16)
+    off = None if offsets is None else np.ascontiguousarray(offsets, dtype=np.float32)
+    return rx._grow_once(partial(rx._L.btle_b200_rx_multi_offset, rx._h, ptr, 8, stride, n_int8, cfgs.ctypes.data, cc.ctypes.data, cfgs.size,
+                                 None if off is None else off.ctypes.data), REC_DTYPE, cfgs.size * (n_int8 // CHUNK) * 34 + 16)
 
 
 def _lay_out_named(buf, iq, stride, rng, random_poison):
@@ -382,15 +472,26 @@ def _lay_out_named(buf, iq, stride, rng, random_poison):
 def test_rx_multi_host_ingest_matrix(rx, source):
     """btle_b200_rx_multi from each kind of host memory with a stride: only the named captures are copied, one copy per
     run of consecutive ones; poisoned captures and padding must not change a record."""
+    _host_ingest(rx, source, (0, 0))
+
+
+@pytest.mark.parametrize("mode", mode_ref.NEW_MODES, ids=mode_ref.mode_id)
+@pytest.mark.parametrize("source", SOURCES)
+def test_rx_multi_host_ingest_matrix_in_modes(rx, source, mode):
+    """The same through btle_b200_rx_multi_offset with the rotated and symbol-spaced kernels."""
+    _host_ingest(rx, source, mode)
+
+
+def _host_ingest(rx, source, mode):
     rng = np.random.default_rng(17)
     for n in (6 * CHUNK, 6 * CHUNK + 1005):
-        iq, cfgs, capture, exp = _host_case(n, seed=n % 977)
+        iq, cfgs, capture, exp, offsets = _host_case(n, seed=n % 977, mode=mode)
         assert ((exp["chunk"] == 0) & (exp["n0"] < 0)).sum() >= 2 and (exp["flags"] & 4).any()
         for extra in (0, 7, 4096):
             buf = HostBuf(source, 8 * (n + extra))
             try:
                 _lay_out_named(buf, iq, n + extra, rng, random_poison=extra != 7)
-                _same(_rx_multi_host(rx, buf.ptr, n + extra, n, cfgs, capture), exp)
+                _same(_rx_multi_host(rx, buf.ptr, n + extra, n, cfgs, capture, offsets), exp)
             finally:
                 buf.close()
 
@@ -398,7 +499,7 @@ def test_rx_multi_host_ingest_matrix(rx, source):
 def test_rx_multi_host_captures_larger_than_a_staging_segment(rx):
     """Pageable captures of 32 MiB + 5 chunks + 3 bytes: every named capture is more than one staging segment."""
     n = SEG + 5 * CHUNK + 3
-    iq, cfgs, capture, exp = _host_case(n, seed=300, device="cuda")
+    iq, cfgs, capture, exp, _ = _host_case(n, seed=300, device="cuda")
     assert (np.bincount(exp["stream"], minlength=len(cfgs)) > 0).sum() >= 7
     buf = HostBuf("pageable", 8 * (n + 4099))
     _lay_out_named(buf, iq, n + 4099, np.random.default_rng(5), random_poison=True)

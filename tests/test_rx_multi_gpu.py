@@ -26,13 +26,13 @@ def replicated(rx, iq, cfgs, capture):
     return rx.rx_batch(np.ascontiguousarray(iq[capture]), cfgs)
 
 
-def device_multi(rx, d_iq, cfgs, capture, stream_ptr=0, with_count=True):
+def device_multi(rx, d_iq, cfgs, capture, stream_ptr=0, with_count=True, offset_hz=None):
     n_units = max(rx.multi_units(d_iq.shape[0], capture, d_iq.shape[1]), 1)
     cap = len(cfgs) * (d_iq.shape[1] // 16384) * 123 + 16
     d_out = torch.zeros(cap * 64, dtype=torch.uint8, device="cuda")
     d_dir = torch.zeros(n_units * 8, dtype=torch.uint8, device="cuda")
     d_count = torch.zeros(1, dtype=torch.int32, device="cuda") if with_count else None
-    rx.rx_multi_device_dir(d_iq, cfgs, capture, d_out, d_count, d_dir, stream_ptr)
+    rx.rx_multi_device_dir(d_iq, cfgs, capture, d_out, d_count, d_dir, stream_ptr, offset_hz=offset_hz)
     return d_out, d_dir, d_count
 
 

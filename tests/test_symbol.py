@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 import golden_util
+import mode_ref
 import multi_fuzz
 import offset_ref
 import symbol_ref
@@ -195,3 +196,29 @@ def test_make_cfgs_flag():
     c = rxmod._with_fields(c, {"symbol_spaced": 0})
     assert list(c["rssi"]) == [4, 4, 4]
     assert _native.CFG_SYMBOL_SPACED == 16
+
+
+@pytest.mark.parametrize("mode", mode_ref.MODES, ids=mode_ref.mode_id)
+def test_mode_ref_rx_multi_equals_rx_stream_per_cfg(mode):
+    """mode_ref.rx_multi (each capture's bits made once for all its cfgs; the oracle in the default mode) equals
+    symbol_ref.rx_stream run once per cfg, on the goldens (with RSSI, -v and recovery) and on multi_fuzz draws"""
+    rng = np.random.default_rng(41 + 2 * mode[0] + mode[1])
+    n = 0
+    for name in golden_util.cases():
+        z, cfg = golden_util.load(name)
+        kw = golden_util.rx_cfg(cfg)
+        iq = np.asarray(z["iq"], dtype=np.int8).reshape(1, -1)
+        cfgs = mode_ref.with_mode(rxmod.make_cfgs(3, **kw), mode)
+        cfgs["rssi"] |= [1, 2 | 4, 4]
+        offsets = mode_ref.draw_offsets(rng, 1, mode)
+        iq = mode_ref.rotate_all(iq, offsets)
+        got = mode_ref.rx_multi(iq, cfgs, np.zeros(3, dtype=np.int32), offsets)
+        assert got.tobytes() == mode_ref.rx_multi_by_stream(iq, cfgs, np.zeros(3, dtype=np.int32), offsets).tobytes(), name
+        n += got.size
+    for _ in range(4):
+        iq, cfgs, capture, offsets = multi_fuzz.draw_mode(rng, mode, max_captures=4, max_chunks=5)
+        cfgs["rssi"][::3] |= rxmod._native.CFG_RECOVER
+        got = mode_ref.rx_multi(iq, cfgs, capture, offsets)
+        assert got.tobytes() == mode_ref.rx_multi_by_stream(iq, cfgs, capture, offsets).tobytes()
+        n += got.size
+    assert n > 100
