@@ -114,13 +114,15 @@ extern "C" long emul_rx_stream(const int8_t *iq, long n_int8, const btle_stream_
 //     make_tapset), and the resolver passes run once per cfg, directory entry cfg * (units per group) + the unit's index in
 //     its group.
 // flags: bit 0 permutes the order in which units reserve their block (on the GPU that is the order they finish in),
-// bit 1 takes the candidate walk for every chunk.  Records carry stream = cfg index.  Returns the number of records (one
+// bit 1 takes the candidate walk for every chunk.  sym: the dense pass of the symbol-spaced variant (dbits_group_sym<false>,
+// launch_rx's choice for cfgs with BTLE_CFG_SYMBOL_SPACED; bytes in front of the capture read 0, as rx_batch's launch
+// without a lead), else dbits_group_dense.  Records carry stream = cfg index.  Returns the number of records (one
 // block per (cfg, unit), stored in reservation order), or -1 for an invalid cfg_capture, an uneven plan under
 // <kMaxCfgsPerCapture> or a directory that is too small.  dir: 2 words per entry; *n_dir_out = entries written.
 // Mirrors btle_rx_persistent_kernel; keep in step with it.
 extern "C" long emul_rx_units(const int8_t *iq, long n_captures, long stride, long n_int8, const btle_stream_cfg *cfgs,
-                              const int32_t *cfg_capture, long n_cfgs, int grid, int flags, btle_pkt_rec *out, long cap, uint32_t *dir,
-                              long dir_cap, long *n_dir_out) {
+                              const int32_t *cfg_capture, long n_cfgs, int grid, int flags, int sym, btle_pkt_rec *out, long cap,
+                              uint32_t *dir, long dir_cap, long *n_dir_out) {
   const int reverse_units = flags & 1, force_walk = (flags >> 1) & 1;
   *n_dir_out = 0;
   std::vector<int> caps, cfg0, ncfg;                       // per capture group: its capture, first cfg, number of cfgs
@@ -171,7 +173,8 @@ extern "C" long emul_rx_units(const int8_t *iq, long n_captures, long stride, lo
       uint32_t acc[4] = {0xDEADBEEFu, 0x12345678u, 0xFFFFFFFFu, 0x80000001u};
       const long goff = base_off + 256L * g;
       auto word = [&](int k) -> uint32_t { return word_at(goff + 4L * k); };
-      dbits_group_dense(word, acc);
+      if (sym) dbits_group_sym<false>(word, 0, 0, acc);
+      else dbits_group_dense(word, acc);
       for (int ph = 0; ph < 4; ++ph) pd[4 * g + ph] = acc[ph];
     }
     TapSet taps[kMaxCfgsPerCapture];
@@ -289,6 +292,39 @@ extern "C" long emul_plan(long n_streams, long nchunks, int grid, int32_t *units
     units[3 * u] = ui.stream; units[3 * u + 1] = ui.chunk0; units[3 * u + 2] = ui.nch;
   }
   return pl.total_units;
+}
+
+// The dense arithmetic of the other variants alone: carrier-offset correction (dbits_group_rot, include/btle_b200.h,
+// BTLE_MAX_OFFSET_HZ) and the symbol-spaced discriminator (dbits_group_sym, BTLE_CFG_SYMBOL_SPACED), plain and rotated.
+// Phase words of ngroups groups of 128 samples: words[0 .. 64 ngroups] are the capture's IQ words (one more behind the last
+// group); pd[4 g + ph] bit i = d[128 g + 4 i + ph] of the rotated discriminator with (c, s).
+extern "C" void emul_rot_phase_words(const uint32_t *words, long ngroups, int c, int s, uint32_t *pd) {
+  for (long g = 0; g < ngroups; ++g) {
+    const uint32_t *w = words + 64 * g;
+    auto word = [&](int k) { return w[k]; };
+    uint32_t acc[4] = {0u, 0u, 0u, 0u};
+    dbits_group_rot(word, c, s, acc);
+    for (int ph = 0; ph < 4; ++ph) pd[4 * g + ph] = acc[ph];
+  }
+}
+
+// Phase words of groups [g0, g0 + ngroups) of one capture of n_int8 bytes at `cap`: pd[4 (g - g0) + ph] bit i =
+// d[128 g + 4 i + ph].  Bytes [-lead, n_int8) of the capture are readable, every other byte reads 0.  rot: rotated by (c, s).
+extern "C" void emul_sym_phase_words(const int8_t *cap, long n_int8, long lead, long g0, long ngroups, int rot, int c, int s, uint32_t *pd) {
+  for (long g = g0; g < g0 + ngroups; ++g) {
+    auto word = [&](int k) -> uint32_t {
+      uint32_t w = 0;
+      for (int b = 0; b < 4; ++b) {
+        const long a = 256L * g + 4L * k + b;
+        if (a >= -lead && a < n_int8) w |= (uint32_t)(uint8_t)cap[a] << (8 * b);
+      }
+      return w;
+    };
+    uint32_t acc[4] = {0xDEADBEEFu, 0x12345678u, 0xFFFFFFFFu, 0x80000001u};   // the walk must shift all of it out
+    if (rot) dbits_group_sym<true>(word, c, s, acc);
+    else dbits_group_sym<false>(word, 0, 0, acc);
+    for (int ph = 0; ph < 4; ++ph) pd[4 * (g - g0) + ph] = acc[ph];
+  }
 }
 
 // Exhaustive check of the dense loop's discriminator (btle_core.cuh, dbits8_dense) on the modelled instruction semantics:

@@ -9,9 +9,10 @@
 using namespace btle;
 
 // recs[0..n): records of captures iq + stream * stride (n_int8 each) decoded with cfgs[stream]; every CRC-failed counted
-// record of a cfg with BTLE_CFG_RECOVER (not raw) is replaced by its first alternative with a good CRC, if any.
-// Returns the number of records replaced.
-extern "C" long emul_recover_records(const int8_t *iq, long stride, long n_int8, const btle_stream_cfg *cfgs,
+// record of a cfg with BTLE_CFG_RECOVER (not raw) is replaced by its first alternative with a good CRC, if any.  rot4:
+// NULL for the unrotated bits (recover_packet<false>), else (C4, S4) of the record's capture at rot4[2 stream],
+// rot4[2 stream + 1] (recover_packet<true>, carrier-offset correction).  Returns the number of records replaced.
+extern "C" long emul_recover_records(const int8_t *iq, long stride, long n_int8, const btle_stream_cfg *cfgs, const int32_t *rot4,
                                      btle_pkt_rec *recs, long n) {
   uint32_t crc4[1024];
   make_crc4(crc4);
@@ -28,7 +29,9 @@ extern "C" long emul_recover_records(const int8_t *iq, long stride, long n_int8,
     if (!sp.recover || !r.crc_bad || (r.flags & BTLE_REC_REJECTED)) continue;
     uint32_t words[11];
     int nbytes = r.n_bytes;
-    const int q = recover_packet(iq_window(iq + (long)r.stream * stride, n_int8, r.chunk), sp, crc4, r.n0, words, nbytes);
+    const IqWindow w = iq_window(iq + (long)r.stream * stride, n_int8, r.chunk);
+    const int q = rot4 ? recover_packet<true>(w, sp, crc4, r.n0, words, nbytes, rot4[2 * r.stream], rot4[2 * r.stream + 1])
+                       : recover_packet<false>(w, sp, crc4, r.n0, words, nbytes);
     if (q < 0) continue;
     memcpy(r.bytes, words, sizeof r.bytes);               // words are zero behind n_bytes (<= 42)
     r.n_bytes = (uint8_t)nbytes;

@@ -1,10 +1,13 @@
 """numpy restatement of BTLE_CFG_RECOVER (definition in include/btle_b200.h): the records of a cfg with the flag from the
-records without it (the oracle's, tests/orc.py) and the capture.  Used by tests/test_recover.py against the CPU emulator
-and by tests/test_recover_gpu.py against every GPU path."""
+records without it (the oracle's, tests/orc.py, or tests/mode_ref.py's in the other modes) and the capture, with the
+symbol-spaced bits rotated by (C4, S4) under carrier-offset correction.  Used by tests/test_recover.py and
+tests/test_offset.py against the CPU emulator, by tests/mode_ref.py, and by tests/test_recover_gpu.py against every GPU
+path."""
 from __future__ import annotations
 
 import numpy as np
 
+import offset_ref
 from btle_b200 import synth
 
 CHUNK = 8192
@@ -24,11 +27,12 @@ def window(iq: np.ndarray, chunk: int) -> np.ndarray:
     return w
 
 
-def sym_bits(w: np.ndarray) -> np.ndarray:
-    """e[s] = (I[s] Q[s+4] - I[s+4] Q[s]) > 0 for s in [0, WIN), samples behind the window read as 0"""
+def sym_bits(w: np.ndarray, c4: int = 16384, s4: int = 0) -> np.ndarray:
+    """e[s] = the discriminator of samples s and s + 4 rotated by (c4, s4) (offset_ref.disc) for s in [0, WIN), samples
+    behind the window read as 0; (16384, 0) is the unrotated (I[s] Q[s+4] - I[s+4] Q[s]) > 0"""
     nxt = np.zeros_like(w)
     nxt[:-4] = w[4:]
-    return (w[:, 0] * nxt[:, 1] - nxt[:, 0] * w[:, 1]) > 0
+    return offset_ref.disc(w[:, 0], w[:, 1], nxt[:, 0], nxt[:, 1], c4, s4)
 
 
 def alternative(e: np.ndarray, n0: int, q: int, nbits: int) -> np.ndarray:
@@ -60,18 +64,20 @@ def recover_one(e: np.ndarray, n0: int, channel: int, crc_init: int):
     return None
 
 
-def apply(recs: np.ndarray, iq: np.ndarray, crc_init: int = 0x555555, raw: int = 0) -> np.ndarray:
-    """recs: one cfg's records (REC_DTYPE) over capture iq without the flag -> the records with it"""
+def apply(recs: np.ndarray, iq: np.ndarray, crc_init: int = 0x555555, raw: int = 0, offset_hz: float = 0.0) -> np.ndarray:
+    """recs: one cfg's records (REC_DTYPE) over capture iq without the flag -> the records with it; offset_hz: the
+    capture's carrier-offset correction (0: none; rot(0, 4) is the unrotated bit)"""
     out = recs.copy()
     if raw:
         return out
+    c4, s4 = offset_ref.rot(offset_hz, 4)
     cache = {}
     for k, r in enumerate(out):
         if not r["crc_bad"] or r["flags"] & 4:
             continue
         c = int(r["chunk"])
         if c not in cache:
-            cache[c] = sym_bits(window(iq, c))
+            cache[c] = sym_bits(window(iq, c), c4, s4)
         got = recover_one(cache[c], int(r["n0"]), int(r["channel"]), crc_init)
         if got is None:
             continue

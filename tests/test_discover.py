@@ -2,54 +2,17 @@
 its BTLE_HD form through the CPU emulator, and the host logic of btle_b200/hop.py (discover_connections,
 follow_connections(discover=True), hop_events) driven by an oracle-backed stand-in for BtleRx.  The checks named
 check_* run again on the GPU with BtleRx (tests/test_discover_gpu.py)."""
-import ctypes
-import os
-import subprocess
-
 import numpy as np
 import pytest
 import torch
 
 import discover_ref as R
+import emul
 from btle_b200 import CAND_DTYPE, synth
 from btle_b200.hop import discover_connections, follow_connections, hop_events
 from test_hop import _capture_with_many_connections, _place
 
 AAS = (0x60850A1B, 0x50850A1C, 0x12345679, 0x8E89BED6)          # preamble 0x55 (bit 0 set) and 0xAA
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-EMUL_SRC = os.path.join(HERE, "emul", "btle_discover_emul.cpp")
-EMUL_SO = os.path.join(HERE, "emul", "libbtle_discover_emul.so")      # built by __graft_entry__.build()
-EMUL_DEPS = [EMUL_SRC, os.path.join(ROOT, "btle_b200", "csrc", "btle_core.cuh"), os.path.join(ROOT, "btle_b200", "csrc", "btle_params.h"),
-             os.path.join(ROOT, "include", "btle_b200.h")]
-_emul_lib = None
-
-
-def _emul():
-    """The CPU emulator of discover_kernel's per-lane logic (tests/emul/btle_discover_emul.cpp)."""
-    global _emul_lib
-    if _emul_lib is not None:
-        return _emul_lib
-    if (not os.path.exists(EMUL_SO)) or any(os.path.getmtime(EMUL_SO) < os.path.getmtime(d) for d in EMUL_DEPS):
-        subprocess.run(["g++", "-O2", "-fPIC", "-shared", "-std=c++17", "-x", "c++", "-o", EMUL_SO, EMUL_SRC], check=True)
-    L = _emul_lib = ctypes.CDLL(EMUL_SO)
-    L.emul_discover.restype = ctypes.c_long
-    L.emul_discover.argtypes = [ctypes.c_void_p, ctypes.c_long, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_long]
-    L.emul_crc24_unwind.restype = ctypes.c_uint32
-    L.emul_crc24_unwind.argtypes = [ctypes.c_uint32, ctypes.c_uint32, ctypes.c_int]
-    return L
-
-
-def emul_discover(iq, channel, stream=0):
-    iq = np.ascontiguousarray(iq, dtype=np.int8)
-    cap = iq.size // 8 + 64
-    out = np.zeros(cap, dtype=CAND_DTYPE)
-    n = _emul().emul_discover(iq.ctypes.data, iq.size, channel, stream, out.ctypes.data, cap)
-    assert n <= cap
-    out = out[:n]
-    return out[np.argsort(out["sample"], kind="stable")]
-
 
 def planted(channel, aa, crc_init=0x227BA7, at=3000, n_samples=8000, seed=1, header=(1, 0, 0, 0)):
     """Noise floor with one empty PDU (LLID, NESN, SN, MD = header) whose preamble starts at sample `at`."""
@@ -116,7 +79,7 @@ def test_crc_init_recovery_round_trip():
 
 def test_btle_hd_rule_equals_restatement():
     """The BTLE_HD functions the kernel runs (through the CPU emulator) == the numpy restatement."""
-    L = _emul()
+    L = emul.lib()
     rng = np.random.default_rng(2)
     for _ in range(2000):
         crc, bits = int(rng.integers(0, 1 << 24)), int(rng.integers(0, 1 << 16))
@@ -127,7 +90,7 @@ def test_btle_hd_rule_equals_restatement():
     cases += [(planted(ch, aa, at=2000 + 37 * ch), ch) for ch in (0, 9, 36) for aa in AAS]
     cases += [(x, 9) for x in edge_captures()]
     for iq, ch in cases:
-        a, b = R.discover(iq, ch), emul_discover(iq, ch)
+        a, b = R.discover(iq, ch), emul.discover(iq, ch)
         assert a.tobytes() == b.tobytes(), (ch, len(a), len(b))
     assert len(R.discover(cases[1][0], 17)) > 0                                 # full-scale noise does pass now and then
 

@@ -387,15 +387,9 @@ def _plan(rx, n_streams, n_int8):
     """(stream, chunk0, n_chunks) of every unit of a launch: make_plan / unit_info through the emulator, at the device's
     grid (one persistent CTA per SM)."""
     import emul
-    L = emul.lib()
-    L.emul_plan.restype = ctypes.c_long
-    L.emul_plan.argtypes = [ctypes.c_long, ctypes.c_long, ctypes.c_int, ctypes.c_void_p, ctypes.c_long]
-    cap = n_streams * ((n_int8 // CHUNK + 15) // 16) * 16 + 16
-    buf = np.zeros((cap, 3), dtype=np.int32)
-    grid = torch.cuda.get_device_properties(0).multi_processor_count
-    k = L.emul_plan(n_streams, n_int8 // CHUNK, grid, buf.ctypes.data, cap)
-    assert k == rx.units(n_streams, n_int8)
-    return buf[:k]
+    units = emul.plan(n_streams, n_int8 // CHUNK, torch.cuda.get_device_properties(0).multi_processor_count)
+    assert len(units) == rx.units(n_streams, n_int8)
+    return units
 
 
 def _check_cut(rx, d_iq, cfgs, exp, plan, cap, with_count):

@@ -1,12 +1,16 @@
 """Carrier-offset correction on the CPU: the dense warps' rotated arithmetic (emulated with the PTX semantics of prmt /
-dp2a) against the definition in include/btle_b200.h, the numpy restatement over the oracle chain against the oracle at
-offset 0, the rotated recovery step against its restatement, and the per-packet estimate on hand-built tones."""
+dp2a) against the definition in include/btle_b200.h, the numpy restatement over the oracle chain (tests/mode_ref.py)
+against the oracle at offset 0, the rotated recovery step against its restatement, and the per-packet estimate on
+hand-built tones."""
 import numpy as np
 import pytest
 
+import emul
 import golden_util
+import mode_ref
 import offset_ref
 import orc
+import recover_ref
 import rx_ber_ref
 from btle_b200 import _native, rx as rxmod
 
@@ -16,7 +20,7 @@ OFFSETS = [0.0, 1.0, -1.0, 25e3, -25e3, 100e3, -100e3, 150e3, -150e3, 122.5e3, 3
 
 def _check_dense(iq, c, s):
     ng = (iq.size - 4) // 256
-    got = offset_ref.emul_dbits(iq, c, s)
+    got = emul.rot_dbits(iq, c, s)
     want = offset_ref.dbits(iq, 128 * ng, c, s)
     bad = np.flatnonzero(got != want)
     assert bad.size == 0, (c, s, bad[:8], iq[2 * bad[0]:2 * bad[0] + 4])
@@ -59,7 +63,7 @@ def test_zero_offset_is_the_reference():
         kw = {k: v for k, v in cfg.items() if k != "report_rejected"}
         for rssi in (flags, flags | 1):
             want = orc.rx_flags(iq, rssi, **kw)
-            got = offset_ref.rx_stream(iq, 0.0, rssi=rssi, **kw)
+            got = mode_ref.rx_stream(iq, 0.0, rssi=rssi, **kw)
             assert got.tobytes() == want.tobytes(), name
 
 
@@ -75,8 +79,8 @@ def test_correction_restores_packets(channel):
     """a 150 kHz capture decodes far worse uncorrected than corrected, and corrected about as the capture at 0"""
     iq, aa = _impaired(150e3, 40.0, channel)
     ok = lambda r: int(((r["crc_bad"] == 0) & ((r["flags"] & 4) == 0)).sum())
-    plain = offset_ref.rx_stream(iq, 0.0, channel=channel, access_addr=aa)
-    fixed = offset_ref.rx_stream(iq, 150e3, channel=channel, access_addr=aa)
+    plain = mode_ref.rx_stream(iq, 0.0, channel=channel, access_addr=aa)
+    fixed = mode_ref.rx_stream(iq, 150e3, channel=channel, access_addr=aa)
     assert ok(fixed) > ok(plain) and ok(fixed) >= 18
 
 
@@ -86,12 +90,11 @@ def test_recover_rotated(hz):
     for channel, snr in ((37, 20.0), (9, 24.0)):
         iq, aa = _impaired(hz, snr, channel, n=32)
         cfgs = rxmod.make_cfgs(1, channel=channel, access_addr=aa, rssi=_native.CFG_RECOVER)
-        plain = offset_ref.rx_stream(iq, hz, channel=channel, access_addr=aa)
-        want = offset_ref.recover(plain, iq, hz)
-        got = offset_ref.emul_recover(plain, iq, cfgs, hz)
+        plain = mode_ref.rx_stream(iq, hz, channel=channel, access_addr=aa)
+        want = recover_ref.apply(plain, iq, offset_hz=hz)
+        got = emul.recover(plain, iq, cfgs, hz)
         assert got.tobytes() == want.tobytes()
         if hz == 0.0:                                            # at 0, BTLE_CFG_RECOVER's own rule
-            import recover_ref
             assert want.tobytes() == recover_ref.apply(plain, iq).tobytes()
 
 
@@ -127,7 +130,7 @@ def test_estimate_bias_follows_the_delay():
     cfg["seed"], cfg["snr_db"], cfg["amplitude"], cfg["slot_samples"], cfg["channel"] = 1, 200.0, 100, 2048, 37
     cfg["crc_init"], cfg["access_addr"] = 0x555555, 0x8E89BED6
     iq, truth, _ = rx_ber_ref.capture(cfg, 0, 80)
-    recs = offset_ref.rx_stream(iq, 0.0)
+    recs = mode_ref.rx_stream(iq, 0.0)
     ok = recs[recs["crc_bad"] == 0]
     assert ok.size == 80
     by = {}

@@ -1,12 +1,13 @@
 """Carrier-offset correction on the GPU (the *_offset entry points and btle_b200_rec_offset; definitions in
 include/btle_b200.h): at offset 0 the rotated kernel returns the default kernel's records byte for byte; at other offsets
-it returns what the numpy restatement over the oracle chain returns (tests/offset_ref.py); corrected error rates approach
+it returns what the numpy restatement over the oracle chain returns (tests/mode_ref.py); corrected error rates approach
 the uncorrected ones at offset 0; the per-packet estimate finds the offset of noiseless and noisy captures."""
 import numpy as np
 import pytest
 import torch
 
 import golden_util
+import mode_ref
 import offset_ref
 import rx_ber_ref as R
 from btle_b200 import BtleRx, ber, make_cfgs
@@ -72,7 +73,7 @@ def test_zero_offset_equals_default_batch_and_multi(rx):
 
 
 def _expected(iq, cfg, hz, rssi=0, raw=0, stream=0):
-    rec = offset_ref.rx_stream(iq, hz, rssi=rssi, raw=raw, **cfg)
+    rec = mode_ref.rx_stream(iq, hz, rssi=rssi, raw=raw, **cfg)
     rec["stream"] = stream
     return rec
 

@@ -5,7 +5,6 @@ import numpy as np
 import pytest
 
 import emul
-import emul_recover as ER
 import golden_util as G
 import orc
 import recover_ref as RR
@@ -28,9 +27,9 @@ def _emul_both(iq, cfg, flags=0):
     stream path and of the unit path (which must agree)"""
     iq2 = np.asarray(iq, dtype=np.int8).reshape(1, -1)
     cfgs = make_cfgs(1, **{k: v for k, v in cfg.items()}, rssi=flags, recover=1)
-    a = ER.recover(emul.rx_stream(iq, span_chunks=4, rssi=flags | RR.CFG_RECOVER, **cfg), iq2, cfgs)
+    a = emul.recover(emul.rx_stream(iq, span_chunks=4, rssi=flags | RR.CFG_RECOVER, **cfg), iq2, cfgs)
     b, d = emul.rx_batch_units(iq2, cfgs, grid=7)
-    b = ER.recover(b, iq2, cfgs)
+    b = emul.recover(b, iq2, cfgs)
     _same(a, b)
     return a
 
@@ -156,7 +155,7 @@ def test_raw_mode_and_rejected_hits_are_untouched():
     iq, cfg = _ber_capture(18, 0, 37, n=40, seed=77)
     raw = dict(cfg, raw=1)
     raw_cfgs = make_cfgs(1, **raw, recover=1)
-    _same(ER.recover(emul.rx_stream(iq, span_chunks=4, rssi=RR.CFG_RECOVER, **raw), iq, raw_cfgs), orc.rx_flags(iq, 0, **raw))
+    _same(emul.recover(emul.rx_stream(iq, span_chunks=4, rssi=RR.CFG_RECOVER, **raw), iq, raw_cfgs), orc.rx_flags(iq, 0, **raw))
     ref = orc.rx_flags(iq, 2, **cfg)
     got = _emul_both(iq, cfg, 2)
     rej = (ref["flags"] & 4) != 0
@@ -172,6 +171,6 @@ def test_emulator_equals_restatement_on_fuzz_goldens(name):
     cfg = dict(cfg)
     cfg.pop("rssi", None)
     cfg.setdefault("crc_init", 0x555555)
-    a = ER.recover(emul.rx_stream(z["iq"], span_chunks=3, rssi=RR.CFG_RECOVER, **cfg), z["iq"], make_cfgs(1, **cfg, recover=1))
+    a = emul.recover(emul.rx_stream(z["iq"], span_chunks=3, rssi=RR.CFG_RECOVER, **cfg), z["iq"], make_cfgs(1, **cfg, recover=1))
     ref = orc.rx_flags(z["iq"], 0, **cfg)
     _same(a, RR.apply(ref, z["iq"], crc_init=cfg["crc_init"], raw=cfg.get("raw", 0)))

@@ -1,53 +1,21 @@
 """The symbol-spaced discriminator (BTLE_CFG_SYMBOL_SPACED) on the CPU: the dense warps' arithmetic in that mode (emulated
-with the PTX semantics of prmt / dp2a, tests/emul/btle_symbol_emul.cpp) against the definition in include/btle_b200.h, and
-the emulated unit path in that mode against the numpy restatement over the oracle chain (tests/symbol_ref.py)."""
-import ctypes
-import os
-
+with the PTX semantics of prmt / dp2a, tests/emul/btle_emul.cpp) against the definition in include/btle_b200.h
+(offset_ref.dbits_sym), and the emulated unit path in that mode against the numpy restatement over the oracle chain
+(tests/mode_ref.py)."""
 import numpy as np
 import pytest
 
+import emul
 import golden_util
 import mode_ref
 import multi_fuzz
 import offset_ref
-import symbol_ref
 import orc
 import rx_ber_ref
 from btle_b200 import _native, rx as rxmod
-from emul import DEPS, HERE
 
 EDGE = np.array([-128, -127, -64, -1, 0, 1, 63, 126, 127], dtype=np.int8)
 OFFSETS = [0.0, 1.0, -1.0, 25e3, -25e3, 100e3, -100e3, 150e3, 300e3, -300e3, 499_999.0, 500e3, -500e3]
-SO = os.path.join(HERE, "emul", "libbtle_symbol_emul.so")
-SRC = os.path.join(HERE, "emul", "btle_symbol_emul.cpp")
-_lib = None
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        if (not os.path.exists(SO)) or any(os.path.getmtime(SO) < os.path.getmtime(d) for d in DEPS + [SRC]):
-            import subprocess
-            subprocess.run(["g++", "-O2", "-fPIC", "-shared", "-std=c++17", "-x", "c++", "-o", SO, SRC], check=True)
-        _lib = ctypes.CDLL(SO)
-        vp, lg = ctypes.c_void_p, ctypes.c_long
-        _lib.emul_sym_phase_words.restype = None
-        _lib.emul_sym_phase_words.argtypes = [vp, lg, lg, lg, lg, ctypes.c_int, ctypes.c_int, ctypes.c_int, vp]
-        _lib.emul_rx_units_sym.restype = lg
-        _lib.emul_rx_units_sym.argtypes = [vp, lg, lg, lg, vp, vp, lg, ctypes.c_int, ctypes.c_int, vp, lg, vp, lg, ctypes.POINTER(lg)]
-    return _lib
-
-
-def emul_bits(buf, at, n_int8, lead, g0, ng, hz=None):
-    """d[128 g0 .. 128 (g0 + ng)) from the emulated dense pass; the capture is buf[at : at + n_int8], buf[at - lead : at]
-    readable in front of it"""
-    buf = np.ascontiguousarray(buf, dtype=np.int8)
-    pd = np.zeros(4 * ng, dtype=np.uint32)
-    c, s = (16384, 0) if hz is None else offset_ref.rot(hz, 4)
-    lib().emul_sym_phase_words(buf.ctypes.data + at, n_int8, lead, g0, ng, int(hz is not None), c, s, pd.ctypes.data)
-    bits = ((pd.reshape(ng, 4, 1) >> np.arange(32, dtype=np.uint32)) & 1).astype(np.uint8)
-    return bits.transpose(0, 2, 1).reshape(-1)
 
 
 def want_bits(buf, at, n_int8, lead, g0, ng, hz=None):
@@ -59,7 +27,7 @@ def want_bits(buf, at, n_int8, lead, g0, ng, hz=None):
         x[2 * (m + 2)] = buf[at + 2 * m]
         x[2 * (m + 2) + 1] = buf[at + 2 * m + 1]
     c, s = (16384, 0) if hz is None else offset_ref.rot(hz, 4)
-    return symbol_ref.dbits_sym(x, 128 * (g0 + ng), c, s)[128 * g0:]
+    return offset_ref.dbits_sym(x, 128 * (g0 + ng), c, s)[128 * g0:]
 
 
 def test_dense_random():
@@ -70,8 +38,8 @@ def test_dense_random():
     x = np.concatenate([np.zeros(4, np.int8), iq])               # sample -2, -1 read 0 (no lead)
     for hz in [None] + OFFSETS:
         c, s = (16384, 0) if hz is None else offset_ref.rot(hz, 4)
-        got = emul_bits(iq, 0, iq.size, 0, 0, ng, hz)
-        want = symbol_ref.dbits_sym(x, 128 * ng, c, s)
+        got = emul.sym_dbits(iq, 0, iq.size, 0, 0, ng, hz)
+        want = offset_ref.dbits_sym(x, 128 * ng, c, s)
         bad = np.flatnonzero(got != want)
         assert bad.size == 0, (hz, bad[:8])
 
@@ -94,10 +62,10 @@ def test_dense_edges(hz):
         iq = samples.reshape(-1)
         iq = np.concatenate([iq, np.zeros(-iq.size % 256, np.int8)])
         ng = iq.size // 256
-        got = emul_bits(iq, 0, iq.size, 0, 0, ng, hz)
+        got = emul.sym_dbits(iq, 0, iq.size, 0, 0, ng, hz)
         c, s = (16384, 0) if hz is None else offset_ref.rot(hz, 4)
         x = np.concatenate([np.zeros(4, np.int8), iq, np.zeros(8, np.int8)])
-        want = symbol_ref.dbits_sym(x, 128 * ng, c, s)
+        want = offset_ref.dbits_sym(x, 128 * ng, c, s)
         bad = np.flatnonzero(got != want)
         assert bad.size == 0, (hz, ph, bad[:8])
 
@@ -112,33 +80,16 @@ def test_dense_capture_edges(lead, hz):
     buf = rng.integers(-128, 128, size=256 + n_int8 + 512, dtype=np.int16).astype(np.int8)
     at = 256
     for g0, ng in [(0, 3), (30, 4), (62, 4), (1022, 4), (1098, 3)]:
-        got = emul_bits(buf, at, n_int8, lead, g0, ng, hz)
+        got = emul.sym_dbits(buf, at, n_int8, lead, g0, ng, hz)
         want = want_bits(buf, at, n_int8, lead, g0, ng, hz)
         bad = np.flatnonzero(got != want)
         assert bad.size == 0, (g0, lead, bad[:8])
 
 
-def emul_units_sym(iq2d, cfgs, capture=None, grid=132):
-    iq2d = np.ascontiguousarray(iq2d, dtype=np.int8)
-    ns, n = iq2d.shape
-    cfgs = np.ascontiguousarray(cfgs).reshape(-1)
-    cc = None if capture is None else np.ascontiguousarray(capture, dtype=np.int32)
-    cap = cfgs.size * (n // 16384) * 123 + 8
-    out = np.zeros(cap, dtype=orc.REC_DTYPE)
-    dir_cap = cfgs.size * ((n // 16384 + 15) // 16 * 16 + 16)
-    d = np.zeros((dir_cap, 2), dtype=np.uint32)
-    nd = ctypes.c_long(0)
-    cnt = lib().emul_rx_units_sym(iq2d.ctypes.data, ns, n, n, cfgs.ctypes.data, None if cc is None else cc.ctypes.data, cfgs.size, grid, 0,
-                                  out.ctypes.data, cap, d.ctypes.data, dir_cap, ctypes.byref(nd))
-    assert 0 <= cnt <= cap
-    d = d[:nd.value]
-    return np.concatenate([out[b:b + c] for b, c in d]) if len(d) else out[:0]
-
-
 def restated(iq, cfg, stream=0):
-    return symbol_ref.rx_stream(iq, 0.0, channel=int(cfg["channel"]), access_addr=int(cfg["access_addr"]),
-                                access_mask=int(cfg["access_mask"]), crc_init=int(cfg["crc_init"]), raw=int(cfg["raw"]),
-                                rssi=int(cfg["rssi"]) & ~_native.CFG_SYMBOL_SPACED, stream=stream, sym=True)
+    return mode_ref.rx_stream(iq, 0.0, True, channel=int(cfg["channel"]), access_addr=int(cfg["access_addr"]),
+                              access_mask=int(cfg["access_mask"]), crc_init=int(cfg["crc_init"]), raw=int(cfg["raw"]),
+                              rssi=int(cfg["rssi"]) & ~_native.CFG_SYMBOL_SPACED, stream=stream)
 
 
 def test_restatement_with_reference_bits_is_the_oracle():
@@ -148,7 +99,7 @@ def test_restatement_with_reference_bits_is_the_oracle():
         flags = 2 if cfg.get("report_rejected") else 0
         kw = {k: v for k, v in cfg.items() if k != "report_rejected"}
         want = orc.rx_flags(z["iq"], flags | 1, **kw)
-        assert symbol_ref.rx_stream(z["iq"], 0.0, rssi=flags | 1, sym=False, **kw).tobytes() == want.tobytes(), name
+        assert mode_ref.rx_stream(z["iq"], 0.0, rssi=flags | 1, **kw).tobytes() == want.tobytes(), name
 
 
 def test_unit_path_goldens():
@@ -158,7 +109,7 @@ def test_unit_path_goldens():
         c = rxmod.make_cfgs(1, **golden_util.rx_cfg(cfg), symbol_spaced=1)
         c["rssi"] |= _native.CFG_RSSI
         iq = np.asarray(z["iq"], dtype=np.int8).reshape(1, -1)
-        got = emul_units_sym(iq, c)
+        got = emul.rx_multi(iq, c, None)
         want = restated(iq[0], c[0])
         assert got.tobytes() == want.tobytes(), name
 
@@ -170,7 +121,7 @@ def test_unit_path_fuzz_and_multi():
         iq, cfgs, capture = multi_fuzz.draw(rng, max_captures=6, max_chunks=20)
         cfgs = cfgs.copy()
         cfgs["rssi"] |= _native.CFG_SYMBOL_SPACED
-        got = emul_units_sym(iq, cfgs, capture)
+        got = emul.rx_multi(iq, cfgs, capture)
         want = np.concatenate([restated(iq[capture[j]], cfgs[j], stream=j) for j in range(cfgs.size)] or [got[:0]])
         assert got.tobytes() == want.tobytes()
 
@@ -183,7 +134,7 @@ def test_unit_path_synthesised_and_gain():
     iq = rx_ber_ref.capture(cfg, 0, 160)[0]
     iq = np.asarray(iq, dtype=np.int8)[: iq.size // 16384 * 16384]
     c = rxmod.make_cfgs(1, channel=37, rssi=_native.CFG_REPORT_REJECTED, symbol_spaced=1)
-    got = emul_units_sym(iq.reshape(1, -1), c)
+    got = emul.rx_multi(iq.reshape(1, -1), c, None)
     assert got.tobytes() == restated(iq, c[0]).tobytes()
     ok = lambda r: int(((r["crc_bad"] == 0) & ((r["flags"] & 4) == 0)).sum())
     plain = orc.rx_flags(iq, 2, channel=37)
@@ -201,7 +152,7 @@ def test_make_cfgs_flag():
 @pytest.mark.parametrize("mode", mode_ref.MODES, ids=mode_ref.mode_id)
 def test_mode_ref_rx_multi_equals_rx_stream_per_cfg(mode):
     """mode_ref.rx_multi (each capture's bits made once for all its cfgs; the oracle in the default mode) equals
-    symbol_ref.rx_stream run once per cfg, on the goldens (with RSSI, -v and recovery) and on multi_fuzz draws"""
+    mode_ref.rx_stream run once per cfg, on the goldens (with RSSI, -v and recovery) and on multi_fuzz draws"""
     rng = np.random.default_rng(41 + 2 * mode[0] + mode[1])
     n = 0
     for name in golden_util.cases():

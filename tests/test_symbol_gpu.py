@@ -1,5 +1,5 @@
 """The symbol-spaced discriminator (BTLE_CFG_SYMBOL_SPACED, include/btle_b200.h) on the GPU: every receive path in that mode
-returns what the numpy restatement over the oracle chain returns (tests/symbol_ref.py); streamed and
+returns what the numpy restatement over the oracle chain returns (tests/mode_ref.py); streamed and
 batched forms equal rx_batch on the whole capture; one mode per launch; and the new mode's error rates against the
 default's."""
 import json
@@ -11,8 +11,8 @@ import pytest
 import torch
 
 import golden_util
+import mode_ref
 import multi_fuzz
-import symbol_ref
 import rx_ber_ref as R
 from btle_b200 import BtleRx, ber, make_cfgs
 from btle_b200._native import BTLE_EINVAL, CFG_SYMBOL_SPACED, DIR_DTYPE, REC_DTYPE, RX_BER_RESULT_DTYPE, BtleError
@@ -47,7 +47,7 @@ def _same(a, b):
 
 
 def _expected(iq, cfg, rssi=0, raw=0, stream=0, hz=0.0, access_mask=0xFFFFFFFF):
-    return symbol_ref.rx_stream(iq, hz, rssi=rssi, raw=raw, stream=stream, access_mask=access_mask, sym=True, **cfg)
+    return mode_ref.rx_stream(iq, hz, True, rssi=rssi, raw=raw, stream=stream, access_mask=access_mask, **cfg)
 
 
 def test_goldens_and_fuzz(rx):
@@ -59,7 +59,7 @@ def test_goldens_and_fuzz(rx):
             rssi = kw.get("rssi", 0) | extra
             k = {a: b for a, b in kw.items() if a != "rssi"}
             got = rx.rx(z["iq"], rssi=rssi, symbol_spaced=1, **k)
-            want = symbol_ref.rx_stream(z["iq"], 0.0, rssi=rssi, sym=True, **k)
+            want = mode_ref.rx_stream(z["iq"], 0.0, True, rssi=rssi, **k)
             _same(got, want)
             n += got.size
     assert n > 0
@@ -69,7 +69,7 @@ def test_goldens_and_fuzz(rx):
         cfgs = cfgs.copy()
         cfgs["rssi"] |= CFG_SYMBOL_SPACED
         got = rx.rx_multi(iq, cfgs, capture)
-        want = np.concatenate([symbol_ref.rx_stream(iq[capture[j]], 0.0, stream=j, sym=True, **{
+        want = np.concatenate([mode_ref.rx_stream(iq[capture[j]], 0.0, True, stream=j, **{
             k: int(cfgs[j][k]) for k in ("channel", "access_addr", "access_mask", "crc_init", "raw")}, rssi=int(cfgs[j]["rssi"]) & 7)
             for j in range(cfgs.size)])
         _same(got, want)
@@ -103,8 +103,8 @@ def test_batch_40_captures_and_multi(rx, caps40):
     got = rx.rx_multi(iq[:3], mc, cap)
     for j, c in enumerate(cap):
         f = mc[j]
-        w = symbol_ref.rx_stream(iq[c], 0.0, channel=int(f["channel"]), access_addr=int(f["access_addr"]), access_mask=int(f["access_mask"]),
-                                 crc_init=int(f["crc_init"]), raw=int(f["raw"]), rssi=int(f["rssi"]) & 7, stream=j, sym=True)
+        w = mode_ref.rx_stream(iq[c], 0.0, True, channel=int(f["channel"]), access_addr=int(f["access_addr"]), access_mask=int(f["access_mask"]),
+                               crc_init=int(f["crc_init"]), raw=int(f["raw"]), rssi=int(f["rssi"]) & 7, stream=j)
         _same(got[got["stream"] == j], w)
     # device form equals the host form (rows of a multiple of 16 bytes)
     iq = np.ascontiguousarray(iq[:, :iq.shape[1] // 16 * 16])
