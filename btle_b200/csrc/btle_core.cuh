@@ -151,7 +151,8 @@ struct StreamParams {
   int32_t raw;                // -r
   int32_t adv;                // channel in {37,38,39}, :2202
   int32_t rssi;               // -R
-  int32_t report_rejected;    // -v: hits the reference drops for their ADV length (:2291-2298) are reported too (not counted)
+  int16_t report_rejected;    // -v: hits the reference drops for their ADV length (:2291-2298) are reported too (not counted)
+  int16_t centre_hits;        // BTLE_CFG_CENTRE_HITS: the chain moves each full-window hit to the centre of its run (centre_hit)
   int32_t recover;            // BTLE_CFG_RECOVER and not raw: CRC-failed counted packets are demodulated again (recover_packet)
   int32_t tz;                // min(31, index of lowest set bit of aa&mask (32 if none))
   int32_t ntaps;              // 0 => every group is flagged (mask == 0)
@@ -160,6 +161,7 @@ struct StreamParams {
   uint32_t tap_xor[kMaxTaps]; // 0 if aa bit p is 1, ~0 if it is 0
   uint32_t whiten[12];        // scramble_table[channel][0..41] packed little-endian (+pad)
 };
+static_assert(sizeof(StreamParams) == 192, "a resolver warp loads a StreamParams with one coalesced load (load_params_warp)");
 
 BTLE_HD uint32_t funnel_r(uint32_t lo, uint32_t hi, uint32_t s) {
 #if defined(__CUDA_ARCH__)
@@ -662,6 +664,20 @@ BTLE_HD uint32_t crc24_words(const uint32_t words[11], int nbody, uint32_t crc, 
 // what is reported: a chunk with more hits is finished by its own lane (btle_rx_kernels.cu, resolver step 4).
 constexpr int kRejectedInHitRow = 16;
 constexpr int kMaxRejectedPerChunk = kRejectedInHitRow;   // former name of the same constant, kept so code using it still builds
+// BTLE_CFG_CENTRE_HITS (include/btle_b200.h): hit n of the search restarted at R moved to the centre of its run of matching
+// window starts n, n + 1, .. (at most 4, below n0_lim and the chunk's 8192 window starts).  A hit through the zeroed
+// history (n < R) stays.  Reads the phase words with win32, so the exact-hit lists and the candidate walk agree.
+BTLE_HD int centre_hit(const uint32_t *pd, const StreamParams &sp, int R, int n0_lim, int n) {
+  if (n < R) return n;
+  int run = 1;
+  for (; run < 4; ++run) {
+    const int c = n + run;
+    if (c >= n0_lim || c >= kChunkSamples) break;
+    if (((win32(pd, c & 3, c >> 2, kWinGroups + 1) ^ sp.aa) & sp.mask) != 0u) break;
+  }
+  return n + ((run - 1) >> 1);
+}
+
 // search(R, n0_lim, n0&) -> bool: the reference's search_unique_bits restarted at sample R (see search_from)
 template <class Search, class Hit>
 BTLE_HD int chain_with(const uint32_t *pd, const StreamParams &sp, Search &search, Hit &hit) {
@@ -674,6 +690,7 @@ BTLE_HD int chain_with(const uint32_t *pd, const StreamParams &sp, Search &searc
     const int n0_lim = R + 4 * left - 124;   // window end n0+124 must stay < R + 4*left
     int n0 = 0;
     if (!search(R, n0_lim, n0)) break;                   // :2218
+    if (sp.centre_hits) n0 = centre_hit(pd, sp, R, n0_lim, n0);   // uniform per cfg
     E = 2 * n0 + 256;                                    // :2226, :2231
     E += 64 * (sp.raw ? 42 : 2);                         // :2254-2257
     if (E > kWinInt8) break;                             // :2259-2263

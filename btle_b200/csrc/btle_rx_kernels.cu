@@ -3781,8 +3781,8 @@ static int check_rx_ber_cfg(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg) {
   }
   if (std::fabs(cfg->ppm) >= 1e6f) { ctx->err = "rx_ber: ppm must have |ppm| < 1e6"; return BTLE_EINVAL; }
   if (cfg->amplitude < 1 || cfg->amplitude > 127) { ctx->err = "rx_ber: amplitude must be 1..127"; return BTLE_EINVAL; }
-  if (cfg->flags & ~(uint32_t)(BTLE_CFG_RECOVER | BTLE_CFG_SYMBOL_SPACED)) {
-    ctx->err = "rx_ber: flags may only hold BTLE_CFG_RECOVER and BTLE_CFG_SYMBOL_SPACED";
+  if (cfg->flags & ~(uint32_t)(BTLE_CFG_RECOVER | BTLE_CFG_SYMBOL_SPACED | BTLE_CFG_CENTRE_HITS)) {
+    ctx->err = "rx_ber: flags may only hold BTLE_CFG_RECOVER, BTLE_CFG_SYMBOL_SPACED and BTLE_CFG_CENTRE_HITS";
     return BTLE_EINVAL;
   }
   if (cfg->slot_samples < rx_ber_len(cfg->channel) || cfg->slot_samples > BTLE_RX_BER_MAX_SLOT) {

@@ -70,7 +70,8 @@ typedef struct {
                             count them (:2291-2298) — come back as records with BTLE_REC_REJECTED set, every one
                             of them, in the reference's order (up to BTLE_MAX_RECS_PER_CHUNK records per chunk);
                             BTLE_CFG_RECOVER 4: CRC-failed packets are demodulated once more (below);
-                            BTLE_CFG_SYMBOL_SPACED 16: the symbol-spaced discriminator (below)                   */
+                            BTLE_CFG_SYMBOL_SPACED 16: the symbol-spaced discriminator (below);
+                            BTLE_CFG_CENTRE_HITS 64: each hit centred on its run of matching phases (below)      */
 } btle_stream_cfg;
 #define BTLE_CFG_RSSI 1
 #define BTLE_CFG_REPORT_REJECTED 2
@@ -110,6 +111,25 @@ typedef struct {
  * last_error set).  A stream session's mode is that of the cfgs given to streams_open; a set_cfg or add_cfg with the other
  * value is BTLE_EINVAL.  btle_rx_ber_cfg.flags accepts it too. */
 #define BTLE_CFG_SYMBOL_SPACED 16
+/* BTLE_CFG_CENTRE_HITS: opt-in hit rule of the greedy chain.  Not part of the reference's receiver; without it the records
+ * are the reference's (or the current mode's), bit for bit.  An access address stays matched for about a symbol around the
+ * eye, so the search's first matching window start lies up to a few samples before the centre; with the flag the chain
+ * moves each such hit to the centre of its run of matching sample phases:
+ *   1. which hits  the search restarted at sample R (window-start limit n0_lim = R + 4 num_symbol_left - 124) returns n.
+ *                  Only a full-window hit, n >= R, moves; a hit through the zeroed history (n < R) stays.
+ *   2. the run     L = 1 + k, k = the number of consecutive q = 1, 2, 3 (in that order) with n + q < n0_lim, n + q < 8192
+ *                  (a window start of the chunk) and the 32 bits d[n + q + 4j], j = 0..31, matching the access address
+ *                  under the mask exactly as the search compares them.
+ *   3. the hit     n0' = n + floor((L - 1) / 2): L = 1 or 2 keeps n, L = 3 or 4 gives n + 1.
+ * Everything the chain derives from a hit then uses n0': the header and its length, the three length guards, the -v
+ * rejected record, the restart point (buf_len_eaten = 2 n0' + 256 + ...), the bytes and the CRC, mag_sum and
+ * BTLE_CFG_RECOVER's alternatives.  A record's n0 is n0', in -124..8191 as always.  The rule reads only the bits d of the
+ * launch's mode, so it applies with and without BTLE_CFG_SYMBOL_SPACED, with and without carrier-offset correction, and in
+ * raw mode; it reads nothing outside the chunk's window.  Since n0' >= n, every restart point lies at or behind the
+ * reference's for the same hit, so the counting arguments of BTLE_MAX_PKTS_PER_CHUNK and BTLE_MAX_RECS_PER_CHUNK hold
+ * unchanged.  The flag is per cfg (like BTLE_CFG_RECOVER): the cfgs of one launch, rx_multi capture or stream session
+ * may mix it freely.  btle_rx_ber_cfg.flags accepts it too. */
+#define BTLE_CFG_CENTRE_HITS 64
 /* Carrier-offset correction: the *_offset entry points take one float offset_hz per capture, the received carrier minus
  * the nominal one in Hz (the sign of btle_rx_ber_cfg.cfo_hz: correcting by cfo_hz undoes that impairment).  Not part of the
  * reference's receiver.  With phi = 2 pi offset_hz / 4 MHz and C = round(2^14 cos phi), S = round(2^14 sin phi) (nearest,
@@ -561,8 +581,8 @@ typedef struct {
   int32_t channel;         /* 0..39                                                                                 */
   uint32_t access_addr;
   uint32_t crc_init;       /* as -k                                                                                 */
-  uint32_t flags;          /* BTLE_CFG_RECOVER and / or BTLE_CFG_SYMBOL_SPACED (given to the receiver); any other
-                              bit: BTLE_EINVAL                                                                        */
+  uint32_t flags;          /* any of BTLE_CFG_RECOVER, BTLE_CFG_SYMBOL_SPACED and BTLE_CFG_CENTRE_HITS (given to the
+                              receiver); any other bit: BTLE_EINVAL                                                   */
   uint32_t reserved;       /* 0                                                                                     */
 } btle_rx_ber_cfg;         /* 48 bytes */
 typedef struct {
@@ -589,8 +609,8 @@ typedef struct {
  * size (every batch starts on a chunk and slot boundary, and its look-ahead behind the last chunk is the next slots'; with
  * BTLE_CFG_SYMBOL_SPACED a batch also reads the 2 samples in front of it and 2 more behind its look-ahead).
  * BTLE_EINVAL with btle_b200_last_error() for: snr_db, ppm or cfo_hz NaN or infinite, |ppm| >= 1e6, amplitude outside
- * 1..127, slot_samples below L or above BTLE_RX_BER_MAX_SLOT, channel > 39, a flags bit other than BTLE_CFG_RECOVER and
- * BTLE_CFG_SYMBOL_SPACED;
+ * 1..127, slot_samples below L or above BTLE_RX_BER_MAX_SLOT, channel > 39, a flags bit other than BTLE_CFG_RECOVER,
+ * BTLE_CFG_SYMBOL_SPACED and BTLE_CFG_CENTRE_HITS;
  * the context stays usable. */
 int btle_b200_rx_ber_run(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg, size_t n_packets, btle_rx_ber_result *out);
 /* the capture and truth of packets first_packet .. first_packet + n_packets - 1 alone: d_iq (16-byte aligned) receives
