@@ -153,7 +153,8 @@ struct StreamParams {
   int32_t rssi;               // -R
   int16_t report_rejected;    // -v: hits the reference drops for their ADV length (:2291-2298) are reported too (not counted)
   int16_t centre_hits;        // BTLE_CFG_CENTRE_HITS: the chain moves each full-window hit to the centre of its run (centre_hit)
-  int32_t recover;            // BTLE_CFG_RECOVER and not raw: CRC-failed counted packets are demodulated again (recover_packet)
+  int16_t recover;            // BTLE_CFG_RECOVER and not raw: CRC-failed counted packets are demodulated again (recover_packet)
+  int16_t correct;            // BTLE_CFG_CORRECT and not raw: CRC-failed counted packets are corrected by syndrome (repair_packet)
   int32_t tz;                // min(31, index of lowest set bit of aa&mask (32 if none))
   int32_t ntaps;              // 0 => every group is flagged (mask == 0)
   int32_t typed;              // 1 => taps [0, kTapsOne) expect a 1 and taps [kTapsOne, kMaxTaps) expect a 0
@@ -824,6 +825,107 @@ BTLE_HD void decode_packet(const uint32_t *pd, const StreamParams &sp, const uin
   crc_bad_out = crc_bad;
 }
 
+// ---- syndrome correction of CRC-failed packets (BTLE_CFG_CORRECT, include/btle_b200.h) -----------------------------------
+// A packet of n_bytes bytes is N = 8 n_bytes bits in the order sent (body, then CRC).  The bit u places from the end (u = 0:
+// the last CRC bit) is bit N - 1 - u.  An error there changes crc24(body) XOR received CRC by the syndrome
+//   u < 24   1 << (23 - u)  (a CRC bit);
+//   u >= 24  the CRC register (crc24_words convention) from 0 after a 1 and u - 24 zero bits (the CRC is linear, and zero
+//            bits in front of the error leave a zero register where it starts),
+// which depends on u alone, so one table serves every packet length.  Pattern code 2 u + w - 1: w = 1 the single bit u,
+// w = 2 the adjacent pair u, u - 1 (u >= 1).  The table holds every pattern of the longest body (39 bytes).
+constexpr int kCorrectMaxBits = 8 * 42;                      // 312 body bits of a 39-byte body + 24 CRC bits
+constexpr int kCorrectPatterns = 2 * kCorrectMaxBits - 1;    // 336 single bits + 335 adjacent pairs = 671
+// open addressing: slot = syndrome_slot(s) + k, k < kSyndromeProbes; entry = s << 32 | code, 0 = empty (no syndrome is 0)
+constexpr int kSyndromeSlots = 4096;
+constexpr int kSyndromeProbes = 6;
+BTLE_HD uint32_t syndrome_slot(uint32_t s) { return (s * 0x9E3779B1u) >> 20; }
+// syndrome of pattern `code`
+BTLE_HD uint32_t pattern_syndrome(int code) {
+  const int u = code >> 1, w = (code & 1) + 1;
+  uint32_t s = 0u;
+  for (int b = u - w + 1; b <= u; ++b) {
+    uint32_t c = 1u << 23;
+    if (b >= 24) {
+      c = 0xDA6000u;                                         // a 1 into the zero register
+      for (int z = 24; z < b; ++z) c = (c >> 1) ^ ((c & 1u) ? 0xDA6000u : 0u);
+    } else {
+      c >>= b;
+    }
+    s ^= c;
+  }
+  return s;
+}
+// Fills tab[kSyndromeSlots] with the kCorrectPatterns patterns; returns their number, or -1 if two share a syndrome, a
+// syndrome is 0, or a pattern would lie kSyndromeProbes or more slots behind its own (none of which happens: tests).
+BTLE_HD int make_syndrome_table(uint64_t *tab) {
+  for (int i = 0; i < kSyndromeSlots; ++i) tab[i] = 0ull;
+  int n = 0;
+  for (int code = 0; code < kCorrectPatterns + 1; ++code) {
+    if (code == 1) continue;                                 // (u = 0, w = 2) is no pattern
+    const uint32_t s = pattern_syndrome(code);
+    if (s == 0u) return -1;
+    const uint32_t h = syndrome_slot(s);
+    int k = 0;
+    for (; k < kSyndromeProbes; ++k) {
+      const uint64_t e = tab[(h + k) & (kSyndromeSlots - 1)];
+      if (e == 0ull) break;
+      if ((uint32_t)(e >> 32) == s) return -1;
+    }
+    if (k == kSyndromeProbes) return -1;
+    tab[(h + k) & (kSyndromeSlots - 1)] = ((uint64_t)s << 32) | (uint32_t)code;
+    ++n;
+  }
+  return n;
+}
+// code of the pattern whose syndrome is s, -1 if none: at most kSyndromeProbes read-only loads
+BTLE_HD int syndrome_lookup(const uint64_t *tab, uint32_t s) {
+  const uint32_t h = syndrome_slot(s);
+#pragma unroll
+  for (int k = 0; k < kSyndromeProbes; ++k) {
+    const uint64_t *p = tab + ((h + k) & (kSyndromeSlots - 1));
+#if defined(__CUDA_ARCH__)
+    const uint64_t e = __ldg(reinterpret_cast<const unsigned long long *>(p));
+#else
+    const uint64_t e = *p;
+#endif
+    if (e == 0ull) return -1;
+    if ((uint32_t)(e >> 32) == s) return (int)(uint32_t)e;
+  }
+  return -1;
+}
+// Packet (words[11] as decode_packet returns them, n_bytes) whose syndrome is s != 0: if s is the syndrome of a pattern
+// that lies inside the packet and does not touch the header's length field (bits 8..13 on advertising channels, 8..12
+// on data channels), flips its bits and returns true; else returns false and leaves words untouched.
+BTLE_HD bool correct_words(uint32_t words[11], int nbytes, const StreamParams &sp, uint32_t s, const uint64_t *tab) {
+  const int code = syndrome_lookup(tab, s);
+  if (code < 0) return false;
+  const int w = (code & 1) + 1, i = 8 * nbytes - 1 - (code >> 1);   // flips bits i .. i + w - 1
+  if (i < 0) return false;                                           // further from the end than this packet is long
+  if (i + w > 8 && i < (sp.adv ? 14 : 13)) return false;             // the length field
+  const uint32_t m = w == 2 ? 3u : 1u;
+#pragma unroll
+  for (int j = 0; j < 11; ++j) {                                     // no dynamic index: words stays in registers
+    const int lo = i - 32 * j;
+    if (lo >= 0 && lo < 32) words[j] ^= m << lo;
+    else if (lo == -1) words[j] ^= m >> 1;                           // the second bit of a pair that straddles a word
+  }
+  return true;
+}
+// The primary decode (words, n_bytes) of a counted, CRC-failed packet, corrected by correct_words if its syndrome allows
+// (returns true).  The syndrome is the one decode_packet compares: crc24(body) XOR the received (dewhitened) CRC bytes.
+BTLE_HD bool correct_packet(uint32_t words[11], int nbytes, const StreamParams &sp, const uint32_t *crc4, const uint64_t *tab) {
+  const int body = nbytes - 3, at = 8 * body;
+  uint32_t lo = 0u, hi = 0u;
+#pragma unroll
+  for (int j = 0; j < 11; ++j) {
+    if (j == (at >> 5)) lo = words[j];
+    if (j == (at >> 5) + 1) hi = words[j];
+  }
+  const uint32_t rx = funnel_r(lo, hi, (uint32_t)(at & 31)) & 0xFFFFFFu;
+  const uint32_t s = crc24_words(words, body, sp.crc_init, crc4) ^ rx;
+  return s != 0u && correct_words(words, nbytes, sp, s, tab);
+}
+
 // ---- recovery of CRC-failed packets (BTLE_CFG_RECOVER, include/btle_b200.h) --------------------------------------------
 // The capture samples one chunk's recovery may read: sample s (relative to the chunk) is iq[2s], iq[2s+1] for 0 <= s < n,
 // n = what the capture holds of the chunk's receiver() window [0, kWinInt8 / 2); every other sample reads 0.
@@ -865,10 +967,19 @@ BTLE_HD uint32_t sym_bits32(const IqWindow &w, int s0, int c4 = 0, int s4 = 0) {
 // q = 0..3 (packet bit j = e[n0 + 4j + q - 2]) in order; the first whose CRC is good wins.  Returns q and writes that
 // alternative's bytes (words[11], zero behind n_bytes, as decode_packet) and n_bytes; returns -1 and leaves both
 // untouched when none passes.  Not for raw mode (sp.recover is 0 there).  ROT: the bits of sym_bits32<true>(.., c4, s4).
+// tab (BTLE_CFG_CORRECT; words, nbytes_out: the primary decode): when no alternative passes, steps on in repair_packet's
+// order: returns 4 when correct_packet corrects the primary decode in words, else 5 + q for the first alternative q that
+// correct_words corrects.  One loop for both, so that the kernel holds one alternative's words, not two.
 template <bool ROT = false>
 BTLE_HD int recover_packet(const IqWindow &w, const StreamParams &sp, const uint32_t *crc4, int n0, uint32_t words[11], int &nbytes_out,
-                           int c4 = 0, int s4 = 0) {
-  for (int q = 0; q < 4; ++q) {
+                           int c4 = 0, int s4 = 0, const uint64_t *tab = nullptr) {
+  const int steps = tab ? 9 : 4;
+  for (int t = 0; t < steps; ++t) {
+    if (t == 4) {
+      if (correct_packet(words, nbytes_out, sp, crc4, tab)) return 4;
+      continue;
+    }
+    const int q = t < 4 ? t : t - 5;                     // exact, then corrected
     const int s0 = n0 + 4 * 32 + q - 2;                  // packet bit 32: the first header bit
     uint32_t alt[11];
     alt[0] = sym_bits32<ROT>(w, s0, c4, s4) ^ sp.whiten[0];
@@ -883,17 +994,30 @@ BTLE_HD int recover_packet(const IqWindow &w, const StreamParams &sp, const uint
       if (j == nw - 1) alt[j] &= last_mask;
     const uint32_t crc = crc24_words(alt, body, sp.crc_init, crc4);
     const uint32_t rx = (sym_bits32<ROT>(w, s0 + 4 * 8 * body, c4, s4) ^ whiten32(sp, body)) & 0xFFFFFFu;
-    if (crc == rx) {
+    if (t < 4 ? crc == rx : correct_words(alt, nbytes, sp, crc ^ rx, tab)) {
 #pragma unroll
       for (int j = 0; j < 11; ++j) words[j] = alt[j];
       nbytes_out = nbytes;
-      return q;
+      return t;
     }
   }
   return -1;
 }
 // flags bits a recovered record carries on top of the primary decode's (alternative q)
 BTLE_HD uint32_t recovered_flags(int q) { return q < 0 ? 0u : (uint32_t)(BTLE_REC_RECOVERED | (q << 4)); }
+
+// BTLE_CFG_RECOVER and BTLE_CFG_CORRECT on one counted packet whose primary decode (words, nbytes) failed the CRC, in the
+// order of include/btle_b200.h (fewer assumed errors win): the alternatives exact, the primary decode corrected, the
+// alternatives corrected.  Returns the flags bits the record gets on top of the primary decode's, with the winner's bytes
+// in words and its n_bytes in nbytes; 0 when nothing passes (words and nbytes untouched).
+template <bool ROT = false>
+BTLE_HD uint32_t repair_packet(const IqWindow &w, const StreamParams &sp, const uint32_t *crc4, const uint64_t *tab, int n0,
+                               uint32_t words[11], int &nbytes, int c4 = 0, int s4 = 0) {
+  if (!sp.recover) return (sp.correct && correct_packet(words, nbytes, sp, crc4, tab)) ? (uint32_t)BTLE_REC_CORRECTED : 0u;
+  const int t = recover_packet<ROT>(w, sp, crc4, n0, words, nbytes, c4, s4, sp.correct ? tab : nullptr);
+  if (t < 4) return recovered_flags(t);                                   // -1: nothing passes
+  return t == 4 ? (uint32_t)BTLE_REC_CORRECTED : recovered_flags(t - 5) | BTLE_REC_CORRECTED;
+}
 
 // Both parts back to back for one chunk (what the test-only CPU emulator runs, lane by lane):
 // emit(n0, n_bytes, crc_bad, words[11], rejected) per counted (or, with report_rejected, rejected) hit, in the reference's order.

@@ -71,6 +71,7 @@ BTLE_HD void make_params(const btle_stream_cfg &cfg, const uint32_t *whiten_word
   sp.report_rejected = (cfg.rssi & BTLE_CFG_REPORT_REJECTED) ? 1 : 0;
   sp.centre_hits = (cfg.rssi & BTLE_CFG_CENTRE_HITS) ? 1 : 0;
   sp.recover = ((cfg.rssi & BTLE_CFG_RECOVER) && !cfg.raw) ? 1 : 0;
+  sp.correct = ((cfg.rssi & BTLE_CFG_CORRECT) && !cfg.raw) ? 1 : 0;
   const uint32_t am = cfg.access_addr & cfg.access_mask;
   int tz = 0;
   while (tz < 31 && !((am >> tz) & 1u)) ++tz;

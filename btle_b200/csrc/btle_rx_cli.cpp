@@ -69,7 +69,8 @@ const char *CTRL_NAME[15] = {"LL_CONNECTION_UPDATE_REQ", "LL_CHANNEL_MAP_REQ", "
                              "LL_REJECT_IND", "LL_RESERVED"};                              // :1060-1076
 
 struct Options {
-  int chan = 37, gain = 6, lna = 32, amp = 0, verbose = 0, raw = 0, hop = 0, json = 0, quiet = 0, rssi = 0, recover = 0, symbol_spaced = 0, centre_hits = 0;
+  int chan = 37, gain = 6, lna = 32, amp = 0, verbose = 0, raw = 0, hop = 0, json = 0, quiet = 0, rssi = 0, recover = 0, symbol_spaced = 0, centre_hits = 0,
+      correct = 0;
   uint32_t aa = 0x8E89BED6u, crc_init = 0x555555u, mask = 0xFFFFFFFFu;
   uint64_t freq_hz = 123;
   const char *pcap = nullptr, *iq_txt = nullptr, *iq_sc16 = nullptr, *iq_dir = nullptr, *iq_bin16 = nullptr;
@@ -115,6 +116,9 @@ void usage() {
       "    -j --json / -Q --quiet-text / -R --rssi-est\n"
       "       --recover\n      packets whose CRC fails are demodulated once more, symbol-spaced on four sample phases; the first\n"
       "      phase whose CRC is ok replaces the packet (printed as CRC0; NDJSON adds \"recovered\":q).  Not with -o or --iq-bin16\n"
+      "       --correct\n      a packet whose CRC fails and whose CRC syndrome is that of one wrong bit or two adjacent wrong bits\n"
+      "      (not in the length field) is corrected (printed as CRC0; NDJSON adds \"corrected\":true); with --recover after\n"
+      "      its exact phases.  Applies to every cfg, --connections included.  Not with -o or --iq-bin16\n"
       "       --offset HZ|auto\n      carrier-offset correction of every capture, HZ = received minus nominal carrier (|HZ| <= 500000); a capture\n"
       "      given as FILE:CH:AA:CRCINIT:HZ takes its own.  auto (regular files only): a first pass without correction, the\n"
       "      median offset estimate of its CRC-ok packets printed on stderr, then the decode with it.  Not with --iq-bin16\n"
@@ -170,7 +174,7 @@ Options parse_commandline(int argc, char **argv) {
       {"filter-pdu-type", required_argument, 0, 'T'}, {"iq-file", required_argument, 0, 'i'},
       {"iq-txt", required_argument, 0, 1000}, {"iq-sc16", required_argument, 0, 1001}, {"device", required_argument, 0, 'd'},
       {"iq-dir", required_argument, 0, 1002}, {"segment-chunks", required_argument, 0, 1003}, {"iq-bin16", required_argument, 0, 1004},
-      {"connections", no_argument, 0, 1005}, {"recover", no_argument, 0, 1006},
+      {"connections", no_argument, 0, 1005}, {"recover", no_argument, 0, 1006}, {"correct", no_argument, 0, 1010},
       {"offset", required_argument, 0, 1007}, {"symbol-spaced", no_argument, 0, 1008},
       {"centre-hits", no_argument, 0, 1009}, {0, 0, 0, 0}};
   for (;;) {
@@ -199,6 +203,7 @@ Options parse_commandline(int argc, char **argv) {
       case 1004: o.iq_bin16 = optarg; break;
       case 1005: o.connections = 1; break;
       case 1006: o.recover = 1; break;
+      case 1010: o.correct = 1; break;
       case 1008: o.symbol_spaced = 1; break;
       case 1009: o.centre_hits = 1; break;
       case 1007:
@@ -237,6 +242,7 @@ Options parse_commandline(int argc, char **argv) {
   if (o.connections && (!o.iq_dir || o.hop)) { printf("--connections needs --iq-dir and cannot be combined with -o\n"); bad_args(); }
   // -o follows as the reference's follower does, from the reference's records; --iq-bin16 has a receiver of its own
   if (o.recover && (o.hop || o.iq_bin16)) { printf("--recover cannot be combined with -o or --iq-bin16\n"); bad_args(); }
+  if (o.correct && (o.hop || o.iq_bin16)) { printf("--correct cannot be combined with -o or --iq-bin16\n"); bad_args(); }
   // the 8-sps model receiver has no carrier-offset correction
   if (o.offset_set && o.iq_bin16) { printf("--offset cannot be combined with --iq-bin16 (the 8-sps receiver has no offset correction)\n"); bad_args(); }
   if (o.symbol_spaced && o.iq_bin16) { printf("--symbol-spaced cannot be combined with --iq-bin16 (the 8-sps receiver has its own discriminator)\n"); bad_args(); }
@@ -472,6 +478,7 @@ struct Sinks {
         printf(",\"payload_hex\":"); json_hex(b + 2, plen);
         if (rssi == INT_MIN) printf(",\"rssi_est\":null"); else printf(",\"rssi_est\":%d", rssi);
         if (r.flags & BTLE_REC_RECOVERED) printf(",\"recovered\":%d", BTLE_REC_RECOVERED_Q(r.flags));
+        if (r.flags & BTLE_REC_CORRECTED) printf(",\"corrected\":true");
         printf("}\n");
       }
     } else {
@@ -494,6 +501,7 @@ struct Sinks {
         json_hex(b + 2, plen);
         if (rssi == INT_MIN) printf(",\"rssi_est\":null"); else printf(",\"rssi_est\":%d", rssi);
         if (r.flags & BTLE_REC_RECOVERED) printf(",\"recovered\":%d", BTLE_REC_RECOVERED_Q(r.flags));
+        if (r.flags & BTLE_REC_CORRECTED) printf(",\"corrected\":true");
         printf("}\n");
       }
     }
@@ -584,7 +592,8 @@ Capture parse_capture(const std::string &spec, const Options &o) {
 
 int cfg_flags(const Options &o) {
   return (o.rssi ? BTLE_CFG_RSSI : 0) | (o.verbose ? BTLE_CFG_REPORT_REJECTED : 0) | (o.recover ? BTLE_CFG_RECOVER : 0) |
-         (o.symbol_spaced ? BTLE_CFG_SYMBOL_SPACED : 0) | (o.centre_hits ? BTLE_CFG_CENTRE_HITS : 0);
+         (o.symbol_spaced ? BTLE_CFG_SYMBOL_SPACED : 0) | (o.centre_hits ? BTLE_CFG_CENTRE_HITS : 0) |
+         (o.correct ? BTLE_CFG_CORRECT : 0);
 }
 
 int fail(btle_b200_ctx *ctx, int rc, const char *what) {
@@ -686,7 +695,7 @@ struct ConnMonitor {
     for (int ch = 0; ch < 37 && !rc; ++ch) {
       const btle_stream_cfg cfg{ch, c.aa, 0xFFFFFFFFu, c.crc_init, 0,
                                 (o.rssi ? BTLE_CFG_RSSI : 0) | (o.recover ? BTLE_CFG_RECOVER : 0) | (o.symbol_spaced ? BTLE_CFG_SYMBOL_SPACED : 0) |
-                                    (o.centre_hits ? BTLE_CFG_CENTRE_HITS : 0)};
+                                    (o.centre_hits ? BTLE_CFG_CENTRE_HITS : 0) | (o.correct ? BTLE_CFG_CORRECT : 0)};
       size_t j = 0;
       rc = btle_b200_streams_add_cfg(ss, (size_t)ch, &cfg, from, &j);
       c.cfgs.push_back(j);

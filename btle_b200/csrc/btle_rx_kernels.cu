@@ -44,6 +44,7 @@ using namespace btle;
 // reference's scramble_table.h / crc_table in tests)
 __constant__ uint32_t c_whiten_words[40][12];
 __constant__ uint32_t c_crc4[1024];
+__device__ uint64_t g_syndrome[kSyndromeSlots];          // BTLE_CFG_CORRECT's table (make_syndrome_table), read through __ldg
 __constant__ int8_t c_cos1024[1024], c_sin1024[1024];   // round(127 cos/sin(2 pi k/1024)), gauss_cos_sin_table.h
 __constant__ int8_t c_cos2048[2048], c_sin2048[2048];   // btlelib.py:52-66 (sin_cos_gen)
 __constant__ int c_gauss4[9] = {2, 11, 32, 53, 60, 53, 32, 11, 2};                       // btle_tx.c gauss_coef_int8[4..12]
@@ -234,18 +235,20 @@ __device__ __forceinline__ void store_record(btle_pkt_rec *dst, int stream, int 
   for (int q = 0; q < 4; ++q) d4[q] = make_uint4(r[4 * q], r[4 * q + 1], r[4 * q + 2], r[4 * q + 3]);
 }
 
-// BTLE_CFG_RECOVER: stores the record of a counted packet whose primary decode failed the CRC when one of its
-// alternatives passes (recover_packet) and returns true; false: nothing stored, the caller stores the primary decode.
-// Out of line, so that the decode pass keeps its registers and the launches of cfgs without the flag pay one branch.
-// ROT: the symbol-spaced bits are rotated by (c4, s4) (carrier-offset correction).
+// BTLE_CFG_RECOVER / BTLE_CFG_CORRECT: stores the record of a counted packet whose primary decode (primary, nbytes) failed
+// the CRC when an alternative passes or a correction applies (repair_packet) and returns true; false: nothing stored, the
+// caller stores the primary decode.  Out of line, so that the decode pass keeps its registers and the launches of cfgs
+// without either flag pay one branch.  ROT: the symbol-spaced bits are rotated by (c4, s4) (carrier-offset correction).
 template <bool ROT>
-__device__ __forceinline__ bool store_recovered(btle_pkt_rec *dst, int stream, int chunk, int n0, const StreamParams &sp, const uint32_t *crc4,
-                                             const int8_t *iq, long long n_int8, long long lead, int c4 = 0, int s4 = 0) {
+__device__ __forceinline__ bool store_repaired(btle_pkt_rec *dst, int stream, int chunk, int n0, const StreamParams &sp, const uint32_t *crc4,
+                                               const uint32_t primary[11], int nbytes, const int8_t *iq, long long n_int8, long long lead,
+                                               int c4 = 0, int s4 = 0) {
   uint32_t words[11];
-  int nbytes = 0;
-  const int q = recover_packet<ROT>(iq_window(iq, n_int8, chunk), sp, crc4, n0, words, nbytes, c4, s4);
-  if (q < 0) return false;
-  store_record(dst, stream, chunk, n0, nbytes, 0, false, words, sp, iq, n_int8, lead, recovered_flags(q));
+#pragma unroll
+  for (int j = 0; j < 11; ++j) words[j] = primary[j];
+  const uint32_t extra = repair_packet<ROT>(iq_window(iq, n_int8, chunk), sp, crc4, g_syndrome, n0, words, nbytes, c4, s4);
+  if (!extra) return false;
+  store_record(dst, stream, chunk, n0, nbytes, 0, false, words, sp, iq, n_int8, lead, extra);
   return true;
 }
 
@@ -752,11 +755,14 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
           }
           // 3b. BTLE_CFG_RECOVER (uniform per cfg): a counted packet whose CRC failed is demodulated again from the
           //     capture's IQ, symbol-spaced on four sample phases; the lanes that need it run it together
+          // 3c. BTLE_CFG_CORRECT (uniform per cfg): such a packet's one-bit or adjacent-pair error is corrected from its CRC
+          //     syndrome, after the exact alternatives and before the corrected ones (repair_packet)
           const unsigned base = __shfl_sync(0xFFFFFFFFu, my_base, 0);
           bool stored = false;
-          if (sp.recover) {
+          if (sp.recover | sp.correct) {
             if (live && crc_bad && !rej && base + (unsigned)j < cap)
-              stored = store_recovered<ROT>(out + base + j, rec_stream, si.chunk0 + c, n0, sp, M.crc4, cap_base, n_int8, lead, c4, s4);
+              stored = store_repaired<ROT>(out + base + j, rec_stream, si.chunk0 + c, n0, sp, M.crc4, words, nbytes, cap_base, n_int8, lead,
+                                           c4, s4);
           }
           if (live && !stored && base + (unsigned)j < cap)
             store_record(out + base + j, rec_stream, si.chunk0 + c, n0, nbytes, crc_bad, rej, words, sp, cap_base, n_int8, lead);
@@ -774,8 +780,9 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
                 uint32_t words[11];
                 int nbytes, crc_bad;
                 decode_packet(pd, sp, crc4, n0, rej, words, nbytes, crc_bad);
-                if (sp.recover && crc_bad && !rej && store_recovered<ROT>(out + first + i, stream, chunk, n0, sp, crc4, iq, n_int8, lead, c4, s4))
-                  return;                                             // as step 3b
+                if ((sp.recover | sp.correct) && crc_bad && !rej &&
+                    store_repaired<ROT>(out + first + i, stream, chunk, n0, sp, crc4, words, nbytes, iq, n_int8, lead, c4, s4))
+                  return;                                             // as steps 3b, 3c
                 store_record(out + first + i, stream, chunk, n0, nbytes, crc_bad, rej, words, sp, iq, n_int8, lead);
               }
             };
@@ -2590,6 +2597,7 @@ int btle_b200_create(btle_b200_ctx **out, int cuda_device) {
       return BTLE_ECUDA;
     }
   }
+  std::vector<uint64_t> syn(kSyndromeSlots);
   uint32_t thr[13];
   for (int k = 0; k < 13; ++k) {                         // P(round(N(-0.3, 0.8)) <= v), v = -7 + k
     const double p = 0.5 * erfc(-(((double)(-7 + k) + 0.5 + 0.3) / 0.8) / sqrt(2.0));
@@ -2597,7 +2605,8 @@ int btle_b200_create(btle_b200_ctx **out, int cuda_device) {
   }
   if (cudaMemcpyToSymbol(c_noise_thr, thr, sizeof thr) != cudaSuccess ||
       cudaMemcpyToSymbol(c_whiten_words, ww, sizeof ww) != cudaSuccess ||
-      cudaMemcpyToSymbol(c_crc4, crc, sizeof crc) != cudaSuccess ||
+      cudaMemcpyToSymbol(c_crc4, crc, sizeof crc) != cudaSuccess || make_syndrome_table(syn.data()) != kCorrectPatterns ||
+      cudaMemcpyToSymbol(g_syndrome, syn.data(), sizeof(uint64_t) * kSyndromeSlots) != cudaSuccess ||
       cudaFuncSetAttribute(btle_rx_persistent_kernel<1, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem<1>)) != cudaSuccess ||
       cudaFuncSetAttribute(btle_rx_persistent_kernel<kMaxCfgsPerCapture, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            (int)sizeof(Smem<kMaxCfgsPerCapture>)) != cudaSuccess ||
@@ -3781,8 +3790,8 @@ static int check_rx_ber_cfg(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg) {
   }
   if (std::fabs(cfg->ppm) >= 1e6f) { ctx->err = "rx_ber: ppm must have |ppm| < 1e6"; return BTLE_EINVAL; }
   if (cfg->amplitude < 1 || cfg->amplitude > 127) { ctx->err = "rx_ber: amplitude must be 1..127"; return BTLE_EINVAL; }
-  if (cfg->flags & ~(uint32_t)(BTLE_CFG_RECOVER | BTLE_CFG_SYMBOL_SPACED | BTLE_CFG_CENTRE_HITS)) {
-    ctx->err = "rx_ber: flags may only hold BTLE_CFG_RECOVER, BTLE_CFG_SYMBOL_SPACED and BTLE_CFG_CENTRE_HITS";
+  if (cfg->flags & ~(uint32_t)(BTLE_CFG_RECOVER | BTLE_CFG_SYMBOL_SPACED | BTLE_CFG_CENTRE_HITS | BTLE_CFG_CORRECT)) {
+    ctx->err = "rx_ber: flags may only hold BTLE_CFG_RECOVER, BTLE_CFG_SYMBOL_SPACED, BTLE_CFG_CENTRE_HITS and BTLE_CFG_CORRECT";
     return BTLE_EINVAL;
   }
   if (cfg->slot_samples < rx_ber_len(cfg->channel) || cfg->slot_samples > BTLE_RX_BER_MAX_SLOT) {

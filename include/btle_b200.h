@@ -71,7 +71,8 @@ typedef struct {
                             of them, in the reference's order (up to BTLE_MAX_RECS_PER_CHUNK records per chunk);
                             BTLE_CFG_RECOVER 4: CRC-failed packets are demodulated once more (below);
                             BTLE_CFG_SYMBOL_SPACED 16: the symbol-spaced discriminator (below);
-                            BTLE_CFG_CENTRE_HITS 64: each hit centred on its run of matching phases (below)      */
+                            BTLE_CFG_CENTRE_HITS 64: each hit centred on its run of matching phases (below);
+                            BTLE_CFG_CORRECT 256: one-bit and adjacent-pair errors corrected by the CRC (below)  */
 } btle_stream_cfg;
 #define BTLE_CFG_RSSI 1
 #define BTLE_CFG_REPORT_REJECTED 2
@@ -95,6 +96,29 @@ typedef struct {
  * Rejected (BTLE_CFG_REPORT_REJECTED) records, raw-mode records and CRC-ok records are never touched; the flag does
  * nothing in raw mode. */
 #define BTLE_CFG_RECOVER 4
+/* BTLE_CFG_CORRECT: opt-in CRC-24 syndrome decoding of packets that fail the CRC.  Not part of the reference's receiver;
+ * without it the records are the reference's (or the current mode's), bit for bit.  It applies only to a COUNTED record
+ * with crc_bad == 1 of a cfg with the flag and raw == 0:
+ *   1. chain     which hits are counted or rejected, their n0, the restart points, the length guards and n_bytes are
+ *                unchanged.  The header's length field is never corrected (another length would move the CRC field).
+ *   2. patterns  the packet bits in the order sent (the dewhitened bytes, LSB first): body bits 0 .. 8 (n_bytes - 3) - 1,
+ *                then the 24 CRC bits.  The patterns are every single bit and every pair of adjacent bits, except those
+ *                touching the length field: header bits 8..13 on channels 37..39, 8..12 on channels 0..36.  (Whitening is
+ *                an XOR, so an error in the air is an error at the same place in the dewhitened bits.)
+ *   3. syndrome  s = crc24(body) XOR the received CRC.  It depends only on an error's distance from the packet's end, so
+ *                one table of the 671 patterns of the longest body (39 bytes) serves every length; their syndromes are
+ *                distinct and non-zero.  If s is the syndrome of exactly one allowed pattern, that pattern's bits are
+ *                flipped in bytes, crc_bad = 0 and flags gets BTLE_REC_CORRECTED.  Otherwise the record stays as it was.
+ *                stream, chunk, n0, channel, n_bytes, access_addr and mag_sum never change.
+ *   4. order     with BTLE_CFG_RECOVER too, fewer assumed errors win: the primary decode exact (the reference), then
+ *                BTLE_CFG_RECOVER's alternatives q = 0..3 exact (a record identical to a RECOVER-only run), then the
+ *                primary decode corrected, then the alternatives q = 0..3 corrected (first q wins; flags gets
+ *                BTLE_REC_RECOVERED, q in bits 4..5 and BTLE_REC_CORRECTED; n_bytes is the alternative's).
+ * A CRC-failed packet with no allowed pattern is "corrected" to wrong bytes when its syndrome happens to equal one of the
+ * allowed ones: about 671 / 2^24 = 4.0e-5 of such packets if their syndromes were uniform.  The flag works in every
+ * discriminator mode, with and without carrier-offset correction and BTLE_CFG_CENTRE_HITS; it is per cfg (like
+ * BTLE_CFG_RECOVER).  btle_rx_ber_cfg.flags accepts it too. */
+#define BTLE_CFG_CORRECT 256
 /* BTLE_CFG_SYMBOL_SPACED: opt-in symbol-spaced discriminator.  Not part of the reference's receiver; without it the records
  * are the reference's, bit for bit.  With it every discriminator bit of the capture is
  *     d[n] = I[n-2] Q[n+2] - I[n+2] Q[n-2] > 0      (int32; x[n] = sample n of the capture)
@@ -155,7 +179,8 @@ typedef struct {
   uint8_t crc_bad;       /* crc_check() verdict, 1 = mismatch (btle_rx.c:2015); 0 in raw mode */
   uint8_t flags;         /* bit0 raw, bit1 advertising channel, bit2 BTLE_REC_REJECTED: not a packet the
                             reference counts — only bytes[0..1] (the header) are valid, n_bytes = 2;
-                            bit3 BTLE_REC_RECOVERED: bytes from alternative q = bits 4..5 (BTLE_CFG_RECOVER) */
+                            bit3 BTLE_REC_RECOVERED: bytes from alternative q = bits 4..5 (BTLE_CFG_RECOVER);
+                            bit6 BTLE_REC_CORRECTED: bytes corrected by the CRC syndrome (BTLE_CFG_CORRECT) */
   uint32_t access_addr;
   uint16_t mag_sum;      /* sum |I|+|Q| over the 128 AA samples if cfg.rssi, else 0           */
   uint8_t bytes[42];     /* == reference tmp_byte[] (btle_rx.c:1485): dewhitened header,
@@ -165,6 +190,7 @@ typedef struct {
 #define BTLE_REC_REJECTED 4
 #define BTLE_REC_RECOVERED 8
 #define BTLE_REC_RECOVERED_Q(flags) (((flags) >> 4) & 3)
+#define BTLE_REC_CORRECTED 64
 
 typedef struct btle_b200_ctx btle_b200_ctx;
 
@@ -581,8 +607,8 @@ typedef struct {
   int32_t channel;         /* 0..39                                                                                 */
   uint32_t access_addr;
   uint32_t crc_init;       /* as -k                                                                                 */
-  uint32_t flags;          /* any of BTLE_CFG_RECOVER, BTLE_CFG_SYMBOL_SPACED and BTLE_CFG_CENTRE_HITS (given to the
-                              receiver); any other bit: BTLE_EINVAL                                                   */
+  uint32_t flags;          /* any of BTLE_CFG_RECOVER, BTLE_CFG_SYMBOL_SPACED, BTLE_CFG_CENTRE_HITS and BTLE_CFG_CORRECT
+                              (given to the receiver); any other bit: BTLE_EINVAL                                     */
   uint32_t reserved;       /* 0                                                                                     */
 } btle_rx_ber_cfg;         /* 48 bytes */
 typedef struct {
@@ -610,7 +636,7 @@ typedef struct {
  * BTLE_CFG_SYMBOL_SPACED a batch also reads the 2 samples in front of it and 2 more behind its look-ahead).
  * BTLE_EINVAL with btle_b200_last_error() for: snr_db, ppm or cfo_hz NaN or infinite, |ppm| >= 1e6, amplitude outside
  * 1..127, slot_samples below L or above BTLE_RX_BER_MAX_SLOT, channel > 39, a flags bit other than BTLE_CFG_RECOVER,
- * BTLE_CFG_SYMBOL_SPACED and BTLE_CFG_CENTRE_HITS;
+ * BTLE_CFG_SYMBOL_SPACED, BTLE_CFG_CENTRE_HITS and BTLE_CFG_CORRECT;
  * the context stays usable. */
 int btle_b200_rx_ber_run(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg, size_t n_packets, btle_rx_ber_result *out);
 /* the capture and truth of packets first_packet .. first_packet + n_packets - 1 alone: d_iq (16-byte aligned) receives
