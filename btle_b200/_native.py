@@ -80,6 +80,7 @@ CFG_RSSI, CFG_REPORT_REJECTED, CFG_RECOVER = 1, 2, 4      # btle_stream_cfg.rssi
 CFG_SYMBOL_SPACED = 16       # BTLE_CFG_SYMBOL_SPACED: symbol-spaced discriminator (one mode per launch / session)
 CFG_CENTRE_HITS = 64         # BTLE_CFG_CENTRE_HITS: each hit moved to the centre of its run of matching sample phases (per cfg)
 CFG_CORRECT = 256            # BTLE_CFG_CORRECT: one-bit and adjacent-pair errors of CRC-failed packets corrected (per cfg)
+CFG_LOWPASS = 512            # BTLE_CFG_LOWPASS: [1, 2, 1] low-pass in front of the symbol-spaced bits (with CFG_SYMBOL_SPACED, one mode per launch)
 MAX_OFFSET_HZ = 500000       # BTLE_MAX_OFFSET_HZ: largest |offset_hz| of the carrier-offset correction
 REC_REJECTED, REC_RECOVERED = 4, 8                        # btle_pkt_rec.flags bits; a recovered record's alternative q is flags >> 4 & 3
 REC_CORRECTED = 64                                        # btle_pkt_rec.flags bit: bytes corrected by the CRC syndrome

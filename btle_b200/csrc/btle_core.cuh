@@ -474,6 +474,24 @@ BTLE_DENSE void dbits_group_sym(WordAt &word, int c, int s, uint32_t acc[4]) {
   }
 }
 
+// ---- low-pass in front of the symbol-spaced bits (BTLE_CFG_LOWPASS, include/btle_b200.h) ---------------------------------
+// F[n] = (x[n-1] + 2 x[n] + x[n+1]) >> 2 per rail = avg(avg(x[n-1], x[n+1]), x[n]) with avg(a, b) = floor((a + b) / 2) (the
+// nested floors are exact).  A signed per-byte avg is the unsigned one in offset binary (bytes XOR 0x80), and the unsigned one
+// is (x & y) + (((x ^ y) >> 1) & 0x7F7F7F7F), which never carries across bytes.
+BTLE_HD uint32_t avg_u8x4(uint32_t x, uint32_t y) { return (x & y) + (((x ^ y) >> 1) & 0x7F7F7F7Fu); }
+// the filtered IQ word of w (samples 2k, 2k + 1) from the words in front of (wprev) and behind (wnext) it
+BTLE_HD uint32_t lp_word(uint32_t wprev, uint32_t w, uint32_t wnext) {
+  const uint32_t p = wprev ^ 0x80808080u, c = w ^ 0x80808080u, n = wnext ^ 0x80808080u;
+  const uint32_t l = funnel_r(p, c, 16u), r = funnel_r(c, n, 16u);   // samples 2k - 1, 2k and 2k + 1, 2k + 2
+  return avg_u8x4(avg_u8x4(l, r), c) ^ 0x80808080u;
+}
+// dbits_group_sym() on the filtered words: word(-2) .. word(65) are read
+template <bool ROT, class WordAt>
+BTLE_DENSE void dbits_group_lowpass(WordAt &word, int c, int s, uint32_t acc[4]) {
+  auto fword = [&](int k) { return lp_word(word(k - 1), word(k), word(k + 1)); };
+  dbits_group_sym<ROT>(fword, c, s, acc);
+}
+
 // Dense-pass prefilter: bit i of the result is 1 iff the window starting at symbol i of `lo`
 // agrees with the access address on the (<=16) prefilter taps.  A superset of the true matches;
 // the sparse pass re-checks every candidate exactly (search_from()).
@@ -929,15 +947,20 @@ BTLE_HD bool correct_packet(uint32_t words[11], int nbytes, const StreamParams &
 // ---- recovery of CRC-failed packets (BTLE_CFG_RECOVER, include/btle_b200.h) --------------------------------------------
 // The capture samples one chunk's recovery may read: sample s (relative to the chunk) is iq[2s], iq[2s+1] for 0 <= s < n,
 // n = what the capture holds of the chunk's receiver() window [0, kWinInt8 / 2); every other sample reads 0.
+// BTLE_CFG_LOWPASS reads the filtered samples F[s] (lp_at) under the same window rule; their neighbours x[s - 1], x[s + 1]
+// come from the capture, readable for lo <= s < hi (`lead` bytes in front of the capture, nothing behind its end).
 struct IqWindow {
   const int8_t *iq;            // the chunk's first sample
   int n;
+  int lo, hi;
 };
-BTLE_HD IqWindow iq_window(const int8_t *capture, long long n_int8, long long chunk) {
+BTLE_HD IqWindow iq_window(const int8_t *capture, long long n_int8, long long chunk, long long lead = 0) {
   const long long base = chunk * kChunkInt8, avail = (n_int8 - base) >> 1;
   IqWindow w;
   w.iq = capture + base;
   w.n = avail < 0 ? 0 : (avail > kWinInt8 / 2 ? kWinInt8 / 2 : (int)avail);
+  w.lo = (base + lead) >= 2 ? -1 : 0;
+  w.hi = avail < 0 ? 0 : (avail > kWinInt8 / 2 + 1 ? kWinInt8 / 2 + 1 : (int)avail);
   return w;
 }
 // I and Q of sample s (0 outside the window)
@@ -945,17 +968,30 @@ BTLE_HD void iq_at(const IqWindow &w, int s, int &i, int &q) {
   i = q = 0;
   if (s >= 0 && s < w.n) { i = w.iq[2 * s]; q = w.iq[2 * s + 1]; }
 }
+// I and Q of the filtered sample F[s] (0 outside the window)
+BTLE_HD void lp_at(const IqWindow &w, int s, int &i, int &q) {
+  i = q = 0;
+  if (s < 0 || s >= w.n) return;
+  int im = 0, qm = 0, ip = 0, qp = 0;
+  if (s - 1 >= w.lo) { im = w.iq[2 * s - 2]; qm = w.iq[2 * s - 1]; }
+  if (s + 1 < w.hi) { ip = w.iq[2 * s + 2]; qp = w.iq[2 * s + 3]; }
+  i = (im + 2 * w.iq[2 * s] + ip) >> 2;
+  q = (qm + 2 * w.iq[2 * s + 1] + qp) >> 2;
+}
 // Symbol-spaced discriminator bits: bit k of the result is e[s0 + 4k], e[s] = (I[s] Q[s+4] - I[s+4] Q[s]) > 0.
 // ROT: e[s] = C4 (I[s] Q[s+4] - I[s+4] Q[s]) - S4 (I[s] I[s+4] + Q[s] Q[s+4]) > 0 (rot_disc with the 4-sample rotation).
-template <bool ROT = false>
+// LP (BTLE_CFG_LOWPASS): the same bits of the filtered samples.
+template <bool ROT = false, bool LP = false>
 BTLE_HD uint32_t sym_bits32(const IqWindow &w, int s0, int c4 = 0, int s4 = 0) {
   int i0, q0;
-  iq_at(w, s0, i0, q0);
+  if constexpr (LP) lp_at(w, s0, i0, q0);
+  else iq_at(w, s0, i0, q0);
   uint32_t r = 0u;
 #pragma unroll 4
   for (int k = 0; k < 32; ++k) {
     int i1, q1;
-    iq_at(w, s0 + 4 * k + 4, i1, q1);
+    if constexpr (LP) lp_at(w, s0 + 4 * k + 4, i1, q1);
+    else iq_at(w, s0 + 4 * k + 4, i1, q1);
     if constexpr (ROT) r |= (uint32_t)(rot_disc(i0, q0, i1, q1, c4, s4) < 0) << k;
     else r |= (uint32_t)(i0 * q1 - i1 * q0 > 0) << k;
     i0 = i1;
@@ -966,11 +1002,12 @@ BTLE_HD uint32_t sym_bits32(const IqWindow &w, int s0, int c4 = 0, int s4 = 0) {
 // One counted packet whose access address starts at sample n0 and whose primary decode failed the CRC: alternatives
 // q = 0..3 (packet bit j = e[n0 + 4j + q - 2]) in order; the first whose CRC is good wins.  Returns q and writes that
 // alternative's bytes (words[11], zero behind n_bytes, as decode_packet) and n_bytes; returns -1 and leaves both
-// untouched when none passes.  Not for raw mode (sp.recover is 0 there).  ROT: the bits of sym_bits32<true>(.., c4, s4).
+// untouched when none passes.  Not for raw mode (sp.recover is 0 there).  ROT: the bits of sym_bits32<true>(.., c4, s4);
+// LP: of the filtered samples (BTLE_CFG_LOWPASS).
 // tab (BTLE_CFG_CORRECT; words, nbytes_out: the primary decode): when no alternative passes, steps on in repair_packet's
 // order: returns 4 when correct_packet corrects the primary decode in words, else 5 + q for the first alternative q that
 // correct_words corrects.  One loop for both, so that the kernel holds one alternative's words, not two.
-template <bool ROT = false>
+template <bool ROT = false, bool LP = false>
 BTLE_HD int recover_packet(const IqWindow &w, const StreamParams &sp, const uint32_t *crc4, int n0, uint32_t words[11], int &nbytes_out,
                            int c4 = 0, int s4 = 0, const uint64_t *tab = nullptr) {
   const int steps = tab ? 9 : 4;
@@ -982,18 +1019,18 @@ BTLE_HD int recover_packet(const IqWindow &w, const StreamParams &sp, const uint
     const int q = t < 4 ? t : t - 5;                     // exact, then corrected
     const int s0 = n0 + 4 * 32 + q - 2;                  // packet bit 32: the first header bit
     uint32_t alt[11];
-    alt[0] = sym_bits32<ROT>(w, s0, c4, s4) ^ sp.whiten[0];
+    alt[0] = sym_bits32<ROT, LP>(w, s0, c4, s4) ^ sp.whiten[0];
     const int plen = (int)((alt[0] >> 8) & (sp.adv ? 0x3Fu : 0x1Fu));
     if (sp.adv && (plen < 6 || plen > 37)) continue;
     const int nbytes = plen + 5, nw = (nbytes + 3) >> 2, body = nbytes - 3;
     const uint32_t last_mask = (nbytes & 3) ? ((1u << (8 * (nbytes & 3))) - 1u) : 0xFFFFFFFFu;
 #pragma unroll
-    for (int j = 1; j < 11; ++j) alt[j] = j < nw ? sym_bits32<ROT>(w, s0 + 4 * 32 * j, c4, s4) ^ sp.whiten[j] : 0u;
+    for (int j = 1; j < 11; ++j) alt[j] = j < nw ? sym_bits32<ROT, LP>(w, s0 + 4 * 32 * j, c4, s4) ^ sp.whiten[j] : 0u;
 #pragma unroll
     for (int j = 0; j < 11; ++j)
       if (j == nw - 1) alt[j] &= last_mask;
     const uint32_t crc = crc24_words(alt, body, sp.crc_init, crc4);
-    const uint32_t rx = (sym_bits32<ROT>(w, s0 + 4 * 8 * body, c4, s4) ^ whiten32(sp, body)) & 0xFFFFFFu;
+    const uint32_t rx = (sym_bits32<ROT, LP>(w, s0 + 4 * 8 * body, c4, s4) ^ whiten32(sp, body)) & 0xFFFFFFu;
     if (t < 4 ? crc == rx : correct_words(alt, nbytes, sp, crc ^ rx, tab)) {
 #pragma unroll
       for (int j = 0; j < 11; ++j) words[j] = alt[j];
@@ -1010,11 +1047,11 @@ BTLE_HD uint32_t recovered_flags(int q) { return q < 0 ? 0u : (uint32_t)(BTLE_RE
 // order of include/btle_b200.h (fewer assumed errors win): the alternatives exact, the primary decode corrected, the
 // alternatives corrected.  Returns the flags bits the record gets on top of the primary decode's, with the winner's bytes
 // in words and its n_bytes in nbytes; 0 when nothing passes (words and nbytes untouched).
-template <bool ROT = false>
+template <bool ROT = false, bool LP = false>
 BTLE_HD uint32_t repair_packet(const IqWindow &w, const StreamParams &sp, const uint32_t *crc4, const uint64_t *tab, int n0,
                                uint32_t words[11], int &nbytes, int c4 = 0, int s4 = 0) {
   if (!sp.recover) return (sp.correct && correct_packet(words, nbytes, sp, crc4, tab)) ? (uint32_t)BTLE_REC_CORRECTED : 0u;
-  const int t = recover_packet<ROT>(w, sp, crc4, n0, words, nbytes, c4, s4, sp.correct ? tab : nullptr);
+  const int t = recover_packet<ROT, LP>(w, sp, crc4, n0, words, nbytes, c4, s4, sp.correct ? tab : nullptr);
   if (t < 4) return recovered_flags(t);                                   // -1: nothing passes
   return t == 4 ? (uint32_t)BTLE_REC_CORRECTED : recovered_flags(t - 5) | BTLE_REC_CORRECTED;
 }

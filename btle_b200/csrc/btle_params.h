@@ -59,6 +59,14 @@ BTLE_HD uint32_t crc_init_reorder(uint32_t k) {
   return r;
 }
 
+// The receive kernel's discriminator mode (its DISC parameter), one per launch: the reference's quarter-symbol bit,
+// BTLE_CFG_SYMBOL_SPACED, or BTLE_CFG_SYMBOL_SPACED with BTLE_CFG_LOWPASS.
+enum : int { kDiscQuarter = 0, kDiscSymbol = 1, kDiscLowpass = 2 };
+BTLE_HD int disc_mode(const btle_stream_cfg &cfg) {
+  if (!(cfg.rssi & BTLE_CFG_SYMBOL_SPACED)) return kDiscQuarter;
+  return (cfg.rssi & BTLE_CFG_LOWPASS) ? kDiscLowpass : kDiscSymbol;
+}
+
 // whiten_words: 12 little-endian words of make_whiten_row(channel).
 BTLE_HD void make_params(const btle_stream_cfg &cfg, const uint32_t *whiten_words, StreamParams &sp) {
   sp.aa = cfg.access_addr;

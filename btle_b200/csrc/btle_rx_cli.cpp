@@ -70,7 +70,7 @@ const char *CTRL_NAME[15] = {"LL_CONNECTION_UPDATE_REQ", "LL_CHANNEL_MAP_REQ", "
 
 struct Options {
   int chan = 37, gain = 6, lna = 32, amp = 0, verbose = 0, raw = 0, hop = 0, json = 0, quiet = 0, rssi = 0, recover = 0, symbol_spaced = 0, centre_hits = 0,
-      correct = 0;
+      correct = 0, lowpass = 0;
   uint32_t aa = 0x8E89BED6u, crc_init = 0x555555u, mask = 0xFFFFFFFFu;
   uint64_t freq_hz = 123;
   const char *pcap = nullptr, *iq_txt = nullptr, *iq_sc16 = nullptr, *iq_dir = nullptr, *iq_bin16 = nullptr;
@@ -124,6 +124,9 @@ void usage() {
       "      median offset estimate of its CRC-ok packets printed on stderr, then the decode with it.  Not with --iq-bin16\n"
       "       --symbol-spaced\n      every discriminator bit compares samples one symbol apart (n-2, n+2) instead of a quarter symbol:\n"
       "      weaker packets are received; not the reference's receiver.  Applies to every capture.  Not with --iq-bin16\n"
+      "       --lowpass\n      with --symbol-spaced: every discriminator bit reads [1, 2, 1] low-pass filtered samples (less noise per\n"
+      "      bit); not the reference's receiver.  Applies to every capture, --recover's phases and the --offset auto pass\n"
+      "      included.  Only with --symbol-spaced, not with --iq-bin16\n"
       "       --centre-hits\n      each access-address hit is moved to the centre of its run of matching sample phases before the\n"
       "      packet is read: fewer length rejects and CRC failures; not the reference's receiver.  Applies to every cfg,\n"
       "      --connections and the --offset auto pass included.  Not with --iq-bin16\n"
@@ -176,7 +179,7 @@ Options parse_commandline(int argc, char **argv) {
       {"iq-dir", required_argument, 0, 1002}, {"segment-chunks", required_argument, 0, 1003}, {"iq-bin16", required_argument, 0, 1004},
       {"connections", no_argument, 0, 1005}, {"recover", no_argument, 0, 1006}, {"correct", no_argument, 0, 1010},
       {"offset", required_argument, 0, 1007}, {"symbol-spaced", no_argument, 0, 1008},
-      {"centre-hits", no_argument, 0, 1009}, {0, 0, 0, 0}};
+      {"centre-hits", no_argument, 0, 1009}, {"lowpass", no_argument, 0, 1011}, {0, 0, 0, 0}};
   for (;;) {
     int idx = 0;
     const int c = getopt_long(argc, argv, "hc:g:l:ba:k:vrf:m:os:jQRF:T:i:d:", longopts, &idx);   // + i:, d:
@@ -206,6 +209,7 @@ Options parse_commandline(int argc, char **argv) {
       case 1010: o.correct = 1; break;
       case 1008: o.symbol_spaced = 1; break;
       case 1009: o.centre_hits = 1; break;
+      case 1011: o.lowpass = 1; break;
       case 1007:
         o.offset_set = 1;
         if (!strcmp(optarg, "auto")) { o.offset_auto = 1; break; }
@@ -247,6 +251,7 @@ Options parse_commandline(int argc, char **argv) {
   if (o.offset_set && o.iq_bin16) { printf("--offset cannot be combined with --iq-bin16 (the 8-sps receiver has no offset correction)\n"); bad_args(); }
   if (o.symbol_spaced && o.iq_bin16) { printf("--symbol-spaced cannot be combined with --iq-bin16 (the 8-sps receiver has its own discriminator)\n"); bad_args(); }
   if (o.centre_hits && o.iq_bin16) { printf("--centre-hits cannot be combined with --iq-bin16 (the 8-sps receiver has its own hit rule)\n"); bad_args(); }
+  if (o.lowpass && (!o.symbol_spaced || o.iq_bin16)) { printf("--lowpass needs --symbol-spaced and cannot be combined with --iq-bin16\n"); bad_args(); }
   return o;
 }
 
@@ -593,7 +598,7 @@ Capture parse_capture(const std::string &spec, const Options &o) {
 int cfg_flags(const Options &o) {
   return (o.rssi ? BTLE_CFG_RSSI : 0) | (o.verbose ? BTLE_CFG_REPORT_REJECTED : 0) | (o.recover ? BTLE_CFG_RECOVER : 0) |
          (o.symbol_spaced ? BTLE_CFG_SYMBOL_SPACED : 0) | (o.centre_hits ? BTLE_CFG_CENTRE_HITS : 0) |
-         (o.correct ? BTLE_CFG_CORRECT : 0);
+         (o.correct ? BTLE_CFG_CORRECT : 0) | (o.lowpass ? BTLE_CFG_LOWPASS : 0);
 }
 
 int fail(btle_b200_ctx *ctx, int rc, const char *what) {
@@ -621,7 +626,7 @@ int rx_batch_grow(btle_b200_ctx *ctx, const int8_t *iq, size_t ns, size_t stride
 // Returns the exit status.
 int estimate_offset(btle_b200_ctx *ctx, const std::vector<int8_t> &iq, btle_stream_cfg cfg, const char *name, float *hz) {
   cfg.raw = 0;
-  cfg.rssi &= BTLE_CFG_SYMBOL_SPACED | BTLE_CFG_CENTRE_HITS;
+  cfg.rssi &= BTLE_CFG_SYMBOL_SPACED | BTLE_CFG_LOWPASS | BTLE_CFG_CENTRE_HITS;
   std::vector<btle_pkt_rec> recs;
   int rc = rx_batch_grow(ctx, iq.data(), 1, iq.size(), iq.size(), &cfg, recs);
   recs.erase(std::remove_if(recs.begin(), recs.end(), [](const btle_pkt_rec &r) { return r.crc_bad || (r.flags & BTLE_REC_REJECTED); }),
@@ -695,7 +700,8 @@ struct ConnMonitor {
     for (int ch = 0; ch < 37 && !rc; ++ch) {
       const btle_stream_cfg cfg{ch, c.aa, 0xFFFFFFFFu, c.crc_init, 0,
                                 (o.rssi ? BTLE_CFG_RSSI : 0) | (o.recover ? BTLE_CFG_RECOVER : 0) | (o.symbol_spaced ? BTLE_CFG_SYMBOL_SPACED : 0) |
-                                    (o.centre_hits ? BTLE_CFG_CENTRE_HITS : 0) | (o.correct ? BTLE_CFG_CORRECT : 0)};
+                                    (o.centre_hits ? BTLE_CFG_CENTRE_HITS : 0) | (o.correct ? BTLE_CFG_CORRECT : 0) |
+                                    (o.lowpass ? BTLE_CFG_LOWPASS : 0)};
       size_t j = 0;
       rc = btle_b200_streams_add_cfg(ss, (size_t)ch, &cfg, from, &j);
       c.cfgs.push_back(j);

@@ -238,15 +238,16 @@ __device__ __forceinline__ void store_record(btle_pkt_rec *dst, int stream, int 
 // BTLE_CFG_RECOVER / BTLE_CFG_CORRECT: stores the record of a counted packet whose primary decode (primary, nbytes) failed
 // the CRC when an alternative passes or a correction applies (repair_packet) and returns true; false: nothing stored, the
 // caller stores the primary decode.  Out of line, so that the decode pass keeps its registers and the launches of cfgs
-// without either flag pay one branch.  ROT: the symbol-spaced bits are rotated by (c4, s4) (carrier-offset correction).
-template <bool ROT>
+// without either flag pay one branch.  ROT: the symbol-spaced bits are rotated by (c4, s4) (carrier-offset correction); LP:
+// they are made from the filtered samples (BTLE_CFG_LOWPASS).
+template <bool ROT, bool LP>
 __device__ __forceinline__ bool store_repaired(btle_pkt_rec *dst, int stream, int chunk, int n0, const StreamParams &sp, const uint32_t *crc4,
                                                const uint32_t primary[11], int nbytes, const int8_t *iq, long long n_int8, long long lead,
                                                int c4 = 0, int s4 = 0) {
   uint32_t words[11];
 #pragma unroll
   for (int j = 0; j < 11; ++j) words[j] = primary[j];
-  const uint32_t extra = repair_packet<ROT>(iq_window(iq, n_int8, chunk), sp, crc4, g_syndrome, n0, words, nbytes, c4, s4);
+  const uint32_t extra = repair_packet<ROT, LP>(iq_window(iq, n_int8, chunk, lead), sp, crc4, g_syndrome, n0, words, nbytes, c4, s4);
   if (!extra) return false;
   store_record(dst, stream, chunk, n0, nbytes, 0, false, words, sp, iq, n_int8, lead, extra);
   return true;
@@ -278,13 +279,56 @@ __device__ __forceinline__ void load_multi_warp(const StreamParams *__restrict__
 // the word behind it (lane rows - 1).  Samples -2, -1 come from the previous lane's last word and 128, 129 from the next
 // lane's first word, both exchanged before the walk, so every bit is final when it is made.  A step needs the word in front
 // of its 16 bytes: the walk loads the next-lower 16 bytes before it decodes the current ones.  ROT: (c, s) = (C4, S4).
-template <bool ROT>
-__device__ __forceinline__ void dense_sym_group(const unsigned char *stage, int rows, int lane, uint32_t head, uint32_t tail, int c, int s,
-                                                uint32_t acc[4]) {
+// LP (BTLE_CFG_LOWPASS): the bits of the filtered words (lp_word), which reach one sample further: two words are exchanged
+// with each neighbour lane, head2 is the word in front of head and tail2 the word behind tail.  Each filtered word is made
+// once: the step's word 3 is the previous step's word in front.
+template <bool ROT, bool LP>
+__device__ __forceinline__ void dense_sym_group(const unsigned char *stage, int rows, int lane, uint32_t head, uint32_t tail, uint32_t head2,
+                                                uint32_t tail2, int c, int s, uint32_t acc[4]) {
   auto word_of = [&](int r, int k) {                       // word k (0..31) of box row r
     return reinterpret_cast<const uint32_t *>(stage + (r << 7) + ((((uint32_t)(k >> 2)) ^ (uint32_t)(r & 7)) << 4))[k & 3];
   };
   const bool mine = lane < rows;
+  if constexpr (LP) {
+    const uint32_t f0 = mine ? word_of(lane, 0) : 0u, f1 = mine ? word_of(lane, 1) : 0u;
+    const uint32_t l0 = mine ? word_of(rows + lane, 30) : 0u, l1 = mine ? word_of(rows + lane, 31) : 0u;
+    const uint32_t m0 = mine ? word_of(lane, 30) : 0u, m1 = mine ? word_of(lane, 31) : 0u;
+    uint32_t n0 = __shfl_down_sync(0xFFFFFFFFu, f0, 1), n1 = __shfl_down_sync(0xFFFFFFFFu, f1, 1);
+    uint32_t p0 = __shfl_up_sync(0xFFFFFFFFu, l0, 1), p1 = __shfl_up_sync(0xFFFFFFFFu, l1, 1);
+    if (lane == rows - 1) { n0 = tail; n1 = tail2; }
+    if (lane == 0) { p0 = head2; p1 = head; }
+    if (!mine) return;
+    uint32_t carry = lp_word(l1, n0, n1), top = lp_word(l0, l1, n0);   // filtered words 64 and 63
+#pragma unroll 1
+    for (int half = 1; half >= 0; --half) {
+      const int r = half * rows + lane;
+      const unsigned char *row = stage + (r << 7);
+      const uint32_t sw = (uint32_t)(r & 7);
+      const uint32_t below2 = half ? m0 : p0, below1 = half ? m1 : p1;   // the two raw words in front of the half
+      uint4 cur = *reinterpret_cast<const uint4 *>(row + ((7u ^ sw) << 4));
+#pragma unroll
+      for (int cc = 7; cc >= 0; --cc) {
+        uint4 nxt = cur;
+        uint32_t r2 = below2, r1 = below1;
+        if (cc > 0) {
+          nxt = *reinterpret_cast<const uint4 *>(row + ((((uint32_t)(cc - 1)) ^ sw) << 4));
+          r2 = nxt.z;
+          r1 = nxt.w;
+        }
+        const uint32_t g0 = lp_word(r1, cur.x, cur.y), g1 = lp_word(cur.x, cur.y, cur.z), g2 = lp_word(cur.y, cur.z, cur.w);
+        const uint32_t gp = lp_word(r2, r1, cur.x);
+        if ((cc & 3) == 3) {
+#pragma unroll
+          for (int ph = 0; ph < 4; ++ph) acc[ph] <<= 8;
+        }
+        dbits8_sym_step<ROT>(cc & 3, gp, g0, g1, g2, top, carry, c, s, acc);
+        carry = g0;
+        top = gp;
+        cur = nxt;
+      }
+    }
+    return;
+  }
   const uint32_t first = mine ? word_of(lane, 0) : 0u, last = mine ? word_of(rows + lane, 31) : 0u, mid = mine ? word_of(lane, 31) : 0u;
   uint32_t nb = __shfl_down_sync(0xFFFFFFFFu, first, 1), pv = __shfl_up_sync(0xFFFFFFFFu, last, 1);
   if (lane == rows - 1) nb = tail;
@@ -337,9 +381,11 @@ __device__ __forceinline__ void dense_sym_group(const unsigned char *stage, int 
 // ROT (the *_offset entry points): rot[i] = {C, S, C4, S4} of cfg i (make_rot); the dense warps build the phase words from
 // the rotated discriminator (dbits8_rot, with the rotation of the capture's first cfg) and recovery rotates its
 // symbol-spaced bits by (C4, S4).  Without ROT, rot is not read.
-// SYM (BTLE_CFG_SYMBOL_SPACED): the dense warps build the phase words from the symbol-spaced discriminator (dense_sym_group;
-// with ROT rotated by the capture's first cfg's (C4, S4)).  Everything behind the phase words is the same code.
-template <int KC, bool ROT, bool SYM>
+// DISC, the discriminator mode: kDiscQuarter is the reference's bit; kDiscSymbol (BTLE_CFG_SYMBOL_SPACED) has the dense
+// warps build the phase words from the symbol-spaced discriminator (dense_sym_group; with ROT rotated by the capture's first
+// cfg's (C4, S4)); kDiscLowpass (with BTLE_CFG_LOWPASS) from the symbol-spaced discriminator of the filtered samples, and
+// recovery reads them too.  Everything behind the phase words is the same code.
+template <int KC, bool ROT, int DISC>
 __global__ void __launch_bounds__(kThreads, kCtasPerSm)
 btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __grid_constant__ CUtensorMap map12,
                           const int8_t *__restrict__ iq, long long stream_stride, long long n_int8,
@@ -347,6 +393,7 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
                           btle_pkt_rec *__restrict__ out, unsigned cap, unsigned *__restrict__ count,
                           uint2 *__restrict__ dir, unsigned *__restrict__ zero_next, long long lead,
                           const int4 *__restrict__ vmap, const int4 *__restrict__ rot) {
+  constexpr bool SYM = DISC != kDiscQuarter, LP = DISC == kDiscLowpass;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Smem<KC> &M = *reinterpret_cast<Smem<KC> *>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -512,6 +559,19 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
                 if (o + bb >= -lead && o + bb < n_int8) head |= (uint32_t)(uint8_t)cap_base[o + bb] << (8 * bb);
           }
         }
+        uint32_t head2 = 0, tail2 = 0;                    // LP: the words in front of head and behind tail
+        if constexpr (LP) {
+          auto word_at = [&](long long o) {
+            uint32_t w = 0;
+            if (o >= -lead && o + 4 <= n_int8) w = __ldg(reinterpret_cast<const uint32_t *>(cap_base + o));
+            else
+              for (int bb = 0; bb < 4; ++bb)
+                if (o + bb >= -lead && o + bb < n_int8) w |= (uint32_t)(uint8_t)cap_base[o + bb] << (8 * bb);
+            return w;
+          };
+          if (lane == 0) head2 = word_at(tile_off - 8);
+          if (lane == rows - 1) tail2 = word_at(tile_off + (long long)rows * 256 + 4);
+        }
         if (tma) {
           w_tma.begin();
           mbar_wait(mbar, tma_phase);
@@ -544,7 +604,7 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
           __syncwarp();
         }
         uint32_t acc[4] = {0u, 0u, 0u, 0u};
-        if constexpr (SYM) dense_sym_group<ROT>(stage, rows, lane, head, tail, rc, rs, acc);
+        if constexpr (SYM) dense_sym_group<ROT, LP>(stage, rows, lane, head, tail, head2, tail2, rc, rs, acc);
         else {
         uint32_t carry = 0u, wtop = 0u;
         int vtop = 0;
@@ -761,7 +821,7 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
           bool stored = false;
           if (sp.recover | sp.correct) {
             if (live && crc_bad && !rej && base + (unsigned)j < cap)
-              stored = store_repaired<ROT>(out + base + j, rec_stream, si.chunk0 + c, n0, sp, M.crc4, words, nbytes, cap_base, n_int8, lead,
+              stored = store_repaired<ROT, DISC == kDiscLowpass>(out + base + j, rec_stream, si.chunk0 + c, n0, sp, M.crc4, words, nbytes, cap_base, n_int8, lead,
                                            c4, s4);
           }
           if (live && !stored && base + (unsigned)j < cap)
@@ -781,7 +841,7 @@ btle_rx_persistent_kernel(const __grid_constant__ CUtensorMap map32, const __gri
                 int nbytes, crc_bad;
                 decode_packet(pd, sp, crc4, n0, rej, words, nbytes, crc_bad);
                 if ((sp.recover | sp.correct) && crc_bad && !rej &&
-                    store_repaired<ROT>(out + first + i, stream, chunk, n0, sp, crc4, words, nbytes, iq, n_int8, lead, c4, s4))
+                    store_repaired<ROT, DISC == kDiscLowpass>(out + first + i, stream, chunk, n0, sp, crc4, words, nbytes, iq, n_int8, lead, c4, s4))
                   return;                                             // as steps 3b, 3c
                 store_record(out + first + i, stream, chunk, n0, nbytes, crc_bad, rej, words, sp, iq, n_int8, lead);
               }
@@ -2012,10 +2072,20 @@ int validate_cfgs(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size_t n) {
       ctx->err = "channel number must be within 0~39";
       return BTLE_EINVAL;
     }
+  for (size_t i = 0; i < n; ++i)
+    if ((cfgs[i].rssi & BTLE_CFG_LOWPASS) && !(cfgs[i].rssi & BTLE_CFG_SYMBOL_SPACED)) {
+      ctx->err = "BTLE_CFG_LOWPASS needs BTLE_CFG_SYMBOL_SPACED";
+      return BTLE_EINVAL;
+    }
   // one dense loop per kernel instantiation: every cfg of a launch (or of a session) is in the same discriminator mode
   for (size_t i = 1; i < n; ++i)
     if ((cfgs[i].rssi ^ cfgs[0].rssi) & BTLE_CFG_SYMBOL_SPACED) {
       ctx->err = "all cfgs of one launch must agree on BTLE_CFG_SYMBOL_SPACED";
+      return BTLE_EINVAL;
+    }
+  for (size_t i = 1; i < n; ++i)
+    if ((cfgs[i].rssi ^ cfgs[0].rssi) & BTLE_CFG_LOWPASS) {
+      ctx->err = "all cfgs of one launch must agree on BTLE_CFG_LOWPASS";
       return BTLE_EINVAL;
     }
   return BTLE_OK;
@@ -2198,11 +2268,11 @@ int make_rots(btle_b200_ctx *ctx, const float *offset_hz, size_t n_captures, con
   return BTLE_OK;
 }
 
-template <int KC, bool ROT, bool SYM>
+template <int KC, bool ROT, int DISC>
 void enqueue_rx(unsigned grid, cudaStream_t st, const MapSlot *ms, const int8_t *d_iq, size_t stride, size_t n_int8, const CfgSlot *cs,
                 const Plan &plan, btle_pkt_rec *d_out, unsigned cap32, unsigned *d_count, btle_unit_dir *d_dir, unsigned *zero_next,
                 long long lead) {
-  btle_rx_persistent_kernel<KC, ROT, SYM><<<grid, kThreads, sizeof(Smem<KC>), st>>>(
+  btle_rx_persistent_kernel<KC, ROT, DISC><<<grid, kThreads, sizeof(Smem<KC>), st>>>(
       ms->map32, ms->map12, d_iq, (long long)stride, (long long)n_int8, cs->d_params, plan, d_out, cap32, d_count,
       reinterpret_cast<uint2 *>(d_dir), zero_next, lead, KC > 1 ? cs->d_vmap.p : nullptr, ROT ? cs->d_rot.p : nullptr);
 }
@@ -2213,7 +2283,8 @@ void enqueue_rx(unsigned grid, cudaStream_t st, const MapSlot *ms, const int8_t 
 // any other list runs <kMaxCfgsPerCapture> over the captures it names, the directory in (cfg, chunk) order.
 // rot != nullptr: one rotation per cfg (make_rot), the rotated kernel variant.  `lead`: bytes readable in front of each
 // capture (the stream session's lead: RSSI of hits at a segment's very start, the symbol-spaced bits of its first samples).
-// cfgs with BTLE_CFG_SYMBOL_SPACED (all or none, validate_cfgs) run the symbol-spaced variant.
+// cfgs with BTLE_CFG_SYMBOL_SPACED (all or none, validate_cfgs) run the symbol-spaced variant, and with BTLE_CFG_LOWPASS too
+// (again all or none) the low-pass one.
 int launch_rx(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8, const btle_stream_cfg *cfgs,
               const int32_t *cfg_capture, size_t n_cfgs, const int4 *rot, btle_pkt_rec *d_out, size_t cap, unsigned *d_count,
               btle_unit_dir *d_dir, cudaStream_t st, long long lead) {
@@ -2259,12 +2330,16 @@ int launch_rx(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t s
     zero_next = ctx->d_count_ring + (ctx->ring_pos + kCountRing / 2) % kCountRing;
   }
   const unsigned grid = (unsigned)std::min<long long>(plan.total_units, (long long)ctx->num_sms * kCtasPerSm);   // one persistent CTA per SM
-  // BTLE_CFG_SYMBOL_SPACED: validate_cfgs made every cfg of the launch agree on it
-  const bool sym = (cfgs[0].rssi & BTLE_CFG_SYMBOL_SPACED) != 0;
-  const auto enqueue = sym ? (multi ? (rot ? enqueue_rx<kMaxCfgsPerCapture, true, true> : enqueue_rx<kMaxCfgsPerCapture, false, true>)
-                                    : (rot ? enqueue_rx<1, true, true> : enqueue_rx<1, false, true>))
-                           : (multi ? (rot ? enqueue_rx<kMaxCfgsPerCapture, true, false> : enqueue_rx<kMaxCfgsPerCapture, false, false>)
-                                    : (rot ? enqueue_rx<1, true, false> : enqueue_rx<1, false, false>));
+  // BTLE_CFG_SYMBOL_SPACED and BTLE_CFG_LOWPASS: validate_cfgs made every cfg of the launch agree on both
+  const int disc = disc_mode(cfgs[0]);
+  const auto enqueue = disc == kDiscLowpass
+                           ? (multi ? (rot ? enqueue_rx<kMaxCfgsPerCapture, true, kDiscLowpass> : enqueue_rx<kMaxCfgsPerCapture, false, kDiscLowpass>)
+                                    : (rot ? enqueue_rx<1, true, kDiscLowpass> : enqueue_rx<1, false, kDiscLowpass>))
+                       : disc == kDiscSymbol
+                           ? (multi ? (rot ? enqueue_rx<kMaxCfgsPerCapture, true, kDiscSymbol> : enqueue_rx<kMaxCfgsPerCapture, false, kDiscSymbol>)
+                                    : (rot ? enqueue_rx<1, true, kDiscSymbol> : enqueue_rx<1, false, kDiscSymbol>))
+                           : (multi ? (rot ? enqueue_rx<kMaxCfgsPerCapture, true, kDiscQuarter> : enqueue_rx<kMaxCfgsPerCapture, false, kDiscQuarter>)
+                                    : (rot ? enqueue_rx<1, true, kDiscQuarter> : enqueue_rx<1, false, kDiscQuarter>));
   enqueue(grid, st, ms, d_iq, stride, n_int8, cs, plan, d_out, (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu), d_count, d_dir, zero_next, lead);
   BTLE_CUDA(ctx, cudaGetLastError());
   if (ring) {                                                 // the position is taken only by a launch that was enqueued
@@ -2618,6 +2693,12 @@ int btle_b200_create(btle_b200_ctx **out, int cuda_device) {
                            (int)sizeof(Smem<kMaxCfgsPerCapture>)) != cudaSuccess ||
       cudaFuncSetAttribute(btle_rx_persistent_kernel<1, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem<1>)) != cudaSuccess ||
       cudaFuncSetAttribute(btle_rx_persistent_kernel<kMaxCfgsPerCapture, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (int)sizeof(Smem<kMaxCfgsPerCapture>)) != cudaSuccess ||
+      cudaFuncSetAttribute(btle_rx_persistent_kernel<1, false, kDiscLowpass>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem<1>)) != cudaSuccess ||
+      cudaFuncSetAttribute(btle_rx_persistent_kernel<kMaxCfgsPerCapture, false, kDiscLowpass>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (int)sizeof(Smem<kMaxCfgsPerCapture>)) != cudaSuccess ||
+      cudaFuncSetAttribute(btle_rx_persistent_kernel<1, true, kDiscLowpass>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem<1>)) != cudaSuccess ||
+      cudaFuncSetAttribute(btle_rx_persistent_kernel<kMaxCfgsPerCapture, true, kDiscLowpass>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            (int)sizeof(Smem<kMaxCfgsPerCapture>)) != cudaSuccess ||
       cudaFuncSetAttribute(sps8_hits_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSps8Smem) != cudaSuccess ||
       cudaFuncSetAttribute(discover_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDiscSmem) != cudaSuccess ||
@@ -3135,11 +3216,11 @@ int streams_index(btle_b200_streams *s, size_t stream) {
   s->ctx->err = "stream index out of range";
   return BTLE_EINVAL;
 }
-// a session decodes in the BTLE_CFG_SYMBOL_SPACED mode of the cfgs it was opened with (entries[0] keeps it), so every
-// round, backfill included, is one launch of one kernel variant
+// a session decodes in the BTLE_CFG_SYMBOL_SPACED and BTLE_CFG_LOWPASS mode of the cfgs it was opened with (entries[0]
+// keeps it), so every round, backfill included, is one launch of one kernel variant
 int streams_check_mode(btle_b200_streams *s, const btle_stream_cfg *cfg) {
-  if (!((cfg->rssi ^ s->entries[0].cfg.rssi) & BTLE_CFG_SYMBOL_SPACED)) return BTLE_OK;
-  s->ctx->err = "a session's cfgs must all agree on BTLE_CFG_SYMBOL_SPACED (the mode of streams_open)";
+  if (!((cfg->rssi ^ s->entries[0].cfg.rssi) & (BTLE_CFG_SYMBOL_SPACED | BTLE_CFG_LOWPASS))) return BTLE_OK;
+  s->ctx->err = "a session's cfgs must all agree on BTLE_CFG_SYMBOL_SPACED and BTLE_CFG_LOWPASS (the mode of streams_open)";
   return BTLE_EINVAL;
 }
 }  // namespace
@@ -3790,8 +3871,12 @@ static int check_rx_ber_cfg(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg) {
   }
   if (std::fabs(cfg->ppm) >= 1e6f) { ctx->err = "rx_ber: ppm must have |ppm| < 1e6"; return BTLE_EINVAL; }
   if (cfg->amplitude < 1 || cfg->amplitude > 127) { ctx->err = "rx_ber: amplitude must be 1..127"; return BTLE_EINVAL; }
-  if (cfg->flags & ~(uint32_t)(BTLE_CFG_RECOVER | BTLE_CFG_SYMBOL_SPACED | BTLE_CFG_CENTRE_HITS | BTLE_CFG_CORRECT)) {
-    ctx->err = "rx_ber: flags may only hold BTLE_CFG_RECOVER, BTLE_CFG_SYMBOL_SPACED, BTLE_CFG_CENTRE_HITS and BTLE_CFG_CORRECT";
+  if (cfg->flags & ~(uint32_t)(BTLE_CFG_RECOVER | BTLE_CFG_SYMBOL_SPACED | BTLE_CFG_CENTRE_HITS | BTLE_CFG_CORRECT | BTLE_CFG_LOWPASS)) {
+    ctx->err = "rx_ber: flags may only hold BTLE_CFG_RECOVER, BTLE_CFG_SYMBOL_SPACED, BTLE_CFG_CENTRE_HITS, BTLE_CFG_CORRECT and BTLE_CFG_LOWPASS";
+    return BTLE_EINVAL;
+  }
+  if ((cfg->flags & BTLE_CFG_LOWPASS) && !(cfg->flags & BTLE_CFG_SYMBOL_SPACED)) {
+    ctx->err = "rx_ber: BTLE_CFG_LOWPASS needs BTLE_CFG_SYMBOL_SPACED";
     return BTLE_EINVAL;
   }
   if (cfg->slot_samples < rx_ber_len(cfg->channel) || cfg->slot_samples > BTLE_RX_BER_MAX_SLOT) {
@@ -3881,10 +3966,11 @@ int btle_b200_rx_ber_run(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg, size_t 
   const size_t max_b = std::min<size_t>(n_packets, (size_t)B);
   const long long max_chunks = ((long long)max_b * S + kChunkSamples - 1) / kChunkSamples;
   // BTLE_CFG_SYMBOL_SPACED: d[n] reads samples n - 2 .. n + 2, so a batch is decoded with the 2 samples in front of it
-  // (kSymLead bytes of lead, the tail of the previous slot, synthesised again into `prev`) and 2 more behind its look-ahead
-  const bool sym = (cfg->flags & BTLE_CFG_SYMBOL_SPACED) != 0;
+  // (kSymLead bytes of lead, the tail of the previous slot, synthesised again into `prev`) and 2 more behind its look-ahead;
+  // with BTLE_CFG_LOWPASS samples n - 3 .. n + 3, so 3 more behind it (the lead holds 8)
+  const bool sym = (cfg->flags & BTLE_CFG_SYMBOL_SPACED) != 0, lp = (cfg->flags & BTLE_CFG_LOWPASS) != 0;
   constexpr size_t kSymLead = 16;                            // keeps the capture 16-byte aligned
-  const size_t lead = sym ? kSymLead : 0, look = BTLE_LOOKAHEAD_INT8 + (sym ? 4 : 0);
+  const size_t lead = sym ? kSymLead : 0, look = BTLE_LOOKAHEAD_INT8 + (lp ? 6 : sym ? 4 : 0);
   const size_t max_int8 = (size_t)max_chunks * kChunkInt8 + look, max_recs = (size_t)max_chunks * BTLE_MAX_RECS_PER_CHUNK;
   const size_t prev_at = (lead + max_int8 + 15) & ~size_t(15);
   if (ctx->d_iq.reserve(ctx, sym ? prev_at + 2 * (size_t)S : max_int8) || ctx->d_out.reserve(ctx, max_recs) ||

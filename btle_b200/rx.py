@@ -20,13 +20,16 @@ DEFAULT_CHANNEL = 37                 # btle_rx.c:230
 
 
 def make_cfgs(n_streams=1, channel=DEFAULT_CHANNEL, access_addr=DEFAULT_ACCESS_ADDR, access_mask=0xFFFFFFFF,
-              crc_init=DEFAULT_CRC_INIT, raw=0, rssi=0, recover=0, symbol_spaced=0, centre_hits=0, correct=0) -> np.ndarray:
+              crc_init=DEFAULT_CRC_INIT, raw=0, rssi=0, recover=0, symbol_spaced=0, centre_hits=0, correct=0,
+              lowpass=0) -> np.ndarray:
     """btle_stream_cfg array; every argument may be a scalar or a per-stream sequence.  rssi holds the BTLE_CFG_* flag
     bits; recover (true) adds BTLE_CFG_RECOVER: counted packets that fail the CRC are demodulated again; symbol_spaced
     (true) adds BTLE_CFG_SYMBOL_SPACED: the discriminator compares samples a symbol apart (all cfgs of one call must
     agree on it; include/btle_b200.h); centre_hits (true) adds BTLE_CFG_CENTRE_HITS: the chain moves each hit to the
     centre of its run of matching sample phases (per cfg); correct (true) adds BTLE_CFG_CORRECT: a one-bit or
-    adjacent-pair error of a counted packet that fails the CRC is corrected from its syndrome (per cfg)."""
+    adjacent-pair error of a counted packet that fails the CRC is corrected from its syndrome (per cfg); lowpass (true)
+    adds BTLE_CFG_LOWPASS: the symbol-spaced bits read [1, 2, 1]-filtered samples (only with symbol_spaced; all cfgs of
+    one call must agree on it)."""
     c = np.zeros(n_streams, dtype=CFG_DTYPE)
     c["channel"], c["access_addr"], c["access_mask"] = channel, access_addr, access_mask
     c["crc_init"], c["raw"], c["rssi"] = crc_init, raw, rssi
@@ -34,14 +37,16 @@ def make_cfgs(n_streams=1, channel=DEFAULT_CHANNEL, access_addr=DEFAULT_ACCESS_A
     c["rssi"] |= np.where(np.asarray(symbol_spaced) != 0, _native.CFG_SYMBOL_SPACED, 0).astype(np.int32)
     c["rssi"] |= np.where(np.asarray(centre_hits) != 0, _native.CFG_CENTRE_HITS, 0).astype(np.int32)
     c["rssi"] |= np.where(np.asarray(correct) != 0, _native.CFG_CORRECT, 0).astype(np.int32)
+    c["rssi"] |= np.where(np.asarray(lowpass) != 0, _native.CFG_LOWPASS, 0).astype(np.int32)
     return c
 
 
 def _with_fields(c: np.ndarray, cfg: dict) -> np.ndarray:
     """c (a btle_stream_cfg array) with the given make_cfgs fields changed; recover / symbol_spaced / centre_hits / correct
-    set or clear BTLE_CFG_RECOVER / BTLE_CFG_SYMBOL_SPACED / BTLE_CFG_CENTRE_HITS / BTLE_CFG_CORRECT"""
+    / lowpass set or clear BTLE_CFG_RECOVER / BTLE_CFG_SYMBOL_SPACED / BTLE_CFG_CENTRE_HITS / BTLE_CFG_CORRECT /
+    BTLE_CFG_LOWPASS"""
     flag = {"recover": _native.CFG_RECOVER, "symbol_spaced": _native.CFG_SYMBOL_SPACED, "centre_hits": _native.CFG_CENTRE_HITS,
-            "correct": _native.CFG_CORRECT}
+            "correct": _native.CFG_CORRECT, "lowpass": _native.CFG_LOWPASS}
     for k, v in cfg.items():
         if k in flag:
             c["rssi"] = (c["rssi"] & ~flag[k]) | (flag[k] if v else 0)

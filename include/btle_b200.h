@@ -72,7 +72,8 @@ typedef struct {
                             BTLE_CFG_RECOVER 4: CRC-failed packets are demodulated once more (below);
                             BTLE_CFG_SYMBOL_SPACED 16: the symbol-spaced discriminator (below);
                             BTLE_CFG_CENTRE_HITS 64: each hit centred on its run of matching phases (below);
-                            BTLE_CFG_CORRECT 256: one-bit and adjacent-pair errors corrected by the CRC (below)  */
+                            BTLE_CFG_CORRECT 256: one-bit and adjacent-pair errors corrected by the CRC (below);
+                            BTLE_CFG_LOWPASS 512: a [1, 2, 1] low-pass in front of the symbol-spaced bits (below)  */
 } btle_stream_cfg;
 #define BTLE_CFG_RSSI 1
 #define BTLE_CFG_REPORT_REJECTED 2
@@ -135,6 +136,21 @@ typedef struct {
  * last_error set).  A stream session's mode is that of the cfgs given to streams_open; a set_cfg or add_cfg with the other
  * value is BTLE_EINVAL.  btle_rx_ber_cfg.flags accepts it too. */
 #define BTLE_CFG_SYMBOL_SPACED 16
+/* BTLE_CFG_LOWPASS: opt-in low-pass filter in front of the symbol-spaced discriminator.  Valid only together with
+ * BTLE_CFG_SYMBOL_SPACED.  Each discriminator bit of a raw sample reads the full 4-MHz noise band while a 1-Mbps GFSK signal
+ * fills little more than 1 MHz of it; with the flag every bit reads filtered samples instead:
+ *     F[n] = (x[n-1] + 2 x[n] + x[n+1]) >> 2       per rail (I and Q), arithmetic shift (floor); always -128..127
+ *     d[n] = FI[n-2] FQ[n+2] - FI[n+2] FQ[n-2] > 0  (rotated by (C4, S4) with the *_offset entry points, as above)
+ * The filter is symmetric, so n0 keeps its meaning.  x outside the capture reads 0 and the launch's lead bytes are readable,
+ * exactly as for the symbol-spaced bits, so F and every chunk's bits are a function of the whole capture, not of how it was
+ * cut.  BTLE_CFG_RECOVER's alternatives read F in place of x, e[s] = FI[s] FQ[s+4] - FI[s+4] FQ[s] > 0, under its window
+ * rule: F[s] reads 0 outside [8192 chunk, 8192 chunk + 9696) and behind the capture's end, and inside it is computed from
+ * the capture (x[s - 1] and x[s + 1] may lie outside the window).  mag_sum, btle_b200_rec_offset and discovery read the raw
+ * samples; the search, BTLE_CFG_CENTRE_HITS, the chain and its guards, decode, the CRC, BTLE_CFG_CORRECT, -v and the record
+ * caps are unchanged.  One mode per launch and per session, as for BTLE_CFG_SYMBOL_SPACED: mixed cfgs in one launch, a
+ * session set_cfg or add_cfg with the other value, and the flag without BTLE_CFG_SYMBOL_SPACED are BTLE_EINVAL (with
+ * last_error set).  btle_rx_ber_cfg.flags accepts it under the same pairing rule. */
+#define BTLE_CFG_LOWPASS 512
 /* BTLE_CFG_CENTRE_HITS: opt-in hit rule of the greedy chain.  Not part of the reference's receiver; without it the records
  * are the reference's (or the current mode's), bit for bit.  An access address stays matched for about a symbol around the
  * eye, so the search's first matching window start lies up to a few samples before the centre; with the flag the chain
@@ -607,8 +623,8 @@ typedef struct {
   int32_t channel;         /* 0..39                                                                                 */
   uint32_t access_addr;
   uint32_t crc_init;       /* as -k                                                                                 */
-  uint32_t flags;          /* any of BTLE_CFG_RECOVER, BTLE_CFG_SYMBOL_SPACED, BTLE_CFG_CENTRE_HITS and BTLE_CFG_CORRECT
-                              (given to the receiver); any other bit: BTLE_EINVAL                                     */
+  uint32_t flags;          /* any of BTLE_CFG_RECOVER, BTLE_CFG_SYMBOL_SPACED, BTLE_CFG_CENTRE_HITS, BTLE_CFG_CORRECT
+                              and BTLE_CFG_LOWPASS (given to the receiver); any other bit: BTLE_EINVAL               */
   uint32_t reserved;       /* 0                                                                                     */
 } btle_rx_ber_cfg;         /* 48 bytes */
 typedef struct {
@@ -633,10 +649,12 @@ typedef struct {
 } btle_rx_ber_result;      /* 88 bytes */
 /* n_packets packets 0 .. n_packets-1, in batches sized from free device memory; the result is independent of the batch
  * size (every batch starts on a chunk and slot boundary, and its look-ahead behind the last chunk is the next slots'; with
- * BTLE_CFG_SYMBOL_SPACED a batch also reads the 2 samples in front of it and 2 more behind its look-ahead).
+ * BTLE_CFG_SYMBOL_SPACED a batch also reads the 2 samples in front of it and 2 more behind its look-ahead, with
+ * BTLE_CFG_LOWPASS 3 and 3).
  * BTLE_EINVAL with btle_b200_last_error() for: snr_db, ppm or cfo_hz NaN or infinite, |ppm| >= 1e6, amplitude outside
  * 1..127, slot_samples below L or above BTLE_RX_BER_MAX_SLOT, channel > 39, a flags bit other than BTLE_CFG_RECOVER,
- * BTLE_CFG_SYMBOL_SPACED, BTLE_CFG_CENTRE_HITS and BTLE_CFG_CORRECT;
+ * BTLE_CFG_SYMBOL_SPACED, BTLE_CFG_CENTRE_HITS, BTLE_CFG_CORRECT and BTLE_CFG_LOWPASS, BTLE_CFG_LOWPASS without
+ * BTLE_CFG_SYMBOL_SPACED;
  * the context stays usable. */
 int btle_b200_rx_ber_run(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg, size_t n_packets, btle_rx_ber_result *out);
 /* the capture and truth of packets first_packet .. first_packet + n_packets - 1 alone: d_iq (16-byte aligned) receives

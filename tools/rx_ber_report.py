@@ -3,7 +3,7 @@
 rx_ber_run goes (CUDA events around its three kernels on one batch).
 
     python tools/rx_ber_report.py [--packets N] [--json out.json] [--recover] [--symbol-spaced] [--centre-hits] [--correct]
-                                  [--snrs 8:31] [--no-cfo]
+                                  [--lowpass] [--snrs 8:31] [--no-cfo]
 
 --recover adds the 4-sps PER / BER with BTLE_CFG_RECOVER (CRC-failed packets demodulated again) next to the plain ones.
 --symbol-spaced adds them with BTLE_CFG_SYMBOL_SPACED (the symbol-spaced discriminator), and with --recover also with both.
@@ -11,6 +11,8 @@ rx_ber_run goes (CUDA events around its three kernels on one batch).
 matching sample phases), and prints the SNR at PER 0.5 and the error breakdown of every 4-sps variant per ppm.
 --correct adds, next to the plain receiver and each of those, the same receiver with BTLE_CFG_CORRECT (one-bit and
 adjacent-pair errors of CRC-failed packets corrected from the syndrome), and prints the same breakdown.
+--lowpass adds, next to each symbol-spaced variant, the same receiver with BTLE_CFG_LOWPASS (the symbol-spaced bits read
+[1, 2, 1]-filtered samples), and prints the same breakdown.
 --snrs LO:HI sweeps SNR LO .. HI-1 dB (default -5:31); --no-cfo leaves out the extra-carrier-offset rows.
 
 Prints a markdown table (one row per point) and the throughput of both flows."""
@@ -95,37 +97,41 @@ def main():
     ap.add_argument("--symbol-spaced", action="store_true", help="also measure the receiver with BTLE_CFG_SYMBOL_SPACED")
     ap.add_argument("--centre-hits", action="store_true", help="also measure every 4-sps variant with BTLE_CFG_CENTRE_HITS")
     ap.add_argument("--correct", action="store_true", help="also measure every 4-sps variant with BTLE_CFG_CORRECT")
+    ap.add_argument("--lowpass", action="store_true", help="also measure every symbol-spaced variant with BTLE_CFG_LOWPASS")
     ap.add_argument("--snrs", default="-5:31", help="LO:HI, SNR points LO .. HI-1 dB")
     ap.add_argument("--no-cfo", action="store_true", help="leave out the extra-carrier-offset rows")
     args = ap.parse_args()
     rx = BtleRx(0)
     lo, hi = (int(v) for v in args.snrs.split(":"))
     snrs = list(range(lo, hi))             # the 4-sps receiver's curve falls between 15 and 30 dB
-    # the 4-sps variants: (key, recover, symbol_spaced, centre_hits, correct)
-    ways = [("rx4_recover", True, False, False, False)] if args.recover else []
+    # the 4-sps variants: (key, recover, symbol_spaced, centre_hits, correct, lowpass)
+    ways = [("rx4_recover", True, False, False, False, False)] if args.recover else []
     if args.symbol_spaced:
-        ways += [("rx4_symbol", False, True, False, False)] + ([("rx4_symbol_recover", True, True, False, False)] if args.recover else [])
+        ways += [("rx4_symbol", False, True, False, False, False)] + ([("rx4_symbol_recover", True, True, False, False, False)] if args.recover else [])
     if args.centre_hits:
-        ways += [("rx4_centre", False, False, True, False)] + [(k + "_centre", rc, sy, True, False) for k, rc, sy, _, _ in ways]
+        ways += [("rx4_centre", False, False, True, False, False)] + [(k + "_centre", rc, sy, True, False, False) for k, rc, sy, _, _, _ in ways]
     if args.correct:
-        ways += [("rx4_correct", False, False, False, True)] + [(k + "_correct", rc, sy, ce, True) for k, rc, sy, ce, _ in ways]
+        ways += [("rx4_correct", False, False, False, True, False)] + [(k + "_correct", rc, sy, ce, True, False) for k, rc, sy, ce, _, _ in ways]
+    if args.lowpass:
+        ways += [(k + "_lowpass", rc, sy, ce, co, True) for k, rc, sy, ce, co, _ in ways if sy]
     rows = []
     for ppm in (0.0, 20.0, 50.0):
         r4 = ber.rx_ber_sweep(snrs, args.packets, ppm=ppm, rx=rx)
         r8 = ber.ber_sweep(snrs, args.packets, ppm=ppm, rx=rx)
-        rw = {k: ber.rx_ber_sweep(snrs, args.packets, ppm=ppm, rx=rx, recover=rc, symbol_spaced=sy, centre_hits=ce, correct=co)
-              for k, rc, sy, ce, co in ways}
+        rw = {k: ber.rx_ber_sweep(snrs, args.packets, ppm=ppm, rx=rx, recover=rc, symbol_spaced=sy, centre_hits=ce, correct=co, lowpass=lp)
+              for k, rc, sy, ce, co, lp in ways}
         for i, (a, b) in enumerate(zip(r4, r8)):
             rows.append({"ppm": ppm, "cfo_hz": 0.0, "rx4": a, "model8": b, **{k: v[i] for k, v in rw.items()}})
     for cfo in () if args.no_cfo else (25e3, 50e3, 100e3, 150e3):
         r4 = ber.rx_ber_sweep(snrs, args.packets, cfo_hz=cfo, rx=rx)
-        rw = {k: ber.rx_ber_sweep(snrs, args.packets, cfo_hz=cfo, rx=rx, recover=rc, symbol_spaced=sy, centre_hits=ce, correct=co)
-              for k, rc, sy, ce, co in ways}
+        rw = {k: ber.rx_ber_sweep(snrs, args.packets, cfo_hz=cfo, rx=rx, recover=rc, symbol_spaced=sy, centre_hits=ce, correct=co, lowpass=lp)
+              for k, rc, sy, ce, co, lp in ways}
         for i, a in enumerate(r4):
             rows.append({"ppm": 0.0, "cfo_hz": cfo, "rx4": a, "model8": None, **{k: v[i] for k, v in rw.items()}})
     label = {"rx4_recover": "recover", "rx4_symbol": "symbol", "rx4_symbol_recover": "symbol+recover"}
     label.update({"rx4_centre": "centre"} | {k + "_centre": v + "+centre" for k, v in label.items()})
     label.update({"rx4_correct": "correct"} | {k + "_correct": v + "+correct" for k, v in label.items()})
+    label.update({k + "_lowpass": v + "+lowpass" for k, v in label.items()})
     extra_h = "".join(f" 4-sps PER {label[k]} | 4-sps BER {label[k]} | aa_miss {label[k]} |" for k, *_ in ways)
     print(f"| ppm | cfo kHz | SNR dB | 4-sps PER | 4-sps BER |{extra_h} aa_miss | len_reject | extra | 8-sps model PER | 8-sps model BER |")
     print("|---:|---:|---:|---:|---:|" + "---:|---:|---:|" * len(ways) + "---:|---:|---:|---:|---:|")
@@ -135,7 +141,7 @@ def main():
         rc = "".join(f" {r[k]['per']:.4f} | {r[k]['ber']:.2e} | {r[k]['aa_miss']} |" for k, *_ in ways)
         print(f"| {r['ppm']:g} | {r['cfo_hz'] / 1e3:g} | {a['snr_db']:g} | {a['per']:.4f} | {a['ber']:.2e} |{rc} {a['aa_miss']} | {a['len_reject']} | "
               f"{a['extra_recs']} | {m} |")
-    if args.centre_hits or args.correct:
+    if args.centre_hits or args.correct or args.lowpass:
         breakdown(rows, ["rx4"] + [k for k, *_ in ways], {"rx4": "default", **label})
     r4 = [r["rx4"] for r in rows]
     r8 = [r["model8"] for r in rows if r["model8"]]
