@@ -82,8 +82,12 @@ CFG_CENTRE_HITS = 64         # BTLE_CFG_CENTRE_HITS: each hit moved to the centr
 CFG_CORRECT = 256            # BTLE_CFG_CORRECT: one-bit and adjacent-pair errors of CRC-failed packets corrected (per cfg)
 CFG_LOWPASS = 512            # BTLE_CFG_LOWPASS: [1, 2, 1] low-pass in front of the symbol-spaced bits (with CFG_SYMBOL_SPACED, one mode per launch)
 MAX_OFFSET_HZ = 500000       # BTLE_MAX_OFFSET_HZ: largest |offset_hz| of the carrier-offset correction
+CFG_OFFSET_SEARCH = 1024     # BTLE_CFG_OFFSET_SEARCH: seven carrier-offset hypotheses per capture, merged per packet (one mode per launch)
+OFFSET_SEARCH_HZ = (0.0, -50e3, 50e3, -100e3, 100e3, -150e3, 150e3)   # BTLE_OFFSET_SEARCH_HZ: the hypotheses, in merge order
+MAX_MERGED_RECS_PER_CHUNK = 429                           # BTLE_MAX_MERGED_RECS_PER_CHUNK = 123 + 6 * 51
 REC_REJECTED, REC_RECOVERED = 4, 8                        # btle_pkt_rec.flags bits; a recovered record's alternative q is flags >> 4 & 3
 REC_CORRECTED = 64                                        # btle_pkt_rec.flags bit: bytes corrected by the CRC syndrome
+REC_OFFSET_SEARCH = 128                                   # btle_pkt_rec.flags bit: found by offset hypothesis 1..6 (CFG_OFFSET_SEARCH)
 
 
 class BtleError(RuntimeError):

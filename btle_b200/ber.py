@@ -45,18 +45,20 @@ def ber_sweep(snr_db, n_packets: int, channel: int = 37, crc_init: int = 0x55555
 # ---- the 4-Msps receive chain (btle_b200_rx_ber_run; definition in include/btle_b200.h) --------------------------------
 def rx_ber_cfg(snr_db: float, ppm: float = 0.0, cfo_hz: float = 0.0, amplitude: int = 64, slot_samples: int = 2048, channel: int = 37,
                crc_init: int = 0x555555, access_addr: int = 0x8E89BED6, seed: int = 1, recover: bool = False,
-               symbol_spaced: bool = False, centre_hits: bool = False, correct: bool = False, lowpass: bool = False) -> np.ndarray:
+               symbol_spaced: bool = False, centre_hits: bool = False, correct: bool = False, lowpass: bool = False,
+               offset_search: bool = False) -> np.ndarray:
     """recover: the receiver runs with BTLE_CFG_RECOVER (CRC-failed packets demodulated again); symbol_spaced: with
     BTLE_CFG_SYMBOL_SPACED (the symbol-spaced discriminator); centre_hits: with BTLE_CFG_CENTRE_HITS (each hit moved to the
     centre of its run of matching sample phases); correct: with BTLE_CFG_CORRECT (one-bit and adjacent-pair errors of
     CRC-failed packets corrected from the syndrome); lowpass: with BTLE_CFG_LOWPASS (the symbol-spaced bits read [1, 2, 1]
-    filtered samples; only with symbol_spaced)"""
+    filtered samples; only with symbol_spaced); offset_search: with BTLE_CFG_OFFSET_SEARCH (seven carrier-offset hypotheses,
+    merged per packet)"""
     cfg = np.zeros(1, dtype=_native.RX_BER_CFG_DTYPE)
     cfg["seed"], cfg["snr_db"], cfg["ppm"], cfg["cfo_hz"], cfg["amplitude"] = seed, snr_db, ppm, cfo_hz, amplitude
     cfg["slot_samples"], cfg["channel"], cfg["crc_init"], cfg["access_addr"] = slot_samples, channel, crc_init, access_addr
     cfg["flags"] = ((_native.CFG_RECOVER if recover else 0) | (_native.CFG_SYMBOL_SPACED if symbol_spaced else 0) |
                     (_native.CFG_CENTRE_HITS if centre_hits else 0) | (_native.CFG_CORRECT if correct else 0) |
-                    (_native.CFG_LOWPASS if lowpass else 0))
+                    (_native.CFG_LOWPASS if lowpass else 0) | (_native.CFG_OFFSET_SEARCH if offset_search else 0))
     return cfg
 
 
@@ -81,7 +83,9 @@ def _rx_ber_corrected(rx: BtleRx, cfg: np.ndarray, n_packets: int, offset_hz: fl
         d_iq = torch.empty((1, chunks * 16384), dtype=torch.int8, device=dev)
         d_truth = torch.empty(n * _native.RX_BER_TRUTH_DTYPE.itemsize, dtype=torch.uint8, device=dev)
         rx._check(rx._L.btle_b200_rx_ber_synth_device(rx._h, cfg.ctypes.data, done, n, d_iq.data_ptr(), d_truth.data_ptr(), st.cuda_stream))
-        cap, units = chunks * 123, rx.units(1, chunks * 16384)           # BTLE_MAX_RECS_PER_CHUNK per chunk
+        # BTLE_MAX_RECS_PER_CHUNK per chunk, or with BTLE_CFG_OFFSET_SEARCH per hypothesis (the merge never overflows then)
+        cap = chunks * 123 * (7 if int(cfg["flags"][0]) & _native.CFG_OFFSET_SEARCH else 1)
+        units = rx.units(1, chunks * 16384)
         d_out = torch.empty(cap * 64, dtype=torch.uint8, device=dev)
         d_dir = torch.empty(max(units, 1) * 8, dtype=torch.uint8, device=dev)
         rx.rx_device_dir(d_iq, scfg, d_out, None, d_dir, st.cuda_stream, offset_hz=offset_hz)
@@ -97,7 +101,7 @@ def _rx_ber_corrected(rx: BtleRx, cfg: np.ndarray, n_packets: int, offset_hz: fl
 def rx_ber_point(rx: BtleRx, snr_db: float, n_packets: int, ppm: float = 0.0, cfo_hz: float = 0.0, amplitude: int = 64,
                  slot_samples: int = 2048, channel: int = 37, crc_init: int = 0x555555, access_addr: int = 0x8E89BED6, seed: int = 1,
                  recover: bool = False, offset_hz: float | None = None, symbol_spaced: bool = False, centre_hits: bool = False,
-                 correct: bool = False, lowpass: bool = False) -> dict:
+                 correct: bool = False, lowpass: bool = False, offset_search: bool = False) -> dict:
     """PER / BER of the reference's 4-Msps int8 receiver (btle_rx_persistent_kernel) at one channel point: ber_point()'s dict
     plus cfo_hz, amplitude and the counters len_reject, crc_ok_wrong, extra_recs, extra_crc_ok and clipped.
     generated_iq_gbytes_per_s counts the int8 capture the run synthesised and decoded (2 bytes per sample).
@@ -105,9 +109,10 @@ def rx_ber_point(rx: BtleRx, snr_db: float, n_packets: int, ppm: float = 0.0, cf
     cfo_hz undoes the impairment); None: btle_b200_rx_ber_run, uncorrected.  symbol_spaced: the receiver uses the
     symbol-spaced discriminator (BTLE_CFG_SYMBOL_SPACED).  centre_hits: the chain centres each hit on its run of matching
     sample phases (BTLE_CFG_CENTRE_HITS).  correct: CRC-failed packets are corrected from their syndrome (BTLE_CFG_CORRECT).
-    lowpass: the symbol-spaced bits read [1, 2, 1]-filtered samples (BTLE_CFG_LOWPASS)."""
+    lowpass: the symbol-spaced bits read [1, 2, 1]-filtered samples (BTLE_CFG_LOWPASS).  offset_search: the receiver decodes at
+    seven carrier offsets around offset_hz (or 0) and merges the packets (BTLE_CFG_OFFSET_SEARCH)."""
     cfg = rx_ber_cfg(snr_db, ppm, cfo_hz, amplitude, slot_samples, channel, crc_init, access_addr, seed, recover, symbol_spaced,
-                     centre_hits, correct, lowpass)
+                     centre_hits, correct, lowpass, offset_search)
     if offset_hz is None:
         res = np.zeros(1, dtype=_native.RX_BER_RESULT_DTYPE)
         rx._check(rx._L.btle_b200_rx_ber_run(rx._h, cfg.ctypes.data, int(n_packets), res.ctypes.data))
@@ -118,6 +123,7 @@ def rx_ber_point(rx: BtleRx, snr_db: float, n_packets: int, ppm: float = 0.0, cf
     sec = float(r["seconds"])
     return {"snr_db": float(snr_db), "ppm": float(ppm), "cfo_hz": float(cfo_hz), "amplitude": int(amplitude), "recover": bool(recover),
             "symbol_spaced": bool(symbol_spaced), "centre_hits": bool(centre_hits), "correct": bool(correct), "lowpass": bool(lowpass),
+            "offset_search": bool(offset_search),
             "offset_hz": offset_hz, **c,
             "ber": c["bit_err"] / max(c["bit_total"], 1), "per": c["pkt_err"] / max(c["packets"], 1), "seconds": sec,
             "packets_per_s": c["packets"] / sec if sec > 0 else 0.0,
@@ -127,8 +133,8 @@ def rx_ber_point(rx: BtleRx, snr_db: float, n_packets: int, ppm: float = 0.0, cf
 def rx_ber_sweep(snr_db, n_packets: int, ppm: float = 0.0, cfo_hz: float = 0.0, amplitude: int = 64, slot_samples: int = 2048,
                  channel: int = 37, crc_init: int = 0x555555, access_addr: int = 0x8E89BED6, seed: int = 1, device: int = 0,
                  rx: BtleRx | None = None, recover: bool = False, offset_hz: float | None = None, symbol_spaced: bool = False,
-                 centre_hits: bool = False, correct: bool = False, lowpass: bool = False):
+                 centre_hits: bool = False, correct: bool = False, lowpass: bool = False, offset_search: bool = False):
     """One rx_ber_point dict per SNR point (seeds as ber_sweep)."""
     rx = rx or BtleRx(device)
     return [rx_ber_point(rx, s, n_packets, ppm, cfo_hz, amplitude, slot_samples, channel, crc_init, access_addr, seed + 7919 * k, recover,
-                         offset_hz, symbol_spaced, centre_hits, correct, lowpass) for k, s in enumerate(snr_db)]
+                         offset_hz, symbol_spaced, centre_hits, correct, lowpass, offset_search) for k, s in enumerate(snr_db)]

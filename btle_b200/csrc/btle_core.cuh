@@ -1129,4 +1129,32 @@ BTLE_HD uint32_t crc24_unwind(uint32_t crc, uint32_t bits, int nbits) {
   return crc;
 }
 
+// ---- the merge of BTLE_CFG_OFFSET_SEARCH's hypotheses (include/btle_b200.h, rule 2) --------------------------------------
+// One record of a chunk's merged list: its n0, whether it is a counted CRC-ok record, and the caller's reference to it.
+struct OsEnt {
+  int32_t n0;
+  uint32_t ok;    // 1: counted with crc_bad == 0 (the records that stay and that hypotheses 1..6 may add)
+  uint32_t ref;
+};
+BTLE_HD uint32_t os_ok(uint8_t flags, uint8_t crc_bad) { return !(flags & (BTLE_REC_REJECTED | 1u)) && crc_bad == 0; }
+// One step of the merge: hypothesis h >= 1's record r (r.ok, else the caller skips it) against the list b[0, nb), which is
+// in n0 order.  Returns the new length: r dropped (a CRC-ok record within 8 samples), or the CRC-failed and rejected records
+// within 8 samples removed and r inserted in n0 order.  No entry left in b has r's n0, so the place is unique.
+BTLE_HD int os_merge_step(OsEnt *b, int nb, const OsEnt &r) {
+  for (int i = 0; i < nb; ++i) {
+    const int d = b[i].n0 - r.n0;
+    if (b[i].ok && d >= -8 && d <= 8) return nb;
+  }
+  int w = 0;
+  for (int i = 0; i < nb; ++i) {
+    const int d = b[i].n0 - r.n0;
+    if (d >= -8 && d <= 8) continue;
+    b[w++] = b[i];
+  }
+  int at = w;
+  while (at > 0 && b[at - 1].n0 > r.n0) { b[at] = b[at - 1]; --at; }
+  b[at] = r;
+  return w + 1;
+}
+
 }  // namespace btle

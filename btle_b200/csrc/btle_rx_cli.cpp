@@ -70,7 +70,7 @@ const char *CTRL_NAME[15] = {"LL_CONNECTION_UPDATE_REQ", "LL_CHANNEL_MAP_REQ", "
 
 struct Options {
   int chan = 37, gain = 6, lna = 32, amp = 0, verbose = 0, raw = 0, hop = 0, json = 0, quiet = 0, rssi = 0, recover = 0, symbol_spaced = 0, centre_hits = 0,
-      correct = 0, lowpass = 0;
+      correct = 0, lowpass = 0, offset_search = 0;
   uint32_t aa = 0x8E89BED6u, crc_init = 0x555555u, mask = 0xFFFFFFFFu;
   uint64_t freq_hz = 123;
   const char *pcap = nullptr, *iq_txt = nullptr, *iq_sc16 = nullptr, *iq_dir = nullptr, *iq_bin16 = nullptr;
@@ -130,6 +130,10 @@ void usage() {
       "       --centre-hits\n      each access-address hit is moved to the centre of its run of matching sample phases before the\n"
       "      packet is read: fewer length rejects and CRC failures; not the reference's receiver.  Applies to every cfg,\n"
       "      --connections and the --offset auto pass included.  Not with --iq-bin16\n"
+      "       --offset-search\n      every capture is decoded at seven carrier offsets around its own (0, +-50, +-100, +-150 kHz from the\n"
+      "      --offset value or the capture's HZ field) and the packets merged: transmitters at different offsets are all\n"
+      "      received; not the reference's receiver.  NDJSON adds \"offset_search\":true to packets the centre offset missed.\n"
+      "      Applies to every cfg, --connections and the --offset auto pass included.  Not with -r or --iq-bin16\n"
       "    -F --filter-adva AA:BB:CC:DD:EE:FF / -T --filter-pdu-type 0,3,4\n"
       "    -d --device N   CUDA device (default 0)\n");
 }
@@ -179,7 +183,8 @@ Options parse_commandline(int argc, char **argv) {
       {"iq-dir", required_argument, 0, 1002}, {"segment-chunks", required_argument, 0, 1003}, {"iq-bin16", required_argument, 0, 1004},
       {"connections", no_argument, 0, 1005}, {"recover", no_argument, 0, 1006}, {"correct", no_argument, 0, 1010},
       {"offset", required_argument, 0, 1007}, {"symbol-spaced", no_argument, 0, 1008},
-      {"centre-hits", no_argument, 0, 1009}, {"lowpass", no_argument, 0, 1011}, {0, 0, 0, 0}};
+      {"centre-hits", no_argument, 0, 1009}, {"lowpass", no_argument, 0, 1011},
+      {"offset-search", no_argument, 0, 1012}, {0, 0, 0, 0}};
   for (;;) {
     int idx = 0;
     const int c = getopt_long(argc, argv, "hc:g:l:ba:k:vrf:m:os:jQRF:T:i:d:", longopts, &idx);   // + i:, d:
@@ -210,6 +215,7 @@ Options parse_commandline(int argc, char **argv) {
       case 1008: o.symbol_spaced = 1; break;
       case 1009: o.centre_hits = 1; break;
       case 1011: o.lowpass = 1; break;
+      case 1012: o.offset_search = 1; break;
       case 1007:
         o.offset_set = 1;
         if (!strcmp(optarg, "auto")) { o.offset_auto = 1; break; }
@@ -252,6 +258,8 @@ Options parse_commandline(int argc, char **argv) {
   if (o.symbol_spaced && o.iq_bin16) { printf("--symbol-spaced cannot be combined with --iq-bin16 (the 8-sps receiver has its own discriminator)\n"); bad_args(); }
   if (o.centre_hits && o.iq_bin16) { printf("--centre-hits cannot be combined with --iq-bin16 (the 8-sps receiver has its own hit rule)\n"); bad_args(); }
   if (o.lowpass && (!o.symbol_spaced || o.iq_bin16)) { printf("--lowpass needs --symbol-spaced and cannot be combined with --iq-bin16\n"); bad_args(); }
+  // raw records have no CRC verdict to merge the hypotheses by
+  if (o.offset_search && (o.raw || o.iq_bin16)) { printf("--offset-search cannot be combined with -r or --iq-bin16\n"); bad_args(); }
   return o;
 }
 
@@ -484,6 +492,7 @@ struct Sinks {
         if (rssi == INT_MIN) printf(",\"rssi_est\":null"); else printf(",\"rssi_est\":%d", rssi);
         if (r.flags & BTLE_REC_RECOVERED) printf(",\"recovered\":%d", BTLE_REC_RECOVERED_Q(r.flags));
         if (r.flags & BTLE_REC_CORRECTED) printf(",\"corrected\":true");
+        if (r.flags & BTLE_REC_OFFSET_SEARCH) printf(",\"offset_search\":true");
         printf("}\n");
       }
     } else {
@@ -507,6 +516,7 @@ struct Sinks {
         if (rssi == INT_MIN) printf(",\"rssi_est\":null"); else printf(",\"rssi_est\":%d", rssi);
         if (r.flags & BTLE_REC_RECOVERED) printf(",\"recovered\":%d", BTLE_REC_RECOVERED_Q(r.flags));
         if (r.flags & BTLE_REC_CORRECTED) printf(",\"corrected\":true");
+        if (r.flags & BTLE_REC_OFFSET_SEARCH) printf(",\"offset_search\":true");
         printf("}\n");
       }
     }
@@ -598,7 +608,7 @@ Capture parse_capture(const std::string &spec, const Options &o) {
 int cfg_flags(const Options &o) {
   return (o.rssi ? BTLE_CFG_RSSI : 0) | (o.verbose ? BTLE_CFG_REPORT_REJECTED : 0) | (o.recover ? BTLE_CFG_RECOVER : 0) |
          (o.symbol_spaced ? BTLE_CFG_SYMBOL_SPACED : 0) | (o.centre_hits ? BTLE_CFG_CENTRE_HITS : 0) |
-         (o.correct ? BTLE_CFG_CORRECT : 0) | (o.lowpass ? BTLE_CFG_LOWPASS : 0);
+         (o.correct ? BTLE_CFG_CORRECT : 0) | (o.lowpass ? BTLE_CFG_LOWPASS : 0) | (o.offset_search ? BTLE_CFG_OFFSET_SEARCH : 0);
 }
 
 int fail(btle_b200_ctx *ctx, int rc, const char *what) {
@@ -622,11 +632,11 @@ int rx_batch_grow(btle_b200_ctx *ctx, const int8_t *iq, size_t ns, size_t stride
 }
 
 // --offset auto: the median of btle_b200_rec_offset over the CRC-ok counted packets of a first pass without correction
-// (not raw, no flags but cfg's discriminator mode and hit rule), 0 when no packet passes; printed on stderr under `name`.
+// (not raw, no flags but cfg's discriminator mode, hit rule and offset bank), 0 when no packet passes; printed on stderr under `name`.
 // Returns the exit status.
 int estimate_offset(btle_b200_ctx *ctx, const std::vector<int8_t> &iq, btle_stream_cfg cfg, const char *name, float *hz) {
   cfg.raw = 0;
-  cfg.rssi &= BTLE_CFG_SYMBOL_SPACED | BTLE_CFG_LOWPASS | BTLE_CFG_CENTRE_HITS;
+  cfg.rssi &= BTLE_CFG_SYMBOL_SPACED | BTLE_CFG_LOWPASS | BTLE_CFG_CENTRE_HITS | BTLE_CFG_OFFSET_SEARCH;
   std::vector<btle_pkt_rec> recs;
   int rc = rx_batch_grow(ctx, iq.data(), 1, iq.size(), iq.size(), &cfg, recs);
   recs.erase(std::remove_if(recs.begin(), recs.end(), [](const btle_pkt_rec &r) { return r.crc_bad || (r.flags & BTLE_REC_REJECTED); }),
@@ -701,7 +711,7 @@ struct ConnMonitor {
       const btle_stream_cfg cfg{ch, c.aa, 0xFFFFFFFFu, c.crc_init, 0,
                                 (o.rssi ? BTLE_CFG_RSSI : 0) | (o.recover ? BTLE_CFG_RECOVER : 0) | (o.symbol_spaced ? BTLE_CFG_SYMBOL_SPACED : 0) |
                                     (o.centre_hits ? BTLE_CFG_CENTRE_HITS : 0) | (o.correct ? BTLE_CFG_CORRECT : 0) |
-                                    (o.lowpass ? BTLE_CFG_LOWPASS : 0)};
+                                    (o.lowpass ? BTLE_CFG_LOWPASS : 0) | (o.offset_search ? BTLE_CFG_OFFSET_SEARCH : 0)};
       size_t j = 0;
       rc = btle_b200_streams_add_cfg(ss, (size_t)ch, &cfg, from, &j);
       c.cfgs.push_back(j);

@@ -1927,6 +1927,97 @@ model_rx_batch_kernel(const int16_t *__restrict__ gi, const int16_t *__restrict_
   for (int b = lane; b < 70; b += 32) o->pdu[b] = (uint8_t)(P[b >> 2] >> (8 * (b & 3)));
 }
 
+// ---- BTLE_CFG_OFFSET_SEARCH: the merge of the seven hypotheses (include/btle_b200.h, rule 2) ---------------------------------
+// The hypotheses were decoded by one btle_rx_persistent_kernel<kMaxCfgsPerCapture, true, DISC> launch over capture groups
+// keyed by (capture, hypothesis): original group g (first cfg f_g, k_g cfgs) became groups 7 g + h, h = 0..6, with first
+// cfg 7 f_g + h k_g (xvmap[7 g + h].y), so cfg j's hypothesis h is expanded cfg xvmap[7 g + h].y + j - f_g.  Its records of
+// chunk k sit in its directory entry xcfg * per_x + k / piece_x, in (chunk, n0) order.
+// One warp per directory entry u of the layout without the flag (cfg j = u / per0, its unit `local` = u % per0, the chunks of
+// unit g * per0 + local of plan0).  Lane 0 runs the merge chunk by chunk (os_merge_step, the code the CPU emulator runs) into
+// the warp's list; the warp sums the counts, reserves the unit's block with one atomic, runs the merge again and stores.
+// xcount > xcap (a hypothesis record was not stored): nothing is merged, and each entry counts the hypotheses' records of the
+// units that start inside it, so the directory sums to the hypotheses' total.
+constexpr int kOsWarps = 4, kOsHyps = BTLE_OFFSET_SEARCH_HYPS;
+__global__ void __launch_bounds__(kOsWarps * 32)
+btle_offset_merge_kernel(const btle_pkt_rec *__restrict__ xrec, const uint2 *__restrict__ xdir, const unsigned *__restrict__ xcount,
+                         unsigned xcap, const int4 *__restrict__ xvmap, int n_groups, const Plan plan0, int per0, int per_x, int piece_x,
+                         int n_units, btle_pkt_rec *__restrict__ out, unsigned cap, unsigned *__restrict__ count, uint2 *__restrict__ dir) {
+  __shared__ OsEnt list[kOsWarps][BTLE_MAX_MERGED_RECS_PER_CHUNK];
+  const int lane = threadIdx.x & 31, u = blockIdx.x * kOsWarps + (threadIdx.x >> 5);
+  if (u >= n_units) return;
+  OsEnt *B = list[threadIdx.x >> 5];
+  const int j = u / per0, local = u - j * per0;
+  int lo = 0, hi = n_groups - 1;                           // j's group: the last g with f_g <= j
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (__ldg(&xvmap[kOsHyps * mid].y) <= kOsHyps * j) lo = mid; else hi = mid - 1;
+  }
+  const int off = j - __ldg(&xvmap[kOsHyps * lo].y) / kOsHyps;
+  int xcfg[kOsHyps];
+#pragma unroll
+  for (int h = 0; h < kOsHyps; ++h) xcfg[h] = __ldg(&xvmap[kOsHyps * lo + h].y) + off;
+  const UnitInfo ui = unit_info(lo * per0 + local, plan0);
+  if (*xcount > xcap) {
+    unsigned t = 0;
+    for (int k = ui.chunk0; k < ui.chunk0 + ui.nch; ++k)
+      if (lane < kOsHyps && k % piece_x == 0) t += xdir[xcfg[lane] * per_x + k / piece_x].y;
+    t = __reduce_add_sync(0xFFFFFFFFu, t);
+    if (lane == 0) dir[u] = make_uint2(t ? atomicAdd(count, t) : 0u, t);
+    return;
+  }
+  // chunk k's merged list into B; returns its length (warp-collective)
+  auto merge = [&](int k) -> int {
+    int rb[kOsHyps], rn[kOsHyps];
+#pragma unroll
+    for (int h = 0; h < kOsHyps; ++h) {
+      const uint2 d = xdir[xcfg[h] * per_x + k / piece_x];
+      int before = 0, at = 0;
+      for (unsigned i = lane; i < d.y; i += 32) {
+        const int c = xrec[d.x + i].chunk;
+        before += c < k;
+        at += c == k;
+      }
+      rb[h] = (int)d.x + __reduce_add_sync(0xFFFFFFFFu, before);
+      rn[h] = __reduce_add_sync(0xFFFFFFFFu, at);
+    }
+    int n = 0;
+    if (lane == 0) {
+      for (int i = 0; i < rn[0]; ++i) {
+        const btle_pkt_rec &r = xrec[rb[0] + i];
+        B[n++] = OsEnt{r.n0, os_ok(r.flags, r.crc_bad), (uint32_t)(rb[0] + i)};
+      }
+      for (int h = 1; h < kOsHyps; ++h)
+        for (int i = 0; i < rn[h]; ++i) {
+          const btle_pkt_rec &r = xrec[rb[h] + i];
+          if (os_ok(r.flags, r.crc_bad)) n = os_merge_step(B, n, OsEnt{r.n0, 1u, (uint32_t)(rb[h] + i)});
+        }
+    }
+    __syncwarp();
+    return __shfl_sync(0xFFFFFFFFu, n, 0);
+  };
+  unsigned total = 0;
+  for (int k = ui.chunk0; k < ui.chunk0 + ui.nch; ++k) total += (unsigned)merge(k);
+  unsigned base = 0;
+  if (lane == 0) {
+    if (total) base = atomicAdd(count, total);
+    dir[u] = make_uint2(base, total);
+  }
+  base = __shfl_sync(0xFFFFFFFFu, base, 0);
+  unsigned pos = 0;
+  for (int k = ui.chunk0; k < ui.chunk0 + ui.nch && base + pos < cap; ++k) {
+    const int n = merge(k);
+    for (int i = lane; i < n; i += 32)
+      if (base + pos + (unsigned)i < cap) {
+        btle_pkt_rec r = xrec[B[i].ref];
+        if (r.stream != xcfg[0]) r.flags |= BTLE_REC_OFFSET_SEARCH;
+        r.stream = j;
+        out[base + pos + i] = r;
+      }
+    pos += (unsigned)n;
+    __syncwarp();
+  }
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -2016,6 +2107,12 @@ struct btle_b200_ctx {
   cudaEvent_t stage_free[2] = {nullptr, nullptr};
   Buf<uint8_t> d_leaf;              // scratch of the leaf entry points (leaf_layout)
   Buf<btle_conn_cand> d_cand;       // device candidates of btle_b200_discover
+  // BTLE_CFG_OFFSET_SEARCH (launch_offset_search): the hypotheses' records, directory and counters [hypotheses, merged], and
+  // the last launch that used them (a flagged launch on another stream waits for it)
+  Buf<btle_pkt_rec> os_out;
+  Buf<btle_unit_dir> os_dir;
+  Buf<unsigned> os_count;
+  StreamUse os_last;
 };
 
 template <class T, bool kHost>
@@ -2088,6 +2185,16 @@ int validate_cfgs(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size_t n) {
       ctx->err = "all cfgs of one launch must agree on BTLE_CFG_LOWPASS";
       return BTLE_EINVAL;
     }
+  for (size_t i = 0; i < n; ++i) {
+    if ((cfgs[i].rssi ^ cfgs[0].rssi) & BTLE_CFG_OFFSET_SEARCH) {
+      ctx->err = "all cfgs of one launch must agree on BTLE_CFG_OFFSET_SEARCH";
+      return BTLE_EINVAL;
+    }
+    if ((cfgs[i].rssi & BTLE_CFG_OFFSET_SEARCH) && cfgs[i].raw) {
+      ctx->err = "BTLE_CFG_OFFSET_SEARCH needs CRC verdicts: not with raw cfgs";
+      return BTLE_EINVAL;
+    }
+  }
   return BTLE_OK;
 }
 
@@ -2095,6 +2202,13 @@ int validate_cfgs(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size_t n) {
 int stream_id(btle_b200_ctx *ctx, cudaStream_t st, unsigned long long *sid) {
   BTLE_CUDA(ctx, cudaStreamGetId(st, sid));
   return BTLE_OK;
+}
+
+// A capture group of a cfg list (vmap): a run of cfgs on one capture at one rotation.  The entry points rotate every cfg of a
+// capture alike, so there it is a run of one capture; BTLE_CFG_OFFSET_SEARCH's hypotheses are groups of their own.
+bool new_group(const int32_t *cfg_capture, const int4 *rot, size_t i) {
+  return !i || cfg_capture[i] != cfg_capture[i - 1] ||
+         (rot && (rot[i].x != rot[i - 1].x || rot[i].y != rot[i - 1].y || rot[i].z != rot[i - 1].z || rot[i].w != rot[i - 1].w));
 }
 
 // The cfg array of a launch must live on the device while the kernel runs.  Uploaded arrays are kept in a small LRU
@@ -2154,7 +2268,7 @@ int upload_cfgs(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size_t n, cudaS
     if (cfg_capture) {
       pick->cfg_capture.assign(cfg_capture, cfg_capture + n);
       for (size_t i = 0; i < n; ++i) {
-        if (!i || cfg_capture[i] != cfg_capture[i - 1]) pick->h_vmap[pick->n_vmap++] = make_int4(cfg_capture[i], (int)i, 0, 0);
+        if (new_group(cfg_capture, rot, i)) pick->h_vmap[pick->n_vmap++] = make_int4(cfg_capture[i], (int)i, 0, 0);
         ++pick->h_vmap[pick->n_vmap - 1].z;
       }
       BTLE_CUDA(ctx, cudaMemcpyAsync(pick->d_vmap, pick->h_vmap, pick->n_vmap * sizeof(int4), cudaMemcpyHostToDevice, st));
@@ -2256,15 +2370,15 @@ int4 make_rot(float hz) {
   return make_int4((int)lrint(16384.0 * cos(ph)), (int)lrint(16384.0 * sin(ph)), (int)lrint(16384.0 * cos(4.0 * ph)),
                    (int)lrint(16384.0 * sin(4.0 * ph)));
 }
-// rotations of n cfgs from one offset per capture (cfg i reads capture cap_of[i], or i when cap_of is nullptr)
-int make_rots(btle_b200_ctx *ctx, const float *offset_hz, size_t n_captures, const int32_t *cap_of, size_t n, std::vector<int4> &rot) {
+// offsets of n cfgs from one offset per capture (cfg i reads capture cap_of[i], or i when cap_of is nullptr)
+int cfg_offsets(btle_b200_ctx *ctx, const float *offset_hz, size_t n_captures, const int32_t *cap_of, size_t n, std::vector<float> &hz) {
   for (size_t c = 0; c < n_captures; ++c)
     if (!std::isfinite(offset_hz[c]) || std::fabs(offset_hz[c]) > (float)BTLE_MAX_OFFSET_HZ) {
       ctx->err = "offset_hz must be finite and within +-BTLE_MAX_OFFSET_HZ";
       return BTLE_EINVAL;
     }
-  rot.resize(n);
-  for (size_t i = 0; i < n; ++i) rot[i] = make_rot(offset_hz[cap_of ? cap_of[i] : i]);
+  hz.resize(n);
+  for (size_t i = 0; i < n; ++i) hz[i] = offset_hz[cap_of ? cap_of[i] : i];
   return BTLE_OK;
 }
 
@@ -2285,19 +2399,25 @@ void enqueue_rx(unsigned grid, cudaStream_t st, const MapSlot *ms, const int8_t 
 // capture (the stream session's lead: RSSI of hits at a segment's very start, the symbol-spaced bits of its first samples).
 // cfgs with BTLE_CFG_SYMBOL_SPACED (all or none, validate_cfgs) run the symbol-spaced variant, and with BTLE_CFG_LOWPASS too
 // (again all or none) the low-pass one.
-int launch_rx(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8, const btle_stream_cfg *cfgs,
-              const int32_t *cfg_capture, size_t n_cfgs, const int4 *rot, btle_pkt_rec *d_out, size_t cap, unsigned *d_count,
-              btle_unit_dir *d_dir, cudaStream_t st, long long lead) {
+// *slot_out: the cfg slot the kernel reads (nullptr when nothing was launched).
+int launch_rx_kernel(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8, const btle_stream_cfg *cfgs,
+                     const int32_t *cfg_capture, size_t n_cfgs, const int4 *rot, btle_pkt_rec *d_out, size_t cap, unsigned *d_count,
+                     btle_unit_dir *d_dir, cudaStream_t st, long long lead, CfgSlot **slot_out) {
   ctx->last_launches = 0;
+  *slot_out = nullptr;
   unsigned *zero_next = nullptr;
   if (d_count) BTLE_CUDA(ctx, cudaMemsetAsync(d_count, 0, sizeof(unsigned), st));
   const long long nchunks = (long long)(n_int8 / kChunkInt8);
   if (nchunks == 0 || n_streams == 0 || n_cfgs == 0) return BTLE_OK;
-  size_t groups = n_streams;                                  // captures the launch reads
+  size_t groups = n_streams;                                  // capture groups the launch reads (new_group)
   if (cfg_capture) {
+    size_t caps = 0;
     groups = 0;
-    for (size_t i = 0; i < n_cfgs; ++i) groups += !i || cfg_capture[i] != cfg_capture[i - 1];
-    if (groups == n_cfgs && n_cfgs == n_streams) cfg_capture = nullptr;   // cfg i on capture i
+    for (size_t i = 0; i < n_cfgs; ++i) {
+      caps += !i || cfg_capture[i] != cfg_capture[i - 1];
+      groups += new_group(cfg_capture, rot, i);
+    }
+    if (groups == n_cfgs && caps == n_cfgs && n_cfgs == n_streams) cfg_capture = nullptr;   // cfg i on capture i
   }
   const bool multi = cfg_capture != nullptr;
   unsigned long long sid = 0;
@@ -2351,7 +2471,92 @@ int launch_rx(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t s
   rc = note_use(ctx, cs, st, sid);
   if (rc) return rc;
   ctx->last_launches = 1;
+  *slot_out = cs;
   return BTLE_OK;
+}
+
+// BTLE_CFG_OFFSET_SEARCH (include/btle_b200.h): the launch of launch_rx with every capture's cfgs expanded into the seven
+// hypotheses, capture-major, decoded by one launch of the rotated multi-cfg kernel into ctx->os_*, then merged into the
+// caller's buffers in the directory layout of the launch without the flag (btle_offset_merge_kernel).
+int launch_offset_search(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8, const btle_stream_cfg *cfgs,
+                         const int32_t *cfg_capture, size_t n_cfgs, const float *hz, btle_pkt_rec *d_out, size_t cap, unsigned *d_count,
+                         btle_unit_dir *d_dir, cudaStream_t st, long long lead) {
+  static const float kDelta[kOsHyps] = BTLE_OFFSET_SEARCH_HZ;
+  ctx->last_launches = 0;
+  for (size_t i = 0; hz && i < n_cfgs; ++i)
+    if (std::fabs(hz[i]) + (float)BTLE_OFFSET_SEARCH_SPAN_HZ > (float)BTLE_MAX_OFFSET_HZ) {
+      ctx->err = "BTLE_CFG_OFFSET_SEARCH: |offset_hz| + 150 kHz must be within BTLE_MAX_OFFSET_HZ";
+      return BTLE_EINVAL;
+    }
+  if (d_count) BTLE_CUDA(ctx, cudaMemsetAsync(d_count, 0, sizeof(unsigned), st));
+  if (n_int8 < (size_t)kChunkInt8 || n_streams == 0 || n_cfgs == 0) return BTLE_OK;
+  std::vector<btle_stream_cfg> xc;
+  std::vector<int32_t> xcap;
+  std::vector<int4> xrot;
+  int groups = 0;
+  for (size_t f = 0; f < n_cfgs; ++groups) {                 // [f, e): the cfgs of one capture
+    const int32_t c = cfg_capture ? cfg_capture[f] : (int32_t)f;
+    size_t e = f + 1;
+    while (cfg_capture && e < n_cfgs && cfg_capture[e] == c) ++e;
+    for (int h = 0; h < kOsHyps; ++h)
+      for (size_t i = f; i < e; ++i) {
+        xc.push_back(cfgs[i]);
+        xcap.push_back(c);
+        xrot.push_back(make_rot((hz ? hz[i] : 0.0f) + kDelta[h]));
+      }
+    f = e;
+  }
+  const Plan plan0 = plan_for(ctx, (size_t)groups, n_int8), plan_x = plan_for(ctx, (size_t)groups * kOsHyps, n_int8);
+  if (plan0.tail_units || (plan0.big_units && plan0.big_units != plan0.total_units)) {
+    ctx->err = "BTLE_CFG_OFFSET_SEARCH: this build's unit plan is not the same for every capture";   // (A/B builds)
+    return BTLE_EINVAL;
+  }
+  const size_t units = rx_units(ctx, (size_t)groups, n_cfgs, n_int8), units_x = rx_units(ctx, (size_t)groups * kOsHyps, xc.size(), n_int8);
+  if (units > 0x7FFFFFFFu) { ctx->err = "batch too large for one launch"; return BTLE_EINVAL; }
+  unsigned long long sid = 0;
+  int rc = stream_id(ctx, st, &sid);
+  if (rc) return rc;
+  StreamUse &last = ctx->os_last;
+  if (!last.ev) BTLE_CUDA(ctx, cudaEventCreateWithFlags(&last.ev, cudaEventDisableTiming));
+  if (last.stamp && last.stream != sid) BTLE_CUDA(ctx, cudaStreamWaitEvent(st, last.ev, 0));
+  if (ctx->os_out.reserve(ctx, std::max<size_t>(cap, 1)) || ctx->os_dir.reserve(ctx, std::max<size_t>(units_x, 1)) ||
+      (ctx->os_count.n < 2 && ctx->os_count.alloc(ctx, 2)))
+    return BTLE_ENOMEM;
+  CfgSlot *cs = nullptr;
+  rc = launch_rx_kernel(ctx, d_iq, n_streams, stride, n_int8, xc.data(), xcap.data(), xc.size(), xrot.data(), ctx->os_out, cap,
+                        ctx->os_count.p, ctx->os_dir, st, lead, &cs);
+  if (rc) return rc;
+  if (!d_count) {
+    d_count = ctx->os_count.p + 1;
+    BTLE_CUDA(ctx, cudaMemsetAsync(d_count, 0, sizeof(unsigned), st));
+  }
+  const int per0 = (int)(plan0.total_units / groups), per_x = (int)(plan_x.total_units / (groups * kOsHyps));
+  const unsigned cap32 = (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu);
+  btle_offset_merge_kernel<<<(unsigned)((units + kOsWarps - 1) / kOsWarps), kOsWarps * 32, 0, st>>>(
+      ctx->os_out, reinterpret_cast<const uint2 *>(ctx->os_dir.p), ctx->os_count.p, cap32, cs->d_vmap, groups, plan0, per0, per_x,
+      plan_x.piece, (int)units, d_out, cap32, d_count, reinterpret_cast<uint2 *>(d_dir));
+  BTLE_CUDA(ctx, cudaGetLastError());
+  rc = note_use(ctx, cs, st, sid);                          // the merge reads the slot's vmap too
+  if (rc) return rc;
+  BTLE_CUDA(ctx, cudaEventRecord(last.ev, st));
+  last.stream = sid;
+  last.stamp = ++ctx->tick;
+  ctx->last_launches = 2;
+  return BTLE_OK;
+}
+
+// The receive launch of every entry point: hz (nullptr: not rotated) = the carrier offset of each cfg, make_rot'd here;
+// with BTLE_CFG_OFFSET_SEARCH (all cfgs or none, validate_cfgs) launch_offset_search.
+int launch_rx(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8, const btle_stream_cfg *cfgs,
+              const int32_t *cfg_capture, size_t n_cfgs, const float *hz, btle_pkt_rec *d_out, size_t cap, unsigned *d_count,
+              btle_unit_dir *d_dir, cudaStream_t st, long long lead) {
+  if (n_cfgs && (cfgs[0].rssi & BTLE_CFG_OFFSET_SEARCH))
+    return launch_offset_search(ctx, d_iq, n_streams, stride, n_int8, cfgs, cfg_capture, n_cfgs, hz, d_out, cap, d_count, d_dir, st, lead);
+  std::vector<int4> rot;
+  for (size_t i = 0; hz && i < n_cfgs; ++i) rot.push_back(make_rot(hz[i]));
+  CfgSlot *cs = nullptr;
+  return launch_rx_kernel(ctx, d_iq, n_streams, stride, n_int8, cfgs, cfg_capture, n_cfgs, hz ? rot.data() : nullptr, d_out, cap, d_count,
+                          d_dir, st, lead, &cs);
 }
 
 bool rec_less(const btle_pkt_rec &a, const btle_pkt_rec &b) {
@@ -2486,10 +2691,10 @@ int rx_device_path(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_captures, si
   if (dir_cap < rx_units(ctx, groups, n_cfgs, n_int8)) { ctx->err = "unit directory too small (btle_b200_rx_units / _rx_multi_units)"; return BTLE_EINVAL; }
   rc = validate_cfgs(ctx, cfgs, n_cfgs);
   if (rc) return rc;
-  std::vector<int4> rot;
-  if (offset_hz && (rc = make_rots(ctx, offset_hz, n_captures, cfg_capture, n_cfgs, rot))) return rc;
+  std::vector<float> hz;
+  if (offset_hz && (rc = cfg_offsets(ctx, offset_hz, n_captures, cfg_capture, n_cfgs, hz))) return rc;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
-  return launch_rx(ctx, d_iq, n_captures, stride, n_int8, cfgs, cfg_capture, n_cfgs, offset_hz ? rot.data() : nullptr, d_out, cap, d_count,
+  return launch_rx(ctx, d_iq, n_captures, stride, n_int8, cfgs, cfg_capture, n_cfgs, offset_hz ? hz.data() : nullptr, d_out, cap, d_count,
                    d_dir, reinterpret_cast<cudaStream_t>(cuda_stream), 0);
 }
 
@@ -2505,8 +2710,8 @@ int rx_host_path(btle_b200_ctx *ctx, const int8_t *iq, size_t n_captures, size_t
   if (rc) return rc;
   rc = validate_cfgs(ctx, cfgs, n_cfgs);
   if (rc) return rc;
-  std::vector<int4> rot;
-  if (offset_hz && (rc = make_rots(ctx, offset_hz, n_captures, cfg_capture, n_cfgs, rot))) return rc;
+  std::vector<float> hz;
+  if (offset_hz && (rc = cfg_offsets(ctx, offset_hz, n_captures, cfg_capture, n_cfgs, hz))) return rc;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
   std::vector<int32_t> caps, local;                          // the captures read, in order; cfg i reads caps[local[i]]
   for (size_t i = 0; cfg_capture && i < n_cfgs; ++i) {
@@ -2518,7 +2723,7 @@ int rx_host_path(btle_b200_ctx *ctx, const int8_t *iq, size_t n_captures, size_t
   if (rc) return rc;
   const size_t units = rx_units(ctx, groups, n_cfgs, n_int8);
   if (ctx->d_out.reserve(ctx, std::max<size_t>(cap, 1)) || ctx->d_dir.reserve(ctx, std::max<size_t>(units, 1))) return BTLE_ENOMEM;
-  rc = launch_rx(ctx, ctx->d_iq, groups, pitch, n_int8, cfgs, cfg_capture ? local.data() : nullptr, n_cfgs, offset_hz ? rot.data() : nullptr,
+  rc = launch_rx(ctx, ctx->d_iq, groups, pitch, n_int8, cfgs, cfg_capture ? local.data() : nullptr, n_cfgs, offset_hz ? hz.data() : nullptr,
                  ctx->d_out, cap, ctx->d_count, ctx->d_dir, ctx->stream, 0);
   if (rc) return rc;
   return fetch_ordered(ctx, ctx->d_out, ctx->d_dir, units, out, cap, n_out, ctx->stream);
@@ -2722,6 +2927,7 @@ void btle_b200_destroy(btle_b200_ctx *ctx) {
     for (StreamUse &u : c.use) if (u.ev) cudaEventDestroy(u.ev);
   }
   for (StreamUse &u : ctx->ring_last) if (u.ev) cudaEventDestroy(u.ev);
+  if (ctx->os_last.ev) cudaEventDestroy(ctx->os_last.ev);
   for (cudaEvent_t e : ctx->stage_free) if (e) cudaEventDestroy(e);
   delete ctx;                                               // frees the buffers
 }
@@ -2965,20 +3171,23 @@ int streams_job(Streams *s, int b, const std::vector<size_t> &idx) {
   std::vector<btle_stream_cfg> cfgs(k);
   std::vector<int32_t> cc(k);
   size_t groups = 0;                                         // captures the round reads
-  std::vector<int4> rot;                                     // H.offset non-empty: the rotated kernel, capture cc[i]'s offset
+  std::vector<float> hz;                                     // H.offset non-empty: the rotated kernel, capture cc[i]'s offset
   for (size_t i = 0; i < k; ++i) {
     cfgs[i] = s->entries[idx[i]].cfg;
     cc[i] = (int32_t)s->entries[idx[i]].capture;
     groups += !i || cc[i] != cc[i - 1];
-    if (!H.offset.empty()) rot.push_back(make_rot(H.offset[cc[i]]));
+    if (!H.offset.empty()) hz.push_back(H.offset[cc[i]]);
   }
   const size_t units = std::max<size_t>(rx_units(ctx, groups, k, H.n_submitted), 1);
-  const size_t cap = k * nch * BTLE_MAX_RECS_PER_CHUNK;      // the most a launch can find: never an overflow
+  // the most a launch can find: never an overflow (BTLE_CFG_OFFSET_SEARCH: the seven hypotheses' records, which bound the
+  // merged ones, share a scratch of `cap` records)
+  const bool os = (cfgs[0].rssi & BTLE_CFG_OFFSET_SEARCH) != 0;
+  const size_t cap = k * nch * BTLE_MAX_RECS_PER_CHUNK * (os ? BTLE_OFFSET_SEARCH_HYPS : 1);
   if (J.d_out.reserve(ctx, cap) || J.d_dir.reserve(ctx, units) || J.h_dir.reserve(ctx, units) ||
       (!J.d_count && (J.d_count.alloc(ctx, 1) || J.h_count.alloc(ctx, 1))))
     return BTLE_ENOMEM;
   const int rc = launch_rx(ctx, H.d + Streams::kLead, s->n, s->stride, H.n_submitted, cfgs.data(), cc.data(), k,
-                           rot.empty() ? nullptr : rot.data(), J.d_out, cap, J.d_count, J.d_dir, H.st, Streams::kLead);
+                           hz.empty() ? nullptr : hz.data(), J.d_out, cap, J.d_count, J.d_dir, H.st, Streams::kLead);
   if (rc) return rc;
   BTLE_CUDA(ctx, cudaMemcpyAsync(J.h_count, J.d_count, sizeof(unsigned), cudaMemcpyDeviceToHost, H.st));
   BTLE_CUDA(ctx, cudaMemcpyAsync(J.h_dir, J.d_dir, units * sizeof(btle_unit_dir), cudaMemcpyDeviceToHost, H.st));
@@ -3219,8 +3428,9 @@ int streams_index(btle_b200_streams *s, size_t stream) {
 // a session decodes in the BTLE_CFG_SYMBOL_SPACED and BTLE_CFG_LOWPASS mode of the cfgs it was opened with (entries[0]
 // keeps it), so every round, backfill included, is one launch of one kernel variant
 int streams_check_mode(btle_b200_streams *s, const btle_stream_cfg *cfg) {
-  if (!((cfg->rssi ^ s->entries[0].cfg.rssi) & (BTLE_CFG_SYMBOL_SPACED | BTLE_CFG_LOWPASS))) return BTLE_OK;
-  s->ctx->err = "a session's cfgs must all agree on BTLE_CFG_SYMBOL_SPACED and BTLE_CFG_LOWPASS (the mode of streams_open)";
+  if (!((cfg->rssi ^ s->entries[0].cfg.rssi) & (BTLE_CFG_SYMBOL_SPACED | BTLE_CFG_LOWPASS | BTLE_CFG_OFFSET_SEARCH))) return BTLE_OK;
+  s->ctx->err = "a session's cfgs must all agree on BTLE_CFG_SYMBOL_SPACED, BTLE_CFG_LOWPASS and BTLE_CFG_OFFSET_SEARCH (the mode of "
+                "streams_open)";
   return BTLE_EINVAL;
 }
 }  // namespace
@@ -3293,8 +3503,12 @@ int btle_b200_streams_set_offset(btle_b200_streams *s, size_t capture, float off
   if (!s) return BTLE_EINVAL;
   int rc = streams_index(s, capture);
   if (rc) return rc;
-  std::vector<int4> rot;
-  if ((rc = make_rots(s->ctx, &offset_hz, 1, nullptr, 1, rot))) return rc;
+  std::vector<float> hz;
+  if ((rc = cfg_offsets(s->ctx, &offset_hz, 1, nullptr, 1, hz))) return rc;
+  if ((s->entries[0].cfg.rssi & BTLE_CFG_OFFSET_SEARCH) && std::fabs(offset_hz) + (float)BTLE_OFFSET_SEARCH_SPAN_HZ > (float)BTLE_MAX_OFFSET_HZ) {
+    s->ctx->err = "BTLE_CFG_OFFSET_SEARCH: |offset_hz| + 150 kHz must be within BTLE_MAX_OFFSET_HZ";
+    return BTLE_EINVAL;
+  }
   if (s->offset.empty()) s->offset.assign(s->n, 0.0f);    // from now on every set takes the rotated kernel
   s->offset[capture] = offset_hz;                           // used from the next submitted segment set on
   return BTLE_OK;
@@ -3871,8 +4085,10 @@ static int check_rx_ber_cfg(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg) {
   }
   if (std::fabs(cfg->ppm) >= 1e6f) { ctx->err = "rx_ber: ppm must have |ppm| < 1e6"; return BTLE_EINVAL; }
   if (cfg->amplitude < 1 || cfg->amplitude > 127) { ctx->err = "rx_ber: amplitude must be 1..127"; return BTLE_EINVAL; }
-  if (cfg->flags & ~(uint32_t)(BTLE_CFG_RECOVER | BTLE_CFG_SYMBOL_SPACED | BTLE_CFG_CENTRE_HITS | BTLE_CFG_CORRECT | BTLE_CFG_LOWPASS)) {
-    ctx->err = "rx_ber: flags may only hold BTLE_CFG_RECOVER, BTLE_CFG_SYMBOL_SPACED, BTLE_CFG_CENTRE_HITS, BTLE_CFG_CORRECT and BTLE_CFG_LOWPASS";
+  if (cfg->flags & ~(uint32_t)(BTLE_CFG_RECOVER | BTLE_CFG_SYMBOL_SPACED | BTLE_CFG_CENTRE_HITS | BTLE_CFG_CORRECT | BTLE_CFG_LOWPASS |
+                               BTLE_CFG_OFFSET_SEARCH)) {
+    ctx->err = "rx_ber: flags may only hold BTLE_CFG_RECOVER, BTLE_CFG_SYMBOL_SPACED, BTLE_CFG_CENTRE_HITS, BTLE_CFG_CORRECT, BTLE_CFG_LOWPASS "
+               "and BTLE_CFG_OFFSET_SEARCH";
     return BTLE_EINVAL;
   }
   if ((cfg->flags & BTLE_CFG_LOWPASS) && !(cfg->flags & BTLE_CFG_SYMBOL_SPACED)) {
@@ -3960,7 +4176,10 @@ int btle_b200_rx_ber_run(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg, size_t 
   const long long q = kChunkSamples / g;                     // packets of the smallest batch: lcm(S, 8192) / S
   size_t free_b = 0, total_b = 0;
   BTLE_CUDA(ctx, cudaMemGetInfo(&free_b, &total_b));
-  const size_t per_chunk = kChunkInt8 + BTLE_MAX_RECS_PER_CHUNK * sizeof(btle_pkt_rec) + 8 * sizeof(btle_rx_ber_truth);
+  // BTLE_CFG_OFFSET_SEARCH: room for the seven hypotheses' records, which bound the merged ones, and as much scratch
+  const size_t recs_per_chunk = BTLE_MAX_RECS_PER_CHUNK * ((cfg->flags & BTLE_CFG_OFFSET_SEARCH) ? BTLE_OFFSET_SEARCH_HYPS : 1);
+  const size_t per_chunk = kChunkInt8 + recs_per_chunk * sizeof(btle_pkt_rec) * ((cfg->flags & BTLE_CFG_OFFSET_SEARCH) ? 2 : 1) +
+                           8 * sizeof(btle_rx_ber_truth);
   const long long want_chunks = (long long)std::min<size_t>(8192, std::max<size_t>(1, free_b / 2 / per_chunk));
   const long long B = std::max(1ll, want_chunks * kChunkSamples / (q * S)) * q;
   const size_t max_b = std::min<size_t>(n_packets, (size_t)B);
@@ -3971,7 +4190,7 @@ int btle_b200_rx_ber_run(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg, size_t 
   const bool sym = (cfg->flags & BTLE_CFG_SYMBOL_SPACED) != 0, lp = (cfg->flags & BTLE_CFG_LOWPASS) != 0;
   constexpr size_t kSymLead = 16;                            // keeps the capture 16-byte aligned
   const size_t lead = sym ? kSymLead : 0, look = BTLE_LOOKAHEAD_INT8 + (lp ? 6 : sym ? 4 : 0);
-  const size_t max_int8 = (size_t)max_chunks * kChunkInt8 + look, max_recs = (size_t)max_chunks * BTLE_MAX_RECS_PER_CHUNK;
+  const size_t max_int8 = (size_t)max_chunks * kChunkInt8 + look, max_recs = (size_t)max_chunks * recs_per_chunk;
   const size_t prev_at = (lead + max_int8 + 15) & ~size_t(15);
   if (ctx->d_iq.reserve(ctx, sym ? prev_at + 2 * (size_t)S : max_int8) || ctx->d_out.reserve(ctx, max_recs) ||
       ctx->d_dir.reserve(ctx, (size_t)(max_chunks + kSpanChunks - 1) / kSpanChunks * kSpanChunks))   // >= units of any batch
@@ -4006,7 +4225,7 @@ int btle_b200_rx_ber_run(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg, size_t 
     }
     rc = launch_rx_ber_synth(ctx, *cfg, done, n_packets, (long long)(n_int8 / 2), (long long)n, d_cap, d_truth, st);
     if (rc) return rc;
-    const size_t cap = (size_t)chunks * BTLE_MAX_RECS_PER_CHUNK, units = btle_b200_rx_units(ctx, 1, n_int8);
+    const size_t cap = (size_t)chunks * recs_per_chunk, units = btle_b200_rx_units(ctx, 1, n_int8);
     rc = launch_rx(ctx, d_cap, 1, n_int8, n_int8, &scfg, nullptr, 1, nullptr, ctx->d_out, cap, ctx->d_count, ctx->d_dir, st, (long long)lead);
     if (rc) return rc;
     rc = launch_rx_ber_score(ctx, d_truth, n, ctx->d_out, cap, ctx->d_dir, units, d_res, st);

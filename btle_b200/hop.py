@@ -266,7 +266,7 @@ def follow_connections(rx, captures: np.ndarray, max_events: int = 10000, discov
 
 
 def decode_connections(rx, captures: np.ndarray, discover: bool = True, offset_hz=None, symbol_spaced: bool = False,
-                       centre_hits: bool = False, correct: bool = False, lowpass: bool = False):
+                       centre_hits: bool = False, correct: bool = False, lowpass: bool = False, offset_search: bool = False):
     """Every known connection's data-channel traffic, decoded without following it.  captures: int8 [40, n_int8] as in
     follow_connections(); `rx` needs rx_batch, rx_multi and, with discover=True, discover (a BtleRx).
     The connections are the CONNECT_REQ ones (tracked or not) plus, with discover=True, the discover_connections() ones
@@ -281,7 +281,9 @@ def decode_connections(rx, captures: np.ndarray, discover: bool = True, offset_h
     those calls carries BTLE_CFG_CENTRE_HITS (each hit centred on its run of matching sample phases); correct: every
     receive cfg of those calls carries BTLE_CFG_CORRECT (one-bit and adjacent-pair errors corrected from the CRC
     syndrome); lowpass: every receive cfg of those calls carries BTLE_CFG_LOWPASS (the symbol-spaced bits of [1, 2, 1]
-    filtered samples; only with symbol_spaced); discovery keeps its own rule.  Returns (adv_records, connections)."""
+    filtered samples; only with symbol_spaced); offset_search: every receive cfg of those calls carries BTLE_CFG_OFFSET_SEARCH
+    (seven carrier-offset hypotheses per capture, merged per packet); discovery keeps its own rule.  Returns (adv_records,
+    connections)."""
     from ._native import MAX_CFGS_PER_CAPTURE
     captures = np.ascontiguousarray(captures, dtype=np.int8)
     assert captures.shape[0] == 40
@@ -290,7 +292,7 @@ def decode_connections(rx, captures: np.ndarray, discover: bool = True, offset_h
     adv_kw = {} if off is None else {"offset_hz": off[37:40]}
     data_kw = {} if off is None else {"offset_hz": off[0:37]}
     adv = rx.rx_batch(captures[37:40], make_cfgs(3, channel=[37, 38, 39], symbol_spaced=symbol_spaced, centre_hits=centre_hits,
-                                                correct=correct, lowpass=lowpass),
+                                                correct=correct, lowpass=lowpass, offset_search=offset_search),
                       **adv_kw).copy()
     adv["stream"] += 37
     conns = []
@@ -310,7 +312,7 @@ def decode_connections(rx, captures: np.ndarray, discover: bool = True, offset_h
         # cfg j = channel * k + i: connection i on data channel j // k (the cfgs of one capture are adjacent)
         cfgs = make_cfgs(37 * k, channel=np.repeat(np.arange(37), k), access_addr=[c["access_addr"] for c in batch] * 37,
                          crc_init=[c["crc_init"] for c in batch] * 37, symbol_spaced=symbol_spaced, centre_hits=centre_hits,
-                         correct=correct, lowpass=lowpass)
+                         correct=correct, lowpass=lowpass, offset_search=offset_search)
         rec = rx.rx_multi(captures[0:37], cfgs, np.repeat(np.arange(37, dtype=np.int32), k), **data_kw)
         owner = rec["stream"] % k
         t = rec["chunk"].astype(np.int64) * 8192 + rec["n0"]
@@ -462,17 +464,18 @@ class ConnectionMonitor:
     starts again, where discover_connections() would continue it).  offset_hz (a scalar or one per capture): the
     session's carrier-offset correction of each capture (RxStreams.set_offset), from the first set on.  symbol_spaced:
     the connection cfgs carry BTLE_CFG_SYMBOL_SPACED; the session must have been opened with cfgs that carry it (a
-    session has one discriminator mode).  lowpass: likewise BTLE_CFG_LOWPASS.  centre_hits / correct: the connection cfgs
+    session has one discriminator mode).  lowpass, offset_search: likewise BTLE_CFG_LOWPASS, BTLE_CFG_OFFSET_SEARCH.  centre_hits / correct: the connection cfgs
     carry BTLE_CFG_CENTRE_HITS / BTLE_CFG_CORRECT (per cfg, so the session's own cfgs may carry them or not).  Discovery
     keeps its own rule."""
 
     N_CAPTURES = 40
 
     def __init__(self, session, min_events: int = 4, idle_s: float | None = None, discover: bool = True, group_s: float = 8.0,
-                 offset_hz=None, symbol_spaced: bool = False, centre_hits: bool = False, correct: bool = False, lowpass: bool = False):
+                 offset_hz=None, symbol_spaced: bool = False, centre_hits: bool = False, correct: bool = False, lowpass: bool = False,
+                 offset_search: bool = False):
         self.session, self.min_events, self.idle_s, self.group_s = session, int(min_events), idle_s, group_s
         self._symbol_spaced, self._centre_hits, self._correct = bool(symbol_spaced), bool(centre_hits), bool(correct)
-        self._lowpass = bool(lowpass)
+        self._lowpass, self._offset_search = bool(lowpass), bool(offset_search)
         if offset_hz is not None:
             for c, hz in enumerate(np.broadcast_to(np.asarray(offset_hz, dtype=np.float32), (self.N_CAPTURES,))):
                 session.set_offset(c, float(hz))
@@ -539,7 +542,7 @@ class ConnectionMonitor:
         for ch in range(37):
             j, _ = s.add_cfg(ch, frm, channel=ch, access_addr=c["access_addr"], access_mask=0xFFFFFFFF, crc_init=c["crc_init"], raw=0, rssi=0,
                            symbol_spaced=self._symbol_spaced, centre_hits=self._centre_hits, correct=self._correct,
-                           lowpass=self._lowpass)
+                           lowpass=self._lowpass, offset_search=self._offset_search)
             c["_cfgs"].append(j)
             self._owner[j] = c
         return 37

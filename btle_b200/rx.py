@@ -21,7 +21,7 @@ DEFAULT_CHANNEL = 37                 # btle_rx.c:230
 
 def make_cfgs(n_streams=1, channel=DEFAULT_CHANNEL, access_addr=DEFAULT_ACCESS_ADDR, access_mask=0xFFFFFFFF,
               crc_init=DEFAULT_CRC_INIT, raw=0, rssi=0, recover=0, symbol_spaced=0, centre_hits=0, correct=0,
-              lowpass=0) -> np.ndarray:
+              lowpass=0, offset_search=0) -> np.ndarray:
     """btle_stream_cfg array; every argument may be a scalar or a per-stream sequence.  rssi holds the BTLE_CFG_* flag
     bits; recover (true) adds BTLE_CFG_RECOVER: counted packets that fail the CRC are demodulated again; symbol_spaced
     (true) adds BTLE_CFG_SYMBOL_SPACED: the discriminator compares samples a symbol apart (all cfgs of one call must
@@ -29,7 +29,8 @@ def make_cfgs(n_streams=1, channel=DEFAULT_CHANNEL, access_addr=DEFAULT_ACCESS_A
     centre of its run of matching sample phases (per cfg); correct (true) adds BTLE_CFG_CORRECT: a one-bit or
     adjacent-pair error of a counted packet that fails the CRC is corrected from its syndrome (per cfg); lowpass (true)
     adds BTLE_CFG_LOWPASS: the symbol-spaced bits read [1, 2, 1]-filtered samples (only with symbol_spaced; all cfgs of
-    one call must agree on it)."""
+    one call must agree on it); offset_search (true) adds BTLE_CFG_OFFSET_SEARCH: each capture is decoded at seven carrier
+    offsets around its own and the packets merged (all cfgs of one call must agree on it; not with raw)."""
     c = np.zeros(n_streams, dtype=CFG_DTYPE)
     c["channel"], c["access_addr"], c["access_mask"] = channel, access_addr, access_mask
     c["crc_init"], c["raw"], c["rssi"] = crc_init, raw, rssi
@@ -38,15 +39,16 @@ def make_cfgs(n_streams=1, channel=DEFAULT_CHANNEL, access_addr=DEFAULT_ACCESS_A
     c["rssi"] |= np.where(np.asarray(centre_hits) != 0, _native.CFG_CENTRE_HITS, 0).astype(np.int32)
     c["rssi"] |= np.where(np.asarray(correct) != 0, _native.CFG_CORRECT, 0).astype(np.int32)
     c["rssi"] |= np.where(np.asarray(lowpass) != 0, _native.CFG_LOWPASS, 0).astype(np.int32)
+    c["rssi"] |= np.where(np.asarray(offset_search) != 0, _native.CFG_OFFSET_SEARCH, 0).astype(np.int32)
     return c
 
 
 def _with_fields(c: np.ndarray, cfg: dict) -> np.ndarray:
     """c (a btle_stream_cfg array) with the given make_cfgs fields changed; recover / symbol_spaced / centre_hits / correct
-    / lowpass set or clear BTLE_CFG_RECOVER / BTLE_CFG_SYMBOL_SPACED / BTLE_CFG_CENTRE_HITS / BTLE_CFG_CORRECT /
-    BTLE_CFG_LOWPASS"""
+    / lowpass / offset_search set or clear BTLE_CFG_RECOVER / BTLE_CFG_SYMBOL_SPACED / BTLE_CFG_CENTRE_HITS / BTLE_CFG_CORRECT /
+    BTLE_CFG_LOWPASS / BTLE_CFG_OFFSET_SEARCH"""
     flag = {"recover": _native.CFG_RECOVER, "symbol_spaced": _native.CFG_SYMBOL_SPACED, "centre_hits": _native.CFG_CENTRE_HITS,
-            "correct": _native.CFG_CORRECT, "lowpass": _native.CFG_LOWPASS}
+            "correct": _native.CFG_CORRECT, "lowpass": _native.CFG_LOWPASS, "offset_search": _native.CFG_OFFSET_SEARCH}
     for k, v in cfg.items():
         if k in flag:
             c["rssi"] = (c["rssi"] & ~flag[k]) | (flag[k] if v else 0)
@@ -194,7 +196,8 @@ class BtleRx:
         dev = torch.device("cuda", self.device)
         st = torch.cuda.current_stream(dev)
         d_iq = torch.from_numpy(np.pad(iq, ((0, 0), (0, -n % 16)))).to(dev)[:, :n]
-        cap = (n // 16384) * 123 + 16                                   # BTLE_MAX_RECS_PER_CHUNK per chunk: never an overflow
+        # BTLE_MAX_RECS_PER_CHUNK per chunk (per hypothesis with offset_search): never an overflow
+        cap = (n // 16384) * 123 * (7 if cfg.get("offset_search") else 1) + 16
         d_out = torch.empty(cap * 64, dtype=torch.uint8, device=dev)
         d_dir = torch.empty(max(self.units(1, n), 1) * 8, dtype=torch.uint8, device=dev)
         self.rx_device_dir(d_iq, make_cfgs(1, **cfg), d_out, None, d_dir, st.cuda_stream)

@@ -73,7 +73,8 @@ typedef struct {
                             BTLE_CFG_SYMBOL_SPACED 16: the symbol-spaced discriminator (below);
                             BTLE_CFG_CENTRE_HITS 64: each hit centred on its run of matching phases (below);
                             BTLE_CFG_CORRECT 256: one-bit and adjacent-pair errors corrected by the CRC (below);
-                            BTLE_CFG_LOWPASS 512: a [1, 2, 1] low-pass in front of the symbol-spaced bits (below)  */
+                            BTLE_CFG_LOWPASS 512: a [1, 2, 1] low-pass in front of the symbol-spaced bits (below);
+                            BTLE_CFG_OFFSET_SEARCH 1024: a bank of seven carrier-offset hypotheses (below)  */
 } btle_stream_cfg;
 #define BTLE_CFG_RSSI 1
 #define BTLE_CFG_REPORT_REJECTED 2
@@ -183,6 +184,43 @@ typedef struct {
  * Q[s] Q[s+4]) > 0.  mag_sum (RSSI) reads the raw samples and is unaffected.  In rx_multi the cfgs of one capture share
  * its offset.  Values that are not finite, or with |offset_hz| > BTLE_MAX_OFFSET_HZ, are BTLE_EINVAL. */
 #define BTLE_MAX_OFFSET_HZ 500000
+/* BTLE_CFG_OFFSET_SEARCH: opt-in bank of carrier-offset hypotheses, so that transmitters at different offsets in one capture
+ * are all received (every advertiser transmits from its own crystal, up to +-150 kHz off).  Not part of the reference's
+ * receiver; without it every record is unchanged, bit for bit.  f_c is capture c's offset (offset_hz[c] of the *_offset
+ * entry points and sessions, else 0).
+ *   1. hypotheses  h = 0..6 decodes capture c at f_c + delta_h, delta = 0, -50, +50, -100, +100, -150, +150 kHz in that order
+ *                  (BTLE_OFFSET_SEARCH_HZ), with every cfg of c, in the launch's discriminator mode, by the rotated kernel's
+ *                  definition above.  Hypothesis 0 is the call without the flag at the same offsets.  The 50-kHz step
+ *                  leaves at most 25 kHz of residual offset inside +-150 kHz.
+ *   2. merge       per (cfg j, chunk k), independently of every other chunk: B starts as hypothesis 0's records of (j, k).
+ *                  Then for h = 1..6 in order, for each of h's records r of (j, k) in n0 order that is counted with
+ *                  crc_bad == 0 (CRC-ok as decoded or after BTLE_CFG_RECOVER / BTLE_CFG_CORRECT): if B holds a counted
+ *                  CRC-ok record with |n0 - r.n0| <= 8 (two symbols), r is dropped; otherwise every CRC-failed or rejected
+ *                  record of B with |n0 - r.n0| <= 8 is removed and r is inserted with flags |= BTLE_REC_OFFSET_SEARCH.
+ *                  CRC-failed and rejected records of h >= 1 are never added.  The result is in (j, chunk, n0) order,
+ *                  stream = j, and every field of a kept hypothesis-0 record is unchanged.
+ *   3. so          the call returns every CRC-ok record of the call without the flag, unchanged; every other record it
+ *                  returns carries BTLE_REC_OFFSET_SEARCH and crc_bad 0; CRC-failed and rejected records can only
+ *                  disappear.  Duplicates across a chunk boundary (one packet found in chunk k by one hypothesis and in
+ *                  k + 1 by another) are not merged.  btle_b200_rec_offset estimates a BTLE_REC_OFFSET_SEARCH record's
+ *                  offset (it reads the raw samples, so it returns the packet's full offset, not the residual).
+ *   4. mode        one mode per launch and per session, as BTLE_CFG_SYMBOL_SPACED: mixed cfgs in one launch, a session set_cfg
+ *                  or add_cfg with the other value, the flag with raw (raw records have no CRC verdict) and |f_c| + 150 kHz >
+ *                  BTLE_MAX_OFFSET_HZ are BTLE_EINVAL with last_error set.  btle_rx_ber_cfg.flags accepts it.
+ *   5. capacity    the directory has the entries and layout of the call without the flag (btle_b200_rx_units and
+ *                  btle_b200_rx_multi_units are unchanged).  The seven hypotheses are decoded into context-owned scratch of
+ *                  `cap` records.  When they find more than that (T > cap), nothing is merged: *d_count / *n_out is T (the
+ *                  merged count is never larger), the directory entries sum to T and their blocks hold no records, and the
+ *                  host entry points return BTLE_EOVERFLOW.  A second call with cap >= T returns the whole result.  Flagged
+ *                  launches of one context on different CUDA streams are ordered one after the other through the scratch. */
+#define BTLE_CFG_OFFSET_SEARCH 1024
+#define BTLE_OFFSET_SEARCH_HYPS 7
+#define BTLE_OFFSET_SEARCH_HZ {0.0f, -50e3f, 50e3f, -100e3f, 100e3f, -150e3f, 150e3f}
+#define BTLE_OFFSET_SEARCH_SPAN_HZ 150000
+/* Records one chunk of one cfg can return with BTLE_CFG_OFFSET_SEARCH: hypothesis 0 contributes at most
+ * BTLE_MAX_RECS_PER_CHUNK, each of hypotheses 1..6 inserts at most its counted packets (BTLE_MAX_PKTS_PER_CHUNK), and no
+ * other step adds a record: 123 + 6 * 51 = 429. */
+#define BTLE_MAX_MERGED_RECS_PER_CHUNK (BTLE_MAX_RECS_PER_CHUNK + (BTLE_OFFSET_SEARCH_HYPS - 1) * BTLE_MAX_PKTS_PER_CHUNK)
 
 /* One packet the reference would have counted (pkt_count++, btle_rx.c:2274/:2319). 64 bytes. */
 typedef struct {
@@ -196,7 +234,8 @@ typedef struct {
   uint8_t flags;         /* bit0 raw, bit1 advertising channel, bit2 BTLE_REC_REJECTED: not a packet the
                             reference counts — only bytes[0..1] (the header) are valid, n_bytes = 2;
                             bit3 BTLE_REC_RECOVERED: bytes from alternative q = bits 4..5 (BTLE_CFG_RECOVER);
-                            bit6 BTLE_REC_CORRECTED: bytes corrected by the CRC syndrome (BTLE_CFG_CORRECT) */
+                            bit6 BTLE_REC_CORRECTED: bytes corrected by the CRC syndrome (BTLE_CFG_CORRECT);
+                            bit7 BTLE_REC_OFFSET_SEARCH: found by offset hypothesis 1..6 (BTLE_CFG_OFFSET_SEARCH) */
   uint32_t access_addr;
   uint16_t mag_sum;      /* sum |I|+|Q| over the 128 AA samples if cfg.rssi, else 0           */
   uint8_t bytes[42];     /* == reference tmp_byte[] (btle_rx.c:1485): dewhitened header,
@@ -207,6 +246,7 @@ typedef struct {
 #define BTLE_REC_RECOVERED 8
 #define BTLE_REC_RECOVERED_Q(flags) (((flags) >> 4) & 3)
 #define BTLE_REC_CORRECTED 64
+#define BTLE_REC_OFFSET_SEARCH 128
 
 typedef struct btle_b200_ctx btle_b200_ctx;
 
@@ -623,8 +663,9 @@ typedef struct {
   int32_t channel;         /* 0..39                                                                                 */
   uint32_t access_addr;
   uint32_t crc_init;       /* as -k                                                                                 */
-  uint32_t flags;          /* any of BTLE_CFG_RECOVER, BTLE_CFG_SYMBOL_SPACED, BTLE_CFG_CENTRE_HITS, BTLE_CFG_CORRECT
-                              and BTLE_CFG_LOWPASS (given to the receiver); any other bit: BTLE_EINVAL               */
+  uint32_t flags;          /* any of BTLE_CFG_RECOVER, BTLE_CFG_SYMBOL_SPACED, BTLE_CFG_CENTRE_HITS, BTLE_CFG_CORRECT,
+                              BTLE_CFG_LOWPASS and BTLE_CFG_OFFSET_SEARCH (given to the receiver); any other bit:
+                              BTLE_EINVAL                                                                             */
   uint32_t reserved;       /* 0                                                                                     */
 } btle_rx_ber_cfg;         /* 48 bytes */
 typedef struct {
@@ -653,7 +694,7 @@ typedef struct {
  * BTLE_CFG_LOWPASS 3 and 3).
  * BTLE_EINVAL with btle_b200_last_error() for: snr_db, ppm or cfo_hz NaN or infinite, |ppm| >= 1e6, amplitude outside
  * 1..127, slot_samples below L or above BTLE_RX_BER_MAX_SLOT, channel > 39, a flags bit other than BTLE_CFG_RECOVER,
- * BTLE_CFG_SYMBOL_SPACED, BTLE_CFG_CENTRE_HITS, BTLE_CFG_CORRECT and BTLE_CFG_LOWPASS, BTLE_CFG_LOWPASS without
+ * BTLE_CFG_SYMBOL_SPACED, BTLE_CFG_CENTRE_HITS, BTLE_CFG_CORRECT, BTLE_CFG_LOWPASS and BTLE_CFG_OFFSET_SEARCH, BTLE_CFG_LOWPASS without
  * BTLE_CFG_SYMBOL_SPACED;
  * the context stays usable. */
 int btle_b200_rx_ber_run(btle_b200_ctx *ctx, const btle_rx_ber_cfg *cfg, size_t n_packets, btle_rx_ber_result *out);
