@@ -51,6 +51,14 @@ SPS8_REC_DTYPE = np.dtype([("sample", "<i8"), ("window", "<i8"), ("rx", MODEL_RE
 CAND_DTYPE = np.dtype([("sample", "<i8"), ("stream", "<i4"), ("access_addr", "<u4"), ("crc_init", "<u4"), ("channel", "u1"),
                        ("header", "u1", 2), ("reserved", "u1", 9)])
 assert CAND_DTYPE.itemsize == 32
+# btle_coded_rec, 304 bytes: one LE Coded PHY packet (btle_b200_rx_coded)
+CODED_MAX_BYTES = 260
+CODED_REC_DTYPE = np.dtype([("sample", "<i8"), ("stream", "<i4"), ("access_addr", "<u4"), ("channel", "u1"), ("s", "u1"), ("ci", "u1"),
+                            ("crc_bad", "u1"), ("flags", "u1"), ("reserved0", "u1"), ("n_bytes", "<u2"), ("dist", "<i4"), ("metric", "<i4"),
+                            ("mag_sum", "<u4"), ("bytes", "u1", CODED_MAX_BYTES), ("reserved", "u1", 8)])
+assert CODED_REC_DTYPE.itemsize == 304
+CODED_MAX_DIST = 96                           # BTLE_CODED_MAX_DIST
+CODED_CI_RESERVED, CODED_TRUNCATED = 1, 2     # btle_coded_rec.flags bits
 assert REC_DTYPE.itemsize == 64 and CFG_DTYPE.itemsize == 24 and MODEL_REC_DTYPE.itemsize == 80 and SPS8_REC_DTYPE.itemsize == 96
 
 EXPORTS = [
@@ -73,7 +81,7 @@ EXPORTS = [
     "btle_b200_streams_add_cfg", "btle_b200_streams_remove_cfg", "btle_b200_streams_resident", "btle_b200_streams_set_discover",
     "btle_b200_streams_take_cands", "btle_b200_rx_batch_offset", "btle_b200_rx_device_dir_offset", "btle_b200_rx_multi_offset",
     "btle_b200_rx_multi_device_dir_offset", "btle_b200_rec_offset_device", "btle_b200_rec_offset",
-    "btle_b200_streams_set_offset", "btle_b200_stream_set_offset",
+    "btle_b200_streams_set_offset", "btle_b200_stream_set_offset", "btle_b200_rx_coded", "btle_b200_rx_coded_device",
 ]
 MAX_CFGS_PER_CAPTURE = 8       # BTLE_MAX_CFGS_PER_CAPTURE
 CFG_RSSI, CFG_REPORT_REJECTED, CFG_RECOVER = 1, 2, 4      # btle_stream_cfg.rssi flag bits (BTLE_CFG_*)
@@ -191,6 +199,8 @@ def load():
     L.btle_b200_rec_offset.argtypes = [vp, vp, sz, sz, sz, vp, sz, vp]
     L.btle_b200_streams_set_offset.argtypes = [vp, sz, ctypes.c_float]
     L.btle_b200_stream_set_offset.argtypes = [vp, ctypes.c_float]
+    L.btle_b200_rx_coded.argtypes = [vp, vp, sz, sz, sz, vp, vp, vp, sz, ctypes.POINTER(sz)]
+    L.btle_b200_rx_coded_device.argtypes = [vp, vp, sz, sz, sz, vp, vp, vp, sz, vp, vp]
     _lib = L
     return L
 

@@ -1505,6 +1505,398 @@ discover_kernel(const int8_t *__restrict__ iq, long long stride, long long n_int
   }
 }
 
+// ---- LE Coded PHY receiver (btle_b200_rx_coded*, include/btle_b200.h "LE Coded PHY") ---------------------------------
+// coded_search_kernel: one CTA = kCodedGroups groups of window starts (128 samples each) of one capture.  D(n0) reads the
+// phase words of the 3 groups in front of n0's group and 8 behind it, and the hit rule reads D 8 samples to each side, so
+// the CTA packs kCodedThreads groups (G0 - 4 .. G0 + 123) and computes D for kCodedDGroups (G0 - 1 .. G0 + 115):
+//   load   cp.async of the groups' IQ and one more row on each side (the low-pass walk reads two words past its group)
+//          into rows of kCodedPitch words; bytes outside the capture read as 0
+//   pack   lane p turns packed group p into its four phase words (dbits_group_lowpass, rotated by (C4, S4))
+//   D      lane dg computes D for the 128 window starts of its group, 11 words of XOR + POPC each (after 7 words a count
+//          above BTLE_CODED_MAX_DIST is stored as 97: every comparison with a hit, D <= 96, comes out the same), into the
+//          freed IQ rows (255 where D is not defined)
+//   hits   lane dg of the tile's own groups applies the local-minimum rule; each hit takes one atomic on the counter and
+//          leaves sample, stream and D in its record slot for coded_decode_kernel
+constexpr int kCodedThreads = 128;
+constexpr int kCodedRows = kCodedThreads + 2;                              // staged IQ rows
+constexpr int kCodedPitch = 68;                                            // words per staged row (64 + 4 of padding)
+constexpr int kCodedDGroups = kCodedThreads - 11;                          // groups whose D is computed (117)
+constexpr int kCodedGroups = kCodedDGroups - 2;                            // window-start groups per CTA (115)
+constexpr int kCodedDPitch = 33;                                           // words of one group's 128 D bytes (+1 of padding)
+constexpr int kCodedPreamble = 80, kCodedBlock1 = 296;                 // symbols of the preamble and of FEC block 1
+constexpr int kCodedMaxSteps = 16 + 8 * 255 + 27;                          // info bits of the longest block 2 (2083)
+constexpr int kCodedNeg = -(1 << 29);                                      // metric of a state not yet reachable
+constexpr size_t kCodedSmem = ((size_t)kCodedRows * kCodedPitch + 4 * (kCodedThreads + 1) + 12) * sizeof(uint32_t);
+static_assert(kCodedDGroups * kCodedDPitch <= kCodedRows * kCodedPitch, "D rows must fit in the freed IQ rows");
+static_assert(sizeof(btle_coded_rec) == 304 && sizeof(btle_coded_rec) % 16 == 0, "coded record must be 304 bytes");
+
+// coded bits (a0, a1) of input bit b from state st = b[t-1] | b[t-2] << 1 | b[t-3] << 2 (G0 = 1 + x + x^2 + x^3, G1 = 1 + x^2 + x^3)
+__host__ __device__ __forceinline__ void coded_fec(int b, int st, int &a0, int &a1) {
+  const int s0 = st & 1, s1 = (st >> 1) & 1, s2 = (st >> 2) & 1;
+  a0 = b ^ s0 ^ s1 ^ s2;
+  a1 = b ^ s1 ^ s2;
+}
+// P of an access address, 336 bits LSB first: the preamble, then the S=8 coding of the 32 AA bits from state 0
+__device__ void coded_pattern(uint32_t aa, uint32_t *P /*11*/) {
+  for (int k = 0; k < 11; ++k) P[k] = 0u;
+  for (int q = 0; q < kCodedPreamble; ++q)
+    if ((q & 7) >= 2 && (q & 7) <= 5) P[q >> 5] |= 1u << (q & 31);
+  int st = 0, q = kCodedPreamble;
+  for (int t = 0; t < 32; ++t) {
+    const int b = (aa >> t) & 1;
+    int a[2];
+    coded_fec(b, st, a[0], a[1]);
+    st = b | ((st & 3) << 1);
+    for (int c = 0; c < 2; ++c, q += 4)                                     // 1 -> 1,1,0,0 and 0 -> 0,0,1,1
+      P[q >> 5] |= (a[c] ? 0x3u : 0xCu) << (q & 31);                        // q is a multiple of 4: never straddles a word
+  }
+}
+
+__global__ void __launch_bounds__(kCodedThreads)
+coded_search_kernel(const int8_t *__restrict__ iq, long long stride, long long n_int8, long long tiles_per_stream,
+                    const StreamParams *__restrict__ params, const int4 *__restrict__ rot, btle_coded_rec *__restrict__ out,
+                    unsigned cap, unsigned *__restrict__ count) {
+  extern __shared__ __align__(16) uint32_t coded_smem[];
+  uint4 *pdw = reinterpret_cast<uint4 *>(coded_smem + kCodedRows * kCodedPitch);   // phase words of packed group p (+1 zero entry)
+  uint32_t *P = coded_smem + kCodedRows * kCodedPitch + 4 * (kCodedThreads + 1);
+  const long long stream = blockIdx.x / tiles_per_stream, tile = blockIdx.x - stream * tiles_per_stream;
+  const int8_t *cap_base = iq + stream * stride;
+  const long long G0 = tile * kCodedGroups;
+  const long long row0 = (G0 - 5) * 256;                                   // first byte of staged row 0
+  const bool interior = row0 >= 0 && row0 + kCodedRows * 256ll <= n_int8;
+  for (int k = threadIdx.x; k < kCodedRows * 16; k += kCodedThreads) {
+    uint32_t *dst = coded_smem + (k >> 4) * kCodedPitch + 4 * (k & 15);
+    const long long b = row0 + 16ll * k;
+    if (interior || (b >= 0 && b + 16 <= n_int8)) {
+      cp_async16(dst, cap_base + b);
+    } else {
+      uint32_t v[4] = {0u, 0u, 0u, 0u};
+      for (int q = 0; q < 16; ++q)
+        if (b + q >= 0 && b + q < n_int8) v[q >> 2] |= (uint32_t)(uint8_t)cap_base[b + q] << (8 * (q & 3));
+      *reinterpret_cast<uint4 *>(dst) = make_uint4(v[0], v[1], v[2], v[3]);
+    }
+  }
+  if (threadIdx.x == 0) {
+    coded_pattern(__ldg(&params[stream].aa), P);
+    pdw[kCodedThreads] = make_uint4(0u, 0u, 0u, 0u);
+  }
+  asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
+  __syncthreads();
+  {
+    const int4 r = __ldg(&rot[stream]);
+    const uint32_t *row = coded_smem + (threadIdx.x + 1) * kCodedPitch;
+    auto word = [&](int k) -> uint32_t {
+      return k < 0 ? row[k - kCodedPitch + 64] : k >= 64 ? row[kCodedPitch + k - 64] : row[k];
+    };
+    uint32_t acc[4] = {0u, 0u, 0u, 0u};
+    dbits_group_lowpass<true>(word, r.z, r.w, acc);
+    pdw[threadIdx.x] = make_uint4(acc[0], acc[1], acc[2], acc[3]);
+  }
+  __syncthreads();                                                          // the IQ rows are free: D goes there
+  uint8_t *Db = reinterpret_cast<uint8_t *>(coded_smem);
+  const long long n_samples = n_int8 / 2, n0_hi = n_samples - 1024;       // D(n0) defined for 323 <= n0 <= n0_hi
+  const int dg = threadIdx.x;
+  if (dg < kCodedDGroups) {
+    const long long g = G0 - 1 + dg;
+    uint32_t p[11];
+#pragma unroll
+    for (int k = 0; k < 11; ++k) p[k] = P[k];
+    p[10] &= 0xFFFFu;
+#pragma unroll
+    for (int ph = 0; ph < 4; ++ph) {
+#pragma unroll
+      for (int half = 0; half < 2; ++half) {
+        uint32_t w[12];
+#pragma unroll
+        for (int k = 0; k < 12; ++k) {
+          const uint4 v = pdw[dg + half + k];
+          w[k] = ph == 0 ? v.x : ph == 1 ? v.y : ph == 2 ? v.z : v.w;
+        }
+        for (int ii = 0; ii < 16; ++ii) {
+          const int i = 16 * half + ii;
+          const uint32_t sh = half ? ii : 16 + ii;                         // symbol m - 80 of window start m = 32 g + i
+          const long long n0 = 128 * g + 4 * i + ph;
+          int d = 255;
+          if (n0 >= 323 && n0 <= n0_hi) {
+            d = 0;
+#pragma unroll
+            for (int k = 0; k < 7; ++k) d += __popc(funnel_r(w[k], w[k + 1], sh) ^ p[k]);
+            if (d > BTLE_CODED_MAX_DIST) {
+              d = BTLE_CODED_MAX_DIST + 1;
+            } else {
+#pragma unroll
+              for (int k = 7; k < 10; ++k) d += __popc(funnel_r(w[k], w[k + 1], sh) ^ p[k]);
+              d += __popc((funnel_r(w[10], w[11], sh) & 0xFFFFu) ^ p[10]);
+              d = min(d, BTLE_CODED_MAX_DIST + 1);
+            }
+          }
+          Db[4 * (dg * kCodedDPitch + i) + ph] = (uint8_t)d;
+        }
+      }
+    }
+  }
+  __syncthreads();
+  if (dg < 1 || dg > kCodedGroups) return;                                 // the halo groups only lend their D
+  const long long g = G0 - 1 + dg;
+  if (128 * g > n0_hi || 128 * g + 127 < 323) return;
+  auto d_at = [&](int idx) -> int {                                         // D of sample (G0 - 1) * 128 + idx
+    return Db[4 * ((idx >> 7) * kCodedDPitch + ((idx & 127) >> 2)) + (idx & 3)];
+  };
+  for (int i = 0; i < 32; ++i) {
+    const uint32_t w4 = reinterpret_cast<const uint32_t *>(Db)[dg * kCodedDPitch + i];
+    uint32_t m = __vcmpleu4(w4, 0x60606060u);                              // bytes <= 96
+    while (m) {
+      const int ph = (__ffs((int)m) - 1) >> 3;
+      m &= ~(0xFFu << (8 * ph));
+      const int idx = 128 * dg + 4 * i + ph, d = (int)((w4 >> (8 * ph)) & 0xFFu);
+      bool hit = true;
+      for (int k = 1; k <= 8; ++k) hit = hit && d < d_at(idx - k) && d <= d_at(idx + k);
+      if (!hit) continue;
+      const unsigned slot = atomicAdd(count, 1u);
+      if (slot < cap) {
+        btle_coded_rec *r = out + slot;
+        r->sample = 128 * g + 4 * i + ph;
+        r->stream = (int32_t)stream;
+        r->dist = d;
+      }
+    }
+  }
+}
+
+// coded_decode_kernel: one warp per hit (a grid-stride loop over the hits counted), warp state in shared memory.  Lanes
+// build the soft values of 32 trellis steps at once from the IQ (coalesced), then the 8 ACS lanes (state = lane & 7)
+// run those steps with two shuffles each; each step's 8 decisions are one byte of the warp's survivor rows.  The header
+// pass is the first 40 steps of the same trellis.  Lane 0 traces back, the lanes pack and dewhiten the bytes, lane 0
+// runs the CRC.
+constexpr int kCodedDecWarps = 4;
+struct CodedWarp {
+  uint8_t surv[kCodedMaxSteps + 13];                                        // decisions of step t: bit s = state s took p | 4
+  uint32_t bits[(kCodedMaxSteps + 31) / 32];                                // traced-back info bits
+  int32_t L[64];                                                            // soft values of 32 steps
+  uint32_t wseq[4];                                                         // the channel's 127 whitening bits
+  uint8_t body[BTLE_CODED_MAX_BYTES + 4];
+};
+struct CodedIq {
+  const int8_t *base;
+  long long n_samples;
+  int c4, s4;
+  __device__ __forceinline__ void x(long long m, int &i, int &q) const {
+    if (m < 0 || m >= n_samples) { i = q = 0; return; }
+    const uint16_t w = __ldg(reinterpret_cast<const uint16_t *>(base) + m);
+    i = (int)(int8_t)(w & 0xFFu);
+    q = (int)(int8_t)(w >> 8);
+  }
+  __device__ __forceinline__ void f(long long m, int &i, int &q) const {     // F[m] = (x[m-1] + 2 x[m] + x[m+1]) >> 2
+    int i0, q0, i1, q1, i2, q2;
+    x(m - 1, i0, q0); x(m, i1, q1); x(m + 1, i2, q2);
+    i = (i0 + 2 * i1 + i2) >> 2;
+    q = (q0 + 2 * q1 + q2) >> 2;
+  }
+  __device__ __forceinline__ int y(long long n) const {                     // clamp(v[n] >> 22, -127, 127)
+    int ia, qa, ib, qb;
+    f(n - 2, ia, qa); f(n + 2, ib, qb);
+    const int v = c4 * (ia * qb - ib * qa) - s4 * (ia * ib + qa * qb);
+    return max(-127, min(127, v >> 22));
+  }
+};
+__device__ __forceinline__ int warp_sum(int v) {
+#pragma unroll
+  for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xFFFFFFFFu, v, o);
+  return v;
+}
+// steps [from, to) of the trellis (lane & 7 holds the metric of its state)
+__device__ __forceinline__ int coded_acs(CodedWarp &W, const CodedIq &X, long long n0, int per, int from, int to, int m) {
+  const int lane = threadIdx.x & 31, ns = lane & 7, b = ns & 1, p0 = ns >> 1, p1 = p0 | 4;
+  int a00, a01, a10, a11;
+  coded_fec(b, p0, a00, a01);
+  coded_fec(b, p1, a10, a11);
+  for (int t0 = from; t0 < to; t0 += 32) {
+    const int t = t0 + lane;
+    if (t < to) {
+      int L[2];
+      for (int c = 0; c < 2; ++c) {
+        const long long n = n0 + 4ll * (kCodedBlock1 + (long long)per * (2 * t + c));
+        L[c] = per == 1 ? X.y(n) : X.y(n) + X.y(n + 4) - X.y(n + 8) - X.y(n + 12);
+      }
+      W.L[2 * lane] = L[0];
+      W.L[2 * lane + 1] = L[1];
+    }
+    __syncwarp();
+    const int nt = min(32, to - t0);
+    for (int tt = 0; tt < nt; ++tt) {
+      const int L0 = W.L[2 * tt], L1 = W.L[2 * tt + 1];
+      const int m0 = __shfl_sync(0xFFFFFFFFu, m, p0), m1 = __shfl_sync(0xFFFFFFFFu, m, p1);
+      const int c0 = m0 + (a00 ? L0 : -L0) + (a01 ? L1 : -L1), c1 = m1 + (a10 ? L0 : -L0) + (a11 ? L1 : -L1);
+      const bool d = c1 > c0;
+      m = d ? c1 : c0;
+      const unsigned bal = __ballot_sync(0xFFFFFFFFu, d);
+      if (lane == 0) W.surv[t0 + tt] = (uint8_t)bal;
+    }
+    __syncwarp();
+  }
+  return m;
+}
+__device__ __forceinline__ int coded_wbit(const CodedWarp &W, int k) {
+  k %= 127;
+  return (W.wseq[k >> 5] >> (k & 31)) & 1;
+}
+
+__global__ void __launch_bounds__(32 * kCodedDecWarps)
+coded_decode_kernel(const int8_t *__restrict__ iq, long long stride, long long n_int8, const StreamParams *__restrict__ params,
+                    const int4 *__restrict__ rot, btle_coded_rec *__restrict__ out, unsigned cap, const unsigned *__restrict__ count) {
+  __shared__ CodedWarp warps[kCodedDecWarps];
+  CodedWarp &W = warps[threadIdx.x >> 5];
+  const int lane = threadIdx.x & 31;
+  const unsigned n = min(*count, cap);
+  for (unsigned k = blockIdx.x * kCodedDecWarps + (threadIdx.x >> 5); k < n; k += gridDim.x * kCodedDecWarps) {
+    btle_coded_rec *rec = out + k;
+    const long long n0 = rec->sample;
+    const int stream = rec->stream, dist = rec->dist;
+    __syncwarp();
+    const StreamParams &sp = params[stream];
+    const int4 r = __ldg(&rot[stream]);
+    const CodedIq X{iq + stream * stride, n_int8 / 2, r.z, r.w};
+    const uint32_t aa = __ldg(&sp.aa);
+    const int channel = __ldg(&sp.channel);
+    if (lane == 0) {
+      uint32_t reg = whiten_seed(channel);
+      W.wseq[0] = W.wseq[1] = W.wseq[2] = W.wseq[3] = 0u;
+      for (int q = 0; q < 127; ++q) W.wseq[q >> 5] |= whiten_step(reg) << (q & 31);
+    }
+    uint32_t mag = 0;
+    if (__ldg(&sp.rssi)) {
+      for (int q = lane; q < 1024; q += 32) {
+        int i, qq;
+        X.x(n0 + q, i, qq);
+        mag += (uint32_t)(abs(i) + abs(qq));
+      }
+      mag = (uint32_t)warp_sum((int)mag);
+    }
+    // CI: the 40 symbols j = 256..295 against the coding of (c0, c1, 0, 0, 0) from the state after the access address
+    const int st_aa = (int)(((aa >> 31) & 1u) | (((aa >> 30) & 1u) << 1) | (((aa >> 29) & 1u) << 2));
+    int M[4] = {0, 0, 0, 0};
+    for (int j = lane; j < 40; j += 32) {
+      const int yj = X.y(n0 + 4ll * (256 + j));
+      for (int c = 0; c < 4; ++c) {
+        int st = st_aa, a0 = 0, a1 = 0;
+        for (int t = 0; t <= (j >> 3); ++t) {                               // info bit j / 8 gives coded bits j / 4
+          const int b = t < 2 ? (c >> t) & 1 : 0;
+          coded_fec(b, st, a0, a1);
+          st = b | ((st & 3) << 1);
+        }
+        const int a = (j >> 2) & 1 ? a1 : a0;
+        const int sym = a ? ((j & 3) < 2) : ((j & 3) >= 2);
+        M[c] += sym ? yj : -yj;
+      }
+    }
+    int ci = 0, best = INT_MIN;
+    for (int c = 0; c < 4; ++c) {
+      const int v = warp_sum(M[c]);
+      if (v > best) { best = v; ci = c; }
+    }
+    int s = 0, nb = 0, crc_bad = 1, metric = 0;
+    uint32_t flags = 0;
+    long long j_last = kCodedBlock1 - 1;
+    if (ci >= 2) {
+      flags = BTLE_CODED_CI_RESERVED;
+    } else {
+      s = ci == 0 ? 8 : 2;
+      const int per = s == 8 ? 4 : 1;
+      int m = (lane & 7) ? kCodedNeg : 0;
+      m = coded_acs(W, X, n0, per, 0, 40, m);
+      // header pass: trace back from the best state after step 40 (the lowest index on a tie)
+      int bm = m, bs = lane & 7;
+#pragma unroll
+      for (int o = 4; o; o >>= 1) {
+        const int om = __shfl_xor_sync(0xFFFFFFFFu, bm, o), os = __shfl_xor_sync(0xFFFFFFFFu, bs, o);
+        if (om > bm || (om == bm && os < bs)) { bm = om; bs = os; }
+      }
+      int len = 0;
+      if (lane == 0) {
+        int state = bs;
+        uint32_t hb = 0;
+        for (int t = 39; t >= 0; --t) {
+          if (t < 16) hb |= (uint32_t)(state & 1) << t;
+          state = (state >> 1) | (((W.surv[t] >> state) & 1) << 2);
+        }
+        for (int t = 0; t < 16; ++t) hb ^= (uint32_t)coded_wbit(W, t) << t;
+        len = (int)((hb >> 8) & 0xFFu);
+      }
+      len = __shfl_sync(0xFFFFFFFFu, len, 0);
+      const int n_steps = 16 + 8 * len + 27;
+      m = coded_acs(W, X, n0, per, 40, n_steps, m);
+      metric = __shfl_sync(0xFFFFFFFFu, m, 0);
+      if (lane == 0) {                                                      // full pass: trace back from state 0
+        for (int q = 0; q < (n_steps + 31) / 32; ++q) W.bits[q] = 0u;
+        int state = 0;
+        for (int t = n_steps - 1; t >= 0; --t) {
+          W.bits[t >> 5] |= (uint32_t)(state & 1) << (t & 31);
+          state = (state >> 1) | (((W.surv[t] >> state) & 1) << 2);
+        }
+      }
+      __syncwarp();
+      nb = len + 5;
+      for (int q = lane; q < nb; q += 32) {
+        uint32_t v = 0;
+        for (int i = 0; i < 8; ++i) {
+          const int t = 8 * q + i;
+          v |= (((W.bits[t >> 5] >> (t & 31)) & 1u) ^ (uint32_t)coded_wbit(W, t)) << i;
+        }
+        W.body[q] = (uint8_t)v;
+      }
+      __syncwarp();
+      if (lane == 0) {
+        const uint32_t crc = crc24_bytes(__ldg(&sp.crc_init), W.body, len + 2);
+        const uint32_t rx = (uint32_t)W.body[len + 2] | (uint32_t)W.body[len + 3] << 8 | (uint32_t)W.body[len + 4] << 16;
+        crc_bad = crc != rx;
+      }
+      crc_bad = __shfl_sync(0xFFFFFFFFu, crc_bad, 0);
+      j_last = kCodedBlock1 + (long long)s * n_steps - 1;
+    }
+    if (n0 + 4 * j_last + 3 >= n_int8 / 2) flags |= BTLE_CODED_TRUNCATED;
+    uint8_t *bytes = rec->bytes;
+    for (int q = lane; q < BTLE_CODED_MAX_BYTES + 8; q += 32) bytes[q] = q < nb ? W.body[q] : 0;   // bytes and reserved
+    if (lane == 0) {
+      rec->access_addr = aa;
+      rec->channel = (uint8_t)channel;
+      rec->s = (uint8_t)s;
+      rec->ci = (uint8_t)ci;
+      rec->crc_bad = (uint8_t)crc_bad;
+      rec->flags = (uint8_t)flags;
+      rec->reserved0 = 0;
+      rec->n_bytes = (uint16_t)nb;
+      rec->dist = dist;
+      rec->metric = metric;
+      rec->mag_sum = mag;
+    }
+    __syncwarp();
+  }
+}
+
+// Order of btle_b200_rx_coded: record k of src goes to dst[rank], rank = the number of records before it in (stream, sample)
+// order (the keys are distinct: two hits of one capture are at least 9 samples apart).
+__global__ void __launch_bounds__(256)
+coded_rank_kernel(const btle_coded_rec *__restrict__ src, unsigned n, btle_coded_rec *__restrict__ dst) {
+  __shared__ unsigned long long keys[256];
+  const unsigned k = blockIdx.x * 256 + threadIdx.x;
+  const unsigned long long mine = k < n ? ((unsigned long long)(uint32_t)src[k].stream << 40) | (unsigned long long)src[k].sample : 0ull;
+  unsigned rank = 0;
+  for (unsigned base = 0; base < n; base += 256) {
+    __syncthreads();
+    if (base + threadIdx.x < n) {
+      const btle_coded_rec &o = src[base + threadIdx.x];
+      keys[threadIdx.x] = ((unsigned long long)(uint32_t)o.stream << 40) | (unsigned long long)o.sample;
+    }
+    __syncthreads();
+    const unsigned m = min(256u, n - base);
+    for (unsigned j = 0; j < m; ++j) rank += keys[j] < mine;
+  }
+  if (k >= n) return;
+  const uint4 *s = reinterpret_cast<const uint4 *>(src + k);
+  uint4 *d = reinterpret_cast<uint4 *>(dst + rank);
+  for (int q = 0; q < (int)(sizeof(btle_coded_rec) / 16); ++q) d[q] = s[q];
+}
+
 // ---- BER flow of python/test_btle_ber.py on the device: packet source + channel + int16 truncation --------------------
 // One CTA per packet: 37 random payload bytes behind the fixed header 42 25 (test_btle_ber.py:27,:49), build_air,
 // the Python model's 8-sps modulator (gfsk_block<8>), add_freq_sampling_error (linear
@@ -2107,6 +2499,7 @@ struct btle_b200_ctx {
   cudaEvent_t stage_free[2] = {nullptr, nullptr};
   Buf<uint8_t> d_leaf;              // scratch of the leaf entry points (leaf_layout)
   Buf<btle_conn_cand> d_cand;       // device candidates of btle_b200_discover
+  Buf<btle_coded_rec> d_coded[2];   // btle_b200_rx_coded: the records as found, and in (stream, sample) order
   // BTLE_CFG_OFFSET_SEARCH (launch_offset_search): the hypotheses' records, directory and counters [hypotheses, merged], and
   // the last launch that used them (a flagged launch on another stream waits for it)
   Buf<btle_pkt_rec> os_out;
@@ -2776,6 +3169,65 @@ int launch_discover(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, si
   rc = note_use(ctx, cs, st, sid);
   if (rc) return rc;
   ctx->last_launches = 1;
+  return BTLE_OK;
+}
+
+// The cfgs of the coded receiver (include/btle_b200.h, btle_b200_rx_coded_device) and the rotation of each capture
+int check_coded(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size_t n_streams, const float *offset_hz, std::vector<int4> &rot) {
+  if (!cfgs && n_streams) { ctx->err = "rx_coded: missing cfg array"; return BTLE_EINVAL; }
+  for (size_t s = 0; s < n_streams; ++s) {
+    const btle_stream_cfg &c = cfgs[s];
+    if (c.channel < 0 || c.channel > 39) { ctx->err = "rx_coded: channel must be within 0~39"; return BTLE_EINVAL; }
+    if (c.raw) { ctx->err = "rx_coded: raw mode has no coded form"; return BTLE_EINVAL; }
+    if (c.access_mask != 0xFFFFFFFFu) { ctx->err = "rx_coded: access_mask must be 0xFFFFFFFF"; return BTLE_EINVAL; }
+    if (c.rssi & ~BTLE_CFG_RSSI) { ctx->err = "rx_coded: the only flag is BTLE_CFG_RSSI"; return BTLE_EINVAL; }
+  }
+  std::vector<float> hz(n_streams, 0.0f);
+  if (offset_hz) {
+    const int rc = cfg_offsets(ctx, offset_hz, n_streams, nullptr, n_streams, hz);
+    if (rc) return rc;
+  }
+  rot.resize(n_streams);
+  for (size_t s = 0; s < n_streams; ++s) rot[s] = make_rot(hz[s]);
+  return BTLE_OK;
+}
+
+// coded_search_kernel, then coded_decode_kernel over the hits it counted, both on `st` (the counter is zeroed here).  The
+// hits wait in d_out's slots between the two kernels, so there is no other scratch, and no hit goes unseen: *d_count is
+// the number found, whatever cap is.
+int launch_coded(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8, const btle_stream_cfg *cfgs,
+                 const std::vector<int4> &rot, btle_coded_rec *d_out, size_t cap, unsigned *d_count, cudaStream_t st) {
+  if (!d_count || (!d_out && cap) || (!d_iq && n_streams && n_int8)) { ctx->err = "rx_coded: missing buffer"; return BTLE_EINVAL; }
+  if ((reinterpret_cast<uintptr_t>(d_iq) & 15) || (n_streams > 1 && (stride & 15))) { ctx->err = "device IQ must be 16-byte aligned"; return BTLE_EINVAL; }
+  if (reinterpret_cast<uintptr_t>(d_out) & 15) { ctx->err = "rx_coded: d_out must be 16-byte aligned"; return BTLE_EINVAL; }
+  if (n_streams > 1 && stride < n_int8) { ctx->err = "stream stride smaller than stream length"; return BTLE_EINVAL; }
+  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
+  ctx->last_launches = 0;
+  BTLE_CUDA(ctx, cudaMemsetAsync(d_count, 0, sizeof(unsigned), st));
+  const long long n_samples = (long long)(n_int8 / 2);
+  if (!n_streams || n_samples < 323 + 1024) return BTLE_OK;                // no window fits
+  const long long groups = (n_samples - 1024) / 128 + 1;                   // groups holding a window start inside the capture
+  const long long tiles = (groups + kCodedGroups - 1) / kCodedGroups;
+  if (tiles * (long long)n_streams > 0x7FFFFFFFll) { ctx->err = "batch too large for one launch"; return BTLE_EINVAL; }
+  unsigned long long sid = 0;
+  int rc = stream_id(ctx, st, &sid);
+  if (rc) return rc;
+  CfgSlot *cs = nullptr;
+  rc = upload_cfgs(ctx, cfgs, n_streams, st, sid, &cs, nullptr, rot.data());
+  if (rc) return rc;
+  const unsigned cap32 = (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu);
+  coded_search_kernel<<<(unsigned)(tiles * (long long)n_streams), kCodedThreads, kCodedSmem, st>>>(
+      d_iq, (long long)stride, (long long)n_int8, tiles, cs->d_params, cs->d_rot, d_out, cap32, d_count);
+  BTLE_CUDA(ctx, cudaGetLastError());
+  if (cap32) {
+    const unsigned grid = (unsigned)std::min<long long>((cap32 + kCodedDecWarps - 1) / kCodedDecWarps, 16ll * ctx->num_sms);
+    coded_decode_kernel<<<grid, 32 * kCodedDecWarps, 0, st>>>(d_iq, (long long)stride, (long long)n_int8, cs->d_params, cs->d_rot, d_out,
+                                                            cap32, d_count);
+    BTLE_CUDA(ctx, cudaGetLastError());
+  }
+  rc = note_use(ctx, cs, st, sid);
+  if (rc) return rc;
+  ctx->last_launches = cap32 ? 2 : 1;
   return BTLE_OK;
 }
 
@@ -3920,6 +4372,45 @@ int btle_b200_discover(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, s
   std::sort(out, out + std::min(*n_out, cap), [](const btle_conn_cand &a, const btle_conn_cand &b) {
     return a.stream != b.stream ? a.stream < b.stream : a.sample < b.sample;
   });
+  if (*n_out > cap) { ctx->err = "output capacity too small"; return BTLE_EOVERFLOW; }
+  return BTLE_OK;
+}
+
+int btle_b200_rx_coded_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8,
+                              const btle_stream_cfg *cfgs, const float *offset_hz, btle_coded_rec *d_out, size_t cap,
+                              uint32_t *d_count, void *cuda_stream) {
+  if (!ctx) return BTLE_EINVAL;
+  std::vector<int4> rot;
+  const int rc = check_coded(ctx, cfgs, n_streams, offset_hz, rot);
+  if (rc) return rc;
+  return launch_coded(ctx, d_iq, n_streams, stride, n_int8, cfgs, rot, d_out, cap, d_count, reinterpret_cast<cudaStream_t>(cuda_stream));
+}
+
+// The records land unordered in ctx->d_coded[0], are put in (stream, sample) order into ctx->d_coded[1] on the device
+// (coded_rank_kernel) and copied out.
+int btle_b200_rx_coded(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stride, size_t n_int8, const btle_stream_cfg *cfgs,
+                       const float *offset_hz, btle_coded_rec *out, size_t cap, size_t *n_out) {
+  if (!ctx) return BTLE_EINVAL;
+  if (!n_out || (!out && cap) || (!iq && n_streams && n_int8)) { ctx->err = "rx_coded: missing buffer"; return BTLE_EINVAL; }
+  *n_out = 0;
+  std::vector<int4> rot;
+  int rc = check_coded(ctx, cfgs, n_streams, offset_hz, rot);               // before any byte is copied
+  if (rc) return rc;
+  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  size_t pitch = 0;
+  rc = ingest(ctx, iq, n_streams, stride, n_int8, nullptr, n_streams, &pitch);
+  if (rc) return rc;
+  if (ctx->d_coded[0].reserve(ctx, std::max<size_t>(cap, 1)) || ctx->d_coded[1].reserve(ctx, std::max<size_t>(cap, 1))) return BTLE_ENOMEM;
+  rc = launch_coded(ctx, ctx->d_iq, n_streams, pitch, n_int8, cfgs, rot, ctx->d_coded[0], cap, ctx->d_count, st);
+  if (rc) return rc;
+  rc = fetch_counted(ctx, st, cap, n_out, [&](size_t n) {
+    coded_rank_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ctx->d_coded[0], (unsigned)n, ctx->d_coded[1]);
+    BTLE_CUDA(ctx, cudaGetLastError());
+    BTLE_CUDA(ctx, cudaMemcpyAsync(out, ctx->d_coded[1], n * sizeof(btle_coded_rec), cudaMemcpyDeviceToHost, st));
+    return BTLE_OK;
+  });
+  if (rc) return rc;
   if (*n_out > cap) { ctx->err = "output capacity too small"; return BTLE_EOVERFLOW; }
   return BTLE_OK;
 }

@@ -12,7 +12,7 @@ from functools import partial
 import numpy as np
 
 from . import _native
-from ._native import BTLE_EOVERFLOW, BtleError, CAND_DTYPE, CFG_DTYPE, DIR_DTYPE, REC_DTYPE
+from ._native import BTLE_EOVERFLOW, BtleError, CAND_DTYPE, CFG_DTYPE, CODED_REC_DTYPE, DIR_DTYPE, REC_DTYPE
 
 DEFAULT_ACCESS_ADDR = 0x8E89BED6     # btle_rx.c:231
 DEFAULT_CRC_INIT = 0x555555          # btle_rx.c:232
@@ -243,6 +243,35 @@ class BtleRx:
         ch = np.ascontiguousarray(np.broadcast_to(np.asarray(channels, dtype=np.int32), (ns,)))
         return self._grow_once(partial(self._L.btle_b200_discover, self._h, iq.ctypes.data, ns, n, n, ch.ctypes.data), CAND_DTYPE,
                                ns * (n // 16384 + 1) * 8 + 256 if cap is None else cap, grow=cap is None)
+
+    def rx_coded(self, iq: np.ndarray, cfgs: np.ndarray | None = None, offset_hz=None, cap: int | None = None, **cfg) -> np.ndarray:
+        """LE Coded PHY packets (btle_b200_rx_coded): iq int8 [n_streams, n_int8] (or [n_int8]); cfgs: CFG_DTYPE [n_streams]
+        (access address, CRC init, channel and BTLE_CFG_RSSI of each capture), or make_cfgs(n_streams, **cfg) when None;
+        offset_hz (a scalar or one per capture): carrier-offset correction.  Returns CODED_REC_DTYPE records sorted by
+        (stream, sample); `cap` defaults to a typical worst case and is grown once to the exact count on overflow."""
+        iq = np.ascontiguousarray(iq, dtype=np.int8)
+        if iq.ndim == 1:
+            iq = iq[None, :]
+        ns, n = iq.shape
+        cfgs = make_cfgs(ns, **cfg) if cfgs is None else np.ascontiguousarray(cfgs, dtype=CFG_DTYPE)
+        assert cfgs.shape == (ns,)
+        off = _offsets(offset_hz, ns)
+        call = partial(self._L.btle_b200_rx_coded, self._h, iq.ctypes.data, ns, n, n, cfgs.ctypes.data, _ptr(off))
+        return self._grow_once(call, CODED_REC_DTYPE, ns * (n // 65536 + 1) * 4 + 64 if cap is None else cap, grow=cap is None)
+
+    def rx_coded_device(self, d_iq, cfgs: np.ndarray, d_out, d_count, stream_ptr: int = 0, offset_hz=None):
+        """d_iq: torch int8 CUDA tensor [n_streams, n_int8] (16-byte aligned rows); cfgs: CFG_DTYPE [n_streams]; d_out: torch
+        CUDA tensor of cap * 304 bytes (16-byte aligned); d_count: torch int32 CUDA tensor [1].  Enqueues on `stream_ptr`
+        (no sync).  Records land unordered in d_out[:min(count, cap)] (view the bytes as CODED_REC_DTYPE)."""
+        ns, n = d_iq.shape
+        assert d_iq.stride(1) == 1
+        cfgs = np.ascontiguousarray(cfgs, dtype=CFG_DTYPE)
+        assert cfgs.shape == (ns,)
+        off = _offsets(offset_hz, ns)
+        cap = d_out.numel() * d_out.element_size() // CODED_REC_DTYPE.itemsize
+        rc = self._L.btle_b200_rx_coded_device(self._h, d_iq.data_ptr(), ns, d_iq.stride(0), n, cfgs.ctypes.data, _ptr(off),
+                                               d_out.data_ptr(), cap, d_count.data_ptr(), ctypes.c_void_p(stream_ptr))
+        self._check(rc)
 
     # ---- unbounded capture, pushed in pieces (btle_b200_stream_*) -----------------------------
     def stream(self, segment_chunks: int = 0, **cfg) -> "RxStream":

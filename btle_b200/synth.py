@@ -234,6 +234,79 @@ def make_pdu_stream(pdus, channel: int, access_addr: int = ADV_ACCESS_ADDR, crc_
     return iq
 
 
+# ---- LE Coded PHY transmitter (include/btle_b200.h, "LE Coded PHY"; Core Spec v5.x Vol 6 Part B §2.2, §3.3) ----
+CODED_PREAMBLE = np.tile(np.array([0, 0, 1, 1, 1, 1, 0, 0], dtype=np.uint8), 10)   # 80 symbols in transmit order
+CODED_CI = {8: 0, 2: 1}                                                          # coding indicator of each S
+
+
+def whitening_bits(channel: int, n: int) -> np.ndarray:
+    """uint8 [n]: the first n whitening bits of the channel's LFSR (period 127), bit k of the stream after the AA."""
+    reg = [1] + [(channel >> (5 - i)) & 1 for i in range(6)]
+    seq = np.zeros(127, dtype=np.uint8)
+    for k in range(127):
+        o = reg[6]
+        seq[k] = o
+        reg = [o, reg[0], reg[1], reg[2], reg[3] ^ o, reg[4], reg[5]]
+    return seq[np.arange(n) % 127]
+
+
+def conv_encode(bits, state: int = 0):
+    """K = 4, rate 1/2 encoder: G0 = 1 + x + x^2 + x^3, G1 = 1 + x^2 + x^3.  Returns (coded bits a0, a1, a0, a1, ...,
+    final state); state = b[t-1] | b[t-2] << 1 | b[t-3] << 2."""
+    out = np.zeros(2 * len(bits), dtype=np.uint8)
+    for t, b in enumerate(bits):
+        b = int(b) & 1
+        s0, s1, s2 = state & 1, (state >> 1) & 1, (state >> 2) & 1
+        out[2 * t], out[2 * t + 1] = b ^ s0 ^ s1 ^ s2, b ^ s1 ^ s2
+        state = b | ((state & 3) << 1)
+    return out, state
+
+
+def pattern_map(coded, s: int) -> np.ndarray:
+    """S=8: coded bit 0 -> 0,0,1,1 and 1 -> 1,1,0,0; S=2: the coded bit as it is."""
+    coded = np.asarray(coded, dtype=np.uint8)
+    if s == 2:
+        return coded.copy()
+    assert s == 8
+    return np.stack([coded, coded, 1 - coded, 1 - coded], axis=1).reshape(-1).astype(np.uint8)
+
+
+def _lsb_bits(value: int, n: int) -> np.ndarray:
+    return np.array([(int(value) >> i) & 1 for i in range(n)], dtype=np.uint8)
+
+
+def coded_symbols(pdu: bytes, channel: int, access_addr: int = ADV_ACCESS_ADDR, crc_init: int = ADV_CRC_INIT, s: int = 8,
+                  ci: int | None = None):
+    """Symbol stream of one LE Coded PHY packet: preamble, FEC block 1 (AA, CI, TERM1; S=8), FEC block 2 (whitened PDU +
+    CRC-24, TERM2; at S).  pdu = 16-bit header (byte 1 = length, 8 bits) + payload.  ci overrides the coding indicator
+    sent (2 and 3 are reserved).  Returns (symbols uint8 [n], packed bytes): packed holds the symbols LSB first, padded
+    with 0 to whole bytes, the input of modulate() / tx_modulate_device."""
+    pdu = bytes(pdu)
+    assert len(pdu) >= 2 and pdu[1] == len(pdu) - 2 and s in CODED_CI
+    ci = CODED_CI[s] if ci is None else int(ci)
+    crc = crc24(pdu, crc_init)
+    body = np.unpackbits(np.frombuffer(pdu + bytes([crc & 0xFF, (crc >> 8) & 0xFF, (crc >> 16) & 0xFF]), dtype=np.uint8),
+                         bitorder="little")
+    body ^= whitening_bits(channel, body.size)
+    b1, st = conv_encode(np.concatenate([_lsb_bits(access_addr, 32), _lsb_bits(ci, 2), np.zeros(3, np.uint8)]))
+    assert st == 0
+    b2, st = conv_encode(np.concatenate([body, np.zeros(3, np.uint8)]))
+    assert st == 0
+    syms = np.concatenate([CODED_PREAMBLE, pattern_map(b1, 8), pattern_map(b2, s)])
+    pad = np.zeros((-syms.size) % 8, dtype=np.uint8)
+    return syms, np.packbits(np.concatenate([syms, pad]), bitorder="little").tobytes()
+
+
+def coded_air(pdu: bytes, channel: int, access_addr: int = ADV_ACCESS_ADDR, crc_init: int = ADV_CRC_INIT, s: int = 8,
+              ci: int | None = None) -> np.ndarray:
+    """int8 interleaved IQ at 4 samples per symbol of one coded packet (modulate() of coded_symbols' packed form).  Symbol j
+    of the access address (preamble symbol 0 is j = -80) is read at sample CODED_AA_SAMPLE + 4 j of the returned array."""
+    return modulate(coded_symbols(pdu, channel, access_addr, crc_init, s, ci)[1])
+
+
+CODED_AA_SAMPLE = 4 * 80 + 7     # n0 of a coded_air() burst placed at sample 0 (the modulator's delay is 7 samples)
+
+
 # ---- 8 samples/symbol modulator of the reference's Python model (input generator of the BER sweep) ----
 GAUSS_TAPS_8SPS = (0, 0, 0, 1, 4, 9, 15, 22, 24, 22, 15, 9, 4, 1, 0, 0, 0)   # btlelib.py:146-160 (int8, x128)
 

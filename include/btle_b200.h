@@ -461,6 +461,85 @@ int btle_b200_discover_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_s
 int btle_b200_discover(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stream_stride_int8, size_t n_int8,
                        const int32_t *channels, btle_conn_cand *out, size_t cap, size_t *n_out);
 
+/* ---- LE Coded PHY (long range, BLE 5): a receiver beside the 1M one, on the same 4-Msps int8 captures --------------
+ * Not part of the reference.  The coded PHY sends the same 1 Msym/s GFSK on the same channels; its access address is
+ * convolutionally coded and spread, so the 1M search never matches it.  Transmitter (Core Spec v5.x, Vol 6 Part B
+ * §2.2, §3.3; btle_b200/synth.py coded_symbols):
+ *   preamble  80 symbols, 10 x 0,0,1,1,1,1,0,0 in transmit order
+ *   block 1   access address (32 bits, LSB first), CI (2 bits, LSB first: 0 S=8, 1 S=2, 2 and 3 reserved), TERM1 (3 zero
+ *             bits); always S=8: 37 bits -> 74 coded bits -> 296 symbols
+ *   block 2   PDU (16-bit header, byte 1 = length L, 8 bits; then L = 0..255 payload bytes), CRC-24, TERM2 (3 zero bits),
+ *             at the S given by CI: (16 + 8L + 27) * S symbols
+ *   order     CRC over the PDU, whitening of PDU + CRC (channel LFSR, as for 1M), FEC, pattern mapping; AA, CI and TERM are
+ *             not whitened
+ *   FEC       K = 4, rate 1/2, G0 = 1 + x + x^2 + x^3, G1 = 1 + x^2 + x^3; per input bit a0 is sent, then a1.  The state is
+ *             zero at the start of block 1, and TERM1 returns it to zero for block 2
+ *   mapper    S=8: coded bit 0 -> 0,0,1,1 and 1 -> 1,1,0,0; S=2: the coded bit as it is
+ * Receiver (btle_b200_rx_coded*).  Positions are absolute samples of the capture; x outside the capture reads 0.
+ *   discriminator  the BTLE_CFG_SYMBOL_SPACED | BTLE_CFG_LOWPASS one, always rotated: F[n] = (x[n-1] + 2 x[n] + x[n+1]) >> 2
+ *             per rail, v[n] = C4 (FI[n-2] FQ[n+2] - FI[n+2] FQ[n-2]) - S4 (FI[n-2] FI[n+2] + FQ[n-2] FQ[n+2]) (int32), (C4,
+ *             S4) from the capture's offset_hz as for the *_offset entry points ((16384, 0) without one).  Hard bit h[n] =
+ *             v[n] > 0, soft value y[n] = clamp(v[n] >> 22, -127, 127).  There are no mode flags.
+ *   symbols   symbol j relative to the access address is read at n0 + 4j; the preamble is j = -80..-1.
+ *   search    P = the 336 known symbols j = -80..255: the preamble and the block-1 coding of the cfg's access address
+ *             (fixed: the encoder starts at zero).  D(n0) = #{j = -80..255 : h[n0 + 4j] != P[j]}, defined only where
+ *             the window lies inside the capture: n0 >= 323 and n0 + 1023 < n_samples.  n0 is a HIT iff D(n0) <=
+ *             BTLE_CODED_MAX_DIST, D(n0) < D(m) for every defined m in [n0 - 8, n0 - 1] and D(n0) <= D(m) for every
+ *             defined m in [n0 + 1, n0 + 8].  Each hit gives exactly one record (two hits are at least 9 samples apart).
+ *   CI        from the state after the access address (its last 3 bits), code (c0, c1, 0, 0, 0) for c = 0..3 into the
+ *             40 symbols j = 256..295; M(c) = sum (2 sym - 1) y.  The largest M wins, the lower c on a tie.  c >= 2: a
+ *             record flagged BTLE_CODED_CI_RESERVED with s = 0, n_bytes = 0, crc_bad = 1.
+ *   soft bits block 2 starts at j = 296.  Coded bit k reads 1 symbol (S=2: L = y) or 4 (S=8: L = y0 + y1 - y2 - y3).
+ *   Viterbi   branch metric (2 a0 - 1) L0 + (2 a1 - 1) L1, maximised; state s = b[t-1] | b[t-2] << 1 | b[t-3] << 2; on
+ *             equal metrics the predecessor with the lower index wins.  int32 metrics (|metric| <= 2.2e6; the states not
+ *             yet reachable start at -2^29).
+ *   header    Viterbi over info bits 0..39 from state 0, traced back from the best final state (lowest index on a tie);
+ *             bits 0..15 dewhitened give the header, L = byte 1.
+ *   full      Viterbi over 16 + 8L + 27 info bits from state 0, traced back from state 0; the bits dewhitened give header +
+ *             payload + CRC, n_bytes = L + 5; crc_bad compares the CRC-24 (crc_init, -k convention) with the received CRC.
+ *             The first 40 steps are the header pass's, so one trellis serves both.
+ *   truncated a record whose symbols (up to j = 295 when CI is reserved, else the last of block 2) read a sample at or past
+ *             the capture's end (n0 + 4 j + 3 >= n_samples) is flagged BTLE_CODED_TRUNCATED; those samples read 0.
+ * Conformance rests on these rules: no third-party coded-PHY test vector was available.  tests/test_coded.py pins the
+ * encoder's impulse response and a hand-checked preamble and block-1 layout. */
+#define BTLE_CODED_MAX_DIST 96
+#define BTLE_CODED_CI_RESERVED 1   /* btle_coded_rec.flags: CI 2 or 3, nothing decoded                                  */
+#define BTLE_CODED_TRUNCATED 2     /* btle_coded_rec.flags: the packet runs past the capture's end (read as 0)          */
+#define BTLE_CODED_MAX_BYTES 260   /* header + 255 payload bytes + CRC                                                */
+typedef struct {
+  int64_t sample;        /* n0: first sample of the access address (symbol j = 0), from the start of the capture        */
+  int32_t stream;
+  uint32_t access_addr;
+  uint8_t channel;
+  uint8_t s;             /* 8 or 2; 0 when CI is reserved                                                             */
+  uint8_t ci;            /* 0..3                                                                                       */
+  uint8_t crc_bad;
+  uint8_t flags;         /* BTLE_CODED_CI_RESERVED, BTLE_CODED_TRUNCATED                                              */
+  uint8_t reserved0;
+  uint16_t n_bytes;      /* L + 5, 0 when CI is reserved                                                              */
+  int32_t dist;          /* D(n0)                                                                                     */
+  int32_t metric;        /* final metric of the full pass (state 0)                                                   */
+  uint32_t mag_sum;      /* sum |I| + |Q| over samples n0 .. n0 + 1023 with BTLE_CFG_RSSI, else 0                       */
+  uint8_t bytes[BTLE_CODED_MAX_BYTES];   /* dewhitened header + payload + CRC, zero beyond n_bytes                    */
+  uint8_t reserved[8];
+} btle_coded_rec;        /* 304 bytes */
+/* device: `d_iq` 16-byte aligned, stride a multiple of 16 and >= n_int8 when n_streams > 1; cfgs[s] (host array) is the
+ * access address, CRC init and channel of capture s; offset_hz (host array, NULL = 0) its carrier offset.  Records are
+ * unordered; *d_count (zeroed by the call) = the number found, d_out[0 .. min(count, cap)) holds that many of them (not
+ * necessarily the first ones: d_out also holds the hits between the two kernels, so no hit is dropped unseen).
+ * Enqueued on cuda_stream, not synchronised.  BTLE_EINVAL with btle_b200_last_error() set: a channel outside 0..39, raw,
+ * access_mask != 0xFFFFFFFF, an rssi flag other than BTLE_CFG_RSSI (the 1M opt-in flags mean nothing here and are
+ * refused), an offset that is not finite or exceeds BTLE_MAX_OFFSET_HZ, a misaligned pointer or stride, a missing
+ * buffer. */
+int btle_b200_rx_coded_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stream_stride_int8,
+                              size_t n_int8, const btle_stream_cfg *cfgs, const float *offset_hz, btle_coded_rec *d_out,
+                              size_t cap, uint32_t *d_count, void *cuda_stream);
+/* host buffers (page-locked or pageable, as btle_b200_rx_batch); out sorted by (stream, sample) on the device before the
+ * copy.  BTLE_EOVERFLOW with *n_out = the number found when that exceeds cap (out then holds cap of them); a second call
+ * with cap >= *n_out returns them all. */
+int btle_b200_rx_coded(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stream_stride_int8, size_t n_int8,
+                       const btle_stream_cfg *cfgs, const float *offset_hz, btle_coded_rec *out, size_t cap, size_t *n_out);
+
 /* ---- connections on a streaming session (btle_b200_streams_*): per-capture cfg lists, backfill, discovery -----------
  * Every cfg of a session has a stable index, never reused: the n_streams cfgs of btle_b200_streams_open are 0..n-1 (cfg
  * i decodes capture i), each added cfg gets the next one.  A record's `stream` is that index.  The records of cfg j equal
