@@ -77,18 +77,23 @@ def distances(cap: Capture, access_addr: int) -> np.ndarray:
 
 
 def distances_bits(h: np.ndarray, access_addr: int) -> np.ndarray:
-    """D(n0) over hard bits h[n] (0/1) of a capture of h.size samples, -1 where it is not defined"""
-    P = pattern(access_addr)
+    """D(n0) over hard bits h[n] (0/1) of a capture of h.size samples, -1 where it is not defined.
+
+    D(n0) = sum_j [h[n0 + 4 j] != P[j + 80]], j = -80..255.  With a = 2 h - 1 and p = 2 P - 1 (+-1), a mismatch is
+    (1 - a p) / 2, so D = (336 - sum_j a[n0 + 4 j] p[j + 80]) / 2: one integer correlation per sample phase n0 % 4."""
+    p = 2 * pattern(access_addr).astype(np.int64) - 1
     N = h.size
     D = np.full(N, -1, np.int64)
     lo, hi = 323, N - 1024                    # defined for lo <= n0 <= hi
     if hi < lo:
         return D
-    n0 = np.arange(lo, hi + 1)
-    acc = np.zeros(n0.size, np.int64)
-    for j in range(-80, 256):
-        acc += h[n0 + 4 * j] != P[j + 80]
-    D[lo:hi + 1] = acc
+    a = 2 * np.asarray(h, dtype=np.int64) - 1
+    for ph in range(4):
+        n0 = np.arange(lo + (ph - lo) % 4, hi + 1, 4)
+        if n0.size == 0:
+            continue
+        m0, m1 = (n0[0] - ph) // 4, (n0[-1] - ph) // 4   # n0 = 4 m + ph reads a[ph + 4 (m + j)], m + j = m - 80 .. m + 255
+        D[n0] = (p.size - np.correlate(a[ph::4][m0 - 80:m1 + 256], p, "valid")) // 2
     return D
 
 
@@ -147,6 +152,17 @@ def coded_soft(cap: Capture, n0: int, s: int, n_coded: int) -> np.ndarray:
     if s == 2:
         return y.reshape(-1)
     return y[:, 0] + y[:, 1] - y[:, 2] - y[:, 3]
+
+
+def path_metric(cap: Capture, n0: int, s: int, body: bytes, channel: int) -> int:
+    """Correlation of block 2 as sent for `body` (the L + 5 bytes of PDU and CRC, before whitening) with the soft values
+    of the hit at n0: the whitened bits and TERM2, coded from state 0, as +-1 against coded_soft.  For the decoded bytes
+    it is the metric of the Viterbi path they lie on, computed without the trellis."""
+    bits = np.unpackbits(np.frombuffer(bytes(body), np.uint8), bitorder="little")
+    bits = np.concatenate([bits ^ synth.whitening_bits(channel, bits.size), np.zeros(3, np.uint8)])
+    coded, st = synth.conv_encode(bits)
+    assert st == 0
+    return int(((2 * coded.astype(np.int64) - 1) * coded_soft(cap, n0, s, coded.size)).sum())
 
 
 def decode(cap: Capture, n0: int, dist: int, stream: int, cfg) -> np.ndarray:

@@ -159,7 +159,56 @@ def test_no_false_alarm_on_random_bits():
     assert cr.hits_from_distances(D).size == 0
 
 
-PER_SNR_DB = -3.0      # the GPU sensitivity point (test_coded_gpu.py): S=8 still decodes, the 1M chain does not
+def _distances_loop(h, access_addr):
+    """D(n0) as the header states it: one pass over the capture per known symbol j = -80..255"""
+    P = cr.pattern(access_addr)
+    D = np.full(h.size, -1, np.int64)
+    lo, hi = 323, h.size - 1024
+    if hi >= lo:
+        n0 = np.arange(lo, hi + 1)
+        D[lo:hi + 1] = sum((h[n0 + 4 * j] != P[j + 80]).astype(np.int64) for j in range(-80, 256))
+    return D
+
+
+def test_fast_distances_equal_the_loop():
+    rng = np.random.default_rng(13)
+    for n in (0, 1346, 1347, 1348, 1349, 1350, 1351, 4096, 50_001):
+        for aa in (AA, 0x12345678, 0xFFFFFFFF, 0):
+            h = rng.integers(0, 2, n).astype(np.uint8)
+            assert np.array_equal(cr.distances_bits(h, aa), _distances_loop(h, aa)), (n, hex(aa))
+    # captures holding bursts at every phase, noiseless and noisy, at a corrected carrier offset
+    specs, n0 = [], 700
+    for k in range(8):
+        specs.append((n0 + k % 4, _pdu(3 * k, seed=k), 2 + 6 * (k % 2)))
+        n0 += 4 * (376 + (43 + 24 * k) * specs[-1][2]) + 900
+    bursts = [(n, synth.coded_air(p, 37, AA, s=s)) for n, p, s in specs]
+    for snr, hz in ((None, 0.0), (0.0, 0.0), (-4.0, 60e3)):
+        rng = np.random.default_rng(17)
+        iq = cr.place(n0 + 1500, bursts, 100, 0.0 if snr is None else cr.sigma_of(snr, 100), rng, offset_hz=hz)
+        cap = cr.Capture(iq, hz)
+        D = cr.distances(cap, AA)
+        assert np.array_equal(D, _distances_loop(cap.h, AA))
+        assert (D[[n for n, _, _ in specs]] <= (0 if snr is None else 120)).all()
+
+
+def test_path_metric_of_the_decoded_bytes_is_the_viterbi_metric():
+    rng = np.random.default_rng(19)
+    for L, s in ((0, 2), (9, 8), (40, 2)):
+        pdu = _pdu(L, seed=s)
+        wav = synth.coded_air(pdu, 12, AA, 0x123456, s=s)
+        iq = cr.place(1001 + wav.size // 2 + 1500, [(1001, wav)], 100, cr.sigma_of(1.0, 100), rng)
+        cap = cr.Capture(iq)
+        r = cr.rx_coded(iq, _cfg(12, crc_init=0x123456))
+        r = r[np.abs(r["sample"] - 1001) <= 3][0]
+        n0 = int(r["sample"])
+        assert r["s"] == s and r["n_bytes"] == L + 5
+        assert cr.path_metric(cap, n0, s, bytes(r["bytes"][:L + 5]), 12) == r["metric"]
+        crc = synth.crc24(pdu, 0x123456)
+        sent = pdu + bytes([crc & 0xFF, (crc >> 8) & 0xFF, crc >> 16])
+        assert cr.path_metric(cap, n0, s, sent, 12) <= r["metric"]
+
+
+PER_SNR_DB = -3.0     # the GPU sensitivity point (test_coded_gpu.py): S=8 still decodes, the 1M chain does not
 PER_S8_BOUND = 0.5     # its bound: twice what this run may measure
 
 
