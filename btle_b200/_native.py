@@ -82,6 +82,7 @@ EXPORTS = [
     "btle_b200_streams_take_cands", "btle_b200_rx_batch_offset", "btle_b200_rx_device_dir_offset", "btle_b200_rx_multi_offset",
     "btle_b200_rx_multi_device_dir_offset", "btle_b200_rec_offset_device", "btle_b200_rec_offset",
     "btle_b200_streams_set_offset", "btle_b200_stream_set_offset", "btle_b200_rx_coded", "btle_b200_rx_coded_device",
+    "btle_b200_rx_coded_multi", "btle_b200_rx_coded_multi_device",
 ]
 MAX_CFGS_PER_CAPTURE = 8       # BTLE_MAX_CFGS_PER_CAPTURE
 CFG_RSSI, CFG_REPORT_REJECTED, CFG_RECOVER = 1, 2, 4      # btle_stream_cfg.rssi flag bits (BTLE_CFG_*)
@@ -201,6 +202,8 @@ def load():
     L.btle_b200_stream_set_offset.argtypes = [vp, ctypes.c_float]
     L.btle_b200_rx_coded.argtypes = [vp, vp, sz, sz, sz, vp, vp, vp, sz, ctypes.POINTER(sz)]
     L.btle_b200_rx_coded_device.argtypes = [vp, vp, sz, sz, sz, vp, vp, vp, sz, vp, vp]
+    L.btle_b200_rx_coded_multi.argtypes = [vp, vp, sz, sz, sz, vp, vp, sz, vp, vp, sz, ctypes.POINTER(sz)]
+    L.btle_b200_rx_coded_multi_device.argtypes = [vp, vp, sz, sz, sz, vp, vp, sz, vp, vp, sz, vp, vp]
     _lib = L
     return L
 

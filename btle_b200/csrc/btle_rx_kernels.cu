@@ -1506,28 +1506,35 @@ discover_kernel(const int8_t *__restrict__ iq, long long stride, long long n_int
 }
 
 // ---- LE Coded PHY receiver (btle_b200_rx_coded*, include/btle_b200.h "LE Coded PHY") ---------------------------------
-// coded_search_kernel: one CTA = kCodedGroups groups of window starts (128 samples each) of one capture.  D(n0) reads the
-// phase words of the 3 groups in front of n0's group and 8 behind it, and the hit rule reads D 8 samples to each side, so
-// the CTA packs kCodedThreads groups (G0 - 4 .. G0 + 123) and computes D for kCodedDGroups (G0 - 1 .. G0 + 115):
+// coded_search_kernel: one CTA = kCodedGroups groups of window starts (128 samples each) of one capture group of the cfg
+// list (upload_cfgs' vmap entry {capture, first cfg, number of cfgs}).  D(n0) reads the phase words of the 3 groups in
+// front of n0's group and 8 behind it, and the hit rule reads D 8 samples to each side, so the CTA packs kCodedThreads
+// groups (G0 - 4 .. G0 + 123) and computes D for kCodedDGroups (G0 - 1 .. G0 + 115):
 //   load   cp.async of the groups' IQ and one more row on each side (the low-pass walk reads two words past its group)
-//          into rows of kCodedPitch words; bytes outside the capture read as 0
-//   pack   lane p turns packed group p into its four phase words (dbits_group_lowpass, rotated by (C4, S4))
-//   D      lane dg computes D for the 128 window starts of its group, 11 words of XOR + POPC each (after 7 words a count
-//          above BTLE_CODED_MAX_DIST is stored as 97: every comparison with a hit, D <= 96, comes out the same), into the
-//          freed IQ rows (255 where D is not defined)
+//          into rows of kCodedPitch words; bytes outside the capture read as 0.  Once per tile, whatever the number of cfgs
+//   pack   lane p turns packed group p into its four phase words (dbits_group_lowpass, rotated by the capture's (C4, S4));
+//          lanes 0 .. count - 1 build the patterns P of the capture's cfgs
+//   then, for each cfg of the capture in turn:
+//   D      lane dg computes D for the 128 window starts of its group, 11 words of XOR + POPC each against the cfg's P (after
+//          7 words a count above BTLE_CODED_MAX_DIST is stored as 97: every comparison with a hit, D <= 96, comes out the
+//          same), into one of two D buffers in the freed IQ rows (255 where D is not defined); the buffers alternate, so one
+//          barrier per cfg separates its D from its hit rule and the next cfg's D from this one's hit rule
 //   hits   lane dg of the tile's own groups applies the local-minimum rule; each hit takes one atomic on the counter and
-//          leaves sample, stream and D in its record slot for coded_decode_kernel
+//          leaves sample, cfg index (`stream`), D and the capture index (in the reserved bytes) in its record slot for
+//          coded_decode_kernel
 constexpr int kCodedThreads = 128;
 constexpr int kCodedRows = kCodedThreads + 2;                              // staged IQ rows
 constexpr int kCodedPitch = 68;                                            // words per staged row (64 + 4 of padding)
 constexpr int kCodedDGroups = kCodedThreads - 11;                          // groups whose D is computed (117)
 constexpr int kCodedGroups = kCodedDGroups - 2;                            // window-start groups per CTA (115)
 constexpr int kCodedDPitch = 33;                                           // words of one group's 128 D bytes (+1 of padding)
+constexpr int kCodedDWords = kCodedDGroups * kCodedDPitch;                 // words of one D buffer
 constexpr int kCodedPreamble = 80, kCodedBlock1 = 296;                 // symbols of the preamble and of FEC block 1
 constexpr int kCodedMaxSteps = 16 + 8 * 255 + 27;                          // info bits of the longest block 2 (2083)
 constexpr int kCodedNeg = -(1 << 29);                                      // metric of a state not yet reachable
-constexpr size_t kCodedSmem = ((size_t)kCodedRows * kCodedPitch + 4 * (kCodedThreads + 1) + 12) * sizeof(uint32_t);
-static_assert(kCodedDGroups * kCodedDPitch <= kCodedRows * kCodedPitch, "D rows must fit in the freed IQ rows");
+constexpr size_t kCodedSmem = ((size_t)kCodedRows * kCodedPitch + 4 * (kCodedThreads + 1) + 11 * kMaxCfgsPerCapture) * sizeof(uint32_t);
+static_assert(2 * kCodedDWords <= kCodedRows * kCodedPitch, "two D buffers must fit in the freed IQ rows");
+static_assert(kMaxCfgsPerCapture <= kCodedThreads, "one lane per cfg builds the patterns");
 static_assert(sizeof(btle_coded_rec) == 304 && sizeof(btle_coded_rec) % 16 == 0, "coded record must be 304 bytes");
 
 // coded bits (a0, a1) of input bit b from state st = b[t-1] | b[t-2] << 1 | b[t-3] << 2 (G0 = 1 + x + x^2 + x^3, G1 = 1 + x^2 + x^3)
@@ -1552,15 +1559,23 @@ __device__ void coded_pattern(uint32_t aa, uint32_t *P /*11*/) {
   }
 }
 
+// D of sample (G0 - 1) * 128 + idx in a D buffer
+__device__ __forceinline__ int coded_d_at(const uint8_t *Db, int idx) {
+  return Db[4 * ((idx >> 7) * kCodedDPitch + ((idx & 127) >> 2)) + (idx & 3)];
+}
+
 __global__ void __launch_bounds__(kCodedThreads)
-coded_search_kernel(const int8_t *__restrict__ iq, long long stride, long long n_int8, long long tiles_per_stream,
-                    const StreamParams *__restrict__ params, const int4 *__restrict__ rot, btle_coded_rec *__restrict__ out,
-                    unsigned cap, unsigned *__restrict__ count) {
+coded_search_kernel(const int8_t *__restrict__ iq, long long stride, long long n_int8, long long tiles_per_group,
+                    const int4 *__restrict__ vmap, const StreamParams *__restrict__ params, const int4 *__restrict__ rot,
+                    btle_coded_rec *__restrict__ out, unsigned cap, unsigned *__restrict__ count) {
   extern __shared__ __align__(16) uint32_t coded_smem[];
   uint4 *pdw = reinterpret_cast<uint4 *>(coded_smem + kCodedRows * kCodedPitch);   // phase words of packed group p (+1 zero entry)
-  uint32_t *P = coded_smem + kCodedRows * kCodedPitch + 4 * (kCodedThreads + 1);
-  const long long stream = blockIdx.x / tiles_per_stream, tile = blockIdx.x - stream * tiles_per_stream;
-  const int8_t *cap_base = iq + stream * stride;
+  uint32_t *P = coded_smem + kCodedRows * kCodedPitch + 4 * (kCodedThreads + 1);  // 11 words per cfg of the group
+  const long long grp = blockIdx.x / tiles_per_group, tile = blockIdx.x - grp * tiles_per_group;
+  // {capture, first cfg, number of cfgs}; no vmap: cfg j on capture j, and the CTA's loads need not wait for one
+  const int4 vm = vmap ? __ldg(&vmap[grp]) : make_int4((int)grp, (int)grp, 1, 0);
+  const int capture = vm.x, first = vm.y, n_cfg = vm.z;
+  const int8_t *cap_base = iq + capture * stride;
   const long long G0 = tile * kCodedGroups;
   const long long row0 = (G0 - 5) * 256;                                   // first byte of staged row 0
   const bool interior = row0 >= 0 && row0 + kCodedRows * 256ll <= n_int8;
@@ -1576,14 +1591,12 @@ coded_search_kernel(const int8_t *__restrict__ iq, long long stride, long long n
       *reinterpret_cast<uint4 *>(dst) = make_uint4(v[0], v[1], v[2], v[3]);
     }
   }
-  if (threadIdx.x == 0) {
-    coded_pattern(__ldg(&params[stream].aa), P);
-    pdw[kCodedThreads] = make_uint4(0u, 0u, 0u, 0u);
-  }
+  if (threadIdx.x < n_cfg) coded_pattern(__ldg(&params[first + threadIdx.x].aa), P + 11 * threadIdx.x);
+  if (threadIdx.x == 0) pdw[kCodedThreads] = make_uint4(0u, 0u, 0u, 0u);
   asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
   __syncthreads();
   {
-    const int4 r = __ldg(&rot[stream]);
+    const int4 r = __ldg(&rot[first]);                                     // every cfg of a capture has its rotation
     const uint32_t *row = coded_smem + (threadIdx.x + 1) * kCodedPitch;
     auto word = [&](int k) -> uint32_t {
       return k < 0 ? row[k - kCodedPitch + 64] : k >= 64 ? row[kCodedPitch + k - 64] : row[k];
@@ -1593,71 +1606,71 @@ coded_search_kernel(const int8_t *__restrict__ iq, long long stride, long long n
     pdw[threadIdx.x] = make_uint4(acc[0], acc[1], acc[2], acc[3]);
   }
   __syncthreads();                                                          // the IQ rows are free: D goes there
-  uint8_t *Db = reinterpret_cast<uint8_t *>(coded_smem);
   const long long n_samples = n_int8 / 2, n0_hi = n_samples - 1024;       // D(n0) defined for 323 <= n0 <= n0_hi
   const int dg = threadIdx.x;
-  if (dg < kCodedDGroups) {
-    const long long g = G0 - 1 + dg;
-    uint32_t p[11];
+  const long long g = G0 - 1 + dg;
+  // the tile's own groups apply the hit rule (the halo groups only lend their D), where a window start is defined
+  const bool rule = dg >= 1 && dg <= kCodedGroups && 128 * g <= n0_hi && 128 * g + 127 >= 323;
+  for (int c = 0; c < n_cfg; ++c) {
+    uint8_t *Db = reinterpret_cast<uint8_t *>(coded_smem + (c & 1) * kCodedDWords);
+    if (dg < kCodedDGroups) {
+      uint32_t p[11];
 #pragma unroll
-    for (int k = 0; k < 11; ++k) p[k] = P[k];
-    p[10] &= 0xFFFFu;
+      for (int k = 0; k < 11; ++k) p[k] = P[11 * c + k];
+      p[10] &= 0xFFFFu;
 #pragma unroll
-    for (int ph = 0; ph < 4; ++ph) {
+      for (int ph = 0; ph < 4; ++ph) {
 #pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        uint32_t w[12];
+        for (int half = 0; half < 2; ++half) {
+          uint32_t w[12];
 #pragma unroll
-        for (int k = 0; k < 12; ++k) {
-          const uint4 v = pdw[dg + half + k];
-          w[k] = ph == 0 ? v.x : ph == 1 ? v.y : ph == 2 ? v.z : v.w;
-        }
-        for (int ii = 0; ii < 16; ++ii) {
-          const int i = 16 * half + ii;
-          const uint32_t sh = half ? ii : 16 + ii;                         // symbol m - 80 of window start m = 32 g + i
-          const long long n0 = 128 * g + 4 * i + ph;
-          int d = 255;
-          if (n0 >= 323 && n0 <= n0_hi) {
-            d = 0;
-#pragma unroll
-            for (int k = 0; k < 7; ++k) d += __popc(funnel_r(w[k], w[k + 1], sh) ^ p[k]);
-            if (d > BTLE_CODED_MAX_DIST) {
-              d = BTLE_CODED_MAX_DIST + 1;
-            } else {
-#pragma unroll
-              for (int k = 7; k < 10; ++k) d += __popc(funnel_r(w[k], w[k + 1], sh) ^ p[k]);
-              d += __popc((funnel_r(w[10], w[11], sh) & 0xFFFFu) ^ p[10]);
-              d = min(d, BTLE_CODED_MAX_DIST + 1);
-            }
+          for (int k = 0; k < 12; ++k) {
+            const uint4 v = pdw[dg + half + k];
+            w[k] = ph == 0 ? v.x : ph == 1 ? v.y : ph == 2 ? v.z : v.w;
           }
-          Db[4 * (dg * kCodedDPitch + i) + ph] = (uint8_t)d;
+          for (int ii = 0; ii < 16; ++ii) {
+            const int i = 16 * half + ii;
+            const uint32_t sh = half ? ii : 16 + ii;                       // symbol m - 80 of window start m = 32 g + i
+            const long long n0 = 128 * g + 4 * i + ph;
+            int d = 255;
+            if (n0 >= 323 && n0 <= n0_hi) {
+              d = 0;
+#pragma unroll
+              for (int k = 0; k < 7; ++k) d += __popc(funnel_r(w[k], w[k + 1], sh) ^ p[k]);
+              if (d > BTLE_CODED_MAX_DIST) {
+                d = BTLE_CODED_MAX_DIST + 1;
+              } else {
+#pragma unroll
+                for (int k = 7; k < 10; ++k) d += __popc(funnel_r(w[k], w[k + 1], sh) ^ p[k]);
+                d += __popc((funnel_r(w[10], w[11], sh) & 0xFFFFu) ^ p[10]);
+                d = min(d, BTLE_CODED_MAX_DIST + 1);
+              }
+            }
+            Db[4 * (dg * kCodedDPitch + i) + ph] = (uint8_t)d;
+          }
         }
       }
     }
-  }
-  __syncthreads();
-  if (dg < 1 || dg > kCodedGroups) return;                                 // the halo groups only lend their D
-  const long long g = G0 - 1 + dg;
-  if (128 * g > n0_hi || 128 * g + 127 < 323) return;
-  auto d_at = [&](int idx) -> int {                                         // D of sample (G0 - 1) * 128 + idx
-    return Db[4 * ((idx >> 7) * kCodedDPitch + ((idx & 127) >> 2)) + (idx & 3)];
-  };
-  for (int i = 0; i < 32; ++i) {
-    const uint32_t w4 = reinterpret_cast<const uint32_t *>(Db)[dg * kCodedDPitch + i];
-    uint32_t m = __vcmpleu4(w4, 0x60606060u);                              // bytes <= 96
-    while (m) {
-      const int ph = (__ffs((int)m) - 1) >> 3;
-      m &= ~(0xFFu << (8 * ph));
-      const int idx = 128 * dg + 4 * i + ph, d = (int)((w4 >> (8 * ph)) & 0xFFu);
-      bool hit = true;
-      for (int k = 1; k <= 8; ++k) hit = hit && d < d_at(idx - k) && d <= d_at(idx + k);
-      if (!hit) continue;
-      const unsigned slot = atomicAdd(count, 1u);
-      if (slot < cap) {
-        btle_coded_rec *r = out + slot;
-        r->sample = 128 * g + 4 * i + ph;
-        r->stream = (int32_t)stream;
-        r->dist = d;
+    __syncthreads();                     // D of cfg c is complete; cfg c + 1 writes the other buffer meanwhile
+    if (!rule) continue;
+    for (int i = 0; i < 32; ++i) {
+      const uint32_t w4 = reinterpret_cast<const uint32_t *>(Db)[dg * kCodedDPitch + i];
+      uint32_t m = __vcmpleu4(w4, 0x60606060u);                            // bytes <= 96
+      while (m) {
+        const int ph = (__ffs((int)m) - 1) >> 3;
+        m &= ~(0xFFu << (8 * ph));
+        const int idx = 128 * dg + 4 * i + ph, d = (int)((w4 >> (8 * ph)) & 0xFFu);
+        bool hit = true;
+        for (int k = 1; k <= 8; ++k) hit = hit && d < coded_d_at(Db, idx - k) && d <= coded_d_at(Db, idx + k);
+        if (!hit) continue;
+        const unsigned slot = atomicAdd(count, 1u);
+        if (slot < cap) {
+          btle_coded_rec *r = out + slot;
+          r->sample = 128 * g + 4 * i + ph;
+          r->stream = first + c;
+          r->dist = d;
+          *reinterpret_cast<int32_t *>(r->reserved) = vmap ? __ldg(&vmap[grp].x) : (int)grp;   // cleared by coded_decode_kernel
+        }
       }
     }
   }
@@ -1667,7 +1680,8 @@ coded_search_kernel(const int8_t *__restrict__ iq, long long stride, long long n
 // build the soft values of 32 trellis steps at once from the IQ (coalesced), then the 8 ACS lanes (state = lane & 7)
 // run those steps with two shuffles each; each step's 8 decisions are one byte of the warp's survivor rows.  The header
 // pass is the first 40 steps of the same trellis.  Lane 0 traces back, the lanes pack and dewhiten the bytes, lane 0
-// runs the CRC.
+// runs the CRC.  A hit's cfg (`stream`) gives the parameters and the rotation, its capture (left in the reserved bytes by
+// coded_search_kernel) the IQ.
 constexpr int kCodedDecWarps = 4;
 struct CodedWarp {
   uint8_t surv[kCodedMaxSteps + 13];                                        // decisions of step t: bit s = state s took p | 4
@@ -1751,11 +1765,11 @@ coded_decode_kernel(const int8_t *__restrict__ iq, long long stride, long long n
   for (unsigned k = blockIdx.x * kCodedDecWarps + (threadIdx.x >> 5); k < n; k += gridDim.x * kCodedDecWarps) {
     btle_coded_rec *rec = out + k;
     const long long n0 = rec->sample;
-    const int stream = rec->stream, dist = rec->dist;
+    const int stream = rec->stream, dist = rec->dist, capture = *reinterpret_cast<const int32_t *>(rec->reserved);
     __syncwarp();
     const StreamParams &sp = params[stream];
     const int4 r = __ldg(&rot[stream]);
-    const CodedIq X{iq + stream * stride, n_int8 / 2, r.z, r.w};
+    const CodedIq X{iq + capture * stride, n_int8 / 2, r.z, r.w};
     const uint32_t aa = __ldg(&sp.aa);
     const int channel = __ldg(&sp.channel);
     if (lane == 0) {
@@ -3172,52 +3186,62 @@ int launch_discover(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, si
   return BTLE_OK;
 }
 
-// The cfgs of the coded receiver (include/btle_b200.h, btle_b200_rx_coded_device) and the rotation of each capture
-int check_coded(btle_b200_ctx *ctx, const btle_stream_cfg *cfgs, size_t n_streams, const float *offset_hz, std::vector<int4> &rot) {
-  if (!cfgs && n_streams) { ctx->err = "rx_coded: missing cfg array"; return BTLE_EINVAL; }
-  for (size_t s = 0; s < n_streams; ++s) {
+// The cfgs of the coded receiver (include/btle_b200.h, btle_b200_rx_coded_multi_device): cfg j decodes capture
+// cfg_capture[j] (check_cfg_capture's rules); rot[j] = the rotation of that capture's offset
+int check_coded(btle_b200_ctx *ctx, size_t n_captures, const btle_stream_cfg *cfgs, const int32_t *cfg_capture, size_t n_cfgs,
+                const float *offset_hz, std::vector<int4> &rot) {
+  if ((!cfgs || !cfg_capture) && n_cfgs) { ctx->err = "rx_coded: missing cfg array"; return BTLE_EINVAL; }
+  for (size_t s = 0; s < n_cfgs; ++s) {
     const btle_stream_cfg &c = cfgs[s];
     if (c.channel < 0 || c.channel > 39) { ctx->err = "rx_coded: channel must be within 0~39"; return BTLE_EINVAL; }
     if (c.raw) { ctx->err = "rx_coded: raw mode has no coded form"; return BTLE_EINVAL; }
     if (c.access_mask != 0xFFFFFFFFu) { ctx->err = "rx_coded: access_mask must be 0xFFFFFFFF"; return BTLE_EINVAL; }
     if (c.rssi & ~BTLE_CFG_RSSI) { ctx->err = "rx_coded: the only flag is BTLE_CFG_RSSI"; return BTLE_EINVAL; }
   }
-  std::vector<float> hz(n_streams, 0.0f);
-  if (offset_hz) {
-    const int rc = cfg_offsets(ctx, offset_hz, n_streams, nullptr, n_streams, hz);
-    if (rc) return rc;
-  }
-  rot.resize(n_streams);
-  for (size_t s = 0; s < n_streams; ++s) rot[s] = make_rot(hz[s]);
+  size_t groups = 0;
+  int rc = check_cfg_capture(ctx, n_captures, cfg_capture, n_cfgs, &groups);
+  if (rc) return rc;
+  std::vector<float> hz(n_cfgs, 0.0f);
+  if (offset_hz && (rc = cfg_offsets(ctx, offset_hz, n_captures, cfg_capture, n_cfgs, hz))) return rc;
+  rot.resize(n_cfgs);
+  for (size_t s = 0; s < n_cfgs; ++s) rot[s] = make_rot(hz[s]);
   return BTLE_OK;
 }
 
-// coded_search_kernel, then coded_decode_kernel over the hits it counted, both on `st` (the counter is zeroed here).  The
-// hits wait in d_out's slots between the two kernels, so there is no other scratch, and no hit goes unseen: *d_count is
-// the number found, whatever cap is.
-int launch_coded(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8, const btle_stream_cfg *cfgs,
-                 const std::vector<int4> &rot, btle_coded_rec *d_out, size_t cap, unsigned *d_count, cudaStream_t st) {
-  if (!d_count || (!d_out && cap) || (!d_iq && n_streams && n_int8)) { ctx->err = "rx_coded: missing buffer"; return BTLE_EINVAL; }
-  if ((reinterpret_cast<uintptr_t>(d_iq) & 15) || (n_streams > 1 && (stride & 15))) { ctx->err = "device IQ must be 16-byte aligned"; return BTLE_EINVAL; }
+// coded_search_kernel over the capture groups of the cfg list (each tile of a capture staged once for all its cfgs), then
+// coded_decode_kernel over the hits it counted, both on `st` (the counter is zeroed here).  The hits wait in d_out's
+// slots between the two kernels, so there is no other scratch, and no hit goes unseen: *d_count is the number found,
+// whatever cap is.  cfgs, cfg_capture and rot as check_coded left them.
+int launch_coded(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_captures, size_t stride, size_t n_int8, const btle_stream_cfg *cfgs,
+                 const int32_t *cfg_capture, size_t n_cfgs, const std::vector<int4> &rot, btle_coded_rec *d_out, size_t cap,
+                 unsigned *d_count, cudaStream_t st) {
+  if (!d_count || (!d_out && cap) || (!d_iq && n_captures && n_int8)) { ctx->err = "rx_coded: missing buffer"; return BTLE_EINVAL; }
+  if ((reinterpret_cast<uintptr_t>(d_iq) & 15) || (n_captures > 1 && (stride & 15))) { ctx->err = "device IQ must be 16-byte aligned"; return BTLE_EINVAL; }
   if (reinterpret_cast<uintptr_t>(d_out) & 15) { ctx->err = "rx_coded: d_out must be 16-byte aligned"; return BTLE_EINVAL; }
-  if (n_streams > 1 && stride < n_int8) { ctx->err = "stream stride smaller than stream length"; return BTLE_EINVAL; }
+  if (n_captures > 1 && stride < n_int8) { ctx->err = "stream stride smaller than stream length"; return BTLE_EINVAL; }
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
   ctx->last_launches = 0;
   BTLE_CUDA(ctx, cudaMemsetAsync(d_count, 0, sizeof(unsigned), st));
   const long long n_samples = (long long)(n_int8 / 2);
-  if (!n_streams || n_samples < 323 + 1024) return BTLE_OK;                // no window fits
+  if (!n_cfgs || n_samples < 323 + 1024) return BTLE_OK;                   // no window fits
   const long long groups = (n_samples - 1024) / 128 + 1;                   // groups holding a window start inside the capture
   const long long tiles = (groups + kCodedGroups - 1) / kCodedGroups;
-  if (tiles * (long long)n_streams > 0x7FFFFFFFll) { ctx->err = "batch too large for one launch"; return BTLE_EINVAL; }
+  size_t n_vmap = 0;
+  bool identity = n_cfgs == n_captures;                                    // cfg j on capture j: the kernel reads no vmap
+  for (size_t j = 0; j < n_cfgs; ++j) {
+    n_vmap += new_group(cfg_capture, rot.data(), j);
+    identity = identity && cfg_capture[j] == (int32_t)j;
+  }
+  if (tiles * (long long)n_vmap > 0x7FFFFFFFll) { ctx->err = "batch too large for one launch"; return BTLE_EINVAL; }
   unsigned long long sid = 0;
   int rc = stream_id(ctx, st, &sid);
   if (rc) return rc;
   CfgSlot *cs = nullptr;
-  rc = upload_cfgs(ctx, cfgs, n_streams, st, sid, &cs, nullptr, rot.data());
+  rc = upload_cfgs(ctx, cfgs, n_cfgs, st, sid, &cs, cfg_capture, rot.data());
   if (rc) return rc;
   const unsigned cap32 = (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu);
-  coded_search_kernel<<<(unsigned)(tiles * (long long)n_streams), kCodedThreads, kCodedSmem, st>>>(
-      d_iq, (long long)stride, (long long)n_int8, tiles, cs->d_params, cs->d_rot, d_out, cap32, d_count);
+  coded_search_kernel<<<(unsigned)(tiles * (long long)cs->n_vmap), kCodedThreads, kCodedSmem, st>>>(
+      d_iq, (long long)stride, (long long)n_int8, tiles, identity ? nullptr : cs->d_vmap.p, cs->d_params, cs->d_rot, d_out, cap32, d_count);
   BTLE_CUDA(ctx, cudaGetLastError());
   if (cap32) {
     const unsigned grid = (unsigned)std::min<long long>((cap32 + kCodedDecWarps - 1) / kCodedDecWarps, 16ll * ctx->num_sms);
@@ -3229,6 +3253,13 @@ int launch_coded(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_
   if (rc) return rc;
   ctx->last_launches = cap32 ? 2 : 1;
   return BTLE_OK;
+}
+
+// One cfg per capture: the cfg list j -> capture j
+std::vector<int32_t> identity_capture(size_t n) {
+  std::vector<int32_t> cc(n);
+  for (size_t j = 0; j < n; ++j) cc[j] = (int32_t)j;
+  return cc;
 }
 
 }  // namespace
@@ -4376,33 +4407,41 @@ int btle_b200_discover(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, s
   return BTLE_OK;
 }
 
-int btle_b200_rx_coded_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8,
-                              const btle_stream_cfg *cfgs, const float *offset_hz, btle_coded_rec *d_out, size_t cap,
-                              uint32_t *d_count, void *cuda_stream) {
+int btle_b200_rx_coded_multi_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_captures, size_t stride, size_t n_int8,
+                                    const btle_stream_cfg *cfgs, const int32_t *cfg_capture, size_t n_cfgs, const float *offset_hz,
+                                    btle_coded_rec *d_out, size_t cap, uint32_t *d_count, void *cuda_stream) {
   if (!ctx) return BTLE_EINVAL;
   std::vector<int4> rot;
-  const int rc = check_coded(ctx, cfgs, n_streams, offset_hz, rot);
+  const int rc = check_coded(ctx, n_captures, cfgs, cfg_capture, n_cfgs, offset_hz, rot);
   if (rc) return rc;
-  return launch_coded(ctx, d_iq, n_streams, stride, n_int8, cfgs, rot, d_out, cap, d_count, reinterpret_cast<cudaStream_t>(cuda_stream));
+  return launch_coded(ctx, d_iq, n_captures, stride, n_int8, cfgs, cfg_capture, n_cfgs, rot, d_out, cap, d_count,
+                      reinterpret_cast<cudaStream_t>(cuda_stream));
 }
 
-// The records land unordered in ctx->d_coded[0], are put in (stream, sample) order into ctx->d_coded[1] on the device
-// (coded_rank_kernel) and copied out.
-int btle_b200_rx_coded(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stride, size_t n_int8, const btle_stream_cfg *cfgs,
-                       const float *offset_hz, btle_coded_rec *out, size_t cap, size_t *n_out) {
+// Only the captures some cfg reads are copied, one after the other, and the list is renumbered to match.  The records
+// land unordered in ctx->d_coded[0], are put in (cfg, sample) order into ctx->d_coded[1] on the device (coded_rank_kernel)
+// and copied out.
+int btle_b200_rx_coded_multi(btle_b200_ctx *ctx, const int8_t *iq, size_t n_captures, size_t stride, size_t n_int8,
+                             const btle_stream_cfg *cfgs, const int32_t *cfg_capture, size_t n_cfgs, const float *offset_hz,
+                             btle_coded_rec *out, size_t cap, size_t *n_out) {
   if (!ctx) return BTLE_EINVAL;
-  if (!n_out || (!out && cap) || (!iq && n_streams && n_int8)) { ctx->err = "rx_coded: missing buffer"; return BTLE_EINVAL; }
+  if (!n_out || (!out && cap) || (!iq && n_captures && n_int8)) { ctx->err = "rx_coded: missing buffer"; return BTLE_EINVAL; }
   *n_out = 0;
   std::vector<int4> rot;
-  int rc = check_coded(ctx, cfgs, n_streams, offset_hz, rot);               // before any byte is copied
+  int rc = check_coded(ctx, n_captures, cfgs, cfg_capture, n_cfgs, offset_hz, rot);   // before any byte is copied
   if (rc) return rc;
   BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
+  std::vector<int32_t> caps, local;                          // the captures read, in order; cfg j reads caps[local[j]]
+  for (size_t j = 0; j < n_cfgs; ++j) {
+    if (!j || cfg_capture[j] != cfg_capture[j - 1]) caps.push_back(cfg_capture[j]);
+    local.push_back((int32_t)caps.size() - 1);
+  }
   size_t pitch = 0;
-  rc = ingest(ctx, iq, n_streams, stride, n_int8, nullptr, n_streams, &pitch);
+  rc = ingest(ctx, iq, n_captures, stride, n_int8, caps.data(), caps.size(), &pitch);
   if (rc) return rc;
   if (ctx->d_coded[0].reserve(ctx, std::max<size_t>(cap, 1)) || ctx->d_coded[1].reserve(ctx, std::max<size_t>(cap, 1))) return BTLE_ENOMEM;
-  rc = launch_coded(ctx, ctx->d_iq, n_streams, pitch, n_int8, cfgs, rot, ctx->d_coded[0], cap, ctx->d_count, st);
+  rc = launch_coded(ctx, ctx->d_iq, caps.size(), pitch, n_int8, cfgs, local.data(), n_cfgs, rot, ctx->d_coded[0], cap, ctx->d_count, st);
   if (rc) return rc;
   rc = fetch_counted(ctx, st, cap, n_out, [&](size_t n) {
     coded_rank_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ctx->d_coded[0], (unsigned)n, ctx->d_coded[1]);
@@ -4413,6 +4452,19 @@ int btle_b200_rx_coded(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, s
   if (rc) return rc;
   if (*n_out > cap) { ctx->err = "output capacity too small"; return BTLE_EOVERFLOW; }
   return BTLE_OK;
+}
+
+int btle_b200_rx_coded_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8,
+                              const btle_stream_cfg *cfgs, const float *offset_hz, btle_coded_rec *d_out, size_t cap,
+                              uint32_t *d_count, void *cuda_stream) {
+  return btle_b200_rx_coded_multi_device(ctx, d_iq, n_streams, stride, n_int8, cfgs, identity_capture(n_streams).data(), n_streams,
+                                         offset_hz, d_out, cap, d_count, cuda_stream);
+}
+
+int btle_b200_rx_coded(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stride, size_t n_int8, const btle_stream_cfg *cfgs,
+                       const float *offset_hz, btle_coded_rec *out, size_t cap, size_t *n_out) {
+  return btle_b200_rx_coded_multi(ctx, iq, n_streams, stride, n_int8, cfgs, identity_capture(n_streams).data(), n_streams, offset_hz, out,
+                                  cap, n_out);
 }
 
 // Streaming form of the Python model's receiver over an 8-Msps interleaved int16 capture (see include/btle_b200.h).

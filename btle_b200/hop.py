@@ -33,14 +33,9 @@ def record_time(rec) -> float:
     return (int(rec["chunk"]) * 8192 + int(rec["n0"])) / SAMPLE_RATE
 
 
-def parse_connect_req(rec):
-    """Fields the reference keeps in `receiver_status` (btle_rx.c:1683-1698), or None."""
-    b = rec["bytes"]
-    if rec["crc_bad"] or (b[0] & 0x0F) != 5 or (b[1] & 0x3F) != 34:
-        return None
-    p = bytes(b[2:36])
+def _ll_data_fields(p: bytes) -> dict:
+    """The 34-byte payload of a CONNECT_IND / AUX_CONNECT_REQ (InitA, AdvA, LLData) as the reference reads it."""
     return {
-        "t": record_time(rec), "adv_channel": int(rec["channel"]),
         "init_a": p[0:6][::-1].hex(), "adv_a": p[6:12][::-1].hex(),
         "access_addr": int.from_bytes(p[12:16], "little"),
         "crc_init": (p[16] << 16) | (p[17] << 8) | p[18],          # as the reference reads it, :1637-1639
@@ -49,6 +44,49 @@ def parse_connect_req(rec):
         "timeout": int.from_bytes(p[26:28], "little"), "chm": p[28:33][::-1].hex(),
         "hop": p[33] & 0x1F, "sca": (p[33] >> 5) & 7,
     }
+
+
+def parse_connect_req(rec):
+    """Fields the reference keeps in `receiver_status` (btle_rx.c:1683-1698), or None."""
+    b = rec["bytes"]
+    if rec["crc_bad"] or (b[0] & 0x0F) != 5 or (b[1] & 0x3F) != 34:
+        return None
+    return {"t": record_time(rec), "adv_channel": int(rec["channel"]), **_ll_data_fields(bytes(b[2:36]))}
+
+
+AUX_CONNECT_REQ = 5          # PDU type of AUX_CONNECT_REQ on a secondary advertising channel (Core Spec Vol 6 Part B §2.3)
+
+
+def parse_aux_connect_req(rec):
+    """An LE Coded PHY record (CODED_REC_DTYPE) of an AUX_CONNECT_REQ -> parse_connect_req()'s fields plus "aux": True, or
+    None.  AUX_CONNECT_REQ carries the same InitA, AdvA and LLData as CONNECT_IND (Core Spec Vol 6 Part B §2.3.3.2); its
+    length field is 8 bits.  `t` is the record's sample / 4 Msps and `adv_channel` the secondary channel it came on."""
+    b = rec["bytes"]
+    if rec["crc_bad"] or (b[0] & 0x0F) != AUX_CONNECT_REQ or b[1] != 34:
+        return None
+    return {"t": int(rec["sample"]) / SAMPLE_RATE, "adv_channel": int(rec["channel"]), **_ll_data_fields(bytes(b[2:36])), "aux": True}
+
+
+def new_connections(conns, found):
+    """found without the connections whose (access address, CRC init) is already in conns or earlier in found."""
+    seen = {(c["access_addr"], c["crc_init"]) for c in conns}
+    out = []
+    for c in found:
+        key = (c["access_addr"], c["crc_init"])
+        if key not in seen:
+            seen.add(key)
+            out.append(c)
+    return out
+
+
+def connection_cfgs(batch, **flags):
+    """The cfgs and capture list of one several-cfgs-per-capture call over the data captures 0..36 for up to
+    MAX_CFGS_PER_CAPTURE connections: cfg j = channel * k + i is connection i on data channel j // k (the cfgs of one
+    capture are adjacent), so a record's connection is stream % k.  flags: make_cfgs() keywords for every cfg."""
+    k = len(batch)
+    cfgs = make_cfgs(37 * k, channel=np.repeat(np.arange(37), k), access_addr=[c["access_addr"] for c in batch] * 37,
+                     crc_init=[c["crc_init"] for c in batch] * 37, **flags)
+    return cfgs, np.repeat(np.arange(37, dtype=np.int32), k)
 
 
 def _walk_events(c, per_ch, n_samples, max_events=10000, first_channel=None):
@@ -266,9 +304,11 @@ def follow_connections(rx, captures: np.ndarray, max_events: int = 10000, discov
 
 
 def decode_connections(rx, captures: np.ndarray, discover: bool = True, offset_hz=None, symbol_spaced: bool = False,
-                       centre_hits: bool = False, correct: bool = False, lowpass: bool = False, offset_search: bool = False):
+                       centre_hits: bool = False, correct: bool = False, lowpass: bool = False, offset_search: bool = False,
+                       coded: bool = False):
     """Every known connection's data-channel traffic, decoded without following it.  captures: int8 [40, n_int8] as in
-    follow_connections(); `rx` needs rx_batch, rx_multi and, with discover=True, discover (a BtleRx).
+    follow_connections(); `rx` needs rx_batch, rx_multi, with discover=True discover, and with coded=True rx_coded and
+    rx_coded_multi (a BtleRx).
     The connections are the CONNECT_REQ ones (tracked or not) plus, with discover=True, the discover_connections() ones
     whose access address no CONNECT_REQ announced (tracked or not: a partial channel map or CSA#2 does not matter here).
     With all 37 data channels captured, a connection's packets are found by its access address and CRC init alone, so
@@ -282,8 +322,17 @@ def decode_connections(rx, captures: np.ndarray, discover: bool = True, offset_h
     receive cfg of those calls carries BTLE_CFG_CORRECT (one-bit and adjacent-pair errors corrected from the CRC
     syndrome); lowpass: every receive cfg of those calls carries BTLE_CFG_LOWPASS (the symbol-spaced bits of [1, 2, 1]
     filtered samples; only with symbol_spaced); offset_search: every receive cfg of those calls carries BTLE_CFG_OFFSET_SEARCH
-    (seven carrier-offset hypotheses per capture, merged per packet); discovery keeps its own rule.  Returns (adv_records,
-    connections)."""
+    (seven carrier-offset hypotheses per capture, merged per packet); discovery keeps its own rule.
+    coded=True adds the LE Coded PHY, in 1 + ceil(connections / MAX_CFGS_PER_CAPTURE) more launches:
+      - one rx_coded over captures[0:37] with the advertising access address and CRC init on each capture's channel: its
+        CRC-ok AUX_CONNECT_REQs (parse_aux_connect_req) become connections with "aux": True and `tracked` False (they use
+        CSA#2), after those whose (access address, CRC init) is already known;
+      - one rx_coded_multi per MAX_CFGS_PER_CAPTURE connections (every connection, AUX_CONNECT_REQ ones included) over
+        captures[0:37], cfgs laid out as for rx_multi: each connection gets `coded_traffic`, its coded records (stream =
+        channel) in (sample, channel) order.  So a 1M connection that moved to the coded PHY is covered too.
+    offset_hz is passed to the coded calls as well; the 1M opt-in flags are not (the coded receiver has none).  AUX_CONNECT_REQ
+    connections get `traffic` like every other one.  With coded=False the result is what it was without the argument.
+    Returns (adv_records, connections)."""
     from ._native import MAX_CFGS_PER_CAPTURE
     captures = np.ascontiguousarray(captures, dtype=np.int8)
     assert captures.shape[0] == 40
@@ -291,9 +340,8 @@ def decode_connections(rx, captures: np.ndarray, discover: bool = True, offset_h
     off = None if offset_hz is None else np.broadcast_to(np.asarray(offset_hz, dtype=np.float32), (40,))
     adv_kw = {} if off is None else {"offset_hz": off[37:40]}
     data_kw = {} if off is None else {"offset_hz": off[0:37]}
-    adv = rx.rx_batch(captures[37:40], make_cfgs(3, channel=[37, 38, 39], symbol_spaced=symbol_spaced, centre_hits=centre_hits,
-                                                correct=correct, lowpass=lowpass, offset_search=offset_search),
-                      **adv_kw).copy()
+    flags = dict(symbol_spaced=symbol_spaced, centre_hits=centre_hits, correct=correct, lowpass=lowpass, offset_search=offset_search)
+    adv = rx.rx_batch(captures[37:40], make_cfgs(3, channel=[37, 38, 39], **flags), **adv_kw).copy()
     adv["stream"] += 37
     conns = []
     for r in adv:
@@ -305,15 +353,18 @@ def decode_connections(rx, captures: np.ndarray, discover: bool = True, offset_h
     if discover:
         announced = {c["access_addr"] for c in conns}
         conns += [c for c in discover_connections(rx, captures) if c["access_addr"] not in announced]
+    if coded:
+        sec = rx.rx_coded(captures[0:37], make_cfgs(37, channel=list(range(37))), **data_kw)
+        aux = [c for c in (parse_aux_connect_req(r) for r in sec) if c is not None]
+        for c in aux:
+            c["tracked"] = False
+        conns += new_connections(conns, aux)
     K = MAX_CFGS_PER_CAPTURE
     for b0 in range(0, len(conns), K):
         batch = conns[b0:b0 + K]
         k = len(batch)
-        # cfg j = channel * k + i: connection i on data channel j // k (the cfgs of one capture are adjacent)
-        cfgs = make_cfgs(37 * k, channel=np.repeat(np.arange(37), k), access_addr=[c["access_addr"] for c in batch] * 37,
-                         crc_init=[c["crc_init"] for c in batch] * 37, symbol_spaced=symbol_spaced, centre_hits=centre_hits,
-                         correct=correct, lowpass=lowpass, offset_search=offset_search)
-        rec = rx.rx_multi(captures[0:37], cfgs, np.repeat(np.arange(37, dtype=np.int32), k), **data_kw)
+        cfgs, capture = connection_cfgs(batch, **flags)
+        rec = rx.rx_multi(captures[0:37], cfgs, capture, **data_kw)
         owner = rec["stream"] % k
         t = rec["chunk"].astype(np.int64) * 8192 + rec["n0"]
         for i, c in enumerate(batch):
@@ -322,6 +373,18 @@ def decode_connections(rx, captures: np.ndarray, discover: bool = True, offset_h
             tr = mine[np.lexsort((mine["channel"], tm))].copy()
             tr["stream"] = tr["channel"]                 # the capture row, as in follow_connections()
             c["traffic"] = tr
+    if coded:
+        for b0 in range(0, len(conns), K):
+            batch = conns[b0:b0 + K]
+            k = len(batch)
+            cfgs, capture = connection_cfgs(batch)
+            rec = rx.rx_coded_multi(captures[0:37], cfgs, capture, **data_kw)
+            owner = rec["stream"] % k
+            for i, c in enumerate(batch):
+                mine = rec[owner == i]
+                tr = mine[np.lexsort((mine["channel"], mine["sample"]))].copy()
+                tr["stream"] = tr["channel"]
+                c["coded_traffic"] = tr
     return adv, conns
 
 

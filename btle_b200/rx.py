@@ -273,6 +273,37 @@ class BtleRx:
                                                d_out.data_ptr(), cap, d_count.data_ptr(), ctypes.c_void_p(stream_ptr))
         self._check(rc)
 
+    def rx_coded_multi(self, iq: np.ndarray, cfgs: np.ndarray, capture, offset_hz=None, cap: int | None = None) -> np.ndarray:
+        """Several LE Coded PHY cfgs per capture in one read of the IQ (btle_b200_rx_coded_multi): iq int8 [n_captures,
+        n_int8] (or [n_int8]); cfgs CFG_DTYPE [n_cfgs]; capture[j] = the capture cfg j decodes (non-decreasing, at most
+        MAX_CFGS_PER_CAPTURE per capture).  Returns what rx_coded() returns on iq[capture] with cfgs: records with stream =
+        cfg index, in (cfg, sample) order.  offset_hz: a scalar or one per capture.  `cap` as rx_coded()."""
+        iq = np.ascontiguousarray(iq, dtype=np.int8)
+        if iq.ndim == 1:
+            iq = iq[None, :]
+        ns, n = iq.shape
+        cfgs = np.ascontiguousarray(cfgs, dtype=CFG_DTYPE).reshape(-1)
+        cc = np.ascontiguousarray(capture, dtype=np.int32).reshape(-1)
+        assert cc.shape == cfgs.shape
+        off = _offsets(offset_hz, ns)
+        call = partial(self._L.btle_b200_rx_coded_multi, self._h, iq.ctypes.data, ns, n, n, cfgs.ctypes.data, cc.ctypes.data, cfgs.size,
+                       _ptr(off))
+        return self._grow_once(call, CODED_REC_DTYPE, cfgs.size * (n // 65536 + 1) * 4 + 64 if cap is None else cap, grow=cap is None)
+
+    def rx_coded_multi_device(self, d_iq, cfgs: np.ndarray, capture, d_out, d_count, stream_ptr: int = 0, offset_hz=None):
+        """rx_coded_multi on device-resident captures, buffers as rx_coded_device: d_iq torch int8 CUDA tensor [n_captures,
+        n_int8] (16-byte aligned rows).  Records land unordered in d_out[:min(count, cap)], `stream` = cfg index."""
+        ns, n = d_iq.shape
+        assert d_iq.stride(1) == 1
+        cfgs = np.ascontiguousarray(cfgs, dtype=CFG_DTYPE).reshape(-1)
+        cc = np.ascontiguousarray(capture, dtype=np.int32).reshape(-1)
+        assert cc.shape == cfgs.shape
+        off = _offsets(offset_hz, ns)
+        cap = d_out.numel() * d_out.element_size() // CODED_REC_DTYPE.itemsize
+        self._check(self._L.btle_b200_rx_coded_multi_device(self._h, d_iq.data_ptr(), ns, d_iq.stride(0), n, cfgs.ctypes.data, cc.ctypes.data,
+                                                            cfgs.size, _ptr(off), d_out.data_ptr(), cap, d_count.data_ptr(),
+                                                            ctypes.c_void_p(stream_ptr)))
+
     # ---- unbounded capture, pushed in pieces (btle_b200_stream_*) -----------------------------
     def stream(self, segment_chunks: int = 0, **cfg) -> "RxStream":
         """Streaming session over one capture of any length: `with rx.stream(channel=37) as s: recs = s.push(iq_piece) ...;

@@ -539,6 +539,22 @@ int btle_b200_rx_coded_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_s
  * with cap >= *n_out returns them all. */
 int btle_b200_rx_coded(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stream_stride_int8, size_t n_int8,
                        const btle_stream_cfg *cfgs, const float *offset_hz, btle_coded_rec *out, size_t cap, size_t *n_out);
+/* Several cfgs per capture, each capture read once (as btle_b200_rx_multi for 1M): cfg j decodes capture cfg_capture[j]
+ * (non-decreasing, in range, at most BTLE_MAX_CFGS_PER_CAPTURE cfgs per capture; captures no cfg names are not read).
+ * offset_hz (host array, NULL = 0) has one entry per capture, shared by all cfgs of that capture.  The result equals
+ * btle_b200_rx_coded on a batch whose stream j is a copy of capture cfg_capture[j], decoded with cfgs[j] and
+ * offset_hz[cfg_capture[j]]: every field of every record is equal, and `stream` is the cfg index j.  The device form
+ * returns the records unordered with the exact count in *d_count, as btle_b200_rx_coded_device; the host form copies
+ * only the captures some cfg names and returns the records in (j, sample) order, BTLE_EOVERFLOW with the exact count as
+ * btle_b200_rx_coded.  Each cfg is checked as in btle_b200_rx_coded_device, and a bad cfg_capture is BTLE_EINVAL too.
+ * btle_b200_rx_coded and _rx_coded_device are these calls with cfg_capture[j] = j. */
+int btle_b200_rx_coded_multi(btle_b200_ctx *ctx, const int8_t *iq, size_t n_captures, size_t stream_stride_int8, size_t n_int8,
+                             const btle_stream_cfg *cfgs, const int32_t *cfg_capture, size_t n_cfgs, const float *offset_hz,
+                             btle_coded_rec *out, size_t cap, size_t *n_out);
+int btle_b200_rx_coded_multi_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_captures, size_t stream_stride_int8,
+                                    size_t n_int8, const btle_stream_cfg *cfgs, const int32_t *cfg_capture, size_t n_cfgs,
+                                    const float *offset_hz, btle_coded_rec *d_out, size_t cap, uint32_t *d_count,
+                                    void *cuda_stream);
 
 /* ---- connections on a streaming session (btle_b200_streams_*): per-capture cfg lists, backfill, discovery -----------
  * Every cfg of a session has a stable index, never reused: the n_streams cfgs of btle_b200_streams_open are 0..n-1 (cfg
