@@ -58,6 +58,10 @@ CODED_REC_DTYPE = np.dtype([("sample", "<i8"), ("stream", "<i4"), ("access_addr"
                             ("mag_sum", "<u4"), ("bytes", "u1", CODED_MAX_BYTES), ("reserved", "u1", 8)])
 assert CODED_REC_DTYPE.itemsize == 304
 CODED_MAX_DIST = 96                           # BTLE_CODED_MAX_DIST
+# btle_coded_cand, 32 bytes: an empty coded PDU candidate of coded connection discovery (first 23 bytes as CAND_DTYPE)
+CODED_CAND_DTYPE = np.dtype([("sample", "<i8"), ("stream", "<i4"), ("access_addr", "<u4"), ("crc_init", "<u4"), ("channel", "u1"),
+                             ("header", "u1", 2), ("s", "u1"), ("dist", "<i2"), ("shift", "i1"), ("reserved", "u1"), ("metric", "<i4")])
+assert CODED_CAND_DTYPE.itemsize == 32
 CODED_CI_RESERVED, CODED_TRUNCATED = 1, 2     # btle_coded_rec.flags bits
 assert REC_DTYPE.itemsize == 64 and CFG_DTYPE.itemsize == 24 and MODEL_REC_DTYPE.itemsize == 80 and SPS8_REC_DTYPE.itemsize == 96
 
@@ -82,7 +86,7 @@ EXPORTS = [
     "btle_b200_streams_take_cands", "btle_b200_rx_batch_offset", "btle_b200_rx_device_dir_offset", "btle_b200_rx_multi_offset",
     "btle_b200_rx_multi_device_dir_offset", "btle_b200_rec_offset_device", "btle_b200_rec_offset",
     "btle_b200_streams_set_offset", "btle_b200_stream_set_offset", "btle_b200_rx_coded", "btle_b200_rx_coded_device",
-    "btle_b200_rx_coded_multi", "btle_b200_rx_coded_multi_device",
+    "btle_b200_rx_coded_multi", "btle_b200_rx_coded_multi_device", "btle_b200_discover_coded", "btle_b200_discover_coded_device",
 ]
 MAX_CFGS_PER_CAPTURE = 8       # BTLE_MAX_CFGS_PER_CAPTURE
 CFG_RSSI, CFG_REPORT_REJECTED, CFG_RECOVER = 1, 2, 4      # btle_stream_cfg.rssi flag bits (BTLE_CFG_*)
@@ -204,6 +208,8 @@ def load():
     L.btle_b200_rx_coded_device.argtypes = [vp, vp, sz, sz, sz, vp, vp, vp, sz, vp, vp]
     L.btle_b200_rx_coded_multi.argtypes = [vp, vp, sz, sz, sz, vp, vp, sz, vp, vp, sz, ctypes.POINTER(sz)]
     L.btle_b200_rx_coded_multi_device.argtypes = [vp, vp, sz, sz, sz, vp, vp, sz, vp, vp, sz, vp, vp]
+    L.btle_b200_discover_coded.argtypes = [vp, vp, sz, sz, sz, vp, vp, vp, sz, ctypes.POINTER(sz)]
+    L.btle_b200_discover_coded_device.argtypes = [vp, vp, sz, sz, sz, vp, vp, vp, sz, vp, vp]
     _lib = L
     return L
 

@@ -1911,6 +1911,269 @@ coded_rank_kernel(const btle_coded_rec *__restrict__ src, unsigned n, btle_coded
   for (int q = 0; q < (int)(sizeof(btle_coded_rec) / 16); ++q) d[q] = s[q];
 }
 
+// ---- LE Coded PHY connection discovery (btle_b200_discover_coded*, include/btle_b200.h "Coded connection discovery") ----
+// coded_discover_kernel: one CTA = kCdGroups groups of window starts (128 samples each) of one capture.  Q(n0) reads the
+// phase words of the 3 groups in front of n0's group and 9 behind it (12 window words), and the hit rule reads Q 256
+// samples (2 groups) to each side, so the CTA packs kCdThreads groups (G0 - 5 .. G0 + 122) and computes Q for
+// kCdQGroups (G0 - 2 .. G0 + 112):
+//   load   cp.async of the groups' IQ and one more row on each side into rows of kCodedPitch words (as coded_search_kernel)
+//   pack   lane p turns packed group p into its four phase words (dbits_group_lowpass, rotated by the capture's (C4, S4))
+//   Q      lane qg computes Q for the 128 window starts of its group into a byte buffer in the freed IQ rows: Dpre and the
+//          block-1 word that shares its last preamble word first, then 4 and 5 more words; once the running sum passes
+//          BTLE_CODED_DISC_T_Q the byte is T_Q + 1 (every comparison with a hit, Q <= T_Q, comes out the same).  Bit 7 marks
+//          Dpre > T_PRE (never a hit itself; its Q still bounds its neighbours); 0xFF where Q is not defined
+//   hits   lane qg of the tile's own groups applies the wide local-minimum rule to its bytes <= T_Q; a hit goes to a
+//          shared list (hits are at least W + 1 samples apart, so a tile holds at most kCdMaxHits)
+//   decode one warp per listed hit: the 2K + 1 alignments (preamble correlation + block-1 trellis ending in state 0),
+//          the block-2 trellis of the winner, dewhitening, the header test and the CRC unwind; each candidate takes one
+//          atomic on the counter.  No hit leaves the CTA, so there is no scratch and *count is exact whatever cap is.
+constexpr int kCdThreads = 128;
+constexpr int kCdQGroups = kCdThreads - 13;                                 // groups whose Q is computed (115)
+constexpr int kCdGroups = kCdQGroups - 4;                                   // window-start groups per CTA (111)
+constexpr int kCdMaxHits = (kCdGroups * 128 + BTLE_CODED_DISC_W) / (BTLE_CODED_DISC_W + 1);   // 56
+constexpr int kCdLo = 323, kCdSpan = 1184;                                  // Q(n0) defined for kCdLo <= n0 <= n_samples - kCdSpan
+constexpr int kCdAligns = 2 * BTLE_CODED_DISC_K + 1;
+constexpr int kCdStep1 = 37, kCdStep2 = 43;                                 // trellis steps of block 1 and of block 2's 40 bits + TERM
+static_assert(kCdQGroups * kCodedDPitch * 4 <= kCodedRows * kCodedPitch * 4, "the Q buffer must fit in the freed IQ rows");
+static_assert(BTLE_CODED_DISC_W == 256 && BTLE_CODED_DISC_T_Q < 127, "the halo is two groups; Q bytes keep 7 bits");
+static_assert(2 * 32 * BTLE_CODED_DISC_K < BTLE_CODED_DISC_W + 1, "two hits never re-align to the same sample");
+static_assert(sizeof(btle_coded_cand) == 32, "coded candidate record must be 32 bytes");
+struct CdWarp {
+  uint8_t surv1[kCdAligns][40];                                             // block-1 decisions of each alignment
+  uint8_t surv2[48];                                                        // block-2 decisions
+  int32_t L[88];                                                            // soft values of one trellis
+};
+struct CdSmem {
+  uint32_t rows[kCodedRows * kCodedPitch];                                  // staged IQ, then the Q bytes
+  uint4 pdw[kCdThreads];                                                    // phase words of packed group p
+  int2 hit[kCdMaxHits];                                                     // {Q index, Q} of the listed hits
+  CdWarp warp[kCdThreads / 32];
+  unsigned n_hits;
+};
+constexpr size_t kCdSmem = sizeof(CdSmem);
+static_assert(kCdSmem <= 48 * 1024, "coded_discover_kernel runs without a shared-memory opt-in");
+
+// Q-buffer byte of sample (G0 - 2) * 128 + idx
+__device__ __forceinline__ int cd_q_at(const uint8_t *Qb, int idx) {
+  return Qb[4 * ((idx >> 7) * kCodedDPitch + ((idx & 127) >> 2)) + (idx & 3)] & 0x7F;
+}
+// block-1 term of one window word: per nibble s0..s3, [s0 != s1] + [s2 != s3] + 2 [s0 = s1 = s2 = s3], over `mask`'s nibbles
+__device__ __forceinline__ int cd_group_dist(uint32_t w, uint32_t mask) {
+  const uint32_t u = (w ^ (w >> 1)) & mask, v = ((w >> 2) ^ (w >> 3)) & mask, x = (w ^ (w >> 2)) & mask;
+  return __popc(u) + __popc(v) + 2 * __popc(~(u | v | x) & mask);
+}
+// steps [0, n) of the coded trellis over W.L (lane & 7 holds its state's metric, state 0 from 0); decisions into surv.
+// Returns the metric of state 0 (every lane).
+__device__ __forceinline__ int cd_acs(const CdWarp &W, uint8_t *surv, int n) {
+  const int lane = threadIdx.x & 31, ns = lane & 7, b = ns & 1, p0 = ns >> 1, p1 = p0 | 4;
+  int a00, a01, a10, a11;
+  coded_fec(b, p0, a00, a01);
+  coded_fec(b, p1, a10, a11);
+  int m = ns ? kCodedNeg : 0;
+  for (int t = 0; t < n; ++t) {
+    const int L0 = W.L[2 * t], L1 = W.L[2 * t + 1];
+    const int m0 = __shfl_sync(0xFFFFFFFFu, m, p0), m1 = __shfl_sync(0xFFFFFFFFu, m, p1);
+    const int c0 = m0 + (a00 ? L0 : -L0) + (a01 ? L1 : -L1), c1 = m1 + (a10 ? L0 : -L0) + (a11 ? L1 : -L1);
+    const bool d = c1 > c0;
+    m = d ? c1 : c0;
+    const unsigned bal = __ballot_sync(0xFFFFFFFFu, d);
+    if (lane == 0) surv[t] = (uint8_t)bal;
+  }
+  __syncwarp();
+  return __shfl_sync(0xFFFFFFFFu, m, 0);
+}
+// info bits 0 .. n - 1 traced back from state 0 (bit t at bit t of the result; n <= 64)
+__device__ __forceinline__ unsigned long long cd_traceback(const uint8_t *surv, int n) {
+  unsigned long long bits = 0;
+  int state = 0;
+  for (int t = n - 1; t >= 0; --t) {
+    bits |= (unsigned long long)(state & 1) << t;
+    state = (state >> 1) | (((surv[t] >> state) & 1) << 2);
+  }
+  return bits;
+}
+
+__global__ void __launch_bounds__(kCdThreads)
+coded_discover_kernel(const int8_t *__restrict__ iq, long long stride, long long n_int8, long long tiles_per_stream,
+                      const StreamParams *__restrict__ params, const int4 *__restrict__ rot, btle_coded_cand *__restrict__ out,
+                      unsigned cap, unsigned *__restrict__ count) {
+  extern __shared__ __align__(16) uint32_t cd_smem_raw[];
+  CdSmem &S = *reinterpret_cast<CdSmem *>(cd_smem_raw);
+  const long long stream = blockIdx.x / tiles_per_stream, tile = blockIdx.x - stream * tiles_per_stream;
+  const int8_t *cap_base = iq + stream * stride;
+  const long long G0 = tile * kCdGroups;
+  const long long row0 = (G0 - 6) * 256;                                   // first byte of staged row 0
+  const bool interior = row0 >= 0 && row0 + kCodedRows * 256ll <= n_int8;
+  for (int k = threadIdx.x; k < kCodedRows * 16; k += kCdThreads) {
+    uint32_t *dst = S.rows + (k >> 4) * kCodedPitch + 4 * (k & 15);
+    const long long b = row0 + 16ll * k;
+    if (interior || (b >= 0 && b + 16 <= n_int8)) {
+      cp_async16(dst, cap_base + b);
+    } else {
+      uint32_t v[4] = {0u, 0u, 0u, 0u};
+      for (int q = 0; q < 16; ++q)
+        if (b + q >= 0 && b + q < n_int8) v[q >> 2] |= (uint32_t)(uint8_t)cap_base[b + q] << (8 * (q & 3));
+      *reinterpret_cast<uint4 *>(dst) = make_uint4(v[0], v[1], v[2], v[3]);
+    }
+  }
+  if (threadIdx.x == 0) S.n_hits = 0;
+  asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
+  __syncthreads();
+  const int4 r = __ldg(&rot[stream]);
+  {
+    const uint32_t *row = S.rows + (threadIdx.x + 1) * kCodedPitch;
+    auto word = [&](int k) -> uint32_t {
+      return k < 0 ? row[k - kCodedPitch + 64] : k >= 64 ? row[kCodedPitch + k - 64] : row[k];
+    };
+    uint32_t acc[4] = {0u, 0u, 0u, 0u};
+    dbits_group_lowpass<true>(word, r.z, r.w, acc);
+    S.pdw[threadIdx.x] = make_uint4(acc[0], acc[1], acc[2], acc[3]);
+  }
+  __syncthreads();                                                          // the IQ rows are free: Q goes there
+  const long long n_samples = n_int8 / 2, n0_hi = n_samples - kCdSpan;
+  uint8_t *Qb = reinterpret_cast<uint8_t *>(S.rows);
+  const int qg = threadIdx.x;
+  const long long g = G0 - 2 + qg;
+  if (qg < kCdQGroups) {
+#pragma unroll 1
+    for (int ph = 0; ph < 4; ++ph) {
+#pragma unroll 1
+      for (int half = 0; half < 2; ++half) {
+        uint32_t w[13];
+#pragma unroll
+        for (int k = 0; k < 13; ++k) {
+          const uint4 v = S.pdw[qg + half + k];
+          w[k] = ph == 0 ? v.x : ph == 1 ? v.y : ph == 2 ? v.z : v.w;
+        }
+        for (int ii = 0; ii < 16; ++ii) {
+          const int i = 16 * half + ii;
+          const uint32_t sh = half ? ii : 16 + ii;                         // preamble symbol 0 of window start 32 g + i
+          const long long n0 = 128 * g + 4 * i + ph;
+          int q = 0xFF;
+          if (n0 >= kCdLo && n0 <= n0_hi) {
+            const uint32_t t2 = funnel_r(w[2], w[3], sh);
+            const int dpre = __popc(funnel_r(w[0], w[1], sh) ^ 0x3C3C3C3Cu) + __popc(funnel_r(w[1], w[2], sh) ^ 0x3C3C3C3Cu) +
+                             __popc((t2 ^ 0x3C3C3C3Cu) & 0xFFFFu);
+            int s = dpre + cd_group_dist(t2, 0x11110000u);
+            if (s <= BTLE_CODED_DISC_T_Q) {
+#pragma unroll
+              for (int k = 3; k < 7; ++k) s += cd_group_dist(funnel_r(w[k], w[k + 1], sh), 0x11111111u);
+              if (s <= BTLE_CODED_DISC_T_Q) {
+#pragma unroll
+                for (int k = 7; k < 11; ++k) s += cd_group_dist(funnel_r(w[k], w[k + 1], sh), 0x11111111u);
+                s += cd_group_dist(funnel_r(w[11], w[12], sh), 0x00111111u);
+              }
+            }
+            q = min(s, BTLE_CODED_DISC_T_Q + 1) | (dpre > BTLE_CODED_DISC_T_PRE ? 0x80 : 0);
+          }
+          Qb[4 * (qg * kCodedDPitch + i) + ph] = (uint8_t)q;
+        }
+      }
+    }
+  }
+  __syncthreads();
+  // the tile's own groups apply the hit rule where a window start is defined
+  if (qg >= 2 && qg < 2 + kCdGroups && 128 * g <= n0_hi && 128 * g + 127 >= kCdLo) {
+    for (int i = 0; i < 32; ++i) {
+      const uint32_t w4 = reinterpret_cast<const uint32_t *>(Qb)[qg * kCodedDPitch + i];
+      uint32_t m = __vcmpleu4(w4, 0x01010101u * BTLE_CODED_DISC_T_Q);     // Q <= T_Q and Dpre <= T_PRE
+      while (m) {
+        const int ph = (__ffs((int)m) - 1) >> 3;
+        m &= ~(0xFFu << (8 * ph));
+        const int idx = 128 * qg + 4 * i + ph, q = (int)((w4 >> (8 * ph)) & 0xFFu);
+        bool hit = true;
+        for (int k = 1; k <= BTLE_CODED_DISC_W && hit; ++k) hit = q < cd_q_at(Qb, idx - k) && q <= cd_q_at(Qb, idx + k);
+        if (!hit) continue;
+        const unsigned slot = atomicAdd(&S.n_hits, 1u);
+        if (slot < kCdMaxHits) S.hit[slot] = make_int2(idx, q);
+      }
+    }
+  }
+  __syncthreads();
+  const unsigned n_hits = min(S.n_hits, (unsigned)kCdMaxHits);
+  const int lane = threadIdx.x & 31;
+  CdWarp &W = S.warp[threadIdx.x >> 5];
+  const CodedIq X{cap_base, n_samples, r.z, r.w};
+  for (unsigned h = threadIdx.x >> 5; h < n_hits; h += kCdThreads / 32) {
+    const long long n0 = (G0 - 2) * 128 + S.hit[h].x;
+    const int qv = S.hit[h].y;
+    // alignment: the preamble's soft correlation plus the block-1 metric ending in state 0; the largest wins, lowest k first
+    int best = INT_MIN, bk = 0;
+    for (int k = 0; k < kCdAligns; ++k) {
+      const long long m = n0 + 32ll * (k - BTLE_CODED_DISC_K);
+      if (m < kCdLo || m > n0_hi) continue;
+      int pre = 0;
+      for (int j = lane; j < kCodedPreamble; j += 32) {
+        const int y = X.y(m + 4ll * (j - kCodedPreamble));
+        pre += ((j & 7) >= 2 && (j & 7) <= 5) ? y : -y;
+      }
+      pre = warp_sum(pre);
+      for (int c = lane; c < 2 * kCdStep1; c += 32) {
+        const long long n = m + 16ll * c;
+        W.L[c] = X.y(n) + X.y(n + 4) - X.y(n + 8) - X.y(n + 12);
+      }
+      __syncwarp();
+      const int score = pre + cd_acs(W, W.surv1[k], kCdStep1);
+      if (score > best) { best = score; bk = k; }
+    }
+    const long long m = n0 + 32ll * (bk - BTLE_CODED_DISC_K);
+    const unsigned long long b1 = cd_traceback(W.surv1[bk], kCdStep1);
+    const uint32_t aa = (uint32_t)b1;
+    const int ci = (int)((b1 >> 32) & 3u);
+    if (ci >= 2) continue;
+    const int per = ci == 0 ? 4 : 1;
+    if (m + 4ll * (kCodedBlock1 + 2 * kCdStep2 * per - 1) + 3 >= n_samples) continue;   // block 2 must lie inside
+    for (int c = lane; c < 2 * kCdStep2; c += 32) {
+      const long long n = m + 4ll * (kCodedBlock1 + (long long)per * c);
+      W.L[c] = per == 1 ? X.y(n) : X.y(n) + X.y(n + 4) - X.y(n + 8) - X.y(n + 12);
+    }
+    __syncwarp();
+    const int metric = cd_acs(W, W.surv2, kCdStep2);
+    if (lane == 0) {
+      const unsigned long long b2 = cd_traceback(W.surv2, kCdStep2);
+      const uint32_t wh0 = __ldg(&params[stream].whiten[0]), wh1 = __ldg(&params[stream].whiten[1]);
+      const uint32_t header = ((uint32_t)b2 ^ wh0) & 0xFFFFu;
+      const uint32_t crc_rx = ((uint32_t)(b2 >> 16) ^ ((wh0 >> 16) | (wh1 << 16))) & 0xFFFFFFu;
+      if ((header & 3u) == 1u && (header >> 8) == 0u) {
+        const uint32_t crc_init = crc_init_reorder(crc24_unwind(crc_rx, header, 16));
+        const unsigned k = atomicAdd(count, 1u);
+        if (k < cap) {
+          uint4 *d = reinterpret_cast<uint4 *>(out + k);
+          d[0] = make_uint4((uint32_t)m, (uint32_t)(m >> 32), (uint32_t)stream, aa);
+          d[1] = make_uint4(crc_init, (uint32_t)__ldg(&params[stream].channel) | (header << 8) | ((per == 4 ? 8u : 2u) << 24),
+                            (uint32_t)(qv & 0xFFFF) | ((uint32_t)(uint8_t)(int8_t)(bk - BTLE_CODED_DISC_K) << 16), (uint32_t)metric);
+        }
+      }
+    }
+    __syncwarp();
+  }
+}
+
+// Order of btle_b200_discover_coded: candidate k of src goes to dst[rank], rank = the number of candidates before it in
+// (stream, sample) order (the keys are distinct: two hits are more than 2 * 32 K samples apart).
+__global__ void __launch_bounds__(256)
+coded_cand_rank_kernel(const btle_coded_cand *__restrict__ src, unsigned n, btle_coded_cand *__restrict__ dst) {
+  __shared__ unsigned long long keys[256];
+  const unsigned k = blockIdx.x * 256 + threadIdx.x;
+  const unsigned long long mine = k < n ? ((unsigned long long)(uint32_t)src[k].stream << 40) | (unsigned long long)src[k].sample : 0ull;
+  unsigned rank = 0;
+  for (unsigned base = 0; base < n; base += 256) {
+    __syncthreads();
+    if (base + threadIdx.x < n) {
+      const btle_coded_cand &o = src[base + threadIdx.x];
+      keys[threadIdx.x] = ((unsigned long long)(uint32_t)o.stream << 40) | (unsigned long long)o.sample;
+    }
+    __syncthreads();
+    const unsigned m = min(256u, n - base);
+    for (unsigned j = 0; j < m; ++j) rank += keys[j] < mine;
+  }
+  if (k >= n) return;
+  const uint4 *s = reinterpret_cast<const uint4 *>(src + k);
+  uint4 *d = reinterpret_cast<uint4 *>(dst + rank);
+  d[0] = s[0];
+  d[1] = s[1];
+}
+
 // ---- BER flow of python/test_btle_ber.py on the device: packet source + channel + int16 truncation --------------------
 // One CTA per packet: 37 random payload bytes behind the fixed header 42 25 (test_btle_ber.py:27,:49), build_air,
 // the Python model's 8-sps modulator (gfsk_block<8>), add_freq_sampling_error (linear
@@ -2514,6 +2777,7 @@ struct btle_b200_ctx {
   Buf<uint8_t> d_leaf;              // scratch of the leaf entry points (leaf_layout)
   Buf<btle_conn_cand> d_cand;       // device candidates of btle_b200_discover
   Buf<btle_coded_rec> d_coded[2];   // btle_b200_rx_coded: the records as found, and in (stream, sample) order
+  Buf<btle_coded_cand> d_ccand[2];  // btle_b200_discover_coded: the candidates as found, and in (stream, sample) order
   // BTLE_CFG_OFFSET_SEARCH (launch_offset_search): the hypotheses' records, directory and counters [hypotheses, merged], and
   // the last launch that used them (a flagged launch on another stream waits for it)
   Buf<btle_pkt_rec> os_out;
@@ -3252,6 +3516,49 @@ int launch_coded(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_captures, size
   rc = note_use(ctx, cs, st, sid);
   if (rc) return rc;
   ctx->last_launches = cap32 ? 2 : 1;
+  return BTLE_OK;
+}
+
+// Checks and launch of coded_discover_kernel (the counter is zeroed here).  The channels travel as btle_stream_cfg through
+// the cfg cache with each capture's rotation, so the kernel reads the whitening words and (C4, S4) by capture.
+int check_coded_discover(btle_b200_ctx *ctx, const int32_t *channels, size_t n_streams, const float *offset_hz, std::vector<int4> &rot) {
+  int rc = check_data_channels(ctx, channels, n_streams);
+  if (rc) return rc;
+  std::vector<float> hz(n_streams, 0.0f);
+  if (offset_hz && (rc = cfg_offsets(ctx, offset_hz, n_streams, nullptr, n_streams, hz))) return rc;
+  rot.resize(n_streams);
+  for (size_t s = 0; s < n_streams; ++s) rot[s] = make_rot(hz[s]);
+  return BTLE_OK;
+}
+
+int launch_coded_discover(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8, const int32_t *channels,
+                          const std::vector<int4> &rot, btle_coded_cand *d_out, size_t cap, unsigned *d_count, cudaStream_t st) {
+  if (!d_count || (!d_out && cap) || (!d_iq && n_streams && n_int8)) { ctx->err = "discover_coded: missing buffer"; return BTLE_EINVAL; }
+  if ((reinterpret_cast<uintptr_t>(d_iq) & 15) || (n_streams > 1 && (stride & 15))) { ctx->err = "device IQ must be 16-byte aligned"; return BTLE_EINVAL; }
+  if (reinterpret_cast<uintptr_t>(d_out) & 15) { ctx->err = "discover_coded: d_out must be 16-byte aligned"; return BTLE_EINVAL; }
+  if (n_streams > 1 && stride < n_int8) { ctx->err = "stream stride smaller than stream length"; return BTLE_EINVAL; }
+  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
+  ctx->last_launches = 0;
+  BTLE_CUDA(ctx, cudaMemsetAsync(d_count, 0, sizeof(unsigned), st));
+  const long long n_samples = (long long)(n_int8 / 2);
+  if (!n_streams || n_samples < kCdLo + kCdSpan) return BTLE_OK;         // no window fits
+  const long long groups = (n_samples - kCdSpan) / 128 + 1;                // groups holding a window start inside the capture
+  const long long tiles = (groups + kCdGroups - 1) / kCdGroups;
+  if (tiles * (long long)n_streams > 0x7FFFFFFFll) { ctx->err = "batch too large for one launch"; return BTLE_EINVAL; }
+  std::vector<btle_stream_cfg> cfgs(n_streams);
+  for (size_t s = 0; s < n_streams; ++s) cfgs[s] = btle_stream_cfg{channels[s], 0x8E89BED6u, 0xFFFFFFFFu, 0x555555u, 0, 0};
+  unsigned long long sid = 0;
+  int rc = stream_id(ctx, st, &sid);
+  if (rc) return rc;
+  CfgSlot *cs = nullptr;
+  rc = upload_cfgs(ctx, cfgs.data(), n_streams, st, sid, &cs, nullptr, rot.data());
+  if (rc) return rc;
+  coded_discover_kernel<<<(unsigned)(tiles * (long long)n_streams), kCdThreads, kCdSmem, st>>>(
+      d_iq, (long long)stride, (long long)n_int8, tiles, cs->d_params, cs->d_rot, d_out, (unsigned)std::min<size_t>(cap, 0xFFFFFFFFu), d_count);
+  BTLE_CUDA(ctx, cudaGetLastError());
+  rc = note_use(ctx, cs, st, sid);
+  if (rc) return rc;
+  ctx->last_launches = 1;
   return BTLE_OK;
 }
 
@@ -4465,6 +4772,46 @@ int btle_b200_rx_coded(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, s
                        const float *offset_hz, btle_coded_rec *out, size_t cap, size_t *n_out) {
   return btle_b200_rx_coded_multi(ctx, iq, n_streams, stride, n_int8, cfgs, identity_capture(n_streams).data(), n_streams, offset_hz, out,
                                   cap, n_out);
+}
+
+int btle_b200_discover_coded_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stride, size_t n_int8,
+                                    const int32_t *channels, const float *offset_hz, btle_coded_cand *d_out, size_t cap,
+                                    uint32_t *d_count, void *cuda_stream) {
+  if (!ctx) return BTLE_EINVAL;
+  std::vector<int4> rot;
+  const int rc = check_coded_discover(ctx, channels, n_streams, offset_hz, rot);
+  if (rc) return rc;
+  return launch_coded_discover(ctx, d_iq, n_streams, stride, n_int8, channels, rot, d_out, cap, d_count,
+                               reinterpret_cast<cudaStream_t>(cuda_stream));
+}
+
+// The candidates land unordered in ctx->d_ccand[0], are put in (stream, sample) order into ctx->d_ccand[1] on the device
+// (coded_cand_rank_kernel) and copied out.
+int btle_b200_discover_coded(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stride, size_t n_int8,
+                             const int32_t *channels, const float *offset_hz, btle_coded_cand *out, size_t cap, size_t *n_out) {
+  if (!ctx) return BTLE_EINVAL;
+  if (!n_out || (!out && cap) || (!iq && n_streams && n_int8)) { ctx->err = "discover_coded: missing buffer"; return BTLE_EINVAL; }
+  *n_out = 0;
+  std::vector<int4> rot;
+  int rc = check_coded_discover(ctx, channels, n_streams, offset_hz, rot);   // before any byte is copied
+  if (rc) return rc;
+  BTLE_CUDA(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  size_t pitch = 0;
+  rc = ingest(ctx, iq, n_streams, stride, n_int8, nullptr, n_streams, &pitch);
+  if (rc) return rc;
+  if (ctx->d_ccand[0].reserve(ctx, std::max<size_t>(cap, 1)) || ctx->d_ccand[1].reserve(ctx, std::max<size_t>(cap, 1))) return BTLE_ENOMEM;
+  rc = launch_coded_discover(ctx, ctx->d_iq, n_streams, pitch, n_int8, channels, rot, ctx->d_ccand[0], cap, ctx->d_count, st);
+  if (rc) return rc;
+  rc = fetch_counted(ctx, st, cap, n_out, [&](size_t n) {
+    coded_cand_rank_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ctx->d_ccand[0], (unsigned)n, ctx->d_ccand[1]);
+    BTLE_CUDA(ctx, cudaGetLastError());
+    BTLE_CUDA(ctx, cudaMemcpyAsync(out, ctx->d_ccand[1], n * sizeof(btle_coded_cand), cudaMemcpyDeviceToHost, st));
+    return BTLE_OK;
+  });
+  if (rc) return rc;
+  if (*n_out > cap) { ctx->err = "output capacity too small"; return BTLE_EOVERFLOW; }
+  return BTLE_OK;
 }
 
 // Streaming form of the Python model's receiver over an 8-Msps interleaved int16 capture (see include/btle_b200.h).

@@ -305,7 +305,7 @@ def follow_connections(rx, captures: np.ndarray, max_events: int = 10000, discov
 
 def decode_connections(rx, captures: np.ndarray, discover: bool = True, offset_hz=None, symbol_spaced: bool = False,
                        centre_hits: bool = False, correct: bool = False, lowpass: bool = False, offset_search: bool = False,
-                       coded: bool = False):
+                       coded: bool = False, coded_discover: bool = False):
     """Every known connection's data-channel traffic, decoded without following it.  captures: int8 [40, n_int8] as in
     follow_connections(); `rx` needs rx_batch, rx_multi, with discover=True discover, and with coded=True rx_coded and
     rx_coded_multi (a BtleRx).
@@ -332,6 +332,10 @@ def decode_connections(rx, captures: np.ndarray, discover: bool = True, offset_h
         channel) in (sample, channel) order.  So a 1M connection that moved to the coded PHY is covered too.
     offset_hz is passed to the coded calls as well; the 1M opt-in flags are not (the coded receiver has none).  AUX_CONNECT_REQ
     connections get `traffic` like every other one.  With coded=False the result is what it was without the argument.
+    coded_discover=True (with coded=True; `rx` then also needs discover_coded) adds one discover_coded call over
+    captures[0:37] after the rx_coded one: the discover_coded_connections() connections whose (access address, CRC init)
+    is not already known are added after the AUX_CONNECT_REQ ones, and get `traffic` and `coded_traffic` like every other
+    connection.  With coded_discover=False the result and the calls are what they were without the argument.
     Returns (adv_records, connections)."""
     from ._native import MAX_CFGS_PER_CAPTURE
     captures = np.ascontiguousarray(captures, dtype=np.int8)
@@ -359,6 +363,8 @@ def decode_connections(rx, captures: np.ndarray, discover: bool = True, offset_h
         for c in aux:
             c["tracked"] = False
         conns += new_connections(conns, aux)
+        if coded_discover:
+            conns += new_connections(conns, discover_coded_connections(rx, captures, offset_hz=off))
     K = MAX_CFGS_PER_CAPTURE
     for b0 in range(0, len(conns), K):
         batch = conns[b0:b0 + K]
@@ -426,7 +432,12 @@ def discover_connections(rx, captures: np.ndarray, min_events: int = 4):
     than `min_events` events are noise and are dropped.  Returns the _connection_from_events() dicts in order of t_first."""
     captures = np.ascontiguousarray(captures, dtype=np.int8)
     assert captures.shape[0] == 40
-    cand = rx.discover(captures[0:37], np.arange(37, dtype=np.int32))
+    return _group_candidates(rx.discover(captures[0:37], np.arange(37, dtype=np.int32)), min_events)
+
+
+def _group_candidates(cand, min_events: int):
+    """discover_connections()' grouping of candidates (any record with sample, access_addr, crc_init and channel) into
+    _connection_from_events() dicts in order of t_first"""
     if len(cand) == 0:
         return []
     cand = cand[np.lexsort((cand["sample"], cand["crc_init"], cand["access_addr"]))]
@@ -443,6 +454,21 @@ def discover_connections(rx, captures: np.ndarray, min_events: int = 4):
         if len(events) >= min_events:
             conns.append(_connection_from_events(int(grp[0]["access_addr"]), int(grp[0]["crc_init"]), events, len(grp)))
     conns.sort(key=lambda c: (c["t_first"], c["access_addr"]))
+    return conns
+
+
+def discover_coded_connections(rx, captures: np.ndarray, min_events: int = 4, offset_hz=None):
+    """LE Coded PHY connections found from their empty coded PDUs alone, without an AUX_CONNECT_REQ (include/btle_b200.h,
+    "Coded connection discovery").  captures: int8 [40, n_int8]; rows 0..36 are scanned in one rx.discover_coded() call
+    (offset_hz: a scalar or one per capture of the 40, passed for rows 0..36 when given).  The candidates are grouped
+    exactly as discover_connections() groups its own.  Each dict carries "coded": True, `tracked` False and no hop or
+    interval (None): coded connections use CSA#2, which neither the hop inference nor the 1M walk follows."""
+    captures = np.ascontiguousarray(captures, dtype=np.int8)
+    assert captures.shape[0] == 40
+    kw = {} if offset_hz is None else {"offset_hz": np.broadcast_to(np.asarray(offset_hz, dtype=np.float32), (40,))[0:37]}
+    conns = _group_candidates(rx.discover_coded(captures[0:37], np.arange(37, dtype=np.int32), **kw), min_events)
+    for c in conns:
+        c.update(coded=True, tracked=False, hop=None, interval=None)
     return conns
 
 

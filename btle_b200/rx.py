@@ -12,7 +12,7 @@ from functools import partial
 import numpy as np
 
 from . import _native
-from ._native import BTLE_EOVERFLOW, BtleError, CAND_DTYPE, CFG_DTYPE, CODED_REC_DTYPE, DIR_DTYPE, REC_DTYPE
+from ._native import BTLE_EOVERFLOW, BtleError, CAND_DTYPE, CFG_DTYPE, CODED_CAND_DTYPE, CODED_REC_DTYPE, DIR_DTYPE, REC_DTYPE
 
 DEFAULT_ACCESS_ADDR = 0x8E89BED6     # btle_rx.c:231
 DEFAULT_CRC_INIT = 0x555555          # btle_rx.c:232
@@ -258,6 +258,33 @@ class BtleRx:
         off = _offsets(offset_hz, ns)
         call = partial(self._L.btle_b200_rx_coded, self._h, iq.ctypes.data, ns, n, n, cfgs.ctypes.data, _ptr(off))
         return self._grow_once(call, CODED_REC_DTYPE, ns * (n // 65536 + 1) * 4 + 64 if cap is None else cap, grow=cap is None)
+
+    def discover_coded(self, iq: np.ndarray, channels, offset_hz=None, cap: int | None = None) -> np.ndarray:
+        """Empty coded PDU candidates of coded connection discovery (btle_b200_discover_coded): iq int8 [n_streams, n_int8]
+        (or [n_int8]) of data-channel captures, channels[s] in 0..36 the channel of capture s; offset_hz (a scalar or one
+        per capture): carrier-offset correction.  Returns CODED_CAND_DTYPE records sorted by (stream, sample); `cap`
+        defaults to a typical worst case and is grown once to the exact count on overflow."""
+        iq = np.ascontiguousarray(iq, dtype=np.int8)
+        if iq.ndim == 1:
+            iq = iq[None, :]
+        ns, n = iq.shape
+        ch = np.ascontiguousarray(np.broadcast_to(np.asarray(channels, dtype=np.int32), (ns,)))
+        off = _offsets(offset_hz, ns)
+        call = partial(self._L.btle_b200_discover_coded, self._h, iq.ctypes.data, ns, n, n, ch.ctypes.data, _ptr(off))
+        return self._grow_once(call, CODED_CAND_DTYPE, ns * (n // 65536 + 1) * 4 + 64 if cap is None else cap, grow=cap is None)
+
+    def discover_coded_device(self, d_iq, channels, d_out, d_count, stream_ptr: int = 0, offset_hz=None):
+        """discover_coded on device-resident captures: d_iq torch int8 CUDA tensor [n_streams, n_int8] (16-byte aligned
+        rows); d_out: torch CUDA tensor of cap * 32 bytes (16-byte aligned); d_count: torch int32 CUDA tensor [1].
+        Enqueues on `stream_ptr` (no sync).  Candidates land unordered in d_out[:min(count, cap)] (view the bytes as
+        CODED_CAND_DTYPE)."""
+        ns, n = d_iq.shape
+        assert d_iq.stride(1) == 1
+        ch = np.ascontiguousarray(np.broadcast_to(np.asarray(channels, dtype=np.int32), (ns,)))
+        off = _offsets(offset_hz, ns)
+        cap = d_out.numel() * d_out.element_size() // CODED_CAND_DTYPE.itemsize
+        self._check(self._L.btle_b200_discover_coded_device(self._h, d_iq.data_ptr(), ns, d_iq.stride(0), n, ch.ctypes.data, _ptr(off),
+                                                            d_out.data_ptr(), cap, d_count.data_ptr(), ctypes.c_void_p(stream_ptr)))
 
     def rx_coded_device(self, d_iq, cfgs: np.ndarray, d_out, d_count, stream_ptr: int = 0, offset_hz=None):
         """d_iq: torch int8 CUDA tensor [n_streams, n_int8] (16-byte aligned rows); cfgs: CFG_DTYPE [n_streams]; d_out: torch

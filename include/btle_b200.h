@@ -556,6 +556,61 @@ int btle_b200_rx_coded_multi_device(btle_b200_ctx *ctx, const int8_t *d_iq, size
                                     const float *offset_hz, btle_coded_rec *d_out, size_t cap, uint32_t *d_count,
                                     void *cuda_stream);
 
+/* ---- Coded connection discovery: empty coded PDUs on data-channel captures, no access address given -----------------
+ * Not part of the reference.  The coded connections whose AUX_CONNECT_REQ was not captured are found from the empty PDUs
+ * of their idle events, as btle_b200_discover finds 1M ones.  Discriminator, positions, hard bits h, soft values y and
+ * the trellis are the coded receiver's ("LE Coded PHY" above).  On a capture of n_samples samples:
+ *   search    for every n0 with 323 <= n0 and n0 + 1184 <= n_samples (the preamble and block 1 inside the capture):
+ *             Dpre(n0) = #{j = -80..-1 : h[n0 + 4j] != preamble[j]}; C(n0) = sum over the 74 groups k = 0..73 of block 1
+ *             (symbols j = 4k..4k+3, s0..s3) of the Hamming distance to the nearer of 0,0,1,1 and 1,1,0,0, i.e.
+ *             [s0 != s1] + [s2 != s3] + 2 [s0 = s1 = s2 = s3] (no access address needed); Q(n0) = Dpre(n0) + C(n0).
+ *   hit       Dpre(n0) <= BTLE_CODED_DISC_T_PRE, Q(n0) <= BTLE_CODED_DISC_T_Q, Q(n0) < Q(m) for every defined m in
+ *             [n0 - W, n0 - 1] and Q(n0) <= Q(m) for every defined m in [n0 + 1, n0 + W], W = BTLE_CODED_DISC_W.  The
+ *             preamble repeats every 8 symbols (32 samples) and the S=8 mapper looks the same at every 4-symbol step, so
+ *             one packet makes a ladder of low Q every 32 samples; W spans it.  Two hits are more than W samples apart.
+ *   align     for k = -K..K (K = BTLE_CODED_DISC_K), m = n0 + 32k with m inside the search range: score(m) = the soft
+ *             correlation sum_{j=-80..-1} (2 preamble[j] - 1) y[m + 4j] plus the metric of state 0 after the 37 block-1
+ *             steps (S=8 soft values of symbols 0..295, the trellis from state 0; TERM1 ends block 1 in state 0).  The
+ *             largest score wins, the lowest k on a tie.  Its traceback from state 0 gives the access address (info bits
+ *             0..31) and CI (bits 32..33).  CI 2 or 3: no candidate.  2 * 32 K < W + 1, so two hits never give one m.
+ *   PDU       block 2 at the S of CI: 43 steps (16 header + 24 CRC + 3 TERM bits) from state 0, traced back from state
+ *             0; bits 0..39 dewhitened with the channel's whitening bits 0..39 are the header and the received CRC.
+ *             Every sample read must lie inside the capture (m + 4 (296 + 86 S/2 - 1) + 3 < n_samples with S/2 the
+ *             symbols per coded bit over 2: 4 at S=8, 1 at S=2) or there is no candidate.  A CANDIDATE needs LLID 1 and
+ *             byte 1 == 0 (btle_b200_discover's header rule); crc_init is the unique -k value whose CRC-24 of the two
+ *             header bytes equals the received CRC.
+ * For a noiseless coded empty PDU of the project's transmitter, sample is the n0 of btle_b200_rx_coded's record. */
+#define BTLE_CODED_DISC_T_PRE 24
+#define BTLE_CODED_DISC_T_Q 80
+#define BTLE_CODED_DISC_W 256
+#define BTLE_CODED_DISC_K 4
+typedef struct {
+  int64_t sample;        /* m: first sample of the access address (symbol j = 0), from the start of the capture         */
+  int32_t stream;
+  uint32_t access_addr;
+  uint32_t crc_init;     /* -k convention (not reordered)                                                              */
+  uint8_t channel;
+  uint8_t header[2];     /* dewhitened: LLID 1, length 0                                                               */
+  uint8_t s;             /* 8 or 2                                                                                     */
+  int16_t dist;          /* Q of the hit                                                                               */
+  int8_t shift;          /* the chosen k: sample = hit + 32 k                                                          */
+  uint8_t reserved;
+  int32_t metric;        /* metric of state 0 after block 2's 43 steps                                                 */
+} btle_coded_cand;       /* 32 bytes; its first 23 bytes are laid out as btle_conn_cand's */
+/* device: d_iq 16-byte aligned, stride a multiple of 16 and >= n_int8 when n_streams > 1; channels[s] (host array) the
+ * data channel of capture s (0..36); offset_hz (host array, NULL = 0) its carrier offset (<= BTLE_MAX_OFFSET_HZ).
+ * Candidates are unordered; *d_count (zeroed by the call) = the number found, d_out[0 .. min(count, cap)) holds that many
+ * (not necessarily the first ones).  Enqueued on cuda_stream, not synchronised; the cfg cache is shared with the other
+ * launches as described for btle_b200_rx_device_dir.  BTLE_EINVAL with btle_b200_last_error() set: a channel outside
+ * 0..36, an offset that is not finite or too large, a misaligned pointer or stride, a missing buffer. */
+int btle_b200_discover_coded_device(btle_b200_ctx *ctx, const int8_t *d_iq, size_t n_streams, size_t stream_stride_int8,
+                                    size_t n_int8, const int32_t *channels, const float *offset_hz, btle_coded_cand *d_out,
+                                    size_t cap, uint32_t *d_count, void *cuda_stream);
+/* host buffers (page-locked or pageable); out sorted by (stream, sample) on the device before the copy.  BTLE_EOVERFLOW
+ * with *n_out = the number found when that exceeds cap; a second call with cap >= *n_out returns them all. */
+int btle_b200_discover_coded(btle_b200_ctx *ctx, const int8_t *iq, size_t n_streams, size_t stream_stride_int8, size_t n_int8,
+                             const int32_t *channels, const float *offset_hz, btle_coded_cand *out, size_t cap, size_t *n_out);
+
 /* ---- connections on a streaming session (btle_b200_streams_*): per-capture cfg lists, backfill, discovery -----------
  * Every cfg of a session has a stable index, never reused: the n_streams cfgs of btle_b200_streams_open are 0..n-1 (cfg
  * i decodes capture i), each added cfg gets the next one.  A record's `stream` is that index.  The records of cfg j equal
